@@ -1,4 +1,4 @@
-"""Reference arm: drive the UNMODIFIED reference scripts from ``baseline/_ref``.
+"""Reference arm: drive the UNMODIFIED reference scripts staged by ``build()`` into ``oracle/_ref`` (oracle/stage_reference.py).
 
 Nothing from ``dist_tuto.pth_b200`` (models, kernels, engine) is on the measured path.  What is used:
 
@@ -32,14 +32,14 @@ ROOT = os.path.dirname(HERE)
 
 
 def load_reference():
-    sys.path.insert(0, HERE)
-    import install_ref
-    ok, why = install_ref.verify()
-    if not ok:
-        ok, why = install_ref.install()
+    """The staged original's ``train_dist`` module (hash-checked), or (None, why) when build() could not stage it."""
+    spec = importlib.util.spec_from_file_location("stage_reference", os.path.join(ROOT, "oracle", "stage_reference.py"))
+    stage = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(stage)
+    ok, why = stage.verify()
     if not ok:
         return None, why
-    spec = importlib.util.spec_from_file_location("ref_train_dist", os.path.join(install_ref.DST, "train_dist.py"))
+    spec = importlib.util.spec_from_file_location("ref_train_dist", os.path.join(stage.DST, "train_dist.py"))
     mod = importlib.util.module_from_spec(spec)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")

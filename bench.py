@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark (driver contract): MNIST-ConvNet synchronous data-parallel SGD, samples/s.
 
-    python bench.py --gpus N --steps K --warmup W [--impl ours|reference]
+    python bench.py --gpus N --steps K --warmup W [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -25,6 +25,8 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+# measure the native extension as the build left it: never rebuild (or take a build lock) inside a possibly read-only tree
+os.environ.setdefault("B200DIST_AUTOBUILD", "0")
 
 
 def parse():
@@ -39,6 +41,10 @@ def parse():
     ap.add_argument("--large-batch", type=int, default=4096,
                     help="per-GPU batch of the extra large-batch (throughput, weak-scaling) measurement; 0 = skip")
     ap.add_argument("--loader-buffers", type=int, default=24, help="pinned ring depth of the native loader (e2e arm)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed steps computed (parameters, momentum and loss accumulator after the last timed step; "
+                         "the large-batch arm's parameters) as DIR/<name>.npy, rank 0; inputs are seeded, so two builds compare "
+                         "output for output")
     return ap.parse_args()
 
 
@@ -51,8 +57,9 @@ def gpu_smi_id(torch, dev):
         return dev.index
 
 
-def large_batch_arm(torch, b2, LB, rank, size, dev, max_over_ranks, steps=12):
-    """Device-timed samples/s of full training steps at per-GPU batch ``LB`` (weak scaling) on the batched tcgen05 engine."""
+def large_batch_arm(torch, b2, LB, rank, size, dev, max_over_ranks, steps, dump=None):
+    """Device-timed samples/s of ``steps`` full training steps (the --steps of the run) at per-GPU batch ``LB`` (weak scaling)
+    on the batched wgmma engine."""
     from dist_tuto.pth_b200.ops.convnet_batched import BatchedTrainer
     tr = BatchedTrainer(LB, lr=0.01, momentum=0.5, seed=1234, device=dev, p_drop=0.5, raw_uint8=True)
     npool = steps + 1
@@ -88,9 +95,11 @@ def large_batch_arm(torch, b2, LB, rank, size, dev, max_over_ranks, steps=12):
     st.synchronize()
     ms = max_over_ranks(e0.elapsed_time(e1), dev)
     loss = float(tr.loss_acc[0].item())
+    if dump is not None:
+        dump["large_batch_params"] = tr.params.detach().double().cpu().numpy()
     out = {"per_gpu_batch": LB, "global_batch": LB * size, "scaling": "weak", "steps": steps, "us_per_step": ms / steps * 1e3,
-           "samples_per_s": LB * size * steps / (ms / 1e3), "dtype": "bf16 tensor-core operands (tcgen05), fp32 accumulate / master weights",
-           "engine": "batched: conv2 fwd/dgrad/wgrad + fc1 on tcgen05 with TMA-fed operands, fused all-reduce+SGD kernel",
+           "samples_per_s": LB * size * steps / (ms / 1e3), "dtype": "bf16 tensor-core operands (wgmma), fp32 accumulate / master weights",
+           "engine": "batched: conv2 fwd/dgrad/wgrad + fc1 on wgmma with TMA-fed operands, fused all-reduce+SGD kernel",
            "launches_per_step": tr.gpu_launches_per_step, "loss_finite": loss == loss,
            "l2": "L2 flushed before the pre-roll; every timed step reads a batch not touched since"}
     del graphs, tr
@@ -153,7 +162,7 @@ def ours(args):
         smi_id = gpu_smi_id(torch, dev)            # physical GPU (UUID): CUDA_VISIBLE_DEVICES re-numbers the logical index
         with ClockSampler(smi_id) as clk:
             with torch.cuda.stream(st):
-                flush_buf.fill_(1)                                     # L2 flush: 256 MB > 126 MB L2
+                flush_buf.fill_(1)                                     # L2 flush: 256 MB > the 50 MB L2 of an H100
                 graphs[0].replay()                                     # pre-roll (untimed)
                 e0.record(st)
                 for s in range(n_full):
@@ -166,6 +175,11 @@ def ours(args):
             torch.cuda.synchronize()
         ms = max_over_ranks(e0.elapsed_time(e1), dev)
         value = bsz * size * K / (ms / 1e3)
+        # what a caller of the timed path receives after its last step (snapshot before the e2e arm trains on)
+        dump = None
+        if args.dump_outputs:
+            dump = {"params": tr.params.detach().double().cpu().numpy(), "momentum": tr.momentum.detach().double().cpu().numpy(),
+                    "loss_acc": tr.loss_acc[:2].detach().double().cpu().numpy()}
         clocks = clk.summary()
         if clocks["samples"] < 3:
             # the timed region (K x ~30 us) is shorter than one nvidia-smi query: sample the clocks under the SAME load by
@@ -225,9 +239,14 @@ def ours(args):
         large = None
         if args.large_batch > 0:
             try:
-                large = large_batch_arm(torch, b2, args.large_batch, rank, size, dev, max_over_ranks)
+                large = large_batch_arm(torch, b2, args.large_batch, rank, size, dev, max_over_ranks, K, dump=dump)
             except Exception as e:      # never take the headline down
                 large = {"error": f"{type(e).__name__}: {e}"[:300]}
+        if rank == 0 and dump is not None:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, arr in dump.items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
         if rank == 0:
             sym = tr.symm.describe() if tr.symm is not None else {"world": 1}
             print(result_line(impl="ours", value=value, ms=ms, n_gpus=size, steps=K, warmup=W, clocks=clocks,

@@ -87,10 +87,9 @@ def body(rank, size):
     variants = [("ll", 3), ("oneshot", 0), ("twoshot", 1)] + ([("nvls", 2)] if w.multicast else [])
 
     def link_bytes(name, nbytes):
-        """Bytes one GPU transmits over its NVLink ports for one all-reduce of ``nbytes`` (receives the same).  Checked against the
-        GPU's own link counters at 2 GPUs (bench/nvlink_bytes.py, profiles/n2/r2_nvlink_bytes_2gpu.json): one-shot 1.008x,
-        two-shot 1.002x and NVLS 1.000x of these formulas; the LL lines are 16-byte stores that the link carries at 32-byte
-        granularity, so LL really moves 1.8x the formula (3.6x the payload per peer) -- it is a latency variant."""
+        """Bytes one GPU transmits over its NVLink ports for one all-reduce of ``nbytes`` (receives the same), by algorithm;
+        bench/nvlink_bytes.py checks these formulas against the GPU's own link counters.  The LL lines are 16-byte stores
+        that carry 8 data bytes each -- it is a latency variant."""
         if name == "ll":
             return 2 * nbytes * (size - 1)                       # 16-byte lines carry 8 data bytes, to every peer
         if name == "oneshot":

@@ -4,13 +4,13 @@ No GPU involved -- this measures the *plumbing*: data sharding + loader, model s
 averaging over gloo, optimizer.  Two arms, same metric (samples/s, wall clock, max over ranks, K timed steps after W
 warm-up steps, global batch 128 = 64 per rank):
 
-  reference : the UNMODIFIED reference from baseline/_ref -- ``train_dist.Net``, ``train_dist.partition_dataset()``
+  reference : the UNMODIFIED reference from oracle/_ref -- ``train_dist.Net``, ``train_dist.partition_dataset()``
               (torchvision MNIST on synthetic idx files + DataLoader), the tutorial-text ``average_gradients``
               (tuto.md:310-314: one all_reduce + one divide per parameter), ``optim.SGD`` -- loop body train_dist.py:115-124
   ours      : ``dist_tuto.pth_b200`` -- ``partition_dataset()`` (C++ prefetch thread into staging buffers), ``Net``,
               gradients as views of ONE flat bucket (one gloo all_reduce per step), ``FlatSGD``
 
-Run here (no GPU):  python bench/cpu_plumbing_bench.py --steps 150 --warmup 10 --out profiles/cpu_plumbing_world2.json
+Run here (no GPU):  python bench/cpu_plumbing_bench.py --steps 150 --warmup 10 --out cpu_plumbing_world2.json
 """
 import argparse
 import json

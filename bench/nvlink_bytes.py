@@ -3,7 +3,7 @@
     python bench/nvlink_bytes.py --gpus N [--out gpurun_out/nvlink_bytes_N.json]
 
 Nsight Compute cannot profile these kernels (they spin on their peers, so a replayed or serialised launch deadlocks:
-profiles/REPORT_r2.md section 7), so the traffic is read from NVML's per-device NVLink data counters
+see DESIGN.md section 6), so the traffic is read from NVML's per-device NVLink data counters
 (``NVML_FI_DEV_NVLINK_THROUGHPUT_DATA_TX / _RX``, KiB, summed over the links; ``nvidia-smi nvlink -gt d`` as fallback)
 before and after ``iters`` back-to-back all-reduces of one variant and size.  Reported per all-reduce and per GPU next to
 the model used in bench/allreduce_sweep.py (`link_bytes()`), for every variant of csrc/allreduce.cu and for NCCL.

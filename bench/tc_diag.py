@@ -1,4 +1,4 @@
-"""Diagnostic: fused ConvNet kernel, SIMT vs tcgen05 conv2 path vs fp64 oracle (errors per tensor, training curves)."""
+"""Diagnostic: fused ConvNet kernel, SIMT vs wgmma conv2 path vs fp64 oracle (errors per tensor, training curves)."""
 import json
 import os
 import sys

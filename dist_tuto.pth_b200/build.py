@@ -1,7 +1,7 @@
 """In-tree build of the native extension ``dist_tuto.pth_b200/_C.so``.
 
-* every ``.cu`` is compiled by nvcc for **sm_100a only**
-  (``-gencode arch=compute_100a,code=sm_100a -lineinfo``) -- no torch headers in
+* every ``.cu`` is compiled by nvcc for **sm_90a only**
+  (``-gencode arch=compute_90a,code=sm_90a -lineinfo``) -- no torch headers in
   the kernels, so a file takes seconds and cross-compiles without a GPU;
 * ``bindings.cpp`` (pybind11 + torch) and the host runtime (``symm_mem.cpp``,
   ``loader.cpp``) are compiled by g++;
@@ -28,7 +28,7 @@ CU_SOURCES = ["allreduce.cu", "convnet.cu", "convnet_cluster.cu", "sgd.cu", "gem
 CPP_SOURCES = ["symm_mem.cpp", "loader.cpp", "executor.cpp", "bindings.cpp"]
 HEADERS = ["common.cuh", "tc_common.cuh", "convnet_args.cuh", "sgd_device.cuh", "loader.h", "executor.h"]
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -83,7 +83,7 @@ def build(verbose: bool = True, force: bool = False) -> str:
         if force or not os.path.exists(obj):
             jobs.append((["g++"] + cxx_flags + incs + ["-c", sp, "-o", obj], obj + ".log"))
     if verbose and jobs:
-        print(f"[build] compiling {len(jobs)} object(s) for sm_100a ...", flush=True)
+        print(f"[build] compiling {len(jobs)} object(s) for sm_90a ...", flush=True)
     with ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         list(ex.map(lambda j: _run(*j), jobs))
 

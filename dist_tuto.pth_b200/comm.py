@@ -8,7 +8,7 @@ Parity map (reference = /root/reference):
   * ``new_group(ranks)``                            tuto.md:176,182
   * ``get_rank()/get_world_size()``                 train_dist.py:84,88,96
 
-Design (B200-first, not a port):
+Design (GPU-first, not a port):
   * plumbing (rendezvous, p2p, the non-hot collectives) rides on
     ``torch.distributed`` -- NCCL for CUDA tensors (NVLink 5 / NVSwitch),
     gloo for CPU tensors;
@@ -166,7 +166,7 @@ def _symm_world_for(tensor: torch.Tensor, group):
 def all_reduce(tensor: torch.Tensor, op=reduce_op.SUM, group=None, async_op: bool = False):
     """In-place all-reduce; result on every rank (tuto.md:176-186,199).
 
-    CUDA float tensors with ``op=SUM`` go through the fused sm_100a peer-memory
+    CUDA float tensors with ``op=SUM`` go through the fused sm_90a peer-memory
     kernels (one-shot / two-shot / NVLS picked by size) when a symmetric world
     exists for the group; everything else goes to NCCL / gloo."""
     _check(tensor)

@@ -1,4 +1,4 @@
-// Fused peer-memory all-reduce kernels for sm_100a (NVLink 5 / NVSwitch).
+// Fused peer-memory all-reduce kernels for sm_90a (NVLink / NVSwitch).
 //
 // Replaces the reference's hot path  `dist.all_reduce(param.grad.data, SUM); param.grad.data /= size`
 // per parameter tensor (train_dist.py:94-100, tuto.md:310-314)  with ONE kernel per flat bucket that

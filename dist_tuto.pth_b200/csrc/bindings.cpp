@@ -1,4 +1,4 @@
-// Python bindings (pybind11 / torch extension) for the native runtime and the sm_100a kernels.
+// Python bindings (pybind11 / torch extension) for the native runtime and the sm_90a kernels.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -68,7 +68,6 @@ int b2_gemm_available();
 int b2_gemm_bf16_launch(const void* a, const void* b, void* c, const float* bias, int M, int N, int K, int relu,
                         int out_bf16, cudaStream_t stream);
 const char* b2_gemm_last_error();
-int b2_gemm_probe_m64(const void* a, const void* b, float* dump, cudaStream_t stream);
 struct FusedTailHost {            // mirrors cn::FusedTailHost (csrc/convnet_args.cuh)
   void* grad_ptrs[8];
   void* inbox_ptrs[8];
@@ -98,8 +97,8 @@ const char* b2_probe_last_error();
 int b2_tma_probe(const void* tensor, int rank, const unsigned long long* dims, const unsigned long long* strides_bytes,
                  const unsigned int* box, int swizzle, const int* coords, unsigned int bytes, unsigned char* out,
                  cudaStream_t stream);
-int b2_umma_probe(const unsigned char* a_img, unsigned int a_bytes, const unsigned char* b_img, unsigned int b_bytes,
-                  unsigned int idesc, const unsigned long long* ops, int n_ops, int ncols, float* dump, cudaStream_t stream);
+int b2_wgmma_probe(const unsigned char* a_img, unsigned int a_bytes, const unsigned char* b_img, unsigned int b_bytes,
+                   int a_mn, const unsigned long long* ops, int n_ops, int n, float* dump, cudaStream_t stream);
 }
 
 namespace {
@@ -252,7 +251,7 @@ struct ExecutorPy {
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "dist_tuto.pth_b200 native runtime: symmetric memory, fused sm_100a kernels, native loader";
+  m.doc() = "dist_tuto.pth_b200 native runtime: symmetric memory, fused sm_90a kernels, native loader";
 
   // ------------------------------------------------------------------ symmetric memory
   m.def("symm_caps", [](int dev) { int c[3]; ck_symm(b2_symm_caps(dev, c), "symm_caps"); return std::vector<int>{c[0], c[1], c[2]}; });
@@ -335,7 +334,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });
-  m.def("convnet_set_tc", [](bool on) { b2_convnet_set_tc(on); }, "route conv2 forward/dgrad of the fused step through tcgen05 (bf16)");
+  m.def("convnet_set_tc", [](bool on) { b2_convnet_set_tc(on); }, "route conv2 forward/dgrad of the fused step through wgmma (bf16)");
   m.def("convnet_get_tc", [] { return b2_convnet_get_tc() != 0; });
   m.def("convnet_smem_bytes", [] { return b2_convnet_smem_bytes(); });
   m.def("convnet_step", [](torch::Tensor params, c10::optional<torch::Tensor> grads, torch::Tensor x, torch::Tensor target,
@@ -425,7 +424,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("partials"), py::arg("n_slots"), py::arg("grads"), py::arg("step") = py::none(), py::arg("grad_stride") = 0,
      py::arg("loss_acc") = py::none());
 
-  // ------------------------------------------------------------------ tcgen05 GEMM
+  // ------------------------------------------------------------------ wgmma GEMM
   m.def("gemm_available", [] { return b2_gemm_available() != 0; });
   m.def("gemm_bf16", [](torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor> bias, bool relu, bool out_bf16) {
     // C[M,N] = A[M,K] @ B[N,K]^T (+bias) (relu) ; A,B bf16 row-major (K contiguous)
@@ -442,15 +441,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     if (rc != 0) throw std::runtime_error(std::string("gemm_bf16: ") + b2_gemm_last_error());
     return c;
   }, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("relu") = false, py::arg("out_bf16") = true);
-
-  m.def("gemm_probe_m64", [](torch::Tensor a, torch::Tensor b) {
-    check_cuda_contig(a, "a"); check_cuda_contig(b, "b");
-    TORCH_CHECK(a.scalar_type() == torch::kBFloat16 && a.size(0) == 64 && a.size(1) == 64 && b.size(0) == 32 && b.size(1) == 64);
-    auto dump = torch::zeros({128, 32}, a.options().dtype(torch::kFloat32));
-    int rc = b2_gemm_probe_m64(a.data_ptr(), b.data_ptr(), dump.data_ptr<float>(), cur_stream());
-    if (rc != 0) throw std::runtime_error(std::string("gemm_probe_m64: ") + b2_gemm_last_error());
-    return dump;
-  });
 
   // ------------------------------------------------------------------ batched tensor-core engine (csrc/convnet_batched.cu)
   // bufs: [P1, P2, H, DH, dP2, DC, W2K, W2R, W3K, W3T, A1, A2, Hrelu, DLOG, G1, B3P] (see ops/convnet_batched.py)
@@ -522,17 +512,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     if (rc != 0) throw std::runtime_error(std::string("tma_probe: ") + b2_probe_last_error());
     return out;
   }, py::arg("tensor"), py::arg("dims"), py::arg("strides_bytes"), py::arg("box"), py::arg("swizzle"), py::arg("coords"));
-  m.def("umma_probe", [](torch::Tensor a_img, torch::Tensor b_img, unsigned int idesc, std::vector<unsigned long long> ops, int ncols) {
-    // ops: flat list of (adesc, bdesc, tmem_col, accumulate) quadruples; returns TMEM[128 lanes, ncols] fp32
+  m.def("wgmma_probe", [](torch::Tensor a_img, torch::Tensor b_img, bool a_mn, std::vector<unsigned long long> ops, int n) {
+    // ops: flat list of (adesc, bdesc, accumulate) triples of one warpgroup; returns D[64, n] fp32
     check_cuda_contig(a_img, "a_img"); check_cuda_contig(b_img, "b_img");
-    TORCH_CHECK(a_img.scalar_type() == torch::kUInt8 && b_img.scalar_type() == torch::kUInt8 && ops.size() % 4 == 0);
-    auto dump = torch::zeros({128, ncols}, a_img.options().dtype(torch::kFloat32));
+    TORCH_CHECK(a_img.scalar_type() == torch::kUInt8 && b_img.scalar_type() == torch::kUInt8 && ops.size() % 3 == 0);
+    auto dump = torch::zeros({64, n}, a_img.options().dtype(torch::kFloat32));
     c10::cuda::CUDAGuard guard(a_img.device());
-    int rc = b2_umma_probe(a_img.data_ptr<uint8_t>(), (unsigned int)a_img.numel(), b_img.data_ptr<uint8_t>(), (unsigned int)b_img.numel(),
-                           idesc, ops.data(), (int)(ops.size() / 4), ncols, dump.data_ptr<float>(), cur_stream());
-    if (rc != 0) throw std::runtime_error(std::string("umma_probe: ") + b2_probe_last_error());
+    int rc = b2_wgmma_probe(a_img.data_ptr<uint8_t>(), (unsigned int)a_img.numel(), b_img.data_ptr<uint8_t>(), (unsigned int)b_img.numel(),
+                            a_mn ? 1 : 0, ops.data(), (int)(ops.size() / 3), n, dump.data_ptr<float>(), cur_stream());
+    if (rc != 0) throw std::runtime_error(std::string("wgmma_probe: ") + b2_probe_last_error());
     return dump;
-  }, py::arg("a_img"), py::arg("b_img"), py::arg("idesc"), py::arg("ops"), py::arg("ncols"));
+  }, py::arg("a_img"), py::arg("b_img"), py::arg("a_mn"), py::arg("ops"), py::arg("n"));
 
   // ------------------------------------------------------------------ native step executor
   py::class_<ExecutorPy>(m, "StepExecutor")

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels (inline PTX; no CUTLASS dependency).
+// Shared device helpers for the sm_90a kernels (inline PTX; no CUTLASS dependency).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -138,8 +138,8 @@ __device__ __forceinline__ void block_barrier_all_ranks(const SignalPads& s, int
     st_release_sys(s.pad[peer] + blockIdx.x * B2_MAX_RANKS + rank, epoch);
     const uint32_t* mine = s.pad[rank] + blockIdx.x * B2_MAX_RANKS + peer;
     unsigned long long spins = 0;
-    // (measured: relaxed polling + one fence.acq_rel.sys afterwards is SLOWER -- 14.9 vs 9.5 us per fused
-    //  all-reduce+SGD call at 2 GPUs -- the sys-scope fence costs more than the acquire loads it replaces)
+    // (acquire loads in the loop rather than relaxed polling + one fence.acq_rel.sys afterwards: the sys-scope fence
+    //  is the more expensive of the two)
     while ((int32_t)(ld_acquire_sys(mine) - epoch) < 0) {
       if (++spins > B2_SPIN_LIMIT) {
         printf("[b200dist] barrier timeout: rank %d block %d waiting for rank %d epoch %u (have %u)\n", rank,

@@ -1,4 +1,4 @@
-// Fused MNIST-ConvNet training step for sm_100a: forward + loss + backward of the tutorial's `Net`
+// Fused MNIST-ConvNet training step for sm_90a: forward + loss + backward of the tutorial's `Net`
 // (train_dist.py:53-71, nll_loss train_dist.py:120, backward :122) in ONE kernel.
 //
 // The reference runs ~35 library/ATen kernels per step (cuDNN convs, pools, relus, dropouts, cuBLAS
@@ -26,7 +26,7 @@ constexpr int T = 512;              // 16 warps per sample: the phases are laten
 
 // The conv2 working set exists in two flavours that share one union:
 //   SIMT path : fp32 weights in two layouts + split-K partial sums + the zero-padded conv2-output gradient
-//   TC path   : bf16 UMMA operand tiles (K-major, 128B swizzle) for the two tcgen05 GEMMs of conv2
+//   TC path   : bf16 wgmma operand tiles (K-major, 128B swizzle) for the conv2 GEMMs (fp32 accumulators in registers)
 //               forward  D[64 pos x 32 co]   = im2col(p1)[64 x 256] * W2[32 x 256]^T
 //               dgrad    D[64 pos x 256 k']  = dC[64 x 32 co]       * W2^T[256 x 32]^T      (k' = (ci/5)*128 + (ci%5)*25 + tap)
 //               wgrad    D[64 co  x 256 k ]  = dC^T[64 x 64 pos]    * im2col(p1)^T[256 x 64]^T
@@ -49,7 +49,7 @@ union Scratch {
 };
 
 struct __align__(1024) Smem {
-  Scratch u;                // first member: 1024-byte aligned (UMMA SWIZZLE_128B tiles)
+  Scratch u;                // first member: 1024-byte aligned (SWIZZLE_128B operand tiles)
   float w1[252];
   float b1[12];
   float b2[20];
@@ -67,8 +67,6 @@ struct __align__(1024) Smem {
   float m2[20];             // dropout2d channel scale
   float rnd[72];            // uniforms: [0,20) dropout2d, [20,70) dropout
   float g[NPAR];            // per-CTA gradient accumulators
-  unsigned long long mma_bar;   // mbarrier: tcgen05.commit -> "accumulator ready"
-  unsigned int tmem_slot;
   int work_ctr;             // dynamic work distribution inside a phase (warp-granular)
   short koff[256];          // im2col LUT: k=(ci,ky,kx) -> offset inside p1, -1 for the K padding
   unsigned char a1[1440];   // conv1 pool argmax (0..3)
@@ -84,9 +82,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x;
-  if (TC && (tc::smem_u32(smem_raw) & 1023u) != 0u) __trap();   // UMMA SWIZZLE_128B tiles need 1024-byte alignment
-  uint32_t mma_phase = 0;            // parity of the next "accumulator ready" wait (uniform across the CTA)
-  uint32_t tmem = 0;
+  if (TC && (tc::smem_u32(smem_raw) & 1023u) != 0u) __trap();   // SWIZZLE_128B operand tiles need 1024-byte alignment
   const float* __restrict__ P = a.params;
 
   // ---------------------------------------------------------------- P0: stage weights, zero accumulators
@@ -123,12 +119,10 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     if (tid < 500) s.w4[tid] = w4v;
     if (tid < 10) s.b1[tid] = bv; else if (tid < 20) s.b4[tid - 10] = bv; else if (tid < 40) s.b2[tid - 20] = bv;
     if (TC) {
-      // zero the bf16 operand tiles (row / K padding must be 0), build the im2col LUT, set up mbarrier + TMEM
+      // zero the bf16 operand tiles (row / K padding must be 0), build the im2col LUT
       uint4* z = reinterpret_cast<uint4*>(s.u.tc.Bw);
       for (int i = tid; i < (16384 + 32768) / 16; i += T) z[i] = make_uint4(0u, 0u, 0u, 0u);
       if (tid < 256) s.koff[tid] = tid < 250 ? (short)p1_idx(tid / 25, (tid % 25) / 5, tid % 5) : (short)-1;
-      if (tid == 0) { tc::mbar_init(reinterpret_cast<uint64_t*>(&s.mma_bar), 1); tc::mbar_fence_init(); }
-      if ((tid >> 5) == 1) tc::tmem_alloc<512>(&s.tmem_slot);
       __syncthreads();
     }
     if (fast) {
@@ -164,9 +158,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   if (tid == 0) { s.loss_local = 0.f; s.correct_local = 0; }
   const unsigned long long step = a.step ? *a.step : 0ull;
   const float keep_scale = 1.f / (1.f - a.p_drop);
-  if (TC) { tc::fence_proxy_async(); tc::fence_before(); }
+  if (TC) tc::fence_proxy_async();
   __syncthreads();
-  if (TC) { tc::fence_after(); tmem = s.tmem_slot; }
 
   for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
     // -------------------------------------------------------------- S0: input, RNG, clear scratch
@@ -228,7 +221,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       s.m2[tid] = a.training ? (s.rnd[tid] >= a.p_drop ? keep_scale : 0.f) : 1.f;
     __syncthreads();
 
-    // -------------------------------------------------------------- S2: conv2 (TC: im2col + tcgen05 GEMM | SIMT: K split 5)
+    // -------------------------------------------------------------- S2: conv2 (TC: im2col + wgmma GEMM | SIMT: K split 5)
     if (TC) {
       // im2col(p1) -> bf16 A operand, 2048 16-byte chunks (row = output position, 8 consecutive k per chunk)
 #pragma unroll
@@ -246,38 +239,29 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         *reinterpret_cast<uint4*>(s.u.tc.A + (c >> 3) * 8192 + (r >> 3) * 1024 + (r & 7) * 128 + ((((c & 7) ^ (r & 7)) & 7) << 4)) = pk;
       }
       tc::fence_proxy_async();
-      tc::fence_before();
       __syncthreads();
-      if (tid == 0) {
-        tc::fence_after();
-        constexpr uint32_t idesc = tc::idesc_bf16(64, 32);
+      if (tid < 128) {                            // warpgroup 0: D[64 pos x 32 co] in registers
+        float d[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d[i] = 0.f;
         const uint32_t a0 = tc::smem_u32(s.u.tc.A), b0 = tc::smem_u32(s.u.tc.Bw);
+        tc::wg_fence();
 #pragma unroll
         for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            tc::umma_bf16(tmem, tc::smem_desc_sw128(a0 + kb * 8192 + k * 32), tc::smem_desc_sw128(b0 + kb * 4096 + k * 32),
-                          idesc, (kb | k) != 0 ? 1u : 0u);
-        tc::commit(reinterpret_cast<uint64_t*>(&s.mma_bar));
-      }
-      tc::mbar_wait(reinterpret_cast<uint64_t*>(&s.mma_bar), mma_phase);
-      mma_phase ^= 1;
-      tc::fence_after();
-      if (tid < 128) {                            // UMMA_M = 64: rows 16q..16q+15 live in TMEM lanes 32q..32q+15
-        const int q = tid >> 5, lane = tid & 31;
-        uint32_t r[32];
-        tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16), r);
-        tc::tmem_ld_wait();
-        if (lane < 16) {
-          const int row = q * 16 + lane;
-          float4* dst = reinterpret_cast<float4*>(s.u.tc.Ad) + row * 8;      // conv2 output staging [64][32] fp32
+            tc::mma<32>(d, tc::smem_desc_sw128(a0 + kb * 8192 + k * 32), tc::smem_desc_sw128(b0 + kb * 4096 + k * 32),
+                        (kb | k) != 0 ? 1u : 0u);
+        tc::wg_commit();
+        tc::wg_wait_all();
+        tc::acc_fence<16>(d);
+        float* dst = reinterpret_cast<float*>(s.u.tc.Ad);   // conv2 output staging [64][32] fp32, float4 index ^= row & 7
 #pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4)
-            dst[c4 ^ (row & 7)] = make_float4(__uint_as_float(r[4 * c4]), __uint_as_float(r[4 * c4 + 1]),
-                                             __uint_as_float(r[4 * c4 + 2]), __uint_as_float(r[4 * c4 + 3]));
+        for (int i = 0; i < 16; i += 2) {
+          const int row = tc::acc_row(tid, i), col = tc::acc_col(tid, i);
+          *reinterpret_cast<float2*>(dst + row * 32 + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) = make_float2(d[i], d[i + 1]);
         }
       }
-      tc::fence_before();
       __syncthreads();
     }
     if (!TC) {
@@ -461,7 +445,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     // -------------------------------------------------------------- S7a: conv2 weight/bias gradient (sparse)
     // Work items are handed out 32 at a time per warp from a shared counter, so the warps that had no (or a short)
     // S7b tile start here immediately and the phase ends balanced.  item < 1000: (co, ci, ky) = 5 taps x 16 pooled
-    // cells; item 1000..1019: bias gradient of channel item-1000.  (TC mode: weight items are done by tcgen05.)
+    // cells; item 1000..1019: bias gradient of channel item-1000.  (TC mode: weight items are done by wgmma.)
     auto s7a = [&]() {
       for (;;) {
         int base = 0;
@@ -497,7 +481,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         }
       }
     };
-    // -------------------------------------------------------------- S7b/S8a: conv2 weight + data gradients on tcgen05
+    // -------------------------------------------------------------- S7b/S8a: conv2 weight + data gradients on wgmma
     if (TC) {
       // (1) dC[64 pos][co] (one non-zero per pool window and channel) as the bf16 A operand of the dgrad GEMM
       if (tid < 256) {
@@ -539,59 +523,44 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         *reinterpret_cast<uint4*>(s.u.tc.A + (k >> 3) * 1024 + (k & 7) * 128 + (((oy ^ (k & 7)) & 7) << 4)) = pk;
       }
       tc::fence_proxy_async();
-      tc::fence_before();
       __syncthreads();
-      if (tid == 0) {
-        tc::fence_after();
-        constexpr uint32_t idesc = tc::idesc_bf16(64, 256);
-        const uint32_t ad = tc::smem_u32(s.u.tc.Ad), bt = tc::smem_u32(s.u.tc.Bt);
-        const uint32_t at = tc::smem_u32(s.u.tc.Adt), bi = tc::smem_u32(s.u.tc.A);
-        tc::umma_bf16(tmem, tc::smem_desc_sw128(ad), tc::smem_desc_sw128(bt), idesc, 0u);               // dgrad: K = co
-        tc::umma_bf16(tmem, tc::smem_desc_sw128(ad + 32), tc::smem_desc_sw128(bt + 32), idesc, 1u);
+      // warpgroup g: dgrad D[64 pos x 64 k'] at columns 64g.. (K = co, 2 steps) and wgrad D[64 co x 64 k] at columns 64g..
+      // (K = pos, 4 steps); the two 32-register accumulators stay in the issuing warpgroup
+      const int wg = tid >> 7, t = tid & 127;
+      float dd[32], dw[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)                                                                      // wgrad: K = pos
-          tc::umma_bf16(tmem + 256, tc::smem_desc_sw128(at + k * 32), tc::smem_desc_sw128(bi + k * 32), idesc, k != 0 ? 1u : 0u);
-        tc::commit(reinterpret_cast<uint64_t*>(&s.mma_bar));
+      for (int i = 0; i < 32; ++i) { dd[i] = 0.f; dw[i] = 0.f; }
+      {
+        const uint32_t ad = tc::smem_u32(s.u.tc.Ad), bt = tc::smem_u32(s.u.tc.Bt) + wg * 8192;
+        const uint32_t at = tc::smem_u32(s.u.tc.Adt), bi = tc::smem_u32(s.u.tc.A) + wg * 8192;
+        tc::wg_fence();
+        tc::mma<64>(dd, tc::smem_desc_sw128(ad), tc::smem_desc_sw128(bt), 0u);                 // dgrad: K = co
+        tc::mma<64>(dd, tc::smem_desc_sw128(ad + 32), tc::smem_desc_sw128(bt + 32), 1u);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)                                                            // wgrad: K = pos
+          tc::mma<64>(dw, tc::smem_desc_sw128(at + k * 32), tc::smem_desc_sw128(bi + k * 32), k != 0 ? 1u : 0u);
+        tc::wg_commit();
       }
-      s7a();                                                  // bias gradient (20 items) while the MMAs run
-      tc::mbar_wait(reinterpret_cast<uint64_t*>(&s.mma_bar), mma_phase);
-      mma_phase ^= 1;
-      tc::fence_after();
+      tc::wg_wait_all();
+      tc::acc_fence<32>(dd);
+      tc::acc_fence<32>(dw);
+      s7a();                                                  // bias gradient (20 items)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {                          // conv2.weight gradient: accumulator row = co, column = k
+        const int co = tc::acc_row(t, i), k = wg * 64 + tc::acc_col(t, i);
+        if (co < 20 && k < 250) s.g[W2 + co * 250 + k] += dw[i];
+      }
+      __syncthreads();                                        // operand tiles consumed: A becomes the dgrad staging tile
       float* stage = reinterpret_cast<float*>(s.u.tc.A);      // [64 rows][128 cols] fp32, float4 index XOR-swizzled by row
 #pragma unroll 1
-      for (int half = 0; half < 2; ++half) {                  // input channels 5*half .. 5*half+4  <->  TMEM columns 128*half ..
-        if (tid < 128) {
-          const int q = tid >> 5, lane = tid & 31, row = q * 16 + (lane & 15);
-#pragma unroll 1
-          for (int cc = 0; cc < 4; ++cc) {
-            uint32_t r[32];
-            tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 128 + cc * 32), r);
-            tc::tmem_ld_wait();
-            if (lane < 16) {
-              float4* dst = reinterpret_cast<float4*>(stage) + row * 32;
+      for (int half = 0; half < 2; ++half) {                  // input channels 5*half .. 5*half+4  <->  columns 128*half ..
+        if ((wg >> 1) == half) {
 #pragma unroll
-              for (int c4 = 0; c4 < 8; ++c4)
-                dst[(cc * 8 + c4) ^ (row & 31)] = make_float4(__uint_as_float(r[4 * c4]), __uint_as_float(r[4 * c4 + 1]),
-                                                              __uint_as_float(r[4 * c4 + 2]), __uint_as_float(r[4 * c4 + 3]));
-            }
-          }
-        } else if (tid < 192) {
-          // conv2.weight gradient: accumulator rows = co (rows 0..15 in lanes 0..15 of quadrant 0, rows 16..19 in quadrant 1)
-          const int q = (tid >> 5) & 3, lane = tid & 31, co = q * 16 + lane;
-#pragma unroll 1
-          for (int cc = 0; cc < 4; ++cc) {
-            uint32_t r[32];
-            tc::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(256 + half * 128 + cc * 32), r);
-            tc::tmem_ld_wait();
-            if (lane < 16 && co < 20) {
-              float* dst = &s.g[W2 + co * 250 + half * 128 + cc * 32];
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (half * 128 + cc * 32 + i < 250) dst[i] += __uint_as_float(r[i]);
-            }
+          for (int i = 0; i < 32; i += 2) {
+            const int row = tc::acc_row(t, i), j = (wg & 1) * 64 + tc::acc_col(t, i);
+            *reinterpret_cast<float2*>(stage + row * 128 + ((((j >> 2) ^ (row & 31)) & 31) << 2) + (j & 3)) = make_float2(dd[i], dd[i + 1]);
           }
         }
-        tc::fence_before();
         __syncthreads();
         // col2im gather: dp1[ci][y][x] = sum_{ky,kx} dA[(y-ky, x-kx)][ci, ky, kx], fused with relu'/pool routing of conv1
         for (int o5 = tid; o5 < 720; o5 += T) {
@@ -730,11 +699,6 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   }
   // ------------------------------------------------------------------ fused tail: gradient exchange + SGD in this kernel
   if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x);   // grid <= B: every CTA flushed
-  if (TC) {
-    tc::fence_before();
-    __syncthreads();
-    if ((tid >> 5) == 1) { tc::fence_after(); tc::tmem_dealloc<512>(tmem); }
-  }
 }
 
 }  // namespace cn

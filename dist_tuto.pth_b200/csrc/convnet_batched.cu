@@ -1,28 +1,28 @@
-// Batched (large per-GPU batch) training engine for the tutorial ConvNet on sm_100a: layer-wise kernels over the whole
-// batch, with the GEMM-shaped layers on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM) fed by TMA.
+// Batched (large per-GPU batch) training engine for the tutorial ConvNet on sm_90a: layer-wise kernels over the whole
+// batch, with the GEMM-shaped layers on the Hopper tensor cores (wgmma.mma_async, accumulators in registers) fed by TMA.
 //
 // The per-sample fused kernels (convnet.cu / convnet_cluster.cu) are built for the reference's latency-bound configuration
 // (global batch 128, train_dist.py:85).  At B >= 1024 per GPU the same network is throughput-bound, and 66 % of its MACs
 // are the three conv2 GEMMs (train_dist.py:59,66 and their backward), so here:
 //
 //   conv1 -> pool -> relu             bt_conv1_fwd     SIMT (K = 25: not GEMM-shaped); writes P1 as bf16 NHWC [B,12,12,16]
-//   conv2 -> dropout2d -> pool -> relu bt_conv2_fwd    tcgen05: implicit GEMM, M = 128 rows = 2 samples x 64 positions,
+//   conv2 -> dropout2d -> pool -> relu bt_conv2_fwd    wgmma: implicit GEMM, M = 128 rows = 2 samples x 64 positions,
 //                                                       N = 32 (20 channels), K = 25 taps x 16 input channels.  TMA IS the
 //                                                       im2col: one 4-D box {16 c, 8 x, 8 y, 2 b} per tap at offset (kx, ky)
 //                                                       lands as a K-major 32B-swizzled A tile (one 32-byte row per output
-//                                                       position); bias/dropout2d/pool/relu run in the tcgen05.ld epilogue.
+//                                                       position); bias/dropout2d/pool/relu run in the register epilogue.
 //                                                       (Channel-last because TMA needs a 16-byte aligned innermost start:
-//                                                       an x-innermost box shifted by kx elements faults -- profiles/probes.)
-//   fc1 (+bias, relu)                  gemm_tcgen05.cu  the library GEMM of this repo (TMA + tcgen05), N = 64
+//                                                       an x-innermost box shifted by kx elements is not a legal box start.)
+//   fc1 (+bias, relu)                  gemm_tcgen05.cu  the library GEMM of this repo (TMA + wgmma), N = 64
 //   dropout, fc2, log_softmax, nll,    bt_head          SIMT, one thread per sample (2 kFLOP/sample)
 //   and their backward down to dH
 //   fc1 data gradient                  gemm_tcgen05.cu  dP2 = dH x W3
 //   pool/relu/dropout2d backward       bt_route         dP2 -> dC (bf16, NCHW [B,32,8,8])
-//   conv2 weight (+bias) gradient      bt_conv2_wgrad   tcgen05: D[(tap,ci), co] = sum over positions; the same 25 TMA tap
+//   conv2 weight (+bias) gradient      bt_conv2_wgrad   wgmma: D[(tap,ci), co] = sum over positions; the same 25 TMA tap
 //                                                       boxes per sample are now the MN-major A operand (M = 8 taps x 16
 //                                                       channels per instruction), dC the K-major B operand; the bias
 //                                                       gradient falls out of a constant-one input channel.
-//   conv2 data gradient                bt_conv2_dgrad   tcgen05: dA[pos, (tap,ci)] = dC x W2 (N = 400 as 208 + 192), then
+//   conv2 data gradient                bt_conv2_dgrad   wgmma: dA[pos, (tap,ci)] = dC x W2 (N = 400 as 5 x 80), then
 //                                                       col2im + relu/pool routing of conv1 in the epilogue
 //   conv1 weight gradient              bt_conv1_wgrad   SIMT (sparse: one of four positions per pooled cell)
 //   fc weight/bias gradients           bt_fc_wgrad      SIMT register tiles
@@ -157,140 +157,122 @@ __global__ void __launch_bounds__(288) bt_conv1_fwd(const float* __restrict__ pa
 }
 
 // =====================================================================================================================
-// conv2 forward on tcgen05: implicit GEMM with TMA as the im2col engine.
+// conv2 forward on wgmma: implicit GEMM with TMA as the im2col engine.
 // =====================================================================================================================
 // One TMA box per tile brings the whole 12x12x16 input of TWO samples into shared memory as [y][b][x][c] (32-byte pixels,
 // 32B swizzle); the 25 filter taps are then 25 shared-memory DESCRIPTORS over that image -- start address shifted by
 // (ky*768 + kx*32) bytes, 8-row groups (one output row of one sample) 384 bytes apart -- so the im2col costs no data movement
 // at all (the first version issued one TMA box per tap: 25x the L2->SM traffic, 70 us at B = 4096).  Accumulator row
-// r = (oy*2 + b)*8 + ox.  Descriptor arithmetic validated on hardware by scripts/tc_probe_matrix.py (umma_window_fwd_*).
+// r = (oy*2 + b)*8 + ox.  Descriptor arithmetic checked on hardware by tests/test_gpu_tc_probe.py.
 constexpr int C2F_NST = 4;
 constexpr int C2F_IMG = 12 * 2 * 12 * 32;     // 9216 B
+constexpr int BT_THREADS = 384;               // warpgroup 0: TMA producer, warpgroups 1, 2: wgmma + epilogue (64 rows each)
 struct __align__(1024) C2fSmem {
   uint8_t w[7][4096];                 // W2 as B operand: 7 K-blocks of [32 co rows x 64 k], k = (tap % 4) * 16 + ci
   uint8_t a[C2F_NST][C2F_IMG];        // [12 y][2 b][12 x][16 c] bf16
   float stage[128][21];
   float m2[2][20];
   float bias[20];
-  uint64_t full[C2F_NST], empty[C2F_NST], wfull, tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  uint64_t full[C2F_NST], empty[C2F_NST], wfull;
 };
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(BT_THREADS, 1)
 bt_conv2_fwd(const __grid_constant__ CUtensorMap map_p1, const __grid_constant__ CUtensorMap map_w2k,
              const float* __restrict__ params, Common cm, __nv_bfloat16* __restrict__ P2, unsigned char* __restrict__ A2) {
   extern __shared__ uint8_t smem_raw[];
   C2fSmem& s = *reinterpret_cast<C2fSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int tiles = (cm.B + 1) / 2;
   if (threadIdx.x == 0) {
     tc::prefetch_tmap(&map_p1); tc::prefetch_tmap(&map_w2k);
-    for (int i = 0; i < C2F_NST; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 1); }
+    for (int i = 0; i < C2F_NST; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 256); }
     tc::mbar_init(&s.wfull, 1);
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&s.tmem_full[i], 1); tc::mbar_init(&s.tmem_empty[i], 4); }
     tc::mbar_fence_init();
   }
   if (threadIdx.x < 20) s.bias[threadIdx.x] = params[B2 + threadIdx.x];
-  if (warp == 1) tc::tmem_alloc<64>(&s.tmem_base);
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem0 = s.tmem_base;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ======================================================== TMA producer: one box per tile
-    if (lane == 0) {
+    if (t == 0) {
       tc::mbar_expect_tx(&s.wfull, 7 * 4096);
       for (int j = 0; j < 7; ++j) tc::tma_load_2d(s.w[j], &map_w2k, &s.wfull, j * 64, 0);
       uint32_t it = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
+      for (int tt = blockIdx.x; tt < tiles; tt += gridDim.x, ++it) {
         const int st = it % C2F_NST;
         tc::mbar_wait(&s.empty[st], ((it / C2F_NST) & 1) ^ 1);
         tc::mbar_expect_tx(&s.full[st], C2F_IMG);
-        tc::tma_load_4d(s.a[st], &map_p1, &s.full[st], 0, 0, 2 * t, 0);       // dims (c, x, b, y)
+        tc::tma_load_4d(s.a[st], &map_p1, &s.full[st], 0, 0, 2 * tt, 0);      // dims (c, x, b, y)
       }
     }
-  } else if (warp == 1) {
-    // ======================================================== MMA issuer: 25 taps = 25 descriptors over the image
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::idesc_bf16_major(128, 32, 0, 0);
-      tc::mbar_wait(&s.wfull, 0);
-      uint32_t it = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
-        const uint32_t acc = it & 1;
-        const int st = it % C2F_NST;
-        tc::mbar_wait(&s.tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-        tc::mbar_wait(&s.full[st], (it / C2F_NST) & 1);
-        tc::fence_after();
-        const uint32_t img = tc::smem_u32(s.a[st]);
-#pragma unroll 5
-        for (int tap = 0; tap < 25; ++tap) {
-          const int ky = tap / 5, kx = tap - ky * 5;
-          const uint64_t ad = tc::smem_desc(img + ky * 768 + kx * 32, 16, /*SBO: next (oy, b) row group*/ 384, /*SWIZZLE_32B*/ 6);
-          const uint64_t bd = tc::smem_desc(tc::smem_u32(s.w[tap >> 2]) + (tap & 3) * 32, 16, 1024, 2);
-          tc::umma_bf16(tmem0 + acc * 32, ad, bd, idesc, tap > 0 ? 1u : 0u);
-        }
-        tc::commit(&s.empty[st]);
-        tc::commit(&s.tmem_full[acc]);
-      }
+    return;
+  }
+  // ========================================================== 25 taps = 25 descriptors over the image, then bias,
+  // dropout2d, 2x2 max-pool, relu.  Warpgroup h owns accumulator rows 64h..64h+63 = row groups (oy*2 + b) 8h..8h+7.
+  const int h = wg - 1, e = threadIdx.x - 128;
+  const float keep = 1.f / (1.f - cm.p_drop);
+  const unsigned long long step = cm.step ? *cm.step : 0ull;
+  tc::mbar_wait(&s.wfull, 0);
+  uint32_t it = 0;
+  for (int tt = blockIdx.x; tt < tiles; tt += gridDim.x, ++it) {
+    const int st = it % C2F_NST;
+    const int b0 = 2 * tt;
+    if (e < 10) {
+      const int sb = e / 5, qq = e % 5;
+      const uint4 rr = b2::Philox::gen(cm.seed, (unsigned long long)(cm.sample_base + b0 + sb), step * 32ull + qq);
+      const float k = 2.3283064365386963e-10f;
+      s.m2[sb][qq * 4 + 0] = drop_scale(rr.x * k, cm.p_drop, keep, cm.training);
+      s.m2[sb][qq * 4 + 1] = drop_scale(rr.y * k, cm.p_drop, keep, cm.training);
+      s.m2[sb][qq * 4 + 2] = drop_scale(rr.z * k, cm.p_drop, keep, cm.training);
+      s.m2[sb][qq * 4 + 3] = drop_scale(rr.w * k, cm.p_drop, keep, cm.training);
     }
-    __syncwarp();
-  } else {
-    // ======================================================== epilogue: bias, dropout2d, 2x2 max-pool, relu
-    const int q = warp & 3, e = (warp - 2) * 32 + lane;          // q: TMEM lane quadrant this warp may read
-    const int r = q * 32 + lane;                                 // accumulator row = (oy*2 + b)*8 + ox
-    const int bl = (r >> 3) & 1, srow = bl * 64 + (r >> 4) * 8 + (r & 7);   // staging row = b*64 + oy*8 + ox
-    const float keep = 1.f / (1.f - cm.p_drop);
-    const unsigned long long step = cm.step ? *cm.step : 0ull;
-    uint32_t li = 0;
-    for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++li) {
-      const uint32_t acc = li & 1;
-      const int b0 = 2 * t;
-      if (e < 10) {
-        const int sb = e / 5, qq = e % 5;
-        const uint4 rr = b2::Philox::gen(cm.seed, (unsigned long long)(cm.sample_base + b0 + sb), step * 32ull + qq);
-        const float k = 2.3283064365386963e-10f;
-        s.m2[sb][qq * 4 + 0] = drop_scale(rr.x * k, cm.p_drop, keep, cm.training);
-        s.m2[sb][qq * 4 + 1] = drop_scale(rr.y * k, cm.p_drop, keep, cm.training);
-        s.m2[sb][qq * 4 + 2] = drop_scale(rr.z * k, cm.p_drop, keep, cm.training);
-        s.m2[sb][qq * 4 + 3] = drop_scale(rr.w * k, cm.p_drop, keep, cm.training);
-      }
-      tc::mbar_wait(&s.tmem_full[acc], (li >> 1) & 1);
-      tc::fence_after();
-      uint32_t v[32];
-      tc::tmem_ld32(tmem0 + acc * 32 + ((uint32_t)(q * 32) << 16), v);
-      tc::tmem_ld_wait();
-      tc::fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.tmem_empty[acc]);         // accumulator drained: the issuer may start tile + 2
-      tc::named_bar_sync(1, 128);                                 // m2 visible
+    tc::mbar_wait(&s.full[st], (it / C2F_NST) & 1);
+    float d[16];
 #pragma unroll
-      for (int co = 0; co < 20; ++co) s.stage[srow][co] = (__uint_as_float(v[co]) + s.bias[co]) * s.m2[bl][co];
-      tc::named_bar_sync(1, 128);
+    for (int i = 0; i < 16; ++i) d[i] = 0.f;
+    const uint32_t img = tc::smem_u32(s.a[st]) + h * 8 * 384;
+    tc::wg_fence();
 #pragma unroll
-      for (int i = 0; i < 5; ++i) {
-        const int o = e + 128 * i, sb = o / 320, oo = o % 320, co = oo >> 4, cell = oo & 15;
-        const int p00 = sb * 64 + (2 * (cell >> 2)) * 8 + 2 * (cell & 3);
-        const float v0 = s.stage[p00][co], v1 = s.stage[p00 + 1][co], v2 = s.stage[p00 + 8][co], v3 = s.stage[p00 + 9][co];
-        float m = v0; int arg = 0;
-        if (v1 > m) { m = v1; arg = 1; }
-        if (v2 > m) { m = v2; arg = 2; }
-        if (v3 > m) { m = v3; arg = 3; }
-        if (b0 + sb < cm.B) {
-          P2[(size_t)(b0 + sb) * 320 + oo] = __float2bfloat16(fmaxf(m, 0.f));
-          A2[(size_t)(b0 + sb) * 320 + oo] = (unsigned char)(arg | (m > 0.f ? 0 : 4));
-        }
+    for (int tap = 0; tap < 25; ++tap) {
+      const int ky = tap / 5, kx = tap - ky * 5;
+      const uint64_t ad = tc::smem_desc(img + ky * 768 + kx * 32, 16, /*SBO: next (oy, b) row group*/ 384, tc::kSw32);
+      const uint64_t bd = tc::smem_desc(tc::smem_u32(s.w[tap >> 2]) + (tap & 3) * 32, 16, 1024, tc::kSw128);
+      tc::mma<32>(d, ad, bd, tap > 0 ? 1u : 0u);
+    }
+    tc::wg_commit();
+    tc::wg_wait_all();
+    tc::acc_fence<16>(d);
+    tc::mbar_arrive(&s.empty[st]);                              // image consumed: the producer may refill the stage
+    tc::named_bar_sync(1, 256);                                 // m2 visible; the previous tile's pooling is done
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int r = h * 64 + tc::acc_row(t, i), co = tc::acc_col(t, i);   // accumulator row = (oy*2 + b)*8 + ox
+      const int bl = (r >> 3) & 1, srow = bl * 64 + (r >> 4) * 8 + (r & 7); // staging row = b*64 + oy*8 + ox
+      if (co < 20) s.stage[srow][co] = (d[i] + s.bias[co]) * s.m2[bl][co];
+    }
+    tc::named_bar_sync(1, 256);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      const int o = e + 256 * i;
+      if (o >= 640) break;
+      const int sb = o / 320, oo = o % 320, co = oo >> 4, cell = oo & 15;
+      const int p00 = sb * 64 + (2 * (cell >> 2)) * 8 + 2 * (cell & 3);
+      const float v0 = s.stage[p00][co], v1 = s.stage[p00 + 1][co], v2 = s.stage[p00 + 8][co], v3 = s.stage[p00 + 9][co];
+      float m = v0; int arg = 0;
+      if (v1 > m) { m = v1; arg = 1; }
+      if (v2 > m) { m = v2; arg = 2; }
+      if (v3 > m) { m = v3; arg = 3; }
+      if (b0 + sb < cm.B) {
+        P2[(size_t)(b0 + sb) * 320 + oo] = __float2bfloat16(fmaxf(m, 0.f));
+        A2[(size_t)(b0 + sb) * 320 + oo] = (unsigned char)(arg | (m > 0.f ? 0 : 4));
       }
     }
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 1) { tc::fence_after(); tc::tmem_dealloc<64>(tmem0); }
 }
 
 // =====================================================================================================================
 // head: dropout(relu(fc1)) -> fc2 -> log_softmax -> nll, and the backward of all of it down to dH.  One thread per sample.
-// Hrelu [B,64] fp32 = relu(fc1 + b3) comes from the tcgen05 GEMM.
+// Hrelu [B,64] fp32 = relu(fc1 + b3) comes from the wgmma GEMM.
 // =====================================================================================================================
 __global__ void __launch_bounds__(128) bt_head(const float* __restrict__ params, const float* __restrict__ Hrelu,
                                                const long long* __restrict__ target, Common cm, int backward, float inv_bsz,
@@ -439,48 +421,42 @@ __global__ void __launch_bounds__(256) bt_route(const __nv_bfloat16* __restrict_
 }
 
 // =====================================================================================================================
-// conv2 weight gradient on tcgen05:  D[(tap, ci), co] = sum_{b, pos} P1[b, ci, oy+ky, ox+kx] * dC[b, co, pos]
+// conv2 weight gradient on wgmma:  D[(tap, ci), co] = sum_{b, pos} P1[b, ci, oy+ky, ox+kx] * dC[b, co, pos]
 // K = the 64 output positions of one sample.  A: the 25 TMA tap boxes [64 pos][16 ci] (32-byte rows, 32B swizzle) read
-// MN-major -- one instruction spans 8 taps (M = 128, atoms of 16 channels LBO = one tap tile apart).  B: the 32 channel rows of
+// MN-major, atoms of 16 channels LBO apart.  B: the 32 channel rows of
 // dC, K-major.  Input channel 10 of P1 is a constant 1 => row (tap 0, ci 10) is the bias gradient.
 // =====================================================================================================================
 // One TMA box per sample brings its 12x12x16 input into shared memory as [y][x][c]; for each kernel row ky ONE instruction
 // covers the kernel columns kx = 0..7 x 16 channels as 8 MN-major atoms 32 bytes apart (atoms 5..7 read the pixels to the
 // right of the window: finite values whose output rows are never read), K = 16 output positions = two rows of the image.
-// 5 accumulators (one per ky) of [128 x 32].  Validated by scripts/tc_probe_matrix.py (umma_window_wgrad_*).
+// 5 accumulators (one per ky) of [128 x 32], split over two warpgroups.  Checked by tests/test_gpu_tc_probe.py.
 constexpr int WG_NST = 8;
 constexpr int WG_IMG = 5120;                          // 4608-byte image + padding the out-of-window atoms may read
 constexpr int WG_STAGE = WG_IMG + 4096;               // + dC [32 co][64 pos]
 struct __align__(1024) WgSmem {
   uint8_t st[WG_NST][WG_STAGE];
-  uint64_t full[WG_NST], empty[WG_NST], done;
-  uint32_t tmem_base;
+  uint64_t full[WG_NST], empty[WG_NST];
 };
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(BT_THREADS, 1)
 bt_conv2_wgrad(const __grid_constant__ CUtensorMap map_p1, const __grid_constant__ CUtensorMap map_dc, int B,
                float* __restrict__ grads) {
   extern __shared__ uint8_t smem_raw[];
   WgSmem& s = *reinterpret_cast<WgSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   for (int stg = 0; stg < WG_NST; ++stg)               // padding behind each image: finite (zero) forever
-    for (int i = threadIdx.x; i < (WG_IMG - 4608) / 16; i += 192)
+    for (int i = threadIdx.x; i < (WG_IMG - 4608) / 16; i += BT_THREADS)
       reinterpret_cast<uint4*>(s.st[stg] + 4608)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (threadIdx.x == 0) {
     tc::prefetch_tmap(&map_p1); tc::prefetch_tmap(&map_dc);
-    for (int i = 0; i < WG_NST; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 1); }
-    tc::mbar_init(&s.done, 1);
+    for (int i = 0; i < WG_NST; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 256); }
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc<256>(&s.tmem_base);
   tc::fence_proxy_async();
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem0 = s.tmem_base;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (t == 0) {
       uint32_t it = 0;
       for (int b = blockIdx.x; b < B; b += gridDim.x, ++it) {
         const int st = it % WG_NST;
@@ -490,200 +466,155 @@ bt_conv2_wgrad(const __grid_constant__ CUtensorMap map_p1, const __grid_constant
         tc::tma_load_2d(s.st[st] + WG_IMG, &map_dc, &s.full[st], 0, 32 * b);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::idesc_bf16_major(128, 32, 1, 0);
-      uint32_t it = 0;
-      for (int b = blockIdx.x; b < B; b += gridDim.x, ++it) {
-        const int st = it % WG_NST;
-        tc::mbar_wait(&s.full[st], (it / WG_NST) & 1);
-        tc::fence_after();
-        const uint32_t img = tc::smem_u32(s.st[st]), d0 = img + WG_IMG;
+    return;
+  }
+  // warpgroup h: accumulator rows 64h.. = kernel columns kx = 4h..4h+3 (atoms 32 bytes apart: start + 4h * 32)
+  const int h = wg - 1;
+  float acc[5][16];
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t bd = tc::smem_desc(d0 + ks * 32, 16, 1024, 2);
-          const uint32_t accf = (it > 0 || ks > 0) ? 1u : 0u;
+  for (int ky = 0; ky < 5; ++ky)
 #pragma unroll
-          for (int ky = 0; ky < 5; ++ky)
-            tc::umma_bf16(tmem0 + ky * 32, tc::smem_desc(img + ky * 384 + ks * 768, /*LBO: next kx*/ 32, /*SBO: next image row*/ 384, 6),
-                          bd, idesc, accf);
-        }
-        tc::commit(&s.empty[st]);
-      }
-      tc::commit(&s.done);
+    for (int i = 0; i < 16; ++i) acc[ky][i] = 0.f;
+  uint32_t it = 0;
+  for (int b = blockIdx.x; b < B; b += gridDim.x, ++it) {
+    const int st = it % WG_NST;
+    tc::mbar_wait(&s.full[st], (it / WG_NST) & 1);
+    const uint32_t img = tc::smem_u32(s.st[st]), d0 = img + WG_IMG;
+    tc::wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t bd = tc::smem_desc(d0 + ks * 32, 16, 1024, tc::kSw128);
+#pragma unroll
+      for (int ky = 0; ky < 5; ++ky)
+        tc::mma<32>(acc[ky], tc::smem_desc(img + h * 128 + ky * 384 + ks * 768, /*LBO: next kx*/ 32, /*SBO: next image row*/ 384, tc::kSw32),
+                    bd, 1u, /*A MN-major*/ 1u);
     }
-    __syncwarp();
-  } else {
-    const int q = warp & 3;
-    tc::mbar_wait(&s.done, 0);
-    tc::fence_after();
-    const int row = q * 32 + lane, kx = row >> 4, ci = row & 15;   // accumulator row = kx*16 + ci
-#pragma unroll 1
-    for (int ky = 0; ky < 5; ++ky) {
-      uint32_t v[32];
-      tc::tmem_ld32(tmem0 + ky * 32 + ((uint32_t)(q * 32) << 16), v);
-      tc::tmem_ld_wait();
-      if (kx < 5 && ci < 10) {
+    tc::wg_commit();
+    tc::wg_wait_all();
 #pragma unroll
-        for (int co = 0; co < 20; ++co) atomicAdd(grads + W2 + co * 250 + ci * 25 + ky * 5 + kx, __uint_as_float(v[co]));
-      } else if (ky == 0 && kx == 0 && ci == 10) {
+    for (int ky = 0; ky < 5; ++ky) tc::acc_fence<16>(acc[ky]);
+    tc::mbar_arrive(&s.empty[st]);
+  }
 #pragma unroll
-        for (int co = 0; co < 20; ++co) atomicAdd(grads + B2 + co, __uint_as_float(v[co]));
-      }
+  for (int ky = 0; ky < 5; ++ky) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int row = h * 64 + tc::acc_row(t, i), kx = row >> 4, ci = row & 15, co = tc::acc_col(t, i);   // row = kx*16 + ci
+      if (co >= 20) continue;
+      if (kx < 5 && ci < 10) atomicAdd(grads + W2 + co * 250 + ci * 25 + ky * 5 + kx, acc[ky][i]);
+      else if (ky == 0 && kx == 0 && ci == 10) atomicAdd(grads + B2 + co, acc[ky][i]);
     }
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 1) { tc::fence_after(); tc::tmem_dealloc<256>(tmem0); }
 }
 
 // =====================================================================================================================
-// conv2 data gradient on tcgen05 + col2im + relu/pool backward of conv1:
+// conv2 data gradient on wgmma + col2im + relu/pool backward of conv1:
 //   dA[(b, pos), (tap, ci)] = sum_co dC[b, co, pos] * W2[co, ci, tap]         M = 128 (2 samples), N = 400, K = 32
 //   dP1[b, ci, y, x] = sum_{ky,kx} dA[(b, (y-ky, x-kx)), (ky*5+kx, ci)]       gathered from a bf16 staging tile
 //   G1 = dP1 masked by relu(conv1-pool) > 0                                    fp32 [B,10,144]
 // =====================================================================================================================
 constexpr int DG_ROW = 816;                            // staging row stride in bytes (conflict-free for 16-byte accesses)
+constexpr int DG_NC = 80;                              // N = 400 as 5 instructions of N = 80 (40 accumulator registers)
 struct __align__(1024) DgSmem {
   uint8_t w[W2R_N * 128];                              // W2R [400 rows (tap, ci)][64 k (co)] K-major
   uint8_t a[2][8192];                                  // dC of 2 samples: [b][32 co][64 pos] = MN-major A (K = co)
   uint8_t stg[128 * DG_ROW];
-  uint64_t full[2], empty[2], wfull, acc_full, acc_empty;
-  uint32_t tmem_base;
+  uint64_t full[2], empty[2], wfull;
 };
 
-constexpr int DG_THREADS = 320;      // warp 0: TMA producer, warp 1: MMA issuer, warps 2..9: epilogue (two warps per TMEM lane quadrant)
-__global__ void __launch_bounds__(DG_THREADS, 1)
+__global__ void __launch_bounds__(BT_THREADS, 1)
 bt_conv2_dgrad(const __grid_constant__ CUtensorMap map_dc, const __grid_constant__ CUtensorMap map_w2r, int B,
                const unsigned char* __restrict__ A1, float* __restrict__ G1) {
   extern __shared__ uint8_t smem_raw[];
   DgSmem& s = *reinterpret_cast<DgSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int tiles = (B + 1) / 2;
   if (threadIdx.x == 0) {
     tc::prefetch_tmap(&map_dc); tc::prefetch_tmap(&map_w2r);
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 1); }
-    tc::mbar_init(&s.wfull, 1); tc::mbar_init(&s.acc_full, 1); tc::mbar_init(&s.acc_empty, 8);
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 256); }
+    tc::mbar_init(&s.wfull, 1);
     tc::mbar_fence_init();
   }
-  if (warp == 1) tc::tmem_alloc<512>(&s.tmem_base);
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem0 = s.tmem_base;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (t == 0) {
       tc::mbar_expect_tx(&s.wfull, W2R_N * 128);
       tc::tma_load_2d(s.w, &map_w2r, &s.wfull, 0, 0);
       tc::tma_load_2d(s.w + 200 * 128, &map_w2r, &s.wfull, 0, 200);
       uint32_t it = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
+      for (int tt = blockIdx.x; tt < tiles; tt += gridDim.x, ++it) {
         const int st = it & 1;
         tc::mbar_wait(&s.empty[st], ((it >> 1) & 1) ^ 1);
         tc::mbar_expect_tx(&s.full[st], 8192);
-        tc::tma_load_2d(s.a[st], &map_dc, &s.full[st], 0, 64 * t);
+        tc::tma_load_2d(s.a[st], &map_dc, &s.full[st], 0, 64 * tt);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t id208 = tc::idesc_bf16_major(128, 208, 1, 0), id192 = tc::idesc_bf16_major(128, 192, 1, 0);
-      tc::mbar_wait(&s.wfull, 0);
-      uint32_t it = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
-        const int st = it & 1;
-        tc::mbar_wait(&s.acc_empty, (it & 1) ^ 1);                 // epilogue drained the (single) accumulator
-        tc::mbar_wait(&s.full[st], (it >> 1) & 1);
-        tc::fence_after();
-        const uint32_t a0 = tc::smem_u32(s.a[st]), w0 = tc::smem_u32(s.w);
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-          const uint64_t ad = tc::smem_desc(a0 + ks * 2048, /*LBO: next sample*/ 4096, 1024, 2);
-          tc::umma_bf16(tmem0, ad, tc::smem_desc(w0 + ks * 32, 16, 1024, 2), id208, ks);
-          tc::umma_bf16(tmem0 + 208, ad, tc::smem_desc(w0 + 208 * 128 + ks * 32, 16, 1024, 2), id192, ks);
-        }
-        tc::commit(&s.empty[st]);
-        tc::commit(&s.acc_full);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int q = warp & 3, e = (warp - 2) * 32 + lane;            // e: 0..255
-    const int half = (warp - 2) >> 2;                              // warps 2..5 drain columns 0..191, warps 6..9 columns 192..399
-    const int r = q * 32 + lane;
-    uint32_t it = 0;
-    for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++it) {
-      const int b0 = 2 * t;
-      tc::mbar_wait(&s.acc_full, it & 1);
-      tc::fence_after();
-      uint8_t* myrow = s.stg + r * DG_ROW;
+    return;
+  }
+  // warpgroup h: sample h of the tile = accumulator rows (positions) 0..63, staged as bf16 rows 64h..64h+63
+  const int h = wg - 1, e = threadIdx.x - 128;            // e: 0..255
+  tc::mbar_wait(&s.wfull, 0);
+  uint32_t it = 0;
+  for (int tt = blockIdx.x; tt < tiles; tt += gridDim.x, ++it) {
+    const int b0 = 2 * tt, st = it & 1;
+    tc::mbar_wait(&s.full[st], (it >> 1) & 1);
+    const uint32_t a0 = tc::smem_u32(s.a[st]) + h * 4096, w0 = tc::smem_u32(s.w);
 #pragma unroll 1
-      for (int c0 = half * 192; c0 < half * 192 + 192; c0 += 32) {
-        uint32_t v[32];
-        tc::tmem_ld32(tmem0 + (uint32_t)c0 + ((uint32_t)(q * 32) << 16), v);
-        tc::tmem_ld_wait();
+    for (int c0 = 0; c0 < W2R_N; c0 += DG_NC) {
+      float d[DG_NC / 2];
 #pragma unroll
-        for (int g = 0; g < 4; ++g)
-          *reinterpret_cast<uint4*>(myrow + c0 * 2 + g * 16) =
-              make_uint4(b2::pack_bf16x2(__uint_as_float(v[8 * g]), __uint_as_float(v[8 * g + 1])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 2]), __uint_as_float(v[8 * g + 3])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 4]), __uint_as_float(v[8 * g + 5])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 6]), __uint_as_float(v[8 * g + 7])));
+      for (int i = 0; i < DG_NC / 2; ++i) d[i] = 0.f;
+      tc::wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks)
+        tc::mma<DG_NC>(d, tc::smem_desc(a0 + ks * 2048, /*LBO: next sample*/ 4096, 1024, tc::kSw128),
+                       tc::smem_desc(w0 + c0 * 128 + ks * 32, 16, 1024, tc::kSw128), ks, /*A MN-major*/ 1u);
+      tc::wg_commit();
+      tc::wg_wait_all();
+      tc::acc_fence<DG_NC / 2>(d);
+#pragma unroll
+      for (int i = 0; i < DG_NC / 2; i += 2) {
+        const int row = h * 64 + tc::acc_row(t, i), col = c0 + tc::acc_col(t, i);
+        *reinterpret_cast<uint32_t*>(s.stg + row * DG_ROW + col * 2) = b2::pack_bf16x2(d[i], d[i + 1]);
       }
-      if (half == 1) {
-        uint32_t v[16];
-        tc::tmem_ld16(tmem0 + 384u + ((uint32_t)(q * 32) << 16), v);
-        tc::tmem_ld_wait();
+    }
+    tc::mbar_arrive(&s.empty[st]);
+    tc::named_bar_sync(1, 256);
+    // col2im gather: item = (sample in tile, y, x) of the 12 x 12 conv1 map
+    for (int item = e; item < 288; item += 256) {
+      const int sb = item / 144, p = item % 144, y = p / 12, x = p % 12;
+      float acc[10];
 #pragma unroll
-        for (int g = 0; g < 2; ++g)
-          *reinterpret_cast<uint4*>(myrow + 384 * 2 + g * 16) =
-              make_uint4(b2::pack_bf16x2(__uint_as_float(v[8 * g]), __uint_as_float(v[8 * g + 1])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 2]), __uint_as_float(v[8 * g + 3])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 4]), __uint_as_float(v[8 * g + 5])),
-                         b2::pack_bf16x2(__uint_as_float(v[8 * g + 6]), __uint_as_float(v[8 * g + 7])));
-      }
-      tc::fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&s.acc_empty);
-      tc::named_bar_sync(1, 256);
-      // col2im gather: item = (sample in tile, y, x) of the 12 x 12 conv1 map
-      for (int item = e; item < 288; item += 256) {
-        const int sb = item / 144, p = item % 144, y = p / 12, x = p % 12;
-        float acc[10];
+      for (int c = 0; c < 10; ++c) acc[c] = 0.f;
 #pragma unroll
-        for (int c = 0; c < 10; ++c) acc[c] = 0.f;
+      for (int ky = 0; ky < 5; ++ky) {
+        const int oy = y - ky;
+        if ((unsigned)oy < 8u) {
 #pragma unroll
-        for (int ky = 0; ky < 5; ++ky) {
-          const int oy = y - ky;
-          if ((unsigned)oy < 8u) {
-#pragma unroll
-            for (int kx = 0; kx < 5; ++kx) {
-              const int ox = x - kx;
-              if ((unsigned)ox < 8u) {
-                const uint8_t* src = s.stg + (sb * 64 + oy * 8 + ox) * DG_ROW + (ky * 5 + kx) * 32;
-                const uint4 u0 = *reinterpret_cast<const uint4*>(src);
-                const uint32_t u1 = *reinterpret_cast<const uint32_t*>(src + 16);
-                acc[0] += b2::bf16lo(u0.x); acc[1] += b2::bf16hi(u0.x); acc[2] += b2::bf16lo(u0.y); acc[3] += b2::bf16hi(u0.y);
-                acc[4] += b2::bf16lo(u0.z); acc[5] += b2::bf16hi(u0.z); acc[6] += b2::bf16lo(u0.w); acc[7] += b2::bf16hi(u0.w);
-                acc[8] += b2::bf16lo(u1); acc[9] += b2::bf16hi(u1);
-              }
+          for (int kx = 0; kx < 5; ++kx) {
+            const int ox = x - kx;
+            if ((unsigned)ox < 8u) {
+              const uint8_t* src = s.stg + (sb * 64 + oy * 8 + ox) * DG_ROW + (ky * 5 + kx) * 32;
+              const uint4 u0 = *reinterpret_cast<const uint4*>(src);
+              const uint32_t u1 = *reinterpret_cast<const uint32_t*>(src + 16);
+              acc[0] += b2::bf16lo(u0.x); acc[1] += b2::bf16hi(u0.x); acc[2] += b2::bf16lo(u0.y); acc[3] += b2::bf16hi(u0.y);
+              acc[4] += b2::bf16lo(u0.z); acc[5] += b2::bf16hi(u0.z); acc[6] += b2::bf16lo(u0.w); acc[7] += b2::bf16hi(u0.w);
+              acc[8] += b2::bf16lo(u1); acc[9] += b2::bf16hi(u1);
             }
           }
         }
-        if (b0 + sb < B) {
+      }
+      if (b0 + sb < B) {
 #pragma unroll
-          for (int c = 0; c < 10; ++c) {
-            const unsigned char code = __ldg(A1 + (size_t)(b0 + sb) * 1440 + c * 144 + p);
-            G1[(size_t)(b0 + sb) * 1440 + c * 144 + p] = (code & 4) ? 0.f : acc[c];
-          }
+        for (int c = 0; c < 10; ++c) {
+          const unsigned char code = __ldg(A1 + (size_t)(b0 + sb) * 1440 + c * 144 + p);
+          G1[(size_t)(b0 + sb) * 1440 + c * 144 + p] = (code & 4) ? 0.f : acc[c];
         }
       }
-      tc::named_bar_sync(1, 256);                                  // staging tile free for the next accumulator
     }
+    tc::named_bar_sync(1, 256);                                  // staging tile free for the next tile
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 1) { tc::fence_after(); tc::tmem_dealloc<512>(tmem0); }
 }
 
 // =====================================================================================================================
@@ -945,7 +876,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -1021,7 +952,7 @@ int b2_bt_step_launch(const float* params, float* grads, const void* x, int x_u8
   }
   if (stage_mask & 2) {
     const int tiles = (B + 1) / 2;
-    bt_conv2_fwd<<<tiles < sms ? tiles : sms, 192, sm_c2f, stream>>>(m_p1_2, m_w2k, params, cm, bf->P2, bf->A2);
+    bt_conv2_fwd<<<tiles < sms ? tiles : sms, BT_THREADS, sm_c2f, stream>>>(m_p1_2, m_w2k, params, cm, bf->P2, bf->A2);
     if (!ck("conv2_fwd")) return -4;
   }
   if (stage_mask & 4) {
@@ -1037,7 +968,7 @@ int b2_bt_step_launch(const float* params, float* grads, const void* x, int x_u8
   }
   // The four gradient kernels are independent after `route`.  Two branches (a side stream forked/joined with events; under
   // graph capture they become parallel graph branches):  main: conv2_dgrad -> conv1_wgrad    side: fc_wgrad -> conv2_wgrad
-  // The SIMT kernels (small shared memory) co-reside with the tensor-core kernels (one 170-180 KB CTA per SM).
+  // The SIMT kernels (small shared memory) co-reside with the tensor-core kernels (one CTA of up to ~175 KB per SM).
   static cudaStream_t side = nullptr;
   static cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   const bool overlap = (stage_mask & 255) == 255;
@@ -1049,18 +980,18 @@ int b2_bt_step_launch(const float* params, float* grads, const void* x, int x_u8
   cudaStream_t s2 = overlap ? side : stream;
   if (overlap) { cudaEventRecord(ev_fork, stream); cudaStreamWaitEvent(side, ev_fork, 0); }
   if (stage_mask & 128) {
-    const int per = B >= 148 * 32 ? (B + 147) / 148 : 32;            // ~one CTA per SM; >= 32 samples amortise the final atomics
+    const int per = B >= sms * 32 ? (B + sms - 1) / sms : 32;        // ~one CTA per SM; >= 32 samples amortise the final atomics
     const int ctas = (B + per - 1) / per;
     bt_fc_wgrad<<<ctas, 512, 0, s2>>>(bf->P2, bf->H, bf->DH, bf->DLOG, B, per, grads);
     if (!ck("fc_wgrad")) return -4;
   }
   if (stage_mask & 16) {
-    bt_conv2_wgrad<<<B < sms ? B : sms, 192, sm_wg, s2>>>(m_p1_1, m_dc32, B, grads);
+    bt_conv2_wgrad<<<B < sms ? B : sms, BT_THREADS, sm_wg, s2>>>(m_p1_1, m_dc32, B, grads);
     if (!ck("conv2_wgrad")) return -4;
   }
   if (stage_mask & 32) {
     const int tiles = (B + 1) / 2;
-    bt_conv2_dgrad<<<tiles < sms ? tiles : sms, DG_THREADS, sm_dg, stream>>>(m_dc64, m_w2r, B, bf->A1, bf->G1);
+    bt_conv2_dgrad<<<tiles < sms ? tiles : sms, BT_THREADS, sm_dg, stream>>>(m_dc64, m_w2r, B, bf->A1, bf->G1);
     if (!ck("conv2_dgrad")) return -4;
   }
   if (stage_mask & 64) {

@@ -1,7 +1,7 @@
 // Fused MNIST-ConvNet training step, ONE THREAD-BLOCK CLUSTER PER SAMPLE (strong-scaling variant of convnet.cu).
 //
 // The reference keeps the global batch at 128 (`bsz = 128 // world_size`, train_dist.py:85), so with N GPUs each GPU
-// only has 128/N samples: one CTA per sample (convnet.cu) leaves most of the 148 SMs idle and the step time is the
+// only has 128/N samples: one CTA per sample (convnet.cu) leaves most of the SMs idle and the step time is the
 // latency of a single sample (~30 us) no matter how many GPUs are used.  Here a sample is carried by a cluster of C CTAs
 // (C = 2, 4, 8 on as many SMs): every phase of the forward/backward pass is split C ways, the small activations every CTA
 // needs next (pooled conv outputs, fc1 activations, their gradients) are broadcast into all peers' shared memory with
@@ -499,7 +499,7 @@ __global__ void __launch_bounds__(T, 1) convnet_cluster_kernel(Args a) {
 
   // ------------------------------------------------------------------ flush: only the gradient slices this CTA owns
   __syncthreads();                                 // S8 of the last sample wrote s.g[W1..], s.g[B1..] from other warps (barrier (6) is
-                                                   // skipped after the last sample; racecheck: profiles/sanitize/r2_det_diag.txt)
+                                                   // skipped after the last sample; found by racecheck)
   if (a.backward && cluster_id < a.B) {
     float* gdst = a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride;
     if (a.det_partials != nullptr) {               // deterministic mode: whole private slot per CTA (zeros outside its slices)

@@ -14,8 +14,8 @@
 // Chunk pipeline (the default when the loader ring is deep enough: num_slots >= 3K): K consecutive steps are issued together,
 //   copy stream    : K cudaMemcpyAsync H2D        (that step's pinned loader slot -> device block g*K + j), then ONE event
 //   compute stream : ONE graph of the K steps' kernels (a pure kernel chain: programmatic dependent launch stays intact across
-//                    the K steps -- round 1's chunk graph had an H2D -> kernel edge in front of every step, which cost as
-//                    much as a graph boundary, profiles/executor_chunk_graphs.json); captured once at construction
+//                    the K steps -- an H2D -> kernel edge in front of every step would cost as much as a graph
+//                    boundary); captured once at construction
 //   d2h stream     : K cudaMemcpyAsync D2H        (the cumulative loss after each step, snapshotted on the device by that
 //                    step's optimizer tail into loss_hist[g*K + j] -> the step's pinned loss word)
 // ordered by three events per chunk.  Chunk c+1's copies run while chunk c computes (two device block groups g), chunk
@@ -106,9 +106,7 @@ StepExecutor::StepExecutor(const StepConfig& cfg, NativeLoader* loader, int max_
   }
   {
     // flag mode of the per-slot ring path: no cross-stream events at all (see run()); needs the stream memory operations.
-    // Opt-in (B200DIST_EXEC_FLAGS=1): measured NOT faster than the event path (profiles/e2e/executor_flag_mode_r2.json:
-    // 3.55 / 3.28 M vs 3.69 M samples/s at 20 steps, 3.96 M vs 4.06 M at 400) -- the event waits were not what separates
-    // the stream-launched steps (32 us) from the graph-replayed ones (28 us).
+    // Opt-in (B200DIST_EXEC_FLAGS=1): an alternative to the event path, not the default.
     const char* e = getenv("B200DIST_EXEC_FLAGS");
     flags_ = (e != nullptr && e[0] == '1') && direct_ && cfg_.ring_base > 0 && cfg_.flags != nullptr && !cfg_.fused_tail &&
              cfg_.loss_hist != nullptr && p_write32() != nullptr && p_wait32() != nullptr;
@@ -454,8 +452,8 @@ int64_t StepExecutor::run(int64_t max_steps, int* pending_slot, int64_t* pending
     cudaMemcpyAsync(cfg_.in_dev[p], loader_->slot(slot).x, loader_->block_bytes(), cudaMemcpyHostToDevice, copy_);
     cudaEventRecord(copied_[p], copy_);
     // kernels.  direct mode (default): plain stream launches with the programmatic-dependent-launch attribute -- the steps
-    // chain on the device exactly as inside one long graph (a graph launch per step costs ~3 us of device time at every
-    // boundary: 31 vs 28 us per step, profiles/e2e/executor_variants_r2.json); graph mode: one 2-kernel graph per step.
+    // chain on the device exactly as inside one long graph (a graph launch per step costs device time at every
+    // boundary); graph mode: one 2-kernel graph per step.
     cudaStreamWaitEvent(compute_, copied_[p], 0);
     float* snap = cfg_.loss_hist != nullptr ? cfg_.loss_hist + 2 * p : nullptr;
     if (snap != nullptr) cudaStreamWaitEvent(compute_, loss_read_[p], 0);   // snapshot slot p was read back (two steps ago)

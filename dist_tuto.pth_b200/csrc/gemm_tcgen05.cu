@@ -1,15 +1,14 @@
-// bf16 GEMM on the 5th-generation tensor cores (sm_100a), hand-written:
-//   C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]) (ReLU)      A, B bf16 K-contiguous; fp32 accumulation in TMEM
+// bf16 GEMM on the Hopper tensor cores (sm_90a), hand-written:
+//   C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]) (ReLU)      A, B bf16 K-contiguous; fp32 accumulation in registers
 //
 // This is the linear-layer engine of the framework (fc1/fc2 of the tutorial Net at large batch,
 // ResNet-18's classifier, and the implicit-GEMM convolutions built on top of it):
-//   warp 0      : TMA producer   -- cp.async.bulk.tensor.2d (128B-swizzled tiles) into a 4-stage smem ring
-//   warp 1      : MMA issuer     -- one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (UMMA 128xBNx16),
-//                                   tcgen05.commit releases smem stages / signals the epilogue
-//   warps 2..5  : epilogue       -- tcgen05.ld (32 lanes x 32b, one accumulator row per thread) -> bias/ReLU ->
-//                                   bf16/fp32 -> 16-byte global stores
-// Synchronisation is mbarrier-only (full/empty per stage, one "accumulator ready" barrier).  Ragged M/N/K
-// edges are handled by TMA out-of-bounds zero fill and predicated stores.
+//   warpgroup 0     : TMA producer  -- one thread issues cp.async.bulk.tensor.2d (128B-swizzled tiles) into a smem ring
+//   warpgroups 1, 2 : consumers     -- wgmma.mma_async m64nBNk16 on rows 0..63 / 64..127 of the 128-row tile, then
+//                                      bias/ReLU -> bf16/fp32 -> global stores straight from the accumulator registers
+// Large GEMMs (N >= 192, K >= 2048, at least one wave of tiles) take a persistent kernel with 128x256 tiles instead.
+// Synchronisation is mbarrier-only (full/empty per stage).  Ragged M/N/K edges are handled by TMA out-of-bounds zero fill
+// and predicated stores.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -20,431 +19,164 @@
 #include <mutex>
 #include <string>
 
+#include "tc_common.cuh"
+
 namespace gemm {
 
 constexpr int BM = 128, BK = 64;
-// stages sized so that TWO CTAs fit per SM (<= ~113 KB each): one CTA's epilogue/prologue overlaps the other's mainloop
+// stages: the TMA ring runs up to STAGES k-blocks ahead of the MMAs
 template <int BN> struct Cfg { static constexpr int STAGES = BN >= 128 ? 3 : 4; };
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major, 128B-swizzled operand tile: rows of 64 bf16 (128 B); 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address  [0,14)
-  d |= (uint64_t)1 << 16;                            // LBO (unused for swizzled K-major) [16,30)
-  d |= (uint64_t)(1024 >> 4) << 32;                  // SBO = 1024 B   [32,46)
-  d |= (uint64_t)1 << 46;                            // descriptor version 1 (Blackwell)
-  d |= (uint64_t)2 << 61;                            // SWIZZLE_128B
-  return d;
-}
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M x N tile
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
+// One warpgroup's share (64 rows) of a 128 x BN tile: K loop over the smem ring.  The MMAs of k-block kb run while the
+// warpgroup waits for k-block kb+1; a stage is released once the MMAs reading it have completed.  `it` is the running
+// k-block counter that selects stage and phase (it continues across the tiles of a persistent CTA).
+template <int BN, int STAGES>
+__device__ __forceinline__ uint32_t mma_tile(float* d, const uint8_t* a_ring, const uint8_t* b_ring, uint64_t* full,
+                                             uint64_t* empty, int half, int num_kb, uint32_t it) {
+  constexpr uint32_t kABytes = BM * BK * 2, kBBytes = BN * BK * 2;
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb, ++it) {
+    const uint32_t st = it % STAGES;
+    tc::mbar_wait(&full[st], (it / STAGES) & 1);
+    const uint32_t a_addr = tc::smem_u32(a_ring) + st * kABytes + half * 64 * 128, b_addr = tc::smem_u32(b_ring) + st * kBBytes;
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)                    // +16 bf16 = 32 B inside the 128 B swizzle row
+      tc::mma<BN>(d, tc::smem_desc_sw128(a_addr + k * 32), tc::smem_desc_sw128(b_addr + k * 32), 1u);
+    tc::wg_commit();
+    tc::wg_wait_1();                                     // k-block kb-1 done: its stage is free
+    if (kb > 0) tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+  }
+  tc::wg_wait_all();
+  tc::acc_fence<BN / 2>(d);
+  tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+  return it;
 }
 
+// bias / ReLU / bf16 or fp32 stores straight from the accumulator registers of one warpgroup (rows row0..row0+63)
 template <int BN>
+__device__ __forceinline__ void store_tile(const float* d, int t, int row0, int n0, void* __restrict__ c,
+                                           const float* __restrict__ bias, int M, int N, int relu, int out_bf16) {
+  const bool pairs = (N % 2) == 0;
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const int row = row0 + tc::acc_row(t, i), col = n0 + tc::acc_col(t, i);
+    if (row >= M || col >= N) continue;
+    float v0 = d[i], v1 = d[i + 1];
+    if (bias != nullptr) {
+      v0 += __ldg(bias + col);
+      if (col + 1 < N) v1 += __ldg(bias + col + 1);
+    }
+    if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+    if (out_bf16) {
+      __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(c) + (size_t)row * N + col;
+      if (pairs) *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+      else { dst[0] = __float2bfloat16(v0); if (col + 1 < N) dst[1] = __float2bfloat16(v1); }
+    } else {
+      float* dst = reinterpret_cast<float*>(c) + (size_t)row * N + col;
+      if (pairs) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+      else { dst[0] = v0; if (col + 1 < N) dst[1] = v1; }
+    }
+  }
+}
+
+template <int BN, int STAGES>
 struct SmemLayout {
-  static constexpr int STAGES = Cfg<BN>::STAGES;
   alignas(1024) uint8_t a[STAGES][BM * BK * 2];
   alignas(1024) uint8_t b[STAGES][BN * BK * 2];
   alignas(8) uint64_t full[STAGES];
   alignas(8) uint64_t empty[STAGES];
-  alignas(8) uint64_t accum_ready;
-  uint32_t tmem_base;
 };
+
+template <int BN, int STAGES>
+__device__ __forceinline__ void init_ring(SmemLayout<BN, STAGES>& s, const CUtensorMap* map_a, const CUtensorMap* map_b) {
+  if (threadIdx.x == 0) {
+    tc::prefetch_tmap(map_a);
+    tc::prefetch_tmap(map_b);
+    for (int i = 0; i < STAGES; ++i) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 2 * 128); }
+    tc::mbar_fence_init();
+  }
+  __syncthreads();
+}
 
 template <int BN>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, void* __restrict__ c,
                  const float* __restrict__ bias, int M, int N, int K, int relu, int out_bf16) {
+  constexpr int STAGES = Cfg<BN>::STAGES;
+  using Smem = SmemLayout<BN, STAGES>;
   extern __shared__ uint8_t smem_raw[];
-  SmemLayout<BN>& s = *reinterpret_cast<SmemLayout<BN>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int num_kb = (K + BK - 1) / BK;
-  constexpr int STAGES = Cfg<BN>::STAGES;
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;       // power of two >= 32
-  constexpr uint32_t kStageBytes = (BM + BN) * BK * 2;
+  init_ring(s, &map_a, &map_b);
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 1); }
-    mbar_init(&s.accum_ready, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {   // TMEM allocation is warp-collective; the allocating warp also frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s.tmem_base)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_acc = s.tmem_base;
-
-  if (warp == 0) {
+  if (wg == 0) {
     // ======================================================== TMA producer
-    if (lane == 0) {
+    if (t == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
         const int st = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&s.empty[st], ph ^ 1);                 // first pass: parity 1 passes on a fresh barrier
-        mbar_expect_tx(&s.full[st], kStageBytes);
-        tma_load_2d(s.a[st], &map_a, &s.full[st], kb * BK, m0);
-        tma_load_2d(s.b[st], &map_b, &s.full[st], kb * BK, n0);
+        tc::mbar_wait(&s.empty[st], ((kb / STAGES) & 1) ^ 1);   // first pass: parity 1 passes on a fresh barrier
+        tc::mbar_expect_tx(&s.full[st], (BM + BN) * BK * 2);
+        tc::tma_load_2d(s.a[st], &map_a, &s.full[st], kb * BK, m0);
+        tc::tma_load_2d(s.b[st], &map_b, &s.full[st], kb * BK, n0);
       }
     }
-  } else if (warp == 1) {
-    // ======================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BM, BN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int st = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&s.full[st], ph);
-        tcgen05_fence_after();
-        const uint32_t a_addr = smem_u32(s.a[st]), b_addr = smem_u32(s.b[st]);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t ad = make_smem_desc(a_addr + k * 32);   // +16 bf16 = 32 B inside the 128 B swizzle row
-          const uint64_t bd = make_smem_desc(b_addr + k * 32);
-          umma_bf16(tmem_acc, ad, bd, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        tcgen05_commit(&s.empty[st]);                     // smem stage reusable once these MMAs retire
-      }
-      tcgen05_commit(&s.accum_ready);                     // accumulator complete
-    }
-    __syncwarp();
-  } else {
-    // ======================================================== epilogue (warps 2..5 -> TMEM lane quadrants 2,3,0,1)
-    const int q = warp & 3;
-    mbar_wait(&s.accum_ready, 0);
-    tcgen05_fence_after();
-    const int row = m0 + q * 32 + lane;
-#pragma unroll
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      uint32_t r[16];
-      tmem_ld16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (row < M) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = n0 + c0 + i;
-          float x = __uint_as_float(r[i]);
-          if (bias != nullptr && col < N) x += __ldg(bias + col);
-          if (relu) x = fmaxf(x, 0.f);
-          v[i] = x;
-        }
-        const int colb = n0 + c0;
-        if (out_bf16) {
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(c) + (size_t)row * N + colb;
-          if (colb + 16 <= N && (N % 8) == 0) {
-            uint4 p0, p1;
-            __nv_bfloat162 t;
-            t = __floats2bfloat162_rn(v[0], v[1]);   p0.x = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[2], v[3]);   p0.y = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[4], v[5]);   p0.z = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[6], v[7]);   p0.w = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[8], v[9]);   p1.x = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[10], v[11]); p1.y = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[12], v[13]); p1.z = *reinterpret_cast<uint32_t*>(&t);
-            t = __floats2bfloat162_rn(v[14], v[15]); p1.w = *reinterpret_cast<uint32_t*>(&t);
-            reinterpret_cast<uint4*>(dst)[0] = p0;
-            reinterpret_cast<uint4*>(dst)[1] = p1;
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (colb + i < N) dst[i] = __float2bfloat16(v[i]);
-          }
-        } else {
-          float* dst = reinterpret_cast<float*>(c) + (size_t)row * N + colb;
-          if (colb + 16 <= N && (N % 4) == 0) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) reinterpret_cast<float4*>(dst)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (colb + i < N) dst[i] = v[i];
-          }
-        }
-      }
-    }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "r"(kTmemCols) : "memory");
-  }
+  // ========================================================== consumers: warpgroup 1 -> rows 0..63, 2 -> rows 64..127
+  const int half = wg - 1;
+  float d[BN / 2];
+  mma_tile<BN, STAGES>(d, &s.a[0][0], &s.b[0][0], s.full, s.empty, half, num_kb, 0u);
+  store_tile<BN>(d, t, m0 + half * 64, n0, c, bias, M, N, relu, out_bf16);
 }
-
 
 // ------------------------------------------------------------------------------------------ persistent 128x256 kernel
-// Large GEMMs: one CTA per SM loops over output tiles; 128x256 tiles halve the operand bytes per FLOP relative to
-// 128x128 (the L2->SM path is the bound at this size), and TWO TMEM accumulators (2 x 256 columns) let the epilogue of
-// tile i overlap the mainloop of tile i+1.
+// Large GEMMs: one CTA per SM loops over output tiles; 128x256 tiles halve the operand bytes per FLOP relative to 128x128,
+// and the producer keeps the 4-stage ring filled with the next tile's k-blocks while the consumers run the epilogue of
+// the current one.  Each consumer warpgroup holds a 64x256 fp32 accumulator (128 registers per thread): the producer
+// warpgroup hands most of its register budget to them (setmaxnreg).
 constexpr int PBN = 256, PSTAGES = 4;
-struct PSmem {
-  alignas(1024) uint8_t a[PSTAGES][BM * BK * 2];
-  alignas(1024) uint8_t b[PSTAGES][PBN * BK * 2];
-  alignas(8) uint64_t full[PSTAGES];
-  alignas(8) uint64_t empty[PSTAGES];
-  alignas(8) uint64_t tmem_full[2];
-  alignas(8) uint64_t tmem_empty[2];
-  uint32_t tmem_base;
-};
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
+using PSmem = SmemLayout<PBN, PSTAGES>;
 
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                             void* __restrict__ c, const float* __restrict__ bias, int M, int N, int K, int relu, int out_bf16) {
   extern __shared__ uint8_t smem_raw[];
   PSmem& s = *reinterpret_cast<PSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int mt = (M + BM - 1) / BM, nt = (N + PBN - 1) / PBN, tiles = mt * nt;
   const int num_kb = (K + BK - 1) / BK;
-  constexpr uint32_t kStageBytes = (BM + PBN) * BK * 2;
+  init_ring(s, &map_a, &map_b);
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    for (int i = 0; i < PSTAGES; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s.tmem_full[i], 1); mbar_init(&s.tmem_empty[i], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s.tmem_base)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem0 = s.tmem_base;
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    tc::regs_dec<40>();
+    if (t == 0) {
       uint32_t it = 0;                                          // global k-block counter -> stage / phase
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-        const int m0 = (t % mt) * BM, n0 = (t / mt) * PBN;      // consecutive CTAs share the B (N) panel
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile % mt) * BM, n0 = (tile / mt) * PBN;   // consecutive CTAs share the B (N) panel
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int st = it % PSTAGES;
-          mbar_wait(&s.empty[st], ((it / PSTAGES) & 1) ^ 1);
-          mbar_expect_tx(&s.full[st], kStageBytes);
-          tma_load_2d(s.a[st], &map_a, &s.full[st], kb * BK, m0);
-          tma_load_2d(s.b[st], &map_b, &s.full[st], kb * BK, n0);
+          tc::mbar_wait(&s.empty[st], ((it / PSTAGES) & 1) ^ 1);
+          tc::mbar_expect_tx(&s.full[st], (BM + PBN) * BK * 2);
+          tc::tma_load_2d(s.a[st], &map_a, &s.full[st], kb * BK, m0);
+          tc::tma_load_2d(s.b[st], &map_b, &s.full[st], kb * BK, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BM, PBN);
-      uint32_t it = 0, li = 0;
-      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++li) {
-        const uint32_t acc = li & 1;
-        mbar_wait(&s.tmem_empty[acc], ((li >> 1) & 1) ^ 1);      // epilogue has drained this accumulator
-        tcgen05_fence_after();
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int st = it % PSTAGES;
-          mbar_wait(&s.full[st], (it / PSTAGES) & 1);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(s.a[st]), b_addr = smem_u32(s.b[st]);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16(tmem0 + acc * PBN, make_smem_desc(a_addr + k * 32), make_smem_desc(b_addr + k * 32), idesc,
-                      (kb > 0 || k > 0) ? 1u : 0u);
-          tcgen05_commit(&s.empty[st]);
-        }
-        tcgen05_commit(&s.tmem_full[acc]);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int q = warp & 3;
-    uint32_t li = 0;
-    for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++li) {
-      const uint32_t acc = li & 1;
-      const int m0 = (t % mt) * BM, n0 = (t / mt) * PBN;
-      mbar_wait(&s.tmem_full[acc], (li >> 1) & 1);
-      tcgen05_fence_after();
-      const int row = m0 + q * 32 + lane;
-#pragma unroll 1
-      for (int c0 = 0; c0 < PBN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem0 + acc * PBN + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const int colb = n0 + c0;
-        if (row < M && colb < N) {
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float x = __uint_as_float(r[i]);
-            if (bias != nullptr && colb + i < N) x += __ldg(bias + colb + i);
-            if (relu) x = fmaxf(x, 0.f);
-            v[i] = x;
-          }
-          if (out_bf16) {
-            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(c) + (size_t)row * N + colb;
-            if (colb + 32 <= N && (N % 8) == 0) {
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                uint4 pk;
-                __nv_bfloat162 t2;
-                t2 = __floats2bfloat162_rn(v[8 * g], v[8 * g + 1]);     pk.x = *reinterpret_cast<uint32_t*>(&t2);
-                t2 = __floats2bfloat162_rn(v[8 * g + 2], v[8 * g + 3]); pk.y = *reinterpret_cast<uint32_t*>(&t2);
-                t2 = __floats2bfloat162_rn(v[8 * g + 4], v[8 * g + 5]); pk.z = *reinterpret_cast<uint32_t*>(&t2);
-                t2 = __floats2bfloat162_rn(v[8 * g + 6], v[8 * g + 7]); pk.w = *reinterpret_cast<uint32_t*>(&t2);
-                reinterpret_cast<uint4*>(dst)[g] = pk;
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (colb + i < N) dst[i] = __float2bfloat16(v[i]);
-            }
-          } else {
-            float* dst = reinterpret_cast<float*>(c) + (size_t)row * N + colb;
-            if (colb + 32 <= N && (N % 4) == 0) {
-#pragma unroll
-              for (int g = 0; g < 8; ++g) reinterpret_cast<float4*>(dst)[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (colb + i < N) dst[i] = v[i];
-            }
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.tmem_empty[acc]);            // this warp's quarter of the accumulator is drained
-    }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem0), "r"(512u) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------------------------------ M=64 layout probe
-// D[64 x 32] = A[64 x 64] * B[32 x 64]^T with a UMMA_M = 64 instruction; the kernel zero-fills TMEM first and then
-// dumps all 128 TMEM lanes x 32 columns, so the host can read off which lane holds which accumulator row.
-__global__ void __launch_bounds__(128, 1)
-probe_m64_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, float* __restrict__ dump) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = base;                 // 64 x 128 B
-  uint8_t* sb = base + 8192;          // 32 x 128 B
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + 8192 + 4096);
-  uint64_t* done = full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(full, 1); mbar_init(done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(32u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  {   // zero all 128 lanes x 32 columns
-    const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-#pragma unroll
-    for (int c0 = 0; c0 < 32; c0 += 16)
-      asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1};" ::"r"(taddr + c0), "r"(0u) : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(full, 8192 + 4096);
-    tma_load_2d(sa, &map_a, full, 0, 0);
-    tma_load_2d(sb, &map_b, full, 0, 0);
-    mbar_wait(full, 0);
-    tcgen05_fence_after();
-    constexpr uint32_t idesc = make_idesc(64, 32);
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      umma_bf16(tmem, make_smem_desc(smem_u32(sa) + k * 32), make_smem_desc(smem_u32(sb) + k * 32), idesc, k > 0 ? 1u : 0u);
-    tcgen05_commit(done);
-  }
-  __syncwarp();
-  mbar_wait(done, 0);
-  tcgen05_fence_after();
-#pragma unroll
-  for (int c0 = 0; c0 < 32; c0 += 16) {
-    uint32_t r[16];
-    tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + c0, r);
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) dump[(warp * 32 + lane) * 32 + c0 + i] = __uint_as_float(r[i]);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(32u) : "memory");
+  tc::regs_inc<232>();
+  const int half = wg - 1;
+  uint32_t it = 0;
+  float d[PBN / 2];
+  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = (tile % mt) * BM, n0 = (tile / mt) * PBN;
+    it = mma_tile<PBN, PSTAGES>(d, &s.a[0][0], &s.b[0][0], s.full, s.empty, half, num_kb, it);
+    store_tile<PBN>(d, t, m0 + half * 64, n0, c, bias, M, N, relu, out_bf16);
   }
 }
 
@@ -487,7 +219,7 @@ int launch(const void* a, const void* b, void* c, const float* bias, int M, int 
            cudaStream_t stream) {
   CUtensorMap ma, mb;
   if (!make_map(&ma, a, M, K, BM) || !make_map(&mb, b, N, K, BN)) return -1;
-  const size_t smem = sizeof(SmemLayout<BN>) + 1024;
+  const size_t smem = sizeof(SmemLayout<BN, Cfg<BN>::STAGES>) + 1024;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -513,7 +245,7 @@ int launch_persistent(const void* a, const void* b, void* c, const float* bias, 
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   const int tiles = ((M + BM - 1) / BM) * ((N + PBN - 1) / PBN);
   const int grid = tiles < sms ? tiles : sms;
@@ -523,19 +255,20 @@ int launch_persistent(const void* a, const void* b, void* c, const float* bias, 
   return 0;
 }
 
+int sm_count() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (sms <= 0) sms = 132;
+  }
+  return sms;
+}
+
 }  // namespace gemm
 
 extern "C" {
-
-// a: [64,64] bf16, b: [32,64] bf16, dump: [128,32] fp32
-int b2_gemm_probe_m64(const void* a, const void* b, float* dump, cudaStream_t stream) {
-  CUtensorMap ma, mb;
-  if (!gemm::make_map(&ma, a, 64, 64, 64) || !gemm::make_map(&mb, b, 32, 64, 32)) return -1;
-  const size_t smem = 8192 + 4096 + 64 + 1024;
-  cudaFuncSetAttribute(gemm::probe_m64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  gemm::probe_m64_kernel<<<1, 128, smem, stream>>>(ma, mb, dump);
-  return (int)cudaGetLastError();
-}
 
 int b2_gemm_available() { return gemm::get_encode() != nullptr; }
 const char* b2_gemm_last_error() { return gemm::g_err.c_str(); }
@@ -545,9 +278,8 @@ int b2_gemm_bf16_launch(const void* a, const void* b, void* c, const float* bias
   if (M <= 0 || N <= 0 || K <= 0 || (K % 8) != 0) { gemm::g_err = "bad shape (K must be a multiple of 8)"; return -4; }
   if (((uintptr_t)a | (uintptr_t)b) & 15) { gemm::g_err = "operands must be 16-byte aligned"; return -5; }
   static const int mode = [] { const char* e = getenv("B200DIST_GEMM_PERSISTENT"); return e ? atoi(e) : 1; }();
-  // persistent 128x256 tiles pay off when there are at least ~one wave of tiles and a long K loop (measured: 8192x4096x4096
-  // 1322 TFLOP/s vs 969 for the 128x128 kernel; 4096x512x1024 and 16384x1000x512 are faster on the 128x128 kernel)
-  if (mode && N >= 192 && K >= 2048 && (long long)((M + 127) / 128) * ((N + 255) / 256) >= 148)
+  // persistent 128x256 tiles: for at least one wave of tiles and a long K loop; small GEMMs stay on 128xBN tiles
+  if (mode && N >= 192 && K >= 2048 && (long long)((M + 127) / 128) * ((N + 255) / 256) >= gemm::sm_count())
     return gemm::launch_persistent(a, b, c, bias, M, N, K, relu, out_bf16, stream);
   if (N <= 32) return gemm::launch<32>(a, b, c, bias, M, N, K, relu, out_bf16, stream);
   if (N <= 64) return gemm::launch<64>(a, b, c, bias, M, N, K, relu, out_bf16, stream);

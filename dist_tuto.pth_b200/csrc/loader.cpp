@@ -2,7 +2,7 @@
 //
 // Stands in for the reference's `torch.utils.data.DataLoader(partition, batch_size=bsz, shuffle=True)`
 // (train_dist.py:89-90), whose per-sample Python __getitem__ + PIL + ToTensor + Normalize + collate costs
-// milliseconds per 128-sample batch -- far more than the whole fused B200 training step.  Here a worker
+// milliseconds per 128-sample batch -- far more than the whole fused training step.  Here a worker
 // thread gathers the uint8 images of the next batches by index, (optionally) fuses the normalisation,
 // and writes them into a ring of page-locked buffers, so the training loop only issues one async H2D
 // copy per step.
@@ -34,8 +34,8 @@ NativeLoader::NativeLoader(const uint8_t* images, const int64_t* labels, int64_t
   {
     const char* e = getenv("B200DIST_LOADER_THREADS");
     const unsigned hc = std::thread::hardware_concurrency();
-    // one thread keeps up with the GPU (a 128 x 784 B gather with software prefetch takes ~10 us); more threads measured
-    // SLOWER end to end on the shared 16-core GPU boxes (3.0 M vs 3.7 M samples/s with 2) -- opt in with the variable
+    // one thread is the default (a 128 x 784 B gather with software prefetch is short next to a step); more threads
+    // compete with the thread that feeds the GPU when the host has few cores -- opt in with the variable
     (void)hc;
     nworkers_ = e ? atoi(e) : 1;
     nworkers_ = std::max(1, std::min({nworkers_, 8, nbuf_ / 2}));

@@ -167,7 +167,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
 // "One kernel per step": the tail of the fused forward/backward kernels (convnet.cu, convnet_cluster.cu).
 //
 // After a CTA has flushed its gradients into the bucket it checks in on a device counter; once all `n_cta` CTAs of the
-// grid have checked in (they are co-resident: <= 148 CTAs, one per SM) the bucket is complete and EVERY CTA takes a
+// grid have checked in (they are co-resident: at most one CTA per SM) the bucket is complete and EVERY CTA takes a
 // 1/n_cta share of the vectors through exchange_apply_vec (push to the peers' inboxes, local reduce, SGD, re-zero).
 // Compared with the separate allreduce_sgd kernel this removes the kernel boundary (launch + drain + PDL hand-off) from the
 // critical path between "last gradient flushed" and "first peer line stored", and spreads the update over all SMs.

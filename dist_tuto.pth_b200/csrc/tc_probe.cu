@@ -1,10 +1,10 @@
-// Layout probes for the sm_100a tensor-core path (no GPU on the dev box: every assumption about TMA swizzle images and
-// UMMA shared-memory descriptors is checked on hardware by tests/test_gpu_tc_probe.py before the training kernels rely on it).
+// Layout probes for the sm_90a tensor-core path: every assumption about TMA swizzle images and wgmma shared-memory
+// descriptors is checked on hardware by tests/test_gpu_tc_probe.py, independently of the training kernels that rely on it.
 //
 //   tma_probe  : ONE cp.async.bulk.tensor.{2..5}d box load with a caller-defined tensor map (uint16 elements, so values are
 //                exact) -> raw shared-memory image of the box, as TMA wrote it (swizzle included).
-//   umma_probe : caller-provided shared-memory images of A and B, a caller-provided instruction descriptor and a list of
-//                (A descriptor, B descriptor, TMEM column, accumulate) MMAs -> dump of TMEM [128 lanes x ncols] fp32.
+//   wgmma_probe: caller-provided shared-memory images of A and B, the A operand major and a list of
+//                (A descriptor, B descriptor, accumulate) m64nNk16 MMAs of one warpgroup -> dump of D [64 x N] fp32.
 //                Descriptors are given relative to the image (start address = byte offset in the image); the kernel
 //                adds the shared-memory base.  Any operand major / swizzle / LBO / SBO hypothesis is testable from Python.
 #include <cuda.h>
@@ -69,7 +69,7 @@ tma_probe_kernel(const __grid_constant__ CUtensorMap map, int rank, int c0, int 
 
 struct MmaOp {
   uint64_t adesc, bdesc;     // start-address fields relative to the A / B image
-  uint32_t tmem_col, accumulate;
+  uint32_t accumulate;
 };
 constexpr int kMaxOps = 64;
 struct MmaList {
@@ -77,52 +77,30 @@ struct MmaList {
   int n;
 };
 
+template <int N>
 __global__ void __launch_bounds__(128, 1)
-umma_probe_kernel(const uint8_t* __restrict__ a_img, uint32_t a_bytes, const uint8_t* __restrict__ b_img, uint32_t b_bytes,
-                  uint32_t idesc, const __grid_constant__ MmaList ops, int ncols, float* __restrict__ dump) {
+wgmma_probe_kernel(const uint8_t* __restrict__ a_img, uint32_t a_bytes, const uint8_t* __restrict__ b_img, uint32_t b_bytes,
+                   uint32_t a_mn, const __grid_constant__ MmaList ops, float* __restrict__ dump) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sa = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sb = sa + ((a_bytes + 1023) & ~1023u);
-  __shared__ __align__(8) uint64_t done;
-  __shared__ uint32_t tmem_slot;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (uint32_t i = threadIdx.x; i < a_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sa)[i] = reinterpret_cast<const uint4*>(a_img)[i];
-  for (uint32_t i = threadIdx.x; i < b_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sb)[i] = reinterpret_cast<const uint4*>(b_img)[i];
-  if (threadIdx.x == 0) { tc::mbar_init(&done, 1); tc::mbar_fence_init(); }
-  if (warp == 0) tc::tmem_alloc<512>(&tmem_slot);
+  const int t = threadIdx.x;
+  for (uint32_t i = t; i < a_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sa)[i] = reinterpret_cast<const uint4*>(a_img)[i];
+  for (uint32_t i = t; i < b_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sb)[i] = reinterpret_cast<const uint4*>(b_img)[i];
   tc::fence_proxy_async();
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem = tmem_slot;
-  // zero the dumped TMEM window first (lanes an instruction does not write must read back as 0)
-  for (int c0 = 0; c0 < ncols; c0 += 16) {
-    const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1,%1};" ::"r"(taddr), "r"(0u) : "memory");
-  }
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  tc::fence_before();
-  __syncthreads();
-  tc::fence_after();
-  if (threadIdx.x == 0) {
-    const uint64_t abase = (uint64_t)((tc::smem_u32(sa) & 0x3FFFF) >> 4), bbase = (uint64_t)((tc::smem_u32(sb) & 0x3FFFF) >> 4);
-    for (int i = 0; i < ops.n; ++i)
-      tc::umma_bf16(tmem + ops.op[i].tmem_col, ops.op[i].adesc + abase, ops.op[i].bdesc + bbase, idesc, ops.op[i].accumulate);
-    tc::commit(&done);
-  }
-  __syncwarp();
-  tc::mbar_wait(&done, 0);
-  tc::fence_after();
-  for (int c0 = 0; c0 < ncols; c0 += 16) {
-    uint32_t r[16];
-    tc::tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-    tc::tmem_ld_wait();
+  const uint64_t abase = (uint64_t)((tc::smem_u32(sa) & 0x3FFFF) >> 4), bbase = (uint64_t)((tc::smem_u32(sb) & 0x3FFFF) >> 4);
+  float d[N / 2];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) dump[(size_t)(warp * 32 + lane) * ncols + c0 + i] = __uint_as_float(r[i]);
-  }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) { tc::fence_after(); tc::tmem_dealloc<512>(tmem); }
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  tc::wg_fence();
+  for (int i = 0; i < ops.n; ++i)
+    tc::mma<N>(d, ops.op[i].adesc + abase, ops.op[i].bdesc + bbase, ops.op[i].accumulate, a_mn);
+  tc::wg_commit();
+  tc::wg_wait_all();
+  tc::acc_fence<N / 2>(d);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) dump[tc::acc_row(t, i) * N + tc::acc_col(t, i)] = d[i];
 }
 
 }  // namespace probe
@@ -157,24 +135,24 @@ int b2_tma_probe(const void* tensor, int rank, const unsigned long long* dims, c
   return 0;
 }
 
-// ops: n x {adesc, bdesc, tmem_col, accumulate} as 4 uint64 each
-int b2_umma_probe(const unsigned char* a_img, unsigned int a_bytes, const unsigned char* b_img, unsigned int b_bytes,
-                  unsigned int idesc, const unsigned long long* ops, int n_ops, int ncols, float* dump, cudaStream_t stream) {
-  if (n_ops < 1 || n_ops > probe::kMaxOps || ncols < 16 || ncols > 512 || (ncols % 16) != 0 || (a_bytes % 16) || (b_bytes % 16)) {
-    probe::g_err = "bad probe arguments";
+// ops: n x {adesc, bdesc, accumulate} as 3 uint64 each; dump: [64 x n] fp32
+int b2_wgmma_probe(const unsigned char* a_img, unsigned int a_bytes, const unsigned char* b_img, unsigned int b_bytes,
+                   int a_mn, const unsigned long long* ops, int n_ops, int n, float* dump, cudaStream_t stream) {
+  if (n_ops < 1 || n_ops > probe::kMaxOps || (n != 32 && n != 64 && n != 80) || (a_bytes % 16) || (b_bytes % 16)) {
+    probe::g_err = "bad probe arguments (n must be 32, 64 or 80)";
     return -1;
   }
   probe::MmaList l;
   memset(&l, 0, sizeof(l));
   l.n = n_ops;
   for (int i = 0; i < n_ops; ++i) {
-    l.op[i].adesc = ops[4 * i]; l.op[i].bdesc = ops[4 * i + 1];
-    l.op[i].tmem_col = (uint32_t)ops[4 * i + 2]; l.op[i].accumulate = (uint32_t)ops[4 * i + 3];
+    l.op[i].adesc = ops[3 * i]; l.op[i].bdesc = ops[3 * i + 1]; l.op[i].accumulate = (uint32_t)ops[3 * i + 2];
   }
   const size_t smem = ((a_bytes + 1023) & ~1023u) + ((b_bytes + 1023) & ~1023u) + 1024;
   if (smem > 200 * 1024) { probe::g_err = "images too large"; return -2; }
-  cudaFuncSetAttribute(probe::umma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  probe::umma_probe_kernel<<<1, 128, smem, stream>>>(a_img, a_bytes, b_img, b_bytes, idesc, l, ncols, dump);
+  auto kern = n == 32 ? probe::wgmma_probe_kernel<32> : n == 64 ? probe::wgmma_probe_kernel<64> : probe::wgmma_probe_kernel<80>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  kern<<<1, 128, smem, stream>>>(a_img, a_bytes, b_img, b_bytes, (uint32_t)(a_mn != 0), l, dump);
   cudaError_t ce = cudaGetLastError();
   if (ce != cudaSuccess) { probe::g_err = std::string("launch: ") + cudaGetErrorString(ce); return -4; }
   return 0;

@@ -8,7 +8,7 @@ Parity map (reference = /root/reference):
       text divides by a float), shard ``rank`` of ``world_size`` equal shards,
       shuffled loader.
 
-B200-first differences:
+GPU-first differences:
   * the dataset is tensor-backed (uint8 images + int64 labels in one block) so a
     batch is produced by a vectorised gather + fused normalise straight into a
     *pinned* staging buffer (optionally by the native C++ prefetcher in

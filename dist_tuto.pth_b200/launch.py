@@ -7,7 +7,7 @@ Parity map (reference = /root/reference):
   * init methods env:// / file:// / tcp://        tuto.md:421-457
   * backends tcp / gloo / mpi                     tuto.md:363-398
 
-What is different on purpose (B200-first, fixes defect D8):
+What is different on purpose (GPU-first, fixes defect D8):
   * one process per GPU; ``backend="b200"`` (alias of nccl + our symmetric
     peer-memory world) binds ``cuda:LOCAL_RANK`` before the group is created,
     bootstraps NCCL for p2p and exchanges peer-memory handles over the store;

@@ -8,7 +8,7 @@ order and under the same names as the reference so state_dicts interchange.
 
 Two execution paths share one set of parameters:
   * ``forward`` -- plain torch ops (CPU, and the oracle for kernel tests);
-  * the fused sm_100a training step in ``ops/convnet_fused.py`` which reads the
+  * the fused sm_90a training step in ``ops/convnet_fused.py`` which reads the
     parameters from a flat fp32 buffer (see ``FlatParams``) and runs
     forward + loss + backward in one kernel.
 """

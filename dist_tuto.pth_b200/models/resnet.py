@@ -1,4 +1,4 @@
-"""ResNet-18 (BASELINE.json config #3: "ResNet-18 bf16 on 8xB200, bucketed fused allreduce").
+"""ResNet-18 (BASELINE.json config #3: "ResNet-18 bf16 on 8 GPUs, bucketed fused allreduce").
 
 The reference repo has no second model; BASELINE.json adds ResNet-18 as the *larger-gradient* workload for
 the data-parallel engine: 11,689,512 parameters in 62 tensors (44.6 MB fp32 / 22.3 MB bf16 per step),
@@ -8,7 +8,7 @@ ConvNet gradient never reaches.
 Architecture = the standard 18-layer residual network (7x7/2 stem, 4 stages of 2 BasicBlocks, 64..512
 channels, global average pool, linear classifier), parameter names compatible with torchvision's
 ``resnet18`` so state_dicts interchange.  Convolutions/batch-norm run on the library kernels (cuDNN) in
-channels_last bf16; the classifier can run on our tcgen05 GEMM (``use_tc_fc=True``, inference/forward);
+channels_last bf16; the classifier can run on our wgmma GEMM (``use_tc_fc=True``, inference/forward);
 gradient communication is entirely ours (``parallel.ddp.DistributedDataParallel``).
 """
 from __future__ import annotations
@@ -44,7 +44,7 @@ class BasicBlock(nn.Module):
 class ResNet18(nn.Module):
     """The larger-gradient model of BASELINE config #3 (11,689,512 parameters at 1000 classes; state_dict keys match
     torchvision's ``resnet18``).  Only its gradients matter here: 45 MB in ~60 tensors exercise the bucketed, overlapped
-    all-reduce.  ``use_tc_fc`` routes the inference-time classifier through the tcgen05 GEMM."""
+    all-reduce.  ``use_tc_fc`` routes the inference-time classifier through the wgmma GEMM."""
 
     def __init__(self, num_classes: int = 1000, in_channels: int = 3, use_tc_fc: bool = False):
         super().__init__()
@@ -74,5 +74,5 @@ class ResNet18(nn.Module):
             from ..ops.gemm import linear_bf16, linear_tc
             if not torch.is_grad_enabled():
                 return linear_bf16(x, self.fc.weight, self.fc.bias, out_dtype=torch.float32)
-            return linear_tc(x.float(), self.fc.weight, self.fc.bias)     # trainable: dgrad + wgrad on the same tcgen05 kernel
+            return linear_tc(x.float(), self.fc.weight, self.fc.bias)     # trainable: dgrad + wgrad on the same wgmma kernel
         return self.fc(x)

@@ -1,1 +1,1 @@
-"""Hand-written sm_100a kernels and their Python entry points (see csrc/)."""
+"""Hand-written sm_90a kernels and their Python entry points (see csrc/)."""

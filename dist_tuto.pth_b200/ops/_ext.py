@@ -1,6 +1,6 @@
 """Loader for the in-tree native extension ``dist_tuto.pth_b200/_C.so``.
 
-The extension is built by ``build.py`` (nvcc, sm_100a only) and lives in the
+The extension is built by ``build.py`` (nvcc, sm_90a only) and lives in the
 package directory so it travels with the repo snapshot.  There is NO silent
 PyTorch fallback for the ops it provides: if it cannot be loaded, ``C()`` raises
 with the build instruction."""
@@ -37,10 +37,13 @@ def _build_locked():
     N spawned ranks all land here at once: an ``flock`` on ``csrc/build/.lock`` lets one of them build while the others
     wait and then find an up-to-date library.  ``build.build()`` is content-hashed (no-op when sources, flags and the
     link stamp match) and links to a temporary file that is ``os.replace``d into place, so nobody can import a
-    half-written library.  When nvcc is not installed (a deployment box) an existing library is used as is."""
+    half-written library.  An up-to-date library is used without taking the lock, so a read-only tree works; when nvcc
+    is not installed (a deployment box) an existing library is used as is."""
     import fcntl
     import shutil
     from .. import build as _b
+    if os.path.isfile(_SO) and _b.up_to_date():
+        return                          # nothing to do: never touch the tree (it may be read-only)
     have_nvcc = os.path.exists(os.path.join(_b._cuda_home(), "bin", "nvcc")) or shutil.which("nvcc") is not None
     if not have_nvcc:
         if os.path.isfile(_SO):

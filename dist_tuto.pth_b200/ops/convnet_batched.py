@@ -4,7 +4,7 @@ The per-sample engine (:mod:`.convnet_fused`) serves the reference's latency-bou
 train_dist.py:85).  This engine is the throughput path -- BASELINE.md B1 "large-batch variant": the same network,
 the same flat fp32 parameter / gradient-bucket layout and the same fused all-reduce + SGD kernel, but the batch flows
 layer by layer through kernels in which the GEMM-shaped layers (conv2 forward / data gradient / weight gradient, fc1
-forward and data gradient) run on tcgen05 tensor cores with TMA-fed operands and TMEM accumulators
+forward and data gradient) run on the wgmma tensor cores with TMA-fed operands and register accumulators
 (csrc/convnet_batched.cu has the kernel-by-kernel map; reference ops: train_dist.py:58-71,120-124).
 
 Parity oracle: :mod:`.batched_reference` (plain PyTorch, same rounding points).
@@ -82,7 +82,7 @@ def batched_forward(params: torch.Tensor, x: torch.Tensor, bufs: Optional[Batche
 class BatchedTrainer:
     """Synchronous data-parallel SGD for the ConvNet with the batched tensor-core engine.
 
-    One step = 8 forward/backward kernels + 2 tcgen05 GEMM launches + the fused [peer-memory all-reduce + 1/world +
+    One step = 8 forward/backward kernels + 2 wgmma GEMM launches + the fused [peer-memory all-reduce + 1/world +
     momentum SGD + re-zero] kernel of the per-sample engine (csrc/sgd.cu) + the bf16 weight re-pack, replayed as one CUDA
     graph.  Same constructor / ``step`` / ``state_dict`` surface as :class:`.convnet_fused.FusedTrainer`; state_dicts
     interchange (same flat layout and parameter names)."""
@@ -128,7 +128,7 @@ class BatchedTrainer:
         self.stream = torch.cuda.Stream(self.device)
         self._graph = None
         self._loss_read = 0.0
-        self.gpu_launches_per_step = 12       # 8 engine kernels + 2 tcgen05 GEMMs + allreduce_sgd + pack_weights
+        self.gpu_launches_per_step = 12       # 8 engine kernels + 2 wgmma GEMMs + allreduce_sgd + pack_weights
         with torch.cuda.stream(self.stream):
             self.C.bt_pack_weights(self.params, self.bufs.as_list())
         self.stream.synchronize()

@@ -1,9 +1,9 @@
-"""tcgen05 bf16 GEMM entry points (csrc/gemm_tcgen05.cu).
+"""wgmma bf16 GEMM entry points (csrc/gemm_tcgen05.cu).
 
 ``linear_bf16(x, w, bias)`` computes ``x @ w.T + bias`` like ``F.linear`` (the op
-behind fc1/fc2, train_dist.py:61-62,68,70) on the 5th-gen tensor cores: TMA-fed
-128B-swizzled smem tiles, ``tcgen05.mma`` with the fp32 accumulator in TMEM,
-bias/ReLU fused in the ``tcgen05.ld`` epilogue.  No cuBLAS on this path.
+behind fc1/fc2, train_dist.py:61-62,68,70) on the Hopper tensor cores: TMA-fed
+128B-swizzled smem tiles, ``wgmma.mma_async`` with fp32 accumulators in registers,
+bias/ReLU fused in the register epilogue.  No cuBLAS on this path.
 
 ``linear_tc`` / ``TcLinear`` make it trainable: the data gradient ``dY @ W`` and the weight
 gradient ``dY^T @ X`` are two more launches of the same kernel (it multiplies two K-major
@@ -89,14 +89,14 @@ class _LinearTC(torch.autograd.Function):
 
 
 def linear_tc(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Differentiable ``F.linear`` on the tcgen05 GEMM (CUDA tensors; falls back to ``F.linear`` on the CPU)."""
+    """Differentiable ``F.linear`` on the wgmma GEMM (CUDA tensors; falls back to ``F.linear`` on the CPU)."""
     if not x.is_cuda:
         return torch.nn.functional.linear(x, w, bias)
     return _LinearTC.apply(x, w, bias)
 
 
 class TcLinear(torch.nn.Linear):
-    """``nn.Linear`` whose forward, data-gradient and weight-gradient GEMMs run on ``tcgen05.mma`` (bf16 operands, fp32
+    """``nn.Linear`` whose forward, data-gradient and weight-gradient GEMMs run on ``wgmma.mma_async`` (bf16 operands, fp32
     accumulation, fp32 master weights stay in ``self.weight``).  State-dict compatible with ``nn.Linear``."""
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:

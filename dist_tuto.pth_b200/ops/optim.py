@@ -4,7 +4,7 @@ Parity: ``optim.SGD(model.parameters(), lr=0.01, momentum=0.5)`` + ``optimizer.s
 of the reference's training loop (train_dist.py:110,118,123; tuto.md:283,291,296).  Same update rule as
 ``torch.optim.SGD`` (``buf = mu*buf + (g + wd*p)``, ``p -= lr*buf``, dampening 0, no Nesterov).
 
-B200-first: the gradients of a model already live in flat (symmetric-memory) buckets
+GPU-first: the gradients of a model already live in flat (symmetric-memory) buckets
 (:class:`~dist_tuto.pth_b200.parallel.ddp.GradBucket`); this optimizer lays the parameters and the momentum out in flat
 buffers with the *same* offsets and strides (``p.data`` becomes a view), so a whole bucket is updated -- and its
 gradients re-zeroed for the next backward -- by ONE ``sgd_flat_kernel`` launch (csrc/sgd.cu) that streams the three

@@ -1,11 +1,11 @@
-"""Host-side model of the shared-memory operand layouts used by the sm_100a tensor-core kernels.
+"""Host-side model of the shared-memory operand layouts used by the sm_90a tensor-core kernels.
 
 The kernels (csrc/convnet_batched.cu, csrc/gemm_tcgen05.cu) hard-code how TMA lays a box out in shared memory
-(128-byte swizzle) and how a UMMA shared-memory descriptor walks it.  These functions state the same rules in numpy so that
+(128-byte swizzle) and how a wgmma shared-memory descriptor walks it.  These functions state the same rules in numpy so that
 (a) CPU tests can cross-check the index arithmetic of the kernels and (b) the hardware probes (tests/test_gpu_tc_probe.py,
 csrc/tc_probe.cu) can compare what the GPU really does against them.
 
-Canonical layouts (cute/atom/mma_traits_sm100.hpp, units of 16 bytes = 8 bf16):
+Canonical layouts (cute/atom/mma_traits_sm90_gmma.hpp, units of 16 bytes = 8 bf16):
   K-major  SW128  ((8,n),2):((8,SBO),1)            row r, 16-byte chunk c of a 128-byte row:
                                                     (r//8)*SBO + (r%8)*128 + ((c ^ (r%8)) * 16)
   MN-major SW128  ((8,n),(8,k)):((1,LBO),(8,SBO))  element (mn, k): the same image as the K-major tile of the transposed
@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import numpy as np
 
-__all__ = ["sw128_offset", "sw32_offset", "image_rows128", "image_rows32", "expected_tma_image_sw32", "smem_desc", "idesc_bf16", "expected_tma_image", "bf16_bits", "bits_to_f32"]
+__all__ = ["sw128_offset", "sw32_offset", "image_rows128", "image_rows32", "expected_tma_image_sw32", "smem_desc", "SW128", "SW32", "expected_tma_image", "bf16_bits", "bits_to_f32"]
 
 
 def sw128_offset(row: int, byte_in_row: int, sbo: int = 1024) -> int:
@@ -83,19 +83,16 @@ def expected_tma_image_sw32(box_vals: np.ndarray) -> np.ndarray:
     return img
 
 
-def smem_desc(start_bytes: int, lbo_bytes: int, sbo_bytes: int, layout: int = 2) -> int:
-    """64-bit UMMA shared-memory descriptor (start address relative to the image; see csrc/tc_common.cuh::smem_desc)."""
+SW128, SW32 = 1, 3       # descriptor layout types (128-byte / 32-byte swizzle)
+
+
+def smem_desc(start_bytes: int, lbo_bytes: int, sbo_bytes: int, layout: int = SW128) -> int:
+    """64-bit wgmma shared-memory descriptor (start address relative to the image; see csrc/tc_common.cuh::smem_desc)."""
     d = (start_bytes >> 4) & 0x3FFF
     d |= ((lbo_bytes >> 4) & 0x3FFF) << 16
     d |= ((sbo_bytes >> 4) & 0x3FFF) << 32
-    d |= 1 << 46
-    d |= (layout & 7) << 61
+    d |= (layout & 3) << 62
     return d
-
-
-def idesc_bf16(m: int, n: int, a_mn: int = 0, b_mn: int = 0) -> int:
-    """kind::f16 instruction descriptor: D=f32, A=B=bf16 (csrc/tc_common.cuh::idesc_bf16_major)."""
-    return (1 << 4) | (1 << 7) | (1 << 10) | ((a_mn & 1) << 15) | ((b_mn & 1) << 16) | ((n >> 3) << 17) | ((m >> 4) << 24)
 
 
 def expected_tma_image(box_vals: np.ndarray) -> np.ndarray:

@@ -5,7 +5,7 @@ after the call every ``param.grad`` holds the mean over ranks.  (The committed
 reference never communicates -- SURVEY §2.6 D1 -- we implement the documented
 semantics.)
 
-B200-first design instead of "one blocking all_reduce + one divide per tensor":
+GPU-first design instead of "one blocking all_reduce + one divide per tensor":
   * :class:`GradBucket` -- all gradients of a model live in ONE flat buffer
     (``param.grad`` are views into it).  On a CUDA symmetric world the buffer is
     allocated in peer-mapped symmetric memory, so the all-reduce kernel reads

@@ -1,4 +1,4 @@
-"""Symmetric peer memory worlds + fused all-reduce dispatch (the B200 comm backend).
+"""Symmetric peer memory worlds + fused all-reduce dispatch (the "b200" comm backend).
 
 What replaces gloo/tcp/mpi for the gradient path (SURVEY §5.1; reference call
 site train_dist.py:99, X1 in SURVEY §2.5b):
@@ -133,8 +133,8 @@ class SymmWorld:
         self._lock = threading.Lock()
         # every CTA of a comm kernel spins on peer flags, so the grid never exceeds what is co-resident (1 CTA / SM)
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
-        self.max_blocks = _env_int("B200DIST_AR_BLOCKS", 0) or min(sms, 148)
-        # size thresholds (wire bytes) from the measured sweeps (profiles/n2, profiles/n8; bench/allreduce_sweep.py):
+        self.max_blocks = _env_int("B200DIST_AR_BLOCKS", 0) or sms
+        # size thresholds (wire bytes) from sweeps with bench/allreduce_sweep.py:
         #   2 GPUs : one-shot wins up to ~64 KB, two-shot above; NVLS never beats two-shot (no fan-in to amortise)
         #   8 GPUs : one-shot wins up to ~8 KB; above that NVLS (in-switch reduction) wins at every size, two-shot next
         # ... superseded per world size by the table bench/allreduce_sweep.py --emit-table writes (nearest measured world)

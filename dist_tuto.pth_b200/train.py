@@ -12,13 +12,12 @@ are made identical by an explicit parameter broadcast, not only by equal seeds.
 Engines:
   * ``engine="torch"``  -- torch ops + ``average_gradients`` (CPU/gloo plumbing
     path, BASELINE.json config #1; also runs on CUDA).
-  * ``engine="fused"``  -- the B200 path: one fused sm_100a forward+backward
+  * ``engine="fused"``  -- the default GPU path: one fused sm_90a forward+backward
     kernel, one fused peer-memory all-reduce + SGD kernel, replayed as a CUDA
     graph (``ops/convnet_fused.py``).  Default on CUDA for per-GPU batches < 2048 (the reference's 128 // world).
   * ``engine="batched"`` -- the throughput path for large per-GPU batches (BASELINE B1 "large-batch variant"): conv2
-    forward / data gradient / weight gradient and fc1 as implicit GEMMs on tcgen05 (``ops/convnet_batched.py``), same
-    fused exchange + SGD kernel.  ``auto`` picks it from 2048 samples per GPU up (measured: 1.1x the per-sample engine at
-    1024, 2.5x at 4096, 2.7x at 16384 -- profiles/REPORT_r2.md section 2).
+    forward / data gradient / weight gradient and fc1 as implicit GEMMs on wgmma (``ops/convnet_batched.py``), same
+    fused exchange + SGD kernel.  ``auto`` picks it from 2048 samples per GPU up.
 """
 from __future__ import annotations
 

@@ -7,7 +7,7 @@
 * :func:`nvtx_range`     -- NVTX ranges when CUDA is present, no-op otherwise.
 * :class:`ClockSampler`  -- samples ``nvidia-smi`` SM clocks + throttle reasons
   in a background thread during a timed region (B200_PROFILING.md recipe).
-* :func:`l2_flush`       -- writes a buffer larger than the 126 MB L2.
+* :func:`l2_flush`       -- writes a buffer larger than the L2 (50 MB on an H100).
 """
 from __future__ import annotations
 
@@ -144,7 +144,7 @@ _L2_BUF = {}
 
 
 def l2_flush(device=None, nbytes: int = 256 << 20):
-    """Overwrite a buffer larger than L2 (126 MB) so the next kernel starts cold."""
+    """Overwrite a buffer larger than L2 (50 MB on an H100) so the next kernel starts cold."""
     if not torch.cuda.is_available():
         return
     dev = torch.device(device or torch.cuda.current_device())

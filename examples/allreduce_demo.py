@@ -7,7 +7,7 @@
     mpirun -n 4 python examples/allreduce_demo.py --backend mpi             # rank/size from the launcher
     torchrun --nproc-per-node 4 examples/allreduce_demo.py --backend mpi
 
-On ``--backend b200`` the collective is the fused sm_100a peer-memory kernel (no NCCL on that call)."""
+On ``--backend b200`` the collective is the fused sm_90a peer-memory kernel (no NCCL on that call)."""
 import argparse
 import os
 import sys

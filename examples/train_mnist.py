@@ -2,8 +2,8 @@
 """Distributed synchronous SGD on (synthetic) MNIST -- the reference's ``train_dist.py`` scenario.
 
     python examples/train_mnist.py                       # CPU, gloo, world 2 (the reference default)
-    python examples/train_mnist.py --backend b200 --size 8     # one process per B200, fused engine
-    python examples/train_mnist.py --backend b200 --size 8 --global-batch 32768   # large batch: tcgen05 batched engine
+    python examples/train_mnist.py --backend b200 --size 8     # one process per GPU, fused engine
+    python examples/train_mnist.py --backend b200 --size 8 --global-batch 32768   # large batch: wgmma batched engine
     python -m dist_tuto.pth_b200.spawn --size 8 --max-restarts 2 examples/train_mnist.py --external --backend b200 \
         --checkpoint run.pt --checkpoint-every 1       # supervised: a failed job is restarted and resumes from run.pt
     torchrun --nproc-per-node 8 examples/train_mnist.py --backend b200 --external

@@ -11,7 +11,7 @@ os.environ.setdefault("PYTHONPATH", ROOT + os.pathsep + os.path.join(ROOT, "test
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
 
 

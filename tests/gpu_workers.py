@@ -12,7 +12,7 @@ from dist_tuto.pth_b200.parallel import symm
 
 def _dev():
     # the torch models these workers compare against must be fp32 references: cuDNN / cuBLAS default to TF32 (10-bit
-    # mantissa) for fp32 convolutions, which by itself moves 5 SGD steps by ~1e-3 (scripts/det_diag.py --tf32)
+    # mantissa) for fp32 convolutions, which by itself moves 5 SGD steps by ~1e-3
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     return torch.device("cuda", torch.cuda.current_device())

@@ -1,6 +1,6 @@
 """The fp32 model of the batched tensor-core engine (ops/batched_reference.py) against autograd of the reference Net.
 
-GPU tests compare the sm_100a kernels with that model at a tight tolerance; this CPU test makes sure the model itself
+GPU tests compare the sm_90a kernels with that model at a tight tolerance; this CPU test makes sure the model itself
 (hand-written backward, im2col/col2im index conventions, dropout scaling) is the network of train_dist.py:53-71."""
 import torch
 import torch.nn.functional as F

@@ -81,7 +81,7 @@ def test_all_reduce_variant_selection_follows_the_threshold_table():
 
     one, two, nvls, ll = VARIANTS["oneshot"], VARIANTS["twoshot"], VARIANTS["nvls"], VARIANTS["ll"]
     assert world(1, False, 0, 0, 0).pick_variant(1 << 20) == one
-    # the 2-GPU sweep of round 2 (profiles/n2): LL wins to 64 KB, one-shot to 1 MB, two-shot above; NVLS never pays at 2
+    # a 2-GPU sweep (bench/allreduce_sweep.py): LL wins to 64 KB, one-shot to 1 MB, two-shot above; NVLS never pays at 2
     w2 = world(2, True, 64 << 10, 1 << 20, 1 << 62)
     assert [w2.pick_variant(b) for b in (1 << 10, 64 << 10, (64 << 10) + 16, 1 << 20, (1 << 20) + 16, 1 << 30)] == [ll, ll, one, one, two, two]
     w8 = world(8, True, 32 << 10, 32 << 10, (32 << 10) + 1)

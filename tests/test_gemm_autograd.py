@@ -1,4 +1,4 @@
-"""Autograd wiring of the trainable tcgen05 linear (ops/gemm.py): the three GEMMs, their K-major re-layouts and paddings.
+"""Autograd wiring of the trainable wgmma linear (ops/gemm.py): the three GEMMs, their K-major re-layouts and paddings.
 
 CPU tier: the extension's ``gemm_bf16`` is replaced by a plain fp32 ``A @ B^T`` of the same bf16 operands, so everything but
 the kernel itself is checked here (shapes not multiples of 8, leading batch dims, no bias); the GPU tier

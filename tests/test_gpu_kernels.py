@@ -1,4 +1,4 @@
-"""GPU-single tier: every sm_100a kernel against a plain PyTorch fp32 oracle (SURVEY §4)."""
+"""GPU-single tier: every sm_90a kernel against a plain PyTorch fp32 oracle (SURVEY §4)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -227,7 +227,7 @@ def test_train_loop_single_gpu_fused(dev):
 
 
 def test_train_loop_picks_the_batched_engine_for_large_batches(dev):
-    """train(): engine="auto" takes the tcgen05 batched engine from 2048 samples per GPU up (short tail batch included)."""
+    """train(): engine="auto" takes the wgmma batched engine from 2048 samples per GPU up (short tail batch included)."""
     import dist_tuto.pth_b200 as b2
     from dist_tuto.pth_b200.data import SyntheticMNIST
     from dist_tuto.pth_b200.ops.convnet_batched import BatchedTrainer
@@ -301,7 +301,7 @@ def tc_mode():
 
 @pytest.mark.parametrize("B", [1, 16, 128, 200])
 def test_convnet_tcgen05_path_matches_fp64_oracle(dev, tc_mode, B):
-    """conv2 forward + data-gradient on the tensor cores (bf16 operands, fp32 accumulate in TMEM).
+    """conv2 forward + data-gradient on the tensor cores (bf16 operands, fp32 accumulate in registers).
 
     bf16 rounding of the conv2 operands can flip a max-pool argmax / relu on near-ties, which reroutes a
     gradient entry completely, so gradients are compared by direction (cosine) and a loose max-error bound,

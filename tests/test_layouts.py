@@ -51,13 +51,13 @@ def test_prearranged_conv2_weights_match_the_kernel_indexing():
 
 
 def test_cluster_policy_keeps_one_wave():
-    # one CTA per sample above 64 samples, clusters below; C * B never exceeds the 148 SMs of a B200
+    # one CTA per sample above 64 samples, clusters below; C * B never exceeds the 132 SMs of an H100
     for b, c in ((128, 1), (64, 2), (32, 4), (16, 4), (8, 8), (1, 8)):
-        assert cf.pick_cluster(b) == c and b * c <= 148
+        assert cf.pick_cluster(b) == c and b * c <= 132
 
 
 def test_tc_layout_model_swizzles_are_involutions_and_window_addresses_stay_inside_the_image():
-    """ops/tc_layouts.py (host model of the TMA / UMMA shared-memory images used by csrc/convnet_batched.cu)."""
+    """ops/tc_layouts.py (host model of the TMA / wgmma shared-memory images used by csrc/convnet_batched.cu)."""
     import numpy as np
     from dist_tuto.pth_b200.ops import tc_layouts as L
     # 32B / 128B swizzles permute 16-byte chunks inside their repeat (256 B / 1024 B) and are their own inverse
@@ -77,6 +77,6 @@ def test_tc_layout_model_swizzles_are_involutions_and_window_addresses_stay_insi
                for ky in range(5) for ks in range(4) for katom in range(2) for pos in range(8) for kx in range(8))
     assert 4608 <= last < 4608 + 512
     # descriptor fields
-    d = L.smem_desc(0x1230, 32, 384, 6)
-    assert d & 0x3FFF == 0x123 and (d >> 16) & 0x3FFF == 2 and (d >> 32) & 0x3FFF == 24 and (d >> 61) == 6 and (d >> 46) & 3 == 1
-    assert L.idesc_bf16(128, 32, a_mn=1) == (1 << 4) | (1 << 7) | (1 << 10) | (1 << 15) | (4 << 17) | (8 << 24)
+    d = L.smem_desc(0x1230, 32, 384, L.SW32)
+    assert d & 0x3FFF == 0x123 and (d >> 16) & 0x3FFF == 2 and (d >> 32) & 0x3FFF == 24 and (d >> 62) == 3 and (d >> 46) & 0xFFFF == 0
+    assert L.smem_desc(0, 16, 1024) >> 62 == 1 and (L.smem_desc(0, 16, 1024) >> 46) & 0xFFFF == 0

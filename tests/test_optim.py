@@ -74,8 +74,12 @@ def test_flat_sgd_rejects_low_precision_master_weights():
 @pytest.mark.parametrize("wd", [0.0, 1e-2])
 def test_flat_sgd_kernel_matches_torch_sgd_gpu(wd):
     dev = torch.device("cuda:0")
-    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    # only the optimizers may differ: both replicas get bit-identical gradients (no TF32, and deterministic cuDNN backward
+    # algorithms -- the default ones sum with atomics, and that run-to-run noise compounds over the steps)
+    prev = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.deterministic,
+            torch.backends.cudnn.benchmark)
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = True, False
     try:
         ref, ours, o_ref, o_ours, xs, ys = _pair(dev, wd)
         l_ref, l_ours = _steps(ref, o_ref, xs, ys), _steps(ours, o_ours, xs, ys)
@@ -84,7 +88,8 @@ def test_flat_sgd_kernel_matches_torch_sgd_gpu(wd):
             assert torch.allclose(a, b, atol=1e-5), n
         assert float(o_ours.buckets[0].flat.abs().max()) == 0.0
     finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+        (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.deterministic,
+         torch.backends.cudnn.benchmark) = prev
 
 
 @pytest.mark.gpu
