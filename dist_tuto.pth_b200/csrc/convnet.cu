@@ -5,14 +5,17 @@
 // linears, log_softmax, nll, and their backward twins) on [B,...] tensors that round-trip through
 // HBM.  The network is per-sample independent and tiny (21,840 parameters, < 8 KB of activations per
 // sample), so here one CTA carries a sample through the whole network and back with everything in
-// shared memory / registers; weight gradients are accumulated in shared memory and flushed once per
-// CTA with vectorised `red.global.add.v4.f32` into the flat gradient bucket -- which is the symmetric
-// buffer the fused all-reduce + SGD kernel (sgd.cu) reads over NVSwitch.  HBM traffic per step is the
-// input batch + one pass over the parameters; launches per step: 1 (+1 for all-reduce/SGD).
+// shared memory / registers.  All weights (fc1.weight included) are staged once per CTA by 1-D bulk copies.
+// Weight gradients are accumulated in shared memory and flushed once per CTA with vectorised
+// `red.global.add.v4.f32` into the flat gradient bucket -- which is the symmetric buffer the fused
+// all-reduce + SGD kernel (sgd.cu) reads over NVSwitch -- except fc1.weight's, which each sample's fc1
+// backward phase red.adds straight into the bucket.  HBM traffic per step is the input batch + one pass
+// over the parameters; launches per step: 1 (+1 for all-reduce/SGD).
 //
 // Flat parameter layout (fp32, every tensor padded to 4 elements so all flushes are 16-byte vectors):
 //   conv1.w 0 | conv1.b 252 | conv2.w 264 | conv2.b 5264 | fc1.w 5284 | fc1.b 21284 | fc2.w 21336 |
 //   fc2.b 21836 | total 21848
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -48,11 +51,20 @@ union Scratch {
   TcBufs tc;
 };
 
+// fc1.weight has no slot in the shared gradient accumulator: S6 sends its per-sample gradient straight to global memory.
+// The accumulator g holds the other parameters in flat order with the fc1.weight range cut out.
+constexpr int NW3 = 16000, NG = NPAR - NW3;
+__host__ __device__ constexpr int gslot(int i) { return i < W3 ? i : i - NW3; }   // flat index (not in fc1.weight) -> g
+
+// Weights arrive by 1-D bulk copies straight from `params` / `aux`, so every staged array starts on a 16-byte boundary and
+// arrays copied together are laid out as in `params`: [w1 | b1] = params[W1, W2), [w3 | b3 | w4 | b4] = params[W3, NPAR).
 struct __align__(1024) Smem {
   Scratch u;                // first member: 1024-byte aligned (SWIZZLE_128B operand tiles)
-  float w1[252];
+  alignas(16) float w1[252];
   float b1[12];
-  float b2[20];
+  alignas(16) float b2[20];
+  alignas(16) float w3[NW3];  // fc1.weight [50][320], resident for the whole kernel (S3 and S6 read it)
+  float b3[52];
   float w4[500];
   float b4[12];
   float x[784];
@@ -66,7 +78,8 @@ struct __align__(1024) Smem {
   float dlog[12];
   float m2[20];             // dropout2d channel scale
   float rnd[72];            // uniforms: [0,20) dropout2d, [20,70) dropout
-  float g[NPAR];            // per-CTA gradient accumulators
+  alignas(16) float g[NG];  // per-CTA gradient accumulators (index with gslot)
+  uint64_t bar[4];          // weight staging: [0] w1,b1,b2  [1] aux w2f  [2] w3,b3,w4,b4  [3] aux w2b
   int work_ctr;             // dynamic work distribution inside a phase (warp-granular)
   short koff[256];          // im2col LUT: k=(ci,ky,kx) -> offset inside p1, -1 for the K padding
   unsigned char a1[1440];   // conv1 pool argmax (0..3)
@@ -74,6 +87,12 @@ struct __align__(1024) Smem {
   float loss_local;
   int correct_local;
 };
+static_assert(sizeof(Smem) + 1024 <= 232448, "one CTA per SM: the launch asks for sizeof(Smem) + 1024 of the 227 KB opt-in");
+static_assert(offsetof(Smem, b1) == offsetof(Smem, w1) + (B1 - W1) * 4 && offsetof(Smem, b3) == offsetof(Smem, w3) + (B3 - W3) * 4 &&
+                  offsetof(Smem, w4) == offsetof(Smem, w3) + (W4 - W3) * 4 && offsetof(Smem, b4) == offsetof(Smem, w3) + (B4 - W3) * 4,
+              "bulk-copied weight groups must be laid out as in params");
+static_assert(W2 % 4 == 0 && B2 % 4 == 0 && W3 % 4 == 0 && NPAR % 4 == 0 && AUX_W2B % 4 == 0 && NG % 4 == 0,
+              "bulk copies and float4 flushes need 16-byte offsets");
 
 template <bool TC>
 __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
@@ -89,22 +108,34 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   b2::pdl_launch_dependents();       // the all-reduce/SGD kernel may pre-launch; it parks in its own pdl_wait
   if (a.backward) {                  // everything that does not depend on the previous kernel happens before pdl_wait
     float4* g4 = reinterpret_cast<float4*>(s.g);
-    for (int i = tid; i < NPAR / 4; i += T) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = tid; i < NG / 4; i += T) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   b2::pdl_wait();                    // parameters / step counter written by the previous all-reduce+SGD kernel
+  // conv2.weight already in both smem layouts (written by sgd.cu): staged by bulk copies like the other weights
+  const bool fast = (a.aux != nullptr) && !TC;
+  if (tid == 0) {
+    // One thread hands all weight staging to the TMA engine, in order of first use; each phase waits only for the group it
+    // reads (S1: bar 0, S2: bar 1, S3: bar 2, S7b: bar 3), so the copies overlap the input load and the earlier phases.
+    for (int i = 0; i < 4; ++i) tc::mbar_init(&s.bar[i], 1);
+    tc::mbar_fence_init();
+    tc::fence_proxy_async_global();  // params / aux were written by the previous kernel through the generic proxy
+    tc::mbar_expect_tx(&s.bar[0], (W2 - W1) * 4 + 80);
+    tc::bulk_g2s(s.w1, P + W1, (W2 - W1) * 4, &s.bar[0]);                  // w1 | b1
+    tc::bulk_g2s(s.b2, P + B2, 80, &s.bar[0]);
+    if (fast) {
+      tc::mbar_expect_tx(&s.bar[1], AUX_W2B * 4);
+      tc::bulk_g2s(s.u.simt.w2f, a.aux + AUX_W2F, AUX_W2B * 4, &s.bar[1]);
+    }
+    tc::mbar_expect_tx(&s.bar[2], (NPAR - W3) * 4);
+    tc::bulk_g2s(s.w3, P + W3, (NPAR - W3) * 4, &s.bar[2]);              // w3 | b3 | w4 | b4
+    if (fast) {
+      tc::mbar_expect_tx(&s.bar[3], (AUX_TOTAL - AUX_W2B) * 4);
+      tc::bulk_g2s(s.u.simt.w2b, a.aux + AUX_W2B, (AUX_TOTAL - AUX_W2B) * 4, &s.bar[3]);
+    }
+  }
   if (tid == T - 1) wait_input(a);   // (executor path) the H2D copy of this step's batch; the barrier that ends staging publishes it
   {
-    // all global loads are issued before their first use (one L2 round trip instead of a dependent chain)
-    const bool fast = (a.aux != nullptr) && !TC;   // conv2.weight already in both smem layouts (written by sgd.cu)
-    float4 fa[3], fb[4];            // pre-arranged conv2.weight: every load is in flight before the first store
-    if (fast) {
-      const float4* __restrict__ af = reinterpret_cast<const float4*>(a.aux + AUX_W2F);
-      const float4* __restrict__ ab = reinterpret_cast<const float4*>(a.aux + AUX_W2B);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) fa[k] = (tid + k * T < 1250) ? __ldg(af + tid + k * T) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) fb[k] = (tid + k * T < 2000) ? __ldg(ab + tid + k * T) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+    // without aux: conv2.weight is scattered into its smem layout(s) from registers (all loads in flight before the first store)
     const float4* __restrict__ P4w2 = reinterpret_cast<const float4*>(P + W2);   // 1250 float4, 16B aligned
     float4 v[3];
 #pragma unroll
@@ -112,26 +143,12 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       const int i4 = tid + k * T;
       v[k] = (!fast && i4 < 1250) ? __ldg(P4w2 + i4) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    const float w1v = tid < 250 ? __ldg(P + W1 + tid) : 0.f;
-    const float w4v = tid < 500 ? __ldg(P + W4 + tid) : 0.f;
-    const float bv = tid < 10 ? __ldg(P + B1 + tid) : (tid < 20 ? __ldg(P + B4 + tid - 10) : (tid < 40 ? __ldg(P + B2 + tid - 20) : 0.f));
-    if (tid < 250) s.w1[tid] = w1v;
-    if (tid < 500) s.w4[tid] = w4v;
-    if (tid < 10) s.b1[tid] = bv; else if (tid < 20) s.b4[tid - 10] = bv; else if (tid < 40) s.b2[tid - 20] = bv;
     if (TC) {
       // zero the bf16 operand tiles (row / K padding must be 0), build the im2col LUT
       uint4* z = reinterpret_cast<uint4*>(s.u.tc.Bw);
       for (int i = tid; i < (16384 + 32768) / 16; i += T) z[i] = make_uint4(0u, 0u, 0u, 0u);
       if (tid < 256) s.koff[tid] = tid < 250 ? (short)p1_idx(tid / 25, (tid % 25) / 5, tid % 5) : (short)-1;
       __syncthreads();
-    }
-    if (fast) {
-      float4* df = reinterpret_cast<float4*>(s.u.simt.w2f);
-      float4* db = reinterpret_cast<float4*>(s.u.simt.w2b);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) if (tid + k * T < 1250) df[tid + k * T] = fa[k];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) if (tid + k * T < 2000) db[tid + k * T] = fb[k];
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -158,8 +175,10 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   if (tid == 0) { s.loss_local = 0.f; s.correct_local = 0; }
   const unsigned long long step = a.step ? *a.step : 0ull;
   const float keep_scale = 1.f / (1.f - a.p_drop);
+  // this step's gradient bucket (double-buffered: see sgd.cu); fc1.weight's share goes there from S6, the rest in the flush
+  float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
   if (TC) tc::fence_proxy_async();
-  __syncthreads();
+  __syncthreads();                   // also publishes the mbarrier initialisation to every waiting thread
 
   for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
     // -------------------------------------------------------------- S0: input, RNG, clear scratch
@@ -188,6 +207,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     __syncthreads();
 
     // -------------------------------------------------------------- S1: conv1 -> maxpool2 -> relu
+    tc::mbar_wait(&s.bar[0], 0);                   // w1, b1, b2 (after the first sample: returns at once)
     for (int o = tid; o < 1440; o += T) {
       const int c = o / 144, r = o % 144, py = r / 12, px = r % 12;
       float patch[6][6];
@@ -265,6 +285,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       __syncthreads();
     }
     if (!TC) {
+    if (fast) tc::mbar_wait(&s.bar[1], 0);         // w2f
     if (tid < 400) {
       const int cell = tid & 15, cg = (tid >> 4) % 5, ks = tid / 80;
       const int py = cell >> 2, px = cell & 3;
@@ -338,14 +359,15 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     __syncthreads();
 
     // -------------------------------------------------------------- S3: fc1 + relu + dropout
+    tc::mbar_wait(&s.bar[2], 0);                   // w3, b3, w4, b4
     {
       const int j = tid >> 3, l8 = tid & 7;
       float sum = 0.f;
       if (j < 50) {
-        const float4* wrow = reinterpret_cast<const float4*>(P + W3 + j * 320);
+        const float4* wrow = reinterpret_cast<const float4*>(s.w3 + j * 320);   // 4 rows x 128 B per warp: no conflicts
 #pragma unroll
         for (int k = 0; k < 10; ++k) {
-          const float4 w = __ldg(wrow + l8 + 8 * k);
+          const float4 w = wrow[l8 + 8 * k];
           const float4 v = *reinterpret_cast<const float4*>(&s.p2[(l8 + 8 * k) * 4]);
           sum = fmaf(w.x, v.x, sum); sum = fmaf(w.y, v.y, sum);
           sum = fmaf(w.z, v.z, sum); sum = fmaf(w.w, v.w, sum);
@@ -355,7 +377,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       sum += __shfl_xor_sync(0xffffffffu, sum, 2);
       sum += __shfl_xor_sync(0xffffffffu, sum, 1);
       if (j < 50 && l8 == 0) {
-        const float pre = sum + __ldg(P + B3 + j);
+        const float pre = sum + s.b3[j];
         const float dm = a.training ? (s.rnd[20 + j] >= a.p_drop ? keep_scale : 0.f) : 1.f;
         s.h[j] = fmaxf(pre, 0.f) * dm;
         s.hm[j] = pre > 0.f ? dm : 0.f;
@@ -402,8 +424,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     if (!a.backward) continue;
 
     // -------------------------------------------------------------- S5: fc2 backward
-    for (int e = tid; e < 500; e += T) s.g[W4 + e] += s.dlog[e / 50] * s.h[e % 50];
-    if (tid < 10) s.g[B4 + tid] += s.dlog[tid];
+    for (int e = tid; e < 500; e += T) s.g[gslot(W4) + e] += s.dlog[e / 50] * s.h[e % 50];
+    if (tid < 10) s.g[gslot(B4) + tid] += s.dlog[tid];
     if (tid >= 64 && tid < 114) {
       const int i = tid - 64;
       float d = 0.f;
@@ -415,28 +437,41 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
 
     // -------------------------------------------------------------- S6: fc1 backward
     {
-      float4* gw3 = reinterpret_cast<float4*>(&s.g[W3]);
-      const float4* p24 = reinterpret_cast<const float4*>(s.p2);
-      for (int e4 = tid; e4 < 4000; e4 += T) {    // fc1.weight gradient: 4 consecutive inputs per thread-iteration
-        const int j = e4 / 80, i4 = e4 - j * 80;
-        const float d = s.dh[j];
-        const float4 pv = p24[i4];
-        float4 gv = gw3[e4];
-        gv.x = fmaf(d, pv.x, gv.x); gv.y = fmaf(d, pv.y, gv.y); gv.z = fmaf(d, pv.z, gv.z); gv.w = fmaf(d, pv.w, gv.w);
-        gw3[e4] = gv;
-      }
-      if (tid >= 320 && tid < 370) s.g[B3 + tid - 320] += s.dh[tid - 320];
+      // data gradient first: S7 waits for it, while the atomics below only have to be issued
+      if (tid >= 320 && tid < 370) s.g[gslot(B3) + tid - 320] += s.dh[tid - 320];
       if (tid == 511) s.work_ctr = 0;
       for (int o = tid; o < 320; o += T) {
         float d = 0.f;
 #pragma unroll 10
-        for (int jj = 0; jj < 50; ++jj) d = fmaf(__ldg(P + W3 + jj * 320 + o), s.dh[jj], d);
+        for (int jj = 0; jj < 50; ++jj) d = fmaf(s.w3[jj * 320 + o], s.dh[jj], d);
         const int co = o >> 4, cell = o & 15, arg = s.a2[o];
         const float gv = s.p2[o] > 0.f ? d * s.m2[co] : 0.f;
         s.g2[o] = gv;
         if (!TC) {
           const int y = 2 * (cell >> 2) + (arg >> 1), x = 2 * (cell & 3) + (arg & 1);
           s.u.simt.dc2pad[co * DC_PLANE + (y + 4) * DC_ROW + (x + 4)] = gv;
+        }
+      }
+      // fc1.weight gradient dh (x) p2 of this sample, 4 consecutive inputs per thread-iteration, goes straight to global memory:
+      // red.add into the bucket (the atomics drain while S7/S8 run), or in deterministic mode into this CTA's private slot.
+      const float4* p24 = reinterpret_cast<const float4*>(s.p2);
+      if (a.det_partials != nullptr) {
+        float4* slot = reinterpret_cast<float4*>(a.det_partials + (size_t)blockIdx.x * DET_STRIDE + W3);
+        const bool first = b == (int)blockIdx.x;  // later samples of the same CTA add to what this thread stored before
+        for (int e4 = tid; e4 < 4000; e4 += T) {
+          const int j = e4 / 80, i4 = e4 - j * 80;
+          const float d = s.dh[j];
+          const float4 pv = p24[i4];
+          float4 gv = first ? make_float4(0.f, 0.f, 0.f, 0.f) : slot[e4];
+          gv.x = fmaf(d, pv.x, gv.x); gv.y = fmaf(d, pv.y, gv.y); gv.z = fmaf(d, pv.z, gv.z); gv.w = fmaf(d, pv.w, gv.w);
+          slot[e4] = gv;
+        }
+      } else {
+        for (int e4 = tid; e4 < 4000; e4 += T) {
+          const int j = e4 / 80, i4 = e4 - j * 80;
+          const float d = s.dh[j];
+          const float4 pv = p24[i4];
+          red_add_v4(gdst + W3 + e4 * 4, d * pv.x, d * pv.y, d * pv.z, d * pv.w);
         }
       }
     }
@@ -468,7 +503,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
                 for (int kx = 0; kx < 5; ++kx) acc[kx] = fmaf(gv, src[kx], acc[kx]);
               }
             }
-            float* dst = &s.g[W2 + co * 250 + ci * 25 + ky * 5];
+            float* dst = &s.g[gslot(W2) + co * 250 + ci * 25 + ky * 5];
 #pragma unroll
             for (int kx = 0; kx < 5; ++kx) dst[kx] += acc[kx];
           }
@@ -477,7 +512,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
           float d = 0.f;
 #pragma unroll
           for (int cell = 0; cell < 16; ++cell) d += s.g2[co * 16 + cell];
-          s.g[B2 + co] += d;
+          s.g[gslot(B2) + co] += d;
         }
       }
     };
@@ -548,7 +583,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) {                          // conv2.weight gradient: accumulator row = co, column = k
         const int co = tc::acc_row(t, i), k = wg * 64 + tc::acc_col(t, i);
-        if (co < 20 && k < 250) s.g[W2 + co * 250 + k] += dw[i];
+        if (co < 20 && k < 250) s.g[gslot(W2) + co * 250 + k] += dw[i];
       }
       __syncthreads();                                        // operand tiles consumed: A becomes the dgrad staging tile
       float* stage = reinterpret_cast<float*>(s.u.tc.A);      // [64 rows][128 cols] fp32, float4 index XOR-swizzled by row
@@ -588,6 +623,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       }
     }
     if (!TC) {
+    if (fast) tc::mbar_wait(&s.bar[3], 0);         // w2b
     if (tid < 432) {
       const int tile = tid % 36, half = (tid / 36) & 1, ks = tid / 72;
       const int y0 = 2 * (tile / 6), x0 = 2 * (tile % 6);
@@ -668,25 +704,35 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       acc += __shfl_xor_sync(0xffffffffu, acc, 1);           // executed by every lane (no divergence at the shuffle)
       gsum += __shfl_xor_sync(0xffffffffu, gsum, 1);
       if (tid < 500 && half == 0) {
-        s.g[W1 + out] += acc;
-        if (k == 0) s.g[B1 + out / 25] += gsum;
+        s.g[gslot(W1) + out] += acc;
+        if (k == 0) s.g[gslot(B1) + out / 25] += gsum;
       }
     }
     __syncthreads();
   }
 
-  // ------------------------------------------------------------------ flush
+  // ------------------------------------------------------------------ flush (everything but fc1.weight, which S6 sent already)
   if (a.backward && blockIdx.x < a.B) {
     if (a.det_partials != nullptr) {        // deterministic mode: a private slot per CTA, summed in CTA order afterwards
-      float4* slot = reinterpret_cast<float4*>(a.det_partials + (size_t)blockIdx.x * DET_STRIDE);
-      for (int v = tid; v < NPAR / 4; v += T) slot[v] = *reinterpret_cast<const float4*>(&s.g[v * 4]);
+      float* slot = a.det_partials + (size_t)blockIdx.x * DET_STRIDE;
+      for (int v = tid; v < NG / 4; v += T) {
+        const int i = v * 4 < W3 ? v * 4 : v * 4 + NW3;   // inverse of gslot
+        *reinterpret_cast<float4*>(slot + i) = *reinterpret_cast<const float4*>(&s.g[v * 4]);
+      }
     } else {
-      float* gdst = a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride;   // double-buffered buckets: see sgd.cu
-      for (int v = tid; v < NPAR / 4; v += T) {
+      for (int v = tid; v < NG / 4; v += T) {
+        const int i = v * 4 < W3 ? v * 4 : v * 4 + NW3;
         const float4 q = *reinterpret_cast<const float4*>(&s.g[v * 4]);
-        red_add_v4(gdst + v * 4, q.x, q.y, q.z, q.w);
+        red_add_v4(gdst + i, q.x, q.y, q.z, q.w);
       }
     }
+  }
+  // no bulk copy may still be writing this CTA's shared memory when it exits (groups no phase waited for: forward-only runs,
+  // a CTA without samples)
+  if (tid == 0) {
+    tc::mbar_wait(&s.bar[0], 0);
+    tc::mbar_wait(&s.bar[2], 0);
+    if (fast) { tc::mbar_wait(&s.bar[1], 0); tc::mbar_wait(&s.bar[3], 0); }
   }
   if (tid == 0 && a.loss_acc != nullptr && blockIdx.x < a.B) {
     if (a.det_partials != nullptr && a.backward) {       // deterministic mode: the slot's padding carries this CTA's loss terms

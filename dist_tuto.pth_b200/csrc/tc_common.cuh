@@ -31,6 +31,15 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 // generic-proxy smem writes -> visible to the async proxy (wgmma operand reads, TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// generic-proxy global writes (e.g. parameters stored by the previous kernel) -> visible to async-proxy reads (bulk copies)
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// 1-D bulk copy (TMA engine, no tensor map) global -> this CTA's shared memory; completion is counted on `bar` in bytes.
+// dst, src and bytes must be multiples of 16.
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
 
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
