@@ -53,7 +53,13 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const void* tail, float* det_partials, const unsigned int* in_flag, unsigned int in_gen, cudaStream_t stream);
+                           const void* tail, float* det_partials, float* factors, const unsigned int* in_flag, unsigned int in_gen,
+                           cudaStream_t stream);
+int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
+                         float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
+                         const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
+                         cudaStream_t stream);
+void b2_set_phase_ts(unsigned long long* p);
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
                          long long grad_stride, size_t n_elems, float* loss_acc, cudaStream_t stream);
 int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
@@ -180,7 +186,8 @@ struct ExecutorPy {
              torch::Tensor done_counter, torch::Tensor loss_acc, torch::Tensor in_dev, bool raw_u8, bool training, int rank,
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
              int max_in_flight, int cluster, torch::Tensor aux, int chunk, std::vector<unsigned long long> inbox,
-             torch::Tensor loss_hist, bool fused_tail, torch::Tensor ticket, bool wire_bf16)
+             torch::Tensor loss_hist, bool fused_tail, torch::Tensor ticket, bool wire_bf16, c10::optional<torch::Tensor> grad_slots,
+             c10::optional<torch::Tensor> factors)
       : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist, ticket} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
@@ -217,6 +224,16 @@ struct ExecutorPy {
     for (size_t i = 0; i < inbox.size() && i < 8; ++i) c.inbox_ptrs[i] = (void*)(uintptr_t)inbox[i];
     c.push = !inbox.empty();
     c.fused_tail = fused_tail ? 1 : 0;
+    if (grad_slots.has_value()) {    // one GPU, one CTA per sample: slots + factors reduced by reduce_sgd (no bucket)
+      TORCH_CHECK(factors.has_value() && world == 1 && cluster <= 1 && !fused_tail, "grad_slots: one GPU, cluster 1, no fused tail");
+      TORCH_CHECK(grad_slots->is_cuda() && grad_slots->scalar_type() == torch::kFloat32 && grad_slots->numel() >= c.B * (int64_t)21888 &&
+                  factors->is_cuda() && factors->scalar_type() == torch::kFloat32 && factors->numel() >= c.B * (int64_t)384,
+                  "grad_slots: [B, 21888] fp32, factors: [B, 384] fp32");
+      keep.push_back(*grad_slots);
+      keep.push_back(*factors);
+      c.grad_slots = grad_slots->data_ptr<float>();
+      c.factors = factors->data_ptr<float>();
+    }
     c.wire_bf16 = wire_bf16 ? 1 : 0;
     if (fused_tail) {
       TORCH_CHECK(ticket.is_cuda() && ticket.scalar_type() == torch::kInt32 && ticket.numel() >= 2, "ticket: CUDA int32 [2]");
@@ -341,7 +358,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                            c10::optional<torch::Tensor> loss_acc, c10::optional<torch::Tensor> out_logp,
                            c10::optional<torch::Tensor> mask_out, c10::optional<torch::Tensor> step, uint64_t seed,
                            int64_t sample_base, bool training, double inv_bsz, double p_drop, int max_ctas, int64_t grad_stride, int cluster,
-                           c10::optional<torch::Tensor> aux, py::object tail, c10::optional<torch::Tensor> det_partials) {
+                           c10::optional<torch::Tensor> aux, py::object tail, c10::optional<torch::Tensor> det_partials,
+                           c10::optional<torch::Tensor> factors) {
     check_cuda_contig(params, "params"); check_cuda_contig(x, "x"); check_cuda_contig(target, "target");
     TORCH_CHECK(params.scalar_type() == torch::kFloat32 && params.numel() >= b2_convnet_npar(), "params: flat fp32 [21848]");
     TORCH_CHECK(target.scalar_type() == torch::kInt64, "target: int64");
@@ -393,9 +411,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     float* dp = nullptr;
     if (det_partials.has_value()) {
       TORCH_CHECK(tp == nullptr, "deterministic mode and the fused tail are mutually exclusive");
+      const int ctas = cluster > 1 ? B * cluster : (max_ctas > 0 ? std::min(B, max_ctas) : B);   // CTAs of the step grid
       TORCH_CHECK(det_partials->is_cuda() && det_partials->scalar_type() == torch::kFloat32 &&
-                  det_partials->numel() >= (int64_t)std::max(1, B * std::max(1, cluster)) * 21888, "det_partials: [ctas, 21888] fp32");
+                  det_partials->numel() >= (int64_t)std::max(1, ctas) * 21888, "det_partials: [ctas, 21888] fp32");
       dp = det_partials->data_ptr<float>();
+    }
+    float* fp = nullptr;
+    if (factors.has_value()) {
+      // per-sample fc1 factors instead of fc1.weight in the slots (summed by reduce_sgd); one CTA per sample group only
+      TORCH_CHECK(dp != nullptr && cluster <= 1, "factors need det_partials and cluster 1");
+      TORCH_CHECK(factors->is_cuda() && factors->scalar_type() == torch::kFloat32 && factors->numel() >= (int64_t)std::max(1, B) * 384,
+                  "factors: [B, 384] fp32");
+      fp = factors->data_ptr<float>();
     }
     if (cluster > 1) {
       TORCH_CHECK(cluster == 2 || cluster == 4 || cluster == 8, "cluster must be 1, 2, 4 or 8");
@@ -406,11 +433,50 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     ck_cuda(b2_convnet_step_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                    la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                   max_ctas, grad_stride, ax, tp, dp, nullptr, 0u, cur_stream()), "convnet_step launch");
+                                   max_ctas, grad_stride, ax, tp, dp, fp, nullptr, 0u, cur_stream()), "convnet_step launch");
   }, py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
      py::arg("mask_out"), py::arg("step"), py::arg("seed"), py::arg("sample_base"), py::arg("training"), py::arg("inv_bsz"),
      py::arg("p_drop") = 0.5, py::arg("max_ctas") = 0, py::arg("grad_stride") = 0, py::arg("cluster") = 1, py::arg("aux") = py::none(),
-     py::arg("tail") = py::none(), py::arg("det_partials") = py::none());
+     py::arg("tail") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none());
+  m.def("reduce_sgd", [](torch::Tensor slots, int n_slots, torch::Tensor factors, int n_samples, torch::Tensor params,
+                         torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
+                         double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,
+                         c10::optional<torch::Tensor> grads, int64_t grad_stride) {
+    // one-GPU optimizer step from convnet_step(..., det_partials=slots, factors=factors): the local gradient is summed from
+    // the first n_slots slots and n_samples factor rows in a fixed order, then SGD is applied to it.  The gradient bucket is
+    // not read; given `grads`, its other-parity half is re-zeroed like allreduce_sgd does, so a bucket step may follow.
+    check_cuda_contig(slots, "slots"); check_cuda_contig(factors, "factors");
+    check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
+    TORCH_CHECK(slots.scalar_type() == torch::kFloat32 && slots.numel() >= (int64_t)n_slots * 21888, "slots: [n_slots, 21888] fp32");
+    TORCH_CHECK(factors.scalar_type() == torch::kFloat32 && factors.numel() >= (int64_t)n_samples * 384, "factors: [n_samples, 384] fp32");
+    TORCH_CHECK(params.scalar_type() == torch::kFloat32 && momentum.scalar_type() == torch::kFloat32 &&
+                params.numel() >= b2_convnet_npar() && params.numel() == momentum.numel(), "fp32 flat buffers");
+    unsigned long long* st = step.has_value() ? reinterpret_cast<unsigned long long*>(step->data_ptr()) : nullptr;
+    unsigned int* dc = done_counter.has_value() ? reinterpret_cast<unsigned int*>(done_counter->data_ptr()) : nullptr;
+    TORCH_CHECK(st == nullptr || dc != nullptr, "a step counter needs a done_counter scratch word");
+    float* ax = nullptr;
+    if (aux.has_value()) { TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000); ax = aux->data_ptr<float>(); }
+    float* la = loss_acc.has_value() ? loss_acc->data_ptr<float>() : nullptr;
+    float* g = nullptr;
+    if (grads.has_value()) {
+      check_cuda_contig(*grads, "grads");
+      TORCH_CHECK(grads->scalar_type() == torch::kFloat32 && grad_stride >= 0 && grads->numel() >= b2_convnet_npar() + grad_stride,
+                  "grads: fp32 [npar + grad_stride]");
+      g = grads->data_ptr<float>();
+    }
+    c10::cuda::CUDAGuard guard(params.device());
+    ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
+                                 nullptr, 0u, slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride,
+                                 cur_stream()),
+            "reduce_sgd launch");
+  }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
+     py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
+     py::arg("grads") = py::none(), py::arg("grad_stride") = 0);
+  m.def("set_phase_ts", [](c10::optional<torch::Tensor> ts) {
+    // opt-in phase timestamps of later step / optimizer launches (bench/step_phases.py); None turns them off
+    if (ts.has_value()) TORCH_CHECK(ts->is_cuda() && ts->scalar_type() == torch::kInt64 && ts->numel() >= 64 * 256 * 16, "ts: int64 [64*256*16]");
+    b2_set_phase_ts(ts.has_value() ? reinterpret_cast<unsigned long long*>(ts->data_ptr()) : nullptr);
+  }, py::arg("ts"));
   m.def("det_reduce", [](torch::Tensor partials, int n_slots, torch::Tensor grads, c10::optional<torch::Tensor> step, int64_t grad_stride,
                          c10::optional<torch::Tensor> loss_acc) {
     // deterministic mode: grads[(step & 1) * grad_stride ...] = sum over the first n_slots per-CTA slots, in slot order
@@ -529,14 +595,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def(py::init<LoaderPy&, torch::Tensor, torch::Tensor, torch::Tensor, std::vector<unsigned long long>,
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
                     int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor, int,
-                    std::vector<unsigned long long>, torch::Tensor, bool, torch::Tensor, bool>(),
+                    std::vector<unsigned long long>, torch::Tensor, bool, torch::Tensor, bool, c10::optional<torch::Tensor>,
+                    c10::optional<torch::Tensor>>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
            py::arg("sample_base"), py::arg("grad_stride"), py::arg("lr"), py::arg("mu"), py::arg("p_drop"),
            py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(), py::arg("chunk") = 1,
            py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(), py::arg("fused_tail") = false,
-           py::arg("ticket") = torch::Tensor(), py::arg("wire_bf16") = false, py::keep_alive<1, 2>())
+           py::arg("ticket") = torch::Tensor(), py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
+           py::arg("factors") = py::none(), py::keep_alive<1, 2>())
       .def("chunking", [](ExecutorPy& e) { return e.impl->chunking(); })
       .def("flag_mode", [](ExecutorPy& e) { return e.impl->flag_mode(); })
       .def("chunk_note", [](ExecutorPy& e) { return e.impl->chunk_note(); })

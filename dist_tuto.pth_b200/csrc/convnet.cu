@@ -6,11 +6,12 @@
 // HBM.  The network is per-sample independent and tiny (21,840 parameters, < 8 KB of activations per
 // sample), so here one CTA carries a sample through the whole network and back with everything in
 // shared memory / registers.  All weights (fc1.weight included) are staged once per CTA by 1-D bulk copies.
-// Weight gradients are accumulated in shared memory and flushed once per CTA with vectorised
-// `red.global.add.v4.f32` into the flat gradient bucket -- which is the symmetric buffer the fused
-// all-reduce + SGD kernel (sgd.cu) reads over NVSwitch -- except fc1.weight's, which each sample's fc1
-// backward phase red.adds straight into the bucket.  HBM traffic per step is the input batch + one pass
-// over the parameters; launches per step: 1 (+1 for all-reduce/SGD).
+// Weight gradients are accumulated in shared memory and flushed once per CTA, except fc1.weight's, which each sample's fc1
+// backward phase sends on by itself.  On one GPU (Args::factors) both leave with plain stores -- the accumulator to the CTA's
+// slot, fc1's per-sample factors dh and p2 to a factor buffer -- and the optimizer kernel sums them in a fixed order
+// (convnet_reduce.cuh).  Otherwise they are red.global.add.v4.f32-ed into the flat gradient bucket, the symmetric buffer the
+// fused all-reduce + SGD kernel (sgd.cu) reads over NVSwitch.  HBM traffic per step is the input batch + one pass over the
+// parameters; launches per step: 1 (+1 for the optimizer).
 //
 // Flat parameter layout (fp32, every tensor padded to 4 elements so all flushes are 16-byte vectors):
 //   conv1.w 0 | conv1.b 252 | conv2.w 264 | conv2.b 5264 | fc1.w 5284 | fc1.b 21284 | fc2.w 21336 |
@@ -103,6 +104,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   const int tid = threadIdx.x;
   if (TC && (tc::smem_u32(smem_raw) & 1023u) != 0u) __trap();   // SWIZZLE_128B operand tiles need 1024-byte alignment
   const float* __restrict__ P = a.params;
+  const unsigned long long t_entry = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
 
   // ---------------------------------------------------------------- P0: stage weights, zero accumulators
   b2::pdl_launch_dependents();       // the all-reduce/SGD kernel may pre-launch; it parks in its own pdl_wait
@@ -111,6 +113,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     for (int i = tid; i < NG / 4; i += T) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   b2::pdl_wait();                    // parameters / step counter written by the previous all-reduce+SGD kernel
+  const unsigned long long t_waited = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
   // conv2.weight already in both smem layouts (written by sgd.cu): staged by bulk copies like the other weights
   const bool fast = (a.aux != nullptr) && !TC;
   if (tid == 0) {
@@ -179,6 +182,13 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
   if (TC) tc::fence_proxy_async();
   __syncthreads();                   // also publishes the mbarrier initialisation to every waiting thread
+  auto stamp = [&](int k) {          // opt-in phase timestamps (bench/step_phases.py); call after a barrier
+    if (a.phase_ts != nullptr && tid == 0) b2::ts_put(a.phase_ts, step, (int)blockIdx.x, k, b2::globaltimer());
+  };
+  if (a.phase_ts != nullptr && tid == 0) {
+    b2::ts_put(a.phase_ts, step, (int)blockIdx.x, b2::TS_ENTRY, t_entry);
+    b2::ts_put(a.phase_ts, step, (int)blockIdx.x, b2::TS_WAITED, t_waited);
+  }
 
   for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
     // -------------------------------------------------------------- S0: input, RNG, clear scratch
@@ -357,6 +367,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       s.a2[o] = (unsigned char)arg;
     }
     __syncthreads();
+    stamp(b2::TS_S2);
 
     // -------------------------------------------------------------- S3: fc1 + relu + dropout
     tc::mbar_wait(&s.bar[2], 0);                   // w3, b3, w4, b4
@@ -421,6 +432,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
           a.training ? (s.rnd[tid] >= a.p_drop ? keep_scale : 0.f) : 1.f;
     }
     __syncthreads();
+    stamp(b2::TS_S4);
     if (!a.backward) continue;
 
     // -------------------------------------------------------------- S5: fc2 backward
@@ -452,10 +464,15 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
           s.u.simt.dc2pad[co * DC_PLANE + (y + 4) * DC_ROW + (x + 4)] = gv;
         }
       }
-      // fc1.weight gradient dh (x) p2 of this sample, 4 consecutive inputs per thread-iteration, goes straight to global memory:
-      // red.add into the bucket (the atomics drain while S7/S8 run), or in deterministic mode into this CTA's private slot.
+      // fc1.weight gradient dh (x) p2 of this sample goes straight to global memory: as its two factors (370 floats, stored
+      // by threads that are idle in this phase; the reduction of convnet_reduce.cuh forms the sum over samples), or as the
+      // product, 4 consecutive inputs per thread-iteration, into this CTA's slot (det_partials) or red.add-ed into the bucket.
       const float4* p24 = reinterpret_cast<const float4*>(s.p2);
-      if (a.det_partials != nullptr) {
+      if (a.factors != nullptr) {
+        float* f = a.factors + (size_t)b * FAC_STRIDE;
+        if (tid >= 370 && tid < 420) f[tid - 370] = s.dh[tid - 370];
+        else if (tid >= 420 && tid < 500) reinterpret_cast<float4*>(f + FAC_P2)[tid - 420] = p24[tid - 420];
+      } else if (a.det_partials != nullptr) {
         float4* slot = reinterpret_cast<float4*>(a.det_partials + (size_t)blockIdx.x * DET_STRIDE + W3);
         const bool first = b == (int)blockIdx.x;  // later samples of the same CTA add to what this thread stored before
         for (int e4 = tid; e4 < 4000; e4 += T) {
@@ -476,6 +493,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       }
     }
     __syncthreads();
+    stamp(b2::TS_S6);
 
     // -------------------------------------------------------------- S7a: conv2 weight/bias gradient (sparse)
     // Work items are handed out 32 at a time per warp from a shared counter, so the warps that had no (or a short)
@@ -683,6 +701,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     }
     __syncthreads();
     }
+    stamp(b2::TS_S8A);
 
     // -------------------------------------------------------------- S8b: conv1 weight/bias gradient (sparse)
     {
@@ -709,6 +728,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       }
     }
     __syncthreads();
+    stamp(b2::TS_S8B);
   }
 
   // ------------------------------------------------------------------ flush (everything but fc1.weight, which S6 sent already)
@@ -727,6 +747,10 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       }
     }
   }
+  if (a.phase_ts != nullptr) {
+    __syncthreads();
+    stamp(b2::TS_FLUSHED);
+  }
   // no bulk copy may still be writing this CTA's shared memory when it exits (groups no phase waited for: forward-only runs,
   // a CTA without samples)
   if (tid == 0) {
@@ -743,6 +767,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       atomicAdd(a.loss_acc + 1, (float)s.correct_local);
     }
   }
+  stamp(b2::TS_EXIT);
   // ------------------------------------------------------------------ fused tail: gradient exchange + SGD in this kernel
   if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x);   // grid <= B: every CTA flushed
 }
@@ -750,6 +775,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
 }  // namespace cn
 
 extern "C" {
+
+unsigned long long* b2_phase_ts();   // sgd.cu
 
 size_t b2_convnet_smem_bytes() { return sizeof(cn::Smem) + 1024; }
 int b2_convnet_npar() { return cn::NPAR; }
@@ -768,8 +795,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const cn::FusedTailHost* tail, float* det_partials, const unsigned int* in_flag, unsigned int in_gen,
-                           cudaStream_t stream) {
+                           const cn::FusedTailHost* tail, float* det_partials, float* factors, const unsigned int* in_flag,
+                           unsigned int in_gen, cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cn::Smem) + 1024;
   if (!configured) {
@@ -786,6 +813,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   a.mean = 0.1307f; a.inv_std = 1.f / 0.3081f; a.grad_stride = grad_stride; a.aux = aux;
   cn::fill_tail(a.tail, backward ? tail : nullptr, grad_stride);
   a.det_partials = backward ? det_partials : nullptr;
+  a.factors = (backward && det_partials != nullptr) ? factors : nullptr;
+  a.phase_ts = b2_phase_ts();
   a.in_flag = in_flag; a.in_gen = in_gen;
   int grid = B;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;

@@ -36,8 +36,12 @@ struct Args {
   long long grad_stride;    // elements between the two gradient buckets (0: single bucket); bucket = step & 1
   const float* aux;         // optional: conv2.weight pre-arranged by the SGD kernel as [w2f 5000 | w2b 8000] (see sgd.cu)
   b2::FusedTail tail;       // enabled: gradient exchange + SGD run in the tail of THIS kernel (sgd_device.cuh)
-  float* det_partials;      // deterministic mode: CTA i stores its gradient sums to det_partials + i * DET_STRIDE (plain
-                            // stores) instead of red.add-ing into the bucket; det_reduce_kernel (sgd.cu) sums the slots in order
+  float* det_partials;      // per-CTA slots: CTA i stores its gradient sums and loss terms to det_partials + i * DET_STRIDE
+                            // (plain stores) instead of red.add-ing into the bucket; they are summed in slot order afterwards,
+                            // by det_reduce_kernel or, with `factors`, by the reduction of convnet_reduce.cuh
+  float* factors;           // with det_partials: sample b stores its fc1 factors dh (50) and p2 (320) to factors + b * FAC_STRIDE
+                            // instead of dh (x) p2 into its slot; the slot's fc1.weight range is then left unwritten
+  unsigned long long* phase_ts;   // optional phase timestamps (sgd_device.cuh: TS_STEPS); nullptr: off
   const unsigned int* in_flag;   // optional "this batch has landed" word: the executor's copy stream writes in_gen there with a
   unsigned int in_gen;           // stream memory op right behind the H2D copy of x / target; the kernel polls it instead of the
                                  // compute stream waiting on an event, so consecutive steps stay one unbroken PDL kernel chain
@@ -52,6 +56,7 @@ __device__ __forceinline__ void wait_input(const Args& a) {
   } while ((int)(v - a.in_gen) < 0);
 }
 constexpr int DET_STRIDE = 21888;   // = NPAR_ALLOC of ops/convnet_fused.py
+constexpr int FAC_STRIDE = 384, FAC_P2 = 64;   // per-sample fc1 factors: dh at [0, 50), p2 at [FAC_P2, FAC_P2 + 320)
 
 // Host-side description of the fused tail (C ABI of the launchers); nullptr / enabled == 0 -> two-kernel step.
 struct FusedTailHost {

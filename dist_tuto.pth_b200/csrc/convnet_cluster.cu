@@ -565,6 +565,7 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
   a.mean = 0.1307f; a.inv_std = 1.f / 0.3081f; a.grad_stride = grad_stride; a.aux = aux;
   cn::fill_tail(a.tail, backward ? tail : nullptr, grad_stride);
   a.det_partials = backward ? det_partials : nullptr;
+  a.factors = nullptr; a.phase_ts = nullptr;
   a.in_flag = in_flag; a.in_gen = in_gen;
   int clusters = B;
   if (max_clusters > 0 && clusters > max_clusters) clusters = max_clusters;

@@ -36,8 +36,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const void* tail, float* det_partials, const unsigned int* in_flag, unsigned int in_gen,
-                           cudaStream_t stream);
+                           const void* tail, float* det_partials, float* factors, const unsigned int* in_flag,
+                           unsigned int in_gen, cudaStream_t stream);
 struct PeerPtrsC { void* p[8]; };
 struct SignalPadsC { uint32_t* pad[8]; };
 int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, float* params, float* momentum,
@@ -45,6 +45,10 @@ int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, floa
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrsC* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
                             unsigned int* snap_flag, unsigned int snap_gen, cudaStream_t stream);
+int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
+                         float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
+                         const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
+                         cudaStream_t stream);
 int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
@@ -178,15 +182,22 @@ void StepExecutor::record_step(const void* x, const long long* y, float* loss_sn
     th.wire_bf16 = cfg_.wire_bf16;
     tp = &th;
   }
+  // one GPU, one CTA per sample: plain stores to the slots / factors, reduced in a fixed order by the optimizer kernel
+  const bool slots = cfg_.grad_slots != nullptr && cfg_.world == 1 && cfg_.cluster <= 1 && !cfg_.fused_tail;
   int rc = cfg_.cluster > 1
                ? b2_convnet_cluster_launch(cfg_.params, cfg_.grads_local, x, cfg_.x_u8, y, cfg_.loss_acc, nullptr, nullptr,
                                            cfg_.step_counter, cfg_.seed, cfg_.sample_base, cfg_.B, cfg_.training, 1,
                                            1.f / cfg_.B, cfg_.p_drop, cfg_.cluster, 0, cfg_.grad_stride, cfg_.aux, tp, nullptr, in_flag, gen, compute_)
                : b2_convnet_step_launch(cfg_.params, cfg_.grads_local, x, cfg_.x_u8, y, cfg_.loss_acc, nullptr, nullptr,
                                         cfg_.step_counter, cfg_.seed, cfg_.sample_base, cfg_.B, cfg_.training, 1, 1.f / cfg_.B,
-                                        cfg_.p_drop, 0, cfg_.grad_stride, cfg_.aux, tp, nullptr, in_flag, gen, compute_);
+                                        cfg_.p_drop, 0, cfg_.grad_stride, cfg_.aux, tp, slots ? cfg_.grad_slots : nullptr,
+                                        slots ? cfg_.factors : nullptr, in_flag, gen, compute_);
   int rc2 = 0;
-  if (!cfg_.fused_tail) {
+  if (slots) {
+    rc2 = b2_reduce_sgd_launch(cfg_.params, cfg_.momentum, cfg_.step_counter, cfg_.done_counter, cfg_.lr, cfg_.mu, cfg_.aux,
+                               cfg_.loss_acc, loss_snapshot, snap_flag, gen, cfg_.grad_slots, cfg_.B, cfg_.factors, cfg_.B, cfg_.grads_local,
+                               cfg_.grad_stride, compute_);
+  } else if (!cfg_.fused_tail) {
     PeerPtrsC g;
     SignalPadsC sg;
     std::memcpy(g.p, cfg_.grad_ptrs, sizeof(g.p));

@@ -36,6 +36,8 @@ struct StepConfig {
   int wire_bf16;                     // push exchange: bf16 on the wire
   int fused_tail;                    // gradient exchange + SGD in the tail of the step kernel (one kernel per step)
   unsigned int* ticket;              // device scratch of the fused tail
+  float* grad_slots;                 // one GPU, one CTA per sample: per-CTA slots [B][21888] and per-sample fc1 factors [B][384]
+  float* factors;                    // of the step kernel, summed by reduce_sgd (sgd.cu) instead of red.add into the bucket
   unsigned int* flags;               // device [num_slots][2] zero-initialised words: {batch landed, loss snapshot written}
                                      // generations of the per-slot ring path's flag mode (nullptr: event mode)
 };

@@ -14,6 +14,7 @@
 #include <cstring>
 #include "common.cuh"
 #include "sgd_device.cuh"
+#include "convnet_reduce.cuh"
 
 namespace b2 {
 
@@ -25,6 +26,7 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
   __shared__ unsigned int s_par;
   pdl_wait();                        // gradients of this step (previous kernel) are complete and visible
   pdl_launch_dependents();           // the next step's forward/backward kernel may pre-launch now (it zeroes its smem, then waits)
+  const unsigned long long t_waited = a.phase_ts != nullptr ? globaltimer() : 0ull;
   snapshot_loss(a);
   unsigned long long st = 0ull;
   unsigned int seen = 0u;
@@ -75,7 +77,65 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
     }
   }
   if (world > 1 && threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+  if (a.phase_ts != nullptr) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_WAITED, t_waited);
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_EXIT, globaltimer());
+    }
+  }
   // the last block to have checked in knows every block has read the step counter: it publishes step + 1
+  if (threadIdx.x == 0 && a.step != nullptr && seen == gridDim.x - 1) { *a.done_counter = 0u; *a.step = st + 1ull; }
+}
+
+// World-1 optimizer of the per-sample step kernel run with per-CTA slots and fc1 factors (convnet.cu, convnet_args.cuh): every
+// CTA reduces its share of the local gradient in a fixed order (convnet_reduce.cuh) and applies SGD to it straight from
+// registers.  No bucket is read or red.add-ed, and the loss terms of the slots are summed in slot order, so the whole step is
+// bit-reproducible.  Also bumps the step counter, snapshots the loss and refreshes aux like the kernels above, and re-zeroes the
+// gradient bucket of the other step parity as they do (a.grads.p[0], optional): a trainer may still run a bucket step next (the
+// fused tail, a batch on another path), and every bucket step relies on finding its bucket zeroed by the step before it.
+__global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const float* __restrict__ slots, int n_slots,
+                                                               const float* __restrict__ factors, int n_samples, float* loss_acc) {
+  __shared__ cn::RedSmem s;
+  __shared__ unsigned long long s_step;
+  pdl_wait();                        // slots and factors of this step are complete and visible
+  pdl_launch_dependents();
+  const unsigned long long t_waited = a.phase_ts != nullptr ? globaltimer() : 0ull;
+  unsigned int seen = 0u;
+  if (threadIdx.x == 0) {
+    s_step = a.step != nullptr ? *reinterpret_cast<volatile unsigned long long*>(a.step) : 0ull;
+    if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);    // consumed at the very end (latency hidden)
+  }
+  if (blockIdx.x == 0 && threadIdx.x >= cn::RED_T - 32 && loss_acc != nullptr) {   // last warp of CTA 0
+    const float2 l = cn::reduce_loss(slots, n_slots);
+    const int i = threadIdx.x - (cn::RED_T - 32);
+    if (i < 2) {                     // the only writer of loss_acc while this kernel runs
+      const float v = loss_acc[i] + (i == 0 ? l.x : l.y);
+      loss_acc[i] = v;
+      if (a.loss_snapshot != nullptr) a.loss_snapshot[i] = v;
+    }
+  }
+  // momentum and parameters of the vectors a thread will update are loaded together with the unit's gradient terms
+  struct MP { float4 m, p; };
+  cn::reduce_local_grad(
+      slots, n_slots, factors, n_samples, (int)blockIdx.x, (int)gridDim.x, s,
+      [&](int v) { return MP{reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]}; },
+      [&](int v, float4 g, const MP& h) {
+        sgd_apply_mp(a, (size_t)v, g, h.m, h.p);
+        if (a.grads.p[0] != nullptr) {                   // s_step: written before the routine's first barrier
+          const size_t z = a.grad_stride > 0 ? (size_t)((s_step & 1ull) ^ 1ull) * (size_t)a.grad_stride : 0;
+          st_cg_v4(reinterpret_cast<float*>(a.grads.p[0]) + z + (size_t)v * 4, make_uint4(0u, 0u, 0u, 0u));
+        }
+      });
+  __syncthreads();                   // s_step and the loss snapshot are visible to thread 0
+  publish_snapshot(a);
+  const unsigned long long st = s_step;
+  if (a.phase_ts != nullptr) {
+    if (threadIdx.x == 0) {
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_WAITED, t_waited);
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_EXIT, globaltimer());
+    }
+  }
   if (threadIdx.x == 0 && a.step != nullptr && seen == gridDim.x - 1) { *a.done_counter = 0u; *a.step = st + 1ull; }
 }
 
@@ -166,12 +226,17 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
 
 extern "C" {
 
+static unsigned long long* g_phase_ts = nullptr;   // opt-in phase timestamps (sgd_device.cuh: TS_STEPS); read at launch
+void b2_set_phase_ts(unsigned long long* p) { g_phase_ts = p; }
+unsigned long long* b2_phase_ts() { return g_phase_ts; }
+
 int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, float* params, float* momentum,
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
                             unsigned int* snap_flag, unsigned int snap_gen, cudaStream_t stream) {
   b2::SgdArgs a;
+  a.phase_ts = g_phase_ts;
   a.wire_bf16 = wire_bf16;
   a.loss_acc = loss_acc; a.loss_snapshot = (loss_acc != nullptr) ? loss_snapshot : nullptr;
   a.snap_flag = (a.loss_snapshot != nullptr) ? snap_flag : nullptr; a.snap_gen = snap_gen;
@@ -202,6 +267,40 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
   cfg.numAttrs = pdl ? 1 : 0;
   return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel, a)
               : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel, a);
+}
+
+int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
+                         float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
+                         const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
+                         cudaStream_t stream) {
+  if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
+  b2::SgdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.params = params; a.momentum = momentum; a.step = step; a.done_counter = done_counter; a.aux = aux;
+  a.n_vec = cn::NPAR / 4; a.lr = lr; a.mu = mu; a.scale = 1.f; a.rank = 0; a.world = 1;
+  a.loss_acc = loss_acc; a.loss_snapshot = loss_acc != nullptr ? loss_snapshot : nullptr;
+  a.snap_flag = a.loss_snapshot != nullptr ? snap_flag : nullptr; a.snap_gen = snap_gen;
+  a.grads.p[0] = grads; a.grad_stride = grad_stride;
+  a.phase_ts = g_phase_ts;
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  const int blocks = sms < cn::RED_UNITS ? sms : cn::RED_UNITS;   // at most one CTA per SM
+  static const int pdl = [] { const char* e = getenv("B200DIST_PDL"); return (e == nullptr || e[0] != '0') ? 1 : 0; }();
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)blocks);
+  cfg.blockDim = dim3((unsigned)cn::RED_T);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl ? 1 : 0;
+  return (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel, a, slots, n_slots, factors, n_samples, loss_acc);
 }
 
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,

@@ -7,6 +7,20 @@ namespace b2 {
 
 constexpr int kSgdThreads = 512;
 
+// Opt-in phase timestamps of the step (bench/step_phases.py; off unless a buffer is set with b2_set_phase_ts): thread 0 of
+// every CTA writes %globaltimer (ns) into row [step % TS_STEPS][cta] of TS_PER_CTA words.  The step kernel uses words
+// 0..8 (TS_ENTRY..TS_EXIT), the optimizer kernel words 12 and 13.
+constexpr int TS_STEPS = 64, TS_CTAS = 256, TS_PER_CTA = 16;
+enum : int { TS_ENTRY = 0, TS_WAITED, TS_S2, TS_S4, TS_S6, TS_S8A, TS_S8B, TS_FLUSHED, TS_EXIT, TS_OPT_WAITED = 12, TS_OPT_EXIT };
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void ts_put(unsigned long long* ts, unsigned long long step, int cta, int k, unsigned long long t) {
+  if (ts != nullptr && cta < TS_CTAS) ts[((step % TS_STEPS) * TS_CTAS + (unsigned long long)cta) * TS_PER_CTA + k] = t;
+}
+
 struct SgdArgs {
   PeerPtrs grads;            // symmetric flat fp32 gradient buckets (grads.p[rank] is ours)
   SignalPads sig;
@@ -28,6 +42,7 @@ struct SgdArgs {
   float* loss_snapshot;      // ... copied here (2 floats) = the cumulative loss as of THIS step (per-step D2H source)
   unsigned int* snap_flag;   // optional: set to snap_gen (release, system scope) once the snapshot is written -- the executor's
   unsigned int snap_gen;     // D2H stream waits on this word (stream memory op) instead of an event behind the kernel
+  unsigned long long* phase_ts;   // optional phase timestamps (see TS_STEPS); nullptr: off
 };
 
 // Call after a __syncthreads() that follows snapshot_loss(): publishes "snapshot of this step is readable".
@@ -45,11 +60,10 @@ __device__ __forceinline__ void snapshot_loss(const SgdArgs& a) {
     a.loss_snapshot[threadIdx.x] = *reinterpret_cast<const volatile float*>(a.loss_acc + threadIdx.x);
 }
 
-// SGD update of one float4 vector (+ the pre-arranged conv2.weight copies), shared by both exchange variants
-__device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g) {
+// SGD update of one float4 vector (+ the pre-arranged conv2.weight copies), shared by both exchange variants; sgd_apply_mp
+// takes the vector's momentum and parameters already loaded
+__device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 g, float4 m, float4 p) {
   g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
-  float4 m = reinterpret_cast<float4*>(a.momentum)[v];
-  float4 p = reinterpret_cast<float4*>(a.params)[v];
   m.x = fmaf(a.mu, m.x, g.x); m.y = fmaf(a.mu, m.y, g.y); m.z = fmaf(a.mu, m.z, g.z); m.w = fmaf(a.mu, m.w, g.w);
   p.x = fmaf(-a.lr, m.x, p.x); p.y = fmaf(-a.lr, m.y, p.y); p.z = fmaf(-a.lr, m.z, p.z); p.w = fmaf(-a.lr, m.w, p.w);
   reinterpret_cast<float4*>(a.momentum)[v] = m;
@@ -64,6 +78,9 @@ __device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g) 
       a.aux[5000 + ((co * 25 + kk) * 2 + ci / 5) * 8 + ci % 5] = pw[e];            // w2b [co][ky][kx][half][8]
     }
   }
+}
+__device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g) {
+  sgd_apply_mp(a, v, g, reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]);
 }
 
 // One float4 vector `v` of the flat bucket through the push ("LL") exchange and the optimizer:

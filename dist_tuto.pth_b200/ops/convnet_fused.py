@@ -7,6 +7,9 @@ is TWO kernels here, replayed as one CUDA graph:
   1. ``convnet_step``   (csrc/convnet.cu, csrc/convnet_cluster.cu)  forward + loss +
      backward, one CTA (or one 2/4/8-CTA cluster) per sample, gradients
      ``red.add``-ed into a flat fp32 bucket that lives in symmetric peer memory;
+     on one GPU at one CTA per sample instead stored to per-CTA slots and per-sample
+     fc1 factors, which ``reduce_sgd`` (csrc/sgd.cu) sums in a fixed order and feeds
+     straight into the SGD update (no bucket, no atomics);
   2. ``allreduce_sgd``  (csrc/sgd.cu)      every rank stores its bucket, flag-in-data,
      into every peer's inbox over NVSwitch (or, ``B200DIST_SGD_PUSH=0``: flag barrier
      + loads of the peers' buckets), averages in fixed rank order, applies momentum
@@ -40,6 +43,7 @@ LAYOUT: Dict[str, int] = {"conv1.weight": 0, "conv1.bias": 252, "conv2.weight": 
                           "fc1.weight": 5284, "fc1.bias": 21284, "fc2.weight": 21336, "fc2.bias": 21836}
 NPAR = 21848
 NPAR_ALLOC = 21888          # multiple of 64 elements (two-shot / NVLS slicing for any world <= 8)
+FAC_STRIDE = 384            # per-sample fc1 factors of the step kernel: dh at [0, 50), p2 at [64, 384) (csrc/convnet_args.cuh)
 
 
 def unpack_params(flat: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -203,11 +207,22 @@ class FusedTrainer:
         # check-in, then every CTA pushes / reduces / updates a share of the bucket).  Needs the push inbox when world > 1.
         # deterministic=True: every step CTA stores its gradient sums to a private slot and `det_reduce` adds the slots in
         # CTA order (instead of float red.add into one bucket) => two runs with the same seed are bit-identical, at the
-        # price of one more small kernel and 128 x 87 KB of extra traffic per step.  (step()/graph path; the C++ executor
-        # and the fused tail keep the atomic flush.)
+        # price of one more small kernel per step.  Used with several GPUs or clusters, by step() / the graph path only (the
+        # C++ executor and the fused tail keep the atomic flush there).  One GPU at one CTA per sample needs no flag: that path
+        # has no atomics (below), in step() and in the executor alike.
         self.deterministic = bool(deterministic)
         self.sms = torch.cuda.get_device_properties(self.device).multi_processor_count
-        self.det_partials = torch.zeros(self.sms * NPAR_ALLOC, dtype=torch.float32, device=self.device) if deterministic else None
+        self.det_partials = None
+        if deterministic and not (self.world == 1 and self.cluster == 1):
+            self.det_partials = torch.zeros(self.sms * NPAR_ALLOC, dtype=torch.float32, device=self.device)
+        # One GPU, one CTA per sample (the flagship, batch >= 65): no atomics at all.  Every step CTA stores its gradient sums
+        # to its own slot and each sample its fc1 factors dh and p2 (plain stores); the optimizer kernel (`reduce_sgd`) sums
+        # them in a fixed order and applies SGD from registers.  Bit-reproducible without `deterministic`.  The buffers
+        # belong to the trainer so that captured graphs see fixed addresses, and are allocated here for every trainer whose
+        # full batch can take this path (cluster 1, or clusters that do not fit one wave and fall back to one CTA per sample).
+        self.grad_slots, self.factors = None, None
+        if self.world == 1 and (self.cluster == 1 or self.bsz * self.cluster > self.sms):
+            self._work_buffers(self.bsz)
         # opt-in (B200DIST_FUSED_TAIL=1): the grid-wide check-in replaces the PDL hand-off to the separate optimizer kernel,
         # and it needs every CTA resident, which 8-CTA clusters do not guarantee.
         self.fused_tail = (os.environ.get("B200DIST_FUSED_TAIL", "0") == "1" and not deterministic and self.cluster <= 4
@@ -243,6 +258,30 @@ class FusedTrainer:
         self.aux[5000:].copy_(wb.reshape(-1))
 
     # ------------------------------------------------------------------ kernels
+    def _step_ctas(self, B):
+        """CTAs of the one-CTA-per-sample step kernel at batch ``B`` (= slots): one per sample, at most 4 per SM beyond that."""
+        return min(B, 4 * self.sms)
+
+    def _work_buffers(self, B):
+        """Slots and factor rows for batch ``B`` (grown, never shrunk).  The full batch's buffers exist from construction;
+        only eager batches larger than it grow them, and never inside graph capture."""
+        n = self._step_ctas(B)
+        grow = (self.grad_slots is None or self.grad_slots.numel() < n * NPAR_ALLOC or self.factors is None
+                or self.factors.numel() < B * FAC_STRIDE)
+        if grow and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError(f"FusedTrainer: slot buffers for batch {B} must exist before graph capture")
+        if self.grad_slots is None or self.grad_slots.numel() < n * NPAR_ALLOC:
+            self.grad_slots = torch.zeros(n * NPAR_ALLOC, dtype=torch.float32, device=self.device)
+        if self.factors is None or self.factors.numel() < B * FAC_STRIDE:
+            self.factors = torch.zeros(B * FAC_STRIDE, dtype=torch.float32, device=self.device)
+
+    def _native_slots(self):
+        """(slots, factors) for the C++ executor when it runs the no-atomics one-GPU path (same condition as ``_kernels``)."""
+        fused = self.fused_tail and self.bsz * self.cluster <= 128
+        if self.world == 1 and self.cluster == 1 and not fused and self._step_ctas(self.bsz) == self.bsz:
+            return self.grad_slots, self.factors
+        return None, None
+
     def _kernels(self, x, y, B):
         cl = self.cluster if B * self.cluster <= self.sms else 1
         if self.fused_tail and B * cl <= 128:       # the tail's grid-wide check-in needs every CTA resident
@@ -250,6 +289,16 @@ class FusedTrainer:
                     self.ticket, None, self.wire_bf16)
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux, tail)
+            return
+        if self.world == 1 and cl == 1:
+            self._work_buffers(B)
+            n = self._step_ctas(B)
+            self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
+                                self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, n if n < B else 0, self.grad_stride,
+                                1, self.aux, None, self.grad_slots, self.factors)
+            # grads: re-zeroes the other-parity bucket, which a bucket step (fused tail, executor) may use next
+            self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
+                              self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride)
             return
         if self.deterministic and B * cl <= self.sms:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
@@ -387,7 +436,8 @@ class FusedTrainer:
                                       self.training, self.rank, self.world, self.seed, self.rank * self.bsz,
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
                                       self.cluster, self.aux, chunk, self._inbox_ptrs, loss_hist,
-                                      self.fused_tail and self.bsz * self.cluster <= 128, self.ticket, self.wire_bf16),
+                                      self.fused_tail and self.bsz * self.cluster <= 128, self.ticket, self.wire_bf16,
+                                      *self._native_slots()),
                   self.training)
             self.exec_chunk = chunk
             self._executors[id(loader)] = ex
