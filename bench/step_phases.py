@@ -5,7 +5,8 @@ Turns on the kernels' opt-in phase timestamps (``C.set_phase_ts``: thread 0 of e
 the phases, see ``csrc/sgd_device.cuh``), replays the graphs and prints one JSON line:
 
 * ``step_kernel_us``: median over CTAs and steps of each phase of ``convnet_step`` (entry -> griddepcontrol.wait returns ->
-  S2 -> S4 -> S6 -> S7/S8a -> S8b -> gradient flush -> exit), and the CTA's whole life;
+  S0 (input, RNG, staging barrier) -> S1 (conv1) -> S2 -> S4 -> S6 -> S7/S8a -> S8b -> gradient flush -> exit), and the CTA's
+  whole life;
 * ``optimizer_us``: from the last step CTA's exit to the optimizer kernel's first return from griddepcontrol.wait (``gap``),
   from there to its last CTA's exit (``work``), and the step period (first optimizer wait of one step to the next).
 
@@ -23,7 +24,8 @@ from dist_tuto.pth_b200.ops import _ext  # noqa: E402
 from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer  # noqa: E402
 
 TS_STEPS, TS_CTAS, TS_PER_CTA = 64, 256, 16          # csrc/sgd_device.cuh
-STEP_MARKS = ["entry", "waited", "s2", "s4", "s6", "s8a", "s8b", "flushed", "exit"]
+STEP_MARKS = ["entry", "waited", "s0", "s1", "s2", "s4", "s6", "s8a", "s8b", "flushed", "exit"]
+EXIT = len(STEP_MARKS) - 1
 OPT_WAITED, OPT_EXIT = 12, 13
 
 
@@ -75,12 +77,12 @@ def main():
             cta = row[:n_cta]
             for k, (a, b) in enumerate(zip(STEP_MARKS[:-1], STEP_MARKS[1:])):
                 phases[f"{a}->{b}"] += ((cta[:, k + 1] - cta[:, k]) / 1e3).tolist()
-            phases["cta_life"] += ((cta[:, 8] - cta[:, 0]) / 1e3).tolist()
+            phases["cta_life"] += ((cta[:, EXIT] - cta[:, 0]) / 1e3).tolist()
             opt = row[row[:, OPT_WAITED] > 0]
             if len(opt) == 0:
                 continue
             w0 = int(opt[:, OPT_WAITED].min())
-            gaps.append((w0 - int(cta[:, 8].max())) / 1e3)
+            gaps.append((w0 - int(cta[:, EXIT].max())) / 1e3)
             works.append((int(opt[:, OPT_EXIT].max()) - w0) / 1e3)
             if prev_wait is not None:
                 periods.append((w0 - prev_wait) / 1e3)

@@ -54,7 +54,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
                            const void* tail, float* det_partials, float* factors, const unsigned int* in_flag, unsigned int in_gen,
-                           cudaStream_t stream);
+                           int input_ready, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
                          const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
@@ -359,7 +359,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                            c10::optional<torch::Tensor> mask_out, c10::optional<torch::Tensor> step, uint64_t seed,
                            int64_t sample_base, bool training, double inv_bsz, double p_drop, int max_ctas, int64_t grad_stride, int cluster,
                            c10::optional<torch::Tensor> aux, py::object tail, c10::optional<torch::Tensor> det_partials,
-                           c10::optional<torch::Tensor> factors) {
+                           c10::optional<torch::Tensor> factors, bool input_ready) {
     check_cuda_contig(params, "params"); check_cuda_contig(x, "x"); check_cuda_contig(target, "target");
     TORCH_CHECK(params.scalar_type() == torch::kFloat32 && params.numel() >= b2_convnet_npar(), "params: flat fp32 [21848]");
     TORCH_CHECK(target.scalar_type() == torch::kInt64, "target: int64");
@@ -431,13 +431,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                         cluster, max_ctas, grad_stride, ax, tp, dp, nullptr, 0u, cur_stream()), "convnet_cluster launch");
       return;
     }
+    // input_ready: x and target were not written by the kernel right before this launch, so the step kernel may read them
+    // before its griddepcontrol.wait (Args::input_ready)
     ck_cuda(b2_convnet_step_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                    la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                   max_ctas, grad_stride, ax, tp, dp, fp, nullptr, 0u, cur_stream()), "convnet_step launch");
+                                   max_ctas, grad_stride, ax, tp, dp, fp, nullptr, 0u, input_ready ? 1 : 0, cur_stream()),
+            "convnet_step launch");
   }, py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
      py::arg("mask_out"), py::arg("step"), py::arg("seed"), py::arg("sample_base"), py::arg("training"), py::arg("inv_bsz"),
      py::arg("p_drop") = 0.5, py::arg("max_ctas") = 0, py::arg("grad_stride") = 0, py::arg("cluster") = 1, py::arg("aux") = py::none(),
-     py::arg("tail") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none());
+     py::arg("tail") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none(),
+     py::arg("input_ready") = false);
   m.def("reduce_sgd", [](torch::Tensor slots, int n_slots, torch::Tensor factors, int n_samples, torch::Tensor params,
                          torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,

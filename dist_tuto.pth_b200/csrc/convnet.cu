@@ -37,7 +37,7 @@ constexpr int T = 512;              // 16 warps per sample: the phases are laten
 struct SimtBufs {
   float w2f[250 * 20];      // [ci][ky][kx][co]          forward: 4 output channels per float4
   float w2b[500 * 16];      // [co][ky][kx][half][8]     backward-data: 5 input channels per (half)
-  float part[6 * 1440];     // conv2 partial sums [5][20][64] (5*1280 used) / dgrad partials [6][10][144]
+  float part[5 * 1440];     // conv2 partial sums [5][20][64] (5*1280 used) / dgrad partials [5][10][144] / S8b partials
   float dc2pad[DC_SIZE];      // conv2-output gradient, zero padded [20][16][16]
 };
 struct TcBufs {
@@ -57,6 +57,19 @@ union Scratch {
 constexpr int NW3 = 16000, NG = NPAR - NW3;
 __host__ __device__ constexpr int gslot(int i) { return i < W3 ? i : i - NW3; }   // flat index (not in fc1.weight) -> g
 
+// The conv1-output gradient g1 is stored cell-major, [144 pooled cells][G1_CELL] with the 10 channels of a cell side by side:
+// S8b reads the 10 channels of 3 cells per warp instruction, and S8a writes consecutive cells of one channel (odd stride:
+// the 16 float2 of a half-warp land on distinct bank pairs).
+constexpr int G1_CELL = 11;
+// S7b splits the 20 output channels of the conv2 data gradient into 5 groups of 4, each summed into its own partial plane set
+// of SimtBufs::part; S8a adds the 5 partials in group order.
+constexpr int S7B_GROUPS = 5;
+static_assert(3 * S7B_GROUPS <= T / 32 && 4 * S7B_GROUPS == 20, "S7b: three warps per group of four output channels");
+// S8b: 8 warps take 6 of the 48 cell triples each; every (warp, cell slot) leaves one partial set of 26 sums x 10 channels.
+constexpr int S8B_WARPS = 8, S8B_SET = 266;
+static_assert(48 % S8B_WARPS == 0 && S8B_WARPS <= T / 32 && S8B_SET >= 260 && S8B_SET % 32 == 10, "S8b partition");
+__host__ __device__ constexpr int g1_idx(int c, int cell) { return cell * G1_CELL + c; }
+
 // Weights arrive by 1-D bulk copies straight from `params` / `aux`, so every staged array starts on a 16-byte boundary and
 // arrays copied together are laid out as in `params`: [w1 | b1] = params[W1, W2), [w3 | b3 | w4 | b4] = params[W3, NPAR).
 struct __align__(1024) Smem {
@@ -72,7 +85,7 @@ struct __align__(1024) Smem {
   float p1[P1_SIZE];        // relu(pool(conv1))  [10][12][12], padded strides (see convnet_args.cuh)
   float p2[320];            // relu(pool(drop(conv2)))  [20][4][4]
   float g2[320];            // gradient at the pooled conv2 argmax
-  float2 g1[1440];          // (gradient at the pooled conv1 argmax, input offset of that position as int bits)
+  float2 g1[144 * G1_CELL]; // (gradient at the pooled conv1 argmax, input offset of that position as int bits), g1_idx
   float h[52];              // fc1 activation after relu+dropout
   float hm[52];             // fc1 backward mask (relu' * dropout scale)
   float dh[52];
@@ -87,7 +100,10 @@ struct __align__(1024) Smem {
   unsigned char a2[320];    // conv2 pool argmax (0..3)
   float loss_local;
   int correct_local;
+  int label;                // target of the current sample (loaded in S0 or, for a CTA's first sample, before pdl_wait)
 };
+static_assert(S7B_GROUPS * 1440 <= 5 * 1440 && 3 * S8B_WARPS * S8B_SET <= 5 * 1440 && 3 * S8B_WARPS * S8B_SET * 4 <= (int)sizeof(TcBufs::A),
+              "S7b and S8b partials fit the scratch they reuse");
 static_assert(sizeof(Smem) + 1024 <= 232448, "one CTA per SM: the launch asks for sizeof(Smem) + 1024 of the 227 KB opt-in");
 static_assert(offsetof(Smem, b1) == offsetof(Smem, w1) + (B1 - W1) * 4 && offsetof(Smem, b3) == offsetof(Smem, w3) + (B3 - W3) * 4 &&
                   offsetof(Smem, w4) == offsetof(Smem, w3) + (W4 - W3) * 4 && offsetof(Smem, b4) == offsetof(Smem, w3) + (B4 - W3) * 4,
@@ -106,11 +122,48 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   const float* __restrict__ P = a.params;
   const unsigned long long t_entry = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
 
+  // sample b's image -> s.x (normalised), its label -> s.label
+  auto load_input = [&](int b) {
+    if (a.x_u8) {
+      const uint4* xs = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(a.x) + (size_t)b * 784);
+      if (tid < 49) {                              // 784 bytes = 49 x 16
+        const uint4 q = __ldcg(xs + tid);
+        const unsigned int wv[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int e = 0; e < 16; ++e)
+          s.x[tid * 16 + e] = ((float)((wv[e >> 2] >> ((e & 3) * 8)) & 0xffu) * (1.f / 255.f) - a.mean) * a.inv_std;
+      }
+    } else {
+      const float4* xs = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.x) + (size_t)b * 784);
+      if (tid < 196) reinterpret_cast<float4*>(s.x)[tid] = __ldcg(xs + tid);
+    }
+    if (tid == 256) s.label = (int)__ldcg(a.target + b);
+  };
+
   // ---------------------------------------------------------------- P0: stage weights, zero accumulators
   b2::pdl_launch_dependents();       // the all-reduce/SGD kernel may pre-launch; it parks in its own pdl_wait
   if (a.backward) {                  // everything that does not depend on the previous kernel happens before pdl_wait
     float4* g4 = reinterpret_cast<float4*>(s.g);
     for (int i = tid; i < NG / 4; i += T) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  // The CTA's first sample is loaded before pdl_wait, so its HBM latency overlaps the wait instead of following it.  The
+  // kernel waited on is the optimizer kernel of the previous step: it writes parameters, momentum, aux, the step counter,
+  // gradient buckets and loss terms, never a batch.  x and target arrive by copies ordered ahead of this launch (CUDA graph
+  // nodes, the executor's copy stream behind an event or the in_flag word polled here).  Callers that cannot promise that
+  // (x converted by the kernel right before this one) leave input_ready off, and the sample is loaded in S0 like later ones.
+  if (tid == 0) {                    // the staging barriers live in this CTA's shared memory: set them up while waiting
+    for (int i = 0; i < 4; ++i) tc::mbar_init(&s.bar[i], 1);
+    tc::mbar_fence_init();
+  }
+  const bool early = a.input_ready && (int)blockIdx.x < a.B;
+  if (early) {
+    if (a.in_flag != nullptr) {      // the acquire of the polling thread must order every thread's loads of x and target
+      if (tid == T - 1) wait_input(a);
+      __syncthreads();
+    }
+    load_input(blockIdx.x);
+    if (!TC && a.backward)
+      for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.simt.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   b2::pdl_wait();                    // parameters / step counter written by the previous all-reduce+SGD kernel
   const unsigned long long t_waited = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
@@ -118,9 +171,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   const bool fast = (a.aux != nullptr) && !TC;
   if (tid == 0) {
     // One thread hands all weight staging to the TMA engine, in order of first use; each phase waits only for the group it
-    // reads (S1: bar 0, S2: bar 1, S3: bar 2, S7b: bar 3), so the copies overlap the input load and the earlier phases.
-    for (int i = 0; i < 4; ++i) tc::mbar_init(&s.bar[i], 1);
-    tc::mbar_fence_init();
+    // reads (S1: bar 0, S2: bar 1, S3: bar 2, S7b: bar 3), so the copies overlap the earlier phases.
     tc::fence_proxy_async_global();  // params / aux were written by the previous kernel through the generic proxy
     tc::mbar_expect_tx(&s.bar[0], (W2 - W1) * 4 + 80);
     tc::bulk_g2s(s.w1, P + W1, (W2 - W1) * 4, &s.bar[0]);                  // w1 | b1
@@ -136,7 +187,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       tc::bulk_g2s(s.u.simt.w2b, a.aux + AUX_W2B, (AUX_TOTAL - AUX_W2B) * 4, &s.bar[3]);
     }
   }
-  if (tid == T - 1) wait_input(a);   // (executor path) the H2D copy of this step's batch; the barrier that ends staging publishes it
+  if (!early && tid == T - 1) wait_input(a);   // (executor path) the H2D copy of this step's batch; the barrier that ends staging publishes it
   {
     // without aux: conv2.weight is scattered into its smem layout(s) from registers (all loads in flight before the first store)
     const float4* __restrict__ P4w2 = reinterpret_cast<const float4*>(P + W2);   // 1250 float4, 16B aligned
@@ -181,7 +232,10 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   // this step's gradient bucket (double-buffered: see sgd.cu); fc1.weight's share goes there from S6, the rest in the flush
   float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
   if (TC) tc::fence_proxy_async();
-  __syncthreads();                   // also publishes the mbarrier initialisation to every waiting thread
+  // The barrier that ends S0 publishes the mbarrier initialisation and the scattered conv2.weight before any phase reads
+  // them, so the RNG of S0 need not wait here for thread 0's copy issue.  A batch polled after the wait (above) must be
+  // published before S0 loads it.
+  if (TC || (!early && a.in_flag != nullptr)) __syncthreads();
   auto stamp = [&](int k) {          // opt-in phase timestamps (bench/step_phases.py); call after a barrier
     if (a.phase_ts != nullptr && tid == 0) b2::ts_put(a.phase_ts, step, (int)blockIdx.x, k, b2::globaltimer());
   };
@@ -192,19 +246,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
 
   for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
     // -------------------------------------------------------------- S0: input, RNG, clear scratch
-    if (a.x_u8) {
-      const uint4* xs = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(a.x) + (size_t)b * 784);
-      if (tid < 49) {                              // 784 bytes = 49 x 16
-        const uint4 q = __ldcg(xs + tid);
-        const unsigned int wv[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int e = 0; e < 16; ++e)
-          s.x[tid * 16 + e] = ((float)((wv[e >> 2] >> ((e & 3) * 8)) & 0xffu) * (1.f / 255.f) - a.mean) * a.inv_std;
-      }
-    } else {
-      const float4* xs = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.x) + (size_t)b * 784);
-      if (tid < 196) reinterpret_cast<float4*>(s.x)[tid] = __ldcg(xs + tid);
-    }
+    const bool loaded = early && b == (int)blockIdx.x;   // first sample: input and cleared dc2pad are in place already
+    if (!loaded) load_input(b);
     if (tid >= 256 && tid < 274) {
       const int q = tid - 256;
       uint4 r = b2::Philox::gen(a.seed, (unsigned long long)(a.sample_base + b), step * 32ull + q);
@@ -212,44 +255,53 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       s.rnd[q * 4 + 0] = r.x * k; s.rnd[q * 4 + 1] = r.y * k;
       s.rnd[q * 4 + 2] = r.z * k; s.rnd[q * 4 + 3] = r.w * k;
     }
-    if (!TC && a.backward)
+    if (!TC && a.backward && !loaded)
       for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.simt.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
+    stamp(b2::TS_S0);
 
     // -------------------------------------------------------------- S1: conv1 -> maxpool2 -> relu
     tc::mbar_wait(&s.bar[0], 0);                   // w1, b1, b2 (after the first sample: returns at once)
-    for (int o = tid; o < 1440; o += T) {
-      const int c = o / 144, r = o % 144, py = r / 12, px = r % 12;
-      float patch[6][6];
+    if (tid < 480) {                               // 48 threads per channel, 3 pooled cells each: the 25 weights stay in registers
+      const int c = tid / 48;
+      float w[25];
 #pragma unroll
-      for (int i = 0; i < 6; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {              // 8-byte aligned pairs: 18 LDS.64 instead of 36 LDS.32
-          const float2 q = *reinterpret_cast<const float2*>(&s.x[(2 * py + i) * 28 + 2 * px + 2 * j]);
-          patch[i][2 * j] = q.x; patch[i][2 * j + 1] = q.y;
-        }
+      for (int k = 0; k < 25; ++k) w[k] = s.w1[c * 25 + k];
       const float bias = s.b1[c];
-      float a00 = bias, a01 = bias, a10 = bias, a11 = bias;
+#pragma unroll 1
+      for (int r = tid - c * 48; r < 144; r += 48) {
+        const int o = c * 144 + r, py = r / 12, px = r % 12;
+        float patch[6][6];
 #pragma unroll
-      for (int ky = 0; ky < 5; ++ky)
+        for (int i = 0; i < 6; ++i)
 #pragma unroll
-        for (int kx = 0; kx < 5; ++kx) {
-          const float w = s.w1[c * 25 + ky * 5 + kx];
-          a00 = fmaf(w, patch[ky][kx], a00);
-          a01 = fmaf(w, patch[ky][kx + 1], a01);
-          a10 = fmaf(w, patch[ky + 1][kx], a10);
-          a11 = fmaf(w, patch[ky + 1][kx + 1], a11);
-        }
-      float m = a00; int arg = 0;
-      if (a01 > m) { m = a01; arg = 1; }
-      if (a10 > m) { m = a10; arg = 2; }
-      if (a11 > m) { m = a11; arg = 3; }
-      s.p1[p1_idx(c, py, px)] = fmaxf(m, 0.f);
-      s.a1[o] = (unsigned char)arg;
+          for (int j = 0; j < 3; ++j) {              // 8-byte aligned pairs: 18 LDS.64 instead of 36 LDS.32
+            const float2 q = *reinterpret_cast<const float2*>(&s.x[(2 * py + i) * 28 + 2 * px + 2 * j]);
+            patch[i][2 * j] = q.x; patch[i][2 * j + 1] = q.y;
+          }
+        float a00 = bias, a01 = bias, a10 = bias, a11 = bias;
+#pragma unroll
+        for (int ky = 0; ky < 5; ++ky)
+#pragma unroll
+          for (int kx = 0; kx < 5; ++kx) {
+            const float wk = w[ky * 5 + kx];
+            a00 = fmaf(wk, patch[ky][kx], a00);
+            a01 = fmaf(wk, patch[ky][kx + 1], a01);
+            a10 = fmaf(wk, patch[ky + 1][kx], a10);
+            a11 = fmaf(wk, patch[ky + 1][kx + 1], a11);
+          }
+        float m = a00; int arg = 0;
+        if (a01 > m) { m = a01; arg = 1; }
+        if (a10 > m) { m = a10; arg = 2; }
+        if (a11 > m) { m = a11; arg = 3; }
+        s.p1[p1_idx(c, py, px)] = fmaxf(m, 0.f);
+        s.a1[o] = (unsigned char)arg;
+      }
     }
     if (tid < 20)
       s.m2[tid] = a.training ? (s.rnd[tid] >= a.p_drop ? keep_scale : 0.f) : 1.f;
     __syncthreads();
+    stamp(b2::TS_S1);
 
     // -------------------------------------------------------------- S2: conv2 (TC: im2col + wgmma GEMM | SIMT: K split 5)
     if (TC) {
@@ -398,7 +450,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
 
     // -------------------------------------------------------------- S4: fc2 + log_softmax + nll
     if (tid < 32) {
-      const long long y = __ldcg(a.target + b);
+      const int y = s.label;
       float logit = -INFINITY;
       if (tid < 10) {
         float acc = s.b4[tid];
@@ -635,33 +687,33 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
           }
           const int o = (half * 5 + cil) * 144 + rem, arg = s.a1[o];
           const int off = (2 * y + (arg >> 1)) * 28 + 2 * x + (arg & 1);
-          s.g1[o] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
+          s.g1[g1_idx(half * 5 + cil, rem)] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
         }
         __syncthreads();
       }
     }
     if (!TC) {
     if (fast) tc::mbar_wait(&s.bar[3], 0);         // w2b
-    if (tid < 432) {
-      const int tile = tid % 36, half = (tid / 36) & 1, ks = tid / 72;
-      const int y0 = 2 * (tile / 6), x0 = 2 * (tile % 6);
-      const int co0 = ks < 2 ? 4 * ks : 8 + 3 * (ks - 2), co1 = ks < 2 ? co0 + 4 : co0 + 3;   // 4,4,3,3,3,3
-      float acc[4][5];
+    // Warp-uniform channel ranges: warps 3g .. 3g+2 take output channels 4g .. 4g+3 (a Dropout2d skip skips the whole warp)
+    // and together cover 12 rows x 4 column triples x 2 input-channel halves; lane = (half, row 4k + r, column triple q).
+    // The 16 (row, triple) dc2pad addresses of a load fall on distinct banks (row stride 20, triple stride 3), and the two
+    // halves read the same words.  Warp 15 and the warps whose channels are dropped go on to the S7a items.
+    if (tid < 32 * 3 * S7B_GROUPS) {
+      const int warp = tid >> 5, lane = tid & 31, cg = warp / 3;
+      const int half = lane >> 4, y = 4 * (warp - 3 * cg) + ((lane >> 2) & 3), x0 = 3 * (lane & 3);
+      float acc[3][5];
 #pragma unroll
-      for (int p = 0; p < 4; ++p)
+      for (int p = 0; p < 3; ++p)
 #pragma unroll
         for (int c = 0; c < 5; ++c) acc[p][c] = 0.f;
-      for (int co = co0; co < co1; ++co) {
-        if (s.m2[co] == 0.f) continue;            // channel dropped by Dropout2d: gradient plane is zero
-        float patch[6][6];
-        const float2* src = reinterpret_cast<const float2*>(&s.u.simt.dc2pad[co * DC_PLANE + y0 * DC_ROW + x0]);   // even offsets
+      for (int co = 4 * cg; co < 4 * cg + 4; ++co) {
+        if (s.m2[co] == 0.f) continue;            // channel dropped by Dropout2d: gradient plane is zero (warp-uniform)
+        float patch[5][7];
+        const float* src = &s.u.simt.dc2pad[co * DC_PLANE + y * DC_ROW + x0];
 #pragma unroll
-        for (int i = 0; i < 6; ++i)
+        for (int i = 0; i < 5; ++i)
 #pragma unroll
-          for (int j = 0; j < 3; ++j) {
-            const float2 q = src[i * (DC_ROW / 2) + j];
-            patch[i][2 * j] = q.x; patch[i][2 * j + 1] = q.y;
-          }
+          for (int jx = 0; jx < 7; ++jx) patch[i][jx] = src[i * DC_ROW + jx];
 #pragma unroll
         for (int ky = 0; ky < 5; ++ky)
 #pragma unroll
@@ -669,22 +721,18 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
             const float* wp = &s.u.simt.w2b[((co * 25 + ky * 5 + kx) * 2 + half) * 8];
             const float4 w = *reinterpret_cast<const float4*>(wp);
             const float w4 = wp[4];
-            const float d00 = patch[4 - ky][4 - kx], d01 = patch[4 - ky][5 - kx];
-            const float d10 = patch[5 - ky][4 - kx], d11 = patch[5 - ky][5 - kx];
-            acc[0][0] = fmaf(w.x, d00, acc[0][0]); acc[0][1] = fmaf(w.y, d00, acc[0][1]);
-            acc[0][2] = fmaf(w.z, d00, acc[0][2]); acc[0][3] = fmaf(w.w, d00, acc[0][3]); acc[0][4] = fmaf(w4, d00, acc[0][4]);
-            acc[1][0] = fmaf(w.x, d01, acc[1][0]); acc[1][1] = fmaf(w.y, d01, acc[1][1]);
-            acc[1][2] = fmaf(w.z, d01, acc[1][2]); acc[1][3] = fmaf(w.w, d01, acc[1][3]); acc[1][4] = fmaf(w4, d01, acc[1][4]);
-            acc[2][0] = fmaf(w.x, d10, acc[2][0]); acc[2][1] = fmaf(w.y, d10, acc[2][1]);
-            acc[2][2] = fmaf(w.z, d10, acc[2][2]); acc[2][3] = fmaf(w.w, d10, acc[2][3]); acc[2][4] = fmaf(w4, d10, acc[2][4]);
-            acc[3][0] = fmaf(w.x, d11, acc[3][0]); acc[3][1] = fmaf(w.y, d11, acc[3][1]);
-            acc[3][2] = fmaf(w.z, d11, acc[3][2]); acc[3][3] = fmaf(w.w, d11, acc[3][3]); acc[3][4] = fmaf(w4, d11, acc[3][4]);
+#pragma unroll
+            for (int p = 0; p < 3; ++p) {
+              const float d = patch[4 - ky][4 - kx + p];
+              acc[p][0] = fmaf(w.x, d, acc[p][0]); acc[p][1] = fmaf(w.y, d, acc[p][1]);
+              acc[p][2] = fmaf(w.z, d, acc[p][2]); acc[p][3] = fmaf(w.w, d, acc[p][3]); acc[p][4] = fmaf(w4, d, acc[p][4]);
+            }
           }
       }
 #pragma unroll
       for (int c = 0; c < 5; ++c) {
-        float* dst = &s.u.simt.part[ks * 1440 + (half * 5 + c) * 144 + y0 * 12 + x0];
-        dst[0] = acc[0][c]; dst[1] = acc[1][c]; dst[12] = acc[2][c]; dst[13] = acc[3][c];
+        float* dst = &s.u.simt.part[cg * 1440 + (half * 5 + c) * 144 + y * 12 + x0];
+        dst[0] = acc[0][c]; dst[1] = acc[1][c]; dst[2] = acc[2][c];
       }
     }
     s7a();
@@ -694,37 +742,50 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     for (int o = tid; o < 1440; o += T) {
       float d = 0.f;
 #pragma unroll
-      for (int ks = 0; ks < 6; ++ks) d += s.u.simt.part[ks * 1440 + o];
+      for (int cg = 0; cg < S7B_GROUPS; ++cg) d += s.u.simt.part[cg * 1440 + o];
       const int cell = o % 144, arg = s.a1[o];
       const int off = (2 * (cell / 12) + (arg >> 1)) * 28 + 2 * (cell % 12) + (arg & 1);
-      s.g1[o] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
+      s.g1[g1_idx(o / 144, cell)] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
     }
     __syncthreads();
     }
     stamp(b2::TS_S8A);
 
     // -------------------------------------------------------------- S8b: conv1 weight/bias gradient (sparse)
+    // Lanes over cells: lane (j, c) of warps 0-7 takes channel c of the pooled cells (py, px0 + 4j), py = t / 4, px0 = t % 4,
+    // for the 6 triples t = w, w + 8, ..., w + 40, and gathers the 5x5 input window at each cell's argmax into 25 register
+    // sums (+ the bias sum).  The addresses of one load differ by 8 banks between the three cells and by an argmax step (0,
+    // 1, 28 or 29 words) inside a cell: all 30 lanes hit distinct banks or share a word.  The 24 partial sets (one per warp
+    // and j) go to shared memory and are added in set order.
     {
-      const int out = tid >> 1, half = tid & 1;              // two lanes per tap: 72 cells each
-      float acc = 0.f, gsum = 0.f;
-      int k = 0;
-      if (tid < 500) {
-        const int c = out / 25;
-        k = out - c * 25;
-        const int koff = (k / 5) * 28 + (k % 5);
-        const float2* gp = &s.g1[c * 144 + half * 72];
-#pragma unroll 8
-        for (int cell = 0; cell < 72; ++cell) {
-          const float2 q = gp[cell];
-          gsum += q.x;                                       // bias gradient rides along (used by the k == 0 lanes)
-          acc = fmaf(q.x, s.x[__float_as_int(q.y) + koff], acc);
+      float* const red = TC ? reinterpret_cast<float*>(s.u.tc.A) : s.u.simt.part;   // [24 sets][S8B_SET], dead after S8a
+      const int lane = tid & 31, warp = tid >> 5, j = lane / 10, c = lane - j * 10;
+      if (warp < S8B_WARPS) {
+        float acc[26];
+#pragma unroll
+        for (int k = 0; k < 26; ++k) acc[k] = 0.f;
+        if (j < 3) {
+#pragma unroll 2
+          for (int t = warp; t < 48; t += S8B_WARPS) {
+            const float2 q = s.g1[g1_idx(c, (t >> 2) * 12 + (t & 3) + 4 * j)];
+            const float* src = &s.x[__float_as_int(q.y)];
+#pragma unroll
+            for (int k = 0; k < 25; ++k) acc[k] = fmaf(q.x, src[(k / 5) * 28 + k % 5], acc[k]);
+            acc[25] += q.x;
+          }
+          float* dst = red + (warp * 3 + j) * S8B_SET + c;   // set stride = 10 (mod 32): the 30 lanes store to 30 banks
+#pragma unroll
+          for (int k = 0; k < 26; ++k) dst[k * 10] = acc[k];
         }
       }
-      acc += __shfl_xor_sync(0xffffffffu, acc, 1);           // executed by every lane (no divergence at the shuffle)
-      gsum += __shfl_xor_sync(0xffffffffu, gsum, 1);
-      if (tid < 500 && half == 0) {
-        s.g[gslot(W1) + out] += acc;
-        if (k == 0) s.g[gslot(B1) + out / 25] += gsum;
+      __syncthreads();
+      if (tid < 260) {
+        float d = 0.f;
+#pragma unroll
+        for (int set = 0; set < 3 * S8B_WARPS; ++set) d += red[set * S8B_SET + tid];
+        const int k = tid / 10, ch = tid - k * 10;
+        if (k < 25) s.g[gslot(W1) + ch * 25 + k] += d;
+        else s.g[gslot(B1) + ch] += d;
       }
     }
     __syncthreads();
@@ -796,7 +857,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
                            const cn::FusedTailHost* tail, float* det_partials, float* factors, const unsigned int* in_flag,
-                           unsigned int in_gen, cudaStream_t stream) {
+                           unsigned int in_gen, int input_ready, cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cn::Smem) + 1024;
   if (!configured) {
@@ -815,7 +876,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   a.det_partials = backward ? det_partials : nullptr;
   a.factors = (backward && det_partials != nullptr) ? factors : nullptr;
   a.phase_ts = b2_phase_ts();
-  a.in_flag = in_flag; a.in_gen = in_gen;
+  a.in_flag = in_flag; a.in_gen = in_gen; a.input_ready = input_ready;
   int grid = B;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   if (grid < 1) grid = 1;

@@ -45,6 +45,8 @@ struct Args {
   const unsigned int* in_flag;   // optional "this batch has landed" word: the executor's copy stream writes in_gen there with a
   unsigned int in_gen;           // stream memory op right behind the H2D copy of x / target; the kernel polls it instead of the
                                  // compute stream waiting on an event, so consecutive steps stay one unbroken PDL kernel chain
+  int input_ready;          // x and target are not written by the kernel this one waits on (griddepcontrol.wait): the kernel
+                            // may read them before that wait returns
 };
 
 // Blocks the calling thread until the batch the kernel is about to read has landed (cyclic compare: generations wrap).

@@ -37,7 +37,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
                            const void* tail, float* det_partials, float* factors, const unsigned int* in_flag,
-                           unsigned int in_gen, cudaStream_t stream);
+                           unsigned int in_gen, int input_ready, cudaStream_t stream);
 struct PeerPtrsC { void* p[8]; };
 struct SignalPadsC { uint32_t* pad[8]; };
 int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, float* params, float* momentum,
@@ -191,7 +191,7 @@ void StepExecutor::record_step(const void* x, const long long* y, float* loss_sn
                : b2_convnet_step_launch(cfg_.params, cfg_.grads_local, x, cfg_.x_u8, y, cfg_.loss_acc, nullptr, nullptr,
                                         cfg_.step_counter, cfg_.seed, cfg_.sample_base, cfg_.B, cfg_.training, 1, 1.f / cfg_.B,
                                         cfg_.p_drop, 0, cfg_.grad_stride, cfg_.aux, tp, slots ? cfg_.grad_slots : nullptr,
-                                        slots ? cfg_.factors : nullptr, in_flag, gen, compute_);
+                                        slots ? cfg_.factors : nullptr, in_flag, gen, /*input_ready=*/1, compute_);
   int rc2 = 0;
   if (slots) {
     rc2 = b2_reduce_sgd_launch(cfg_.params, cfg_.momentum, cfg_.step_counter, cfg_.done_counter, cfg_.lr, cfg_.mu, cfg_.aux,

@@ -9,9 +9,11 @@ constexpr int kSgdThreads = 512;
 
 // Opt-in phase timestamps of the step (bench/step_phases.py; off unless a buffer is set with b2_set_phase_ts): thread 0 of
 // every CTA writes %globaltimer (ns) into row [step % TS_STEPS][cta] of TS_PER_CTA words.  The step kernel uses words
-// 0..8 (TS_ENTRY..TS_EXIT), the optimizer kernel words 12 and 13.
+// 0..10 (TS_ENTRY..TS_EXIT), the optimizer kernel words 12 and 13.
 constexpr int TS_STEPS = 64, TS_CTAS = 256, TS_PER_CTA = 16;
-enum : int { TS_ENTRY = 0, TS_WAITED, TS_S2, TS_S4, TS_S6, TS_S8A, TS_S8B, TS_FLUSHED, TS_EXIT, TS_OPT_WAITED = 12, TS_OPT_EXIT };
+enum : int { TS_ENTRY = 0, TS_WAITED, TS_S0, TS_S1, TS_S2, TS_S4, TS_S6, TS_S8A, TS_S8B, TS_FLUSHED, TS_EXIT,
+             TS_OPT_WAITED = 12, TS_OPT_EXIT };
+static_assert(TS_EXIT < TS_OPT_WAITED, "the step kernel's marks must stay in front of the optimizer's");
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

@@ -282,7 +282,10 @@ class FusedTrainer:
             return self.grad_slots, self.factors
         return None, None
 
-    def _kernels(self, x, y, B):
+    def _kernels(self, x, y, B, input_ready=True):
+        """Enqueue one step.  ``input_ready``: ``x`` and ``y`` were not written by the kernel enqueued right before this
+        step (they come from copies or from work that finished earlier), so the step kernel may load them while it waits
+        for the previous step's optimizer kernel."""
         cl = self.cluster if B * self.cluster <= self.sms else 1
         if self.fused_tail and B * cl <= 128:       # the tail's grid-wide check-in needs every CTA resident
             tail = (self._grad_ptrs, self._inbox_ptrs, self.momentum, self.lr, self.mu, 1.0 / self.world, self.rank, self.world,
@@ -295,7 +298,7 @@ class FusedTrainer:
             n = self._step_ctas(B)
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, n if n < B else 0, self.grad_stride,
-                                1, self.aux, None, self.grad_slots, self.factors)
+                                1, self.aux, None, self.grad_slots, self.factors, input_ready)
             # grads: re-zeroes the other-parity bucket, which a bucket step (fused tail, executor) may use next
             self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
                               self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride)
@@ -398,7 +401,7 @@ class FusedTrainer:
             y = target.to(self.device, non_blocking=True).contiguous()
             if x.dtype not in (torch.uint8, torch.float32):
                 x = x.to(torch.float32)
-            self._kernels(x, y, B)
+            self._kernels(x, y, B, input_ready=False)   # x may come from a conversion kernel right before the step
         self.stream.synchronize()
         self._last_loss_cum = float(self.loss_acc[0].item())
         self._nstep += 1
