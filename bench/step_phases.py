@@ -8,7 +8,10 @@ the phases, see ``csrc/sgd_device.cuh``), replays the graphs and prints one JSON
   S0 (input, RNG, staging barrier) -> S1 (conv1) -> S2 -> S4 -> S6 -> S7/S8a -> S8b -> gradient flush -> exit), and the CTA's
   whole life;
 * ``optimizer_us``: from the last step CTA's exit to the optimizer kernel's first return from griddepcontrol.wait (``gap``),
-  from there to its last CTA's exit (``work``), and the step period (first optimizer wait of one step to the next).
+  from there to its last CTA's exit (``work``), and the step period (first optimizer wait of one step to the next);
+* ``optimizer_units_us``: per kind of reduction unit of ``reduce_sgd`` (``fc1``: fc1.weight tiles, ``other``: the other
+  vectors), median and maximum over CTAs and steps of the optimizer's first wait -> this CTA's wait, wait -> the unit's loads
+  have landed (its first barrier), loads -> emit done, emit -> exit; and how often each kind was the last CTA to exit.
 
 The stamps cost a few barriers; ``bench.py`` never turns them on.  Run: ``python bench/step_phases.py [--out FILE]``."""
 import argparse
@@ -26,7 +29,8 @@ from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer  # noqa: E402
 TS_STEPS, TS_CTAS, TS_PER_CTA = 64, 256, 16          # csrc/sgd_device.cuh
 STEP_MARKS = ["entry", "waited", "s0", "s1", "s2", "s4", "s6", "s8a", "s8b", "flushed", "exit"]
 EXIT = len(STEP_MARKS) - 1
-OPT_WAITED, OPT_EXIT = 12, 13
+OPT_UNIT, OPT_WAITED, OPT_EXIT, OPT_LOADED, OPT_EMITTED = 11, 12, 13, 14, 15
+UNIT_KINDS = {1: "fc1", 2: "other"}
 
 
 def main():
@@ -64,6 +68,10 @@ def main():
     phases = {f"{a}->{b}": [] for a, b in zip(STEP_MARKS[:-1], STEP_MARKS[1:])}
     phases["cta_life"] = []
     gaps, works, periods = [], [], []
+    unit_marks = [("first_wait->wait", None, OPT_WAITED), ("wait->loaded", OPT_WAITED, OPT_LOADED),
+                  ("loaded->emitted", OPT_LOADED, OPT_EMITTED), ("emitted->exit", OPT_EMITTED, OPT_EXIT)]
+    units = {kind: {name: [] for name, _, _ in unit_marks} for kind in UNIT_KINDS.values()}
+    last_exit = {kind: 0 for kind in UNIT_KINDS.values()}
     for _ in range(args.replays):
         with torch.cuda.stream(st):                     # the clear is ordered before the replay on the same stream
             ts.zero_()
@@ -84,14 +92,28 @@ def main():
             w0 = int(opt[:, OPT_WAITED].min())
             gaps.append((w0 - int(cta[:, EXIT].max())) / 1e3)
             works.append((int(opt[:, OPT_EXIT].max()) - w0) / 1e3)
+            for code, kind in UNIT_KINDS.items():
+                u = opt[opt[:, OPT_UNIT] == code]
+                for name, a, b in unit_marks:
+                    start = u[:, a] if a is not None else w0
+                    units[kind][name] += ((u[:, b] - start) / 1e3).tolist()
+            last = int(opt[:, OPT_UNIT][opt[:, OPT_EXIT].argmax()])
+            if last in UNIT_KINDS:
+                last_exit[UNIT_KINDS[last]] += 1
             if prev_wait is not None:
                 periods.append((w0 - prev_wait) / 1e3)
             prev_wait = w0
     med = lambda xs: round(statistics.median(xs), 2) if xs else None  # noqa: E731
+    mx = lambda xs: round(max(xs), 2) if xs else None  # noqa: E731
+    last_row = t[(end - 1) % TS_STEPS]
     res = {"gpu": torch.cuda.get_device_name(dev), "bsz": bsz, "steps": len(gaps),
            "step_kernel_us": {k: med(v) for k, v in phases.items()},
            "optimizer_us": {"gap_last_step_exit_to_wait": med(gaps), "work": med(works), "step_period": med(periods),
-                            "ctas": int((t[(end - 1) % TS_STEPS][:, OPT_WAITED] > 0).sum())}}
+                            "ctas": int((last_row[:, OPT_WAITED] > 0).sum())},
+           "optimizer_units_us": {kind: {"ctas": int((last_row[:, OPT_UNIT] == code).sum()),
+                                         **{name: {"median": med(v), "max": mx(v)} for name, v in units[kind].items()}}
+                                  for code, kind in UNIT_KINDS.items()},
+           "optimizer_last_exit": last_exit}
     line = json.dumps(res)
     print(line, flush=True)
     if args.out:

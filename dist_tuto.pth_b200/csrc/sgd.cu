@@ -101,22 +101,25 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
   pdl_wait();                        // slots and factors of this step are complete and visible
   pdl_launch_dependents();
   const unsigned long long t_waited = a.phase_ts != nullptr ? globaltimer() : 0ull;
+  // Thread 0 issues the step-counter read here.  It waits for the value, stores it and checks in on done_counter only once
+  // its first unit's loads are in flight (RED_AT_ISSUED), so the read adds no round trip.  The check-in follows the read, so
+  // no CTA can see the step + 1 that the last CTA to check in publishes.
+  const unsigned long long st_read = threadIdx.x == 0 && a.step != nullptr ? *reinterpret_cast<volatile unsigned long long*>(a.step) : 0ull;
   unsigned int seen = 0u;
-  if (threadIdx.x == 0) {
-    s_step = a.step != nullptr ? *reinterpret_cast<volatile unsigned long long*>(a.step) : 0ull;
-    if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);    // consumed at the very end (latency hidden)
-  }
-  if (blockIdx.x == 0 && threadIdx.x >= cn::RED_T - 32 && loss_acc != nullptr) {   // last warp of CTA 0
-    const float2 l = cn::reduce_loss(slots, n_slots);
+  if (blockIdx.x == 0 && threadIdx.x >= cn::RED_T - 32 && loss_acc != nullptr) {   // last warp of CTA 0 (no fc1 loads)
     const int i = threadIdx.x - (cn::RED_T - 32);
+    const float prev = i < 2 ? loss_acc[i] : 0.f;    // in flight with the slot loads
+    const float2 l = cn::reduce_loss(slots, n_slots);
     if (i < 2) {                     // the only writer of loss_acc while this kernel runs
-      const float v = loss_acc[i] + (i == 0 ? l.x : l.y);
+      const float v = prev + (i == 0 ? l.x : l.y);
       loss_acc[i] = v;
       if (a.loss_snapshot != nullptr) a.loss_snapshot[i] = v;
     }
   }
   // momentum and parameters of the vectors a thread will update are loaded together with the unit's gradient terms
   struct MP { float4 m, p; };
+  unsigned long long t_mark[3] = {0ull, 0ull, 0ull};
+  int last_unit = 0;
   cn::reduce_local_grad(
       slots, n_slots, factors, n_samples, (int)blockIdx.x, (int)gridDim.x, s,
       [&](int v) { return MP{reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]}; },
@@ -126,12 +129,22 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
           const size_t z = a.grad_stride > 0 ? (size_t)((s_step & 1ull) ^ 1ull) * (size_t)a.grad_stride : 0;
           st_cg_v4(reinterpret_cast<float*>(a.grads.p[0]) + z + (size_t)v * 4, make_uint4(0u, 0u, 0u, 0u));
         }
+      },
+      [&](int point, int u) {                            // thread 0 only
+        if (point == cn::RED_AT_ISSUED && u == (int)blockIdx.x) {   // the CTA's first unit
+          s_step = st_read;
+          if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);   // consumed at the very end (latency hidden)
+        }
+        if (a.phase_ts != nullptr) { t_mark[point] = globaltimer(); last_unit = u; }
       });
   __syncthreads();                   // s_step and the loss snapshot are visible to thread 0
   publish_snapshot(a);
   const unsigned long long st = s_step;
   if (a.phase_ts != nullptr) {
     if (threadIdx.x == 0) {
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_UNIT, last_unit < cn::RED_FC1_TILES ? 1ull : 2ull);
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_LOADED, t_mark[cn::RED_AT_LOADED]);
+      ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_EMITTED, t_mark[cn::RED_AT_EMITTED]);
       ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_WAITED, t_waited);
       ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_EXIT, globaltimer());
     }

@@ -9,11 +9,12 @@ constexpr int kSgdThreads = 512;
 
 // Opt-in phase timestamps of the step (bench/step_phases.py; off unless a buffer is set with b2_set_phase_ts): thread 0 of
 // every CTA writes %globaltimer (ns) into row [step % TS_STEPS][cta] of TS_PER_CTA words.  The step kernel uses words
-// 0..10 (TS_ENTRY..TS_EXIT), the optimizer kernel words 12 and 13.
+// 0..10 (TS_ENTRY..TS_EXIT), the optimizer kernels words 11..15: reduce_sgd_kernel writes the kind of its last reduction unit
+// (TS_OPT_UNIT: 1 = fc1.weight tile, 2 = other vectors; not a time) and when that unit's loads landed and its emit was done.
 constexpr int TS_STEPS = 64, TS_CTAS = 256, TS_PER_CTA = 16;
 enum : int { TS_ENTRY = 0, TS_WAITED, TS_S0, TS_S1, TS_S2, TS_S4, TS_S6, TS_S8A, TS_S8B, TS_FLUSHED, TS_EXIT,
-             TS_OPT_WAITED = 12, TS_OPT_EXIT };
-static_assert(TS_EXIT < TS_OPT_WAITED, "the step kernel's marks must stay in front of the optimizer's");
+             TS_OPT_UNIT = 11, TS_OPT_WAITED, TS_OPT_EXIT, TS_OPT_LOADED, TS_OPT_EMITTED };
+static_assert(TS_EXIT < TS_OPT_UNIT && TS_OPT_EMITTED < TS_PER_CTA, "the step kernel's marks must stay in front of the optimizer's");
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
