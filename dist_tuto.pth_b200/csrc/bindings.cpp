@@ -44,7 +44,7 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            unsigned int* snap_flag, unsigned int snap_gen, cudaStream_t stream);
+                            cudaStream_t stream);
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad,
                        cudaStream_t stream);
 size_t b2_convnet_smem_bytes();
@@ -53,12 +53,10 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const void* tail, float* det_partials, float* factors, const unsigned int* in_flag, unsigned int in_gen,
-                           int input_ready, cudaStream_t stream);
+                           const void* tail, float* det_partials, float* factors, int input_ready, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
-                         float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
-                         const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
-                         cudaStream_t stream);
+                         float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
+                         int n_samples, float* grads, long long grad_stride, cudaStream_t stream);
 void b2_set_phase_ts(unsigned long long* p);
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
                          long long grad_stride, size_t n_elems, float* loss_acc, cudaStream_t stream);
@@ -66,8 +64,7 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
                               float inv_bsz, float p_drop, int cluster, int max_clusters, long long grad_stride,
-                              const float* aux, const void* tail, float* det_partials, const unsigned int* in_flag, unsigned int in_gen,
-                              cudaStream_t stream);
+                              const float* aux, const void* tail, float* det_partials, cudaStream_t stream);
 void b2_convnet_set_tc(int on);
 int b2_convnet_get_tc();
 int b2_gemm_available();
@@ -185,24 +182,18 @@ struct ExecutorPy {
              std::vector<unsigned long long> grad_ptrs, std::vector<unsigned long long> sig_ptrs, torch::Tensor step,
              torch::Tensor done_counter, torch::Tensor loss_acc, torch::Tensor in_dev, bool raw_u8, bool training, int rank,
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
-             int max_in_flight, int cluster, torch::Tensor aux, int chunk, std::vector<unsigned long long> inbox,
+             int max_in_flight, int cluster, torch::Tensor aux, std::vector<unsigned long long> inbox,
              torch::Tensor loss_hist, bool fused_tail, torch::Tensor ticket, bool wire_bf16, c10::optional<torch::Tensor> grad_slots,
              c10::optional<torch::Tensor> factors)
       : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist, ticket} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
     const size_t block = (l.impl->block_bytes() + 255) / 256 * 256;
-    chunk = std::max(1, std::min(chunk, 8));
-    const size_t base_blk = (size_t)std::max(2, 2 * chunk);
-    // when the caller provides room for one block per loader slot behind the chunk blocks, the per-step path uses them
-    const size_t ring = (size_t)l.impl->num_slots();
-    const bool per_slot = (size_t)in_dev.numel() >= (base_blk + ring) * block && (size_t)loss_hist.numel() >= 2 * (base_blk + ring) &&
-                          base_blk + ring <= 96;
-    const size_t nblk = per_slot ? base_blk + ring : base_blk;
+    const size_t nblk = (size_t)l.impl->num_slots();      // one device block and one loss snapshot per loader slot
     TORCH_CHECK(in_dev.is_cuda() && in_dev.scalar_type() == torch::kUInt8 && (size_t)in_dev.numel() >= nblk * block,
-                "in_dev: CUDA uint8 buffer of >= max(2, 2 * chunk) * block bytes");
-    TORCH_CHECK(loss_hist.is_cuda() && loss_hist.scalar_type() == torch::kFloat32 && (size_t)loss_hist.numel() >= 2 * base_blk,
-                "loss_hist: CUDA fp32 [2 * chunk, 2]");
+                "in_dev: CUDA uint8 buffer of >= num_slots * block bytes");
+    TORCH_CHECK(loss_hist.is_cuda() && loss_hist.scalar_type() == torch::kFloat32 && (size_t)loss_hist.numel() >= 2 * nblk,
+                "loss_hist: CUDA fp32 [num_slots, 2]");
     b2::StepConfig c;
     std::memset(&c, 0, sizeof(c));
     c.params = params.data_ptr<float>(); c.momentum = momentum.data_ptr<float>(); c.grads_local = grads.data_ptr<float>();
@@ -211,10 +202,9 @@ struct ExecutorPy {
     c.step_counter = reinterpret_cast<unsigned long long*>(step.data_ptr());
     c.done_counter = reinterpret_cast<unsigned int*>(done_counter.data_ptr());
     c.loss_acc = loss_acc.data_ptr<float>();
-    for (size_t i = 0; i < nblk; ++i) c.in_dev[i] = in_dev.data_ptr<uint8_t>() + i * block;
+    c.in_dev = in_dev.data_ptr<uint8_t>();
+    c.in_stride = block;
     c.loss_hist = loss_hist.data_ptr<float>();
-    c.ring_base = per_slot ? (int)base_blk : 0;
-    c.chunk = chunk;
     c.B = (int)l.impl->batch(); c.x_u8 = raw_u8; c.training = training;
     c.rank = rank; c.world = world; c.seed = seed; c.sample_base = sample_base; c.grad_stride = grad_stride;
     c.lr = (float)lr; c.mu = (float)mu; c.p_drop = (float)p_drop; c.cluster = cluster;
@@ -242,14 +232,8 @@ struct ExecutorPy {
     }
     const int cap = std::max(1, l.impl->num_slots() - 2);
     c10::cuda::CUDAGuard guard(params.device());
-    if (per_slot) {      // generation words of the ring path's flag mode (executor.cpp)
-      torch::Tensor flags = torch::zeros({2 * (int64_t)ring}, torch::TensorOptions().dtype(torch::kInt32).device(params.device()));
-      c10::cuda::getCurrentCUDAStream().synchronize();
-      c.flags = reinterpret_cast<unsigned int*>(flags.data_ptr());
-      keep.push_back(flags);
-    }
+    c10::cuda::getCurrentCUDAStream().synchronize();     // the executor's streams do not wait for work queued on this one
     impl = std::make_unique<b2::StepExecutor>(c, l.impl.get(), std::min(max_in_flight, cap));
-    if (!impl->prepare()) throw std::runtime_error("StepExecutor: " + impl->error());
   }
   py::tuple run(int64_t max_steps) {
     int pending = -1, epoch_done = 0;
@@ -334,7 +318,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_allreduce_sgd_launch(&g, &s, params.data_ptr<float>(), momentum.data_ptr<float>(), st, (size_t)params.numel(),
                                     (float)lr, (float)mu, (float)scale, rank, world, zero_grads, grad_stride, dc, ax,
-                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, nullptr, 0u, cur_stream()),
+                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, cur_stream()),
             "allreduce_sgd launch");
   }, py::arg("grads"), py::arg("sigs"), py::arg("params"), py::arg("momentum"), py::arg("step"), py::arg("lr"), py::arg("mu"),
      py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("zero_grads"), py::arg("grad_stride") = 0,
@@ -428,14 +412,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       TORCH_CHECK(cluster == 2 || cluster == 4 || cluster == 8, "cluster must be 1, 2, 4 or 8");
       ck_cuda(b2_convnet_cluster_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                         la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                        cluster, max_ctas, grad_stride, ax, tp, dp, nullptr, 0u, cur_stream()), "convnet_cluster launch");
+                                        cluster, max_ctas, grad_stride, ax, tp, dp, cur_stream()), "convnet_cluster launch");
       return;
     }
     // input_ready: x and target were not written by the kernel right before this launch, so the step kernel may read them
     // before its griddepcontrol.wait (Args::input_ready)
     ck_cuda(b2_convnet_step_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                    la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                   max_ctas, grad_stride, ax, tp, dp, fp, nullptr, 0u, input_ready ? 1 : 0, cur_stream()),
+                                   max_ctas, grad_stride, ax, tp, dp, fp, input_ready ? 1 : 0, cur_stream()),
             "convnet_step launch");
   }, py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
      py::arg("mask_out"), py::arg("step"), py::arg("seed"), py::arg("sample_base"), py::arg("training"), py::arg("inv_bsz"),
@@ -470,8 +454,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
-                                 nullptr, 0u, slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride,
-                                 cur_stream()),
+                                 slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, cur_stream()),
             "reduce_sgd launch");
   }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
      py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
@@ -598,25 +581,24 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   py::class_<ExecutorPy>(m, "StepExecutor")
       .def(py::init<LoaderPy&, torch::Tensor, torch::Tensor, torch::Tensor, std::vector<unsigned long long>,
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
-                    int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor, int,
+                    int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor,
                     std::vector<unsigned long long>, torch::Tensor, bool, torch::Tensor, bool, c10::optional<torch::Tensor>,
                     c10::optional<torch::Tensor>>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
            py::arg("sample_base"), py::arg("grad_stride"), py::arg("lr"), py::arg("mu"), py::arg("p_drop"),
-           py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(), py::arg("chunk") = 1,
+           py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(),
            py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(), py::arg("fused_tail") = false,
            py::arg("ticket") = torch::Tensor(), py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
            py::arg("factors") = py::none(), py::keep_alive<1, 2>())
-      .def("chunking", [](ExecutorPy& e) { return e.impl->chunking(); })
-      .def("flag_mode", [](ExecutorPy& e) { return e.impl->flag_mode(); })
-      .def("chunk_note", [](ExecutorPy& e) { return e.impl->chunk_note(); })
+      .def("chunking", [](ExecutorPy&) { return false; })      // read by bench.py: every step is issued on its own
+      .def("flag_mode", [](ExecutorPy&) { return false; })     // read by bench.py: the streams are ordered by events
       .def("stats", [](ExecutorPy& e) {
         const auto& s = e.impl->stats();
         py::dict d;
-        d["next_us"] = s.next_ns / 1e3; d["copy_wait_us"] = s.copy_wait_ns / 1e3; d["retire_us"] = s.retire_ns / 1e3;
-        d["total_us"] = s.total_ns / 1e3; d["chunk_steps"] = s.chunk_steps; d["single_steps"] = s.single_steps;
+        d["next_us"] = s.next_ns / 1e3; d["retire_us"] = s.retire_ns / 1e3; d["total_us"] = s.total_ns / 1e3;
+        d["steps"] = s.steps;
         return d;
       })
       .def("reset_stats", [](ExecutorPy& e) { e.impl->reset_stats(); })

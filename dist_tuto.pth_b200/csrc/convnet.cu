@@ -149,18 +149,14 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   // The CTA's first sample is loaded before pdl_wait, so its HBM latency overlaps the wait instead of following it.  The
   // kernel waited on is the optimizer kernel of the previous step: it writes parameters, momentum, aux, the step counter,
   // gradient buckets and loss terms, never a batch.  x and target arrive by copies ordered ahead of this launch (CUDA graph
-  // nodes, the executor's copy stream behind an event or the in_flag word polled here).  Callers that cannot promise that
-  // (x converted by the kernel right before this one) leave input_ready off, and the sample is loaded in S0 like later ones.
+  // nodes, or the executor's copy stream behind an event).  Callers that cannot promise that (x converted by the kernel
+  // right before this one) leave input_ready off, and the sample is loaded in S0 like later ones.
   if (tid == 0) {                    // the staging barriers live in this CTA's shared memory: set them up while waiting
     for (int i = 0; i < 4; ++i) tc::mbar_init(&s.bar[i], 1);
     tc::mbar_fence_init();
   }
   const bool early = a.input_ready && (int)blockIdx.x < a.B;
   if (early) {
-    if (a.in_flag != nullptr) {      // the acquire of the polling thread must order every thread's loads of x and target
-      if (tid == T - 1) wait_input(a);
-      __syncthreads();
-    }
     load_input(blockIdx.x);
     if (!TC && a.backward)
       for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.simt.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -187,7 +183,6 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       tc::bulk_g2s(s.u.simt.w2b, a.aux + AUX_W2B, (AUX_TOTAL - AUX_W2B) * 4, &s.bar[3]);
     }
   }
-  if (!early && tid == T - 1) wait_input(a);   // (executor path) the H2D copy of this step's batch; the barrier that ends staging publishes it
   {
     // without aux: conv2.weight is scattered into its smem layout(s) from registers (all loads in flight before the first store)
     const float4* __restrict__ P4w2 = reinterpret_cast<const float4*>(P + W2);   // 1250 float4, 16B aligned
@@ -233,9 +228,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
   if (TC) tc::fence_proxy_async();
   // The barrier that ends S0 publishes the mbarrier initialisation and the scattered conv2.weight before any phase reads
-  // them, so the RNG of S0 need not wait here for thread 0's copy issue.  A batch polled after the wait (above) must be
-  // published before S0 loads it.
-  if (TC || (!early && a.in_flag != nullptr)) __syncthreads();
+  // them, so the RNG of S0 need not wait here for thread 0's copy issue.
+  if (TC) __syncthreads();
   auto stamp = [&](int k) {          // opt-in phase timestamps (bench/step_phases.py); call after a barrier
     if (a.phase_ts != nullptr && tid == 0) b2::ts_put(a.phase_ts, step, (int)blockIdx.x, k, b2::globaltimer());
   };
@@ -856,8 +850,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const cn::FusedTailHost* tail, float* det_partials, float* factors, const unsigned int* in_flag,
-                           unsigned int in_gen, int input_ready, cudaStream_t stream) {
+                           const cn::FusedTailHost* tail, float* det_partials, float* factors, int input_ready,
+                           cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cn::Smem) + 1024;
   if (!configured) {
@@ -876,7 +870,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   a.det_partials = backward ? det_partials : nullptr;
   a.factors = (backward && det_partials != nullptr) ? factors : nullptr;
   a.phase_ts = b2_phase_ts();
-  a.in_flag = in_flag; a.in_gen = in_gen; a.input_ready = input_ready;
+  a.input_ready = input_ready;
   int grid = B;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   if (grid < 1) grid = 1;

@@ -42,21 +42,10 @@ struct Args {
   float* factors;           // with det_partials: sample b stores its fc1 factors dh (50) and p2 (320) to factors + b * FAC_STRIDE
                             // instead of dh (x) p2 into its slot; the slot's fc1.weight range is then left unwritten
   unsigned long long* phase_ts;   // optional phase timestamps (sgd_device.cuh: TS_STEPS); nullptr: off
-  const unsigned int* in_flag;   // optional "this batch has landed" word: the executor's copy stream writes in_gen there with a
-  unsigned int in_gen;           // stream memory op right behind the H2D copy of x / target; the kernel polls it instead of the
-                                 // compute stream waiting on an event, so consecutive steps stay one unbroken PDL kernel chain
   int input_ready;          // x and target are not written by the kernel this one waits on (griddepcontrol.wait): the kernel
                             // may read them before that wait returns
 };
 
-// Blocks the calling thread until the batch the kernel is about to read has landed (cyclic compare: generations wrap).
-__device__ __forceinline__ void wait_input(const Args& a) {
-  if (a.in_flag == nullptr) return;
-  unsigned int v;
-  do {
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.in_flag) : "memory");
-  } while ((int)(v - a.in_gen) < 0);
-}
 constexpr int DET_STRIDE = 21888;   // = NPAR_ALLOC of ops/convnet_fused.py
 constexpr int FAC_STRIDE = 384, FAC_P2 = 64;   // per-sample fc1 factors: dh at [0, 50), p2 at [FAC_P2, FAC_P2 + 320)
 

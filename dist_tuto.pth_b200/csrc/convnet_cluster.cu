@@ -89,7 +89,6 @@ __global__ void __launch_bounds__(T, 1) convnet_cluster_kernel(Args a) {
     for (int i = tid; i < NPAR / 4; i += T) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   b2::pdl_wait();
-  if (tid == T - 1) wait_input(a);   // (executor path) the H2D copy of this step's batch; the cluster barrier below publishes it
   {
     const bool fast = (a.aux != nullptr);   // conv2.weight already in both smem layouts (written by sgd.cu)
     float4 fa[3], fb[4];            // pre-arranged conv2.weight: every load is in flight before the first store
@@ -547,8 +546,7 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
                               float inv_bsz, float p_drop, int cluster, int max_clusters, long long grad_stride,
-                              const float* aux, const cn::FusedTailHost* tail, float* det_partials, const unsigned int* in_flag,
-                              unsigned int in_gen, cudaStream_t stream) {
+                              const float* aux, const cn::FusedTailHost* tail, float* det_partials, cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cnc::Smem);
   if (!configured) {
@@ -566,7 +564,6 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
   cn::fill_tail(a.tail, backward ? tail : nullptr, grad_stride);
   a.det_partials = backward ? det_partials : nullptr;
   a.factors = nullptr; a.phase_ts = nullptr;
-  a.in_flag = in_flag; a.in_gen = in_gen;
   int clusters = B;
   if (max_clusters > 0 && clusters > max_clusters) clusters = max_clusters;
   if (clusters < 1) clusters = 1;

@@ -139,11 +139,6 @@ int NativeLoader::next(int64_t* count) {
   return slot;
 }
 
-int64_t NativeLoader::full_batches_left() {
-  std::lock_guard<std::mutex> lk(mu_);
-  return std::max<int64_t>(0, (int64_t)index_.size() / batch_ - consumed_);
-}
-
 int64_t NativeLoader::consumed() {
   std::lock_guard<std::mutex> lk(mu_);
   return consumed_;

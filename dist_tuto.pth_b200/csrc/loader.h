@@ -22,7 +22,6 @@ class NativeLoader {
   int64_t num_batches() const;
   void start_epoch(int64_t epoch);
   int next(int64_t* count);
-  int64_t full_batches_left();   // full-size batches of this epoch not handed out yet
   int64_t consumed();            // batches handed out this epoch (slot of batch b = b % num_slots())
   void release();
   void stop();

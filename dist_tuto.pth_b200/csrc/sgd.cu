@@ -36,7 +36,6 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
     if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);    // result is only consumed at the very end (latency hidden)
   }
   __syncthreads();
-  publish_snapshot(a);
   uint32_t epoch = 0;
   if (world > 1) {
     epoch = barrier_epoch_load(a.sig, rank);
@@ -137,8 +136,7 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
         }
         if (a.phase_ts != nullptr) { t_mark[point] = globaltimer(); last_unit = u; }
       });
-  __syncthreads();                   // s_step and the loss snapshot are visible to thread 0
-  publish_snapshot(a);
+  __syncthreads();                   // s_step is visible to every thread
   const unsigned long long st = s_step;
   if (a.phase_ts != nullptr) {
     if (threadIdx.x == 0) {
@@ -173,7 +171,6 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_push_kernel(SgdArgs
     seen = atomicAdd(a.done_counter, 1u);
   }
   __syncthreads();
-  publish_snapshot(a);
   const unsigned long long st = s_step;
   const size_t stride = (size_t)gridDim.x * kSgdThreads;
   for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st);
@@ -247,12 +244,11 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            unsigned int* snap_flag, unsigned int snap_gen, cudaStream_t stream) {
+                            cudaStream_t stream) {
   b2::SgdArgs a;
   a.phase_ts = g_phase_ts;
   a.wire_bf16 = wire_bf16;
   a.loss_acc = loss_acc; a.loss_snapshot = (loss_acc != nullptr) ? loss_snapshot : nullptr;
-  a.snap_flag = (a.loss_snapshot != nullptr) ? snap_flag : nullptr; a.snap_gen = snap_gen;
   memset(&a.inbox, 0, sizeof(a.inbox));
   // push ("LL") exchange: needs an inbox on every rank, the double-buffered buckets and the device step counter (its epoch)
   const bool push = inbox != nullptr && world > 1;
@@ -283,16 +279,14 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
 }
 
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
-                         float* aux, float* loss_acc, float* loss_snapshot, unsigned int* snap_flag, unsigned int snap_gen,
-                         const float* slots, int n_slots, const float* factors, int n_samples, float* grads, long long grad_stride,
-                         cudaStream_t stream) {
+                         float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
+                         int n_samples, float* grads, long long grad_stride, cudaStream_t stream) {
   if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
   b2::SgdArgs a;
   memset(&a, 0, sizeof(a));
   a.params = params; a.momentum = momentum; a.step = step; a.done_counter = done_counter; a.aux = aux;
   a.n_vec = cn::NPAR / 4; a.lr = lr; a.mu = mu; a.scale = 1.f; a.rank = 0; a.world = 1;
   a.loss_acc = loss_acc; a.loss_snapshot = loss_acc != nullptr ? loss_snapshot : nullptr;
-  a.snap_flag = a.loss_snapshot != nullptr ? snap_flag : nullptr; a.snap_gen = snap_gen;
   a.grads.p[0] = grads; a.grad_stride = grad_stride;
   a.phase_ts = g_phase_ts;
   static int sms = 0;

@@ -43,18 +43,8 @@ struct SgdArgs {
                              // sums the same rounded values, so replicas stay bit-identical
   const float* loss_acc;     // optional: the step kernels' running [sum of batch-mean nll, #correct] ...
   float* loss_snapshot;      // ... copied here (2 floats) = the cumulative loss as of THIS step (per-step D2H source)
-  unsigned int* snap_flag;   // optional: set to snap_gen (release, system scope) once the snapshot is written -- the executor's
-  unsigned int snap_gen;     // D2H stream waits on this word (stream memory op) instead of an event behind the kernel
   unsigned long long* phase_ts;   // optional phase timestamps (see TS_STEPS); nullptr: off
 };
-
-// Call after a __syncthreads() that follows snapshot_loss(): publishes "snapshot of this step is readable".
-__device__ __forceinline__ void publish_snapshot(const SgdArgs& a) {
-  if (a.snap_flag != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {
-    __threadfence_system();
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.snap_flag), "r"(a.snap_gen) : "memory");
-  }
-}
 
 // The previous kernel of the stream (this step's forward/backward) is complete and the next step's kernel cannot pass its
 // own griddepcontrol.wait before this kernel ends, so loss_acc holds exactly the loss up to and including this step.

@@ -423,26 +423,17 @@ class FusedTrainer:
             if loader.batch_size != self.bsz:
                 raise ValueError("loader batch size != trainer batch size")
             block = (int(loader._l.block_bytes()) + 255) // 256 * 256
-            # Default: step by step, every kernel a plain PDL stream launch ("direct mode", csrc/executor.cpp), one device
-            # block + loss-snapshot slot per loader slot (9 driver calls per step).  Alternative: K-step direct chunks
-            # (B200DIST_EXEC_CHUNK=K: fewer calls, but the first kernel of a chunk waits for all K copies).
-            env = os.environ.get("B200DIST_EXEC_CHUNK")
-            chunk = int(env) if env is not None else 1
-            chunk = max(1, min(8, chunk))
-            while chunk > 1 and loader.num_buffers < 3 * chunk:
-                chunk -= 1
-            nblk = max(2, 2 * chunk) + loader.num_buffers          # chunk blocks + one block per loader slot
-            in_dev = torch.zeros(nblk * block, dtype=torch.uint8, device=self.device)
-            loss_hist = torch.zeros(2 * nblk, dtype=torch.float32, device=self.device)
+            # every step: plain PDL stream launches (csrc/executor.cpp), one device block + loss snapshot per loader slot
+            in_dev = torch.zeros(loader.num_buffers * block, dtype=torch.uint8, device=self.device)
+            loss_hist = torch.zeros(2 * loader.num_buffers, dtype=torch.float32, device=self.device)
             ex = (self.C.StepExecutor(loader._l, self.params, self.momentum, self.grads, self._grad_ptrs, self._sig_ptrs,
                                       self.step_counter, self.done_counter, self.loss_acc, in_dev, self.raw_uint8,
                                       self.training, self.rank, self.world, self.seed, self.rank * self.bsz,
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
-                                      self.cluster, self.aux, chunk, self._inbox_ptrs, loss_hist,
+                                      self.cluster, self.aux, self._inbox_ptrs, loss_hist,
                                       self.fused_tail and self.bsz * self.cluster <= 128, self.ticket, self.wire_bf16,
                                       *self._native_slots()),
                   self.training)
-            self.exec_chunk = chunk
             self._executors[id(loader)] = ex
         if new_epoch:
             loader.begin_epoch()
