@@ -57,6 +57,10 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, cudaStream_t stream);
+int b2_convnet_eval_max_ctas(int dev);
+int b2_convnet_eval_samples_per_cta();
+int b2_convnet_eval_launch(const float* params, const void* x, int x_u8, const long long* target, double* result, int* slots,
+                           float* out_logp, long long N, float mean, float std, int dev, cudaStream_t stream);
 void b2_set_phase_ts(unsigned long long* p);
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
                          long long grad_stride, size_t n_elems, float* loss_acc, cudaStream_t stream);
@@ -426,6 +430,48 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("p_drop") = 0.5, py::arg("max_ctas") = 0, py::arg("grad_stride") = 0, py::arg("cluster") = 1, py::arg("aux") = py::none(),
      py::arg("tail") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none(),
      py::arg("input_ready") = false);
+  // ------------------------------------------------------------------ forward-only evaluation (csrc/convnet_eval.cu)
+  m.def("convnet_eval_slot_words", [](int dev) {
+    const int n = b2_convnet_eval_max_ctas(dev);
+    TORCH_CHECK(n > 0, "convnet_eval: cannot configure the kernel on device ", dev);
+    return 2 + 2 * n;
+  }, "int32 words of the slot buffer convnet_eval needs on device `dev` (ticket + one (loss, #correct) pair per CTA)");
+  m.def("convnet_eval_samples_per_cta", [] { return b2_convnet_eval_samples_per_cta(); });
+  m.def("convnet_eval", [](torch::Tensor params, torch::Tensor x, torch::Tensor target, torch::Tensor result, torch::Tensor slots,
+                           double mean, double std, c10::optional<torch::Tensor> out_logp) {
+    check_cuda_contig(params, "params"); check_cuda_contig(x, "x"); check_cuda_contig(target, "target");
+    check_cuda_contig(result, "result"); check_cuda_contig(slots, "slots");
+    TORCH_CHECK(params.scalar_type() == torch::kFloat32 && params.numel() >= b2_convnet_npar(), "params: flat fp32 [21848]");
+    TORCH_CHECK(target.scalar_type() == torch::kInt64, "target: int64");
+    const bool u8 = x.scalar_type() == torch::kUInt8;
+    TORCH_CHECK(u8 || x.scalar_type() == torch::kFloat32, "x: float32 (normalised) or uint8 (raw)");
+    const int64_t N = target.numel();
+    TORCH_CHECK(x.numel() == N * 784, "x must be [N,28,28] (uint8) or [N,1,28,28] (float32)");
+    TORCH_CHECK(result.scalar_type() == torch::kFloat64 && result.numel() >= 3, "result: CUDA float64 [3]");
+    TORCH_CHECK(slots.scalar_type() == torch::kInt32, "slots: CUDA int32");
+    TORCH_CHECK(std > 0.0, "std must be positive");
+    const auto dev = params.device();
+    TORCH_CHECK(x.device() == dev && target.device() == dev && result.device() == dev && slots.device() == dev,
+                "params, x, target, result and slots must be on one device");
+    // the weights and each group's images arrive by 1-D bulk copies: 16-byte aligned sources
+    TORCH_CHECK(((uintptr_t)params.data_ptr() | (uintptr_t)x.data_ptr()) % 16 == 0, "params and x must be 16-byte aligned");
+    float* lp = nullptr;
+    if (out_logp.has_value()) {
+      check_cuda_contig(*out_logp, "out_logp");
+      TORCH_CHECK(out_logp->numel() == N * 10 && out_logp->scalar_type() == torch::kFloat32 && out_logp->device() == dev,
+                  "out_logp: CUDA float32 [N,10]");
+      lp = out_logp->data_ptr<float>();
+    }
+    c10::cuda::CUDAGuard guard(dev);
+    const int max_ctas = b2_convnet_eval_max_ctas(dev.index());
+    TORCH_CHECK(max_ctas > 0, "convnet_eval: cannot configure the kernel on ", dev);
+    TORCH_CHECK(slots.numel() >= 2 + 2 * (int64_t)max_ctas, "slots: int32 [convnet_eval_slot_words(device)], zero-initialised");
+    ck_cuda(b2_convnet_eval_launch(params.data_ptr<float>(), x.data_ptr(), u8 ? 1 : 0,
+                                   reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), result.data_ptr<double>(),
+                                   slots.data_ptr<int>(), lp, N, (float)mean, (float)std, dev.index(), cur_stream()),
+            "convnet_eval launch");
+  }, py::arg("params"), py::arg("x"), py::arg("target"), py::arg("result"), py::arg("slots"), py::arg("mean"), py::arg("std"),
+     py::arg("out_logp") = py::none());
   m.def("reduce_sgd", [](torch::Tensor slots, int n_slots, torch::Tensor factors, int n_samples, torch::Tensor params,
                          torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,

@@ -32,7 +32,8 @@ import torch
 from . import comm
 
 __all__ = ["Partition", "DataPartitioner", "partition_dataset", "SyntheticMNIST", "TensorImageDataset",
-           "BatchLoader", "NativeBatchLoader", "load_mnist", "write_idx", "MNIST_MEAN", "MNIST_STD", "GLOBAL_BATCH"]
+           "BatchLoader", "NativeBatchLoader", "load_mnist", "write_idx", "MNIST_MEAN", "MNIST_STD", "GLOBAL_BATCH",
+           "partition_eval_dataset", "default_eval_dataset", "eval_shard_range", "EVAL_SEED"]
 
 MNIST_MEAN, MNIST_STD = 0.1307, 0.3081   # train_dist.py:82
 GLOBAL_BATCH = 128                       # train_dist.py:85
@@ -348,6 +349,40 @@ def default_dataset(root: str = "./data", n: int = 60000, seed: int = 1234) -> T
         ds = load_mnist(root, train=True) or SyntheticMNIST(n=n, seed=seed)
         _DATASET_CACHE[key] = ds
     return ds
+
+
+EVAL_SEED = 4321        # synthetic test set: same class prototypes as the training set, different samples
+
+
+def default_eval_dataset(root: str = "./data", n: int = 10000) -> TensorImageDataset:
+    """The real MNIST test split (``t10k``) when its idx files are on disk, else ``SyntheticMNIST(n, seed=EVAL_SEED)``."""
+    key = (os.path.abspath(root), n, "eval")
+    ds = _DATASET_CACHE.get(key)
+    if ds is None:
+        ds = load_mnist(root, train=False) or SyntheticMNIST(n=n, seed=EVAL_SEED)
+        _DATASET_CACHE[key] = ds
+    return ds
+
+
+def eval_shard_range(n: int, rank: int, world_size: int) -> Tuple[int, int]:
+    """``[lo, hi)`` of rank ``rank``'s evaluation shard: ``n // world_size`` samples, one more on the first
+    ``n % world_size`` ranks, in rank order."""
+    q, r = divmod(n, world_size)
+    lo = rank * q + min(rank, r)
+    return lo, lo + q + (1 if rank < r else 0)
+
+
+def partition_eval_dataset(dataset=None, rank: Optional[int] = None, world_size: Optional[int] = None) -> Partition:
+    """This rank's contiguous shard of an evaluation set, without shuffling and without dropping a remainder: over all
+    ranks every sample is evaluated exactly once (``DataPartitioner`` drops the remainder, which is right for training)."""
+    size = comm.get_world_size() if world_size is None else world_size
+    rank = comm.get_rank() if rank is None else rank
+    if dataset is None:
+        dataset = default_eval_dataset()
+    if not 0 <= rank < size:
+        raise ValueError(f"rank {rank} outside a world of {size}")
+    lo, hi = eval_shard_range(len(dataset), rank, size)
+    return Partition(dataset, range(lo, hi))
 
 
 def partition_dataset(dataset=None, global_batch: int = GLOBAL_BATCH, seed: int = 1234,

@@ -129,6 +129,7 @@ class BatchedTrainer:
         self._graph = None
         self._loss_read = 0.0
         self.gpu_launches_per_step = 12       # 8 engine kernels + 2 wgmma GEMMs + allreduce_sgd + pack_weights
+        self._evaluator = None                # ops/convnet_eval.Evaluator, made on the first evaluate()
         with torch.cuda.stream(self.stream):
             self.C.bt_pack_weights(self.params, self.bufs.as_list())
         self.stream.synchronize()
@@ -202,6 +203,15 @@ class BatchedTrainer:
         if x.dtype != torch.uint8:
             x = x.to(torch.float32)
         return batched_forward(self.params, x)
+
+    def evaluate(self, dataset=None) -> Dict:
+        """Test loss and accuracy of the current parameters on the fp32 eval kernel (``ops.convnet_eval.evaluate``;
+        collective over the trainer's group), ordered after every step issued on the trainer's stream.  Reads only the
+        parameters; the bf16 forward of ``__call__`` is not used, since it flips near-tie argmaxes."""
+        from .convnet_eval import Evaluator
+        if self._evaluator is None:
+            self._evaluator = Evaluator(self.device, self.group)
+        return self._evaluator.run(self.params, dataset, stream=self.stream)
 
     def state_dict(self) -> Dict:
         self.stream.synchronize()

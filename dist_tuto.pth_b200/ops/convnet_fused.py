@@ -229,6 +229,7 @@ class FusedTrainer:
                            and (self.world == 1 or self.inbox_handle is not None))
         self.ticket = torch.zeros(2, dtype=torch.int32, device=self.device)
         self.gpu_launches_per_step = 1 if self.fused_tail else 2     # convnet_step (+ allreduce_sgd)
+        self._evaluator = None                      # ops/convnet_eval.Evaluator, made on the first evaluate()
         self._warm()
 
     def _reset_exchange(self):
@@ -487,6 +488,16 @@ class FusedTrainer:
         if x.dtype != torch.uint8:
             x = x.to(torch.float32)
         return convnet_forward(self.params, x)
+
+    def evaluate(self, dataset=None) -> Dict:
+        """Test loss and accuracy of the current parameters (``ops.convnet_eval.evaluate``; collective over the trainer's
+        group).  Launched on the trainer's stream, so it follows every step issued so far (graph replays, eager steps;
+        ``run_native`` returns drained), and it reads only the parameters: momentum, step counter, loss terms, exchange
+        state, captured graphs and the train / eval mode are left as they are."""
+        from .convnet_eval import Evaluator
+        if self._evaluator is None:
+            self._evaluator = Evaluator(self.device, self.group)
+        return self._evaluator.run(self.params, dataset, stream=self.stream)
 
     def state_dict(self):
         """``{'model': ..., 'momentum': ..., 'steps': ...}`` with the reference's parameter names (CPU copies)."""

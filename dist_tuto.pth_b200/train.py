@@ -30,8 +30,9 @@ import torch
 import torch.nn.functional as F
 
 from . import comm
-from .data import partition_dataset
+from .data import default_eval_dataset, partition_dataset
 from .models.convnet import Net
+from .ops.convnet_eval import evaluate
 from .ops.optim import FlatSGD
 from .utils import say
 from .utils.checkpoint import load_checkpoint, restore_optimizer, save_checkpoint
@@ -50,7 +51,8 @@ class TrainConfig:
                  global_batch: int = 128, engine: str = "auto", device: Optional[str] = None,
                  max_steps: Optional[int] = None, dataset=None, log: Callable[..., None] = say,
                  p_drop: float = 0.5, checkpoint: Optional[str] = None, resume: Optional[str] = None,
-                 checkpoint_every: Optional[int] = None, trace: Optional[str] = None):
+                 checkpoint_every: Optional[int] = None, trace: Optional[str] = None, eval_dataset=None,
+                 eval_every: int = 1):
         self.epochs, self.lr, self.momentum, self.seed = epochs, lr, momentum, seed
         self.global_batch, self.engine, self.device = global_batch, engine, device
         self.max_steps, self.dataset, self.log, self.p_drop = max_steps, dataset, log, p_drop
@@ -61,6 +63,13 @@ class TrainConfig:
         # trace: path of a Chrome / Perfetto trace (utils/trace.py) -- host spans per epoch / step phase and one device span per
         # step (torch engine) or per epoch (fused engines: their steps are launched by C++ / CUDA graphs), all ranks in one file
         self.trace = trace
+        # eval_dataset: test loss / accuracy (ops/convnet_eval.evaluate) after every `eval_every`-th epoch and after the last
+        # one; "default" = data.default_eval_dataset() (the MNIST test split, or its synthetic stand-in); None = off
+        if isinstance(eval_dataset, str) and eval_dataset != "default":
+            raise ValueError(f"TrainConfig.eval_dataset must be None, 'default' or a dataset, got {eval_dataset!r}")
+        if int(eval_every) < 1:
+            raise ValueError("TrainConfig.eval_every must be >= 1")
+        self.eval_dataset, self.eval_every = eval_dataset, int(eval_every)
 
 
 def _spans_machines() -> bool:
@@ -183,6 +192,10 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
             acc.zero_()
             return v
 
+    eval_set = None
+    if cfg.eval_dataset is not None:
+        eval_set = default_eval_dataset() if isinstance(cfg.eval_dataset, str) else cfg.eval_dataset
+    evals, eval_seconds = [], 0.0
     history, steps, t0 = [], 0, time.perf_counter()
     start_epoch = 0
     if resume_blob.get("in_progress"):            # a periodic checkpoint of an unfinished run: do the REMAINING epochs
@@ -224,6 +237,13 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         mean_loss = loss_sum / denom
         history.append(mean_loss)
         cfg.log("Rank ", comm.get_rank(), ", epoch ", epoch, ": ", mean_loss)
+        if eval_set is not None and (done or (epoch + 1) % cfg.eval_every == 0 or epoch + 1 == cfg.epochs):
+            te = time.perf_counter()
+            with tracer.span("evaluate", cat="eval", epoch=epoch):
+                r = evaluate(model, eval_set)
+            eval_seconds += time.perf_counter() - te           # kept out of `seconds` / `samples_per_s`
+            evals.append({"epoch": epoch, "loss": r["loss"], "accuracy": r["accuracy"], "correct": r["correct"], "n": r["n"]})
+            cfg.log("Rank ", rank, ", epoch ", epoch, ": test loss ", r["loss"], ", accuracy ", r["accuracy"])
         if done:
             break
         epochs_done = epoch + 1
@@ -233,13 +253,14 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
                                 epoch=epochs_done, in_progress=True)
             if size > 1:
                 comm.barrier()                   # nobody runs ahead into a failure before the checkpoint is on disk
-    elapsed = time.perf_counter() - t0
+    elapsed = time.perf_counter() - t0 - eval_seconds
     if cfg.checkpoint and comm.get_rank() == 0:
         save_checkpoint(cfg.checkpoint, model, optimizer=optimizer, steps=start_steps + steps, history=history,
                         epoch=max(0, len(history) - (1 if done else 0)), in_progress=False)
     trace_file = tracer.save(cfg.trace) if cfg.trace else None          # collective: rank 0 writes every rank's rows
     return {"loss": history, "steps": steps, "seconds": elapsed, "bsz": bsz,
-            "samples_per_s": steps * bsz * size / max(elapsed, 1e-9), "model": model, "trace": trace_file}
+            "samples_per_s": steps * bsz * size / max(elapsed, 1e-9), "model": model, "trace": trace_file,
+            "eval": evals, "eval_seconds": eval_seconds}
 
 
 def run(rank: int, size: int):

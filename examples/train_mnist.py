@@ -4,6 +4,7 @@
     python examples/train_mnist.py                       # CPU, gloo, world 2 (the reference default)
     python examples/train_mnist.py --backend b200 --size 8     # one process per GPU, fused engine
     python examples/train_mnist.py --backend b200 --size 8 --global-batch 32768   # large batch: wgmma batched engine
+    python examples/train_mnist.py --backend b200 --size 8 --eval   # + test loss / accuracy after every epoch
     python -m dist_tuto.pth_b200.spawn --size 8 --max-restarts 2 examples/train_mnist.py --external --backend b200 \
         --checkpoint run.pt --checkpoint-every 1       # supervised: a failed job is restarted and resumes from run.pt
     torchrun --nproc-per-node 8 examples/train_mnist.py --backend b200 --external
@@ -26,7 +27,8 @@ def run(rank, size):
         resume = CFG["ckpt"]                              # restarted by the launcher: continue from our own last checkpoint
     cfg = dist.TrainConfig(epochs=CFG["epochs"], lr=CFG["lr"], max_steps=CFG["max_steps"], checkpoint=CFG["ckpt"],
                            checkpoint_every=CFG["ckpt_every"], resume=resume, global_batch=CFG["global_batch"],
-                           engine=CFG["engine"], trace=CFG["trace"])
+                           engine=CFG["engine"], trace=CFG["trace"],
+                           eval_dataset="default" if CFG["eval"] else None, eval_every=CFG["eval_every"])
     out = dist.train(rank, size, cfg)
     if rank == 0:
         print(f"{out['steps']} steps, {out['samples_per_s']:.0f} samples/s (wall clock, whole job)")
@@ -46,9 +48,14 @@ if __name__ == "__main__":
     ap.add_argument("--global-batch", type=int, default=128, help="split over the ranks (train_dist.py:85: 128 // world)")
     ap.add_argument("--engine", default="auto", choices=["auto", "torch", "fused", "batched"])
     ap.add_argument("--external", action="store_true", help="rank/size from torchrun/mpirun env")
+    ap.add_argument("--eval", action="store_true",
+                    help="test loss / accuracy on the MNIST test split (or its synthetic stand-in) after every "
+                         "--eval-every-th epoch and after the last one")
+    ap.add_argument("--eval-every", type=int, default=1, help="with --eval: evaluate after every N-th epoch (default 1)")
     a = ap.parse_args()
     os.environ["B2_TRAIN_CFG"] = json.dumps(dict(epochs=a.epochs, lr=a.lr, max_steps=a.max_steps, ckpt=a.checkpoint, ckpt_every=a.checkpoint_every, resume=a.resume, trace=a.trace,
-                                                 global_batch=a.global_batch, engine=a.engine))
+                                                 global_batch=a.global_batch, engine=a.engine, eval=a.eval,
+                                                 eval_every=a.eval_every))
     if a.external:
         dist.init_from_env(run, backend=a.backend)
     else:
