@@ -46,6 +46,23 @@ def test_unrounded_model_is_the_reference_network():
             assert torch.allclose(mine[n], g, atol=2e-6, rtol=1e-4), (n, training, float((mine[n] - g).abs().max()))
 
 
+def test_overrides_with_the_models_own_values_change_nothing():
+    """Feeding the model's own conv1 output and codes, conv2 codes, P2 and fc1 output back through the overrides (as the
+    GPU tests do with the engine's) must reproduce every output bit for bit."""
+    for training in (False, True):
+        net, x, y, m2, dm = _setup(16, 7, training)
+        params = pack_params(net)
+        out = R.forward_backward(params, x, y, m2, dm)
+        again = R.forward_backward(params, x, y, m2, dm, p1_override=out["p1"],
+                                   a1_override=R.pool_codes(out["a1"], out["m1"], 24),
+                                   a2_override=R.pool_codes(out["a2"], out["mp2"], 8), p2_override=out["p2"],
+                                   hrelu_override=out["hrelu"])
+        assert bool(((R.pool_codes(out["a2"], out["mp2"], 8) & 4) != 0).any())      # the dead bit is exercised
+        for k, v in out.items():
+            if k != "named":
+                assert torch.equal(again[k], v), (k, training)
+
+
 def test_bf16_emulation_stays_within_bf16_accuracy():
     net, x, y, m2, dm = _setup(64, 5, True)
     loss, grads = _oracle(net, x, y, m2, dm)
