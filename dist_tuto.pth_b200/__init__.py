@@ -27,7 +27,7 @@ from .data import (Partition, DataPartitioner, partition_dataset, SyntheticMNIST
 from .models.convnet import Net  # noqa: F401
 from .parallel.ddp import (average_gradients, GradBucket, DistributedDataParallel,  # noqa: F401
                            broadcast_parameters)
-from .ops.optim import FlatSGD  # noqa: F401
+from .ops.optim import FlatSGD, LRSchedule  # noqa: F401
 from .ops.convnet_eval import evaluate  # noqa: F401
 from .train import run, train, TrainConfig  # noqa: F401
 

@@ -44,7 +44,9 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            cudaStream_t stream);
+                            const b2::LrSchedule* sched, cudaStream_t stream);
+int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const long long* steps, float* out, long long n,
+                               cudaStream_t stream);
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad,
                        cudaStream_t stream);
 size_t b2_convnet_smem_bytes();
@@ -56,7 +58,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            const void* tail, float* det_partials, float* factors, int input_ready, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
-                         int n_samples, float* grads, long long grad_stride, cudaStream_t stream);
+                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, cudaStream_t stream);
 int b2_convnet_eval_max_ctas(int dev);
 int b2_convnet_eval_samples_per_cta();
 int b2_convnet_eval_launch(const float* params, const void* x, int x_u8, const long long* target, double* result, int* slots,
@@ -88,6 +90,7 @@ struct FusedTailHost {            // mirrors cn::FusedTailHost (csrc/convnet_arg
   float lr, mu, scale;
   int rank, world;
   int wire_bf16;
+  b2::LrSchedule sched;
 };
 struct BtBuffers {
   void *P1, *P2, *H, *DH, *dP2, *DC, *W2K, *W2R, *W3K, *W3T;
@@ -133,6 +136,26 @@ SignalPadsH to_sig(const std::vector<unsigned long long>& v) {
 
 void check_cuda_contig(const torch::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.is_contiguous(), name, " must be a contiguous CUDA tensor");
+}
+
+// An lr schedule from its plain-tuple form (ops/optim.LRSchedule.as_tuple):
+//   (kind, warmup, total, start, gamma, min_factor, milestones); None -> no schedule (the lr as given)
+b2::LrSchedule to_sched(const py::object& o) {
+  b2::LrSchedule s;
+  std::memset(&s, 0, sizeof(s));
+  if (o.is_none()) return s;
+  auto t = o.cast<py::tuple>();
+  TORCH_CHECK(t.size() == 7, "lr_schedule: (kind, warmup, total, start, gamma, min_factor, milestones)");
+  s.kind = t[0].cast<int>();
+  TORCH_CHECK(s.kind >= b2::LRS_NONE && s.kind <= b2::LRS_COSINE, "lr_schedule: unknown kind ", s.kind);
+  s.warmup = t[1].cast<long long>(); s.total = t[2].cast<long long>();
+  s.start = t[3].cast<double>(); s.gamma = t[4].cast<double>(); s.min_factor = t[5].cast<double>();
+  auto ms = t[6].cast<std::vector<long long>>();
+  TORCH_CHECK((int)ms.size() <= b2::LRS_MAX_MILESTONES, "lr_schedule: at most 8 milestones");
+  TORCH_CHECK(s.warmup >= 0 && (s.kind != b2::LRS_COSINE || s.total > s.warmup), "lr_schedule: bad warmup / total");
+  s.n_milestones = (int)ms.size();
+  for (size_t i = 0; i < ms.size(); ++i) s.milestones[i] = ms[i];
+  return s;
 }
 
 torch::Tensor tensor_from_ptr(unsigned long long ptr, int64_t numel, py::object dtype, int device) {
@@ -188,7 +211,7 @@ struct ExecutorPy {
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
              int max_in_flight, int cluster, torch::Tensor aux, std::vector<unsigned long long> inbox,
              torch::Tensor loss_hist, bool fused_tail, torch::Tensor ticket, bool wire_bf16, c10::optional<torch::Tensor> grad_slots,
-             c10::optional<torch::Tensor> factors)
+             c10::optional<torch::Tensor> factors, py::object lr_schedule)
       : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist, ticket} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
@@ -229,6 +252,7 @@ struct ExecutorPy {
       c.factors = factors->data_ptr<float>();
     }
     c.wire_bf16 = wire_bf16 ? 1 : 0;
+    c.sched = to_sched(lr_schedule);
     if (fused_tail) {
       TORCH_CHECK(ticket.is_cuda() && ticket.scalar_type() == torch::kInt32 && ticket.numel() >= 2, "ticket: CUDA int32 [2]");
       TORCH_CHECK(world == 1 || c.push, "the fused tail needs the push inbox when world > 1");
@@ -307,8 +331,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("allreduce_sgd", [](std::vector<unsigned long long> grads, std::vector<unsigned long long> sigs, torch::Tensor params,
                             torch::Tensor momentum, c10::optional<torch::Tensor> step, double lr, double mu, double scale,
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,
-                            c10::optional<torch::Tensor> aux, std::vector<unsigned long long> inbox, bool wire_bf16) {
+                            c10::optional<torch::Tensor> aux, std::vector<unsigned long long> inbox, bool wire_bf16,
+                            py::object lr_schedule) {
     check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
+    const b2::LrSchedule sched = to_sched(lr_schedule);
     TORCH_CHECK(inbox.empty() || (int)inbox.size() == world, "inbox: one pointer per rank (or none)");
     PeerPtrs ib = to_ptrs(inbox);
     TORCH_CHECK(params.scalar_type() == torch::kFloat32 && momentum.scalar_type() == torch::kFloat32, "fp32 flat buffers");
@@ -322,12 +348,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_allreduce_sgd_launch(&g, &s, params.data_ptr<float>(), momentum.data_ptr<float>(), st, (size_t)params.numel(),
                                     (float)lr, (float)mu, (float)scale, rank, world, zero_grads, grad_stride, dc, ax,
-                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, cur_stream()),
+                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, &sched, cur_stream()),
             "allreduce_sgd launch");
   }, py::arg("grads"), py::arg("sigs"), py::arg("params"), py::arg("momentum"), py::arg("step"), py::arg("lr"), py::arg("mu"),
      py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("zero_grads"), py::arg("grad_stride") = 0,
      py::arg("done_counter") = py::none(), py::arg("aux") = py::none(), py::arg("inbox") = std::vector<unsigned long long>(),
-     py::arg("wire_bf16") = false);
+     py::arg("wire_bf16") = false, py::arg("lr_schedule") = py::none());
   m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad) {
     check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
     TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32);
@@ -367,12 +393,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     const float* ax = nullptr;
     if (aux.has_value()) { TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000); ax = aux->data_ptr<float>(); }
     // fused tail (gradient exchange + SGD inside the step kernel):
-    //   tail = (grad_ptrs, inbox_ptrs, momentum, lr, mu, scale, rank, world, ticket, loss_snapshot | None)
+    //   tail = (grad_ptrs, inbox_ptrs, momentum, lr, mu, scale, rank, world, ticket, loss_snapshot | None[, wire_bf16[, lr_schedule]])
     FusedTailHost th;
     const void* tp = nullptr;
     if (!tail.is_none()) {
       auto t = tail.cast<py::tuple>();
-      TORCH_CHECK(t.size() == 10 || t.size() == 11, "tail: 10/11-tuple");
+      TORCH_CHECK(t.size() >= 10 && t.size() <= 12, "tail: 10/11/12-tuple");
       th.wire_bf16 = 0;
       TORCH_CHECK(g != nullptr && st != nullptr && la != nullptr, "the fused tail needs grads, a step counter and loss_acc");
       auto gp = t[0].cast<std::vector<unsigned long long>>();
@@ -394,6 +420,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       th.ticket = reinterpret_cast<unsigned int*>(tick.data_ptr());
       th.lr = t[3].cast<float>(); th.mu = t[4].cast<float>(); th.scale = t[5].cast<float>();
       th.wire_bf16 = t.size() > 10 ? (t[10].cast<bool>() ? 1 : 0) : 0;
+      th.sched = to_sched(t.size() > 11 ? py::object(t[11]) : py::none());
       tp = &th;
     }
     float* dp = nullptr;
@@ -475,7 +502,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("reduce_sgd", [](torch::Tensor slots, int n_slots, torch::Tensor factors, int n_samples, torch::Tensor params,
                          torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,
-                         c10::optional<torch::Tensor> grads, int64_t grad_stride) {
+                         c10::optional<torch::Tensor> grads, int64_t grad_stride, py::object lr_schedule) {
     // one-GPU optimizer step from convnet_step(..., det_partials=slots, factors=factors): the local gradient is summed from
     // the first n_slots slots and n_samples factor rows in a fixed order, then SGD is applied to it.  The gradient bucket is
     // not read; given `grads`, its other-parity half is re-zeroed like allreduce_sgd does, so a bucket step may follow.
@@ -498,13 +525,26 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                   "grads: fp32 [npar + grad_stride]");
       g = grads->data_ptr<float>();
     }
+    const b2::LrSchedule sched = to_sched(lr_schedule);
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
-                                 slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, cur_stream()),
+                                 slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, &sched,
+                                 cur_stream()),
             "reduce_sgd launch");
   }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
      py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
-     py::arg("grads") = py::none(), py::arg("grad_stride") = 0);
+     py::arg("grads") = py::none(), py::arg("grad_stride") = 0, py::arg("lr_schedule") = py::none());
+  m.def("lr_schedule_eval", [](py::object schedule, double lr, torch::Tensor steps) {
+    // the fp32 lr the optimizer kernels apply at each step-counter value of `steps`, computed by the same device function
+    check_cuda_contig(steps, "steps");
+    TORCH_CHECK(steps.scalar_type() == torch::kInt64, "steps: CUDA int64");
+    const b2::LrSchedule sched = to_sched(schedule);
+    auto out = torch::empty({steps.numel()}, steps.options().dtype(torch::kFloat32));
+    c10::cuda::CUDAGuard guard(steps.device());
+    ck_cuda(b2_lr_schedule_eval_launch(&sched, (float)lr, reinterpret_cast<const long long*>(steps.data_ptr<int64_t>()),
+                                       out.data_ptr<float>(), steps.numel(), cur_stream()), "lr_schedule_eval launch");
+    return out;
+  }, py::arg("schedule"), py::arg("lr"), py::arg("steps"));
   m.def("set_phase_ts", [](c10::optional<torch::Tensor> ts) {
     // opt-in phase timestamps of later step / optimizer launches (bench/step_phases.py); None turns them off
     if (ts.has_value()) TORCH_CHECK(ts->is_cuda() && ts->scalar_type() == torch::kInt64 && ts->numel() >= 64 * 256 * 16, "ts: int64 [64*256*16]");
@@ -629,7 +669,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
                     int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor,
                     std::vector<unsigned long long>, torch::Tensor, bool, torch::Tensor, bool, c10::optional<torch::Tensor>,
-                    c10::optional<torch::Tensor>>(),
+                    c10::optional<torch::Tensor>, py::object>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
@@ -637,7 +677,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(),
            py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(), py::arg("fused_tail") = false,
            py::arg("ticket") = torch::Tensor(), py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
-           py::arg("factors") = py::none(), py::keep_alive<1, 2>())
+           py::arg("factors") = py::none(), py::arg("lr_schedule") = py::none(), py::keep_alive<1, 2>())
       .def("chunking", [](ExecutorPy&) { return false; })      // read by bench.py: every step is issued on its own
       .def("flag_mode", [](ExecutorPy&) { return false; })     // read by bench.py: the streams are ordered by events
       .def("stats", [](ExecutorPy& e) {

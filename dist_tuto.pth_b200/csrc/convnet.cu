@@ -824,7 +824,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   }
   stamp(b2::TS_EXIT);
   // ------------------------------------------------------------------ fused tail: gradient exchange + SGD in this kernel
-  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x);   // grid <= B: every CTA flushed
+  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x, reinterpret_cast<float*>(smem_raw));   // grid <= B: every CTA flushed
 }
 
 }  // namespace cn

@@ -63,6 +63,7 @@ struct FusedTailHost {
   float lr, mu, scale;
   int rank, world;
   int wire_bf16;
+  b2::LrSchedule sched;     // lr schedule of the tail's update (zero: constant lr)
 };
 
 inline void fill_tail(b2::FusedTail& t, const FusedTailHost* h, long long grad_stride) {
@@ -74,6 +75,7 @@ inline void fill_tail(b2::FusedTail& t, const FusedTailHost* h, long long grad_s
   t.sgd.n_vec = NPAR / 4; t.sgd.lr = h->lr; t.sgd.mu = h->mu; t.sgd.scale = h->scale; t.sgd.rank = h->rank; t.sgd.world = h->world;
   t.sgd.zero_grads = 1; t.sgd.grad_stride = grad_stride; t.sgd.aux = h->aux;
   t.sgd.wire_bf16 = h->wire_bf16;
+  t.sgd.sched = h->sched;
   t.sgd.loss_acc = h->loss_acc; t.sgd.loss_snapshot = h->loss_acc ? h->loss_snapshot : nullptr;
   t.ticket = h->ticket;
 }

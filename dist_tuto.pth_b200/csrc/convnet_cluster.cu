@@ -534,7 +534,7 @@ __global__ void __launch_bounds__(T, 1) convnet_cluster_kernel(Args a) {
   }
   cl.sync();                                       // no CTA exits while a peer may still address its shared memory
   // fused tail: gradient exchange + SGD in this kernel (every cluster carried >= 1 sample: gridDim.x / C <= B)
-  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x);
+  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x, reinterpret_cast<float*>(smem_raw));
 }
 
 }  // namespace cnc

@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "loader.h"
+#include "lr_schedule.h"
 
 namespace b2 {
 
@@ -35,6 +36,7 @@ struct StepConfig {
   unsigned int* ticket;              // device scratch of the fused tail
   float* grad_slots;                 // one GPU, one CTA per sample: per-CTA slots [B][21888] and per-sample fc1 factors [B][384]
   float* factors;                    // of the step kernel, summed by reduce_sgd (sgd.cu) instead of red.add into the bucket
+  LrSchedule sched;                  // lr schedule of every step's update (zero: constant lr)
 };
 
 class StepExecutor {

@@ -24,6 +24,7 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
   // checks in with an atomic; the LAST block to check in knows every block has read it and bumps it right away, so
   // the atomic's latency hides behind the rest of the kernel and no block can see the new value.
   __shared__ unsigned int s_par;
+  __shared__ float s_lr;
   pdl_wait();                        // gradients of this step (previous kernel) are complete and visible
   pdl_launch_dependents();           // the next step's forward/backward kernel may pre-launch now (it zeroes its smem, then waits)
   const unsigned long long t_waited = a.phase_ts != nullptr ? globaltimer() : 0ull;
@@ -34,8 +35,10 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
     st = a.step != nullptr ? *reinterpret_cast<volatile unsigned long long*>(a.step) : 0ull;
     s_par = (unsigned int)(st & 1ull);
     if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);    // result is only consumed at the very end (latency hidden)
+    s_lr = step_lr(a, st);
   }
   __syncthreads();
+  const float lr = s_lr;
   uint32_t epoch = 0;
   if (world > 1) {
     epoch = barrier_epoch_load(a.sig, rank);
@@ -64,7 +67,7 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
           g.x += __uint_as_float(raw[r].x); g.y += __uint_as_float(raw[r].y);
           g.z += __uint_as_float(raw[r].z); g.w += __uint_as_float(raw[r].w);
         }
-      sgd_apply(a, v, g);
+      sgd_apply(a, v, g, lr);
     }
     if (a.zero_grads) {
       if (dbuf) {
@@ -93,10 +96,16 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
 // bit-reproducible.  Also bumps the step counter, snapshots the loss and refreshes aux like the kernels above, and re-zeroes the
 // gradient bucket of the other step parity as they do (a.grads.p[0], optional): a trainer may still run a bucket step next (the
 // fused tail, a batch on another path), and every bucket step relies on finding its bucket zeroed by the step before it.
+//
+// kSched: a.sched is a schedule (kind != LRS_NONE).  Thread 0 then also evaluates the step's lr where it waits for the
+// step counter, and the emits read it from shared memory.  Without a schedule the kernel is compiled without that code:
+// the fp64 schedule code costs this latency-bound kernel registers and instruction order even where it does not run.
+template <bool kSched>
 __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const float* __restrict__ slots, int n_slots,
                                                                const float* __restrict__ factors, int n_samples, float* loss_acc) {
   __shared__ cn::RedSmem s;
   __shared__ unsigned long long s_step;
+  __shared__ float s_lr;
   pdl_wait();                        // slots and factors of this step are complete and visible
   pdl_launch_dependents();
   const unsigned long long t_waited = a.phase_ts != nullptr ? globaltimer() : 0ull;
@@ -123,8 +132,8 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
       slots, n_slots, factors, n_samples, (int)blockIdx.x, (int)gridDim.x, s,
       [&](int v) { return MP{reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]}; },
       [&](int v, float4 g, const MP& h) {
-        sgd_apply_mp(a, (size_t)v, g, h.m, h.p);
-        if (a.grads.p[0] != nullptr) {                   // s_step: written before the routine's first barrier
+        sgd_apply_mp(a, (size_t)v, g, h.m, h.p, kSched ? s_lr : a.lr);   // s_lr, s_step: written before the first barrier
+        if (a.grads.p[0] != nullptr) {
           const size_t z = a.grad_stride > 0 ? (size_t)((s_step & 1ull) ^ 1ull) * (size_t)a.grad_stride : 0;
           st_cg_v4(reinterpret_cast<float*>(a.grads.p[0]) + z + (size_t)v * 4, make_uint4(0u, 0u, 0u, 0u));
         }
@@ -133,6 +142,7 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
         if (point == cn::RED_AT_ISSUED && u == (int)blockIdx.x) {   // the CTA's first unit
           s_step = st_read;
           if (a.step != nullptr) seen = atomicAdd(a.done_counter, 1u);   // consumed at the very end (latency hidden)
+          if (kSched) s_lr = step_lr(a, st_read);
         }
         if (a.phase_ts != nullptr) { t_mark[point] = globaltimer(); last_unit = u; }
       });
@@ -162,6 +172,7 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
 // step in between, which I issue after I finished reading parity p.
 __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_push_kernel(SgdArgs a) {
   __shared__ unsigned long long s_step;
+  __shared__ float s_lr;
   pdl_wait();
   pdl_launch_dependents();
   snapshot_loss(a);
@@ -169,11 +180,13 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_push_kernel(SgdArgs
   if (threadIdx.x == 0) {
     s_step = *reinterpret_cast<volatile unsigned long long*>(a.step);
     seen = atomicAdd(a.done_counter, 1u);
+    s_lr = step_lr(a, s_step);
   }
   __syncthreads();
   const unsigned long long st = s_step;
+  const float lr = s_lr;
   const size_t stride = (size_t)gridDim.x * kSgdThreads;
-  for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st);
+  for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st, lr);
   if (threadIdx.x == 0 && seen == gridDim.x - 1) { *a.done_counter = 0u; *a.step = st + 1ull; }
 }
 
@@ -232,6 +245,13 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
   }
 }
 
+// out[i] = the lr the optimizer kernels apply when the step counter reads steps[i] (tests tie it to ops/optim.LRSchedule)
+__global__ void __launch_bounds__(256) lr_schedule_eval_kernel(LrSchedule s, float base, const long long* __restrict__ steps,
+                                                               float* __restrict__ out, long long n) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i < n) out[i] = lr_schedule_lr(s, base, (unsigned long long)steps[i]);
+}
+
 }  // namespace b2
 
 extern "C" {
@@ -244,9 +264,11 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            cudaStream_t stream) {
+                            const b2::LrSchedule* sched, cudaStream_t stream) {
   b2::SgdArgs a;
   a.phase_ts = g_phase_ts;
+  memset(&a.sched, 0, sizeof(a.sched));
+  if (sched != nullptr) a.sched = *sched;
   a.wire_bf16 = wire_bf16;
   a.loss_acc = loss_acc; a.loss_snapshot = (loss_acc != nullptr) ? loss_snapshot : nullptr;
   memset(&a.inbox, 0, sizeof(a.inbox));
@@ -280,10 +302,11 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
 
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
-                         int n_samples, float* grads, long long grad_stride, cudaStream_t stream) {
+                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, cudaStream_t stream) {
   if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
   b2::SgdArgs a;
   memset(&a, 0, sizeof(a));
+  if (sched != nullptr) a.sched = *sched;
   a.params = params; a.momentum = momentum; a.step = step; a.done_counter = done_counter; a.aux = aux;
   a.n_vec = cn::NPAR / 4; a.lr = lr; a.mu = mu; a.scale = 1.f; a.rank = 0; a.world = 1;
   a.loss_acc = loss_acc; a.loss_snapshot = loss_acc != nullptr ? loss_snapshot : nullptr;
@@ -307,7 +330,9 @@ int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* ste
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel, a, slots, n_slots, factors, n_samples, loss_acc);
+  return a.sched.kind != b2::LRS_NONE
+             ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true>, a, slots, n_slots, factors, n_samples, loss_acc)
+             : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false>, a, slots, n_slots, factors, n_samples, loss_acc);
 }
 
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
@@ -324,6 +349,13 @@ int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stri
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return (int)cudaLaunchKernelEx(&cfg, b2::det_reduce_kernel, partials, n_slots, slot_stride, grads, step, grad_stride, n_vec, loss_acc);
+}
+
+int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const long long* steps, float* out, long long n,
+                               cudaStream_t stream) {
+  if (n <= 0) return 0;
+  b2::lr_schedule_eval_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(*sched, base, steps, out, n);
+  return (int)cudaGetLastError();
 }
 
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad,

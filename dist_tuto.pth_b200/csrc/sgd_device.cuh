@@ -2,6 +2,7 @@
 // kernels (sgd.cu) and by the tail of the fused step kernels (convnet.cu / convnet_cluster.cu, "one kernel per step").
 #pragma once
 #include "common.cuh"
+#include "lr_schedule.h"
 
 namespace b2 {
 
@@ -44,7 +45,17 @@ struct SgdArgs {
   const float* loss_acc;     // optional: the step kernels' running [sum of batch-mean nll, #correct] ...
   float* loss_snapshot;      // ... copied here (2 floats) = the cumulative loss as of THIS step (per-step D2H source)
   unsigned long long* phase_ts;   // optional phase timestamps (see TS_STEPS); nullptr: off
+  LrSchedule sched;          // lr of the update = lr_schedule_lr(sched, lr, step counter); kind LRS_NONE: lr as it is
 };
+
+// The lr of the update run at step counter `st`; the kernels evaluate it in thread 0 and share it through shared memory.
+__device__ __forceinline__ float step_lr(const SgdArgs& a, unsigned long long st) { return lr_schedule_lr(a.sched, a.lr, st); }
+// The same, out of line, for the tail of the step kernels: their code and register allocation stay those of a kernel
+// without the fp64 schedule code, which only runs (behind one call from thread 0) when there is a schedule.  The schedule
+// is passed by value, so the kernel parameters are not copied to local memory.
+static __device__ __noinline__ float scheduled_lr(LrSchedule s, float base, unsigned long long st) {
+  return lr_schedule_lr(s, base, st);
+}
 
 // The previous kernel of the stream (this step's forward/backward) is complete and the next step's kernel cannot pass its
 // own griddepcontrol.wait before this kernel ends, so loss_acc holds exactly the loss up to and including this step.
@@ -54,11 +65,11 @@ __device__ __forceinline__ void snapshot_loss(const SgdArgs& a) {
 }
 
 // SGD update of one float4 vector (+ the pre-arranged conv2.weight copies), shared by both exchange variants; sgd_apply_mp
-// takes the vector's momentum and parameters already loaded
-__device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 g, float4 m, float4 p) {
+// takes the vector's momentum and parameters already loaded; `lr` is this step's (step_lr)
+__device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 g, float4 m, float4 p, float lr) {
   g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
   m.x = fmaf(a.mu, m.x, g.x); m.y = fmaf(a.mu, m.y, g.y); m.z = fmaf(a.mu, m.z, g.z); m.w = fmaf(a.mu, m.w, g.w);
-  p.x = fmaf(-a.lr, m.x, p.x); p.y = fmaf(-a.lr, m.y, p.y); p.z = fmaf(-a.lr, m.z, p.z); p.w = fmaf(-a.lr, m.w, p.w);
+  p.x = fmaf(-lr, m.x, p.x); p.y = fmaf(-lr, m.y, p.y); p.z = fmaf(-lr, m.z, p.z); p.w = fmaf(-lr, m.w, p.w);
   reinterpret_cast<float4*>(a.momentum)[v] = m;
   reinterpret_cast<float4*>(a.params)[v] = p;
   if (a.aux != nullptr && v >= 264 / 4 && v < (264 + 5000) / 4) {      // conv2.weight (flat offset 264, 5000 elements)
@@ -72,15 +83,15 @@ __device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 
     }
   }
 }
-__device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g) {
-  sgd_apply_mp(a, v, g, reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]);
+__device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g, float lr) {
+  sgd_apply_mp(a, v, g, reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v], lr);
 }
 
 // One float4 vector `v` of the flat bucket through the push ("LL") exchange and the optimizer:
 //   store my value, flag-in-data, into every peer's inbox (16-byte lines {v0, epoch, v1, epoch}); sum the world lines of this
 //   vector out of MY inbox in fixed rank order (own contribution from registers) => bit-identical replicas; SGD; re-zero the
-//   other-parity bucket.  world == 1: no exchange.  `st` = step index (epoch = st + 1, parity = st & 1).
-__device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, unsigned long long st) {
+//   other-parity bucket.  world == 1: no exchange.  `st` = step index (epoch = st + 1, parity = st & 1), `lr` = step_lr(a, st).
+__device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, unsigned long long st, float lr) {
   const int rank = a.rank, world = a.world;
   const uint32_t epoch = (uint32_t)(st + 1ull);
   const size_t ipar = (size_t)(st & 1ull);                              // inbox lines are double-buffered by step parity
@@ -166,7 +177,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
   } else {
     g = make_float4(__uint_as_float(mine.x), __uint_as_float(mine.y), __uint_as_float(mine.z), __uint_as_float(mine.w));
   }
-  sgd_apply(a, v, g);
+  sgd_apply(a, v, g, lr);
   if (a.zero_grads) {
     const size_t z_off = a.grad_stride > 0 ? (par ^ 1) * (size_t)a.grad_stride * sizeof(float) : 0;
     st_cg_v4(reinterpret_cast<uint4*>(reinterpret_cast<char*>(a.grads.p[rank]) + z_off) + v, make_uint4(0u, 0u, 0u, 0u));
@@ -195,8 +206,9 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* addr) {
 }
 
 // All threads of every participating CTA call this after their gradient flush / loss atomics.  `st` = step index read at
-// kernel start, `cta` in [0, n_cta).
-__device__ __forceinline__ void fused_tail(const FusedTail& t, unsigned long long st, int n_cta, int cta) {
+// kernel start, `cta` in [0, n_cta).  `lr_word`: a word of the CTA's shared memory that nothing uses any more once every
+// thread has arrived here; thread 0 passes the step's lr to the other threads through it.
+__device__ __forceinline__ void fused_tail(const FusedTail& t, unsigned long long st, int n_cta, int cta, float* lr_word) {
   __syncthreads();                                   // this CTA's red.adds and loss atomics are issued
   if (threadIdx.x == 0) {
     __threadfence();                                 // ... and ordered before the check-in (cumulative over the barrier)
@@ -208,10 +220,12 @@ __device__ __forceinline__ void fused_tail(const FusedTail& t, unsigned long lon
         __trap();
       }
     }
+    *lr_word = t.sgd.sched.kind == LRS_NONE ? t.sgd.lr : scheduled_lr(t.sgd.sched, t.sgd.lr, st);
   }
   __syncthreads();
+  const float lr = *lr_word;
   for (size_t v = (size_t)cta * blockDim.x + threadIdx.x; v < t.sgd.n_vec; v += (size_t)n_cta * blockDim.x)
-    exchange_apply_vec(t.sgd, v, st);
+    exchange_apply_vec(t.sgd, v, st, lr);
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();

@@ -19,6 +19,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import Net
 from . import _ext
+from .optim import LRSchedule, schedule_tuple
 from .convnet_fused import LAYOUT, NPAR, NPAR_ALLOC, pack_params, unpack_params  # noqa: F401
 
 __all__ = ["BatchedBuffers", "batched_loss_and_grads", "batched_forward", "BatchedTrainer", "STAGES"]
@@ -89,10 +90,12 @@ class BatchedTrainer:
 
     def __init__(self, bsz: int, lr: float = 0.01, momentum: float = 0.5, seed: int = 1234, device=None,
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, use_graph: bool = True,
-                 init_from: Optional[Net] = None):
+                 init_from: Optional[Net] = None, lr_schedule: Optional[LRSchedule] = None):
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
-        self.bsz, self.lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        self._sched = schedule_tuple(lr_schedule)       # computed per update by the optimizer kernel (csrc/lr_schedule.h)
+        self.lr_schedule = lr_schedule
         self.group = group
         self.world = comm.get_world_size(group)
         self.rank = comm.group_ranks(group).index(comm.get_rank()) if comm.is_initialized() else 0
@@ -144,7 +147,8 @@ class BatchedTrainer:
         # re-zero) -- at >= 100 us per step the exchange latency is irrelevant, the fusion (no separate /world, SGD,
         # zero_grad passes) is what is kept
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
-                             self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, 0, self.done_counter, None, [])
+                             self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, 0, self.done_counter, None, [],
+                             lr_schedule=self._sched)
         self.C.bt_pack_weights(self.params, self.bufs.as_list())
 
     def step_device(self, x: torch.Tensor, y: torch.Tensor) -> None:
@@ -184,6 +188,30 @@ class BatchedTrainer:
         self._loss_read = cum
         return out
 
+    # ------------------------------------------------------------------ learning rate
+    @property
+    def lr(self) -> float:
+        """Base learning rate.  Assigning it takes effect from the next step (the step graph is re-captured)."""
+        return self._lr
+
+    @lr.setter
+    def lr(self, value: float) -> None:
+        self.stream.synchronize()
+        self._lr, self._graph = float(value), None
+
+    def set_lr_schedule(self, schedule: Optional[LRSchedule]) -> None:
+        """Replace the lr schedule (``None``: constant ``lr``) from the next step on."""
+        tup = schedule_tuple(schedule)
+        self.stream.synchronize()
+        self._sched, self.lr_schedule, self._graph = tup, schedule, None
+
+    def lr_at(self, step: Optional[int] = None) -> float:
+        """The lr the optimizer kernel applies when the step counter reads ``step`` (default: its current value)."""
+        if step is None:
+            self.stream.synchronize()
+            step = int(self.step_counter.item())
+        return self._lr if self.lr_schedule is None else self.lr_schedule.lr_at(self._lr, step)
+
     # ------------------------------------------------------------------ nn.Module-like surface
     def train(self, mode: bool = True):
         if mode != self.training:
@@ -218,7 +246,8 @@ class BatchedTrainer:
         p, m = unpack_params(self.params), unpack_params(self.momentum)
         return {"model": {k: v.detach().cpu().clone() for k, v in p.items()},
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
-                "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu}
+                "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
+                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict()}
 
     def load_state_dict(self, sd) -> None:
         self.stream.synchronize()

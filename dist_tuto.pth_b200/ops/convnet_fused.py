@@ -34,6 +34,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import PARAM_SHAPES, Net
 from . import _ext
+from .optim import LRSchedule, schedule_tuple
 
 __all__ = ["LAYOUT", "NPAR", "pack_params", "unpack_params", "convnet_loss_and_grads", "convnet_forward",
            "FusedTrainer"]
@@ -122,10 +123,15 @@ class FusedTrainer:
     def __init__(self, bsz: int, lr: float = 0.01, momentum: float = 0.5, seed: int = 1234, device=None,
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, num_slots: int = 4,
                  use_graph: bool = True, init_from: Optional[Net] = None, cluster: Optional[int] = None,
-                 deterministic: bool = False, grad_wire: Optional[torch.dtype] = None):
+                 deterministic: bool = False, grad_wire: Optional[torch.dtype] = None,
+                 lr_schedule: Optional[LRSchedule] = None):
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
-        self.bsz, self.lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        # lr_schedule (ops/optim.LRSchedule, step units): the optimizer kernels compute each update's lr from the device step
+        # counter (csrc/lr_schedule.h), so graph replays, run_native and the fused tail follow it with fixed launch arguments
+        self._sched = schedule_tuple(lr_schedule)
+        self.lr_schedule = lr_schedule
         self.group = group
         # grad_wire=torch.bfloat16: the push exchange sends the locally reduced gradients as bf16 (one 16-byte line per
         # float4 instead of two: half the NVLink bytes, stores and polling loads); accumulation and master weights stay fp32
@@ -290,7 +296,7 @@ class FusedTrainer:
         cl = self.cluster if B * self.cluster <= self.sms else 1
         if self.fused_tail and B * cl <= 128:       # the tail's grid-wide check-in needs every CTA resident
             tail = (self._grad_ptrs, self._inbox_ptrs, self.momentum, self.lr, self.mu, 1.0 / self.world, self.rank, self.world,
-                    self.ticket, None, self.wire_bf16)
+                    self.ticket, None, self.wire_bf16, self._sched)
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux, tail)
             return
@@ -302,7 +308,8 @@ class FusedTrainer:
                                 1, self.aux, None, self.grad_slots, self.factors, input_ready)
             # grads: re-zeroes the other-parity bucket, which a bucket step (fused tail, executor) may use next
             self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
-                              self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride)
+                              self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride,
+                              lr_schedule=self._sched)
             return
         if self.deterministic and B * cl <= self.sms:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
@@ -314,7 +321,7 @@ class FusedTrainer:
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux)
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
                              self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, self.grad_stride,
-                             self.done_counter, self.aux, self._inbox_ptrs, self.wire_bf16)
+                             self.done_counter, self.aux, self._inbox_ptrs, self.wire_bf16, lr_schedule=self._sched)
 
     def _warm(self):
         # forward-only launch: sets the kernel's dynamic-smem attribute outside of graph capture
@@ -433,7 +440,7 @@ class FusedTrainer:
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
                                       self.cluster, self.aux, self._inbox_ptrs, loss_hist,
                                       self.fused_tail and self.bsz * self.cluster <= 128, self.ticket, self.wire_bf16,
-                                      *self._native_slots()),
+                                      *self._native_slots(), lr_schedule=self._sched),
                   self.training)
             self._executors[id(loader)] = ex
         if new_epoch:
@@ -462,6 +469,39 @@ class FusedTrainer:
     def last_loss_cumulative(self) -> float:
         """Cumulative loss as of the most recently *retired* step (read from the pinned D2H copy)."""
         return self._last_loss_cum
+
+    # ------------------------------------------------------------------ learning rate
+    def _relaunch(self):
+        """Drop what baked the lr in: captured graphs and native executors are rebuilt on their next use."""
+        self.sync_lag(0)
+        self.stream.synchronize()
+        for s in list(self.slots) + list(self._ext_slots.values()):
+            s.graph = None
+        self._executors = {}
+
+    @property
+    def lr(self) -> float:
+        """Base learning rate.  Assigning it takes effect from the next step on every path (graphs are re-captured)."""
+        return self._lr
+
+    @lr.setter
+    def lr(self, value: float) -> None:
+        self._relaunch()
+        self._lr = float(value)
+
+    def set_lr_schedule(self, schedule: Optional[LRSchedule]) -> None:
+        """Replace the lr schedule (``None``: constant ``lr``) from the next step on."""
+        tup = schedule_tuple(schedule)
+        self._relaunch()
+        self._sched, self.lr_schedule = tup, schedule
+
+    def lr_at(self, step: Optional[int] = None) -> float:
+        """The lr the optimizer kernels apply when the step counter reads ``step`` (default: its current value)."""
+        if step is None:
+            self.sync_lag(0)
+            self.stream.synchronize()
+            step = int(self.step_counter.item())
+        return self._lr if self.lr_schedule is None else self.lr_schedule.lr_at(self._lr, step)
 
     # ------------------------------------------------------------------ nn.Module-like surface
     def train(self, mode: bool = True):
@@ -506,11 +546,13 @@ class FusedTrainer:
         p, m = unpack_params(self.params), unpack_params(self.momentum)
         return {"model": {k: v.detach().cpu().clone() for k, v in p.items()},
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
-                "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu}
+                "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
+                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict()}
 
     def load_state_dict(self, sd):
         """Accepts a trainer checkpoint or a plain ``Net`` state_dict.  Collective when ``steps`` is present (the bucket
-        parity and the exchange epochs derive from the step counter, see :meth:`_reset_exchange`)."""
+        parity and the exchange epochs derive from the step counter, see :meth:`_reset_exchange`).  The lr and the lr
+        schedule stay the constructor's: ``steps`` is where a schedule continues from."""
         self.sync_lag(0)
         model = sd.get("model", sd)
         views = unpack_params(self.params)

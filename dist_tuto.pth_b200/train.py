@@ -33,7 +33,7 @@ from . import comm
 from .data import default_eval_dataset, partition_dataset
 from .models.convnet import Net
 from .ops.convnet_eval import evaluate
-from .ops.optim import FlatSGD
+from .ops.optim import FlatSGD, LRSchedule
 from .utils import say
 from .utils.checkpoint import load_checkpoint, restore_optimizer, save_checkpoint
 from .utils.trace import NullTracer, Tracer
@@ -52,7 +52,7 @@ class TrainConfig:
                  max_steps: Optional[int] = None, dataset=None, log: Callable[..., None] = say,
                  p_drop: float = 0.5, checkpoint: Optional[str] = None, resume: Optional[str] = None,
                  checkpoint_every: Optional[int] = None, trace: Optional[str] = None, eval_dataset=None,
-                 eval_every: int = 1):
+                 eval_every: int = 1, lr_schedule: Optional[LRSchedule] = None):
         self.epochs, self.lr, self.momentum, self.seed = epochs, lr, momentum, seed
         self.global_batch, self.engine, self.device = global_batch, engine, device
         self.max_steps, self.dataset, self.log, self.p_drop = max_steps, dataset, log, p_drop
@@ -70,6 +70,11 @@ class TrainConfig:
         if int(eval_every) < 1:
             raise ValueError("TrainConfig.eval_every must be >= 1")
         self.eval_dataset, self.eval_every = eval_dataset, int(eval_every)
+        # lr_schedule: warmup / decay of `lr` (ops/optim.LRSchedule) in step or epoch units; train() resolves epochs with its
+        # number of batches per epoch and every engine applies it per update, counted from the run's first step
+        if lr_schedule is not None and not isinstance(lr_schedule, LRSchedule):
+            raise ValueError(f"TrainConfig.lr_schedule must be an LRSchedule or None, got {type(lr_schedule).__name__}")
+        self.lr_schedule = lr_schedule
 
 
 def _spans_machines() -> bool:
@@ -114,12 +119,13 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     train_set, bsz = partition_dataset(cfg.dataset, global_batch=cfg.global_batch, seed=cfg.seed,
                                        **({"raw_uint8": True} if fused_raw else {}))
     num_batches = ceil(len(train_set.dataset) / float(bsz))      # train_dist.py:112
+    schedule = cfg.lr_schedule.resolve(num_batches) if cfg.lr_schedule is not None else None
     start_steps, optimizer, resume_blob = 0, None, {}
     copies_in_flight = collections.deque()                       # torch engine on CUDA, see step_fn
     if engine == "fused":
         from .ops.convnet_fused import FusedTrainer
         trainer = FusedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
-                               p_drop=cfg.p_drop, raw_uint8=fused_raw)
+                               p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -127,7 +133,7 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     elif engine == "batched":
         from .ops.convnet_batched import BatchedTrainer
         trainer = BatchedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
-                                 p_drop=cfg.p_drop, raw_uint8=fused_raw)
+                                 p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -153,9 +159,10 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         broadcast_parameters(model)
         model._grad_bucket = GradBucket(list(model.parameters()))
         # optim.SGD(lr=0.01, momentum=0.5) of train_dist.py:110, over flat buffers: update + zero_grad in one pass
-        optimizer = FlatSGD(model, lr=cfg.lr, momentum=cfg.momentum)
+        optimizer = FlatSGD(model, lr=cfg.lr, momentum=cfg.momentum, lr_schedule=schedule)
         if cfg.resume:
             restore_optimizer(optimizer, model, resume_blob)         # momentum: FlatSGD layout or per-name (fused engine's)
+            optimizer.steps = start_steps                            # the schedule continues where the checkpoint stopped
         acc = torch.zeros((), device=device)
 
         # The native loader recycles its pinned staging buffers; the async H2D copies below must have left a buffer
@@ -195,7 +202,7 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     eval_set = None
     if cfg.eval_dataset is not None:
         eval_set = default_eval_dataset() if isinstance(cfg.eval_dataset, str) else cfg.eval_dataset
-    evals, eval_seconds = [], 0.0
+    evals, eval_seconds, epoch_lrs = [], 0.0, []
     history, steps, t0 = [], 0, time.perf_counter()
     start_epoch = 0
     if resume_blob.get("in_progress"):            # a periodic checkpoint of an unfinished run: do the REMAINING epochs
@@ -236,6 +243,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
                 loss_sum = epoch_loss_fn()
         mean_loss = loss_sum / denom
         history.append(mean_loss)
+        last = start_steps + steps - 1                             # step counter of the epoch's last update
+        epoch_lrs.append(cfg.lr if schedule is None else schedule.lr_at(cfg.lr, max(last, 0)))
         cfg.log("Rank ", comm.get_rank(), ", epoch ", epoch, ": ", mean_loss)
         if eval_set is not None and (done or (epoch + 1) % cfg.eval_every == 0 or epoch + 1 == cfg.epochs):
             te = time.perf_counter()
@@ -260,7 +269,7 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     trace_file = tracer.save(cfg.trace) if cfg.trace else None          # collective: rank 0 writes every rank's rows
     return {"loss": history, "steps": steps, "seconds": elapsed, "bsz": bsz,
             "samples_per_s": steps * bsz * size / max(elapsed, 1e-9), "model": model, "trace": trace_file,
-            "eval": evals, "eval_seconds": eval_seconds}
+            "eval": evals, "eval_seconds": eval_seconds, "lr": epoch_lrs}
 
 
 def run(rank: int, size: int):
