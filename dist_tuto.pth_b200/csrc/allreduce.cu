@@ -248,7 +248,9 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
 // receiver of a line agree on epoch and parity without any cross-block coordination.  Parity double-buffers the inbox: a
 // peer can write my parity-p region of block b again only two participations of block b later, which needs my lines of the
 // participation in between, which I store after I finished reading parity p (same argument as sgd_device.cuh, model-checked
-// in tests/test_protocol_models.py).  epoch 0 never occurs as a flag: counters are pre-incremented and the inbox starts zeroed.
+// in tests/test_protocol_models.py).  That needs the vector -> block map to be the same in every call on an inbox, so the
+// launcher sizes the LL grid by n_vec alone.  epoch 0 never occurs as a flag: counters are pre-incremented, the inbox starts
+// zeroed, and the one epoch in 2^32 that wraps to 0 uses flag 1 (epoch 1 has the other parity).
 template <bool BF16>
 __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   using W = Wire<BF16>;
@@ -320,10 +322,15 @@ __global__ void __launch_bounds__(32) barrier_kernel(SignalPads sig, int rank, i
 // ============================================================================================ launchers
 extern "C" {
 
-// variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  Returns cudaError_t as int.
+// variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  Returns cudaError_t as int; cudaErrorInvalidValue,
+// without a launch, for an unknown variant, a world outside 1..8, a rank outside [0, world) or a two-shot / NVLS n_vec that
+// is not a multiple of world (the remainder would be left unreduced).
 int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
                         const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
                         int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream) {
+  if (variant < 0 || variant > 3 || world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world)
+    return (int)cudaErrorInvalidValue;
+  if ((variant == 1 || variant == 2) && n_vec % (size_t)world != 0) return (int)cudaErrorInvalidValue;  // slice = n_vec / world
   b2::ARArgs a;
   memset(&a.inbox, 0, sizeof(a.inbox));
   a.ll_cap = 0;
@@ -339,7 +346,12 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::S
   size_t blocks = (work + b2::kThreads - 1) / b2::kThreads;
   if (variant == 1 || variant == 2) blocks = (blocks + 1) / 2;
   if (blocks < 1) blocks = 1;
-  if (blocks > (size_t)max_blocks) blocks = max_blocks;
+  // LL: the grid follows the message, never the per-call cap.  Vector v belongs to block (v / kThreads) % grid, whose own epoch
+  // word gives the line's flag and parity; if the cap could change the grid between two calls on one inbox, v could move to a
+  // block whose next flag equals the one its line already holds, and that stale line would be accepted.  n_vec <= ll_cap keeps
+  // the grid at ceil(4096 / 512) = 8 CTAs for the inbox parallel/symm.py allocates.
+  const size_t cap = variant == 3 ? (size_t)B2_MAX_BLOCKS : (size_t)max_blocks;
+  if (blocks > cap) blocks = cap;
   dim3 grid((unsigned)blocks), block(b2::kThreads);
   if (variant == 0) {
     if (bf16) b2::allreduce_oneshot_kernel<true><<<grid, block, 0, stream>>>(a);

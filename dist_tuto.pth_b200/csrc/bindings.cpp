@@ -134,6 +134,12 @@ SignalPadsH to_sig(const std::vector<unsigned long long>& v) {
   return s;
 }
 
+// The comm kernels index their per-rank pointer lists by rank: a missing entry would be a null device pointer.
+void check_world(int rank, int world, const char* what) {
+  TORCH_CHECK(world >= 1 && world <= B2_MAX_RANKS, what, ": world must be in 1..8, got ", world);
+  TORCH_CHECK(rank >= 0 && rank < world, what, ": rank ", rank, " is outside [0, ", world, ")");
+}
+
 void check_cuda_contig(const torch::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.is_contiguous(), name, " must be a contiguous CUDA tensor");
 }
@@ -314,6 +320,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                         unsigned long long mc, c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst,
                         size_t n_vec, double scale, int rank, int world, int max_blocks, std::vector<unsigned long long> inbox,
                         size_t ll_cap) {
+    check_world(rank, world, "allreduce");
+    TORCH_CHECK(variant >= 0 && variant <= 3, "allreduce: variant must be 0 (one-shot), 1 (two-shot), 2 (NVLS) or 3 (LL), got ",
+                variant);
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, "allreduce: one buffer and one signal pad per rank, got ",
+                bufs.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK(variant == 3 ? (int)inbox.size() == world : inbox.empty() || (int)inbox.size() == world,
+                "allreduce: one LL inbox per rank, got ", inbox.size(), " for world ", world);
+    TORCH_CHECK((variant != 1 && variant != 2) || n_vec % (size_t)world == 0,
+                "allreduce: two-shot and NVLS reduce n_vec / world vectors per rank, so n_vec must be a multiple of world "
+                "(pad the buffer), got n_vec ", n_vec, " for world ", world);
     PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
     PeerPtrs ib = to_ptrs(inbox);
     const void* sp = nullptr; void* dp = nullptr; int sf = 0, df = 0;
@@ -325,6 +341,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("n_vec"), py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0,
      py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
   m.def("barrier", [](std::vector<unsigned long long> sigs, int rank, int world) {
+    check_world(rank, world, "barrier");
+    TORCH_CHECK((int)sigs.size() == world, "barrier: one signal pad per rank, got ", sigs.size(), " for world ", world);
     SignalPadsH s = to_sig(sigs);
     ck_cuda(b2_barrier_launch(&s, rank, world, cur_stream()), "barrier launch");
   });
@@ -333,6 +351,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,
                             c10::optional<torch::Tensor> aux, std::vector<unsigned long long> inbox, bool wire_bf16,
                             py::object lr_schedule) {
+    check_world(rank, world, "allreduce_sgd");
+    TORCH_CHECK((int)grads.size() == world && (int)sigs.size() == world, "allreduce_sgd: one gradient bucket and one signal pad "
+                "per rank, got ", grads.size(), " and ", sigs.size(), " for world ", world);
     check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
     const b2::LrSchedule sched = to_sched(lr_schedule);
     TORCH_CHECK(inbox.empty() || (int)inbox.size() == world, "inbox: one pointer per rank (or none)");

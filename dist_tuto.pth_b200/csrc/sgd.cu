@@ -167,9 +167,9 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
 // each element out of its OWN memory, polling until both flags of a line carry this step's epoch.  Compared with
 // barrier + peer loads (flag crossing, then a load round trip) the critical path is ONE one-way crossing.  The sum
 // runs in fixed rank order with the own contribution taken from registers at position `rank`, so replicas stay
-// bit-identical and equal to the barrier variant.  epoch = step + 1 (never 0 = freshly zeroed inbox); lines are
-// double-buffered by step parity: a peer can only write parity p again two steps later, which needs my push of the
-// step in between, which I issue after I finished reading parity p.
+// bit-identical and equal to the barrier variant.  epoch = step + 1 (its wrap to 0, the value of a freshly zeroed line,
+// is sent as 1: epoch 1 has the other parity); lines are double-buffered by step parity: a peer can only write parity p
+// again two steps later, which needs my push of the step in between, which I issue after I finished reading parity p.
 __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_push_kernel(SgdArgs a) {
   __shared__ unsigned long long s_step;
   __shared__ float s_lr;
@@ -265,6 +265,7 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
                             const b2::LrSchedule* sched, cudaStream_t stream) {
+  if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return (int)cudaErrorInvalidValue;
   b2::SgdArgs a;
   a.phase_ts = g_phase_ts;
   memset(&a.sched, 0, sizeof(a.sched));

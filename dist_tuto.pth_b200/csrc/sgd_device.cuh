@@ -90,10 +90,12 @@ __device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g, 
 // One float4 vector `v` of the flat bucket through the push ("LL") exchange and the optimizer:
 //   store my value, flag-in-data, into every peer's inbox (16-byte lines {v0, epoch, v1, epoch}); sum the world lines of this
 //   vector out of MY inbox in fixed rank order (own contribution from registers) => bit-identical replicas; SGD; re-zero the
-//   other-parity bucket.  world == 1: no exchange.  `st` = step index (epoch = st + 1, parity = st & 1), `lr` = step_lr(a, st).
+//   other-parity bucket.  world == 1: no exchange.  `st` = step index (flag = (uint32)(st + 1), or 1 where that wraps to 0;
+//   parity = st & 1), `lr` = step_lr(a, st).
 __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, unsigned long long st, float lr) {
   const int rank = a.rank, world = a.world;
   const uint32_t epoch = (uint32_t)(st + 1ull);
+  const uint32_t flag = epoch == 0u ? 1u : epoch;                       // 0 is "never written"; epoch 1 has the other parity
   const size_t ipar = (size_t)(st & 1ull);                              // inbox lines are double-buffered by step parity
   const size_t par = a.grad_stride > 0 ? ipar : 0;                       // ... and so are the gradient buckets when there are two
   const size_t cur_off = par * (size_t)a.grad_stride * sizeof(float);
@@ -103,7 +105,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
     // one line per vector: {bf16(x),bf16(y) | flag | bf16(z),bf16(w) | flag}
     const uint32_t lo = pack_bf16x2(__uint_as_float(mine.x), __uint_as_float(mine.y));
     const uint32_t hi = pack_bf16x2(__uint_as_float(mine.z), __uint_as_float(mine.w));
-    const uint4 l0 = make_uint4(lo, epoch, hi, epoch);
+    const uint4 l0 = make_uint4(lo, flag, hi, flag);
     const size_t dst_line = (ipar * (size_t)world + (size_t)rank) * a.n_vec + v;
 #pragma unroll
     for (int i = 1; i < B2_MAX_RANKS; ++i) {
@@ -125,7 +127,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
           unsigned long long spins = 0;
           for (;;) {
             q0 = ld_volatile_v4(src);
-            if (q0.y == epoch && q0.w == epoch) break;
+            if (q0.y == flag && q0.w == flag) break;
             if (++spins > B2_SPIN_LIMIT) {
               printf("[b200dist] push all-reduce (bf16 wire): rank %d timed out waiting for rank %d (step %llu, vector %llu)\n", rank, r,
                      st, (unsigned long long)v);
@@ -138,7 +140,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
     }
   } else if (world > 1) {
     const size_t dst_line = ((ipar * (size_t)world + (size_t)rank) * a.n_vec + v) * 2;   // ((parity * world + source) * n_vec + v) * 2
-    const uint4 l0 = make_uint4(mine.x, epoch, mine.y, epoch), l1 = make_uint4(mine.z, epoch, mine.w, epoch);
+    const uint4 l0 = make_uint4(mine.x, flag, mine.y, flag), l1 = make_uint4(mine.z, flag, mine.w, flag);
 #pragma unroll
     for (int i = 1; i < B2_MAX_RANKS; ++i) {          // start with the next rank so the ranks do not all hit one peer first
       if (i < world) {
@@ -162,7 +164,7 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
           for (;;) {
             q0 = ld_volatile_v4(src);
             q1 = ld_volatile_v4(src + 1);
-            if (q0.y == epoch && q0.w == epoch && q1.y == epoch && q1.w == epoch) break;
+            if (q0.y == flag && q0.w == flag && q1.y == flag && q1.w == flag) break;
             if (++spins > B2_SPIN_LIMIT) {
               printf("[b200dist] push all-reduce: rank %d timed out waiting for rank %d (step %llu, vector %llu)\n", rank, r, st,
                      (unsigned long long)v);

@@ -392,44 +392,6 @@ def test_fused_trainer_uses_clusters_for_small_batches(dev):
     assert torch.allclose(res[0][1], res[1][1], atol=1e-5, rtol=1e-4)
 
 
-def test_push_allreduce_sgd_two_ranks_emulated_on_one_gpu(dev):
-    """Protocol check of allreduce_sgd_push_kernel without a second GPU: two 'ranks' = two concurrent launches on two
-    streams, each with its own params/momentum/buckets/inbox.  4 steps: both parities, epochs 1..4."""
-    from dist_tuto.pth_b200.ops import _ext
-    from dist_tuto.pth_b200.ops.convnet_fused import NPAR_ALLOC
-    C = _ext.C()
-    n, world, lr, mu = NPAR_ALLOC, 2, 0.1, 0.5
-    torch.manual_seed(0)
-    p0 = torch.randn(n, device=dev)
-    params = [p0.clone(), p0.clone()]
-    mom = [torch.zeros(n, device=dev) for _ in range(world)]
-    grads = [torch.zeros(2 * n, device=dev) for _ in range(world)]
-    step = [torch.zeros(1, dtype=torch.int64, device=dev) for _ in range(world)]
-    done = [torch.zeros(1, dtype=torch.int32, device=dev) for _ in range(world)]
-    inbox = [torch.zeros(2 * world * (n // 4) * 8, dtype=torch.int32, device=dev) for _ in range(world)]
-    streams = [torch.cuda.Stream(dev) for _ in range(world)]
-    ref_p, ref_m = p0.double().clone(), torch.zeros(n, dtype=torch.float64, device=dev)
-    for it in range(4):
-        gs = [torch.randn(n, device=dev) for _ in range(world)]
-        for r in range(world):
-            grads[r][(it & 1) * n:(it & 1) * n + n].copy_(gs[r])
-            grads[r][((it + 1) & 1) * n:((it + 1) & 1) * n + n].fill_(7.0)      # must come back zeroed
-        torch.cuda.synchronize()
-        for r in range(world):
-            with torch.cuda.stream(streams[r]):
-                C.allreduce_sgd([g.data_ptr() for g in grads], [0, 0], params[r], mom[r], step[r], lr, mu, 1.0 / world, r, world,
-                                True, n, done[r], None, [b.data_ptr() for b in inbox])
-        torch.cuda.synchronize()
-        g = (gs[0] + gs[1]) * (1.0 / world)                   # fp32, rank order: what the kernel computes
-        ref_m = mu * ref_m + g.double()
-        ref_p = ref_p - lr * ref_m
-        assert torch.equal(params[0], params[1]) and torch.equal(mom[0], mom[1])
-        assert torch.allclose(params[0].double(), ref_p, atol=1e-5), it
-        for r in range(world):
-            assert int(step[r].item()) == it + 1 and int(done[r].item()) == 0
-            assert float(grads[r][((it + 1) & 1) * n:((it + 1) & 1) * n + n].abs().max()) == 0.0
-
-
 def test_load_state_dict_rewinds_step_parity_and_buckets(dev):
     """load_state_dict() may move the step counter to the other parity: the double-buffered gradient buckets must both be
     clean afterwards (the kernels only re-zero the bucket of the previous parity)."""

@@ -196,20 +196,31 @@ def test_flag_barrier_needs_the_monotonic_compare():
 
 # ---------------------------------------------------------------------------------------------------------------------
 # The generic LL all-reduce of csrc/allreduce.cu (`allreduce_ll_kernel`) shares its per-block call counter (the signal pad's
-# epoch word) with the barrier-based variants, and consecutive calls may have different sizes: a call only advances the
-# epochs of the blocks it launches, and only exchanges the vectors below its n_vec.  Claim (kernel comment): sender and
+# epoch word) with the barrier-based variants, and consecutive calls may have different sizes and caps: a call only advances
+# the epochs of the blocks it launches, and only exchanges the vectors below its n_vec.  Claim (kernel comment): sender and
 # receiver of a line always agree on epoch and parity, and a line is never overwritten before its reader consumed it --
-# for ANY call sequence mixing LL calls of different sizes with barrier-type calls (one-shot / two-shot / NVLS / barrier
-# kernel advance a block's epoch by 1..3 and are full cross-rank barriers for that block).
+# for ANY call sequence mixing LL calls of different sizes and per-call caps (max_blocks) with barrier-type calls (one-shot /
+# two-shot / NVLS / barrier kernel advance a block's epoch by 1..3 and are full cross-rank barriers for that block).
+def launcher_ll_grid(n_vec, cap, vpb):
+    """Grid of an LL call as b2_allreduce_launch sizes it: by the message alone, whatever the per-call cap."""
+    return (n_vec + vpb - 1) // vpb
+
+
+def capped_ll_grid(n_vec, cap, vpb):
+    """A grid that follows the per-call cap (the launcher before it ignored the cap for LL): the negative control."""
+    return min((n_vec + vpb - 1) // vpb, cap)
+
+
 class LLRank:
     """One rank executing a fixed call list in stream order: call k+1 starts after every thread of call k finished.  Inside a
     call every vector (LL) / every block (barrier-type call) is its own thread of control: the GPU runs them concurrently,
     so the scheduler may interleave them freely."""
 
-    def __init__(self, r, world, calls, nblocks, vec_per_block):
+    def __init__(self, r, world, calls, nblocks, vec_per_block, ll_grid=launcher_ll_grid):
         self.r, self.world, self.calls = r, world, calls
         self.epoch = [0] * nblocks                      # per-block epoch word in this rank's signal pad
         self.vpb = vec_per_block
+        self.ll_grid = ll_grid
         self.k = -1
         self.threads = {}                               # thread id -> pending atomic actions
         self.bumps = []
@@ -223,9 +234,10 @@ class LLRank:
         if self.k >= len(self.calls):
             return
         kind, blocks, arg = self.calls[self.k]
-        if kind == "ll":                                # arg = n_vec: vectors v < n_vec, vector v lives in block v // vpb
-            for b in range(blocks):
-                vs = [v for v in range(b * self.vpb, (b + 1) * self.vpb) if v < arg]
+        if kind == "ll":                                # blocks = the call's cap, arg = n_vec: vectors v < n_vec, grid-stride,
+            grid = self.ll_grid(arg, blocks, self.vpb)  # so vector v lives in block (v // vpb) % grid
+            for b in range(grid):
+                vs = [v for v in range(arg) if (v // self.vpb) % grid == b]
                 if not vs:
                     continue
                 ep = self.epoch[b] + 1
@@ -246,13 +258,13 @@ class LLRank:
         return self.k >= len(self.calls)
 
 
-def run_ll(world, calls, nblocks, vpb, choose, max_ticks=400000, double_buffered=True):
+def run_ll(world, calls, nblocks, vpb, choose, max_ticks=400000, double_buffered=True, ll_grid=launcher_ll_grid):
     cap = nblocks * vpb
     par = (lambda ep: ep & 1) if double_buffered else (lambda ep: 0)
     # inbox[dst][parity][src][v][half] = (payload, flag); flags[dst][block][src] = barrier epochs
     inbox = [[[[[(None, 0), (None, 0)] for _ in range(cap)] for _ in range(world)] for _ in range(2)] for _ in range(world)]
     flags = [[[0] * world for _ in range(nblocks)] for _ in range(world)]
-    ranks = [LLRank(r, world, calls, nblocks, vpb) for r in range(world)]
+    ranks = [LLRank(r, world, calls, nblocks, vpb, ll_grid) for r in range(world)]
     for _ in range(max_ticks):
         for k in ranks:
             while not k.done() and not k.threads:       # call finished (or launched nothing): stream order -> next call
@@ -302,7 +314,7 @@ def _random_calls(rng, nblocks, vpb, n):
     for _ in range(n):
         if rng.random() < 0.65:
             n_vec = rng.randint(1, nblocks * vpb)
-            calls.append(("ll", (n_vec + vpb - 1) // vpb, n_vec))       # grid sized by the message, like b2_allreduce_launch
+            calls.append(("ll", rng.randint(1, nblocks), n_vec))        # per-call cap (max_blocks), n_vec
         else:
             calls.append(("bar", rng.randint(1, nblocks), rng.randint(1, 3)))
     return calls
@@ -331,3 +343,28 @@ def test_ll_model_catches_a_single_buffered_inbox():
         if found:
             break
     assert found is not None and ("consumed" in found or "deadlock" in found), found
+
+
+# The three calls of a cap that changes on one inbox (n_vec, cap), scaled to 2 vectors per block: the first gives blocks 0 and 1
+# epoch 1; if the second call's grid followed its cap of 1, block 0 would take vector 2 at epoch 2, parity 0; in the third,
+# block 1 would take vector 2 at ITS epoch 2, parity 0, and find the second call's line already carrying flag 2.
+MIXED_CAP_CALLS = [("ll", 2, 4), ("ll", 1, 3), ("ll", 2, 3)]
+
+
+def _first_runnable(rs):
+    return rs[0]                                        # rank 0 runs whenever it can: it reaches the third call first
+
+
+def test_ll_allreduce_with_a_cap_that_changes_between_calls_is_safe():
+    assert run_ll(2, MIXED_CAP_CALLS, 2, 2, _first_runnable) is None
+    for seed in range(200):
+        rng = random.Random(seed)
+        weights = [rng.choice([1, 5, 25]) for _ in range(3)]
+        bad = run_ll(3, MIXED_CAP_CALLS, 2, 2, lambda rs: rng.choices(rs, weights=[weights[k.r] for k, _ in rs])[0])
+        assert bad is None, (seed, bad)
+
+
+def test_ll_model_catches_a_grid_that_follows_the_cap():
+    """Negative control: with the grid capped per call, the third call accepts the second call's line for vector 2."""
+    bad = run_ll(2, MIXED_CAP_CALLS, 2, 2, _first_runnable, ll_grid=capped_ll_grid)
+    assert bad is not None and "call 2 consumed (1, 1, 2, 0)" in bad, bad
