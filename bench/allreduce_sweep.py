@@ -14,6 +14,10 @@ Bandwidth columns:
             NVLS  bytes * (1 + 1/N) ... see `link_bytes()` (formulas checked against the NVLink counters, bench/nvlink_bytes.py);
             reported as link_GBs = link_tx / t against 770 GB/s measured peer copy.
 ``--emit-table`` writes parallel/allreduce_table.json (per-world variant thresholds) from the measured winners.
+
+``--collective {reduce,broadcast,allgather}`` or ``--op {product,max,min}`` time that collective instead: every variant of
+ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the NCCL call on the same tensor, per size
+(for an all-gather, the size of one rank's input).  It compares GPUs, so it refuses to run on one.
 """
 import argparse
 import json
@@ -71,7 +75,62 @@ def time_op(fn, iters, dev, graph=False):
     return tmax(e0.elapsed_time(e1) / iters, dev)
 
 
+OPS = {"sum": dist.ReduceOp.SUM, "product": dist.ReduceOp.PRODUCT, "max": dist.ReduceOp.MAX, "min": dist.ReduceOp.MIN}
+
+
+def body_collective(rank, size):
+    """``--collective`` / ``--op``: ours per forced variant vs NCCL, per size, rows printed and written to ``--out``."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    w = symm.lookup_world(None)
+    op = OPS[ARGS.op]
+    coll = ARGS.collective
+    rows = []
+    s = 1024
+    while s <= ARGS.max_mb << 20:
+        n = s // 4
+        t = torch.ones(n, device=dev)
+        outs = [torch.empty_like(t) for _ in range(size)]
+        iters = 100 if s <= (1 << 20) else 20
+        row = {"bytes": s, "collective": coll, "op": ARGS.op}
+        arms = []
+        for name, v in (("ll", 3), ("oneshot", 0), ("twoshot", 1)):
+            if name == "ll" and s > symm.LL_CAP_VEC * 16:
+                continue
+            if coll == "allreduce":
+                arms.append((name, lambda v=v: w.all_reduce_(t, variant=v, op=op)))
+            elif coll == "reduce":
+                arms.append((name, lambda v=v: w.reduce_(t, 0, op, variant=v)))
+            elif coll == "broadcast":
+                arms.append((name, lambda v=v: w.broadcast_(t, 0, variant=v)))
+            else:
+                arms.append((name, lambda v=v: w.all_gather_(outs, t, variant=v)))
+        nccl = {"allreduce": lambda: dist.all_reduce(t, op=op), "reduce": lambda: dist.reduce(t, 0, op=op),
+                "broadcast": lambda: dist.broadcast(t, 0), "allgather": lambda: dist.all_gather(outs, t)}[coll]
+        arms.append(("nccl", nccl))
+        best = {}
+        for order in (arms, arms[::-1]):
+            for name, fn in order:
+                t.fill_(1.0)
+                best[name] = min(best.get(name, 1e30), time_op(fn, iters, dev, False))
+        for name, ms in best.items():
+            row[name + "_us"] = ms * 1e3
+        ours = min((row[k], k) for k in row if k.endswith("_us") and k != "nccl_us")
+        row["best"], row["speedup_vs_nccl"] = ours[1][:-3], row["nccl_us"] / ours[0]
+        rows.append(row)
+        if rank == 0:
+            print(json.dumps(row), flush=True)
+        s *= 4
+    if rank == 0:
+        os.makedirs(os.path.dirname(ARGS.out) or ".", exist_ok=True)
+        json.dump({"n_gpus": size, "symm": w.describe(), "rows": rows, "timing": "eager, CUDA events"}, open(ARGS.out, "w"),
+                  indent=1)
+        print("WROTE", ARGS.out, flush=True)
+    dist.barrier()
+
+
 def body(rank, size):
+    if ARGS.collective != "allreduce" or ARGS.op != "sum":
+        return body_collective(rank, size)
     dev = torch.device("cuda", torch.cuda.current_device())
     w = symm.lookup_world(None)
     max_bytes = ARGS.max_mb << 20
@@ -198,9 +257,18 @@ if __name__ == "__main__":
     ap.add_argument("--max-mb", type=int, default=1024)
     ap.add_argument("--out", default=None)
     ap.add_argument("--emit-table", action="store_true", help="write the measured variant thresholds of this world size")
+    ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather"], default="allreduce")
+    ap.add_argument("--op", choices=sorted(OPS), default="sum")
     ARGS = ap.parse_args()
+    if ARGS.gpus < 2:
+        ap.error("the sweep compares collectives across GPUs; it needs --gpus 2 or more")
+    if ARGS.emit_table and (ARGS.collective != "allreduce" or ARGS.op != "sum"):
+        ap.error("--emit-table measures the SUM all-reduce thresholds")
     if ARGS.out is None:
         ARGS.out = f"gpurun_out/sweep_{ARGS.gpus}.json"
+        if (ARGS.collective, ARGS.op) != ("allreduce", "sum"):    # one file per collective and op
+            stem, ext = os.path.splitext(ARGS.out)
+            ARGS.out = f"{stem}_{ARGS.collective}_{ARGS.op}{ext}"
     os.environ["B2_BENCH_ARGS"] = json.dumps(vars(ARGS))
     if "RANK" in os.environ:
         b2.init_from_env(body, backend="b200")

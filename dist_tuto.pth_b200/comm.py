@@ -12,9 +12,13 @@ Design (GPU-first, not a port):
   * plumbing (rendezvous, p2p, the non-hot collectives) rides on
     ``torch.distributed`` -- NCCL for CUDA tensors (NVLink 5 / NVSwitch),
     gloo for CPU tensors;
-  * the hot collective -- ``all_reduce(SUM)`` on CUDA floats -- is routed to
-    our own fused peer-memory kernels (``parallel.symm``) when a symmetric
-    world has been set up for the group; that path never calls NCCL.
+  * when a symmetric world has been set up for the group (``backend="b200"``),
+    blocking ``all_reduce`` and ``reduce`` (SUM, PRODUCT, MAX, MIN on CUDA
+    fp32 / bf16) and ``broadcast`` and ``all_gather`` (CUDA, any dtype, copied
+    bit for bit) run on our own fused peer-memory kernels (``parallel.symm``);
+    that path never calls NCCL.  ``async_op=True``, CPU tensors, other dtypes
+    and ops, ``scatter`` and ``gather`` go to NCCL / gloo, and so does every op
+    but SUM on a world that serves only the sum (no ``supports_op``).
   * ``group=0`` (the 2017 spelling of "world", train_dist.py:99, ptp.py:26)
     is accepted and mapped to the default group (fixes defect D2).
 """
@@ -163,30 +167,53 @@ def _symm_world_for(tensor: torch.Tensor, group):
     return symm.lookup_world(_g(group))
 
 
+def _reduces(w, tensor: torch.Tensor, op) -> bool:
+    """Does world ``w`` run this reduction natively?  SUM on any world that takes the tensor; the other ops only on a
+    world that says it supports them (a hierarchical world reduces SUM only)."""
+    if w is None or not w.supports(tensor):
+        return False
+    if op == reduce_op.SUM:
+        return True
+    return hasattr(w, "supports_op") and w.supports_op(op)
+
+
 def all_reduce(tensor: torch.Tensor, op=reduce_op.SUM, group=None, async_op: bool = False):
     """In-place all-reduce; result on every rank (tuto.md:176-186,199).
 
-    CUDA float tensors with ``op=SUM`` go through the fused sm_90a peer-memory
-    kernels (one-shot / two-shot / NVLS picked by size) when a symmetric world
-    exists for the group; everything else goes to NCCL / gloo."""
+    CUDA fp32 / bf16 tensors go through the fused sm_90a peer-memory kernels
+    (variant picked by size) for SUM, PRODUCT, MAX and MIN when a symmetric
+    world exists for the group; everything else goes to NCCL / gloo."""
     _check(tensor)
-    if op == reduce_op.SUM and not async_op:
+    if not async_op:
         w = _symm_world_for(tensor, group)
-        if w is not None and w.supports(tensor):
-            w.all_reduce_(tensor, scale=1.0)
+        if _reduces(w, tensor, op):
+            if op == reduce_op.SUM:
+                w.all_reduce_(tensor, scale=1.0)
+            else:
+                w.all_reduce_(tensor, op=op)
             return None
     return dist.all_reduce(tensor, op=op, group=_g(group), async_op=async_op)
 
 
 def reduce(tensor: torch.Tensor, dst: int, op=reduce_op.SUM, group=None):
-    """Reduce to ``dst`` only (tuto.md:198)."""
+    """Reduce to ``dst`` only (tuto.md:198); ``dst`` is a global rank.  Other ranks' tensors are left as they were.
+    Routed like ``all_reduce``."""
     _check(tensor)
+    w = _symm_world_for(tensor, group)
+    if _reduces(w, tensor, op) and hasattr(w, "reduce_"):
+        w.reduce_(tensor, dst, op)
+        return None
     return dist.reduce(tensor, dst=dst, op=op, group=_g(group))
 
 
 def broadcast(tensor: torch.Tensor, src: int, group=None):
-    """Copy ``tensor`` from ``src`` to all ranks (tuto.md:197)."""
+    """Copy ``tensor`` from global rank ``src`` to all ranks (tuto.md:197).  On a symmetric world any CUDA dtype is
+    copied bit for bit by the peer-memory kernels."""
     _check(tensor)
+    w = _symm_world_for(tensor, group)
+    if w is not None and hasattr(w, "broadcast_") and w.supports_raw(tensor):
+        w.broadcast_(tensor, src)
+        return None
     return dist.broadcast(tensor, src=src, group=_g(group))
 
 
@@ -232,8 +259,15 @@ def gather_to_root(tensor: torch.Tensor, rank: int, tensor_list: Optional[List[t
 
 
 def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group=None):
-    """Every rank receives every rank's tensor (tuto.md:202)."""
+    """Every rank receives every rank's tensor (tuto.md:202).  On a symmetric world, CUDA tensors of any dtype are gathered
+    bit for bit by the peer-memory kernels."""
     _check(tensor)
+    w = _symm_world_for(tensor, group)
+    if w is not None and hasattr(w, "all_gather_") and w.supports_raw(tensor) and \
+            all(isinstance(t, torch.Tensor) and w.supports_raw(t) and t.dtype == tensor.dtype and t.numel() == tensor.numel()
+                for t in tensor_list) and len(tensor_list) == w.world:
+        w.all_gather_(tensor_list, tensor)
+        return None
     return dist.all_gather(tensor_list, tensor, group=_g(group))
 
 

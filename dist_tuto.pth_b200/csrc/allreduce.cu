@@ -16,11 +16,60 @@
 //
 // Work mapping invariant: element-vector j of a slice is always handled by the same (block, thread) on
 // every rank and in every phase, which is what makes the *per-block* cross-GPU barriers sufficient.
+//
+// The same three data movements serve six collectives, selected by the OP template parameter:
+//   SUM / PRODUCT / MAX / MIN : fp32 accumulator combined in rank order; `root` >= 0 makes it a reduce (only the root
+//                               stores its output; every rank still runs every barrier and every LL push)
+//   BCAST                     : raw 16-byte copies of the root's vectors (any dtype; never through the fp32 accumulator,
+//                               so -0, subnormals, NaN payloads and integers survive)
+//   GATHER                    : raw copies; rank r's input (n_vec / world vectors) lands at vector r * n_vec / world
+// Every rank of one call runs the same barrier sequence whatever the op and root, so calls of any kind may follow each
+// other on one buffer, signal pad and inbox.
 #include <cstdio>
 #include <cstring>
 #include "common.cuh"
 
 namespace b2 {
+
+enum : int { kSum = 0, kProd = 1, kMax = 2, kMin = 3, kBcast = 4, kGather = 5 };
+
+// The combine step of a reduction: identity, one fp32 combine, and the final scale (SUM only; the launcher refuses a
+// scale for the other ops, and skipping the multiply keeps their results bit-exact under --use_fast_math).
+template <int OP>
+struct Op;
+template <>
+struct Op<kSum> {
+  static constexpr float kIdentity = 0.f;
+  __device__ static __forceinline__ float combine(float a, float b) { return a + b; }
+  __device__ static __forceinline__ float fin(float a, float s) { return a * s; }
+};
+template <>
+struct Op<kProd> {
+  static constexpr float kIdentity = 1.f;
+  __device__ static __forceinline__ float combine(float a, float b) { return a * b; }
+  __device__ static __forceinline__ float fin(float a, float) { return a; }
+};
+// IEEE 754-2019 maximum / minimum: NaN if either term is NaN (max.NaN / min.NaN), and -0 < +0.
+template <>
+struct Op<kMax> {
+  static constexpr float kIdentity = -__builtin_huge_valf();
+  __device__ static __forceinline__ float combine(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+  }
+  __device__ static __forceinline__ float fin(float a, float) { return a; }
+};
+template <>
+struct Op<kMin> {
+  static constexpr float kIdentity = __builtin_huge_valf();
+  __device__ static __forceinline__ float combine(float a, float b) {
+    float r;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+  }
+  __device__ static __forceinline__ float fin(float a, float) { return a; }
+};
 
 template <bool BF16>
 struct Wire;  // one "vec" = 16 bytes on the wire
@@ -28,30 +77,40 @@ struct Wire;  // one "vec" = 16 bytes on the wire
 template <>
 struct Wire<false> {                      // fp32 wire: 4 elements per vec
   static constexpr int kElems = 4;
-  __device__ static __forceinline__ void zero(float* a) { a[0] = a[1] = a[2] = a[3] = 0.f; }
+  template <int OP>
+  __device__ static __forceinline__ void zero(float* a) { a[0] = a[1] = a[2] = a[3] = Op<OP>::kIdentity; }
+  template <int OP>
   __device__ static __forceinline__ void add(float* a, uint4 v) {
-    a[0] += __uint_as_float(v.x); a[1] += __uint_as_float(v.y);
-    a[2] += __uint_as_float(v.z); a[3] += __uint_as_float(v.w);
+    a[0] = Op<OP>::combine(a[0], __uint_as_float(v.x)); a[1] = Op<OP>::combine(a[1], __uint_as_float(v.y));
+    a[2] = Op<OP>::combine(a[2], __uint_as_float(v.z)); a[3] = Op<OP>::combine(a[3], __uint_as_float(v.w));
   }
+  template <int OP>
   __device__ static __forceinline__ uint4 pack(const float* a, float s) {
-    return make_uint4(__float_as_uint(a[0] * s), __float_as_uint(a[1] * s), __float_as_uint(a[2] * s),
-                      __float_as_uint(a[3] * s));
+    return make_uint4(__float_as_uint(Op<OP>::fin(a[0], s)), __float_as_uint(Op<OP>::fin(a[1], s)),
+                      __float_as_uint(Op<OP>::fin(a[2], s)), __float_as_uint(Op<OP>::fin(a[3], s)));
   }
 };
 template <>
 struct Wire<true> {                       // bf16 wire: 8 elements per vec, fp32 accumulation
   static constexpr int kElems = 8;
+  template <int OP>
   __device__ static __forceinline__ void zero(float* a) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) a[i] = 0.f;
+    for (int i = 0; i < 8; ++i) a[i] = Op<OP>::kIdentity;
   }
+  template <int OP>
   __device__ static __forceinline__ void add(float* a, uint4 v) {
-    a[0] += bf16lo(v.x); a[1] += bf16hi(v.x); a[2] += bf16lo(v.y); a[3] += bf16hi(v.y);
-    a[4] += bf16lo(v.z); a[5] += bf16hi(v.z); a[6] += bf16lo(v.w); a[7] += bf16hi(v.w);
+    const float t[8] = {bf16lo(v.x), bf16hi(v.x), bf16lo(v.y), bf16hi(v.y),
+                        bf16lo(v.z), bf16hi(v.z), bf16lo(v.w), bf16hi(v.w)};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a[i] = Op<OP>::combine(a[i], t[i]);
   }
+  template <int OP>
   __device__ static __forceinline__ uint4 pack(const float* a, float s) {
-    return make_uint4(pack_bf16x2(a[0] * s, a[1] * s), pack_bf16x2(a[2] * s, a[3] * s),
-                      pack_bf16x2(a[4] * s, a[5] * s), pack_bf16x2(a[6] * s, a[7] * s));
+    return make_uint4(pack_bf16x2(Op<OP>::fin(a[0], s), Op<OP>::fin(a[1], s)),
+                      pack_bf16x2(Op<OP>::fin(a[2], s), Op<OP>::fin(a[3], s)),
+                      pack_bf16x2(Op<OP>::fin(a[4], s), Op<OP>::fin(a[5], s)),
+                      pack_bf16x2(Op<OP>::fin(a[6], s), Op<OP>::fin(a[7], s)));
   }
 };
 
@@ -66,11 +125,11 @@ __device__ __forceinline__ uint4 load_local_as_wire(const void* base, size_t vec
                     pack_bf16x2(__uint_as_float(b.x), __uint_as_float(b.y)),
                     pack_bf16x2(__uint_as_float(b.z), __uint_as_float(b.w)));
 }
-template <bool BF16>
+template <bool BF16, int OP>
 __device__ __forceinline__ void store_acc_local(void* base, size_t vec, const float* acc, float s, bool local_f32) {
-  if (!BF16 || !local_f32) {
-    st_cg_v4(reinterpret_cast<uint4*>(base) + vec, Wire<BF16>::pack(acc, s));
-  } else {  // bf16 wire, fp32 local: keep the fp32 accumulator precision
+  if (!BF16 || !local_f32 || OP != kSum) {
+    st_cg_v4(reinterpret_cast<uint4*>(base) + vec, Wire<BF16>::template pack<OP>(acc, s));
+  } else {  // bf16 wire, fp32 local (SUM only): keep the fp32 accumulator precision
     st_cg_v4(reinterpret_cast<uint4*>(base) + 2 * vec,
              make_uint4(__float_as_uint(acc[0] * s), __float_as_uint(acc[1] * s), __float_as_uint(acc[2] * s),
                         __float_as_uint(acc[3] * s)));
@@ -97,61 +156,86 @@ struct ARArgs {
   PeerPtrs bufs;          // symmetric wire buffer of every rank
   SignalPads sig;         // signal pad of every rank (one pad per symmetric buffer)
   void* mc;               // multicast VA of the symmetric buffer (NVLS) or nullptr
-  const void* src;        // optional local source (copied/cast into bufs.p[rank] first)
+  const void* src;        // optional local source (copied/cast into bufs.p[rank] first; GATHER: into slice rank)
   void* dst;              // optional local destination (else result stays in bufs.p[rank])
-  size_t n_vec;           // 16-byte vectors on the wire (padded)
+  size_t n_vec;           // 16-byte vectors on the wire (padded); GATHER: of the output, world x the per-rank input
   float scale;
   int rank, world;
   int src_f32, dst_f32;   // local dtypes: 1 = fp32, 0 = wire dtype
   PeerPtrs inbox;         // LL variant: every rank's inbox [2 parities][world sources][ll_cap vectors][2 lines of 16 B]
   size_t ll_cap;          // vectors per (parity, source) region of the inbox
+  int root;               // reductions: -1 = every rank stores the result, else only this rank; BCAST: the source rank
 };
 
 constexpr int kThreads = 512;
 constexpr int kUnroll = 2;        // peer-load variants: 2 x world 16-byte loads in flight per thread
 constexpr int kUnrollNvls = 4;    // NVLS: one multimem.ld_reduce per vector
 
+// Does this rank store its output?  Only a reduce (ROOT: a reduction with root >= 0) suppresses stores, never barriers.
+// ROOT is a template parameter so that the all-reduce instances carry no root test at all.
+template <bool ROOT>
+__device__ __forceinline__ bool stores_output(const ARArgs& a) {
+  return !ROOT || a.root == a.rank;
+}
+
 // ------------------------------------------------------------------------------------------ one-shot
-template <bool BF16>
+// Reductions read vector v of every rank; BCAST reads it from the root only; GATHER reads it from its owner v / seg.
+template <bool BF16, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
   using W = Wire<BF16>;
+  constexpr bool kRaw = OP >= kBcast;
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
   const size_t stride = (size_t)gridDim.x * kThreads;
   const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  if (a.src != nullptr) {
-    for (size_t v = first; v < a.n_vec; v += stride)
-      st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[rank]) + v, load_local_as_wire<BF16>(a.src, v, a.src_f32));
+  const size_t seg = a.n_vec / world;                   // GATHER: vectors per rank
+  if (a.src != nullptr && (OP != kBcast || rank == a.root)) {
+    uint4* stage = reinterpret_cast<uint4*>(a.bufs.p[rank]) + (OP == kGather ? (size_t)rank * seg : 0);
+    for (size_t v = first; v < (OP == kGather ? seg : a.n_vec); v += stride)
+      st_cg_v4(stage + v, load_local_as_wire<BF16>(a.src, v, a.src_f32));
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's data is in place
   const bool inplace = (a.dst == nullptr);
   void* out = inplace ? a.bufs.p[rank] : a.dst;
   const bool out_f32 = inplace ? false : (a.dst_f32 != 0);
+  const bool store = stores_output<ROOT>(a);
   // block-uniform trip count (the in-place variant has a barrier inside the loop); identical on every rank
   for (size_t base0 = (size_t)blockIdx.x * kThreads; base0 < a.n_vec; base0 += stride * kUnroll) {
     const size_t base = base0 + threadIdx.x;
     float acc[kUnroll][W::kElems];
     uint4 raw[kUnroll][B2_MAX_RANKS];
+    if constexpr (kRaw) {
 #pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const size_t v = base + (size_t)u * stride;
+      for (int u = 0; u < kUnroll; ++u) {
+        const size_t v = base + (size_t)u * stride;
+        const int from = OP == kBcast ? a.root : (int)(v / seg);
+        if (v < a.n_vec) raw[u][0] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[from]) + v);
+      }
+    } else {
 #pragma unroll
-      for (int r = 0; r < B2_MAX_RANKS; ++r)
-        if (r < world && v < a.n_vec) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[r]) + v);
-    }
+      for (int u = 0; u < kUnroll; ++u) {
+        const size_t v = base + (size_t)u * stride;
 #pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      W::zero(acc[u]);
-      const size_t v = base + (size_t)u * stride;
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world && v < a.n_vec) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[r]) + v);
+      }
 #pragma unroll
-      for (int r = 0; r < B2_MAX_RANKS; ++r)
-        if (r < world && v < a.n_vec) W::add(acc[u], raw[u][r]);
+      for (int u = 0; u < kUnroll; ++u) {
+        W::template zero<OP>(acc[u]);
+        const size_t v = base + (size_t)u * stride;
+#pragma unroll
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world && v < a.n_vec) W::template add<OP>(acc[u], raw[u][r]);
+      }
     }
     if (inplace) block_barrier_all_ranks(a.sig, rank, world, ++epoch);   // all peers finished reading this pass
 #pragma unroll
     for (int u = 0; u < kUnroll; ++u) {
       const size_t v = base + (size_t)u * stride;
-      if (v < a.n_vec) store_acc_local<BF16>(out, v, acc[u], a.scale, out_f32);
+      if (v < a.n_vec && store) {
+        if constexpr (kRaw) st_cg_v4(reinterpret_cast<uint4*>(out) + v, raw[u][0]);
+        else store_acc_local<BF16, OP>(out, v, acc[u], a.scale, out_f32);
+      }
     }
   }
   if (!inplace) block_barrier_all_ranks(a.sig, rank, world, ++epoch);    // staging may be overwritten now
@@ -159,27 +243,32 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------ two-shot / NVLS
-// Slice s = vectors [s*slice, (s+1)*slice) is reduced by rank s and pushed to every rank.
-template <bool BF16, bool NVLS>
+// Slice s = vectors [s*slice, (s+1)*slice) is reduced by rank s and pushed to every rank (a reduce pushes it to the root
+// only).  BCAST: rank s loads slice s from the root and pushes it; GATHER: rank s pushes its own input, staged at slice s.
+template <bool BF16, bool NVLS, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
   using W = Wire<BF16>;
+  constexpr bool kRaw = OP >= kBcast;
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
   const size_t slice = a.n_vec / world;                 // host pads n_vec to a multiple of world
   const size_t stride = (size_t)gridDim.x * kThreads;
   const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  if (a.src != nullptr) {
-    for (int s = 0; s < world; ++s)
+  if (a.src != nullptr && (OP != kBcast || rank == a.root)) {
+    for (int s = 0; s < world; ++s) {
+      if (OP == kGather && s != rank) continue;
       for (size_t j = first; j < slice; j += stride) {
         const size_t v = (size_t)s * slice + j;
-        st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[rank]) + v, load_local_as_wire<BF16>(a.src, v, a.src_f32));
+        st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[rank]) + v,
+                 load_local_as_wire<BF16>(a.src, OP == kGather ? j : v, a.src_f32));
       }
+    }
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);
   const size_t off = (size_t)rank * slice;
   constexpr int U = NVLS ? kUnrollNvls : kUnroll;
   for (size_t base = first; base < slice; base += stride * U) {
-    if (NVLS) {
+    if constexpr (NVLS) {
       uint4 red[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -199,9 +288,9 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
         const size_t j = base + (size_t)u * stride;
         if (j < slice) {
           float acc[W::kElems];
-          W::zero(acc);
-          W::add(acc, red[u]);
-          multimem_st_v4(reinterpret_cast<uint4*>(a.mc) + off + j, W::pack(acc, a.scale));
+          W::template zero<OP>(acc);
+          W::template add<OP>(acc, red[u]);
+          multimem_st_v4(reinterpret_cast<uint4*>(a.mc) + off + j, W::template pack<OP>(acc, a.scale));
         }
       }
     } else {
@@ -209,29 +298,38 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const size_t j = base + (size_t)u * stride;
+        if constexpr (kRaw) {
+          if (j < slice) raw[u][0] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[OP == kBcast ? a.root : rank]) + off + j);
+        } else {
 #pragma unroll
-        for (int r = 0; r < B2_MAX_RANKS; ++r)
-          if (r < world && j < slice) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[r]) + off + j);
+          for (int r = 0; r < B2_MAX_RANKS; ++r)
+            if (r < world && j < slice) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[r]) + off + j);
+        }
       }
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const size_t j = base + (size_t)u * stride;
         if (j < slice) {
-          float acc[W::kElems];
-          W::zero(acc);
+          uint4 o;
+          if constexpr (kRaw) {
+            o = raw[u][0];
+          } else {
+            float acc[W::kElems];
+            W::template zero<OP>(acc);
+#pragma unroll
+            for (int r = 0; r < B2_MAX_RANKS; ++r)
+              if (r < world) W::template add<OP>(acc, raw[u][r]);
+            o = W::template pack<OP>(acc, a.scale);
+          }
 #pragma unroll
           for (int r = 0; r < B2_MAX_RANKS; ++r)
-            if (r < world) W::add(acc, raw[u][r]);
-          const uint4 o = W::pack(acc, a.scale);
-#pragma unroll
-          for (int r = 0; r < B2_MAX_RANKS; ++r)
-            if (r < world) st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[r]) + off + j, o);
+            if (r < world && (!ROOT || r == a.root)) st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[r]) + off + j, o);
         }
       }
     }
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every slice has landed everywhere
-  if (a.dst != nullptr) {
+  if (a.dst != nullptr && stores_output<ROOT>(a)) {
     for (int s = 0; s < world; ++s)
       for (size_t j = first; j < slice; j += stride) {
         const size_t v = (size_t)s * slice + j;
@@ -249,9 +347,11 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
 // peer can write my parity-p region of block b again only two participations of block b later, which needs my lines of the
 // participation in between, which I store after I finished reading parity p (same argument as sgd_device.cuh, model-checked
 // in tests/test_protocol_models.py).  That needs the vector -> block map to be the same in every call on an inbox, so the
-// launcher sizes the LL grid by n_vec alone.  epoch 0 never occurs as a flag: counters are pre-incremented, the inbox starts
-// zeroed, and the one epoch in 2^32 that wraps to 0 uses flag 1 (epoch 1 has the other parity).
-template <bool BF16>
+// launcher sizes the LL grid by the pushed vectors alone.  epoch 0 never occurs as a flag: counters are pre-incremented, the
+// inbox starts zeroed, and the one epoch in 2^32 that wraps to 0 uses flag 1 (epoch 1 has the other parity).
+// Every op pushes and waits for the same lines: BCAST keeps the root's line (the others are the acknowledgements the parity
+// argument needs), GATHER stores source r's line at vector r * n_vec / world instead of combining it.
+template <bool BF16, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   using W = Wire<BF16>;
   const int rank = a.rank, world = a.world;
@@ -259,11 +359,14 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   const uint32_t flag = epoch == 0u ? 1u : epoch;                     // 0 is "never written"
   const size_t par = (size_t)(epoch & 1u);
   const size_t stride = (size_t)gridDim.x * kThreads;
-  const void* in_local = a.src != nullptr ? a.src : a.bufs.p[rank];
+  const size_t n_push = OP == kGather ? a.n_vec / world : a.n_vec;    // vectors each rank pushes
+  const void* in_local = a.src != nullptr ? a.src
+                                          : reinterpret_cast<const uint4*>(a.bufs.p[rank]) + (OP == kGather ? rank * n_push : 0);
   const bool in_f32 = a.src != nullptr && a.src_f32 != 0;
   void* out = a.dst != nullptr ? a.dst : a.bufs.p[rank];
   const bool out_f32 = a.dst != nullptr && a.dst_f32 != 0;
-  for (size_t v = (size_t)blockIdx.x * kThreads + threadIdx.x; v < a.n_vec; v += stride) {
+  const bool store = stores_output<ROOT>(a);
+  for (size_t v = (size_t)blockIdx.x * kThreads + threadIdx.x; v < n_push; v += stride) {
     const uint4 mine = load_local_as_wire<BF16>(in_local, v, in_f32);
     const uint4 l0 = make_uint4(mine.x, flag, mine.y, flag), l1 = make_uint4(mine.z, flag, mine.w, flag);
     const size_t line = ((par * (size_t)world + (size_t)rank) * a.ll_cap + v) * 2;
@@ -278,7 +381,8 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
       }
     }
     float acc[W::kElems];
-    W::zero(acc);
+    if constexpr (OP < kBcast) W::template zero<OP>(acc);
+    uint4 kept = mine;                                                // BCAST: the root's vector
     const uint4* in = reinterpret_cast<const uint4*>(a.inbox.p[rank]);
 #pragma unroll
     for (int r = 0; r < B2_MAX_RANKS; ++r) {
@@ -301,10 +405,15 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
           }
           w = make_uint4(q0.x, q0.z, q1.x, q1.z);
         }
-        W::add(acc, w);                                               // fixed rank order => bit-identical on every rank
+        if constexpr (OP == kGather) st_cg_v4(reinterpret_cast<uint4*>(out) + (size_t)r * n_push + v, w);
+        else if constexpr (OP == kBcast) kept = r == a.root ? w : kept;
+        else W::template add<OP>(acc, w);                             // fixed rank order => bit-identical on every rank
       }
     }
-    store_acc_local<BF16>(out, v, acc, a.scale, out_f32);
+    if constexpr (OP == kBcast) st_cg_v4(reinterpret_cast<uint4*>(out) + v, kept);
+    else if constexpr (OP != kGather) {
+      if (store) store_acc_local<BF16, OP>(out, v, acc, a.scale, out_f32);
+    }
   }
   __syncthreads();
   if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
@@ -319,53 +428,81 @@ __global__ void __launch_bounds__(32) barrier_kernel(SignalPads sig, int rank, i
 
 }  // namespace b2
 
+namespace b2 {
+
+template <bool BF16, int OP, bool ROOT>
+void launch_kernel(int variant, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+  if (variant == 0) allreduce_oneshot_kernel<BF16, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if (variant == 1) allreduce_twoshot_kernel<BF16, false, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if (variant == 3) allreduce_ll_kernel<BF16, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if constexpr (OP == kSum && !ROOT) allreduce_twoshot_kernel<BF16, true, kSum, false><<<grid, kThreads, 0, stream>>>(a);
+}
+
+template <int OP>
+void launch_op(int variant, int bf16, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+  if constexpr (OP < kBcast) {
+    if (a.root >= 0) return bf16 ? launch_kernel<true, OP, true>(variant, grid, a, stream)
+                                 : launch_kernel<false, OP, true>(variant, grid, a, stream);
+    if (bf16) return launch_kernel<true, OP, false>(variant, grid, a, stream);
+  }
+  launch_kernel<false, OP, false>(variant, grid, a, stream);
+}
+
+}  // namespace b2
+
 // ============================================================================================ launchers
 extern "C" {
 
-// variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  Returns cudaError_t as int; cudaErrorInvalidValue,
-// without a launch, for an unknown variant, a world outside 1..8, a rank outside [0, world) or a two-shot / NVLS n_vec that
-// is not a multiple of world (the remainder would be left unreduced).
+// variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN, 4 broadcast
+// from `root`, 5 all-gather; a reduction with root >= 0 is a reduce to that rank.  Returns cudaError_t as int;
+// cudaErrorInvalidValue, without a launch, for an unknown variant or op, a world outside 1..8, a rank outside [0, world), a
+// root outside [-1, world) (a broadcast needs one, an all-gather takes none), a scale other than 1, fp32 locals over a bf16
+// wire or NVLS for any op but SUM, a bf16 wire for the raw moves, a two-shot / NVLS / all-gather n_vec that is not a
+// multiple of world (the remainder would be left out) or an LL message larger than the inbox.
 int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
                         const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
-                        int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream) {
+                        int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root,
+                        cudaStream_t stream) {
   if (variant < 0 || variant > 3 || world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world)
     return (int)cudaErrorInvalidValue;
-  if ((variant == 1 || variant == 2) && n_vec % (size_t)world != 0) return (int)cudaErrorInvalidValue;  // slice = n_vec / world
+  if (op < b2::kSum || op > b2::kGather || root < -1 || root >= world) return (int)cudaErrorInvalidValue;
+  if (op == b2::kBcast ? root < 0 : (op == b2::kGather && root >= 0)) return (int)cudaErrorInvalidValue;
+  if (op != b2::kSum && (scale != 1.f || src_f32 || dst_f32)) return (int)cudaErrorInvalidValue;
+  if (variant == 2 && (op != b2::kSum || root >= 0)) return (int)cudaErrorInvalidValue;   // NVLS: the SUM all-reduce only
+  if (op >= b2::kBcast && bf16) return (int)cudaErrorInvalidValue;
+  if ((variant == 1 || variant == 2 || op == b2::kGather) && n_vec % (size_t)world != 0)
+    return (int)cudaErrorInvalidValue;                                     // slice = n_vec / world
+  const size_t n_push = op == b2::kGather ? n_vec / world : n_vec;        // LL: vectors each rank pushes
   b2::ARArgs a;
   memset(&a.inbox, 0, sizeof(a.inbox));
   a.ll_cap = 0;
   a.bufs = *bufs; a.sig = *sig; a.mc = mc; a.src = src; a.dst = dst; a.n_vec = n_vec; a.scale = scale;
-  a.rank = rank; a.world = world; a.src_f32 = src_f32; a.dst_f32 = dst_f32;
+  a.rank = rank; a.world = world; a.src_f32 = src_f32; a.dst_f32 = dst_f32; a.root = root;
   if (variant == 3) {
-    if (inbox == nullptr || ll_cap < n_vec) return (int)cudaErrorInvalidValue;
+    if (inbox == nullptr || ll_cap < n_push) return (int)cudaErrorInvalidValue;
     a.inbox = *inbox;
     a.ll_cap = ll_cap;
   }
+  if (variant == 2 && mc == nullptr) return (int)cudaErrorInvalidValue;
   if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
-  const size_t work = (variant == 0 || variant == 3) ? n_vec : n_vec / world;
+  const size_t work = variant == 0 ? n_vec : variant == 3 ? n_push : n_vec / world;
   size_t blocks = (work + b2::kThreads - 1) / b2::kThreads;
   if (variant == 1 || variant == 2) blocks = (blocks + 1) / 2;
   if (blocks < 1) blocks = 1;
   // LL: the grid follows the message, never the per-call cap.  Vector v belongs to block (v / kThreads) % grid, whose own epoch
   // word gives the line's flag and parity; if the cap could change the grid between two calls on one inbox, v could move to a
-  // block whose next flag equals the one its line already holds, and that stale line would be accepted.  n_vec <= ll_cap keeps
-  // the grid at ceil(4096 / 512) = 8 CTAs for the inbox parallel/symm.py allocates.
+  // block whose next flag equals the one its line already holds, and that stale line would be accepted.  n_push <= ll_cap keeps
+  // the grid at ceil(4096 / 512) = 8 CTAs for the inbox parallel/symm.py allocates, so v's block is v / kThreads in every op.
   const size_t cap = variant == 3 ? (size_t)B2_MAX_BLOCKS : (size_t)max_blocks;
   if (blocks > cap) blocks = cap;
-  dim3 grid((unsigned)blocks), block(b2::kThreads);
-  if (variant == 0) {
-    if (bf16) b2::allreduce_oneshot_kernel<true><<<grid, block, 0, stream>>>(a);
-    else b2::allreduce_oneshot_kernel<false><<<grid, block, 0, stream>>>(a);
-  } else if (variant == 1) {
-    if (bf16) b2::allreduce_twoshot_kernel<true, false><<<grid, block, 0, stream>>>(a);
-    else b2::allreduce_twoshot_kernel<false, false><<<grid, block, 0, stream>>>(a);
-  } else if (variant == 3) {
-    if (bf16) b2::allreduce_ll_kernel<true><<<grid, block, 0, stream>>>(a);
-    else b2::allreduce_ll_kernel<false><<<grid, block, 0, stream>>>(a);
-  } else {
-    if (mc == nullptr) return (int)cudaErrorInvalidValue;
-    if (bf16) b2::allreduce_twoshot_kernel<true, true><<<grid, block, 0, stream>>>(a);
-    else b2::allreduce_twoshot_kernel<false, true><<<grid, block, 0, stream>>>(a);
+  const dim3 grid((unsigned)blocks);
+  switch (op) {
+    case b2::kSum: b2::launch_op<b2::kSum>(variant, bf16, grid, a, stream); break;
+    case b2::kProd: b2::launch_op<b2::kProd>(variant, bf16, grid, a, stream); break;
+    case b2::kMax: b2::launch_op<b2::kMax>(variant, bf16, grid, a, stream); break;
+    case b2::kMin: b2::launch_op<b2::kMin>(variant, bf16, grid, a, stream); break;
+    case b2::kBcast: b2::launch_op<b2::kBcast>(variant, bf16, grid, a, stream); break;
+    default: b2::launch_op<b2::kGather>(variant, bf16, grid, a, stream); break;
   }
   return (int)cudaGetLastError();
 }

@@ -38,7 +38,7 @@ int b2_ipc_free(unsigned long long ptr);
 
 int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const SignalPadsH* sig, void* mc, const void* src,
                         int src_f32, void* dst, int dst_f32, size_t n_vec, float scale, int rank, int world,
-                        int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream);
+                        int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root, cudaStream_t stream);
 int b2_barrier_launch(const SignalPadsH* sig, int rank, int world, cudaStream_t stream);
 int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float* params, float* momentum,
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
@@ -316,30 +316,60 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("tensor_from_ptr", &tensor_from_ptr, "wrap device memory as a 1-D tensor (no ownership)");
 
   // ------------------------------------------------------------------ collectives
-  m.def("allreduce", [](int variant, bool bf16, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
-                        unsigned long long mc, c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst,
-                        size_t n_vec, double scale, int rank, int world, int max_blocks, std::vector<unsigned long long> inbox,
-                        size_t ll_cap) {
-    check_world(rank, world, "allreduce");
-    TORCH_CHECK(variant >= 0 && variant <= 3, "allreduce: variant must be 0 (one-shot), 1 (two-shot), 2 (NVLS) or 3 (LL), got ",
+  // op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN (reductions; root >= 0 stores on that rank only), 4 broadcast from root, 5 all-gather
+  // (n_vec counts the output, world x the per-rank input).  The raw moves take any dtype and copy bytes.
+  auto collective = [](const char* what, int op, int variant, bool bf16, const std::vector<unsigned long long>& bufs,
+                       const std::vector<unsigned long long>& sigs, unsigned long long mc, const c10::optional<torch::Tensor>& src,
+                       const c10::optional<torch::Tensor>& dst, size_t n_vec, double scale, int root, int rank, int world,
+                       int max_blocks, const std::vector<unsigned long long>& inbox, size_t ll_cap) {
+    check_world(rank, world, what);
+    TORCH_CHECK(variant >= 0 && variant <= 3, what, ": variant must be 0 (one-shot), 1 (two-shot), 2 (NVLS) or 3 (LL), got ",
                 variant);
-    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, "allreduce: one buffer and one signal pad per rank, got ",
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, what, ": one buffer and one signal pad per rank, got ",
                 bufs.size(), " and ", sigs.size(), " for world ", world);
     TORCH_CHECK(variant == 3 ? (int)inbox.size() == world : inbox.empty() || (int)inbox.size() == world,
-                "allreduce: one LL inbox per rank, got ", inbox.size(), " for world ", world);
-    TORCH_CHECK((variant != 1 && variant != 2) || n_vec % (size_t)world == 0,
-                "allreduce: two-shot and NVLS reduce n_vec / world vectors per rank, so n_vec must be a multiple of world "
+                what, ": one LL inbox per rank, got ", inbox.size(), " for world ", world);
+    TORCH_CHECK((variant != 1 && variant != 2 && op != 5) || n_vec % (size_t)world == 0,
+                what, ": two-shot, NVLS and all-gather split n_vec into world slices, so n_vec must be a multiple of world "
                 "(pad the buffer), got n_vec ", n_vec, " for world ", world);
+    TORCH_CHECK(root >= -1 && root < world, what, ": root must be -1 (every rank) or in [0, world), got ", root,
+                " for world ", world);
+    TORCH_CHECK(op == 0 || scale == 1.0, what, ": scale applies to SUM only, got ", scale, " for op ", op);
+    TORCH_CHECK(variant != 2 || (op == 0 && root < 0), what, ": NVLS runs the SUM all-reduce only");
+    TORCH_CHECK(variant != 3 || (op == 5 ? n_vec / world : n_vec) <= ll_cap, what, ": LL pushes ",
+                op == 5 ? n_vec / world : n_vec, " vectors per rank, more than the inbox holds (", ll_cap, ")");
     PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
     PeerPtrs ib = to_ptrs(inbox);
     const void* sp = nullptr; void* dp = nullptr; int sf = 0, df = 0;
     if (src.has_value()) { check_cuda_contig(*src, "src"); sp = src->data_ptr(); sf = src->scalar_type() == torch::kFloat32 && bf16; }
     if (dst.has_value()) { check_cuda_contig(*dst, "dst"); dp = dst->data_ptr(); df = dst->scalar_type() == torch::kFloat32 && bf16; }
+    TORCH_CHECK(op == 0 || (sf == 0 && df == 0), what, ": a bf16 wire for fp32 tensors is for SUM only");
     ck_cuda(b2_allreduce_launch(variant, bf16, &b, &s, (void*)(uintptr_t)mc, sp, sf, dp, df, n_vec, (float)scale, rank,
-                                world, max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, cur_stream()), "allreduce launch");
+                                world, max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, op, root, cur_stream()), what);
+  };
+  m.def("allreduce", [collective](int variant, bool bf16, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                                  unsigned long long mc, c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst,
+                                  size_t n_vec, double scale, int rank, int world, int max_blocks, std::vector<unsigned long long> inbox,
+                                  size_t ll_cap, int op, int root) {
+    TORCH_CHECK(op >= 0 && op <= 3, "allreduce: op must be 0 (SUM), 1 (PRODUCT), 2 (MAX) or 3 (MIN), got ", op);
+    collective("allreduce", op, variant, bf16, bufs, sigs, mc, src, dst, n_vec, scale, root, rank, world, max_blocks, inbox, ll_cap);
   }, py::arg("variant"), py::arg("bf16"), py::arg("bufs"), py::arg("sigs"), py::arg("mc"), py::arg("src"), py::arg("dst"),
      py::arg("n_vec"), py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0,
-     py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
+     py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0, py::arg("op") = 0, py::arg("root") = -1);
+  m.def("broadcast", [collective](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                                  c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int root,
+                                  int rank, int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {
+    TORCH_CHECK(root >= 0, "broadcast: root must be in [0, world), got ", root);
+    collective("broadcast", 4, variant, false, bufs, sigs, 0, src, dst, n_vec, 1.0, root, rank, world, max_blocks, inbox, ll_cap);
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("root"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(),
+     py::arg("ll_cap") = 0);
+  m.def("allgather", [collective](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                                  c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int rank,
+                                  int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {
+    collective("allgather", 5, variant, false, bufs, sigs, 0, src, dst, n_vec, 1.0, -1, rank, world, max_blocks, inbox, ll_cap);
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
   m.def("barrier", [](std::vector<unsigned long long> sigs, int rank, int world) {
     check_world(rank, world, "barrier");
     TORCH_CHECK((int)sigs.size() == world, "barrier: one signal pad per rank, got ", sigs.size(), " for world ", world);

@@ -17,6 +17,11 @@ A :class:`SymmHandle` is one symmetric allocation = [8 KiB signal pad | data].
 Each allocation owns its signal pad, so collectives on different buffers may be
 in flight on different streams at once.  All collectives must be issued in the
 same order on every rank of the world (as with any communicator).
+
+Collectives: ``all_reduce_`` and ``reduce_`` (SUM, PRODUCT, MAX, MIN on fp32 /
+bf16), ``broadcast_`` and ``all_gather_`` (raw bytes, any dtype).  Each call
+picks its kernel variant with :func:`plan_variant` and never synchronises the
+host.
 """
 from __future__ import annotations
 
@@ -32,7 +37,8 @@ import torch.distributed as dist
 
 from ..ops import _ext
 
-__all__ = ["SymmWorld", "SymmHandle", "init_world", "lookup_world", "destroy_all", "VARIANTS"]
+__all__ = ["SymmWorld", "SymmHandle", "init_world", "lookup_world", "destroy_all", "VARIANTS", "COLLECTIVES",
+           "op_code", "plan_variant"]
 
 PAD_BYTES = 8192                      # signal pad at the head of every allocation (B2_SIGNAL_WORDS*4 = 6016 B)
 VARIANTS = {"oneshot": 0, "twoshot": 1, "nvls": 2, "ll": 3}
@@ -50,6 +56,44 @@ def _load_table():
         return {}
 _WORLDS: Dict[object, "SymmWorld"] = {}
 _DTYPES = (torch.float32, torch.bfloat16)
+COLLECTIVES = ("allreduce", "reduce", "broadcast", "allgather")
+_OPS = {dist.ReduceOp.SUM: 0, dist.ReduceOp.PRODUCT: 1, dist.ReduceOp.MAX: 2, dist.ReduceOp.MIN: 3}
+
+
+def op_code(op) -> Optional[int]:
+    """The kernels' code of a reduction (0 SUM, 1 PRODUCT, 2 MAX, 3 MIN) for a ``torch.distributed.ReduceOp`` or one of
+    those codes; ``None`` for any other op (e.g. AVG, or a pre-multiplied sum)."""
+    if isinstance(op, int) and not isinstance(op, bool):
+        return op if 0 <= op <= 3 else None
+    try:
+        return _OPS.get(op)
+    except TypeError:                                      # an unhashable op object
+        return None
+
+
+def plan_variant(collective: str, op: int, nbytes: int, world: int, ll_max: int, oneshot_max: int, nvls_min: int,
+                 multicast: bool, forced: Optional[str] = None) -> int:
+    """Kernel variant (0 one-shot, 1 two-shot, 2 NVLS, 3 LL) of one collective from the measured thresholds.
+
+    ``nbytes`` is the message: the wire bytes of a reduction or broadcast, one rank's input for an all-gather.  An all-gather
+    uses LL while one rank's input is at most ``ll_max`` (which never exceeds the LL inbox), one-shot while its whole output
+    is at most ``oneshot_max``, two-shot above.  NVLS reduces in the switch and so serves only the SUM all-reduce; ``forced``
+    (``B200DIST_AR_VARIANT``) names a variant, and NVLS falls back to two-shot where it cannot run."""
+    if collective not in COLLECTIVES:
+        raise ValueError(f"unknown collective {collective!r}")
+    if world == 1:
+        return 0
+    nvls_ok = multicast and collective == "allreduce" and op == 0
+    if forced in VARIANTS:
+        v = VARIANTS[forced]
+        return v if (v != 2 or nvls_ok) else 1
+    if collective == "allgather":
+        return 3 if nbytes <= ll_max else 0 if world * nbytes <= oneshot_max else 1
+    if nbytes <= ll_max:
+        return 3
+    if nbytes <= oneshot_max:
+        return 0
+    return 2 if (nvls_ok and nbytes >= nvls_min) else 1
 
 
 def _env_int(name, default):
@@ -317,53 +361,85 @@ class SymmWorld:
 
     # ------------------------------------------------------------------ collectives
     def supports(self, t: torch.Tensor) -> bool:
-        """Can ``all_reduce_`` take this tensor (CUDA, this device, fp32/bf16, contiguous)?"""
+        """Can ``all_reduce_`` / ``reduce_`` take this tensor (CUDA, this device, fp32/bf16, contiguous)?"""
         return t.is_cuda and t.device == self.device and t.dtype in _DTYPES and t.is_contiguous()
 
     def pick_variant(self, wire_bytes: int) -> int:
         """Message size -> kernel (0 one-shot, 1 two-shot, 2 NVLS) from the measured thresholds; ``B200DIST_AR_VARIANT``
         forces one."""
-        if self.world == 1:
-            return 0
-        forced = os.environ.get("B200DIST_AR_VARIANT")
-        if forced in VARIANTS:
-            v = VARIANTS[forced]
-            return v if (v != 2 or self.multicast) else 1
-        if wire_bytes <= self.ll_max:
-            return 3
-        if wire_bytes <= self.oneshot_max:
-            return 0
-        return 2 if (self.multicast and wire_bytes >= self.nvls_min) else 1
+        return self.plan("allreduce", 0, wire_bytes)
+
+    def plan(self, collective: str, op: int, nbytes: int) -> int:
+        """:func:`plan_variant` with this world's thresholds and ``B200DIST_AR_VARIANT``."""
+        return plan_variant(collective, op, nbytes, self.world, self.ll_max, self.oneshot_max, self.nvls_min,
+                            self.multicast, os.environ.get("B200DIST_AR_VARIANT"))
 
     def _launch(self, hd: SymmHandle, bf16: bool, n_vec: int, scale: float, src, dst, variant: Optional[int],
-                max_blocks: Optional[int] = None):
-        wire_bytes = n_vec * 16
-        v = self.pick_variant(wire_bytes) if variant is None else variant
-        if v == 2 and not hd.mc_ptr:
+                max_blocks: Optional[int] = None, collective: str = "allreduce", op: int = 0, root: int = -1):
+        """One kernel call on ``hd``.  ``n_vec``: 16-byte vectors of the message (of the output for an all-gather, a multiple
+        of world there); ``root``: local rank (-1 for the all-to-all collectives)."""
+        n_push = n_vec // self.world if collective == "allgather" else n_vec
+        v = self.plan(collective, op, n_push * 16) if variant is None else variant
+        if v == 2 and (not hd.mc_ptr or collective != "allreduce" or op != 0):
             v = 1
-        if v == 3 and (hd.ll is None or n_vec > LL_CAP_VEC):
+        if v == 3 and (hd.ll is None or n_push > LL_CAP_VEC):
             v = 0
         if v in (1, 2):
             n_vec = (n_vec + self.world - 1) // self.world * self.world
-        if v == 3:
-            self.C.allreduce(v, bf16, hd.ptrs, hd.sig_ptrs, hd.mc_ptr, src, dst, n_vec, float(scale), self.rank,
-                             self.world, self.max_blocks if max_blocks is None else max_blocks, hd.ll.ptrs, LL_CAP_VEC)
+        ll = (hd.ll.ptrs, LL_CAP_VEC) if v == 3 else ([], 0)
+        mb = self.max_blocks if max_blocks is None else max_blocks
+        if collective == "broadcast":
+            self.C.broadcast(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
+        elif collective == "allgather":
+            self.C.allgather(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, self.rank, self.world, mb, *ll)
         else:
             self.C.allreduce(v, bf16, hd.ptrs, hd.sig_ptrs, hd.mc_ptr, src, dst, n_vec, float(scale), self.rank,
-                             self.world, self.max_blocks if max_blocks is None else max_blocks)
+                             self.world, mb, *ll, op, root)
         return v
+
+    def supports_op(self, op) -> bool:
+        """Can ``all_reduce_`` / ``reduce_`` run this reduction (SUM, PRODUCT, MAX, MIN)?"""
+        return op_code(op) is not None
+
+    def supports_raw(self, t: torch.Tensor) -> bool:
+        """Can ``broadcast_`` / ``all_gather_`` take this tensor (CUDA, this device, contiguous, any dtype)?"""
+        return t.is_cuda and t.device == self.device and t.is_contiguous()
+
+    def local_rank(self, root: int) -> int:
+        """The rank within this world of global rank ``root``."""
+        if root not in self.ranks:
+            raise ValueError(f"rank {root} is not in this world (global ranks {self.ranks})")
+        return self.ranks.index(root)
 
     def all_reduce_(self, t: torch.Tensor, scale: float = 1.0, handle: Optional[SymmHandle] = None,
                     variant: Optional[int] = None, wire: Optional[torch.dtype] = None,
-                    max_blocks: Optional[int] = None) -> torch.Tensor:
-        """In-place ``t <- scale * sum_ranks t`` with the fused peer-memory kernels.
+                    max_blocks: Optional[int] = None, op=dist.ReduceOp.SUM) -> torch.Tensor:
+        """In-place ``t <- scale * sum_ranks t`` with the fused peer-memory kernels; ``op`` PRODUCT / MAX / MIN combine
+        instead of summing (fp32 in rank order, IEEE maximum / minimum: NaN wins, -0 < +0) and take no scale.
 
         ``handle`` given and ``t`` aliasing its data  -> zero-copy symmetric path;
         otherwise ``t`` is staged through a world-owned symmetric buffer with the
         copy-in / copy-out fused into the same kernel.  ``wire=torch.bfloat16``
-        sends fp32 tensors as bf16 over NVLink (fp32 accumulate, fp32 result)."""
+        sends fp32 tensors as bf16 over NVLink (fp32 accumulate, fp32 result; SUM only)."""
+        return self._reduce(t, scale, handle, variant, wire, max_blocks, op, -1)
+
+    def reduce_(self, t: torch.Tensor, root: int, op=dist.ReduceOp.SUM, handle: Optional[SymmHandle] = None,
+                variant: Optional[int] = None, wire: Optional[torch.dtype] = None,
+                max_blocks: Optional[int] = None) -> torch.Tensor:
+        """In-place reduce to global rank ``root``: its ``t`` receives the all-reduce result, every other rank's ``t`` is
+        left as it was."""
+        return self._reduce(t, 1.0, handle, variant, wire, max_blocks, op, self.local_rank(root))
+
+    def _reduce(self, t, scale, handle, variant, wire, max_blocks, op, root):
+        code = op_code(op)
+        if code is None:
+            raise ValueError(f"the fused reductions are SUM, PRODUCT, MAX and MIN, got {op!r}")
+        if code != 0 and scale != 1.0:
+            raise ValueError("scale applies to SUM only")
         if not self.supports(t):
             raise TypeError("fused all_reduce needs a contiguous CUDA float32/bfloat16 tensor on this device")
+        if code != 0 and wire is not None and wire != t.dtype:
+            raise TypeError("a bf16 wire for an fp32 tensor is for SUM only")
         if self.world == 1:
             if scale != 1.0:
                 t.mul_(scale)
@@ -373,7 +449,8 @@ class SymmWorld:
                 t.data_ptr() + t.numel() * es <= handle.ptrs[self.rank] + handle.nbytes and \
                 t.data_ptr() == handle.ptrs[self.rank] and (wire is None or wire == t.dtype):
             nbytes = (t.numel() * es + 15) // 16 * 16
-            self._launch(handle, t.dtype == torch.bfloat16, nbytes // 16, scale, None, None, variant, max_blocks)
+            self._launch(handle, t.dtype == torch.bfloat16, nbytes // 16, scale, None, None, variant, max_blocks,
+                         "reduce" if root >= 0 else "allreduce", code, root)
             return t
         wire_dt = wire or t.dtype
         if wire_dt not in _DTYPES or (wire_dt == torch.float32 and t.dtype == torch.bfloat16):
@@ -382,15 +459,86 @@ class SymmWorld:
         wire_bytes = t.numel() * wes
         st = self._staging_for(wire_dt, wire_bytes)
         flat = t.view(-1)
+        kind = "reduce" if root >= 0 else "allreduce"
         if wire_bytes % (16 * self.world) == 0 and t.data_ptr() % 16 == 0:
-            self._launch(st, wire_dt == torch.bfloat16, wire_bytes // 16, scale, flat, flat, variant, max_blocks)
+            self._launch(st, wire_dt == torch.bfloat16, wire_bytes // 16, scale, flat, flat, variant, max_blocks, kind, code,
+                         root)
         else:  # ragged size: torch copies around an in-place symmetric all-reduce
             buf = st.view(wire_dt, (wire_bytes + 15) // 16 * 16 // wes + 64 * 8)
             buf[:flat.numel()].copy_(flat)
             buf[flat.numel():].zero_()
-            self._launch(st, wire_dt == torch.bfloat16, (wire_bytes + 15) // 16, scale, None, None, variant, max_blocks)
-            flat.copy_(buf[:flat.numel()])
+            self._launch(st, wire_dt == torch.bfloat16, (wire_bytes + 15) // 16, scale, None, None, variant, max_blocks,
+                         kind, code, root)
+            if root < 0 or root == self.rank:
+                flat.copy_(buf[:flat.numel()])
         return t
+
+    def broadcast_(self, t: torch.Tensor, root: int, handle: Optional[SymmHandle] = None, variant: Optional[int] = None,
+                   max_blocks: Optional[int] = None) -> torch.Tensor:
+        """In place: every rank's ``t`` receives global rank ``root``'s bytes (any dtype; copied bit for bit)."""
+        r = self.local_rank(root)
+        if not self.supports_raw(t):
+            raise TypeError("fused broadcast needs a contiguous CUDA tensor on this device")
+        if self.world == 1:
+            return t
+        nbytes = t.numel() * t.element_size()
+        n_vec = (nbytes + 15) // 16
+        if handle is not None and t.data_ptr() == handle.ptrs[self.rank] and n_vec * 16 <= handle.nbytes:
+            self._launch(handle, False, n_vec, 1.0, None, None, variant, max_blocks, "broadcast", 0, r)
+            return t
+        st = self._staging_for(torch.float32, nbytes)
+        flat = t.view(-1)
+        if nbytes % (16 * self.world) == 0 and t.data_ptr() % 16 == 0:
+            self._launch(st, False, n_vec, 1.0, flat, flat, variant, max_blocks, "broadcast", 0, r)
+        else:  # ragged size: torch copies around an in-place symmetric broadcast
+            raw = flat.view(torch.uint8)
+            buf = st.view(torch.uint8, st.nbytes)
+            if self.rank == r:
+                buf[:nbytes].copy_(raw)
+            self._launch(st, False, n_vec, 1.0, None, None, variant, max_blocks, "broadcast", 0, r)
+            if self.rank != r:
+                raw.copy_(buf[:nbytes])
+        return t
+
+    def all_gather_(self, outs: List[torch.Tensor], t: torch.Tensor, handle: Optional[SymmHandle] = None,
+                    variant: Optional[int] = None, max_blocks: Optional[int] = None) -> List[torch.Tensor]:
+        """``outs[r]`` <- rank r's ``t`` on every rank (any dtype; copied bit for bit).  With ``handle``, ``t`` may sit at
+        byte ``rank * len`` of the handle's buffer (``len`` a multiple of 16): the call then gathers in place there, and
+        ``outs`` entries that already alias their slice are not copied."""
+        if len(outs) != self.world:
+            raise ValueError(f"all_gather needs {self.world} output tensors, got {len(outs)}")
+        if not self.supports_raw(t) or not all(self.supports_raw(o) for o in outs):
+            raise TypeError("fused all_gather needs contiguous CUDA tensors on this device")
+        if any(o.dtype != t.dtype or o.numel() != t.numel() for o in outs):
+            raise ValueError("every output of all_gather must have the input's dtype and size")
+        if self.world == 1:
+            outs[0].copy_(t)
+            return outs
+        nbytes = t.numel() * t.element_size()
+        seg = (nbytes + 15) // 16                              # vectors per rank
+        n_vec = seg * self.world
+        slot = seg * 16
+        if handle is not None and nbytes % 16 == 0 and t.data_ptr() == handle.ptrs[self.rank] + self.rank * slot and \
+                n_vec * 16 <= handle.nbytes:
+            self._launch(handle, False, n_vec, 1.0, None, None, variant, max_blocks, "allgather")
+            base, buf = handle.ptrs[self.rank], handle.view(torch.uint8)
+        else:
+            st = self._staging_for(torch.float32, n_vec * 16)
+            base, buf = st.ptrs[self.rank], st.view(torch.uint8, st.nbytes)
+            if nbytes % 16 == 0 and t.data_ptr() % 16 == 0:
+                o0 = outs[0].data_ptr()
+                contiguous = o0 % 16 == 0 and all(o.data_ptr() == o0 + r * nbytes for r, o in enumerate(outs))
+                dst = self.C.tensor_from_ptr(o0, n_vec * 16, torch.uint8, self.device.index) if contiguous else None
+                self._launch(st, False, n_vec, 1.0, t.view(-1), dst, variant, max_blocks, "allgather")
+                if contiguous:
+                    return outs
+            else:  # ragged size: stage this rank's bytes at its slot, gather in place
+                buf[self.rank * slot:self.rank * slot + nbytes].copy_(t.view(-1).view(torch.uint8))
+                self._launch(st, False, n_vec, 1.0, None, None, variant, max_blocks, "allgather")
+        for r, o in enumerate(outs):
+            if o.data_ptr() != base + r * slot:
+                o.view(-1).view(torch.uint8).copy_(buf[r * slot:r * slot + nbytes])
+        return outs
 
     def _staging_for(self, dtype, nbytes: int) -> SymmHandle:
         st = self._staging.get(dtype)
