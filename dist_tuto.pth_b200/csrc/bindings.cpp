@@ -55,7 +55,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const void* tail, float* det_partials, float* factors, int input_ready, cudaStream_t stream);
+                           float* det_partials, float* factors, int input_ready, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, cudaStream_t stream);
@@ -70,28 +70,11 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
                               float inv_bsz, float p_drop, int cluster, int max_clusters, long long grad_stride,
-                              const float* aux, const void* tail, float* det_partials, cudaStream_t stream);
-void b2_convnet_set_tc(int on);
-int b2_convnet_get_tc();
+                              const float* aux, float* det_partials, cudaStream_t stream);
 int b2_gemm_available();
 int b2_gemm_bf16_launch(const void* a, const void* b, void* c, const float* bias, int M, int N, int K, int relu,
                         int out_bf16, cudaStream_t stream);
 const char* b2_gemm_last_error();
-struct FusedTailHost {            // mirrors cn::FusedTailHost (csrc/convnet_args.cuh)
-  void* grad_ptrs[8];
-  void* inbox_ptrs[8];
-  float* params;
-  float* momentum;
-  unsigned long long* step;
-  float* aux;
-  const float* loss_acc;
-  float* loss_snapshot;
-  unsigned int* ticket;
-  float lr, mu, scale;
-  int rank, world;
-  int wire_bf16;
-  b2::LrSchedule sched;
-};
 struct BtBuffers {
   void *P1, *P2, *H, *DH, *dP2, *DC, *W2K, *W2R, *W3K, *W3T;
   unsigned char *A1, *A2;
@@ -216,9 +199,9 @@ struct ExecutorPy {
              torch::Tensor done_counter, torch::Tensor loss_acc, torch::Tensor in_dev, bool raw_u8, bool training, int rank,
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
              int max_in_flight, int cluster, torch::Tensor aux, std::vector<unsigned long long> inbox,
-             torch::Tensor loss_hist, bool fused_tail, torch::Tensor ticket, bool wire_bf16, c10::optional<torch::Tensor> grad_slots,
-             c10::optional<torch::Tensor> factors, py::object lr_schedule)
-      : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist, ticket} {
+             torch::Tensor loss_hist, bool wire_bf16, c10::optional<torch::Tensor> grad_slots, c10::optional<torch::Tensor> factors,
+             py::object lr_schedule)
+      : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
     const size_t block = (l.impl->block_bytes() + 255) / 256 * 256;
@@ -246,9 +229,8 @@ struct ExecutorPy {
     TORCH_CHECK(inbox.empty() || (int)inbox.size() == world, "inbox: one pointer per rank (or none)");
     for (size_t i = 0; i < inbox.size() && i < 8; ++i) c.inbox_ptrs[i] = (void*)(uintptr_t)inbox[i];
     c.push = !inbox.empty();
-    c.fused_tail = fused_tail ? 1 : 0;
     if (grad_slots.has_value()) {    // one GPU, one CTA per sample: slots + factors reduced by reduce_sgd (no bucket)
-      TORCH_CHECK(factors.has_value() && world == 1 && cluster <= 1 && !fused_tail, "grad_slots: one GPU, cluster 1, no fused tail");
+      TORCH_CHECK(factors.has_value() && world == 1 && cluster <= 1, "grad_slots: one GPU, cluster 1");
       TORCH_CHECK(grad_slots->is_cuda() && grad_slots->scalar_type() == torch::kFloat32 && grad_slots->numel() >= c.B * (int64_t)21888 &&
                   factors->is_cuda() && factors->scalar_type() == torch::kFloat32 && factors->numel() >= c.B * (int64_t)384,
                   "grad_slots: [B, 21888] fp32, factors: [B, 384] fp32");
@@ -259,11 +241,6 @@ struct ExecutorPy {
     }
     c.wire_bf16 = wire_bf16 ? 1 : 0;
     c.sched = to_sched(lr_schedule);
-    if (fused_tail) {
-      TORCH_CHECK(ticket.is_cuda() && ticket.scalar_type() == torch::kInt32 && ticket.numel() >= 2, "ticket: CUDA int32 [2]");
-      TORCH_CHECK(world == 1 || c.push, "the fused tail needs the push inbox when world > 1");
-      c.ticket = reinterpret_cast<unsigned int*>(ticket.data_ptr());
-    }
     const int cap = std::max(1, l.impl->num_slots() - 2);
     c10::cuda::CUDAGuard guard(params.device());
     c10::cuda::getCurrentCUDAStream().synchronize();     // the executor's streams do not wait for work queued on this one
@@ -416,14 +393,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });
-  m.def("convnet_set_tc", [](bool on) { b2_convnet_set_tc(on); }, "route conv2 forward/dgrad of the fused step through wgmma (bf16)");
-  m.def("convnet_get_tc", [] { return b2_convnet_get_tc() != 0; });
   m.def("convnet_smem_bytes", [] { return b2_convnet_smem_bytes(); });
   m.def("convnet_step", [](torch::Tensor params, c10::optional<torch::Tensor> grads, torch::Tensor x, torch::Tensor target,
                            c10::optional<torch::Tensor> loss_acc, c10::optional<torch::Tensor> out_logp,
                            c10::optional<torch::Tensor> mask_out, c10::optional<torch::Tensor> step, uint64_t seed,
                            int64_t sample_base, bool training, double inv_bsz, double p_drop, int max_ctas, int64_t grad_stride, int cluster,
-                           c10::optional<torch::Tensor> aux, py::object tail, c10::optional<torch::Tensor> det_partials,
+                           c10::optional<torch::Tensor> aux, py::none, c10::optional<torch::Tensor> det_partials,
                            c10::optional<torch::Tensor> factors, bool input_ready) {
     check_cuda_contig(params, "params"); check_cuda_contig(x, "x"); check_cuda_contig(target, "target");
     TORCH_CHECK(params.scalar_type() == torch::kFloat32 && params.numel() >= b2_convnet_npar(), "params: flat fp32 [21848]");
@@ -443,40 +418,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(params.device());
     const float* ax = nullptr;
     if (aux.has_value()) { TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000); ax = aux->data_ptr<float>(); }
-    // fused tail (gradient exchange + SGD inside the step kernel):
-    //   tail = (grad_ptrs, inbox_ptrs, momentum, lr, mu, scale, rank, world, ticket, loss_snapshot | None[, wire_bf16[, lr_schedule]])
-    FusedTailHost th;
-    const void* tp = nullptr;
-    if (!tail.is_none()) {
-      auto t = tail.cast<py::tuple>();
-      TORCH_CHECK(t.size() >= 10 && t.size() <= 12, "tail: 10/11/12-tuple");
-      th.wire_bf16 = 0;
-      TORCH_CHECK(g != nullptr && st != nullptr && la != nullptr, "the fused tail needs grads, a step counter and loss_acc");
-      auto gp = t[0].cast<std::vector<unsigned long long>>();
-      auto ib = t[1].cast<std::vector<unsigned long long>>();
-      auto mom = t[2].cast<torch::Tensor>();
-      auto tick = t[8].cast<torch::Tensor>();
-      std::memset(&th, 0, sizeof(th));
-      th.world = t[7].cast<int>(); th.rank = t[6].cast<int>();
-      TORCH_CHECK((int)gp.size() == std::max(1, th.world) && (th.world == 1 || (int)ib.size() == th.world), "tail: one bucket / inbox pointer per rank");
-      for (size_t i = 0; i < gp.size() && i < 8; ++i) th.grad_ptrs[i] = (void*)(uintptr_t)gp[i];
-      for (size_t i = 0; i < ib.size() && i < 8; ++i) th.inbox_ptrs[i] = (void*)(uintptr_t)ib[i];
-      check_cuda_contig(mom, "momentum");
-      TORCH_CHECK(mom.scalar_type() == torch::kFloat32 && mom.numel() == params.numel());
-      TORCH_CHECK(tick.is_cuda() && tick.scalar_type() == torch::kInt32 && tick.numel() >= 2, "ticket: CUDA int32 [2]");
-      th.params = params.data_ptr<float>(); th.momentum = mom.data_ptr<float>();
-      th.step = const_cast<unsigned long long*>(st);
-      th.aux = const_cast<float*>(ax); th.loss_acc = la;
-      th.loss_snapshot = t[9].is_none() ? nullptr : t[9].cast<torch::Tensor>().data_ptr<float>();
-      th.ticket = reinterpret_cast<unsigned int*>(tick.data_ptr());
-      th.lr = t[3].cast<float>(); th.mu = t[4].cast<float>(); th.scale = t[5].cast<float>();
-      th.wire_bf16 = t.size() > 10 ? (t[10].cast<bool>() ? 1 : 0) : 0;
-      th.sched = to_sched(t.size() > 11 ? py::object(t[11]) : py::none());
-      tp = &th;
-    }
     float* dp = nullptr;
     if (det_partials.has_value()) {
-      TORCH_CHECK(tp == nullptr, "deterministic mode and the fused tail are mutually exclusive");
       const int ctas = cluster > 1 ? B * cluster : (max_ctas > 0 ? std::min(B, max_ctas) : B);   // CTAs of the step grid
       TORCH_CHECK(det_partials->is_cuda() && det_partials->scalar_type() == torch::kFloat32 &&
                   det_partials->numel() >= (int64_t)std::max(1, ctas) * 21888, "det_partials: [ctas, 21888] fp32");
@@ -494,19 +437,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       TORCH_CHECK(cluster == 2 || cluster == 4 || cluster == 8, "cluster must be 1, 2, 4 or 8");
       ck_cuda(b2_convnet_cluster_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                         la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                        cluster, max_ctas, grad_stride, ax, tp, dp, cur_stream()), "convnet_cluster launch");
+                                        cluster, max_ctas, grad_stride, ax, dp, cur_stream()), "convnet_cluster launch");
       return;
     }
     // input_ready: x and target were not written by the kernel right before this launch, so the step kernel may read them
     // before its griddepcontrol.wait (Args::input_ready)
     ck_cuda(b2_convnet_step_launch(params.data_ptr<float>(), g, x.data_ptr(), u8, reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
                                    la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
-                                   max_ctas, grad_stride, ax, tp, dp, fp, input_ready ? 1 : 0, cur_stream()),
+                                   max_ctas, grad_stride, ax, dp, fp, input_ready ? 1 : 0, cur_stream()),
             "convnet_step launch");
   }, py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
      py::arg("mask_out"), py::arg("step"), py::arg("seed"), py::arg("sample_base"), py::arg("training"), py::arg("inv_bsz"),
      py::arg("p_drop") = 0.5, py::arg("max_ctas") = 0, py::arg("grad_stride") = 0, py::arg("cluster") = 1, py::arg("aux") = py::none(),
-     py::arg("tail") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none(),
+     // "reserved": an unused slot that takes only None, so calls passing det_partials, factors and input_ready by position
+     // keep their meaning
+     py::arg("reserved") = py::none(), py::arg("det_partials") = py::none(), py::arg("factors") = py::none(),
      py::arg("input_ready") = false);
   // ------------------------------------------------------------------ forward-only evaluation (csrc/convnet_eval.cu)
   m.def("convnet_eval_slot_words", [](int dev) {
@@ -719,15 +664,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def(py::init<LoaderPy&, torch::Tensor, torch::Tensor, torch::Tensor, std::vector<unsigned long long>,
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
                     int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor,
-                    std::vector<unsigned long long>, torch::Tensor, bool, torch::Tensor, bool, c10::optional<torch::Tensor>,
+                    std::vector<unsigned long long>, torch::Tensor, bool, c10::optional<torch::Tensor>,
                     c10::optional<torch::Tensor>, py::object>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
            py::arg("sample_base"), py::arg("grad_stride"), py::arg("lr"), py::arg("mu"), py::arg("p_drop"),
            py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(),
-           py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(), py::arg("fused_tail") = false,
-           py::arg("ticket") = torch::Tensor(), py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
+           py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(),
+           py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
            py::arg("factors") = py::none(), py::arg("lr_schedule") = py::none(), py::keep_alive<1, 2>())
       .def("chunking", [](ExecutorPy&) { return false; })      // read by bench.py: every step is issued on its own
       .def("flag_mode", [](ExecutorPy&) { return false; })     // read by bench.py: the streams are ordered by events

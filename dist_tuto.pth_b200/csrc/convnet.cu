@@ -28,28 +28,12 @@ namespace cn {
 
 constexpr int T = 512;              // 16 warps per sample: the phases are latency-bound, so more warps per CTA
 
-// The conv2 working set exists in two flavours that share one union:
-//   SIMT path : fp32 weights in two layouts + split-K partial sums + the zero-padded conv2-output gradient
-//   TC path   : bf16 wgmma operand tiles (K-major, 128B swizzle) for the conv2 GEMMs (fp32 accumulators in registers)
-//               forward  D[64 pos x 32 co]   = im2col(p1)[64 x 256] * W2[32 x 256]^T
-//               dgrad    D[64 pos x 256 k']  = dC[64 x 32 co]       * W2^T[256 x 32]^T      (k' = (ci/5)*128 + (ci%5)*25 + tap)
-//               wgrad    D[64 co  x 256 k ]  = dC^T[64 x 64 pos]    * im2col(p1)^T[256 x 64]^T
+// The conv2 working set: fp32 weights in two layouts + split-K partial sums + the zero-padded conv2-output gradient
 struct SimtBufs {
   float w2f[250 * 20];      // [ci][ky][kx][co]          forward: 4 output channels per float4
   float w2b[500 * 16];      // [co][ky][kx][half][8]     backward-data: 5 input channels per (half)
   float part[5 * 1440];     // conv2 partial sums [5][20][64] (5*1280 used) / dgrad partials [5][10][144] / S8b partials
   float dc2pad[DC_SIZE];      // conv2-output gradient, zero padded [20][16][16]
-};
-struct TcBufs {
-  unsigned char Bw[4 * 4096];   // W2 as B operand (fwd): 4 K-blocks x [32 rows x 128 B]
-  unsigned char Bt[32768];      // W2^T as B operand (dgrad): [256 rows x 128 B] (K = co, 32 used)
-  unsigned char A[4 * 8192];    // im2col(p1) as A operand: 4 K-blocks x [64 rows x 128 B]; later dA staging [64][128] fp32
-  unsigned char Ad[8192];       // dC as A operand (dgrad) [64 rows x 128 B]; fwd: conv2 output staging [64][32] fp32
-  unsigned char Adt[8192];      // dC^T as A operand (wgrad) [64 rows (co) x 64 positions]
-};
-union Scratch {
-  SimtBufs simt;
-  TcBufs tc;
 };
 
 // fc1.weight has no slot in the shared gradient accumulator: S6 sends its per-sample gradient straight to global memory.
@@ -73,7 +57,7 @@ __host__ __device__ constexpr int g1_idx(int c, int cell) { return cell * G1_CEL
 // Weights arrive by 1-D bulk copies straight from `params` / `aux`, so every staged array starts on a 16-byte boundary and
 // arrays copied together are laid out as in `params`: [w1 | b1] = params[W1, W2), [w3 | b3 | w4 | b4] = params[W3, NPAR).
 struct __align__(1024) Smem {
-  Scratch u;                // first member: 1024-byte aligned (SWIZZLE_128B operand tiles)
+  SimtBufs u;
   alignas(16) float w1[252];
   float b1[12];
   alignas(16) float b2[20];
@@ -95,15 +79,13 @@ struct __align__(1024) Smem {
   alignas(16) float g[NG];  // per-CTA gradient accumulators (index with gslot)
   uint64_t bar[4];          // weight staging: [0] w1,b1,b2  [1] aux w2f  [2] w3,b3,w4,b4  [3] aux w2b
   int work_ctr;             // dynamic work distribution inside a phase (warp-granular)
-  short koff[256];          // im2col LUT: k=(ci,ky,kx) -> offset inside p1, -1 for the K padding
   unsigned char a1[1440];   // conv1 pool argmax (0..3)
   unsigned char a2[320];    // conv2 pool argmax (0..3)
   float loss_local;
   int correct_local;
   int label;                // target of the current sample (loaded in S0 or, for a CTA's first sample, before pdl_wait)
 };
-static_assert(S7B_GROUPS * 1440 <= 5 * 1440 && 3 * S8B_WARPS * S8B_SET <= 5 * 1440 && 3 * S8B_WARPS * S8B_SET * 4 <= (int)sizeof(TcBufs::A),
-              "S7b and S8b partials fit the scratch they reuse");
+static_assert(S7B_GROUPS * 1440 <= 5 * 1440 && 3 * S8B_WARPS * S8B_SET <= 5 * 1440, "S7b and S8b partials fit the scratch they reuse");
 static_assert(sizeof(Smem) + 1024 <= 232448, "one CTA per SM: the launch asks for sizeof(Smem) + 1024 of the 227 KB opt-in");
 static_assert(offsetof(Smem, b1) == offsetof(Smem, w1) + (B1 - W1) * 4 && offsetof(Smem, b3) == offsetof(Smem, w3) + (B3 - W3) * 4 &&
                   offsetof(Smem, w4) == offsetof(Smem, w3) + (W4 - W3) * 4 && offsetof(Smem, b4) == offsetof(Smem, w3) + (B4 - W3) * 4,
@@ -111,14 +93,12 @@ static_assert(offsetof(Smem, b1) == offsetof(Smem, w1) + (B1 - W1) * 4 && offset
 static_assert(W2 % 4 == 0 && B2 % 4 == 0 && W3 % 4 == 0 && NPAR % 4 == 0 && AUX_W2B % 4 == 0 && NG % 4 == 0,
               "bulk copies and float4 flushes need 16-byte offsets");
 
-template <bool TC>
 __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   // the kernel has no static shared memory, so the dynamic window starts at offset 0 of the CTA's (1024-byte aligned)
   // shared space: addresses stay compile-time constants (a run-time round-up costs an extra add on every access)
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x;
-  if (TC && (tc::smem_u32(smem_raw) & 1023u) != 0u) __trap();   // SWIZZLE_128B operand tiles need 1024-byte alignment
   const float* __restrict__ P = a.params;
   const unsigned long long t_entry = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
 
@@ -158,13 +138,13 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   const bool early = a.input_ready && (int)blockIdx.x < a.B;
   if (early) {
     load_input(blockIdx.x);
-    if (!TC && a.backward)
-      for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.simt.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (a.backward)
+      for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   b2::pdl_wait();                    // parameters / step counter written by the previous all-reduce+SGD kernel
   const unsigned long long t_waited = a.phase_ts != nullptr ? b2::globaltimer() : 0ull;
   // conv2.weight already in both smem layouts (written by sgd.cu): staged by bulk copies like the other weights
-  const bool fast = (a.aux != nullptr) && !TC;
+  const bool fast = a.aux != nullptr;
   if (tid == 0) {
     // One thread hands all weight staging to the TMA engine, in order of first use; each phase waits only for the group it
     // reads (S1: bar 0, S2: bar 1, S3: bar 2, S7b: bar 3), so the copies overlap the earlier phases.
@@ -174,30 +154,23 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     tc::bulk_g2s(s.b2, P + B2, 80, &s.bar[0]);
     if (fast) {
       tc::mbar_expect_tx(&s.bar[1], AUX_W2B * 4);
-      tc::bulk_g2s(s.u.simt.w2f, a.aux + AUX_W2F, AUX_W2B * 4, &s.bar[1]);
+      tc::bulk_g2s(s.u.w2f, a.aux + AUX_W2F, AUX_W2B * 4, &s.bar[1]);
     }
     tc::mbar_expect_tx(&s.bar[2], (NPAR - W3) * 4);
     tc::bulk_g2s(s.w3, P + W3, (NPAR - W3) * 4, &s.bar[2]);              // w3 | b3 | w4 | b4
     if (fast) {
       tc::mbar_expect_tx(&s.bar[3], (AUX_TOTAL - AUX_W2B) * 4);
-      tc::bulk_g2s(s.u.simt.w2b, a.aux + AUX_W2B, (AUX_TOTAL - AUX_W2B) * 4, &s.bar[3]);
+      tc::bulk_g2s(s.u.w2b, a.aux + AUX_W2B, (AUX_TOTAL - AUX_W2B) * 4, &s.bar[3]);
     }
   }
   {
-    // without aux: conv2.weight is scattered into its smem layout(s) from registers (all loads in flight before the first store)
+    // without aux: conv2.weight is scattered into its smem layouts from registers (all loads in flight before the first store)
     const float4* __restrict__ P4w2 = reinterpret_cast<const float4*>(P + W2);   // 1250 float4, 16B aligned
     float4 v[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       const int i4 = tid + k * T;
       v[k] = (!fast && i4 < 1250) ? __ldg(P4w2 + i4) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (TC) {
-      // zero the bf16 operand tiles (row / K padding must be 0), build the im2col LUT
-      uint4* z = reinterpret_cast<uint4*>(s.u.tc.Bw);
-      for (int i = tid; i < (16384 + 32768) / 16; i += T) z[i] = make_uint4(0u, 0u, 0u, 0u);
-      if (tid < 256) s.koff[tid] = tid < 250 ? (short)p1_idx(tid / 25, (tid % 25) / 5, tid % 5) : (short)-1;
-      __syncthreads();
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -208,28 +181,19 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         for (int e = 0; e < 4; ++e) {             // conv2.weight [co][ci][ky][kx]
           const int i = i4 * 4 + e;
           const int co = i / 250, r = i % 250, ci = r / 25, kk = r % 25;
-          if (TC) {
-            const __nv_bfloat16 wb = __float2bfloat16(w[e]);
-            *reinterpret_cast<__nv_bfloat16*>(s.u.tc.Bw + (r >> 6) * 4096 + tc::sw128_offset(co, r & 63)) = wb;
-            const int n = (ci / 5) * 128 + (ci % 5) * 25 + kk;      // dgrad output column (ci groups on 128 boundaries)
-            *reinterpret_cast<__nv_bfloat16*>(s.u.tc.Bt + tc::sw128_offset(n, co)) = wb;
-          } else {
-            s.u.simt.w2f[(ci * 25 + kk) * 20 + co] = w[e];
-            s.u.simt.w2b[((co * 25 + kk) * 2 + ci / 5) * 8 + ci % 5] = w[e];
-          }
+          s.u.w2f[(ci * 25 + kk) * 20 + co] = w[e];
+          s.u.w2b[((co * 25 + kk) * 2 + ci / 5) * 8 + ci % 5] = w[e];
         }
       }
     }
-    }
+  }
   if (tid == 0) { s.loss_local = 0.f; s.correct_local = 0; }
   const unsigned long long step = a.step ? *a.step : 0ull;
   const float keep_scale = 1.f / (1.f - a.p_drop);
   // this step's gradient bucket (double-buffered: see sgd.cu); fc1.weight's share goes there from S6, the rest in the flush
   float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
-  if (TC) tc::fence_proxy_async();
   // The barrier that ends S0 publishes the mbarrier initialisation and the scattered conv2.weight before any phase reads
   // them, so the RNG of S0 need not wait here for thread 0's copy issue.
-  if (TC) __syncthreads();
   auto stamp = [&](int k) {          // opt-in phase timestamps (bench/step_phases.py); call after a barrier
     if (a.phase_ts != nullptr && tid == 0) b2::ts_put(a.phase_ts, step, (int)blockIdx.x, k, b2::globaltimer());
   };
@@ -249,8 +213,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       s.rnd[q * 4 + 0] = r.x * k; s.rnd[q * 4 + 1] = r.y * k;
       s.rnd[q * 4 + 2] = r.z * k; s.rnd[q * 4 + 3] = r.w * k;
     }
-    if (!TC && a.backward && !loaded)
-      for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.simt.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (a.backward && !loaded)
+      for (int i = tid; i < DC_SIZE / 4; i += T) reinterpret_cast<float4*>(s.u.dc2pad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
     stamp(b2::TS_S0);
 
@@ -297,50 +261,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     __syncthreads();
     stamp(b2::TS_S1);
 
-    // -------------------------------------------------------------- S2: conv2 (TC: im2col + wgmma GEMM | SIMT: K split 5)
-    if (TC) {
-      // im2col(p1) -> bf16 A operand, 2048 16-byte chunks (row = output position, 8 consecutive k per chunk)
-#pragma unroll
-      for (int m = 0; m < 4; ++m) {
-        const int chunk = tid + m * T, r = chunk >> 5, c = chunk & 31;
-        const int base = (r >> 3) * P1_ROW + (r & 7);
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int ko = s.koff[c * 8 + e];
-          f[e] = ko >= 0 ? s.p1[ko + base] : 0.f;
-        }
-        const uint4 pk = make_uint4(b2::pack_bf16x2(f[0], f[1]), b2::pack_bf16x2(f[2], f[3]), b2::pack_bf16x2(f[4], f[5]),
-                                    b2::pack_bf16x2(f[6], f[7]));
-        *reinterpret_cast<uint4*>(s.u.tc.A + (c >> 3) * 8192 + (r >> 3) * 1024 + (r & 7) * 128 + ((((c & 7) ^ (r & 7)) & 7) << 4)) = pk;
-      }
-      tc::fence_proxy_async();
-      __syncthreads();
-      if (tid < 128) {                            // warpgroup 0: D[64 pos x 32 co] in registers
-        float d[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) d[i] = 0.f;
-        const uint32_t a0 = tc::smem_u32(s.u.tc.A), b0 = tc::smem_u32(s.u.tc.Bw);
-        tc::wg_fence();
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc::mma<32>(d, tc::smem_desc_sw128(a0 + kb * 8192 + k * 32), tc::smem_desc_sw128(b0 + kb * 4096 + k * 32),
-                        (kb | k) != 0 ? 1u : 0u);
-        tc::wg_commit();
-        tc::wg_wait_all();
-        tc::acc_fence<16>(d);
-        float* dst = reinterpret_cast<float*>(s.u.tc.Ad);   // conv2 output staging [64][32] fp32, float4 index ^= row & 7
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-          const int row = tc::acc_row(tid, i), col = tc::acc_col(tid, i);
-          *reinterpret_cast<float2*>(dst + row * 32 + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) = make_float2(d[i], d[i + 1]);
-        }
-      }
-      __syncthreads();
-    }
-    if (!TC) {
+    // -------------------------------------------------------------- S2: conv2 (K split 5)
     if (fast) tc::mbar_wait(&s.bar[1], 0);         // w2f
     if (tid < 400) {
       const int cell = tid & 15, cg = (tid >> 4) % 5, ks = tid / 80;
@@ -362,7 +283,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         for (int ky = 0; ky < 5; ++ky)
 #pragma unroll
           for (int kx = 0; kx < 5; ++kx) {
-            const float4 w = *reinterpret_cast<const float4*>(&s.u.simt.w2f[((ci * 5 + ky) * 5 + kx) * 20 + cg * 4]);
+            const float4 w = *reinterpret_cast<const float4*>(&s.u.w2f[((ci * 5 + ky) * 5 + kx) * 20 + cg * 4]);
             const float i00 = patch[ky][kx], i01 = patch[ky][kx + 1], i10 = patch[ky + 1][kx], i11 = patch[ky + 1][kx + 1];
             acc[0][0] = fmaf(w.x, i00, acc[0][0]); acc[0][1] = fmaf(w.y, i00, acc[0][1]);
             acc[0][2] = fmaf(w.z, i00, acc[0][2]); acc[0][3] = fmaf(w.w, i00, acc[0][3]);
@@ -377,31 +298,19 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       // part[ks][co][cell][pos]  (pos = dy*2+dx inside the pool window)
 #pragma unroll
       for (int c = 0; c < 4; ++c)
-        *reinterpret_cast<float4*>(&s.u.simt.part[ks * 1440 + ((cg * 4 + c) * 16 + cell) * 4]) =
+        *reinterpret_cast<float4*>(&s.u.part[ks * 1440 + ((cg * 4 + c) * 16 + cell) * 4]) =
             make_float4(acc[0][c], acc[1][c], acc[2][c], acc[3][c]);
     }
     __syncthreads();
-    }
 
     // -------------------------------------------------------------- S2b: +bias, dropout2d, maxpool2, relu
     for (int o = tid; o < 320; o += T) {
       const int co = o >> 4;
-      float4 q;
-      if (TC) {
-        const int cell = o & 15, p00 = (2 * (cell >> 2)) * 8 + 2 * (cell & 3);
-        const float* c2 = reinterpret_cast<const float*>(s.u.tc.Ad);
-        const int cb = co >> 2, cl = co & 3;
-        q.x = c2[(p00) * 32 + ((cb ^ ((p00) & 7)) << 2) + cl];
-        q.y = c2[(p00 + 1) * 32 + ((cb ^ ((p00 + 1) & 7)) << 2) + cl];
-        q.z = c2[(p00 + 8) * 32 + ((cb ^ ((p00 + 8) & 7)) << 2) + cl];
-        q.w = c2[(p00 + 9) * 32 + ((cb ^ ((p00 + 9) & 7)) << 2) + cl];
-      } else {
-        q = *reinterpret_cast<const float4*>(&s.u.simt.part[o * 4]);
+      float4 q = *reinterpret_cast<const float4*>(&s.u.part[o * 4]);
 #pragma unroll
-        for (int ks = 1; ks < 5; ++ks) {
-          const float4 t = *reinterpret_cast<const float4*>(&s.u.simt.part[ks * 1440 + o * 4]);
-          q.x += t.x; q.y += t.y; q.z += t.z; q.w += t.w;
-        }
+      for (int ks = 1; ks < 5; ++ks) {
+        const float4 t = *reinterpret_cast<const float4*>(&s.u.part[ks * 1440 + o * 4]);
+        q.x += t.x; q.y += t.y; q.z += t.z; q.w += t.w;
       }
       const float bias = s.b2[co], sc = s.m2[co];
       const float v0 = (q.x + bias) * sc, v1 = (q.y + bias) * sc, v2 = (q.z + bias) * sc, v3 = (q.w + bias) * sc;
@@ -505,10 +414,8 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         const int co = o >> 4, cell = o & 15, arg = s.a2[o];
         const float gv = s.p2[o] > 0.f ? d * s.m2[co] : 0.f;
         s.g2[o] = gv;
-        if (!TC) {
-          const int y = 2 * (cell >> 2) + (arg >> 1), x = 2 * (cell & 3) + (arg & 1);
-          s.u.simt.dc2pad[co * DC_PLANE + (y + 4) * DC_ROW + (x + 4)] = gv;
-        }
+        const int y = 2 * (cell >> 2) + (arg >> 1), x = 2 * (cell & 3) + (arg & 1);
+        s.u.dc2pad[co * DC_PLANE + (y + 4) * DC_ROW + (x + 4)] = gv;
       }
       // fc1.weight gradient dh (x) p2 of this sample goes straight to global memory: as its two factors (370 floats, stored
       // by threads that are idle in this phase; the reduction of convnet_reduce.cuh forms the sum over samples), or as the
@@ -544,7 +451,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     // -------------------------------------------------------------- S7a: conv2 weight/bias gradient (sparse)
     // Work items are handed out 32 at a time per warp from a shared counter, so the warps that had no (or a short)
     // S7b tile start here immediately and the phase ends balanced.  item < 1000: (co, ci, ky) = 5 taps x 16 pooled
-    // cells; item 1000..1019: bias gradient of channel item-1000.  (TC mode: weight items are done by wgmma.)
+    // cells; item 1000..1019: bias gradient of channel item-1000.
     auto s7a = [&]() {
       for (;;) {
         int base = 0;
@@ -553,24 +460,22 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         if (base >= 1020) break;
         const int item = base + (tid & 31);
         if (item < 1000) {
-          if (!TC) {
-            const int co = item / 50, r = item - co * 50, ci = r / 5, ky = r - ci * 5;
-            float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+          const int co = item / 50, r = item - co * 50, ci = r / 5, ky = r - ci * 5;
+          float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll 4
-            for (int cell = 0; cell < 16; ++cell) {
-              const float gv = s.g2[co * 16 + cell];
-              if (gv != 0.f) {
-                const int arg = s.a2[co * 16 + cell];
-                const int ay = 2 * (cell >> 2) + (arg >> 1), ax = 2 * (cell & 3) + (arg & 1);
-                const float* src = &s.p1[p1_idx(ci, ay + ky, ax)];
+          for (int cell = 0; cell < 16; ++cell) {
+            const float gv = s.g2[co * 16 + cell];
+            if (gv != 0.f) {
+              const int arg = s.a2[co * 16 + cell];
+              const int ay = 2 * (cell >> 2) + (arg >> 1), ax = 2 * (cell & 3) + (arg & 1);
+              const float* src = &s.p1[p1_idx(ci, ay + ky, ax)];
 #pragma unroll
-                for (int kx = 0; kx < 5; ++kx) acc[kx] = fmaf(gv, src[kx], acc[kx]);
-              }
+              for (int kx = 0; kx < 5; ++kx) acc[kx] = fmaf(gv, src[kx], acc[kx]);
             }
-            float* dst = &s.g[gslot(W2) + co * 250 + ci * 25 + ky * 5];
-#pragma unroll
-            for (int kx = 0; kx < 5; ++kx) dst[kx] += acc[kx];
           }
+          float* dst = &s.g[gslot(W2) + co * 250 + ci * 25 + ky * 5];
+#pragma unroll
+          for (int kx = 0; kx < 5; ++kx) dst[kx] += acc[kx];
         } else if (item < 1020) {
           const int co = item - 1000;
           float d = 0.f;
@@ -580,113 +485,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         }
       }
     };
-    // -------------------------------------------------------------- S7b/S8a: conv2 weight + data gradients on wgmma
-    if (TC) {
-      // (1) dC[64 pos][co] (one non-zero per pool window and channel) as the bf16 A operand of the dgrad GEMM
-      if (tid < 256) {
-        const int r = tid >> 2, c8 = tid & 3, oy = r >> 3, ox = r & 7;
-        const int cell = (oy >> 1) * 4 + (ox >> 1), sub = (oy & 1) * 2 + (ox & 1);
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int co = c8 * 8 + e;
-          f[e] = (co < 20 && s.a2[co * 16 + cell] == sub) ? s.g2[co * 16 + cell] : 0.f;
-        }
-        const uint4 pk = make_uint4(b2::pack_bf16x2(f[0], f[1]), b2::pack_bf16x2(f[2], f[3]), b2::pack_bf16x2(f[4], f[5]),
-                                    b2::pack_bf16x2(f[6], f[7]));
-        *reinterpret_cast<uint4*>(s.u.tc.Ad + (r >> 3) * 1024 + (r & 7) * 128 + (((c8 ^ (r & 7)) & 7) << 4)) = pk;
-      } else if (tid < 256 + 160) {
-        // (2) dC^T[co][pos] as the A operand of the wgrad GEMM (rows >= 20 are never read back)
-        const int q = tid - 256, co = q >> 3, oy = q & 7;              // chunk = 8 positions of output row oy
-        float f[8];
-#pragma unroll
-        for (int ox = 0; ox < 8; ++ox) {
-          const int cell = (oy >> 1) * 4 + (ox >> 1), sub = (oy & 1) * 2 + (ox & 1);
-          f[ox] = s.a2[co * 16 + cell] == sub ? s.g2[co * 16 + cell] : 0.f;
-        }
-        const uint4 pk = make_uint4(b2::pack_bf16x2(f[0], f[1]), b2::pack_bf16x2(f[2], f[3]), b2::pack_bf16x2(f[4], f[5]),
-                                    b2::pack_bf16x2(f[6], f[7]));
-        *reinterpret_cast<uint4*>(s.u.tc.Adt + (co >> 3) * 1024 + (co & 7) * 128 + (((oy ^ (co & 7)) & 7) << 4)) = pk;
-      }
-      // (3) im2col(p1)^T[k][pos] as the B operand of the wgrad GEMM: 256 rows x 8 chunks of 8 consecutive ox
-#pragma unroll
-      for (int m = 0; m < 4; ++m) {
-        const int chunk = tid + m * T, k = chunk >> 3, oy = chunk & 7;
-        const int ko = s.koff[k];
-        uint4 pk = make_uint4(0u, 0u, 0u, 0u);
-        if (ko >= 0) {
-          const float* src = &s.p1[ko + oy * P1_ROW];
-          pk = make_uint4(b2::pack_bf16x2(src[0], src[1]), b2::pack_bf16x2(src[2], src[3]), b2::pack_bf16x2(src[4], src[5]),
-                          b2::pack_bf16x2(src[6], src[7]));
-        }
-        *reinterpret_cast<uint4*>(s.u.tc.A + (k >> 3) * 1024 + (k & 7) * 128 + (((oy ^ (k & 7)) & 7) << 4)) = pk;
-      }
-      tc::fence_proxy_async();
-      __syncthreads();
-      // warpgroup g: dgrad D[64 pos x 64 k'] at columns 64g.. (K = co, 2 steps) and wgrad D[64 co x 64 k] at columns 64g..
-      // (K = pos, 4 steps); the two 32-register accumulators stay in the issuing warpgroup
-      const int wg = tid >> 7, t = tid & 127;
-      float dd[32], dw[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) { dd[i] = 0.f; dw[i] = 0.f; }
-      {
-        const uint32_t ad = tc::smem_u32(s.u.tc.Ad), bt = tc::smem_u32(s.u.tc.Bt) + wg * 8192;
-        const uint32_t at = tc::smem_u32(s.u.tc.Adt), bi = tc::smem_u32(s.u.tc.A) + wg * 8192;
-        tc::wg_fence();
-        tc::mma<64>(dd, tc::smem_desc_sw128(ad), tc::smem_desc_sw128(bt), 0u);                 // dgrad: K = co
-        tc::mma<64>(dd, tc::smem_desc_sw128(ad + 32), tc::smem_desc_sw128(bt + 32), 1u);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)                                                            // wgrad: K = pos
-          tc::mma<64>(dw, tc::smem_desc_sw128(at + k * 32), tc::smem_desc_sw128(bi + k * 32), k != 0 ? 1u : 0u);
-        tc::wg_commit();
-      }
-      tc::wg_wait_all();
-      tc::acc_fence<32>(dd);
-      tc::acc_fence<32>(dw);
-      s7a();                                                  // bias gradient (20 items)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {                          // conv2.weight gradient: accumulator row = co, column = k
-        const int co = tc::acc_row(t, i), k = wg * 64 + tc::acc_col(t, i);
-        if (co < 20 && k < 250) s.g[gslot(W2) + co * 250 + k] += dw[i];
-      }
-      __syncthreads();                                        // operand tiles consumed: A becomes the dgrad staging tile
-      float* stage = reinterpret_cast<float*>(s.u.tc.A);      // [64 rows][128 cols] fp32, float4 index XOR-swizzled by row
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {                  // input channels 5*half .. 5*half+4  <->  columns 128*half ..
-        if ((wg >> 1) == half) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const int row = tc::acc_row(t, i), j = (wg & 1) * 64 + tc::acc_col(t, i);
-            *reinterpret_cast<float2*>(stage + row * 128 + ((((j >> 2) ^ (row & 31)) & 31) << 2) + (j & 3)) = make_float2(dd[i], dd[i + 1]);
-          }
-        }
-        __syncthreads();
-        // col2im gather: dp1[ci][y][x] = sum_{ky,kx} dA[(y-ky, x-kx)][ci, ky, kx], fused with relu'/pool routing of conv1
-        for (int o5 = tid; o5 < 720; o5 += T) {
-          const int cil = o5 / 144, rem = o5 - cil * 144, y = rem / 12, x = rem - y * 12;
-          float d = 0.f;
-#pragma unroll
-          for (int ky = 0; ky < 5; ++ky) {
-            const int oy = y - ky;
-            if ((unsigned)oy < 8u) {
-#pragma unroll
-              for (int kx = 0; kx < 5; ++kx) {
-                const int ox = x - kx;
-                if ((unsigned)ox < 8u) {
-                  const int row = oy * 8 + ox, j = cil * 25 + ky * 5 + kx;
-                  d += stage[row * 128 + ((((j >> 2) ^ (row & 31)) & 31) << 2) + (j & 3)];
-                }
-              }
-            }
-          }
-          const int o = (half * 5 + cil) * 144 + rem, arg = s.a1[o];
-          const int off = (2 * y + (arg >> 1)) * 28 + 2 * x + (arg & 1);
-          s.g1[g1_idx(half * 5 + cil, rem)] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
-        }
-        __syncthreads();
-      }
-    }
-    if (!TC) {
+    // -------------------------------------------------------------- S7b: conv2 data gradient
     if (fast) tc::mbar_wait(&s.bar[3], 0);         // w2b
     // Warp-uniform channel ranges: warps 3g .. 3g+2 take output channels 4g .. 4g+3 (a Dropout2d skip skips the whole warp)
     // and together cover 12 rows x 4 column triples x 2 input-channel halves; lane = (half, row 4k + r, column triple q).
@@ -703,7 +502,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       for (int co = 4 * cg; co < 4 * cg + 4; ++co) {
         if (s.m2[co] == 0.f) continue;            // channel dropped by Dropout2d: gradient plane is zero (warp-uniform)
         float patch[5][7];
-        const float* src = &s.u.simt.dc2pad[co * DC_PLANE + y * DC_ROW + x0];
+        const float* src = &s.u.dc2pad[co * DC_PLANE + y * DC_ROW + x0];
 #pragma unroll
         for (int i = 0; i < 5; ++i)
 #pragma unroll
@@ -712,7 +511,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
         for (int ky = 0; ky < 5; ++ky)
 #pragma unroll
           for (int kx = 0; kx < 5; ++kx) {
-            const float* wp = &s.u.simt.w2b[((co * 25 + ky * 5 + kx) * 2 + half) * 8];
+            const float* wp = &s.u.w2b[((co * 25 + ky * 5 + kx) * 2 + half) * 8];
             const float4 w = *reinterpret_cast<const float4*>(wp);
             const float w4 = wp[4];
 #pragma unroll
@@ -725,7 +524,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
       }
 #pragma unroll
       for (int c = 0; c < 5; ++c) {
-        float* dst = &s.u.simt.part[cg * 1440 + (half * 5 + c) * 144 + y * 12 + x0];
+        float* dst = &s.u.part[cg * 1440 + (half * 5 + c) * 144 + y * 12 + x0];
         dst[0] = acc[0][c]; dst[1] = acc[1][c]; dst[2] = acc[2][c];
       }
     }
@@ -736,13 +535,12 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     for (int o = tid; o < 1440; o += T) {
       float d = 0.f;
 #pragma unroll
-      for (int cg = 0; cg < S7B_GROUPS; ++cg) d += s.u.simt.part[cg * 1440 + o];
+      for (int cg = 0; cg < S7B_GROUPS; ++cg) d += s.u.part[cg * 1440 + o];
       const int cell = o % 144, arg = s.a1[o];
       const int off = (2 * (cell / 12) + (arg >> 1)) * 28 + 2 * (cell % 12) + (arg & 1);
       s.g1[g1_idx(o / 144, cell)] = make_float2(s.p1[p1_of(o)] > 0.f ? d : 0.f, __int_as_float(off));
     }
     __syncthreads();
-    }
     stamp(b2::TS_S8A);
 
     // -------------------------------------------------------------- S8b: conv1 weight/bias gradient (sparse)
@@ -752,7 +550,7 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     // 1, 28 or 29 words) inside a cell: all 30 lanes hit distinct banks or share a word.  The 24 partial sets (one per warp
     // and j) go to shared memory and are added in set order.
     {
-      float* const red = TC ? reinterpret_cast<float*>(s.u.tc.A) : s.u.simt.part;   // [24 sets][S8B_SET], dead after S8a
+      float* const red = s.u.part;   // [24 sets][S8B_SET], dead after S8a
       const int lane = tid & 31, warp = tid >> 5, j = lane / 10, c = lane - j * 10;
       if (warp < S8B_WARPS) {
         float acc[26];
@@ -823,8 +621,6 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
     }
   }
   stamp(b2::TS_EXIT);
-  // ------------------------------------------------------------------ fused tail: gradient exchange + SGD in this kernel
-  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x, reinterpret_cast<float*>(smem_raw));   // grid <= B: every CTA flushed
 }
 
 }  // namespace cn
@@ -836,28 +632,15 @@ unsigned long long* b2_phase_ts();   // sgd.cu
 size_t b2_convnet_smem_bytes() { return sizeof(cn::Smem) + 1024; }
 int b2_convnet_npar() { return cn::NPAR; }
 
-static int g_convnet_tc = -1;      // -1: read B200DIST_CONVNET_TC on first use
-void b2_convnet_set_tc(int on) { g_convnet_tc = on ? 1 : 0; }
-int b2_convnet_get_tc() {
-  if (g_convnet_tc < 0) {
-    const char* e = getenv("B200DIST_CONVNET_TC");
-    g_convnet_tc = (e != nullptr && e[0] == '1') ? 1 : 0;
-  }
-  return g_convnet_tc;
-}
-
 int b2_convnet_step_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const cn::FusedTailHost* tail, float* det_partials, float* factors, int input_ready,
-                           cudaStream_t stream) {
+                           float* det_partials, float* factors, int input_ready, cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cn::Smem) + 1024;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(cn::convnet_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(cn::convnet_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = cudaFuncSetAttribute(cn::convnet_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
@@ -866,7 +649,6 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   a.mask_out = mask_out; a.step = step; a.seed = seed; a.sample_base = sample_base; a.B = B; a.x_u8 = x_u8;
   a.training = training; a.backward = backward; a.inv_bsz = inv_bsz; a.p_drop = p_drop;
   a.mean = 0.1307f; a.inv_std = 1.f / 0.3081f; a.grad_stride = grad_stride; a.aux = aux;
-  cn::fill_tail(a.tail, backward ? tail : nullptr, grad_stride);
   a.det_partials = backward ? det_partials : nullptr;
   a.factors = (backward && det_partials != nullptr) ? factors : nullptr;
   a.phase_ts = b2_phase_ts();
@@ -874,12 +656,6 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   int grid = B;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   if (grid < 1) grid = 1;
-  if (a.tail.enabled) {       // the tail's grid-wide check-in spins: every CTA must be resident (one CTA per SM)
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (grid > sms) grid = sms;                 // CTAs loop over samples (b += gridDim.x)
-  }
   static const int pdl = [] { const char* e = getenv("B200DIST_PDL"); return (e == nullptr || e[0] != '0') ? 1 : 0; }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -892,9 +668,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e = b2_convnet_get_tc() ? cudaLaunchKernelEx(&cfg, cn::convnet_step_kernel<true>, a)
-                                      : cudaLaunchKernelEx(&cfg, cn::convnet_step_kernel<false>, a);
-  return (int)e;
+  return (int)cudaLaunchKernelEx(&cfg, cn::convnet_step_kernel, a);
 }
 
 }  // extern "C"

@@ -2,8 +2,6 @@
 #pragma once
 #include <cuda_runtime.h>
 
-#include <cstring>
-
 #include "sgd_device.cuh"
 
 namespace cn {
@@ -35,7 +33,6 @@ struct Args {
   float mean, inv_std;      // uint8 normalisation
   long long grad_stride;    // elements between the two gradient buckets (0: single bucket); bucket = step & 1
   const float* aux;         // optional: conv2.weight pre-arranged by the SGD kernel as [w2f 5000 | w2b 8000] (see sgd.cu)
-  b2::FusedTail tail;       // enabled: gradient exchange + SGD run in the tail of THIS kernel (sgd_device.cuh)
   float* det_partials;      // per-CTA slots: CTA i stores its gradient sums and loss terms to det_partials + i * DET_STRIDE
                             // (plain stores) instead of red.add-ing into the bucket; they are summed in slot order afterwards,
                             // by det_reduce_kernel or, with `factors`, by the reduction of convnet_reduce.cuh
@@ -48,37 +45,6 @@ struct Args {
 
 constexpr int DET_STRIDE = 21888;   // = NPAR_ALLOC of ops/convnet_fused.py
 constexpr int FAC_STRIDE = 384, FAC_P2 = 64;   // per-sample fc1 factors: dh at [0, 50), p2 at [FAC_P2, FAC_P2 + 320)
-
-// Host-side description of the fused tail (C ABI of the launchers); nullptr / enabled == 0 -> two-kernel step.
-struct FusedTailHost {
-  void* grad_ptrs[8];
-  void* inbox_ptrs[8];
-  float* params;
-  float* momentum;
-  unsigned long long* step;
-  float* aux;
-  const float* loss_acc;
-  float* loss_snapshot;
-  unsigned int* ticket;
-  float lr, mu, scale;
-  int rank, world;
-  int wire_bf16;
-  b2::LrSchedule sched;     // lr schedule of the tail's update (zero: constant lr)
-};
-
-inline void fill_tail(b2::FusedTail& t, const FusedTailHost* h, long long grad_stride) {
-  memset(&t, 0, sizeof(t));
-  if (h == nullptr) return;
-  t.enabled = 1;
-  for (int i = 0; i < 8; ++i) { t.sgd.grads.p[i] = h->grad_ptrs[i]; t.sgd.inbox.p[i] = h->inbox_ptrs[i]; }
-  t.sgd.params = h->params; t.sgd.momentum = h->momentum; t.sgd.step = h->step; t.sgd.done_counter = nullptr;
-  t.sgd.n_vec = NPAR / 4; t.sgd.lr = h->lr; t.sgd.mu = h->mu; t.sgd.scale = h->scale; t.sgd.rank = h->rank; t.sgd.world = h->world;
-  t.sgd.zero_grads = 1; t.sgd.grad_stride = grad_stride; t.sgd.aux = h->aux;
-  t.sgd.wire_bf16 = h->wire_bf16;
-  t.sgd.sched = h->sched;
-  t.sgd.loss_acc = h->loss_acc; t.sgd.loss_snapshot = h->loss_acc ? h->loss_snapshot : nullptr;
-  t.ticket = h->ticket;
-}
 
 constexpr int AUX_W2F = 0, AUX_W2B = 5000, AUX_TOTAL = 13000;
 

@@ -533,8 +533,6 @@ __global__ void __launch_bounds__(T, 1) convnet_cluster_kernel(Args a) {
     }
   }
   cl.sync();                                       // no CTA exits while a peer may still address its shared memory
-  // fused tail: gradient exchange + SGD in this kernel (every cluster carried >= 1 sample: gridDim.x / C <= B)
-  if (a.tail.enabled && a.backward) b2::fused_tail(a.tail, step, (int)gridDim.x, (int)blockIdx.x, reinterpret_cast<float*>(smem_raw));
 }
 
 }  // namespace cnc
@@ -546,7 +544,7 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
                               float inv_bsz, float p_drop, int cluster, int max_clusters, long long grad_stride,
-                              const float* aux, const cn::FusedTailHost* tail, float* det_partials, cudaStream_t stream) {
+                              const float* aux, float* det_partials, cudaStream_t stream) {
   static bool configured = false;
   const size_t smem = sizeof(cnc::Smem);
   if (!configured) {
@@ -561,13 +559,11 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
   a.mask_out = mask_out; a.step = step; a.seed = seed; a.sample_base = sample_base; a.B = B; a.x_u8 = x_u8;
   a.training = training; a.backward = backward; a.inv_bsz = inv_bsz; a.p_drop = p_drop;
   a.mean = 0.1307f; a.inv_std = 1.f / 0.3081f; a.grad_stride = grad_stride; a.aux = aux;
-  cn::fill_tail(a.tail, backward ? tail : nullptr, grad_stride);
   a.det_partials = backward ? det_partials : nullptr;
   a.factors = nullptr; a.phase_ts = nullptr;
   int clusters = B;
   if (max_clusters > 0 && clusters > max_clusters) clusters = max_clusters;
   if (clusters < 1) clusters = 1;
-  if (a.tail.enabled && clusters * cluster > 128) return (int)cudaErrorInvalidConfiguration;   // check-in needs one resident wave
   static const int pdl = [] { const char* e = getenv("B200DIST_PDL"); return (e == nullptr || e[0] != '0') ? 1 : 0; }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));

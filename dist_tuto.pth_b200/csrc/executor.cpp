@@ -24,7 +24,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                            unsigned long long seed, long long sample_base, int B, int training, int backward,
                            float inv_bsz, float p_drop, int max_ctas, long long grad_stride, const float* aux,
-                           const void* tail, float* det_partials, float* factors, int input_ready, cudaStream_t stream);
+                           float* det_partials, float* factors, int input_ready, cudaStream_t stream);
 struct PeerPtrsC { void* p[8]; };
 struct SignalPadsC { uint32_t* pad[8]; };
 int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, float* params, float* momentum,
@@ -39,23 +39,8 @@ int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, 
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
                               float inv_bsz, float p_drop, int cluster, int max_clusters, long long grad_stride,
-                              const float* aux, const void* tail, float* det_partials, cudaStream_t stream);
+                              const float* aux, float* det_partials, cudaStream_t stream);
 int b2_convnet_npar();
-struct FusedTailHostC {            // mirrors cn::FusedTailHost (csrc/convnet_args.cuh)
-  void* grad_ptrs[8];
-  void* inbox_ptrs[8];
-  float* params;
-  float* momentum;
-  unsigned long long* step;
-  float* aux;
-  const float* loss_acc;
-  float* loss_snapshot;
-  unsigned int* ticket;
-  float lr, mu, scale;
-  int rank, world;
-  int wire_bf16;
-  b2::LrSchedule sched;
-};
 }
 
 namespace b2 {
@@ -99,35 +84,22 @@ StepExecutor::~StepExecutor() {
 
 // Enqueues the two kernels of one step on the compute stream.
 void StepExecutor::record_step(const void* x, const long long* y, float* loss_snapshot) {
-  FusedTailHostC th;
-  const void* tp = nullptr;
-  if (cfg_.fused_tail) {
-    std::memset(&th, 0, sizeof(th));
-    std::memcpy(th.grad_ptrs, cfg_.grad_ptrs, sizeof(th.grad_ptrs));
-    std::memcpy(th.inbox_ptrs, cfg_.inbox_ptrs, sizeof(th.inbox_ptrs));
-    th.params = cfg_.params; th.momentum = cfg_.momentum; th.step = cfg_.step_counter; th.aux = cfg_.aux;
-    th.loss_acc = cfg_.loss_acc; th.loss_snapshot = loss_snapshot; th.ticket = cfg_.ticket;
-    th.lr = cfg_.lr; th.mu = cfg_.mu; th.scale = 1.f / cfg_.world; th.rank = cfg_.rank; th.world = cfg_.world;
-    th.wire_bf16 = cfg_.wire_bf16;
-    th.sched = cfg_.sched;
-    tp = &th;
-  }
   // one GPU, one CTA per sample: plain stores to the slots / factors, reduced in a fixed order by the optimizer kernel
-  const bool slots = cfg_.grad_slots != nullptr && cfg_.world == 1 && cfg_.cluster <= 1 && !cfg_.fused_tail;
+  const bool slots = cfg_.grad_slots != nullptr && cfg_.world == 1 && cfg_.cluster <= 1;
   int rc = cfg_.cluster > 1
                ? b2_convnet_cluster_launch(cfg_.params, cfg_.grads_local, x, cfg_.x_u8, y, cfg_.loss_acc, nullptr, nullptr,
                                            cfg_.step_counter, cfg_.seed, cfg_.sample_base, cfg_.B, cfg_.training, 1,
-                                           1.f / cfg_.B, cfg_.p_drop, cfg_.cluster, 0, cfg_.grad_stride, cfg_.aux, tp, nullptr, compute_)
+                                           1.f / cfg_.B, cfg_.p_drop, cfg_.cluster, 0, cfg_.grad_stride, cfg_.aux, nullptr, compute_)
                : b2_convnet_step_launch(cfg_.params, cfg_.grads_local, x, cfg_.x_u8, y, cfg_.loss_acc, nullptr, nullptr,
                                         cfg_.step_counter, cfg_.seed, cfg_.sample_base, cfg_.B, cfg_.training, 1, 1.f / cfg_.B,
-                                        cfg_.p_drop, 0, cfg_.grad_stride, cfg_.aux, tp, slots ? cfg_.grad_slots : nullptr,
+                                        cfg_.p_drop, 0, cfg_.grad_stride, cfg_.aux, slots ? cfg_.grad_slots : nullptr,
                                         slots ? cfg_.factors : nullptr, /*input_ready=*/1, compute_);
   int rc2 = 0;
   if (slots) {
     rc2 = b2_reduce_sgd_launch(cfg_.params, cfg_.momentum, cfg_.step_counter, cfg_.done_counter, cfg_.lr, cfg_.mu, cfg_.aux,
                                cfg_.loss_acc, loss_snapshot, cfg_.grad_slots, cfg_.B, cfg_.factors, cfg_.B, cfg_.grads_local,
                                cfg_.grad_stride, &cfg_.sched, compute_);
-  } else if (!cfg_.fused_tail) {
+  } else {
     PeerPtrsC g;
     SignalPadsC sg;
     std::memcpy(g.p, cfg_.grad_ptrs, sizeof(g.p));

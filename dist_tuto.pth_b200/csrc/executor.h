@@ -32,8 +32,6 @@ struct StepConfig {
   void* inbox_ptrs[8];               // push exchange (sgd.cu): every rank's inbox
   int push;
   int wire_bf16;                     // push exchange: bf16 on the wire
-  int fused_tail;                    // gradient exchange + SGD in the tail of the step kernel (one kernel per step)
-  unsigned int* ticket;              // device scratch of the fused tail
   float* grad_slots;                 // one GPU, one CTA per sample: per-CTA slots [B][21888] and per-sample fc1 factors [B][384]
   float* factors;                    // of the step kernel, summed by reduce_sgd (sgd.cu) instead of red.add into the bucket
   LrSchedule sched;                  // lr schedule of every step's update (zero: constant lr)

@@ -1,8 +1,8 @@
 // Learning-rate schedule of the optimizer kernels: the device (and host C++) twin of ops/optim.LRSchedule.
 //
 // The lr of an update is a closed-form function of the device step counter's value when the update runs (the number of
-// updates applied before it), so captured graphs, the native executor's launches and the fused tail replay the same
-// arguments and still follow the schedule.  Every operation is an explicitly rounded fp64 one (no fused multiply-add on
+// updates applied before it), so captured graphs and the native executor's launches replay the same arguments and still
+// follow the schedule.  Every operation is an explicitly rounded fp64 one (no fused multiply-add on
 // the device), and the product with the base lr is rounded to fp32 once: the device and LRSchedule.lr_at agree bit for
 // bit except for the cosine, which the device takes as cospi(d / span) and the host as cos(pi * d / span); the two may
 // differ in the last fp64 bits, and so the fp32 lr by at most one ulp.

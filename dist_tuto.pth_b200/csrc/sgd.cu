@@ -94,8 +94,9 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
 // CTA reduces its share of the local gradient in a fixed order (convnet_reduce.cuh) and applies SGD to it straight from
 // registers.  No bucket is read or red.add-ed, and the loss terms of the slots are summed in slot order, so the whole step is
 // bit-reproducible.  Also bumps the step counter, snapshots the loss and refreshes aux like the kernels above, and re-zeroes the
-// gradient bucket of the other step parity as they do (a.grads.p[0], optional): a trainer may still run a bucket step next (the
-// fused tail, a batch on another path), and every bucket step relies on finding its bucket zeroed by the step before it.
+// gradient bucket of the other step parity as they do (a.grads.p[0], optional): a trainer may still run a bucket step next (a
+// batch on another path, such as the native executor's), and every bucket step relies on finding its bucket zeroed by the step
+// before it.
 //
 // kSched: a.sched is a schedule (kind != LRS_NONE).  Thread 0 then also evaluates the step's lr where it waits for the
 // step counter, and the emits read it from shared memory.  Without a schedule the kernel is compiled without that code:

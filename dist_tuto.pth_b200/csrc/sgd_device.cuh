@@ -1,5 +1,5 @@
-// Device-side pieces of the fused [gradient exchange + 1/world + momentum SGD + re-zero] step, shared by the stand-alone
-// kernels (sgd.cu) and by the tail of the fused step kernels (convnet.cu / convnet_cluster.cu, "one kernel per step").
+// Device-side pieces of the fused [gradient exchange + 1/world + momentum SGD + re-zero] step of the optimizer kernels
+// (sgd.cu), and the phase timestamps the step kernels (convnet.cu) share with them.
 #pragma once
 #include "common.cuh"
 #include "lr_schedule.h"
@@ -50,12 +50,6 @@ struct SgdArgs {
 
 // The lr of the update run at step counter `st`; the kernels evaluate it in thread 0 and share it through shared memory.
 __device__ __forceinline__ float step_lr(const SgdArgs& a, unsigned long long st) { return lr_schedule_lr(a.sched, a.lr, st); }
-// The same, out of line, for the tail of the step kernels: their code and register allocation stay those of a kernel
-// without the fp64 schedule code, which only runs (behind one call from thread 0) when there is a schedule.  The schedule
-// is passed by value, so the kernel parameters are not copied to local memory.
-static __device__ __noinline__ float scheduled_lr(LrSchedule s, float base, unsigned long long st) {
-  return lr_schedule_lr(s, base, st);
-}
 
 // The previous kernel of the stream (this step's forward/backward) is complete and the next step's kernel cannot pass its
 // own griddepcontrol.wait before this kernel ends, so loss_acc holds exactly the loss up to and including this step.
@@ -183,64 +177,6 @@ __device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, u
   if (a.zero_grads) {
     const size_t z_off = a.grad_stride > 0 ? (par ^ 1) * (size_t)a.grad_stride * sizeof(float) : 0;
     st_cg_v4(reinterpret_cast<uint4*>(reinterpret_cast<char*>(a.grads.p[rank]) + z_off) + v, make_uint4(0u, 0u, 0u, 0u));
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// "One kernel per step": the tail of the fused forward/backward kernels (convnet.cu, convnet_cluster.cu).
-//
-// After a CTA has flushed its gradients into the bucket it checks in on a device counter; once all `n_cta` CTAs of the
-// grid have checked in (they are co-resident: at most one CTA per SM) the bucket is complete and EVERY CTA takes a
-// 1/n_cta share of the vectors through exchange_apply_vec (push to the peers' inboxes, local reduce, SGD, re-zero).
-// Compared with the separate allreduce_sgd kernel this removes the kernel boundary (launch + drain + PDL hand-off) from the
-// critical path between "last gradient flushed" and "first peer line stored", and spreads the update over all SMs.
-// The last CTA to finish resets the counters, snapshots the running loss and publishes step + 1.
-struct FusedTail {
-  int enabled;
-  SgdArgs sgd;
-  unsigned int* ticket;      // device scratch: [0] check-ins, [1] finishers (both zero between steps)
-};
-
-__device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* addr) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(addr) : "memory");
-  return v;
-}
-
-// All threads of every participating CTA call this after their gradient flush / loss atomics.  `st` = step index read at
-// kernel start, `cta` in [0, n_cta).  `lr_word`: a word of the CTA's shared memory that nothing uses any more once every
-// thread has arrived here; thread 0 passes the step's lr to the other threads through it.
-__device__ __forceinline__ void fused_tail(const FusedTail& t, unsigned long long st, int n_cta, int cta, float* lr_word) {
-  __syncthreads();                                   // this CTA's red.adds and loss atomics are issued
-  if (threadIdx.x == 0) {
-    __threadfence();                                 // ... and ordered before the check-in (cumulative over the barrier)
-    atomicAdd(t.ticket, 1u);
-    unsigned long long spins = 0;
-    while (ld_acquire_gpu_u32(t.ticket) < (uint32_t)n_cta) {
-      if (++spins > B2_SPIN_LIMIT) {
-        printf("[b200dist] fused step: CTA %d timed out waiting for the grid (%u of %d checked in)\n", cta, *t.ticket, n_cta);
-        __trap();
-      }
-    }
-    *lr_word = t.sgd.sched.kind == LRS_NONE ? t.sgd.lr : scheduled_lr(t.sgd.sched, t.sgd.lr, st);
-  }
-  __syncthreads();
-  const float lr = *lr_word;
-  for (size_t v = (size_t)cta * blockDim.x + threadIdx.x; v < t.sgd.n_vec; v += (size_t)n_cta * blockDim.x)
-    exchange_apply_vec(t.sgd, v, st, lr);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(t.ticket + 1, 1u) == (uint32_t)(n_cta - 1)) {      // last finisher: every CTA is past the check-in spin
-      t.ticket[0] = 0u;
-      t.ticket[1] = 0u;
-      if (t.sgd.loss_snapshot != nullptr) {
-        t.sgd.loss_snapshot[0] = *reinterpret_cast<const volatile float*>(t.sgd.loss_acc);
-        t.sgd.loss_snapshot[1] = *reinterpret_cast<const volatile float*>(t.sgd.loss_acc + 1);
-      }
-      __threadfence();
-      *t.sgd.step = st + 1ull;
-    }
   }
 }
 

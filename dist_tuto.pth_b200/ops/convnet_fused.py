@@ -129,7 +129,7 @@ class FusedTrainer:
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
         # lr_schedule (ops/optim.LRSchedule, step units): the optimizer kernels compute each update's lr from the device step
-        # counter (csrc/lr_schedule.h), so graph replays, run_native and the fused tail follow it with fixed launch arguments
+        # counter (csrc/lr_schedule.h), so graph replays and run_native follow it with fixed launch arguments
         self._sched = schedule_tuple(lr_schedule)
         self.lr_schedule = lr_schedule
         self.group = group
@@ -209,12 +209,10 @@ class FusedTrainer:
         self._nstep = 0
         self._loss_read = 0.0                       # cumulative loss already returned by pop_loss_sum
         self._last_loss_cum = 0.0
-        # "one kernel per step": gradient exchange + SGD run in the tail of the step kernel (csrc/sgd_device.cuh: grid-wide
-        # check-in, then every CTA pushes / reduces / updates a share of the bucket).  Needs the push inbox when world > 1.
         # deterministic=True: every step CTA stores its gradient sums to a private slot and `det_reduce` adds the slots in
         # CTA order (instead of float red.add into one bucket) => two runs with the same seed are bit-identical, at the
         # price of one more small kernel per step.  Used with several GPUs or clusters, by step() / the graph path only (the
-        # C++ executor and the fused tail keep the atomic flush there).  One GPU at one CTA per sample needs no flag: that path
+        # C++ executor keeps the atomic flush there).  One GPU at one CTA per sample needs no flag: that path
         # has no atomics (below), in step() and in the executor alike.
         self.deterministic = bool(deterministic)
         self.sms = torch.cuda.get_device_properties(self.device).multi_processor_count
@@ -229,12 +227,10 @@ class FusedTrainer:
         self.grad_slots, self.factors = None, None
         if self.world == 1 and (self.cluster == 1 or self.bsz * self.cluster > self.sms):
             self._work_buffers(self.bsz)
-        # opt-in (B200DIST_FUSED_TAIL=1): the grid-wide check-in replaces the PDL hand-off to the separate optimizer kernel,
-        # and it needs every CTA resident, which 8-CTA clusters do not guarantee.
-        self.fused_tail = (os.environ.get("B200DIST_FUSED_TAIL", "0") == "1" and not deterministic and self.cluster <= 4
-                           and (self.world == 1 or self.inbox_handle is not None))
-        self.ticket = torch.zeros(2, dtype=torch.int32, device=self.device)
-        self.gpu_launches_per_step = 1 if self.fused_tail else 2     # convnet_step (+ allreduce_sgd)
+        # Read by bench.py, whose result line names the step's kernels and counts its launches: every step is the step
+        # kernel followed by one optimizer kernel.
+        self.fused_tail = False
+        self.gpu_launches_per_step = 2
         self._evaluator = None                      # ops/convnet_eval.Evaluator, made on the first evaluate()
         self._warm()
 
@@ -250,8 +246,6 @@ class FusedTrainer:
         self.grads.zero_()
         if self.inbox_handle is not None:
             self.inbox_handle.local.zero_()
-        if getattr(self, "ticket", None) is not None:
-            self.ticket.zero_()
         torch.cuda.synchronize(self.device)
         if self.world > 1:
             comm.barrier(self.group)
@@ -284,8 +278,7 @@ class FusedTrainer:
 
     def _native_slots(self):
         """(slots, factors) for the C++ executor when it runs the no-atomics one-GPU path (same condition as ``_kernels``)."""
-        fused = self.fused_tail and self.bsz * self.cluster <= 128
-        if self.world == 1 and self.cluster == 1 and not fused and self._step_ctas(self.bsz) == self.bsz:
+        if self.world == 1 and self.cluster == 1 and self._step_ctas(self.bsz) == self.bsz:
             return self.grad_slots, self.factors
         return None, None
 
@@ -294,19 +287,13 @@ class FusedTrainer:
         step (they come from copies or from work that finished earlier), so the step kernel may load them while it waits
         for the previous step's optimizer kernel."""
         cl = self.cluster if B * self.cluster <= self.sms else 1
-        if self.fused_tail and B * cl <= 128:       # the tail's grid-wide check-in needs every CTA resident
-            tail = (self._grad_ptrs, self._inbox_ptrs, self.momentum, self.lr, self.mu, 1.0 / self.world, self.rank, self.world,
-                    self.ticket, None, self.wire_bf16, self._sched)
-            self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
-                                self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux, tail)
-            return
         if self.world == 1 and cl == 1:
             self._work_buffers(B)
             n = self._step_ctas(B)
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, n if n < B else 0, self.grad_stride,
-                                1, self.aux, None, self.grad_slots, self.factors, input_ready)
-            # grads: re-zeroes the other-parity bucket, which a bucket step (fused tail, executor) may use next
+                                1, self.aux, det_partials=self.grad_slots, factors=self.factors, input_ready=input_ready)
+            # grads: re-zeroes the other-parity bucket, which a bucket step (the executor's) may use next
             self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
                               self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride,
                               lr_schedule=self._sched)
@@ -314,7 +301,7 @@ class FusedTrainer:
         if self.deterministic and B * cl <= self.sms:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux,
-                                None, self.det_partials)
+                                det_partials=self.det_partials)
             self.C.det_reduce(self.det_partials, B * cl, self.grads, self.step_counter, self.grad_stride, self.loss_acc)
         else:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
@@ -438,8 +425,7 @@ class FusedTrainer:
                                       self.step_counter, self.done_counter, self.loss_acc, in_dev, self.raw_uint8,
                                       self.training, self.rank, self.world, self.seed, self.rank * self.bsz,
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
-                                      self.cluster, self.aux, self._inbox_ptrs, loss_hist,
-                                      self.fused_tail and self.bsz * self.cluster <= 128, self.ticket, self.wire_bf16,
+                                      self.cluster, self.aux, self._inbox_ptrs, loss_hist, self.wire_bf16,
                                       *self._native_slots(), lr_schedule=self._sched),
                   self.training)
             self._executors[id(loader)] = ex

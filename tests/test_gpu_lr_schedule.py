@@ -117,15 +117,6 @@ def test_cluster_path_applies_the_scheduled_lr(dev, sched):
     _check_each_step(tr, _batches(32, 16, 5, raw=False), sched, 0.05)
 
 
-@pytest.mark.parametrize("sched", [WARM_MS, WARM_COS], ids=["multistep", "cosine"])
-def test_fused_tail_applies_the_scheduled_lr(dev, sched, monkeypatch):
-    from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer
-    monkeypatch.setenv("B200DIST_FUSED_TAIL", "1")
-    tr = FusedTrainer(16, lr=0.05, seed=3, device=dev, lr_schedule=sched)
-    assert tr.fused_tail and tr.gpu_launches_per_step == 1
-    _check_each_step(tr, _batches(32, 16, 6, raw=False), sched, 0.05)
-
-
 def test_batched_engine_applies_the_scheduled_lr_on_graph_replays_and_eager_tail(dev):
     from dist_tuto.pth_b200.ops.convnet_batched import BatchedTrainer
     tr = BatchedTrainer(2048, lr=0.3, seed=3, device=dev, raw_uint8=True, lr_schedule=WARM_MS)

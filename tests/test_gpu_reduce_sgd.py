@@ -72,55 +72,6 @@ def test_ctas_carrying_several_samples_match_torch_sgd(dev):
     assert float(tr.grads.abs().max()) == 0.0            # no bucket on this path
 
 
-def test_fused_tail_matches_default_path(dev, monkeypatch):
-    """The opt-in fused tail (exchange + SGD inside the step kernel, atomic bucket) at batch 128 == the default path."""
-    from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer
-    batches = [_batch(dev, 128, seed=500 + i) for i in range(4)]
-    res = []
-    for tail in ("0", "1"):
-        monkeypatch.setenv("B200DIST_FUSED_TAIL", tail)
-        tr = FusedTrainer(128, lr=0.05, momentum=0.5, seed=19, device=dev, p_drop=0.5)
-        assert tr.fused_tail == (tail == "1")
-        for x, y in batches:
-            tr.step(x.cpu().pin_memory(), y.cpu().pin_memory())
-        tr.sync_lag(0)
-        torch.cuda.synchronize()
-        res.append((tr.params.clone(), tr.momentum.clone(), tr.pop_loss_sum()))
-    assert torch.allclose(res[0][0], res[1][0], atol=1e-5, rtol=1e-4)
-    assert torch.allclose(res[0][1], res[1][1], atol=1e-5, rtol=1e-4)
-    assert abs(res[0][2] - res[1][2]) < 1e-4 * abs(res[1][2])
-
-
-def test_fused_tail_short_batches_between_slot_steps_match_torch_sgd(dev, monkeypatch):
-    """One trainer on both paths: with the fused tail on, full batches of 136 (> 128) take the slots path and the short batches
-    of 40 take the fused tail, whose bucket is double-buffered by step parity.  Steps 3 and 7 are both tail steps of parity 1:
-    step 7 must find its bucket zeroed (by the slots step 4), or it would apply step 3's gradient again.  Two epochs of
-    3 x 136 + 40 samples == Net autograd + torch SGD."""
-    from dist_tuto.pth_b200.models.convnet import Net
-    from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer, unpack_params
-    monkeypatch.setenv("B200DIST_FUSED_TAIL", "1")
-    torch.manual_seed(23)
-    ref = Net(p_drop=0.0).to(dev)
-    tr = FusedTrainer(136, lr=0.05, momentum=0.5, seed=23, device=dev, p_drop=0.0, init_from=ref)
-    assert tr.fused_tail and tr.cluster == 1
-    opt = torch.optim.SGD(ref.parameters(), lr=0.05, momentum=0.5)
-    losses = []
-    for i, B in enumerate([136, 136, 136, 40] * 2):
-        x, y = _batch(dev, B, seed=600 + i)
-        tr.step(x.cpu().pin_memory(), y.cpu().pin_memory())
-        opt.zero_grad()
-        loss = F.nll_loss(ref(x), y)
-        loss.backward()
-        opt.step()
-        losses.append(loss.item())
-    got = tr.pop_loss_sum()
-    assert int(tr.step_counter.item()) == 8
-    assert abs(got - sum(losses)) < 1e-3 * max(1.0, abs(sum(losses)))
-    views = unpack_params(tr.params)
-    for name, p in ref.named_parameters():
-        assert torch.allclose(views[name], p.detach(), atol=2e-4, rtol=1e-3), name
-
-
 def test_native_executor_bucket_steps_between_slot_steps(dev):
     """Batch 544 (> 4 CTAs per SM): the C++ executor runs the full batches on the bucket path while the short tail batch of
     every epoch takes the slots path eagerly.  The bucket step after a slots step must find its bucket zeroed; two epochs
