@@ -15,9 +15,10 @@ Bandwidth columns:
             reported as link_GBs = link_tx / t against 770 GB/s measured peer copy.
 ``--emit-table`` writes parallel/allreduce_table.json (per-world variant thresholds) from the measured winners.
 
-``--collective {reduce,broadcast,allgather}`` or ``--op {product,max,min}`` time that collective instead: every variant of
-ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the NCCL call on the same tensor, per size
-(for an all-gather, the size of one rank's input).  It compares GPUs, so it refuses to run on one.
+``--collective {reduce,broadcast,allgather,scatter,gather}`` or ``--op {product,max,min}`` time that collective instead:
+every variant of ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the NCCL call on the same
+tensor, per size (for an all-gather, a scatter and a gather, the size of one rank's segment; the root is rank 0 and its
+list is one block).  It compares GPUs, so it refuses to run on one.
 """
 import argparse
 import json
@@ -90,6 +91,7 @@ def body_collective(rank, size):
         n = s // 4
         t = torch.ones(n, device=dev)
         outs = [torch.empty_like(t) for _ in range(size)]
+        lst = list(torch.empty(size * n, device=dev).view(size, n).unbind(0)) if rank == 0 else None  # scatter / gather
         iters = 100 if s <= (1 << 20) else 20
         row = {"bytes": s, "collective": coll, "op": ARGS.op}
         arms = []
@@ -102,10 +104,16 @@ def body_collective(rank, size):
                 arms.append((name, lambda v=v: w.reduce_(t, 0, op, variant=v)))
             elif coll == "broadcast":
                 arms.append((name, lambda v=v: w.broadcast_(t, 0, variant=v)))
+            elif coll == "scatter":
+                arms.append((name, lambda v=v: w.scatter_(t, lst, 0, variant=v)))
+            elif coll == "gather":
+                arms.append((name, lambda v=v: w.gather_(t, lst, 0, variant=v)))
             else:
                 arms.append((name, lambda v=v: w.all_gather_(outs, t, variant=v)))
         nccl = {"allreduce": lambda: dist.all_reduce(t, op=op), "reduce": lambda: dist.reduce(t, 0, op=op),
-                "broadcast": lambda: dist.broadcast(t, 0), "allgather": lambda: dist.all_gather(outs, t)}[coll]
+                "broadcast": lambda: dist.broadcast(t, 0), "allgather": lambda: dist.all_gather(outs, t),
+                "scatter": lambda: dist.scatter(t, scatter_list=lst, src=0),
+                "gather": lambda: dist.gather(t, gather_list=lst, dst=0)}[coll]
         arms.append(("nccl", nccl))
         best = {}
         for order in (arms, arms[::-1]):
@@ -257,7 +265,7 @@ if __name__ == "__main__":
     ap.add_argument("--max-mb", type=int, default=1024)
     ap.add_argument("--out", default=None)
     ap.add_argument("--emit-table", action="store_true", help="write the measured variant thresholds of this world size")
-    ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather"], default="allreduce")
+    ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather", "scatter", "gather"], default="allreduce")
     ap.add_argument("--op", choices=sorted(OPS), default="sum")
     ARGS = ap.parse_args()
     if ARGS.gpus < 2:

@@ -14,11 +14,13 @@ Design (GPU-first, not a port):
     gloo for CPU tensors;
   * when a symmetric world has been set up for the group (``backend="b200"``),
     blocking ``all_reduce`` and ``reduce`` (SUM, PRODUCT, MAX, MIN on CUDA
-    fp32 / bf16) and ``broadcast`` and ``all_gather`` (CUDA, any dtype, copied
-    bit for bit) run on our own fused peer-memory kernels (``parallel.symm``);
-    that path never calls NCCL.  ``async_op=True``, CPU tensors, other dtypes
-    and ops, ``scatter`` and ``gather`` go to NCCL / gloo, and so does every op
-    but SUM on a world that serves only the sum (no ``supports_op``).
+    fp32 / bf16) and ``broadcast``, ``all_gather``, ``scatter`` and ``gather``
+    (CUDA, any dtype, copied bit for bit) run on our own fused peer-memory
+    kernels (``parallel.symm``); that path never calls NCCL.
+    ``async_op=True``, CPU tensors, other dtypes and ops go to NCCL / gloo,
+    and so does every op but SUM on a world that serves only the sum (no
+    ``supports_op``) and ``scatter`` / ``gather`` on a world without
+    ``scatter_`` / ``gather_`` (the two-level world of several machines).
   * ``group=0`` (the 2017 spelling of "world", train_dist.py:99, ptp.py:26)
     is accepted and mapped to the default group (fixes defect D2).
 """
@@ -222,11 +224,20 @@ def scatter(tensor: torch.Tensor, src: int = 0, scatter_list: Optional[List[torc
     """i-th element of ``scatter_list`` on ``src`` goes to rank i (tuto.md:200).
 
     Unlike modern torch, a ``scatter_list`` passed on non-source ranks is
-    ignored (the tutorial era accepted it)."""
+    ignored (the tutorial era accepted it).
+
+    On a symmetric world a CUDA ``tensor`` of any dtype is scattered bit for bit by the peer-memory kernels.  Whether the
+    call takes that path depends on ``tensor`` and the group alone, never on ``scatter_list``, which only ``src`` holds:
+    every rank must enter the same kernel.  A ``scatter_list`` of the wrong length, dtype or size raises on ``src``, as
+    torch does; its peers are then left waiting inside the kernel until its spin limit reports them."""
     _check(tensor)
     g = _g(group)
     if dist.get_rank() != src:
         scatter_list = None
+    w = _symm_world_for(tensor, group)
+    if w is not None and hasattr(w, "scatter_") and w.supports_raw(tensor):
+        w.scatter_(tensor, scatter_list, src)
+        return None
     return dist.scatter(tensor, scatter_list=scatter_list, src=src, group=g)
 
 
@@ -235,13 +246,21 @@ def gather(tensor: torch.Tensor, dst: int = 0, gather_list: Optional[List[torch.
     """All ranks' tensors land in ``gather_list`` on ``dst`` (tuto.md:201, ptp.py:26).
 
     The reference passes ``gather_list`` on every rank (ptp.py:25-26); modern
-    torch rejects that, so it is dropped on non-destination ranks here."""
+    torch rejects that, so it is dropped on non-destination ranks here.
+
+    On a symmetric world a CUDA ``tensor`` of any dtype is gathered bit for bit by the peer-memory kernels, routed by
+    ``tensor`` and the group alone as in ``scatter``; a ``gather_list`` of the wrong length, dtype or size raises on
+    ``dst``, and its peers are then left waiting inside the kernel until its spin limit reports them."""
     _check(tensor)
     g = _g(group)
     if dist.get_rank() != dst:
         gather_list = None
     elif gather_list is not None and len({id(t) for t in gather_list}) != len(gather_list):
         raise ValueError("gather_list must hold distinct tensors ([zeros(1)] * n aliases one buffer)")
+    w = _symm_world_for(tensor, group)
+    if w is not None and hasattr(w, "gather_") and w.supports_raw(tensor):
+        w.gather_(tensor, gather_list, dst)
+        return None
     return dist.gather(tensor, gather_list=gather_list, dst=dst, group=g)
 
 

@@ -22,7 +22,10 @@
 //                               stores its output; every rank still runs every barrier and every LL push)
 //   BCAST                     : raw 16-byte copies of the root's vectors (any dtype; never through the fp32 accumulator,
 //                               so -0, subnormals, NaN payloads and integers survive)
-//   GATHER                    : raw copies; rank r's input (n_vec / world vectors) lands at vector r * n_vec / world
+//   GATHER                    : raw copies; rank r's input (n_vec / world vectors) lands at vector r * n_vec / world of every
+//                               rank's output (all-gather) or, with `root` >= 0, of the root's only (gather)
+//   SCATTER                   : raw copies; the root's input holds world segments of n_vec / world vectors and rank r
+//                               receives segment r (at vector r * n_vec / world of its symmetric buffer when in place)
 // Every rank of one call runs the same barrier sequence whatever the op and root, so calls of any kind may follow each
 // other on one buffer, signal pad and inbox.
 #include <cstdio>
@@ -31,7 +34,7 @@
 
 namespace b2 {
 
-enum : int { kSum = 0, kProd = 1, kMax = 2, kMin = 3, kBcast = 4, kGather = 5 };
+enum : int { kSum = 0, kProd = 1, kMax = 2, kMin = 3, kBcast = 4, kGather = 5, kScatter = 6 };
 
 // The combine step of a reduction: identity, one fp32 combine, and the final scale (SUM only; the launcher refuses a
 // scale for the other ops, and skipping the multiply keeps their results bit-exact under --use_fast_math).
@@ -157,29 +160,37 @@ struct ARArgs {
   SignalPads sig;         // signal pad of every rank (one pad per symmetric buffer)
   void* mc;               // multicast VA of the symmetric buffer (NVLS) or nullptr
   const void* src;        // optional local source (copied/cast into bufs.p[rank] first; GATHER: into slice rank)
-  void* dst;              // optional local destination (else result stays in bufs.p[rank])
-  size_t n_vec;           // 16-byte vectors on the wire (padded); GATHER: of the output, world x the per-rank input
+  void* dst;              // optional local destination (else result stays in bufs.p[rank]; SCATTER: in its slice rank)
+  size_t n_vec;           // 16-byte vectors on the wire (padded); GATHER: of the output, SCATTER: of the root's input,
+                          // world x the per-rank segment in both
   float scale;
   int rank, world;
   int src_f32, dst_f32;   // local dtypes: 1 = fp32, 0 = wire dtype
   PeerPtrs inbox;         // LL variant: every rank's inbox [2 parities][world sources][ll_cap vectors][2 lines of 16 B]
   size_t ll_cap;          // vectors per (parity, source) region of the inbox
-  int root;               // reductions: -1 = every rank stores the result, else only this rank; BCAST: the source rank
+  int root;               // reductions and GATHER: -1 = every rank stores the result, else only this rank; BCAST and
+                          // SCATTER: the source rank
 };
 
 constexpr int kThreads = 512;
 constexpr int kUnroll = 2;        // peer-load variants: 2 x world 16-byte loads in flight per thread
 constexpr int kUnrollNvls = 4;    // NVLS: one multimem.ld_reduce per vector
 
-// Does this rank store its output?  Only a reduce (ROOT: a reduction with root >= 0) suppresses stores, never barriers.
+// Does this rank store its output?  Only a reduce or a gather (ROOT: root >= 0) suppresses stores, never barriers.
 // ROOT is a template parameter so that the all-reduce instances carry no root test at all.
 template <bool ROOT>
 __device__ __forceinline__ bool stores_output(const ARArgs& a) {
   return !ROOT || a.root == a.rank;
 }
 
+// Broadcast and scatter read the root's input only: the other ranks' src is never read (it is passed all the same, so that
+// every rank runs the same barriers).
+template <int OP>
+constexpr bool kFromRoot = OP == kBcast || OP == kScatter;
+
 // ------------------------------------------------------------------------------------------ one-shot
-// Reductions read vector v of every rank; BCAST reads it from the root only; GATHER reads it from its owner v / seg.
+// Reductions read vector v of every rank; BCAST reads it from the root only; GATHER reads it from its owner v / seg (a gather:
+// on the root only); SCATTER: rank r reads the seg vectors of slot r from the root.
 template <bool BF16, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
   using W = Wire<BF16>;
@@ -188,19 +199,20 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
   const size_t stride = (size_t)gridDim.x * kThreads;
   const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  const size_t seg = a.n_vec / world;                   // GATHER: vectors per rank
-  if (a.src != nullptr && (OP != kBcast || rank == a.root)) {
+  const size_t seg = a.n_vec / world;                   // GATHER / SCATTER: vectors per rank
+  const size_t n_out = OP == kScatter ? seg : a.n_vec;  // vectors this rank reads and stores
+  if (a.src != nullptr && (!kFromRoot<OP> || rank == a.root)) {
     uint4* stage = reinterpret_cast<uint4*>(a.bufs.p[rank]) + (OP == kGather ? (size_t)rank * seg : 0);
     for (size_t v = first; v < (OP == kGather ? seg : a.n_vec); v += stride)
       st_cg_v4(stage + v, load_local_as_wire<BF16>(a.src, v, a.src_f32));
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's data is in place
   const bool inplace = (a.dst == nullptr);
-  void* out = inplace ? a.bufs.p[rank] : a.dst;
+  void* out = inplace ? reinterpret_cast<uint4*>(a.bufs.p[rank]) + (OP == kScatter ? (size_t)rank * seg : 0) : a.dst;
   const bool out_f32 = inplace ? false : (a.dst_f32 != 0);
   const bool store = stores_output<ROOT>(a);
   // block-uniform trip count (the in-place variant has a barrier inside the loop); identical on every rank
-  for (size_t base0 = (size_t)blockIdx.x * kThreads; base0 < a.n_vec; base0 += stride * kUnroll) {
+  for (size_t base0 = (size_t)blockIdx.x * kThreads; base0 < n_out; base0 += stride * kUnroll) {
     const size_t base = base0 + threadIdx.x;
     float acc[kUnroll][W::kElems];
     uint4 raw[kUnroll][B2_MAX_RANKS];
@@ -208,8 +220,9 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const size_t v = base + (size_t)u * stride;
-        const int from = OP == kBcast ? a.root : (int)(v / seg);
-        if (v < a.n_vec) raw[u][0] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[from]) + v);
+        const int from = OP == kGather ? (int)(v / seg) : a.root;
+        const size_t at = OP == kScatter ? (size_t)rank * seg + v : v;
+        if (v < n_out && store) raw[u][0] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[from]) + at);
       }
     } else {
 #pragma unroll
@@ -232,7 +245,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
 #pragma unroll
     for (int u = 0; u < kUnroll; ++u) {
       const size_t v = base + (size_t)u * stride;
-      if (v < a.n_vec && store) {
+      if (v < n_out && store) {
         if constexpr (kRaw) st_cg_v4(reinterpret_cast<uint4*>(out) + v, raw[u][0]);
         else store_acc_local<BF16, OP>(out, v, acc[u], a.scale, out_f32);
       }
@@ -244,7 +257,8 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
 
 // ------------------------------------------------------------------------------------------ two-shot / NVLS
 // Slice s = vectors [s*slice, (s+1)*slice) is reduced by rank s and pushed to every rank (a reduce pushes it to the root
-// only).  BCAST: rank s loads slice s from the root and pushes it; GATHER: rank s pushes its own input, staged at slice s.
+// only).  BCAST: rank s loads slice s from the root and pushes it; GATHER: rank s pushes its own input, staged at slice s (a
+// gather: to the root only); SCATTER: the root pushes slice s of its input into rank s's slice s, and rank s copies it out.
 template <bool BF16, bool NVLS, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
   using W = Wire<BF16>;
@@ -254,7 +268,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
   const size_t slice = a.n_vec / world;                 // host pads n_vec to a multiple of world
   const size_t stride = (size_t)gridDim.x * kThreads;
   const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
-  if (a.src != nullptr && (OP != kBcast || rank == a.root)) {
+  if (a.src != nullptr && (!kFromRoot<OP> || rank == a.root)) {
     for (int s = 0; s < world; ++s) {
       if (OP == kGather && s != rank) continue;
       for (size_t j = first; j < slice; j += stride) {
@@ -268,7 +282,26 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
   const size_t off = (size_t)rank * slice;
   constexpr int U = NVLS ? kUnrollNvls : kUnroll;
   for (size_t base = first; base < slice; base += stride * U) {
-    if constexpr (NVLS) {
+    if constexpr (OP == kScatter) {
+      if (rank != a.root) break;                                  // only the root pushes; no barrier inside this loop
+      uint4 raw[kUnroll][B2_MAX_RANKS];
+#pragma unroll
+      for (int u = 0; u < kUnroll; ++u) {
+        const size_t j = base + (size_t)u * stride;
+#pragma unroll
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world && r != rank && j < slice)
+            raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[rank]) + (size_t)r * slice + j);
+      }
+#pragma unroll
+      for (int u = 0; u < kUnroll; ++u) {
+        const size_t j = base + (size_t)u * stride;
+#pragma unroll
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world && r != rank && j < slice)
+            st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[r]) + (size_t)r * slice + j, raw[u][r]);
+      }
+    } else if constexpr (NVLS) {
       uint4 red[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -330,11 +363,14 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every slice has landed everywhere
   if (a.dst != nullptr && stores_output<ROOT>(a)) {
-    for (int s = 0; s < world; ++s)
+    for (int s = 0; s < world; ++s) {
+      if (OP == kScatter && s != rank) continue;
       for (size_t j = first; j < slice; j += stride) {
         const size_t v = (size_t)s * slice + j;
-        store_wire_local<BF16>(a.dst, v, ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[rank]) + v), a.dst_f32);
+        store_wire_local<BF16>(a.dst, OP == kScatter ? j : v, ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[rank]) + v),
+                               a.dst_f32);
       }
+    }
   }
   if (a.src != nullptr) block_barrier_all_ranks(a.sig, rank, world, ++epoch);  // staging reusable (eager path)
   if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
@@ -350,7 +386,8 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
 // launcher sizes the LL grid by the pushed vectors alone.  epoch 0 never occurs as a flag: counters are pre-incremented, the
 // inbox starts zeroed, and the one epoch in 2^32 that wraps to 0 uses flag 1 (epoch 1 has the other parity).
 // Every op pushes and waits for the same lines: BCAST keeps the root's line (the others are the acknowledgements the parity
-// argument needs), GATHER stores source r's line at vector r * n_vec / world instead of combining it.
+// argument needs), GATHER stores source r's line at vector r * n_vec / world instead of combining it (a gather: on the root
+// only), and SCATTER is BCAST except that the root's line to rank r carries segment r of its input.
 template <bool BF16, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   using W = Wire<BF16>;
@@ -359,15 +396,18 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   const uint32_t flag = epoch == 0u ? 1u : epoch;                     // 0 is "never written"
   const size_t par = (size_t)(epoch & 1u);
   const size_t stride = (size_t)gridDim.x * kThreads;
-  const size_t n_push = OP == kGather ? a.n_vec / world : a.n_vec;    // vectors each rank pushes
+  const size_t n_push = OP == kGather || OP == kScatter ? a.n_vec / world : a.n_vec;    // vectors each rank pushes
   const void* in_local = a.src != nullptr ? a.src
                                           : reinterpret_cast<const uint4*>(a.bufs.p[rank]) + (OP == kGather ? rank * n_push : 0);
   const bool in_f32 = a.src != nullptr && a.src_f32 != 0;
-  void* out = a.dst != nullptr ? a.dst : a.bufs.p[rank];
+  void* out = a.dst != nullptr ? a.dst : reinterpret_cast<uint4*>(a.bufs.p[rank]) + (OP == kScatter ? rank * n_push : 0);
   const bool out_f32 = a.dst != nullptr && a.dst_f32 != 0;
   const bool store = stores_output<ROOT>(a);
   for (size_t v = (size_t)blockIdx.x * kThreads + threadIdx.x; v < n_push; v += stride) {
-    const uint4 mine = load_local_as_wire<BF16>(in_local, v, in_f32);
+    // SCATTER: the root's own segment; a non-root reads no input (its src may be any size) and pushes zeros
+    const uint4 mine = OP == kScatter && rank != a.root
+                           ? make_uint4(0u, 0u, 0u, 0u)
+                           : load_local_as_wire<BF16>(in_local, OP == kScatter ? (size_t)rank * n_push + v : v, in_f32);
     const uint4 l0 = make_uint4(mine.x, flag, mine.y, flag), l1 = make_uint4(mine.z, flag, mine.w, flag);
     const size_t line = ((par * (size_t)world + (size_t)rank) * a.ll_cap + v) * 2;
 #pragma unroll
@@ -376,13 +416,19 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
         int r = rank + i;
         if (r >= world) r -= world;
         uint4* d = reinterpret_cast<uint4*>(a.inbox.p[r]) + line;
-        st_volatile_v4(d, l0);
-        st_volatile_v4(d + 1, l1);
+        if constexpr (OP == kScatter) {                               // the root's line to rank r carries segment r
+          const uint4 w = rank == a.root ? load_local_as_wire<BF16>(in_local, (size_t)r * n_push + v, in_f32) : mine;
+          st_volatile_v4(d, make_uint4(w.x, flag, w.y, flag));
+          st_volatile_v4(d + 1, make_uint4(w.z, flag, w.w, flag));
+        } else {
+          st_volatile_v4(d, l0);
+          st_volatile_v4(d + 1, l1);
+        }
       }
     }
     float acc[W::kElems];
     if constexpr (OP < kBcast) W::template zero<OP>(acc);
-    uint4 kept = mine;                                                // BCAST: the root's vector
+    uint4 kept = mine;                                                // BCAST / SCATTER: the root's vector
     const uint4* in = reinterpret_cast<const uint4*>(a.inbox.p[rank]);
 #pragma unroll
     for (int r = 0; r < B2_MAX_RANKS; ++r) {
@@ -405,12 +451,16 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
           }
           w = make_uint4(q0.x, q0.z, q1.x, q1.z);
         }
-        if constexpr (OP == kGather) st_cg_v4(reinterpret_cast<uint4*>(out) + (size_t)r * n_push + v, w);
-        else if constexpr (OP == kBcast) kept = r == a.root ? w : kept;
-        else W::template add<OP>(acc, w);                             // fixed rank order => bit-identical on every rank
+        if constexpr (OP == kGather) {
+          if (store) st_cg_v4(reinterpret_cast<uint4*>(out) + (size_t)r * n_push + v, w);
+        } else if constexpr (kFromRoot<OP>) {
+          kept = r == a.root ? w : kept;
+        } else {
+          W::template add<OP>(acc, w);                                // fixed rank order => bit-identical on every rank
+        }
       }
     }
-    if constexpr (OP == kBcast) st_cg_v4(reinterpret_cast<uint4*>(out) + v, kept);
+    if constexpr (kFromRoot<OP>) st_cg_v4(reinterpret_cast<uint4*>(out) + v, kept);
     else if constexpr (OP != kGather) {
       if (store) store_acc_local<BF16, OP>(out, v, acc, a.scale, out_f32);
     }
@@ -445,6 +495,9 @@ void launch_op(int variant, int bf16, dim3 grid, const ARArgs& a, cudaStream_t s
                                  : launch_kernel<false, OP, true>(variant, grid, a, stream);
     if (bf16) return launch_kernel<true, OP, false>(variant, grid, a, stream);
   }
+  if constexpr (OP == kGather) {
+    if (a.root >= 0) return launch_kernel<false, kGather, true>(variant, grid, a, stream);
+  }
   launch_kernel<false, OP, false>(variant, grid, a, stream);
 }
 
@@ -454,25 +507,27 @@ void launch_op(int variant, int bf16, dim3 grid, const ARArgs& a, cudaStream_t s
 extern "C" {
 
 // variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN, 4 broadcast
-// from `root`, 5 all-gather; a reduction with root >= 0 is a reduce to that rank.  Returns cudaError_t as int;
-// cudaErrorInvalidValue, without a launch, for an unknown variant or op, a world outside 1..8, a rank outside [0, world), a
-// root outside [-1, world) (a broadcast needs one, an all-gather takes none), a scale other than 1, fp32 locals over a bf16
-// wire or NVLS for any op but SUM, a bf16 wire for the raw moves, a two-shot / NVLS / all-gather n_vec that is not a
-// multiple of world (the remainder would be left out) or an LL message larger than the inbox.
+// from `root`, 5 all-gather, or with root >= 0 gather to `root`, 6 scatter from `root`; a reduction with root >= 0 is a
+// reduce to that rank.  Returns cudaError_t as int; cudaErrorInvalidValue, without a launch, for an unknown variant or op, a
+// world outside 1..8, a rank outside [0, world), a root outside [-1, world) (a broadcast and a scatter need one), a scale
+// other than 1, fp32 locals over a bf16 wire or NVLS for any op but SUM, a bf16 wire for the raw moves, a two-shot / NVLS /
+// gather / scatter n_vec that is not a multiple of world (the remainder would be left out) or an LL message larger than the
+// inbox.
 int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
                         const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
                         int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root,
                         cudaStream_t stream) {
   if (variant < 0 || variant > 3 || world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world)
     return (int)cudaErrorInvalidValue;
-  if (op < b2::kSum || op > b2::kGather || root < -1 || root >= world) return (int)cudaErrorInvalidValue;
-  if (op == b2::kBcast ? root < 0 : (op == b2::kGather && root >= 0)) return (int)cudaErrorInvalidValue;
+  if (op < b2::kSum || op > b2::kScatter || root < -1 || root >= world) return (int)cudaErrorInvalidValue;
+  if ((op == b2::kBcast || op == b2::kScatter) && root < 0) return (int)cudaErrorInvalidValue;
   if (op != b2::kSum && (scale != 1.f || src_f32 || dst_f32)) return (int)cudaErrorInvalidValue;
   if (variant == 2 && (op != b2::kSum || root >= 0)) return (int)cudaErrorInvalidValue;   // NVLS: the SUM all-reduce only
   if (op >= b2::kBcast && bf16) return (int)cudaErrorInvalidValue;
-  if ((variant == 1 || variant == 2 || op == b2::kGather) && n_vec % (size_t)world != 0)
+  const bool segmented = op == b2::kGather || op == b2::kScatter;          // one segment of n_vec / world per rank
+  if ((variant == 1 || variant == 2 || segmented) && n_vec % (size_t)world != 0)
     return (int)cudaErrorInvalidValue;                                     // slice = n_vec / world
-  const size_t n_push = op == b2::kGather ? n_vec / world : n_vec;        // LL: vectors each rank pushes
+  const size_t n_push = segmented ? n_vec / world : n_vec;                // LL: vectors each rank pushes
   b2::ARArgs a;
   memset(&a.inbox, 0, sizeof(a.inbox));
   a.ll_cap = 0;
@@ -485,7 +540,7 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::S
   }
   if (variant == 2 && mc == nullptr) return (int)cudaErrorInvalidValue;
   if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
-  const size_t work = variant == 0 ? n_vec : variant == 3 ? n_push : n_vec / world;
+  const size_t work = variant == 0 ? (op == b2::kScatter ? n_push : n_vec) : variant == 3 ? n_push : n_vec / world;
   size_t blocks = (work + b2::kThreads - 1) / b2::kThreads;
   if (variant == 1 || variant == 2) blocks = (blocks + 1) / 2;
   if (blocks < 1) blocks = 1;
@@ -502,7 +557,8 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::S
     case b2::kMax: b2::launch_op<b2::kMax>(variant, bf16, grid, a, stream); break;
     case b2::kMin: b2::launch_op<b2::kMin>(variant, bf16, grid, a, stream); break;
     case b2::kBcast: b2::launch_op<b2::kBcast>(variant, bf16, grid, a, stream); break;
-    default: b2::launch_op<b2::kGather>(variant, bf16, grid, a, stream); break;
+    case b2::kGather: b2::launch_op<b2::kGather>(variant, bf16, grid, a, stream); break;
+    default: b2::launch_op<b2::kScatter>(variant, bf16, grid, a, stream); break;
   }
   return (int)cudaGetLastError();
 }

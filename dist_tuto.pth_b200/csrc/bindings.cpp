@@ -294,7 +294,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ------------------------------------------------------------------ collectives
   // op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN (reductions; root >= 0 stores on that rank only), 4 broadcast from root, 5 all-gather
-  // (n_vec counts the output, world x the per-rank input).  The raw moves take any dtype and copy bytes.
+  // (n_vec counts the output, world x the per-rank input; root >= 0: gather to that rank), 6 scatter from root (n_vec counts
+  // the root's input, world x the per-rank output).  The raw moves take any dtype and copy bytes.
   auto collective = [](const char* what, int op, int variant, bool bf16, const std::vector<unsigned long long>& bufs,
                        const std::vector<unsigned long long>& sigs, unsigned long long mc, const c10::optional<torch::Tensor>& src,
                        const c10::optional<torch::Tensor>& dst, size_t n_vec, double scale, int root, int rank, int world,
@@ -306,15 +307,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                 bufs.size(), " and ", sigs.size(), " for world ", world);
     TORCH_CHECK(variant == 3 ? (int)inbox.size() == world : inbox.empty() || (int)inbox.size() == world,
                 what, ": one LL inbox per rank, got ", inbox.size(), " for world ", world);
-    TORCH_CHECK((variant != 1 && variant != 2 && op != 5) || n_vec % (size_t)world == 0,
-                what, ": two-shot, NVLS and all-gather split n_vec into world slices, so n_vec must be a multiple of world "
-                "(pad the buffer), got n_vec ", n_vec, " for world ", world);
+    const bool segmented = op == 5 || op == 6;              // all-gather, gather, scatter: one segment per rank
+    TORCH_CHECK((variant != 1 && variant != 2 && !segmented) || n_vec % (size_t)world == 0,
+                what, ": two-shot, NVLS, all-gather, gather and scatter split n_vec into world slices, so n_vec must be a "
+                "multiple of world (pad the buffer), got n_vec ", n_vec, " for world ", world);
     TORCH_CHECK(root >= -1 && root < world, what, ": root must be -1 (every rank) or in [0, world), got ", root,
                 " for world ", world);
     TORCH_CHECK(op == 0 || scale == 1.0, what, ": scale applies to SUM only, got ", scale, " for op ", op);
     TORCH_CHECK(variant != 2 || (op == 0 && root < 0), what, ": NVLS runs the SUM all-reduce only");
-    TORCH_CHECK(variant != 3 || (op == 5 ? n_vec / world : n_vec) <= ll_cap, what, ": LL pushes ",
-                op == 5 ? n_vec / world : n_vec, " vectors per rank, more than the inbox holds (", ll_cap, ")");
+    TORCH_CHECK(variant != 3 || (segmented ? n_vec / world : n_vec) <= ll_cap, what, ": LL pushes ",
+                segmented ? n_vec / world : n_vec, " vectors per rank, more than the inbox holds (", ll_cap, ")");
     PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
     PeerPtrs ib = to_ptrs(inbox);
     const void* sp = nullptr; void* dp = nullptr; int sf = 0, df = 0;
@@ -347,6 +349,24 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     collective("allgather", 5, variant, false, bufs, sigs, 0, src, dst, n_vec, 1.0, -1, rank, world, max_blocks, inbox, ll_cap);
   }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("rank"),
      py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
+  // gather / scatter: every rank of one call must pass the same src / dst nullness (the one-shot and two-shot barriers depend
+  // on it); src of a scatter and dst of a gather are used on the root only.
+  m.def("gather", [collective](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                               c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int root,
+                               int rank, int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {
+    TORCH_CHECK(root >= 0, "gather: root must be in [0, world), got ", root);
+    collective("gather", 5, variant, false, bufs, sigs, 0, src, dst, n_vec, 1.0, root, rank, world, max_blocks, inbox, ll_cap);
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("root"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(),
+     py::arg("ll_cap") = 0);
+  m.def("scatter", [collective](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                                c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int root,
+                                int rank, int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {
+    TORCH_CHECK(root >= 0, "scatter: root must be in [0, world), got ", root);
+    collective("scatter", 6, variant, false, bufs, sigs, 0, src, dst, n_vec, 1.0, root, rank, world, max_blocks, inbox, ll_cap);
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("root"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(),
+     py::arg("ll_cap") = 0);
   m.def("barrier", [](std::vector<unsigned long long> sigs, int rank, int world) {
     check_world(rank, world, "barrier");
     TORCH_CHECK((int)sigs.size() == world, "barrier: one signal pad per rank, got ", sigs.size(), " for world ", world);

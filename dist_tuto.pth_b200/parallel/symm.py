@@ -19,9 +19,10 @@ in flight on different streams at once.  All collectives must be issued in the
 same order on every rank of the world (as with any communicator).
 
 Collectives: ``all_reduce_`` and ``reduce_`` (SUM, PRODUCT, MAX, MIN on fp32 /
-bf16), ``broadcast_`` and ``all_gather_`` (raw bytes, any dtype).  Each call
-picks its kernel variant with :func:`plan_variant` and never synchronises the
-host.
+bf16), ``broadcast_``, ``all_gather_``, ``scatter_`` and ``gather_`` (raw
+bytes, any dtype).  Each call picks its kernel variant with
+:func:`plan_variant` (scatter and gather by the all-gather rule, on one rank's
+segment) and never synchronises the host.
 """
 from __future__ import annotations
 
@@ -376,10 +377,12 @@ class SymmWorld:
 
     def _launch(self, hd: SymmHandle, bf16: bool, n_vec: int, scale: float, src, dst, variant: Optional[int],
                 max_blocks: Optional[int] = None, collective: str = "allreduce", op: int = 0, root: int = -1):
-        """One kernel call on ``hd``.  ``n_vec``: 16-byte vectors of the message (of the output for an all-gather, a multiple
-        of world there); ``root``: local rank (-1 for the all-to-all collectives)."""
-        n_push = n_vec // self.world if collective == "allgather" else n_vec
-        v = self.plan(collective, op, n_push * 16) if variant is None else variant
+        """One kernel call on ``hd``.  ``n_vec``: 16-byte vectors of the message (of the output for an all-gather or a gather,
+        of the root's input for a scatter, a multiple of world for those three); ``root``: local rank (-1 for the all-to-all
+        collectives)."""
+        segmented = collective in ("allgather", "gather", "scatter")
+        n_push = n_vec // self.world if segmented else n_vec
+        v = self.plan("allgather" if segmented else collective, op, n_push * 16) if variant is None else variant
         if v == 2 and (not hd.mc_ptr or collective != "allreduce" or op != 0):
             v = 1
         if v == 3 and (hd.ll is None or n_push > LL_CAP_VEC):
@@ -392,6 +395,10 @@ class SymmWorld:
             self.C.broadcast(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
         elif collective == "allgather":
             self.C.allgather(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, self.rank, self.world, mb, *ll)
+        elif collective == "gather":
+            self.C.gather(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
+        elif collective == "scatter":
+            self.C.scatter(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
         else:
             self.C.allreduce(v, bf16, hd.ptrs, hd.sig_ptrs, hd.mc_ptr, src, dst, n_vec, float(scale), self.rank,
                              self.world, mb, *ll, op, root)
@@ -402,7 +409,8 @@ class SymmWorld:
         return op_code(op) is not None
 
     def supports_raw(self, t: torch.Tensor) -> bool:
-        """Can ``broadcast_`` / ``all_gather_`` take this tensor (CUDA, this device, contiguous, any dtype)?"""
+        """Can ``broadcast_`` / ``all_gather_`` / ``scatter_`` / ``gather_`` take this tensor (CUDA, this device, contiguous,
+        any dtype)?"""
         return t.is_cuda and t.device == self.device and t.is_contiguous()
 
     def local_rank(self, root: int) -> int:
@@ -539,6 +547,96 @@ class SymmWorld:
             if o.data_ptr() != base + r * slot:
                 o.view(-1).view(torch.uint8).copy_(buf[r * slot:r * slot + nbytes])
         return outs
+
+    def _root_list(self, what: str, lst, t: torch.Tensor) -> None:
+        """The root's list of a scatter or gather: ``world`` contiguous CUDA tensors on this device with ``t``'s dtype and
+        size.  Raised on the root only, before any launch: its peers are then left inside the kernel until its spin limit
+        reports them (B2_SPIN_LIMIT), as with a collective that one rank never joins."""
+        if lst is None or len(lst) != self.world:
+            raise ValueError(f"{what} needs {self.world} tensors on the root, got {None if lst is None else len(lst)}")
+        if not all(isinstance(o, torch.Tensor) and self.supports_raw(o) for o in lst):
+            raise TypeError(f"fused {what} needs contiguous CUDA tensors on this device")
+        if any(o.dtype != t.dtype or o.numel() != t.numel() for o in lst):
+            raise ValueError(f"every tensor of {what}'s list must have the tensor's dtype and size")
+
+    def _one_block(self, lst: List[torch.Tensor], nbytes: int) -> Optional[torch.Tensor]:
+        """``lst`` as one uint8 tensor when its entries are consecutive views of one 16-byte aligned block, else None."""
+        o0 = lst[0].data_ptr()
+        if o0 % 16 or any(o.data_ptr() != o0 + r * nbytes for r, o in enumerate(lst)):
+            return None
+        return self.C.tensor_from_ptr(o0, self.world * nbytes, torch.uint8, self.device.index)
+
+    def scatter_(self, t: torch.Tensor, scatter_list: Optional[List[torch.Tensor]], root: int,
+                 variant: Optional[int] = None, max_blocks: Optional[int] = None) -> torch.Tensor:
+        """``t`` <- global rank ``root``'s ``scatter_list[rank]`` on every rank (any dtype; copied bit for bit).
+        ``scatter_list`` is read on the root only.
+
+        Whether src and dst are fused into the kernel depends on ``t``'s size alone, so every rank makes the same choice
+        (the kernels' barriers depend on it) while only the root holds the list: a multiple of 16 bytes is fused (an
+        unaligned ``t`` through an aligned scratch tensor, a root list that is not one block through the staging buffer),
+        any other size goes through the staging buffer in place."""
+        r0 = self.local_rank(root)
+        if not self.supports_raw(t):
+            raise TypeError("fused scatter needs a contiguous CUDA tensor on this device")
+        if self.rank == r0:
+            self._root_list("scatter", scatter_list, t)
+        if self.world == 1:
+            t.copy_(scatter_list[0])
+            return t
+        nbytes = t.numel() * t.element_size()
+        seg = (nbytes + 15) // 16                              # vectors per rank
+        n_vec, slot = seg * self.world, seg * 16
+        st = self._staging_for(torch.float32, n_vec * 16)      # the same size on every rank: allocation is collective
+        buf = st.view(torch.uint8, st.nbytes)
+        block = self._one_block(scatter_list, nbytes) if self.rank == r0 and nbytes % 16 == 0 else None
+        if self.rank == r0 and block is None:
+            for r, o in enumerate(scatter_list):
+                buf[r * slot:r * slot + nbytes].copy_(o.view(-1).view(torch.uint8))
+        out = t.view(-1).view(torch.uint8)
+        if nbytes % 16 == 0:
+            dst = out if out.data_ptr() % 16 == 0 else torch.empty_like(out)
+            src = block if block is not None else buf[:n_vec * 16]
+            self._launch(st, False, n_vec, 1.0, src, dst, variant, max_blocks, "scatter", 0, r0)
+            if dst is not out:
+                out.copy_(dst)
+        else:  # ragged size: scatter in place, then copy this rank's slot out
+            self._launch(st, False, n_vec, 1.0, None, None, variant, max_blocks, "scatter", 0, r0)
+            out.copy_(buf[self.rank * slot:self.rank * slot + nbytes])
+        return t
+
+    def gather_(self, t: torch.Tensor, gather_list: Optional[List[torch.Tensor]], root: int,
+                variant: Optional[int] = None, max_blocks: Optional[int] = None) -> Optional[List[torch.Tensor]]:
+        """Global rank ``root``'s ``gather_list[r]`` <- rank r's ``t`` (any dtype; copied bit for bit).  ``gather_list`` is
+        read and written on the root only; the others' outputs are left alone.  src and dst are chosen as in
+        :meth:`scatter_`, by ``t``'s size alone; a root list that is not one block is filled from the staging buffer."""
+        r0 = self.local_rank(root)
+        if not self.supports_raw(t):
+            raise TypeError("fused gather needs a contiguous CUDA tensor on this device")
+        if self.rank == r0:
+            self._root_list("gather", gather_list, t)
+        if self.world == 1:
+            gather_list[0].copy_(t)
+            return gather_list
+        nbytes = t.numel() * t.element_size()
+        seg = (nbytes + 15) // 16
+        n_vec, slot = seg * self.world, seg * 16
+        st = self._staging_for(torch.float32, n_vec * 16)
+        buf = st.view(torch.uint8, st.nbytes)
+        block = self._one_block(gather_list, nbytes) if self.rank == r0 and nbytes % 16 == 0 else None
+        inp = t.view(-1).view(torch.uint8)
+        if nbytes % 16 == 0:
+            src = inp if inp.data_ptr() % 16 == 0 else inp.clone()
+            dst = block if block is not None else buf[:n_vec * 16]
+            self._launch(st, False, n_vec, 1.0, src, dst, variant, max_blocks, "gather", 0, r0)
+        else:  # ragged size: stage this rank's bytes at its slot, gather in place
+            buf[self.rank * slot:self.rank * slot + nbytes].copy_(inp)
+            self._launch(st, False, n_vec, 1.0, None, None, variant, max_blocks, "gather", 0, r0)
+        if self.rank != r0:
+            return None
+        if block is None:
+            for r, o in enumerate(gather_list):
+                o.view(-1).view(torch.uint8).copy_(buf[r * slot:r * slot + nbytes])
+        return gather_list
 
     def _staging_for(self, dtype, nbytes: int) -> SymmHandle:
         st = self._staging.get(dtype)
