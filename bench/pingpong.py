@@ -1,10 +1,12 @@
 """send/recv ping-pong latency at 2 GPUs over NVSwitch (BASELINE.json config #5; ptp.py / tuto.md:82-91).
 
-Our ``send``/``recv`` ride on NCCL p2p (by design: the tutorial's point-to-point stays on NCCL), so this
-reports the library's latency through our API next to raw ``torch.distributed`` for reference."""
+Runs with ``backend="b200"``, so the ``b2`` arm is our ``send``/``recv`` on the peer-memory point-to-point kernels
+(``csrc/p2p.cu``) and the ``torch`` arm is raw ``torch.distributed`` on NCCL.  The JSON output records the card and its
+power limit, read in the same run."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -18,11 +20,16 @@ import types
 ARGS = types.SimpleNamespace(**json.loads(os.environ["B2_BENCH_ARGS"])) if "B2_BENCH_ARGS" in os.environ else None
 
 
+def gpu_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i",
+                        str(torch.cuda.current_device())], capture_output=True, text=True, timeout=60)
+    name, power = [s.strip() for s in q.stdout.strip().splitlines()[0].split(",")]
+    return {"device": name, "power_limit_w": float(power)}
+
+
 def body(rank, size):
     dev = torch.device("cuda", torch.cuda.current_device())
     rows = []
-    if rank < 2:
-        pass
     for nbytes in [4, 64, 1024, 16 << 10, 256 << 10, 1 << 20, 16 << 20]:
         t = torch.zeros(max(1, nbytes // 4), device=dev)
         iters = 200 if nbytes <= (1 << 20) else 40
@@ -56,7 +63,7 @@ def body(rank, size):
             print(json.dumps(res), flush=True)
     if rank == 0:
         os.makedirs(os.path.dirname(ARGS.out) or ".", exist_ok=True)
-        json.dump({"rows": rows}, open(ARGS.out, "w"), indent=1)
+        json.dump({"rows": rows, "backend": "b200", "gpu": gpu_info()}, open(ARGS.out, "w"), indent=1)
     dist.barrier()
 
 
@@ -65,4 +72,4 @@ if __name__ == "__main__":
     ap.add_argument("--out", default="gpurun_out/pingpong.json")
     ARGS = ap.parse_args()
     os.environ["B2_BENCH_ARGS"] = json.dumps(vars(ARGS))
-    b2.launch(body, size=2, backend="nccl", join_timeout_s=600)
+    b2.launch(body, size=2, backend="b200", join_timeout_s=600)

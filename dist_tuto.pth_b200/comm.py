@@ -9,7 +9,7 @@ Parity map (reference = /root/reference):
   * ``get_rank()/get_world_size()``                 train_dist.py:84,88,96
 
 Design (GPU-first, not a port):
-  * plumbing (rendezvous, p2p, the non-hot collectives) rides on
+  * plumbing (rendezvous, anything without a symmetric world) rides on
     ``torch.distributed`` -- NCCL for CUDA tensors (NVLink 5 / NVSwitch),
     gloo for CPU tensors;
   * when a symmetric world has been set up for the group (``backend="b200"``),
@@ -21,6 +21,12 @@ Design (GPU-first, not a port):
     and so does every op but SUM on a world that serves only the sum (no
     ``supports_op``) and ``scatter`` / ``gather`` on a world without
     ``scatter_`` / ``gather_`` (the two-level world of several machines).
+  * on such a world ``send``, ``recv``, ``isend`` and ``irecv`` of a CUDA
+    tensor (any dtype, bit for bit) run on our own point-to-point kernels
+    (``csrc/p2p.cu``) when the peer is given: messages between a pair are
+    matched in issue order and ``tag`` is ignored, as NCCL ignores it.
+    ``recv(src=None)``, CPU tensors and the two-level world (no ``send_``)
+    stay on torch.
   * ``group=0`` (the 2017 spelling of "world", train_dist.py:99, ptp.py:26)
     is accepted and mapped to the default group (fixes defect D2).
 """
@@ -133,27 +139,56 @@ def _check(t: torch.Tensor):
 
 
 # ----------------------------------------------------------------- p2p -------
+# On a symmetric world (``backend="b200"``) a CUDA tensor with a given peer goes through the peer-memory mailbox of
+# ``SymmWorld.send_`` / ``recv_`` / ``isend_`` / ``irecv_``: both sides must use this module with the same byte count, and
+# messages between one pair are matched in the order they are issued (``tag`` is ignored there, as NCCL ignores it).
+def _p2p_world(tensor: torch.Tensor, group, peer: Optional[int]):
+    """The symmetric world whose point-to-point kernels take this call, or None (torch.distributed)."""
+    if peer is None:
+        return None
+    w = _symm_world_for(tensor, group)
+    if w is None or not hasattr(w, "send_") or not w.supports_raw(tensor):
+        return None
+    return w
+
+
 def send(tensor: torch.Tensor, dst: int, group=None, tag: int = 0) -> None:
-    """Blocking send (tuto.md:87).  Returns when the buffer may be reused."""
+    """Blocking send (tuto.md:87).  Returns when the buffer may be reused: on CUDA, as with NCCL, once the current stream is
+    ordered after the transfer (the host is not synchronised).  ``dst`` is a global rank."""
     _check(tensor)
+    w = _p2p_world(tensor, group, dst)
+    if w is not None:
+        w.send_(tensor, dst)
+        return None
     dist.send(tensor, dst=dst, group=_g(group), tag=tag)
 
 
 def recv(tensor: torch.Tensor, src: Optional[int] = None, group=None, tag: int = 0) -> int:
-    """Blocking receive into a pre-allocated tensor (tuto.md:90)."""
+    """Blocking receive into a pre-allocated tensor (tuto.md:90); returns the sender's rank.  ``src=None`` (any source)
+    always goes to torch.distributed."""
     _check(tensor)
+    w = _p2p_world(tensor, group, src)
+    if w is not None:
+        w.recv_(tensor, src)
+        return src
     return dist.recv(tensor, src=src, group=_g(group), tag=tag)
 
 
 def isend(tensor: torch.Tensor, dst: int, group=None, tag: int = 0) -> Request:
     """Non-blocking send (tuto.md:108)."""
     _check(tensor)
+    w = _p2p_world(tensor, group, dst)
+    if w is not None:
+        return Request(w.isend_(tensor, dst), tensor)
     return Request(dist.isend(tensor, dst=dst, group=_g(group), tag=tag), tensor)
 
 
 def irecv(tensor: torch.Tensor, src: Optional[int] = None, group=None, tag: int = 0) -> Request:
     """Non-blocking receive (tuto.md:112)."""
     _check(tensor)
+    w = _p2p_world(tensor, group, src)
+    if w is not None:
+        return Request(w.irecv_(tensor, src), tensor)
     return Request(dist.irecv(tensor, src=src, group=_g(group), tag=tag), tensor)
 
 

@@ -40,6 +40,11 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const Signa
                         int src_f32, void* dst, int dst_f32, size_t n_vec, float scale, int rank, int world,
                         int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root, cudaStream_t stream);
 int b2_barrier_launch(const SignalPadsH* sig, int rank, int world, cudaStream_t stream);
+void b2_p2p_config(int* ctas, int* slots, size_t* chunk, int* pad_words);
+int b2_p2p_send_launch(const PeerPtrs* box, const SignalPadsH* sig, const void* src, size_t nbytes, int rank, int peer,
+                       int world, cudaStream_t stream);
+int b2_p2p_recv_launch(const PeerPtrs* box, const SignalPadsH* sig, void* dst, size_t nbytes, int rank, int peer,
+                       int world, cudaStream_t stream);
 int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float* params, float* momentum,
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
@@ -373,6 +378,50 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     SignalPadsH s = to_sig(sigs);
     ck_cuda(b2_barrier_launch(&s, rank, world, cur_stream()), "barrier launch");
   });
+
+  // ------------------------------------------------------------------ point-to-point (csrc/p2p.cu)
+  // bufs / sigs: the mailbox data and signal pad of every rank.  Both sides of a transfer must pass the same byte count (as
+  // with NCCL); a zero-byte message launches nothing.  Messages between one pair are matched in issue order.
+  m.def("p2p_config", [] {
+    int ctas = 0, slots = 0, pad_words = 0;
+    size_t chunk = 0;
+    b2_p2p_config(&ctas, &slots, &chunk, &pad_words);
+    return py::make_tuple(ctas, slots, chunk, pad_words);
+  }, "(CTAs per transfer, slots per CTA, bytes per slot, signal-pad words) of the point-to-point mailbox");
+  // A stream of its own, not one of torch's pooled streams (handed out round robin, so two of them can be one CUDA stream):
+  // a send and a receive that wait for their peers must never be queued on one stream.
+  m.def("stream_create", [](int device) {
+    c10::cuda::CUDAGuard guard(device);
+    cudaStream_t s = nullptr;
+    ck_cuda((int)cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), "cudaStreamCreateWithFlags");
+    return (unsigned long long)(uintptr_t)s;
+  }, py::arg("device"));
+  m.def("stream_destroy", [](unsigned long long s) {
+    ck_cuda((int)cudaStreamDestroy((cudaStream_t)(uintptr_t)s), "cudaStreamDestroy");
+  }, py::arg("stream"));
+  auto p2p = [](const char* what, bool send, const std::vector<unsigned long long>& bufs,
+                const std::vector<unsigned long long>& sigs, const torch::Tensor& t, int peer, int rank, int world) {
+    check_world(rank, world, what);
+    TORCH_CHECK(world >= 2, what, ": a point-to-point transfer needs a world of at least 2, got ", world);
+    TORCH_CHECK(peer >= 0 && peer < world, what, ": peer ", peer, " is outside [0, ", world, ")");
+    TORCH_CHECK(peer != rank, what, ": rank ", rank, " cannot be its own peer");
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, what, ": one mailbox and one signal pad per rank, got ",
+                bufs.size(), " and ", sigs.size(), " for world ", world);
+    check_cuda_contig(t, send ? "src" : "dst");
+    TORCH_CHECK((uintptr_t)t.data_ptr() % 16 == 0, what, ": the tensor must be 16-byte aligned");
+    const size_t nbytes = (size_t)t.numel() * t.element_size();
+    if (nbytes == 0) return;
+    PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(t.device());
+    ck_cuda(send ? b2_p2p_send_launch(&b, &s, t.data_ptr(), nbytes, rank, peer, world, cur_stream())
+                 : b2_p2p_recv_launch(&b, &s, t.data_ptr(), nbytes, rank, peer, world, cur_stream()), what);
+  };
+  m.def("p2p_send", [p2p](std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs, torch::Tensor src, int peer,
+                          int rank, int world) { p2p("p2p_send", true, bufs, sigs, src, peer, rank, world); },
+        py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("peer"), py::arg("rank"), py::arg("world"));
+  m.def("p2p_recv", [p2p](std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs, torch::Tensor dst, int peer,
+                          int rank, int world) { p2p("p2p_recv", false, bufs, sigs, dst, peer, rank, world); },
+        py::arg("bufs"), py::arg("sigs"), py::arg("dst"), py::arg("peer"), py::arg("rank"), py::arg("world"));
   m.def("allreduce_sgd", [](std::vector<unsigned long long> grads, std::vector<unsigned long long> sigs, torch::Tensor params,
                             torch::Tensor momentum, c10::optional<torch::Tensor> step, double lr, double mu, double scale,
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,

@@ -23,6 +23,10 @@ bf16), ``broadcast_``, ``all_gather_``, ``scatter_`` and ``gather_`` (raw
 bytes, any dtype).  Each call picks its kernel variant with
 :func:`plan_variant` (scatter and gather by the all-gather rule, on one rank's
 segment) and never synchronises the host.
+
+Point-to-point: ``send_``, ``recv_``, ``isend_`` and ``irecv_`` (raw bytes, any dtype) move messages through a mailbox
+every world of more than one rank allocates when it is built (``csrc/p2p.cu``).  Each (peer, direction) pair has its own
+stream, so a receive is never queued behind a send that waits for its peer; like NCCL they never synchronise the host.
 """
 from __future__ import annotations
 
@@ -38,7 +42,7 @@ import torch.distributed as dist
 
 from ..ops import _ext
 
-__all__ = ["SymmWorld", "SymmHandle", "init_world", "lookup_world", "destroy_all", "VARIANTS", "COLLECTIVES",
+__all__ = ["SymmWorld", "SymmHandle", "P2PWork", "init_world", "lookup_world", "destroy_all", "VARIANTS", "COLLECTIVES",
            "op_code", "plan_variant"]
 
 PAD_BYTES = 8192                      # signal pad at the head of every allocation (B2_SIGNAL_WORDS*4 = 6016 B)
@@ -132,6 +136,22 @@ class SymmHandle:
         return _ext.C().tensor_from_ptr(self.ptrs[r], n, dtype, self.world.device.index)
 
 
+class P2PWork:
+    """The work object of :meth:`SymmWorld.isend_` / :meth:`SymmWorld.irecv_` (``comm.Request`` wraps it)."""
+
+    def __init__(self, event: torch.cuda.Event, device: torch.device):
+        self.event, self.device = event, device
+
+    def wait(self) -> bool:
+        """Order the current stream after the transfer (the host is not synchronised), as NCCL's work objects do."""
+        torch.cuda.current_stream(self.device).wait_event(self.event)
+        return True
+
+    def is_completed(self) -> bool:
+        """Has the transfer finished on the GPU?  (Never blocks.)"""
+        return self.event.query()
+
+
 class SymmWorld:
     """Symmetric-memory communicator over the ranks of a process group (<= 8 GPUs, one node)."""
 
@@ -196,6 +216,13 @@ class SymmWorld:
         self.oneshot_max = _env_int("B200DIST_ONESHOT_MAX", defaults["oneshot_max"])
         self.nvls_min = _env_int("B200DIST_NVLS_MIN", defaults["nvls_min"])
         self.nvls_error: Optional[str] = None
+        # point-to-point mailbox (csrc/p2p.cu): allocated here because allocation is collective and a send involves two
+        # ranks only; one stream per (peer, direction), as NCCL point-to-point has one communicator stream per pair
+        self.p2p: Optional[SymmHandle] = None
+        self._p2p_streams: Dict[tuple, torch.cuda.Stream] = {}
+        if self.world > 1:
+            ctas, slots, chunk, _ = self.C.p2p_config()
+            self.p2p = self.alloc_bytes((self.world - 1) * ctas * slots * chunk, ll=False)
 
     # ------------------------------------------------------------------ plumbing
     def _addr(self, r: int) -> bytes:
@@ -638,6 +665,58 @@ class SymmWorld:
                 o.view(-1).view(torch.uint8).copy_(buf[r * slot:r * slot + nbytes])
         return gather_list
 
+    # ------------------------------------------------------------------ point-to-point
+    def send_(self, t: torch.Tensor, dst: int) -> None:
+        """Send ``t``'s bytes to global rank ``dst`` (any dtype; copied bit for bit).  Like ``dist.send`` on NCCL it returns
+        without synchronising the host: the current stream is ordered after the transfer, so ``t`` may then be reused.
+
+        The receiver must post a receive of the same byte count from this rank; messages between one pair are matched in
+        the order they are issued (there are no tags)."""
+        self._p2p(True, t, dst).wait()
+
+    def recv_(self, t: torch.Tensor, src: int) -> torch.Tensor:
+        """Receive into ``t`` the bytes global rank ``src`` sends (same byte count); the current stream is ordered after
+        the transfer, the host is not synchronised."""
+        self._p2p(False, t, src).wait()
+        return t
+
+    def isend_(self, t: torch.Tensor, dst: int) -> "P2PWork":
+        """Non-blocking :meth:`send_`: ``t`` must not be written before the returned work's ``wait()``."""
+        return self._p2p(True, t, dst)
+
+    def irecv_(self, t: torch.Tensor, src: int) -> "P2PWork":
+        """Non-blocking :meth:`recv_`: ``t`` must not be read or written before the returned work's ``wait()``."""
+        return self._p2p(False, t, src)
+
+    def _p2p(self, send: bool, t: torch.Tensor, peer_rank: int) -> "P2PWork":
+        """One transfer on the (peer, direction) stream: that stream waits for the current one, the kernel runs on it, and
+        the returned work holds an event recorded after it.  A data pointer that is not 16-byte aligned goes through an
+        aligned scratch copy made on the same stream."""
+        what = "send" if send else "recv"
+        peer = self.local_rank(peer_rank)
+        if peer == self.rank:
+            raise ValueError(f"{what}: rank {peer_rank} cannot {what} to itself")
+        if not self.supports_raw(t):
+            raise TypeError(f"peer-memory {what} needs a contiguous CUDA tensor on this device")
+        stream = self._p2p_streams.get((peer, send))
+        if stream is None:                                     # a CUDA stream of its own, never one of torch's pooled ones
+            stream = torch.cuda.ExternalStream(self.C.stream_create(self.device.index), device=self.device)
+            self._p2p_streams[(peer, send)] = stream
+        stream.wait_stream(torch.cuda.current_stream(self.device))
+        raw = t.view(-1).view(torch.uint8)
+        with torch.cuda.stream(stream):
+            buf = raw if raw.data_ptr() % 16 == 0 else (raw.clone() if send else torch.empty_like(raw))
+            if send:
+                self.C.p2p_send(self.p2p.ptrs, self.p2p.sig_ptrs, buf, peer, self.rank, self.world)
+            else:
+                self.C.p2p_recv(self.p2p.ptrs, self.p2p.sig_ptrs, buf, peer, self.rank, self.world)
+                if buf is not raw:
+                    raw.copy_(buf)
+        t.record_stream(stream)                                # t's memory is not reused while the transfer runs
+        done = torch.cuda.Event()
+        done.record(stream)
+        return P2PWork(done, self.device)
+
     def _staging_for(self, dtype, nbytes: int) -> SymmHandle:
         st = self._staging.get(dtype)
         if st is None or st.nbytes < nbytes + 2048:
@@ -686,6 +765,13 @@ class SymmWorld:
                 pass
         self._handles.clear()
         self._staging.clear()
+        self.p2p = None
+        for st in self._p2p_streams.values():
+            try:
+                self.C.stream_destroy(st.cuda_stream)
+            except Exception:
+                pass
+        self._p2p_streams.clear()
 
 
 def init_world(group=None, **kw) -> SymmWorld:

@@ -15,8 +15,9 @@ buffer with an ``isend`` in flight is never overwritten.
 bandwidth-optimal ring (reduce-scatter + all-gather over 1/N-sized chunks),
 2(N-1)/N * M bytes per rank instead of (N-1) * M.
 
-Both run on whatever p2p backend the tensors call for: NCCL send/recv over
-NVLink for CUDA tensors, gloo for CPU tensors.  The *hot* gradient all-reduce
+Both run on whatever p2p backend ``comm`` picks for the tensors: the
+peer-memory kernels of ``csrc/p2p.cu`` for CUDA tensors on ``backend="b200"``,
+NCCL send/recv otherwise, gloo for CPU tensors.  The *hot* gradient all-reduce
 of the framework does not use this file -- see ``parallel/symm.py``.
 """
 from __future__ import annotations

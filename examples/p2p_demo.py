@@ -5,7 +5,8 @@
 
 blocking:      rank 0 increments a tensor and ``send``s it, rank 1 ``recv``s it -> both print 1.0
 non-blocking:  same with ``isend``/``irecv``; the data is only valid after ``req.wait()``.
-On ``--backend b200`` the tensors live on the GPUs and the transfer is NCCL p2p over NVSwitch."""
+On ``--backend b200`` the tensors live on the GPUs and the transfer runs on the library's peer-memory point-to-point
+kernels (``csrc/p2p.cu``) over NVSwitch; on ``--backend nccl`` it is NCCL p2p."""
 import argparse
 import os
 import sys
