@@ -18,7 +18,8 @@ Bandwidth columns:
 ``--collective {reduce,broadcast,allgather,scatter,gather}`` or ``--op {product,max,min}`` time that collective instead:
 every variant of ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the NCCL call on the same
 tensor, per size (for an all-gather, a scatter and a gather, the size of one rank's segment; the root is rank 0 and its
-list is one block).  It compares GPUs, so it refuses to run on one.
+list is one block).  ``--dtype {bf16,fp16,fp64,int8,uint8,int32,int64,bool}`` times the reductions (and the raw moves) on
+a tensor of that dtype.  It compares GPUs, so it refuses to run on one.
 """
 import argparse
 import json
@@ -77,6 +78,8 @@ def time_op(fn, iters, dev, graph=False):
 
 
 OPS = {"sum": dist.ReduceOp.SUM, "product": dist.ReduceOp.PRODUCT, "max": dist.ReduceOp.MAX, "min": dist.ReduceOp.MIN}
+DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16, "fp64": torch.float64, "int8": torch.int8,
+          "uint8": torch.uint8, "int32": torch.int32, "int64": torch.int64, "bool": torch.bool}
 
 
 def body_collective(rank, size):
@@ -88,12 +91,13 @@ def body_collective(rank, size):
     rows = []
     s = 1024
     while s <= ARGS.max_mb << 20:
-        n = s // 4
-        t = torch.ones(n, device=dev)
+        dtype = DTYPES[ARGS.dtype]
+        n = s // torch.empty((), dtype=dtype).element_size()
+        t = torch.ones(n, dtype=dtype, device=dev)
         outs = [torch.empty_like(t) for _ in range(size)]
-        lst = list(torch.empty(size * n, device=dev).view(size, n).unbind(0)) if rank == 0 else None  # scatter / gather
+        lst = list(torch.empty(size * n, dtype=dtype, device=dev).view(size, n).unbind(0)) if rank == 0 else None  # scatter / gather
         iters = 100 if s <= (1 << 20) else 20
-        row = {"bytes": s, "collective": coll, "op": ARGS.op}
+        row = {"bytes": s, "collective": coll, "op": ARGS.op, "dtype": ARGS.dtype}
         arms = []
         for name, v in (("ll", 3), ("oneshot", 0), ("twoshot", 1)):
             if name == "ll" and s > symm.LL_CAP_VEC * 16:
@@ -137,7 +141,7 @@ def body_collective(rank, size):
 
 
 def body(rank, size):
-    if ARGS.collective != "allreduce" or ARGS.op != "sum":
+    if ARGS.collective != "allreduce" or ARGS.op != "sum" or ARGS.dtype != "fp32":
         return body_collective(rank, size)
     dev = torch.device("cuda", torch.cuda.current_device())
     w = symm.lookup_world(None)
@@ -267,16 +271,17 @@ if __name__ == "__main__":
     ap.add_argument("--emit-table", action="store_true", help="write the measured variant thresholds of this world size")
     ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather", "scatter", "gather"], default="allreduce")
     ap.add_argument("--op", choices=sorted(OPS), default="sum")
+    ap.add_argument("--dtype", choices=list(DTYPES), default="fp32", help="tensor dtype of the reductions")
     ARGS = ap.parse_args()
     if ARGS.gpus < 2:
         ap.error("the sweep compares collectives across GPUs; it needs --gpus 2 or more")
-    if ARGS.emit_table and (ARGS.collective != "allreduce" or ARGS.op != "sum"):
-        ap.error("--emit-table measures the SUM all-reduce thresholds")
+    if ARGS.emit_table and (ARGS.collective != "allreduce" or ARGS.op != "sum" or ARGS.dtype != "fp32"):
+        ap.error("--emit-table measures the fp32 SUM all-reduce thresholds")
     if ARGS.out is None:
         ARGS.out = f"gpurun_out/sweep_{ARGS.gpus}.json"
-        if (ARGS.collective, ARGS.op) != ("allreduce", "sum"):    # one file per collective and op
+        if (ARGS.collective, ARGS.op, ARGS.dtype) != ("allreduce", "sum", "fp32"):    # one file per collective, op, dtype
             stem, ext = os.path.splitext(ARGS.out)
-            ARGS.out = f"{stem}_{ARGS.collective}_{ARGS.op}{ext}"
+            ARGS.out = f"{stem}_{ARGS.collective}_{ARGS.op}" + ("" if ARGS.dtype == "fp32" else f"_{ARGS.dtype}") + ext
     os.environ["B2_BENCH_ARGS"] = json.dumps(vars(ARGS))
     if "RANK" in os.environ:
         b2.init_from_env(body, backend="b200")

@@ -14,13 +14,17 @@ Design (GPU-first, not a port):
     gloo for CPU tensors;
   * when a symmetric world has been set up for the group (``backend="b200"``),
     blocking ``all_reduce`` and ``reduce`` (SUM, PRODUCT, MAX, MIN on CUDA
-    fp32 / bf16) and ``broadcast``, ``all_gather``, ``scatter`` and ``gather``
-    (CUDA, any dtype, copied bit for bit) run on our own fused peer-memory
-    kernels (``parallel.symm``); that path never calls NCCL.
-    ``async_op=True``, CPU tensors, other dtypes and ops go to NCCL / gloo,
-    and so does every op but SUM on a world that serves only the sum (no
-    ``supports_op``) and ``scatter`` / ``gather`` on a world without
-    ``scatter_`` / ``gather_`` (the two-level world of several machines).
+    fp32, bf16, fp16, fp64, int8, uint8, int32, int64 and bool -- torch's NCCL
+    dtypes; integers wrap and a bool SUM is a MAX, as with NCCL) and
+    ``broadcast``, ``all_gather``, ``scatter`` and ``gather`` (CUDA, any
+    dtype, copied bit for bit) run on our own fused peer-memory kernels
+    (``parallel.symm``); that path never calls NCCL.
+    ``async_op=True``, CPU tensors, AVG and other dtypes (int16, the wider
+    unsigned types, complex, fp8) go to NCCL / gloo, and so does every op but
+    SUM on a world that serves only the sum (no ``supports_op``), every dtype
+    but fp32 / bf16 on a world without ``supports_reduction``, and
+    ``scatter`` / ``gather`` on a world without ``scatter_`` / ``gather_``
+    (the two-level world of several machines has none of the three).
   * on such a world ``send``, ``recv``, ``isend`` and ``irecv`` of a CUDA
     tensor (any dtype, bit for bit) run on our own point-to-point kernels
     (``csrc/p2p.cu``) when the peer is given: messages between a pair are
@@ -206,8 +210,11 @@ def _symm_world_for(tensor: torch.Tensor, group):
 
 def _reduces(w, tensor: torch.Tensor, op) -> bool:
     """Does world ``w`` run this reduction natively?  SUM on any world that takes the tensor; the other ops only on a
-    world that says it supports them (a hierarchical world reduces SUM only)."""
-    if w is None or not w.supports(tensor):
+    world that says it supports them (a hierarchical world reduces SUM only).  A world with ``supports_reduction`` takes
+    the dtypes beyond fp32 / bf16 too; one without it (the hierarchical world) only what ``supports`` takes."""
+    if w is None:
+        return False
+    if not (w.supports_reduction if hasattr(w, "supports_reduction") else w.supports)(tensor):
         return False
     if op == reduce_op.SUM:
         return True
@@ -217,9 +224,13 @@ def _reduces(w, tensor: torch.Tensor, op) -> bool:
 def all_reduce(tensor: torch.Tensor, op=reduce_op.SUM, group=None, async_op: bool = False):
     """In-place all-reduce; result on every rank (tuto.md:176-186,199).
 
-    CUDA fp32 / bf16 tensors go through the fused sm_90a peer-memory kernels
-    (variant picked by size) for SUM, PRODUCT, MAX and MIN when a symmetric
-    world exists for the group; everything else goes to NCCL / gloo."""
+    CUDA tensors go through the fused sm_90a peer-memory kernels (variant
+    picked by size) for SUM, PRODUCT, MAX and MIN when a symmetric world
+    exists for the group: fp32 / bf16 (fp32 accumulator), fp16 (fp32
+    accumulator, rounded once), fp64, int8, uint8, int32 and int64 (SUM and
+    PRODUCT wrap, as NCCL's do) and bool (SUM is MAX, as torch maps it for
+    NCCL).  Everything else (AVG, other dtypes, CPU tensors, ``async_op``)
+    goes to NCCL / gloo."""
     _check(tensor)
     if not async_op:
         w = _symm_world_for(tensor, group)
@@ -234,7 +245,7 @@ def all_reduce(tensor: torch.Tensor, op=reduce_op.SUM, group=None, async_op: boo
 
 def reduce(tensor: torch.Tensor, dst: int, op=reduce_op.SUM, group=None):
     """Reduce to ``dst`` only (tuto.md:198); ``dst`` is a global rank.  Other ranks' tensors are left as they were.
-    Routed like ``all_reduce``."""
+    Routed like ``all_reduce``, with the same ops and dtypes."""
     _check(tensor)
     w = _symm_world_for(tensor, group)
     if _reduces(w, tensor, op) and hasattr(w, "reduce_"):

@@ -30,6 +30,8 @@
 // other on one buffer, signal pad and inbox.
 #include <cstdio>
 #include <cstring>
+#include <cuda_fp16.h>
+#include <type_traits>
 #include "common.cuh"
 
 namespace b2 {
@@ -74,12 +76,17 @@ struct Op<kMin> {
   __device__ static __forceinline__ float fin(float a, float) { return a; }
 };
 
-template <bool BF16>
-struct Wire;  // one "vec" = 16 bytes on the wire
+// Lane types: how one 16-byte vector on the wire splits into accumulator lanes, per dtype class.  Every lane type has
+// `Acc` (the lane's accumulator type), kElems lanes per vector, zero<OP> (the identity), add<OP> (combine one vector into the
+// lanes) and pack<OP> (the lanes back to a vector).  kF32Local: the local tensor may be fp32 over this wire (bf16 SUM only);
+// kNvls: the switch can reduce this wire (multimem.ld_reduce).  Only fp32 / bf16 take a scale; the launcher refuses one for
+// the others, whose pack ignores it.
+enum : int { kF32 = 0, kBF16 = 1, kF16 = 2, kF64 = 3, kI8 = 4, kU8 = 5, kI32 = 6, kI64 = 7, kBool = 8 };
 
-template <>
-struct Wire<false> {                      // fp32 wire: 4 elements per vec
+struct LaneF32 {                          // fp32 wire: 4 elements per vec
+  using Acc = float;
   static constexpr int kElems = 4;
+  static constexpr bool kF32Local = false, kNvls = true;
   template <int OP>
   __device__ static __forceinline__ void zero(float* a) { a[0] = a[1] = a[2] = a[3] = Op<OP>::kIdentity; }
   template <int OP>
@@ -93,9 +100,10 @@ struct Wire<false> {                      // fp32 wire: 4 elements per vec
                       __float_as_uint(Op<OP>::fin(a[2], s)), __float_as_uint(Op<OP>::fin(a[3], s)));
   }
 };
-template <>
-struct Wire<true> {                       // bf16 wire: 8 elements per vec, fp32 accumulation
+struct LaneBF16 {                         // bf16 wire: 8 elements per vec, fp32 accumulation
+  using Acc = float;
   static constexpr int kElems = 8;
+  static constexpr bool kF32Local = true, kNvls = true;
   template <int OP>
   __device__ static __forceinline__ void zero(float* a) {
 #pragma unroll
@@ -117,10 +125,153 @@ struct Wire<true> {                       // bf16 wire: 8 elements per vec, fp32
   }
 };
 
-// local tensor <-> wire vec (local dtype is either the wire dtype or fp32)
-template <bool BF16>
+__device__ __forceinline__ float f16lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xffffu))); }
+__device__ __forceinline__ float f16hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+  __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
+struct LaneF16 {                          // fp16 wire: 8 elements per vec, fp32 accumulation, one RN-even rounding at the end
+  using Acc = float;
+  static constexpr int kElems = 8;
+  static constexpr bool kF32Local = false, kNvls = false;
+  template <int OP>
+  __device__ static __forceinline__ void zero(float* a) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a[i] = Op<OP>::kIdentity;
+  }
+  template <int OP>
+  __device__ static __forceinline__ void add(float* a, uint4 v) {
+    const float t[8] = {f16lo(v.x), f16hi(v.x), f16lo(v.y), f16hi(v.y), f16lo(v.z), f16hi(v.z), f16lo(v.w), f16hi(v.w)};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a[i] = Op<OP>::combine(a[i], t[i]);
+  }
+  template <int OP>
+  __device__ static __forceinline__ uint4 pack(const float* a, float) {
+    return make_uint4(pack_f16x2(a[0], a[1]), pack_f16x2(a[2], a[3]), pack_f16x2(a[4], a[5]), pack_f16x2(a[6], a[7]));
+  }
+};
+
+// fp64: 2 lanes, combined in fp64.  MAX / MIN are IEEE 754-2019 maximum / minimum by hand (PTX has no max.NaN.f64): NaN if
+// either term is NaN, returned as 0x7FFFFFFFFFFFFFFF like the fp32 kernels' 0x7FFFFFFF, and -0 < +0.
+struct LaneF64 {
+  using Acc = double;
+  static constexpr int kElems = 2;
+  static constexpr bool kF32Local = false, kNvls = false;
+  template <int OP>
+  __device__ static __forceinline__ double combine(double a, double b) {
+    if constexpr (OP == kSum) return a + b;
+    else if constexpr (OP == kProd) return a * b;
+    else {
+      const unsigned long long ia = __double_as_longlong(a), ib = __double_as_longlong(b);
+      const unsigned long long kAbs = 0x7FFFFFFFFFFFFFFFull, kInf = 0x7FF0000000000000ull;
+      if ((ia & kAbs) > kInf || (ib & kAbs) > kInf) return __longlong_as_double((long long)kAbs);
+      if (a == b) return __longlong_as_double((long long)(OP == kMax ? ia & ib : ia | ib));   // +-0: the sign decides
+      return (OP == kMax ? a > b : a < b) ? a : b;
+    }
+  }
+  template <int OP>
+  __device__ static __forceinline__ void zero(double* a) {
+    a[0] = a[1] = OP == kSum ? 0.0 : OP == kProd ? 1.0 : OP == kMax ? -__builtin_huge_val() : __builtin_huge_val();
+  }
+  template <int OP>
+  __device__ static __forceinline__ void add(double* a, uint4 v) {
+    double t[2];
+    memcpy(t, &v, 16);
+    a[0] = combine<OP>(a[0], t[0]);
+    a[1] = combine<OP>(a[1], t[1]);
+  }
+  template <int OP>
+  __device__ static __forceinline__ uint4 pack(const double* a, float) {
+    uint4 v;
+    memcpy(&v, a, 16);
+    return v;
+  }
+};
+
+// int32 / int64: two's-complement lanes (4 or 2 per vec).  SUM and PRODUCT wrap mod 2^bits (unsigned arithmetic, as NCCL
+// does), MAX / MIN compare signed.
+template <class U, class S>
+struct LaneInt {
+  using Acc = U;
+  static constexpr int kElems = 16 / sizeof(U);
+  static constexpr bool kF32Local = false, kNvls = false;
+  template <int OP>
+  __device__ static __forceinline__ U combine(U a, U b) {
+    if constexpr (OP == kSum) return a + b;
+    else if constexpr (OP == kProd) return a * b;
+    else if constexpr (OP == kMax) return (S)a > (S)b ? a : b;
+    else return (S)a < (S)b ? a : b;
+  }
+  template <int OP>
+  __device__ static __forceinline__ void zero(U* a) {
+    const U top = (U)1 << (8 * sizeof(U) - 1);                            // the most negative value
+#pragma unroll
+    for (int i = 0; i < kElems; ++i) a[i] = OP == kSum ? (U)0 : OP == kProd ? (U)1 : OP == kMax ? top : top - 1;
+  }
+  template <int OP>
+  __device__ static __forceinline__ void add(U* a, uint4 v) {
+    U t[kElems];
+    memcpy(t, &v, 16);
+#pragma unroll
+    for (int i = 0; i < kElems; ++i) a[i] = combine<OP>(a[i], t[i]);
+  }
+  template <int OP>
+  __device__ static __forceinline__ uint4 pack(const U* a, float) {
+    uint4 v;
+    memcpy(&v, a, 16);
+    return v;
+  }
+};
+using LaneI32 = LaneInt<uint32_t, int32_t>;
+using LaneI64 = LaneInt<unsigned long long, long long>;
+
+// int8 / uint8 (and bool): 16 bytes as four packed 32-bit words of byte SIMD.  SUM (__vadd4) and PRODUCT (per byte) wrap
+// mod 256 and are the same bits for both signs, so uint8 takes the int8 instances for them; MAX / MIN compare signed or
+// unsigned bytes.
+template <bool SIGNED>
+struct LaneI8 {
+  using Acc = uint32_t;
+  static constexpr int kElems = 4;
+  static constexpr bool kF32Local = false, kNvls = false;
+  template <int OP>
+  __device__ static __forceinline__ uint32_t combine(uint32_t a, uint32_t b) {
+    if constexpr (OP == kSum) {
+      return __vadd4(a, b);
+    } else if constexpr (OP == kProd) {
+      uint32_t p[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) p[i] = __byte_perm(a, 0u, 0x4440u + i) * __byte_perm(b, 0u, 0x4440u + i);
+      return __byte_perm(__byte_perm(p[0], p[1], 0x0040u), __byte_perm(p[2], p[3], 0x0040u), 0x5410u);
+    } else {
+      uint32_t m[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {                                  // byte i, sign- or zero-extended to 32 bits
+        const uint32_t sel = SIGNED ? (0x8880u | (i << 12) | (i << 8) | (i << 4)) + i : 0x4440u + i;
+        const uint32_t x = __byte_perm(a, 0u, sel), y = __byte_perm(b, 0u, sel);
+        m[i] = OP == kMax ? (SIGNED ? (uint32_t)max((int)x, (int)y) : max(x, y)) : (SIGNED ? (uint32_t)min((int)x, (int)y) : min(x, y));
+      }
+      return __byte_perm(__byte_perm(m[0], m[1], 0x0040u), __byte_perm(m[2], m[3], 0x0040u), 0x5410u);
+    }
+  }
+  template <int OP>
+  __device__ static __forceinline__ void zero(uint32_t* a) {
+    a[0] = a[1] = a[2] = a[3] = OP == kSum ? 0u : OP == kProd ? 0x01010101u
+                              : OP == kMax ? (SIGNED ? 0x80808080u : 0u) : (SIGNED ? 0x7F7F7F7Fu : 0xFFFFFFFFu);
+  }
+  template <int OP>
+  __device__ static __forceinline__ void add(uint32_t* a, uint4 v) {
+    a[0] = combine<OP>(a[0], v.x); a[1] = combine<OP>(a[1], v.y); a[2] = combine<OP>(a[2], v.z); a[3] = combine<OP>(a[3], v.w);
+  }
+  template <int OP>
+  __device__ static __forceinline__ uint4 pack(const uint32_t* a, float) { return make_uint4(a[0], a[1], a[2], a[3]); }
+};
+
+// local tensor <-> wire vec (local dtype is either the wire dtype or, on a kF32Local wire, fp32)
+template <class L>
 __device__ __forceinline__ uint4 load_local_as_wire(const void* base, size_t vec, bool local_f32) {
-  if (!BF16 || !local_f32) return ld_cg_v4(reinterpret_cast<const uint4*>(base) + vec);
+  if (!L::kF32Local || !local_f32) return ld_cg_v4(reinterpret_cast<const uint4*>(base) + vec);
   const uint4 a = ld_cg_v4(reinterpret_cast<const uint4*>(base) + 2 * vec);
   const uint4 b = ld_cg_v4(reinterpret_cast<const uint4*>(base) + 2 * vec + 1);
   return make_uint4(pack_bf16x2(__uint_as_float(a.x), __uint_as_float(a.y)),
@@ -128,10 +279,12 @@ __device__ __forceinline__ uint4 load_local_as_wire(const void* base, size_t vec
                     pack_bf16x2(__uint_as_float(b.x), __uint_as_float(b.y)),
                     pack_bf16x2(__uint_as_float(b.z), __uint_as_float(b.w)));
 }
-template <bool BF16, int OP>
-__device__ __forceinline__ void store_acc_local(void* base, size_t vec, const float* acc, float s, bool local_f32) {
-  if (!BF16 || !local_f32 || OP != kSum) {
-    st_cg_v4(reinterpret_cast<uint4*>(base) + vec, Wire<BF16>::template pack<OP>(acc, s));
+template <class L, int OP>
+__device__ __forceinline__ void store_acc_local(void* base, size_t vec, const typename L::Acc* acc, float s, bool local_f32) {
+  if constexpr (!L::kF32Local) {
+    st_cg_v4(reinterpret_cast<uint4*>(base) + vec, L::template pack<OP>(acc, s));
+  } else if (!local_f32 || OP != kSum) {
+    st_cg_v4(reinterpret_cast<uint4*>(base) + vec, L::template pack<OP>(acc, s));
   } else {  // bf16 wire, fp32 local (SUM only): keep the fp32 accumulator precision
     st_cg_v4(reinterpret_cast<uint4*>(base) + 2 * vec,
              make_uint4(__float_as_uint(acc[0] * s), __float_as_uint(acc[1] * s), __float_as_uint(acc[2] * s),
@@ -141,9 +294,9 @@ __device__ __forceinline__ void store_acc_local(void* base, size_t vec, const fl
                         __float_as_uint(acc[7] * s)));
   }
 }
-template <bool BF16>
+template <class L>
 __device__ __forceinline__ void store_wire_local(void* base, size_t vec, uint4 w, bool local_f32) {
-  if (!BF16 || !local_f32) {
+  if (!L::kF32Local || !local_f32) {
     st_cg_v4(reinterpret_cast<uint4*>(base) + vec, w);
   } else {
     st_cg_v4(reinterpret_cast<uint4*>(base) + 2 * vec,
@@ -191,9 +344,9 @@ constexpr bool kFromRoot = OP == kBcast || OP == kScatter;
 // ------------------------------------------------------------------------------------------ one-shot
 // Reductions read vector v of every rank; BCAST reads it from the root only; GATHER reads it from its owner v / seg (a gather:
 // on the root only); SCATTER: rank r reads the seg vectors of slot r from the root.
-template <bool BF16, int OP, bool ROOT>
+template <class L, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
-  using W = Wire<BF16>;
+  using W = L;
   constexpr bool kRaw = OP >= kBcast;
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
@@ -204,7 +357,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
   if (a.src != nullptr && (!kFromRoot<OP> || rank == a.root)) {
     uint4* stage = reinterpret_cast<uint4*>(a.bufs.p[rank]) + (OP == kGather ? (size_t)rank * seg : 0);
     for (size_t v = first; v < (OP == kGather ? seg : a.n_vec); v += stride)
-      st_cg_v4(stage + v, load_local_as_wire<BF16>(a.src, v, a.src_f32));
+      st_cg_v4(stage + v, load_local_as_wire<L>(a.src, v, a.src_f32));
   }
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's data is in place
   const bool inplace = (a.dst == nullptr);
@@ -214,7 +367,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
   // block-uniform trip count (the in-place variant has a barrier inside the loop); identical on every rank
   for (size_t base0 = (size_t)blockIdx.x * kThreads; base0 < n_out; base0 += stride * kUnroll) {
     const size_t base = base0 + threadIdx.x;
-    float acc[kUnroll][W::kElems];
+    typename W::Acc acc[kUnroll][W::kElems];
     uint4 raw[kUnroll][B2_MAX_RANKS];
     if constexpr (kRaw) {
 #pragma unroll
@@ -247,7 +400,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
       const size_t v = base + (size_t)u * stride;
       if (v < n_out && store) {
         if constexpr (kRaw) st_cg_v4(reinterpret_cast<uint4*>(out) + v, raw[u][0]);
-        else store_acc_local<BF16, OP>(out, v, acc[u], a.scale, out_f32);
+        else store_acc_local<L, OP>(out, v, acc[u], a.scale, out_f32);
       }
     }
   }
@@ -259,9 +412,9 @@ __global__ void __launch_bounds__(kThreads) allreduce_oneshot_kernel(ARArgs a) {
 // Slice s = vectors [s*slice, (s+1)*slice) is reduced by rank s and pushed to every rank (a reduce pushes it to the root
 // only).  BCAST: rank s loads slice s from the root and pushes it; GATHER: rank s pushes its own input, staged at slice s (a
 // gather: to the root only); SCATTER: the root pushes slice s of its input into rank s's slice s, and rank s copies it out.
-template <bool BF16, bool NVLS, int OP, bool ROOT>
+template <class L, bool NVLS, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
-  using W = Wire<BF16>;
+  using W = L;
   constexpr bool kRaw = OP >= kBcast;
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
@@ -274,7 +427,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
       for (size_t j = first; j < slice; j += stride) {
         const size_t v = (size_t)s * slice + j;
         st_cg_v4(reinterpret_cast<uint4*>(a.bufs.p[rank]) + v,
-                 load_local_as_wire<BF16>(a.src, OP == kGather ? j : v, a.src_f32));
+                 load_local_as_wire<L>(a.src, OP == kGather ? j : v, a.src_f32));
       }
     }
   }
@@ -308,7 +461,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
         const size_t j = base + (size_t)u * stride;
         if (j < slice) {
           const uint4* p = reinterpret_cast<const uint4*>(a.mc) + off + j;
-          if (BF16) {
+          if (std::is_same<L, LaneBF16>::value) {   // only the fp32 and bf16 lanes reach NVLS
             red[u] = multimem_ld_reduce_bf16x8(p);
           } else {
             float4 f = multimem_ld_reduce_f32x4(p);
@@ -320,7 +473,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
       for (int u = 0; u < U; ++u) {
         const size_t j = base + (size_t)u * stride;
         if (j < slice) {
-          float acc[W::kElems];
+          typename W::Acc acc[W::kElems];
           W::template zero<OP>(acc);
           W::template add<OP>(acc, red[u]);
           multimem_st_v4(reinterpret_cast<uint4*>(a.mc) + off + j, W::template pack<OP>(acc, a.scale));
@@ -347,7 +500,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
           if constexpr (kRaw) {
             o = raw[u][0];
           } else {
-            float acc[W::kElems];
+            typename W::Acc acc[W::kElems];
             W::template zero<OP>(acc);
 #pragma unroll
             for (int r = 0; r < B2_MAX_RANKS; ++r)
@@ -367,7 +520,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
       if (OP == kScatter && s != rank) continue;
       for (size_t j = first; j < slice; j += stride) {
         const size_t v = (size_t)s * slice + j;
-        store_wire_local<BF16>(a.dst, OP == kScatter ? j : v, ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[rank]) + v),
+        store_wire_local<L>(a.dst, OP == kScatter ? j : v, ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[rank]) + v),
                                a.dst_f32);
       }
     }
@@ -388,9 +541,9 @@ __global__ void __launch_bounds__(kThreads) allreduce_twoshot_kernel(ARArgs a) {
 // Every op pushes and waits for the same lines: BCAST keeps the root's line (the others are the acknowledgements the parity
 // argument needs), GATHER stores source r's line at vector r * n_vec / world instead of combining it (a gather: on the root
 // only), and SCATTER is BCAST except that the root's line to rank r carries segment r of its input.
-template <bool BF16, int OP, bool ROOT>
+template <class L, int OP, bool ROOT>
 __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
-  using W = Wire<BF16>;
+  using W = L;
   const int rank = a.rank, world = a.world;
   const uint32_t epoch = barrier_epoch_load(a.sig, rank) + 1u;
   const uint32_t flag = epoch == 0u ? 1u : epoch;                     // 0 is "never written"
@@ -407,7 +560,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
     // SCATTER: the root's own segment; a non-root reads no input (its src may be any size) and pushes zeros
     const uint4 mine = OP == kScatter && rank != a.root
                            ? make_uint4(0u, 0u, 0u, 0u)
-                           : load_local_as_wire<BF16>(in_local, OP == kScatter ? (size_t)rank * n_push + v : v, in_f32);
+                           : load_local_as_wire<L>(in_local, OP == kScatter ? (size_t)rank * n_push + v : v, in_f32);
     const uint4 l0 = make_uint4(mine.x, flag, mine.y, flag), l1 = make_uint4(mine.z, flag, mine.w, flag);
     const size_t line = ((par * (size_t)world + (size_t)rank) * a.ll_cap + v) * 2;
 #pragma unroll
@@ -417,7 +570,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
         if (r >= world) r -= world;
         uint4* d = reinterpret_cast<uint4*>(a.inbox.p[r]) + line;
         if constexpr (OP == kScatter) {                               // the root's line to rank r carries segment r
-          const uint4 w = rank == a.root ? load_local_as_wire<BF16>(in_local, (size_t)r * n_push + v, in_f32) : mine;
+          const uint4 w = rank == a.root ? load_local_as_wire<L>(in_local, (size_t)r * n_push + v, in_f32) : mine;
           st_volatile_v4(d, make_uint4(w.x, flag, w.y, flag));
           st_volatile_v4(d + 1, make_uint4(w.z, flag, w.w, flag));
         } else {
@@ -426,7 +579,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
         }
       }
     }
-    float acc[W::kElems];
+    typename W::Acc acc[W::kElems];
     if constexpr (OP < kBcast) W::template zero<OP>(acc);
     uint4 kept = mine;                                                // BCAST / SCATTER: the root's vector
     const uint4* in = reinterpret_cast<const uint4*>(a.inbox.p[rank]);
@@ -462,7 +615,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
     }
     if constexpr (kFromRoot<OP>) st_cg_v4(reinterpret_cast<uint4*>(out) + v, kept);
     else if constexpr (OP != kGather) {
-      if (store) store_acc_local<BF16, OP>(out, v, acc, a.scale, out_f32);
+      if (store) store_acc_local<L, OP>(out, v, acc, a.scale, out_f32);
     }
   }
   __syncthreads();
@@ -480,25 +633,41 @@ __global__ void __launch_bounds__(32) barrier_kernel(SignalPads sig, int rank, i
 
 namespace b2 {
 
-template <bool BF16, int OP, bool ROOT>
+template <class L, int OP, bool ROOT>
 void launch_kernel(int variant, dim3 grid, const ARArgs& a, cudaStream_t stream) {
-  if (variant == 0) allreduce_oneshot_kernel<BF16, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
-  else if (variant == 1) allreduce_twoshot_kernel<BF16, false, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
-  else if (variant == 3) allreduce_ll_kernel<BF16, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
-  else if constexpr (OP == kSum && !ROOT) allreduce_twoshot_kernel<BF16, true, kSum, false><<<grid, kThreads, 0, stream>>>(a);
+  if (variant == 0) allreduce_oneshot_kernel<L, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if (variant == 1) allreduce_twoshot_kernel<L, false, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if (variant == 3) allreduce_ll_kernel<L, OP, ROOT><<<grid, kThreads, 0, stream>>>(a);
+  else if constexpr (OP == kSum && !ROOT && L::kNvls) allreduce_twoshot_kernel<L, true, kSum, false><<<grid, kThreads, 0, stream>>>(a);
+}
+
+template <class L, int OP>
+void launch_lane(int variant, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+  if (a.root >= 0) launch_kernel<L, OP, true>(variant, grid, a, stream);
+  else launch_kernel<L, OP, false>(variant, grid, a, stream);
 }
 
 template <int OP>
-void launch_op(int variant, int bf16, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+void launch_op(int variant, int dtype, dim3 grid, const ARArgs& a, cudaStream_t stream) {
   if constexpr (OP < kBcast) {
-    if (a.root >= 0) return bf16 ? launch_kernel<true, OP, true>(variant, grid, a, stream)
-                                 : launch_kernel<false, OP, true>(variant, grid, a, stream);
-    if (bf16) return launch_kernel<true, OP, false>(variant, grid, a, stream);
+    switch (dtype) {
+      case kBF16: return launch_lane<LaneBF16, OP>(variant, grid, a, stream);
+      case kF16: return launch_lane<LaneF16, OP>(variant, grid, a, stream);
+      case kF64: return launch_lane<LaneF64, OP>(variant, grid, a, stream);
+      case kI32: return launch_lane<LaneI32, OP>(variant, grid, a, stream);
+      case kI64: return launch_lane<LaneI64, OP>(variant, grid, a, stream);
+      case kI8: return launch_lane<LaneI8<true>, OP>(variant, grid, a, stream);
+      case kU8:
+      case kBool:                             // SUM / PRODUCT wrap to the same bits for both signs: one instance
+        if constexpr (OP == kSum || OP == kProd) return launch_lane<LaneI8<true>, OP>(variant, grid, a, stream);
+        else return launch_lane<LaneI8<false>, OP>(variant, grid, a, stream);
+      default: return launch_lane<LaneF32, OP>(variant, grid, a, stream);
+    }
   }
   if constexpr (OP == kGather) {
-    if (a.root >= 0) return launch_kernel<false, kGather, true>(variant, grid, a, stream);
+    if (a.root >= 0) return launch_kernel<LaneF32, kGather, true>(variant, grid, a, stream);
   }
-  launch_kernel<false, OP, false>(variant, grid, a, stream);
+  launch_kernel<LaneF32, OP, false>(variant, grid, a, stream);
 }
 
 }  // namespace b2
@@ -508,22 +677,27 @@ extern "C" {
 
 // variant: 0 one-shot, 1 two-shot, 2 NVLS, 3 LL (needs inbox / ll_cap).  op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN, 4 broadcast
 // from `root`, 5 all-gather, or with root >= 0 gather to `root`, 6 scatter from `root`; a reduction with root >= 0 is a
-// reduce to that rank.  Returns cudaError_t as int; cudaErrorInvalidValue, without a launch, for an unknown variant or op, a
-// world outside 1..8, a rank outside [0, world), a root outside [-1, world) (a broadcast and a scatter need one), a scale
-// other than 1, fp32 locals over a bf16 wire or NVLS for any op but SUM, a bf16 wire for the raw moves, a two-shot / NVLS /
-// gather / scatter n_vec that is not a multiple of world (the remainder would be left out) or an LL message larger than the
-// inbox.
-int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
-                        const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
-                        int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root,
-                        cudaStream_t stream) {
+// reduce to that rank.  dtype: the wire dtype of a reduction, 0 fp32, 1 bf16 (the locals may be fp32 for SUM), 2 fp16,
+// 3 fp64, 4 int8, 5 uint8, 6 int32, 7 int64, 8 bool (the uint8 ops; the caller maps a bool SUM to MAX); 0 for the raw moves.
+// Returns cudaError_t as int; cudaErrorInvalidValue, without a launch, for an unknown variant, op or dtype, a world outside
+// 1..8, a rank outside [0, world), a root outside [-1, world) (a broadcast and a scatter need one), a scale other than 1,
+// fp32 locals over a bf16 wire or NVLS for any op but SUM, a scale, fp32 locals or NVLS for any dtype but fp32 / bf16, a bool
+// SUM, a dtype other than 0 for the raw moves, a two-shot / NVLS / gather / scatter n_vec that is not a multiple of world (the
+// remainder would be left out) or an LL message larger than the inbox.
+int b2_allreduce_dtype_launch(int variant, int dtype, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
+                              const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
+                              int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root,
+                              cudaStream_t stream) {
   if (variant < 0 || variant > 3 || world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world)
     return (int)cudaErrorInvalidValue;
   if (op < b2::kSum || op > b2::kScatter || root < -1 || root >= world) return (int)cudaErrorInvalidValue;
+  if (dtype < b2::kF32 || dtype > b2::kBool) return (int)cudaErrorInvalidValue;
   if ((op == b2::kBcast || op == b2::kScatter) && root < 0) return (int)cudaErrorInvalidValue;
   if (op != b2::kSum && (scale != 1.f || src_f32 || dst_f32)) return (int)cudaErrorInvalidValue;
   if (variant == 2 && (op != b2::kSum || root >= 0)) return (int)cudaErrorInvalidValue;   // NVLS: the SUM all-reduce only
-  if (op >= b2::kBcast && bf16) return (int)cudaErrorInvalidValue;
+  if (op >= b2::kBcast && dtype != b2::kF32) return (int)cudaErrorInvalidValue;
+  if (dtype >= b2::kF16 && (scale != 1.f || src_f32 || dst_f32 || variant == 2)) return (int)cudaErrorInvalidValue;
+  if (dtype == b2::kBool && op == b2::kSum) return (int)cudaErrorInvalidValue;
   const bool segmented = op == b2::kGather || op == b2::kScatter;          // one segment of n_vec / world per rank
   if ((variant == 1 || variant == 2 || segmented) && n_vec % (size_t)world != 0)
     return (int)cudaErrorInvalidValue;                                     // slice = n_vec / world
@@ -552,15 +726,24 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::S
   if (blocks > cap) blocks = cap;
   const dim3 grid((unsigned)blocks);
   switch (op) {
-    case b2::kSum: b2::launch_op<b2::kSum>(variant, bf16, grid, a, stream); break;
-    case b2::kProd: b2::launch_op<b2::kProd>(variant, bf16, grid, a, stream); break;
-    case b2::kMax: b2::launch_op<b2::kMax>(variant, bf16, grid, a, stream); break;
-    case b2::kMin: b2::launch_op<b2::kMin>(variant, bf16, grid, a, stream); break;
-    case b2::kBcast: b2::launch_op<b2::kBcast>(variant, bf16, grid, a, stream); break;
-    case b2::kGather: b2::launch_op<b2::kGather>(variant, bf16, grid, a, stream); break;
-    default: b2::launch_op<b2::kScatter>(variant, bf16, grid, a, stream); break;
+    case b2::kSum: b2::launch_op<b2::kSum>(variant, dtype, grid, a, stream); break;
+    case b2::kProd: b2::launch_op<b2::kProd>(variant, dtype, grid, a, stream); break;
+    case b2::kMax: b2::launch_op<b2::kMax>(variant, dtype, grid, a, stream); break;
+    case b2::kMin: b2::launch_op<b2::kMin>(variant, dtype, grid, a, stream); break;
+    case b2::kBcast: b2::launch_op<b2::kBcast>(variant, dtype, grid, a, stream); break;
+    case b2::kGather: b2::launch_op<b2::kGather>(variant, dtype, grid, a, stream); break;
+    default: b2::launch_op<b2::kScatter>(variant, dtype, grid, a, stream); break;
   }
   return (int)cudaGetLastError();
+}
+
+// The fp32 / bf16 launcher of the collectives before the dtype code: `bf16` selects the bf16 wire.
+int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::SignalPads* sig, void* mc,
+                        const void* src, int src_f32, void* dst, int dst_f32, size_t n_vec, float scale,
+                        int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root,
+                        cudaStream_t stream) {
+  return b2_allreduce_dtype_launch(variant, bf16 ? b2::kBF16 : b2::kF32, bufs, sig, mc, src, src_f32, dst, dst_f32, n_vec,
+                                   scale, rank, world, max_blocks, inbox, ll_cap, op, root, stream);
 }
 
 int b2_barrier_launch(const b2::SignalPads* sig, int rank, int world, cudaStream_t stream) {

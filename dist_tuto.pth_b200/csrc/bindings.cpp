@@ -39,6 +39,9 @@ int b2_ipc_free(unsigned long long ptr);
 int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const SignalPadsH* sig, void* mc, const void* src,
                         int src_f32, void* dst, int dst_f32, size_t n_vec, float scale, int rank, int world,
                         int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root, cudaStream_t stream);
+int b2_allreduce_dtype_launch(int variant, int dtype, const PeerPtrs* bufs, const SignalPadsH* sig, void* mc, const void* src,
+                              int src_f32, void* dst, int dst_f32, size_t n_vec, float scale, int rank, int world,
+                              int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root, cudaStream_t stream);
 int b2_barrier_launch(const SignalPadsH* sig, int rank, int world, cudaStream_t stream);
 void b2_p2p_config(int* ctas, int* slots, size_t* chunk, int* pad_words);
 int b2_p2p_send_launch(const PeerPtrs* box, const SignalPadsH* sig, const void* src, size_t nbytes, int rank, int peer,
@@ -301,10 +304,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // op: 0 SUM, 1 PRODUCT, 2 MAX, 3 MIN (reductions; root >= 0 stores on that rank only), 4 broadcast from root, 5 all-gather
   // (n_vec counts the output, world x the per-rank input; root >= 0: gather to that rank), 6 scatter from root (n_vec counts
   // the root's input, world x the per-rank output).  The raw moves take any dtype and copy bytes.
+  // dtype (reductions): the kernels' wire dtype code, 0 fp32, 1 bf16, 2 fp16, 3 fp64, 4 int8, 5 uint8, 6 int32, 7 int64,
+  // 8 bool; -1 takes fp32 or bf16 from `bf16`.  Codes 2..8 take locals of that dtype only, no scale, no bf16 wire and no NVLS.
+  static const torch::ScalarType kDtypes[] = {torch::kFloat32, torch::kBFloat16, torch::kFloat16, torch::kFloat64, torch::kInt8,
+                                              torch::kUInt8, torch::kInt32, torch::kInt64, torch::kBool};
   auto collective = [](const char* what, int op, int variant, bool bf16, const std::vector<unsigned long long>& bufs,
                        const std::vector<unsigned long long>& sigs, unsigned long long mc, const c10::optional<torch::Tensor>& src,
                        const c10::optional<torch::Tensor>& dst, size_t n_vec, double scale, int root, int rank, int world,
-                       int max_blocks, const std::vector<unsigned long long>& inbox, size_t ll_cap) {
+                       int max_blocks, const std::vector<unsigned long long>& inbox, size_t ll_cap, int dtype = -1) {
     check_world(rank, world, what);
     TORCH_CHECK(variant >= 0 && variant <= 3, what, ": variant must be 0 (one-shot), 1 (two-shot), 2 (NVLS) or 3 (LL), got ",
                 variant);
@@ -322,24 +329,41 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(variant != 2 || (op == 0 && root < 0), what, ": NVLS runs the SUM all-reduce only");
     TORCH_CHECK(variant != 3 || (segmented ? n_vec / world : n_vec) <= ll_cap, what, ": LL pushes ",
                 segmented ? n_vec / world : n_vec, " vectors per rank, more than the inbox holds (", ll_cap, ")");
+    TORCH_CHECK(dtype >= -1 && dtype <= 8, what, ": dtype must be -1 (fp32 / bf16 from the bf16 flag) or a code in 0..8, got ",
+                dtype);
+    TORCH_CHECK(dtype < 0 || dtype >= 2 || dtype == (int)bf16, what, ": dtype ", dtype, " contradicts the bf16 flag (",
+                bf16, ")");
+    const bool narrow = dtype >= 2;                        // a dtype beyond fp32 / bf16
+    TORCH_CHECK(!narrow || !bf16, what, ": a bf16 wire is for fp32 / bf16 tensors, not dtype ", dtype);
+    TORCH_CHECK(!narrow || scale == 1.0, what, ": scale applies to fp32 / bf16 SUM only, got ", scale, " for dtype ", dtype);
+    TORCH_CHECK(!narrow || variant != 2, what, ": NVLS reduces fp32 / bf16 only, not dtype ", dtype);
+    TORCH_CHECK(dtype != 8 || op != 0, what, ": a bool SUM is a MAX (as torch.distributed maps it); pass op 2");
+    if (narrow) {
+      for (const auto* t : {&src, &dst})
+        TORCH_CHECK(!t->has_value() || (*t)->scalar_type() == kDtypes[dtype], what, ": ", t == &src ? "src" : "dst",
+                    " is ", (*t)->scalar_type(), " but dtype ", dtype, " is ", kDtypes[dtype]);
+    }
     PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
     PeerPtrs ib = to_ptrs(inbox);
     const void* sp = nullptr; void* dp = nullptr; int sf = 0, df = 0;
     if (src.has_value()) { check_cuda_contig(*src, "src"); sp = src->data_ptr(); sf = src->scalar_type() == torch::kFloat32 && bf16; }
     if (dst.has_value()) { check_cuda_contig(*dst, "dst"); dp = dst->data_ptr(); df = dst->scalar_type() == torch::kFloat32 && bf16; }
     TORCH_CHECK(op == 0 || (sf == 0 && df == 0), what, ": a bf16 wire for fp32 tensors is for SUM only");
-    ck_cuda(b2_allreduce_launch(variant, bf16, &b, &s, (void*)(uintptr_t)mc, sp, sf, dp, df, n_vec, (float)scale, rank,
-                                world, max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, op, root, cur_stream()), what);
+    ck_cuda(b2_allreduce_dtype_launch(variant, dtype < 0 ? (int)bf16 : dtype, &b, &s, (void*)(uintptr_t)mc, sp, sf, dp, df,
+                                      n_vec, (float)scale, rank, world, max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, op,
+                                      root, cur_stream()), what);
   };
   m.def("allreduce", [collective](int variant, bool bf16, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
                                   unsigned long long mc, c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst,
                                   size_t n_vec, double scale, int rank, int world, int max_blocks, std::vector<unsigned long long> inbox,
-                                  size_t ll_cap, int op, int root) {
+                                  size_t ll_cap, int op, int root, int dtype) {
     TORCH_CHECK(op >= 0 && op <= 3, "allreduce: op must be 0 (SUM), 1 (PRODUCT), 2 (MAX) or 3 (MIN), got ", op);
-    collective("allreduce", op, variant, bf16, bufs, sigs, mc, src, dst, n_vec, scale, root, rank, world, max_blocks, inbox, ll_cap);
+    collective("allreduce", op, variant, bf16, bufs, sigs, mc, src, dst, n_vec, scale, root, rank, world, max_blocks, inbox, ll_cap,
+               dtype);
   }, py::arg("variant"), py::arg("bf16"), py::arg("bufs"), py::arg("sigs"), py::arg("mc"), py::arg("src"), py::arg("dst"),
      py::arg("n_vec"), py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0,
-     py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0, py::arg("op") = 0, py::arg("root") = -1);
+     py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0, py::arg("op") = 0, py::arg("root") = -1,
+     py::arg("dtype") = -1);
   m.def("broadcast", [collective](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
                                   c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int root,
                                   int rank, int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {

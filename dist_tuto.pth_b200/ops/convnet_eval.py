@@ -64,9 +64,12 @@ def _shard_tensors(dataset, rank: int, world: int) -> Tuple[torch.Tensor, torch.
 
 
 def _group_sum(t: torch.Tensor, group) -> torch.Tensor:
-    """Sum a float64 ``[3]`` tensor over the group (NCCL takes it on the device, gloo on the host)."""
+    """Sum a float64 ``[3]`` tensor over the group (NCCL or a symmetric world that reduces fp64, ``backend="b200"``, takes
+    it on the device; otherwise gloo on the host)."""
     if comm.is_initialized() and comm.get_world_size(group) > 1:
-        if t.is_cuda and dist.get_backend(comm._g(group)) != "nccl":
+        on_device = dist.get_backend(comm._g(group)) == "nccl" or comm._reduces(comm._symm_world_for(t, group), t,
+                                                                                   comm.reduce_op.SUM)
+        if t.is_cuda and not on_device:
             t = t.cpu()
         comm.all_reduce(t, group=group)
     return t

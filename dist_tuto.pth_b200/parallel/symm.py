@@ -18,8 +18,8 @@ Each allocation owns its signal pad, so collectives on different buffers may be
 in flight on different streams at once.  All collectives must be issued in the
 same order on every rank of the world (as with any communicator).
 
-Collectives: ``all_reduce_`` and ``reduce_`` (SUM, PRODUCT, MAX, MIN on fp32 /
-bf16), ``broadcast_``, ``all_gather_``, ``scatter_`` and ``gather_`` (raw
+Collectives: ``all_reduce_`` and ``reduce_`` (SUM, PRODUCT, MAX, MIN on fp32,
+bf16, fp16, fp64, int8, uint8, int32, int64 and bool), ``broadcast_``, ``all_gather_``, ``scatter_`` and ``gather_`` (raw
 bytes, any dtype).  Each call picks its kernel variant with
 :func:`plan_variant` (scatter and gather by the all-gather rule, on one rank's
 segment) and never synchronises the host.
@@ -43,7 +43,7 @@ import torch.distributed as dist
 from ..ops import _ext
 
 __all__ = ["SymmWorld", "SymmHandle", "P2PWork", "init_world", "lookup_world", "destroy_all", "VARIANTS", "COLLECTIVES",
-           "op_code", "plan_variant"]
+           "op_code", "plan_variant", "DTYPE_CODES"]
 
 PAD_BYTES = 8192                      # signal pad at the head of every allocation (B2_SIGNAL_WORDS*4 = 6016 B)
 VARIANTS = {"oneshot": 0, "twoshot": 1, "nvls": 2, "ll": 3}
@@ -61,6 +61,10 @@ def _load_table():
         return {}
 _WORLDS: Dict[object, "SymmWorld"] = {}
 _DTYPES = (torch.float32, torch.bfloat16)
+# The reductions' dtypes (torch's NCCL process group table) -> the kernels' wire dtype code (csrc/allreduce.cu).  Beyond fp32
+# and bf16 the local dtype is the wire dtype: no scale, no bf16 wire, no NVLS.
+DTYPE_CODES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.float64: 3, torch.int8: 4, torch.uint8: 5,
+               torch.int32: 6, torch.int64: 7, torch.bool: 8}
 COLLECTIVES = ("allreduce", "reduce", "broadcast", "allgather")
 _OPS = {dist.ReduceOp.SUM: 0, dist.ReduceOp.PRODUCT: 1, dist.ReduceOp.MAX: 2, dist.ReduceOp.MIN: 3}
 
@@ -389,8 +393,14 @@ class SymmWorld:
 
     # ------------------------------------------------------------------ collectives
     def supports(self, t: torch.Tensor) -> bool:
-        """Can ``all_reduce_`` / ``reduce_`` take this tensor (CUDA, this device, fp32/bf16, contiguous)?"""
+        """Can ``all_reduce_`` / ``reduce_`` take this tensor with a scale or a bf16 wire (CUDA, this device, fp32/bf16,
+        contiguous)?"""
         return t.is_cuda and t.device == self.device and t.dtype in _DTYPES and t.is_contiguous()
+
+    def supports_reduction(self, t: torch.Tensor) -> bool:
+        """Can ``all_reduce_`` / ``reduce_`` take this tensor at all (CUDA, this device, contiguous, one of
+        :data:`DTYPE_CODES`)?  The dtypes beyond :meth:`supports` take no scale and no wire conversion."""
+        return t.is_cuda and t.device == self.device and t.dtype in DTYPE_CODES and t.is_contiguous()
 
     def pick_variant(self, wire_bytes: int) -> int:
         """Message size -> kernel (0 one-shot, 1 two-shot, 2 NVLS) from the measured thresholds; ``B200DIST_AR_VARIANT``
@@ -403,14 +413,16 @@ class SymmWorld:
                             self.multicast, os.environ.get("B200DIST_AR_VARIANT"))
 
     def _launch(self, hd: SymmHandle, bf16: bool, n_vec: int, scale: float, src, dst, variant: Optional[int],
-                max_blocks: Optional[int] = None, collective: str = "allreduce", op: int = 0, root: int = -1):
+                max_blocks: Optional[int] = None, collective: str = "allreduce", op: int = 0, root: int = -1,
+                dtype: Optional[int] = None):
         """One kernel call on ``hd``.  ``n_vec``: 16-byte vectors of the message (of the output for an all-gather or a gather,
         of the root's input for a scatter, a multiple of world for those three); ``root``: local rank (-1 for the all-to-all
-        collectives)."""
+        collectives); ``dtype``: a reduction's code in :data:`DTYPE_CODES` beyond fp32 / bf16 (``None``: fp32 or bf16 by
+        ``bf16``), which NVLS cannot reduce, so it runs two-shot instead."""
         segmented = collective in ("allgather", "gather", "scatter")
         n_push = n_vec // self.world if segmented else n_vec
         v = self.plan("allgather" if segmented else collective, op, n_push * 16) if variant is None else variant
-        if v == 2 and (not hd.mc_ptr or collective != "allreduce" or op != 0):
+        if v == 2 and (not hd.mc_ptr or collective != "allreduce" or op != 0 or dtype is not None):
             v = 1
         if v == 3 and (hd.ll is None or n_push > LL_CAP_VEC):
             v = 0
@@ -426,6 +438,9 @@ class SymmWorld:
             self.C.gather(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
         elif collective == "scatter":
             self.C.scatter(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, root, self.rank, self.world, mb, *ll)
+        elif dtype is not None:
+            self.C.allreduce(v, False, hd.ptrs, hd.sig_ptrs, hd.mc_ptr, src, dst, n_vec, float(scale), self.rank,
+                             self.world, mb, *ll, op, root, dtype=dtype)
         else:
             self.C.allreduce(v, bf16, hd.ptrs, hd.sig_ptrs, hd.mc_ptr, src, dst, n_vec, float(scale), self.rank,
                              self.world, mb, *ll, op, root)
@@ -452,6 +467,9 @@ class SymmWorld:
         """In-place ``t <- scale * sum_ranks t`` with the fused peer-memory kernels; ``op`` PRODUCT / MAX / MIN combine
         instead of summing (fp32 in rank order, IEEE maximum / minimum: NaN wins, -0 < +0) and take no scale.
 
+        Beyond fp32 / bf16, ``t`` may be fp16 (fp32 accumulator, rounded once), fp64, int8, uint8, int32, int64 (wrapping
+        SUM / PRODUCT, as NCCL) or bool (SUM is MAX, as torch.distributed maps it); those take no scale and no ``wire``.
+
         ``handle`` given and ``t`` aliasing its data  -> zero-copy symmetric path;
         otherwise ``t`` is staged through a world-owned symmetric buffer with the
         copy-in / copy-out fused into the same kernel.  ``wire=torch.bfloat16``
@@ -471,8 +489,11 @@ class SymmWorld:
             raise ValueError(f"the fused reductions are SUM, PRODUCT, MAX and MIN, got {op!r}")
         if code != 0 and scale != 1.0:
             raise ValueError("scale applies to SUM only")
+        if not self.supports_reduction(t):
+            raise TypeError(f"fused all_reduce needs a contiguous CUDA tensor on this device of one of "
+                            f"{[str(d).replace('torch.', '') for d in DTYPE_CODES]}, got {t.dtype}")
         if not self.supports(t):
-            raise TypeError("fused all_reduce needs a contiguous CUDA float32/bfloat16 tensor on this device")
+            return self._reduce_same_dtype(t, scale, handle, variant, wire, max_blocks, code, root)
         if code != 0 and wire is not None and wire != t.dtype:
             raise TypeError("a bf16 wire for an fp32 tensor is for SUM only")
         if self.world == 1:
@@ -506,6 +527,37 @@ class SymmWorld:
                          kind, code, root)
             if root < 0 or root == self.rank:
                 flat.copy_(buf[:flat.numel()])
+        return t
+
+    def _reduce_same_dtype(self, t, scale, handle, variant, wire, max_blocks, code, root):
+        """The reductions beyond fp32 / bf16: the wire dtype is ``t``'s, staged through the byte staging buffer the raw
+        moves use."""
+        if scale != 1.0:
+            raise ValueError(f"scale applies to fp32 / bf16 SUM only, not to {t.dtype}")
+        if wire is not None and wire != t.dtype:
+            raise TypeError(f"a wire dtype conversion is for fp32 / bf16 tensors only, not {t.dtype}")
+        if t.dtype == torch.bool and code == 0:
+            code = 2                                           # torch.distributed's NCCL group reduces a bool SUM as MAX
+        if self.world == 1:
+            return t
+        dt = DTYPE_CODES[t.dtype]
+        kind = "reduce" if root >= 0 else "allreduce"
+        nbytes = t.numel() * t.element_size()
+        n_vec = (nbytes + 15) // 16
+        if handle is not None and t.data_ptr() == handle.ptrs[self.rank] and n_vec * 16 <= handle.nbytes:
+            self._launch(handle, False, n_vec, 1.0, None, None, variant, max_blocks, kind, code, root, dtype=dt)
+            return t
+        st = self._staging_for(torch.float32, nbytes)
+        flat = t.view(-1)
+        if nbytes % (16 * self.world) == 0 and t.data_ptr() % 16 == 0:
+            self._launch(st, False, n_vec, 1.0, flat, flat, variant, max_blocks, kind, code, root, dtype=dt)
+        else:  # ragged size: torch copies around an in-place symmetric reduction (nobody reads the padding's results)
+            raw = flat.view(torch.uint8)
+            buf = st.view(torch.uint8, st.nbytes)
+            buf[:nbytes].copy_(raw)
+            self._launch(st, False, n_vec, 1.0, None, None, variant, max_blocks, kind, code, root, dtype=dt)
+            if root < 0 or root == self.rank:
+                raw.copy_(buf[:nbytes])
         return t
 
     def broadcast_(self, t: torch.Tensor, root: int, handle: Optional[SymmHandle] = None, variant: Optional[int] = None,
