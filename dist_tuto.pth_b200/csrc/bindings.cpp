@@ -493,15 +493,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                            int64_t sample_base, bool training, double inv_bsz, double p_drop, int max_ctas, int64_t grad_stride, int cluster,
                            c10::optional<torch::Tensor> aux, py::none, c10::optional<torch::Tensor> det_partials,
                            c10::optional<torch::Tensor> factors, bool input_ready) {
+    // The kernels read params, x and aux with bulk copies and 16-byte vector loads, and write grads, det_partials and
+    // factors with 16-byte vector stores / red.add.v4: a buffer that is not 16-byte aligned would fault on the device.
+    auto check_aligned16 = [](const torch::Tensor& t, const char* what) {
+      TORCH_CHECK(((uintptr_t)t.data_ptr() & 15u) == 0, "convnet_step: ", what, " must be 16-byte aligned");
+    };
     check_cuda_contig(params, "params"); check_cuda_contig(x, "x"); check_cuda_contig(target, "target");
     TORCH_CHECK(params.scalar_type() == torch::kFloat32 && params.numel() >= b2_convnet_npar(), "params: flat fp32 [21848]");
     TORCH_CHECK(target.scalar_type() == torch::kInt64, "target: int64");
+    check_aligned16(params, "params"); check_aligned16(x, "x");
     const bool u8 = x.scalar_type() == torch::kUInt8;
     TORCH_CHECK(u8 || x.scalar_type() == torch::kFloat32, "x: float32 (normalised) or uint8 (raw)");
     const int B = (int)target.numel();
     TORCH_CHECK(x.numel() == (int64_t)B * 784, "x must be [B,1,28,28]");
     float* g = nullptr;
-    if (grads.has_value()) { check_cuda_contig(*grads, "grads"); TORCH_CHECK(grads->scalar_type() == torch::kFloat32 && grads->numel() >= b2_convnet_npar() + grad_stride); g = grads->data_ptr<float>(); }
+    if (grads.has_value()) {
+      check_cuda_contig(*grads, "grads"); check_aligned16(*grads, "grads");
+      TORCH_CHECK(grad_stride >= 0 && grad_stride % 4 == 0, "convnet_step: grad_stride must be a non-negative multiple of 4 "
+                  "(the second bucket is written with 16-byte vectors), got ", grad_stride);
+      TORCH_CHECK(grads->scalar_type() == torch::kFloat32 && grads->numel() >= b2_convnet_npar() + grad_stride);
+      g = grads->data_ptr<float>();
+    }
     float* la = loss_acc.has_value() ? loss_acc->data_ptr<float>() : nullptr;
     float* lp = nullptr;
     if (out_logp.has_value()) { TORCH_CHECK(out_logp->numel() == (int64_t)B * 10 && out_logp->scalar_type() == torch::kFloat32); lp = out_logp->data_ptr<float>(); }
@@ -510,12 +522,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     const unsigned long long* st = step.has_value() ? reinterpret_cast<const unsigned long long*>(step->data_ptr()) : nullptr;
     c10::cuda::CUDAGuard guard(params.device());
     const float* ax = nullptr;
-    if (aux.has_value()) { TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000); ax = aux->data_ptr<float>(); }
+    if (aux.has_value()) {
+      TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000);
+      check_aligned16(*aux, "aux");
+      ax = aux->data_ptr<float>();
+    }
     float* dp = nullptr;
     if (det_partials.has_value()) {
       const int ctas = cluster > 1 ? B * cluster : (max_ctas > 0 ? std::min(B, max_ctas) : B);   // CTAs of the step grid
       TORCH_CHECK(det_partials->is_cuda() && det_partials->scalar_type() == torch::kFloat32 &&
                   det_partials->numel() >= (int64_t)std::max(1, ctas) * 21888, "det_partials: [ctas, 21888] fp32");
+      check_aligned16(*det_partials, "det_partials");
       dp = det_partials->data_ptr<float>();
     }
     float* fp = nullptr;
@@ -524,6 +541,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       TORCH_CHECK(dp != nullptr && cluster <= 1, "factors need det_partials and cluster 1");
       TORCH_CHECK(factors->is_cuda() && factors->scalar_type() == torch::kFloat32 && factors->numel() >= (int64_t)std::max(1, B) * 384,
                   "factors: [B, 384] fp32");
+      check_aligned16(*factors, "factors");
       fp = factors->data_ptr<float>();
     }
     if (cluster > 1) {
@@ -539,7 +557,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                    la, lp, mo, st, seed, sample_base, B, training, g != nullptr, (float)inv_bsz, (float)p_drop,
                                    max_ctas, grad_stride, ax, dp, fp, input_ready ? 1 : 0, cur_stream()),
             "convnet_step launch");
-  }, py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
+  }, "Fused forward (+ loss and backward when grads is given) of the ConvNet on one CTA or one 2/4/8-CTA cluster per "
+     "sample.  params, x, grads, aux, det_partials and factors must be 16-byte aligned (refused otherwise), and "
+     "grad_stride a multiple of 4.",
+     py::arg("params"), py::arg("grads"), py::arg("x"), py::arg("target"), py::arg("loss_acc"), py::arg("out_logp"),
      py::arg("mask_out"), py::arg("step"), py::arg("seed"), py::arg("sample_base"), py::arg("training"), py::arg("inv_bsz"),
      py::arg("p_drop") = 0.5, py::arg("max_ctas") = 0, py::arg("grad_stride") = 0, py::arg("cluster") = 1, py::arg("aux") = py::none(),
      // "reserved": an unused slot that takes only None, so calls passing det_partials, factors and input_ready by position

@@ -189,7 +189,9 @@ __global__ void __launch_bounds__(T, 1) convnet_step_kernel(Args a) {
   }
   if (tid == 0) { s.loss_local = 0.f; s.correct_local = 0; }
   const unsigned long long step = a.step ? *a.step : 0ull;
-  const float keep_scale = 1.f / (1.f - a.p_drop);
+  // correctly rounded 1 / (1 - p): --use_fast_math would turn the division into the approximate MUFU reciprocal, 1 ulp off
+  // for some p (0.9), and the scale would differ from the one the host and the other engines apply
+  const float keep_scale = __frcp_rn(1.f - a.p_drop);
   // this step's gradient bucket (double-buffered: see sgd.cu); fc1.weight's share goes there from S6, the rest in the flush
   float* const gdst = a.backward ? a.grads + (size_t)(step & 1ull) * (size_t)a.grad_stride : nullptr;
   // The barrier that ends S0 publishes the mbarrier initialisation and the scattered conv2.weight before any phase reads

@@ -210,7 +210,7 @@ bt_conv2_fwd(const __grid_constant__ CUtensorMap map_p1, const __grid_constant__
   // ========================================================== 25 taps = 25 descriptors over the image, then bias,
   // dropout2d, 2x2 max-pool, relu.  Warpgroup h owns accumulator rows 64h..64h+63 = row groups (oy*2 + b) 8h..8h+7.
   const int h = wg - 1, e = threadIdx.x - 128;
-  const float keep = 1.f / (1.f - cm.p_drop);
+  const float keep = __frcp_rn(1.f - cm.p_drop);   // correctly rounded, like bt_route's host-side scale (see convnet.cu)
   const unsigned long long step = cm.step ? *cm.step : 0ull;
   tc::mbar_wait(&s.wfull, 0);
   uint32_t it = 0;
@@ -286,7 +286,7 @@ __global__ void __launch_bounds__(128) bt_head(const float* __restrict__ params,
   if (threadIdx.x < 10) b4s[threadIdx.x] = params[B4 + threadIdx.x];
   __syncthreads();
   const int tid = threadIdx.x, b = blockIdx.x * 128 + tid;
-  const float keep = 1.f / (1.f - cm.p_drop);
+  const float keep = __frcp_rn(1.f - cm.p_drop);   // correctly rounded, like bt_route's host-side scale (see convnet.cu)
   const unsigned long long step = cm.step ? *cm.step : 0ull;
   float nll = 0.f, corr = 0.f;
   if (b < cm.B) {

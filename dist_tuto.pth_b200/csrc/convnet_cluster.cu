@@ -138,7 +138,9 @@ __global__ void __launch_bounds__(T, 1) convnet_cluster_kernel(Args a) {
     }
   if (tid == 0) { s.loss_local = 0.f; s.correct_local = 0; }
   const unsigned long long step = a.step ? *a.step : 0ull;
-  const float keep_scale = 1.f / (1.f - a.p_drop);
+  // correctly rounded 1 / (1 - p): --use_fast_math would turn the division into the approximate MUFU reciprocal, 1 ulp off
+  // for some p (0.9), and the scale would differ from the one the host and the other engines apply
+  const float keep_scale = __frcp_rn(1.f - a.p_drop);
   cl.sync();                                       // every CTA of the cluster is running (DSMEM stores may begin)
 
   for (int b = cluster_id; b < a.B; b += n_clusters) {

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import batched_checks as BC
+import step_oracle as SO
 import dist_tuto.pth_b200 as b2
 from dist_tuto.pth_b200.ops import _ext
 from dist_tuto.pth_b200.ops import batched_reference as R
@@ -51,6 +52,7 @@ def _case(B, seed, training, u8=False, sample_base=0, step_value=3):
     if training:      # the dropout masks of this (seed, sample, step): exported by the per-sample engine (same Philox stream)
         _, _, masks = convnet_loss_and_grads(params, x, y, training=True, seed=77, step=step, sample_base=sample_base,
                                              return_masks=True)
+        assert torch.equal(masks.cpu(), SO.dropout_masks(77, sample_base, B, step_value, 0.5)), "masks != host Philox"
         m2, dm = masks[:, :20].contiguous(), masks[:, 20:70].contiguous()
     return params, xin, x, y, step, m2, dm
 

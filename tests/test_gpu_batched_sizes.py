@@ -15,6 +15,7 @@ import pytest
 import torch
 
 import batched_checks as BC
+import step_oracle as SO
 from dist_tuto.pth_b200.ops import _ext
 from dist_tuto.pth_b200.ops.convnet_batched import BatchedBuffers, BatchedTrainer
 from dist_tuto.pth_b200.ops.convnet_fused import convnet_loss_and_grads
@@ -130,7 +131,9 @@ def test_trainer_steps_match_the_model_one_at_a_time(B):
         step_t = torch.full((1,), step0, dtype=torch.int64, device=DEV)
         _, _, masks = convnet_loss_and_grads(p0, xd, yd, training=True, seed=tr.seed, step=step_t, sample_base=0,
                                              p_drop=0.5, return_masks=True)
-        loss = float(tr.loss_acc[0].item()) - loss0
+        if not torch.equal(masks.cpu(), SO.dropout_masks(tr.seed, 0, n, step0, 0.5)):
+            bad.append(f"step {k}: the per-sample engine's masks differ from the host Philox reference")
+        loss =float(tr.loss_acc[0].item()) - loss0
         with torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
             bad += [f"step {k}: {b}" for b in BC.compare_pipeline(rep, tr.bufs, p0, xd, yd, masks[:, :20].contiguous(),
                                                                   masks[:, 20:70].contiguous(), grads=grad, loss=loss)[0]]
