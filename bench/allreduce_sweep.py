@@ -15,10 +15,11 @@ Bandwidth columns:
             reported as link_GBs = link_tx / t against 770 GB/s measured peer copy.
 ``--emit-table`` writes parallel/allreduce_table.json (per-world variant thresholds) from the measured winners.
 
-``--collective {reduce,broadcast,allgather,scatter,gather}`` or ``--op {product,max,min}`` time that collective instead:
-every variant of ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the NCCL call on the same
-tensor, per size (for an all-gather, a scatter and a gather, the size of one rank's segment; the root is rank 0 and its
-list is one block).  ``--dtype {bf16,fp16,fp64,int8,uint8,int32,int64,bool}`` times the reductions (and the raw moves) on
+``--collective {reduce,broadcast,allgather,scatter,gather,reducescatter,alltoall}`` or ``--op {product,max,min}`` time
+that collective instead: every variant of ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the
+NCCL call on the same tensor, per size (for an all-gather, a scatter, a gather, a reduce-scatter and an all-to-all, the
+size of one rank's segment; the root is rank 0 and its list is one block; reduce-scatter and all-to-all have an LL and a
+pull arm only).  ``--dtype {bf16,fp16,fp64,int8,uint8,int32,int64,bool}`` times the reductions (and the raw moves) on
 a tensor of that dtype.  It compares GPUs, so it refuses to run on one.
 """
 import argparse
@@ -97,12 +98,19 @@ def body_collective(rank, size):
         outs = [torch.empty_like(t) for _ in range(size)]
         lst = list(torch.empty(size * n, dtype=dtype, device=dev).view(size, n).unbind(0)) if rank == 0 else None  # scatter / gather
         iters = 100 if s <= (1 << 20) else 20
+        whole = torch.ones(size * n, dtype=dtype, device=dev)  # reduce-scatter / all-to-all: world segments of s bytes
+        outs_whole = torch.empty_like(whole)
         row = {"bytes": s, "collective": coll, "op": ARGS.op, "dtype": ARGS.dtype}
         arms = []
-        for name, v in (("ll", 3), ("oneshot", 0), ("twoshot", 1)):
+        segmented = coll in ("reducescatter", "alltoall")     # two kernels only: LL and pull
+        for name, v in ((("ll", 3), ("pull", 0)) if segmented else (("ll", 3), ("oneshot", 0), ("twoshot", 1))):
             if name == "ll" and s > symm.LL_CAP_VEC * 16:
                 continue
-            if coll == "allreduce":
+            if coll == "reducescatter":
+                arms.append((name, lambda v=v: w.reduce_scatter_(t, whole, op, variant=v)))
+            elif coll == "alltoall":
+                arms.append((name, lambda v=v: w.all_to_all_(outs_whole, whole, variant=v)))
+            elif coll == "allreduce":
                 arms.append((name, lambda v=v: w.all_reduce_(t, variant=v, op=op)))
             elif coll == "reduce":
                 arms.append((name, lambda v=v: w.reduce_(t, 0, op, variant=v)))
@@ -117,7 +125,9 @@ def body_collective(rank, size):
         nccl = {"allreduce": lambda: dist.all_reduce(t, op=op), "reduce": lambda: dist.reduce(t, 0, op=op),
                 "broadcast": lambda: dist.broadcast(t, 0), "allgather": lambda: dist.all_gather(outs, t),
                 "scatter": lambda: dist.scatter(t, scatter_list=lst, src=0),
-                "gather": lambda: dist.gather(t, gather_list=lst, dst=0)}[coll]
+                "gather": lambda: dist.gather(t, gather_list=lst, dst=0),
+                "reducescatter": lambda: dist.reduce_scatter_tensor(t, whole, op=op),
+                "alltoall": lambda: dist.all_to_all_single(outs_whole, whole)}[coll]
         arms.append(("nccl", nccl))
         best = {}
         for order in (arms, arms[::-1]):
@@ -269,7 +279,8 @@ if __name__ == "__main__":
     ap.add_argument("--max-mb", type=int, default=1024)
     ap.add_argument("--out", default=None)
     ap.add_argument("--emit-table", action="store_true", help="write the measured variant thresholds of this world size")
-    ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather", "scatter", "gather"], default="allreduce")
+    ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather", "scatter", "gather", "reducescatter",
+                                                 "alltoall"], default="allreduce")
     ap.add_argument("--op", choices=sorted(OPS), default="sum")
     ap.add_argument("--dtype", choices=list(DTYPES), default="fp32", help="tensor dtype of the reductions")
     ARGS = ap.parse_args()

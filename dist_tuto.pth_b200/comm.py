@@ -25,6 +25,12 @@ Design (GPU-first, not a port):
     but fp32 / bf16 on a world without ``supports_reduction``, and
     ``scatter`` / ``gather`` on a world without ``scatter_`` / ``gather_``
     (the two-level world of several machines has none of the three).
+  * beyond the tutorial, torch's ``reduce_scatter_tensor`` and
+    ``reduce_scatter`` (the ops and dtypes of ``all_reduce``) and the
+    equal-segment ``all_to_all_single`` (any dtype) run on peer-memory
+    kernels of their own on such a world, and ``all_gather_into_tensor`` on
+    the all-gather's; given split sizes, ``async_op=True``, AVG, other dtypes,
+    CPU tensors and the two-level world go to torch.distributed.
   * on such a world ``send``, ``recv``, ``isend`` and ``irecv`` of a CUDA
     tensor (any dtype, bit for bit) run on our own point-to-point kernels
     (``csrc/p2p.cu``) when the peer is given: messages between a pair are
@@ -45,7 +51,8 @@ import torch.distributed as dist
 __all__ = [
     "reduce_op", "ReduceOp", "send", "recv", "isend", "irecv", "broadcast", "reduce",
     "all_reduce", "scatter", "gather", "gather_to_root", "all_gather", "barrier", "new_group",
-    "get_rank", "get_world_size", "is_initialized", "Request", "group_ranks",
+    "get_rank", "get_world_size", "is_initialized", "Request", "group_ranks", "reduce_scatter", "reduce_scatter_tensor",
+    "all_to_all_single", "all_gather_into_tensor",
 ]
 
 
@@ -334,6 +341,85 @@ def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group=None
         w.all_gather_(tensor_list, tensor)
         return None
     return dist.all_gather(tensor_list, tensor, group=_g(group))
+
+
+def _reduce_scatter_world(output: torch.Tensor, op, group, async_op: bool):
+    """The symmetric world whose reduce-scatter kernels take this call, or None (torch.distributed).  The route depends on
+    ``output``, ``op``, the group and ``async_op`` alone -- the same on every rank of a correct call -- never on the input,
+    whose faults raise inside ``reduce_scatter_`` on the rank that has them."""
+    if async_op:
+        return None
+    w = _symm_world_for(output, group)
+    if w is None or not hasattr(w, "reduce_scatter_") or not _reduces(w, output, op):
+        return None
+    return w
+
+
+def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, op=reduce_op.SUM, group=None,  # noqa: A002
+                          async_op: bool = False):
+    """``input`` holds world equal segments of ``output``'s size; rank r's ``output`` receives segment r of their reduction
+    over the ranks (torch's ``reduce_scatter_tensor``).
+
+    On a symmetric world (``backend="b200"``) a CUDA ``output`` takes the peer-memory kernels for the ops and dtypes of
+    ``all_reduce`` (a bool SUM is a MAX), bit for bit slice r of what ``all_reduce`` leaves; AVG, other dtypes, CPU tensors
+    and ``async_op=True`` go to torch.distributed."""
+    _check(output)
+    _check(input)
+    w = _reduce_scatter_world(output, op, group, async_op)
+    if w is not None:
+        w.reduce_scatter_(output, input, op)
+        return None
+    return dist.reduce_scatter_tensor(output, input, op=op, group=_g(group), async_op=async_op)
+
+
+def reduce_scatter(output: torch.Tensor, input_list: List[torch.Tensor], op=reduce_op.SUM, group=None,
+                   async_op: bool = False):
+    """``input_list[p]`` of every rank is reduced into rank p's ``output`` (torch's ``reduce_scatter``).  Routed like
+    :func:`reduce_scatter_tensor`, by ``output`` alone: an ``input_list`` of the wrong length, dtype or size raises on the rank
+    that passed it, before any launch, and its peers are then left waiting inside the kernel until its spin limit reports
+    them.  A list of consecutive views of one 16-byte aligned block is read in place; any other list is copied into the
+    staging buffer first."""
+    _check(output)
+    w = _reduce_scatter_world(output, op, group, async_op)
+    if w is not None:
+        w.reduce_scatter_(output, list(input_list), op)
+        return None
+    return dist.reduce_scatter(output, list(input_list), op=op, group=_g(group), async_op=async_op)
+
+
+def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes=None,  # noqa: A002
+                      input_split_sizes=None, group=None, async_op: bool = False):
+    """Segment p of rank r's ``output`` receives segment r of rank p's ``input`` (torch's ``all_to_all_single``).
+
+    On a symmetric world the equal-segment form (both split lists ``None``) of a CUDA tensor of any dtype is copied bit for
+    bit by the peer-memory kernels.  Given split sizes always go to torch.distributed, even equal ones: a rank cannot tell
+    from its own arguments whether its peers' segments match, and every rank must enter the same kernel."""
+    _check(output)
+    _check(input)
+    if not async_op and output_split_sizes is None and input_split_sizes is None:
+        w = _symm_world_for(output, group)
+        if w is not None and hasattr(w, "all_to_all_") and w.supports_raw(output):
+            w.all_to_all_(output, input)
+            return None
+    return dist.all_to_all_single(output, input, output_split_sizes=output_split_sizes,
+                                  input_split_sizes=input_split_sizes, group=_g(group), async_op=async_op)
+
+
+def all_gather_into_tensor(output_tensor: torch.Tensor, input_tensor: torch.Tensor, group=None, async_op: bool = False):
+    """Rank r's ``input_tensor`` lands at segment r of every rank's ``output_tensor`` (torch's ``all_gather_into_tensor``).
+    On a symmetric world the CUDA tensors go through :func:`all_gather`'s peer-memory kernels, with ``output_tensor``'s
+    segments as the (contiguous) output list.  As in :func:`all_gather`, the route also looks at ``output_tensor``: one
+    whose dtype or size does not fit (world x the input's elements) goes to torch.distributed, which raises on that rank,
+    while its peers are left waiting inside the kernel until its spin limit reports them (B2_SPIN_LIMIT)."""
+    _check(output_tensor)
+    _check(input_tensor)
+    if not async_op:
+        w = _symm_world_for(input_tensor, group)
+        if w is not None and hasattr(w, "all_gather_") and w.supports_raw(input_tensor) and w.supports_raw(output_tensor) \
+                and output_tensor.dtype == input_tensor.dtype and output_tensor.numel() == w.world * input_tensor.numel():
+            w.all_gather_(list(output_tensor.view(w.world, -1).unbind(0)), input_tensor.view(-1))
+            return None
+    return dist.all_gather_into_tensor(output_tensor, input_tensor, group=_g(group), async_op=async_op)
 
 
 def barrier(group=None):

@@ -28,6 +28,8 @@
 //                               receives segment r (at vector r * n_vec / world of its symmetric buffer when in place)
 // Every rank of one call runs the same barrier sequence whatever the op and root, so calls of any kind may follow each
 // other on one buffer, signal pad and inbox.
+// Reduce-scatter and all-to-all have kernels of their own (segments_pull_kernel, segments_ll_kernel: a pull with barriers
+// and an LL push) on the same lanes, per-block epoch words and inbox, so they too may follow any call on one buffer.
 #include <cstdio>
 #include <cstring>
 #include <cuda_fp16.h>
@@ -622,6 +624,129 @@ __global__ void __launch_bounds__(kThreads) allreduce_ll_kernel(ARArgs a) {
   if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
 }
 
+// ------------------------------------------------------------------------------------------ reduce-scatter / all-to-all
+// n_vec = world segments of seg = n_vec / world vectors on every rank.  Reduce-scatter (A2A false): rank r's output is
+// segment r of the reduction, combined exactly as the all-reduce combines it (identity, then every rank's term in rank order,
+// pack with scale 1), so it is bit for bit slice r of the all-reduce of the same inputs.  All-to-all (A2A true, raw 16-byte
+// copies): segment p of rank r's output is segment r of rank p's input.  Vector j of every segment is handled by the same
+// (block, thread) in every phase and on every rank, so the per-block barriers suffice.
+//
+// Pull: stage src into this rank's buffer (unless it is already there), barrier, load segment `rank` of every rank's buffer,
+// store to dst (reduce-scatter in place: to segment `rank` of this rank's buffer, which no peer reads), barrier (the peers
+// have finished reading this buffer, so the caller may overwrite it).  The all-to-all needs a dst: in place, storing segment
+// p would overwrite what rank p is still reading.
+template <class L, int OP, bool A2A>
+__global__ void __launch_bounds__(kThreads) segments_pull_kernel(ARArgs a) {
+  const int rank = a.rank, world = a.world;
+  uint32_t epoch = barrier_epoch_load(a.sig, rank);
+  const size_t seg = a.n_vec / world;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
+  uint4* mine = reinterpret_cast<uint4*>(a.bufs.p[rank]);
+  if (a.src != nullptr) {
+    for (int s = 0; s < world; ++s)
+      for (size_t j = first; j < seg; j += stride)
+        st_cg_v4(mine + (size_t)s * seg + j, ld_cg_v4(reinterpret_cast<const uint4*>(a.src) + (size_t)s * seg + j));
+  }
+  block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's segments are in place
+  const size_t off = (size_t)rank * seg;
+  uint4* out = a.dst != nullptr ? reinterpret_cast<uint4*>(a.dst) : mine + off;
+  for (size_t base = first; base < seg; base += stride * kUnroll) {
+    uint4 raw[kUnroll][B2_MAX_RANKS];
+#pragma unroll
+    for (int u = 0; u < kUnroll; ++u) {
+      const size_t j = base + (size_t)u * stride;
+#pragma unroll
+      for (int r = 0; r < B2_MAX_RANKS; ++r)
+        if (r < world && j < seg) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.bufs.p[r]) + off + j);
+    }
+#pragma unroll
+    for (int u = 0; u < kUnroll; ++u) {
+      const size_t j = base + (size_t)u * stride;
+      if (j >= seg) continue;
+      if constexpr (A2A) {
+#pragma unroll
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world) st_cg_v4(out + (size_t)r * seg + j, raw[u][r]);
+      } else {
+        typename L::Acc acc[L::kElems];
+        L::template zero<OP>(acc);
+#pragma unroll
+        for (int r = 0; r < B2_MAX_RANKS; ++r)
+          if (r < world) L::template add<OP>(acc, raw[u][r]);
+        st_cg_v4(out + j, L::template pack<OP>(acc, 1.f));
+      }
+    }
+  }
+  block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // no peer reads this buffer any more
+  if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+}
+
+// LL: vector v of segment d goes as flag-in-data lines to rank d's inbox, in the region of source `rank`, for every d != rank;
+// then the W - 1 lines of this rank's own segment are awaited.  Reduce-scatter combines them with its own vector in rank order;
+// all-to-all stores the line from source p at output segment p.  Per vector every rank pushes one line to every peer and waits
+// for one from every peer, and vector v belongs to block v / kThreads, so the parity argument of allreduce_ll_kernel holds for
+// any mix of calls on one inbox.  In place (no src / dst) the input is this rank's buffer and the reduce-scatter's output its
+// segment `rank`; a thread reads every input vector it needs before it stores.
+template <class L, int OP, bool A2A>
+__global__ void __launch_bounds__(kThreads) segments_ll_kernel(ARArgs a) {
+  const int rank = a.rank, world = a.world;
+  const uint32_t epoch = barrier_epoch_load(a.sig, rank) + 1u;
+  const uint32_t flag = epoch == 0u ? 1u : epoch;
+  const size_t par = (size_t)(epoch & 1u);
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  const size_t seg = a.n_vec / world;
+  const uint4* in = reinterpret_cast<const uint4*>(a.src != nullptr ? a.src : a.bufs.p[rank]);
+  uint4* out = a.dst != nullptr ? reinterpret_cast<uint4*>(a.dst) : reinterpret_cast<uint4*>(a.bufs.p[rank]) + (size_t)rank * seg;
+  for (size_t v = (size_t)blockIdx.x * kThreads + threadIdx.x; v < seg; v += stride) {
+    const size_t line = ((par * (size_t)world + (size_t)rank) * a.ll_cap + v) * 2;
+#pragma unroll
+    for (int i = 1; i < B2_MAX_RANKS; ++i) {
+      if (i < world) {
+        int d = rank + i;
+        if (d >= world) d -= world;
+        const uint4 w = ld_cg_v4(in + (size_t)d * seg + v);
+        uint4* dl = reinterpret_cast<uint4*>(a.inbox.p[d]) + line;
+        st_volatile_v4(dl, make_uint4(w.x, flag, w.y, flag));
+        st_volatile_v4(dl + 1, make_uint4(w.z, flag, w.w, flag));
+      }
+    }
+    const uint4 own = ld_cg_v4(in + (size_t)rank * seg + v);
+    typename L::Acc acc[L::kElems];
+    if constexpr (!A2A) L::template zero<OP>(acc);
+    const uint4* box = reinterpret_cast<const uint4*>(a.inbox.p[rank]);
+#pragma unroll
+    for (int r = 0; r < B2_MAX_RANKS; ++r) {
+      if (r < world) {
+        uint4 w;
+        if (r == rank) {
+          w = own;
+        } else {
+          const uint4* src = box + ((par * (size_t)world + (size_t)r) * a.ll_cap + v) * 2;
+          uint4 q0, q1;
+          unsigned long long spins = 0;
+          for (;;) {
+            q0 = ld_volatile_v4(src);
+            q1 = ld_volatile_v4(src + 1);
+            if (q0.y == flag && q0.w == flag && q1.y == flag && q1.w == flag) break;
+            if (++spins > B2_SPIN_LIMIT) {
+              printf("[b200dist] LL %s: rank %d timed out waiting for rank %d (block %d, epoch %u)\n",
+                     A2A ? "all-to-all" : "reduce-scatter", rank, r, (int)blockIdx.x, flag);
+              __trap();
+            }
+          }
+          w = make_uint4(q0.x, q0.z, q1.x, q1.z);
+        }
+        if constexpr (A2A) st_cg_v4(out + (size_t)r * seg + v, w);
+        else L::template add<OP>(acc, w);                             // fixed rank order, as the all-reduce
+      }
+    }
+    if constexpr (!A2A) st_cg_v4(out + v, L::template pack<OP>(acc, 1.f));
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+}
+
 // ------------------------------------------------------------------------------------------ barrier only
 __global__ void __launch_bounds__(32) barrier_kernel(SignalPads sig, int rank, int world) {
   uint32_t epoch = barrier_epoch_load(sig, rank);
@@ -668,6 +793,55 @@ void launch_op(int variant, int dtype, dim3 grid, const ARArgs& a, cudaStream_t 
     if (a.root >= 0) return launch_kernel<LaneF32, kGather, true>(variant, grid, a, stream);
   }
   launch_kernel<LaneF32, OP, false>(variant, grid, a, stream);
+}
+
+template <class L, int OP, bool A2A>
+void launch_segments(int variant, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+  if (variant == 3) segments_ll_kernel<L, OP, A2A><<<grid, kThreads, 0, stream>>>(a);
+  else segments_pull_kernel<L, OP, A2A><<<grid, kThreads, 0, stream>>>(a);
+}
+
+template <int OP>
+void launch_reduce_scatter(int variant, int dtype, dim3 grid, const ARArgs& a, cudaStream_t stream) {
+  switch (dtype) {
+    case kBF16: return launch_segments<LaneBF16, OP, false>(variant, grid, a, stream);
+    case kF16: return launch_segments<LaneF16, OP, false>(variant, grid, a, stream);
+    case kF64: return launch_segments<LaneF64, OP, false>(variant, grid, a, stream);
+    case kI32: return launch_segments<LaneI32, OP, false>(variant, grid, a, stream);
+    case kI64: return launch_segments<LaneI64, OP, false>(variant, grid, a, stream);
+    case kI8: return launch_segments<LaneI8<true>, OP, false>(variant, grid, a, stream);
+    case kU8:
+    case kBool:                               // as launch_op: SUM / PRODUCT share the int8 instance
+      if constexpr (OP == kSum || OP == kProd) return launch_segments<LaneI8<true>, OP, false>(variant, grid, a, stream);
+      else return launch_segments<LaneI8<false>, OP, false>(variant, grid, a, stream);
+    default: return launch_segments<LaneF32, OP, false>(variant, grid, a, stream);
+  }
+}
+
+// The grid of a reduce-scatter or all-to-all: one thread per vector of a segment.  LL: sized by the segment alone (<= ll_cap),
+// never by max_blocks, so vector v belongs to block v / kThreads as in every LL call on the inbox.
+inline dim3 segments_grid(int variant, size_t seg, int max_blocks) {
+  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
+  size_t blocks = (seg + kThreads - 1) / kThreads;
+  if (blocks < 1) blocks = 1;
+  const size_t cap = variant == 3 ? (size_t)B2_MAX_BLOCKS : (size_t)max_blocks;
+  return dim3((unsigned)(blocks > cap ? cap : blocks));
+}
+
+// Shared checks and arguments of the two segmented launchers; false for a call they refuse.
+inline bool segments_args(int variant, const PeerPtrs* bufs, const SignalPads* sig, const void* src, void* dst, size_t n_vec,
+                          int rank, int world, const PeerPtrs* inbox, size_t ll_cap, ARArgs* a) {
+  if ((variant != 0 && variant != 3) || world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return false;
+  if (bufs == nullptr || sig == nullptr || n_vec % (size_t)world != 0) return false;
+  memset(a, 0, sizeof(*a));
+  a->bufs = *bufs; a->sig = *sig; a->src = src; a->dst = dst; a->n_vec = n_vec; a->scale = 1.f;
+  a->rank = rank; a->world = world; a->root = -1;
+  if (variant == 3) {
+    if (inbox == nullptr || ll_cap < n_vec / world) return false;
+    a->inbox = *inbox;
+    a->ll_cap = ll_cap;
+  }
+  return true;
 }
 
 }  // namespace b2
@@ -744,6 +918,41 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const b2::S
                         cudaStream_t stream) {
   return b2_allreduce_dtype_launch(variant, bf16 ? b2::kBF16 : b2::kF32, bufs, sig, mc, src, src_f32, dst, dst_f32, n_vec,
                                    scale, rank, world, max_blocks, inbox, ll_cap, op, root, stream);
+}
+
+// Reduce-scatter: n_vec 16-byte vectors of input on every rank, world segments of n_vec / world; rank r's output (dst, or
+// with dst null segment r of its own buffer) is segment r of the reduction.  src null: the input already is the buffer.
+// variant 0 pull (barriers), 3 LL (needs inbox / ll_cap).  op and dtype as b2_allreduce_dtype_launch (wire dtype = local
+// dtype, no scale; a bool SUM is refused, the caller maps it to MAX).  Returns cudaError_t as int; cudaErrorInvalidValue,
+// without a launch, for a variant other than 0 / 3, an unknown op or dtype, a bool SUM, a world outside 1..8, a rank outside
+// [0, world), an n_vec that is not a multiple of world, or an LL segment larger than the inbox.
+int b2_reduce_scatter_launch(int variant, int dtype, int op, const PeerPtrs* bufs, const b2::SignalPads* sig, const void* src,
+                             void* dst, size_t n_vec, int rank, int world, int max_blocks, const PeerPtrs* inbox,
+                             size_t ll_cap, cudaStream_t stream) {
+  if (op < b2::kSum || op > b2::kMin || dtype < b2::kF32 || dtype > b2::kBool) return (int)cudaErrorInvalidValue;
+  if (dtype == b2::kBool && op == b2::kSum) return (int)cudaErrorInvalidValue;
+  b2::ARArgs a;
+  if (!b2::segments_args(variant, bufs, sig, src, dst, n_vec, rank, world, inbox, ll_cap, &a)) return (int)cudaErrorInvalidValue;
+  const dim3 grid = b2::segments_grid(variant, n_vec / world, max_blocks);
+  switch (op) {
+    case b2::kSum: b2::launch_reduce_scatter<b2::kSum>(variant, dtype, grid, a, stream); break;
+    case b2::kProd: b2::launch_reduce_scatter<b2::kProd>(variant, dtype, grid, a, stream); break;
+    case b2::kMax: b2::launch_reduce_scatter<b2::kMax>(variant, dtype, grid, a, stream); break;
+    default: b2::launch_reduce_scatter<b2::kMin>(variant, dtype, grid, a, stream); break;
+  }
+  return (int)cudaGetLastError();
+}
+
+// All-to-all of raw 16-byte vectors: segment p of rank r's dst receives segment r of rank p's input (src, or with src null
+// this rank's buffer).  dst is required: an in-place all-to-all would overwrite segments its peers are still reading.
+// Refusals as b2_reduce_scatter_launch, plus a null dst.
+int b2_alltoall_launch(int variant, const PeerPtrs* bufs, const b2::SignalPads* sig, const void* src, void* dst, size_t n_vec,
+                       int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream) {
+  if (dst == nullptr) return (int)cudaErrorInvalidValue;
+  b2::ARArgs a;
+  if (!b2::segments_args(variant, bufs, sig, src, dst, n_vec, rank, world, inbox, ll_cap, &a)) return (int)cudaErrorInvalidValue;
+  b2::launch_segments<b2::LaneF32, b2::kSum, true>(variant, b2::segments_grid(variant, n_vec / world, max_blocks), a, stream);
+  return (int)cudaGetLastError();
 }
 
 int b2_barrier_launch(const b2::SignalPads* sig, int rank, int world, cudaStream_t stream) {

@@ -42,6 +42,11 @@ int b2_allreduce_launch(int variant, int bf16, const PeerPtrs* bufs, const Signa
 int b2_allreduce_dtype_launch(int variant, int dtype, const PeerPtrs* bufs, const SignalPadsH* sig, void* mc, const void* src,
                               int src_f32, void* dst, int dst_f32, size_t n_vec, float scale, int rank, int world,
                               int max_blocks, const PeerPtrs* inbox, size_t ll_cap, int op, int root, cudaStream_t stream);
+int b2_reduce_scatter_launch(int variant, int dtype, int op, const PeerPtrs* bufs, const SignalPadsH* sig, const void* src,
+                             void* dst, size_t n_vec, int rank, int world, int max_blocks, const PeerPtrs* inbox,
+                             size_t ll_cap, cudaStream_t stream);
+int b2_alltoall_launch(int variant, const PeerPtrs* bufs, const SignalPadsH* sig, const void* src, void* dst, size_t n_vec,
+                       int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream);
 int b2_barrier_launch(const SignalPadsH* sig, int rank, int world, cudaStream_t stream);
 void b2_p2p_config(int* ctas, int* slots, size_t* chunk, int* pad_words);
 int b2_p2p_send_launch(const PeerPtrs* box, const SignalPadsH* sig, const void* src, size_t nbytes, int rank, int peer,
@@ -396,6 +401,64 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("root"),
      py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(),
      py::arg("ll_cap") = 0);
+  // reduce-scatter / all-to-all: n_vec counts one rank's input, world segments of n_vec / world vectors.  variant 0 pull
+  // (one-shot, two-shot and NVLS all map to it on the Python side), 3 LL.  src null: the input is this rank's buffer; dst
+  // null (reduce-scatter only): the output is segment `rank` of it.  Every rank of one call must pass the same n_vec.
+  auto segments = [](const char* what, int variant, const std::vector<unsigned long long>& bufs,
+                     const std::vector<unsigned long long>& sigs, const c10::optional<torch::Tensor>& src,
+                     const c10::optional<torch::Tensor>& dst, size_t n_vec, int rank, int world,
+                     const std::vector<unsigned long long>& inbox, size_t ll_cap, PeerPtrs* b, SignalPadsH* s, PeerPtrs* ib) {
+    check_world(rank, world, what);
+    TORCH_CHECK(variant == 0 || variant == 3, what, ": variant must be 0 (pull) or 3 (LL), got ", variant);
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, what, ": one buffer and one signal pad per rank, got ",
+                bufs.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK(variant == 3 ? (int)inbox.size() == world : inbox.empty() || (int)inbox.size() == world,
+                what, ": one LL inbox per rank, got ", inbox.size(), " for world ", world);
+    TORCH_CHECK(n_vec % (size_t)world == 0, what, ": n_vec holds world segments, so it must be a multiple of world, got n_vec ",
+                n_vec, " for world ", world);
+    TORCH_CHECK(variant != 3 || n_vec / world <= ll_cap, what, ": LL pushes ", n_vec / world,
+                " vectors per peer, more than the inbox holds (", ll_cap, ")");
+    for (const auto* t : {&src, &dst}) {
+      if (t->has_value()) {
+        check_cuda_contig(**t, t == &src ? "src" : "dst");
+        TORCH_CHECK((size_t)(*t)->nbytes() >= n_vec * 16, what, ": ", t == &src ? "src" : "dst", " holds ", (*t)->nbytes(),
+                    " bytes, the call needs ", n_vec * 16);
+      }
+    }
+    *b = to_ptrs(bufs); *s = to_sig(sigs); *ib = to_ptrs(inbox);
+  };
+  m.def("reduce_scatter", [segments](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                                     c10::optional<torch::Tensor> src, c10::optional<torch::Tensor> dst, size_t n_vec, int rank,
+                                     int world, int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap, int op,
+                                     int dtype) {
+    TORCH_CHECK(op >= 0 && op <= 3, "reduce_scatter: op must be 0 (SUM), 1 (PRODUCT), 2 (MAX) or 3 (MIN), got ", op);
+    TORCH_CHECK(dtype >= 0 && dtype <= 8, "reduce_scatter: dtype must be a code in 0..8, got ", dtype);
+    TORCH_CHECK(dtype != 8 || op != 0, "reduce_scatter: a bool SUM is a MAX (as torch.distributed maps it); pass op 2");
+    for (const auto* t : {&src, &dst})
+      TORCH_CHECK(!t->has_value() || (*t)->scalar_type() == kDtypes[dtype], "reduce_scatter: ", t == &src ? "src" : "dst",
+                  " is ", (*t)->scalar_type(), " but dtype ", dtype, " is ", kDtypes[dtype]);
+    PeerPtrs b, ib; SignalPadsH s;
+    segments("reduce_scatter", variant, bufs, sigs, src, c10::nullopt, n_vec, rank, world, inbox, ll_cap, &b, &s, &ib);
+    if (dst.has_value()) {
+      check_cuda_contig(*dst, "dst");
+      TORCH_CHECK((size_t)dst->nbytes() >= n_vec / world * 16, "reduce_scatter: dst holds ", dst->nbytes(),
+                  " bytes, one segment is ", n_vec / world * 16);
+    }
+    ck_cuda(b2_reduce_scatter_launch(variant, dtype, op, &b, &s, src.has_value() ? src->data_ptr() : nullptr,
+                                     dst.has_value() ? dst->data_ptr() : nullptr, n_vec, rank, world, max_blocks,
+                                     inbox.empty() ? nullptr : &ib, ll_cap, cur_stream()), "reduce_scatter");
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0,
+     py::arg("op") = 0, py::arg("dtype") = 0);
+  m.def("alltoall", [segments](int variant, std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                               c10::optional<torch::Tensor> src, torch::Tensor dst, size_t n_vec, int rank, int world,
+                               int max_blocks, std::vector<unsigned long long> inbox, size_t ll_cap) {
+    PeerPtrs b, ib; SignalPadsH s;
+    segments("alltoall", variant, bufs, sigs, src, dst, n_vec, rank, world, inbox, ll_cap, &b, &s, &ib);
+    ck_cuda(b2_alltoall_launch(variant, &b, &s, src.has_value() ? src->data_ptr() : nullptr, dst.data_ptr(), n_vec, rank, world,
+                               max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, cur_stream()), "alltoall");
+  }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
   m.def("barrier", [](std::vector<unsigned long long> sigs, int rank, int world) {
     check_world(rank, world, "barrier");
     TORCH_CHECK((int)sigs.size() == world, "barrier: one signal pad per rank, got ", sigs.size(), " for world ", world);

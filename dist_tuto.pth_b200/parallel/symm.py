@@ -65,7 +65,7 @@ _DTYPES = (torch.float32, torch.bfloat16)
 # and bf16 the local dtype is the wire dtype: no scale, no bf16 wire, no NVLS.
 DTYPE_CODES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.float64: 3, torch.int8: 4, torch.uint8: 5,
                torch.int32: 6, torch.int64: 7, torch.bool: 8}
-COLLECTIVES = ("allreduce", "reduce", "broadcast", "allgather")
+COLLECTIVES = ("allreduce", "reduce", "broadcast", "allgather", "reducescatter", "alltoall")
 _OPS = {dist.ReduceOp.SUM: 0, dist.ReduceOp.PRODUCT: 1, dist.ReduceOp.MAX: 2, dist.ReduceOp.MIN: 3}
 
 
@@ -87,11 +87,19 @@ def plan_variant(collective: str, op: int, nbytes: int, world: int, ll_max: int,
     ``nbytes`` is the message: the wire bytes of a reduction or broadcast, one rank's input for an all-gather.  An all-gather
     uses LL while one rank's input is at most ``ll_max`` (which never exceeds the LL inbox), one-shot while its whole output
     is at most ``oneshot_max``, two-shot above.  NVLS reduces in the switch and so serves only the SUM all-reduce; ``forced``
-    (``B200DIST_AR_VARIANT``) names a variant, and NVLS falls back to two-shot where it cannot run."""
+    (``B200DIST_AR_VARIANT``) names a variant, and NVLS falls back to two-shot where it cannot run.  A reduce-scatter or an
+    all-to-all (``nbytes``: one rank's segment) is LL (3) or pull (0) only, and any forced variant but LL runs pull."""
     if collective not in COLLECTIVES:
         raise ValueError(f"unknown collective {collective!r}")
     if world == 1:
         return 0
+    if collective in ("reducescatter", "alltoall"):
+        # Two kernels only: pull (0) and LL (3); a forced one-shot, two-shot or NVLS runs pull.  ``nbytes`` is one rank's
+        # segment.  LL while it fits ll_max, pull above: unmeasured starting values, to be replaced by a sweep of
+        # bench/allreduce_sweep.py --collective reducescatter|alltoall on a multi-GPU H100 machine.
+        if forced in VARIANTS:
+            return 3 if forced == "ll" else 0
+        return 3 if nbytes <= ll_max else 0
     nvls_ok = multicast and collective == "allreduce" and op == 0
     if forced in VARIANTS:
         v = VARIANTS[forced]
@@ -716,6 +724,126 @@ class SymmWorld:
             for r, o in enumerate(gather_list):
                 o.view(-1).view(torch.uint8).copy_(buf[r * slot:r * slot + nbytes])
         return gather_list
+
+    # ------------------------------------------------------------------ reduce-scatter / all-to-all
+    def _launch_segments(self, kind: str, hd: SymmHandle, src, dst, seg_vec: int, variant: Optional[int],
+                         max_blocks: Optional[int], op: int = 0, dtype: int = 0) -> int:
+        """One reduce-scatter or all-to-all kernel on ``hd``: world segments of ``seg_vec`` vectors; ``src`` None reads this
+        rank's buffer, ``dst`` None (reduce-scatter) leaves the result at segment ``rank`` of it."""
+        v = self.plan(kind, op, seg_vec * 16) if variant is None else variant
+        v = 3 if v == 3 and hd.ll is not None and seg_vec <= LL_CAP_VEC else 0
+        ll = (hd.ll.ptrs, LL_CAP_VEC) if v == 3 else ([], 0)
+        mb = self.max_blocks if max_blocks is None else max_blocks
+        n_vec = seg_vec * self.world
+        if kind == "reducescatter":
+            self.C.reduce_scatter(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, self.rank, self.world, mb, *ll, op, dtype)
+        else:
+            self.C.alltoall(v, hd.ptrs, hd.sig_ptrs, src, dst, n_vec, self.rank, self.world, mb, *ll)
+        return v
+
+    def reduce_scatter_(self, out: torch.Tensor, inp, op=dist.ReduceOp.SUM, variant: Optional[int] = None,
+                        max_blocks: Optional[int] = None) -> torch.Tensor:
+        """``out`` <- segment ``rank`` of the reduction over the ranks of ``inp``: a tensor of world x ``out``'s elements, or
+        a list of world tensors of ``out``'s size.  Ops and dtypes as :meth:`all_reduce_` without scale or wire (a bool SUM
+        is a MAX); the result is bit for bit slice ``rank`` of the all-reduce of the same inputs.
+
+        The kernel reads ``inp`` in place when it is one 16-byte aligned block of segments of a multiple of 16 bytes, and
+        writes ``out`` directly when that is aligned too and is not a part of that block other than a whole segment;
+        anything else goes through the staging buffer: the segments are
+        copied to 16-byte aligned slots, and the result is copied out of slot ``rank``.  The staging size depends on
+        ``out``'s size alone, so it is the same on every rank (allocation is collective), and no call allocates device
+        memory.  A malformed ``inp`` raises before any launch, on this rank only: its peers are then left inside the kernel
+        until its spin limit reports them (B2_SPIN_LIMIT)."""
+        code = op_code(op)
+        if code is None:
+            raise ValueError(f"the fused reductions are SUM, PRODUCT, MAX and MIN, got {op!r}")
+        if not self.supports_reduction(out):
+            raise TypeError(f"fused reduce_scatter needs a contiguous CUDA tensor on this device of one of "
+                            f"{[str(d).replace('torch.', '') for d in DTYPE_CODES]}, got {out.dtype}")
+        if isinstance(inp, torch.Tensor):
+            if not self.supports_raw(inp) or inp.dtype != out.dtype or inp.numel() != self.world * out.numel():
+                raise ValueError(f"reduce_scatter needs a contiguous CUDA input of {out.dtype} with world x the output's "
+                                 f"elements ({self.world * out.numel()}), got {inp.dtype} x {inp.numel()}")
+            segs = list(inp.view(-1).view(self.world, -1).unbind(0)) if out.numel() else [inp.view(-1)] * self.world
+        else:
+            segs = list(inp) if inp is not None else []
+            if len(segs) != self.world:
+                raise ValueError(f"reduce_scatter needs {self.world} input tensors, got {len(segs)}")
+            if not all(isinstance(s, torch.Tensor) and self.supports_raw(s) for s in segs):
+                raise TypeError("fused reduce_scatter needs contiguous CUDA tensors on this device")
+            if any(s.dtype != out.dtype or s.numel() != out.numel() for s in segs):
+                raise ValueError("every tensor of reduce_scatter's list must have the output's dtype and size")
+        if out.dtype == torch.bool and code == 0:
+            code = 2                                           # torch.distributed's NCCL group reduces a bool SUM as MAX
+        if self.world == 1:
+            s0 = segs[0].view(out.shape)
+            a0, b0, nb = s0.data_ptr(), out.data_ptr(), out.numel() * out.element_size()
+            out.copy_(s0.clone() if a0 != b0 and a0 < b0 + nb and b0 < a0 + nb else s0)   # torch refuses a partial overlap
+            return out
+        dt = DTYPE_CODES[out.dtype]
+        nbytes = out.numel() * out.element_size()
+        seg = (nbytes + 15) // 16
+        slot = seg * 16
+        st = self._staging_for(torch.float32, self.world * slot)   # the same size on every rank: allocation is collective
+        buf = st.view(torch.uint8, st.nbytes)
+        raw_out = out.view(-1).view(torch.uint8)
+        block = self._one_block(segs, nbytes) if nbytes % 16 == 0 else None
+        src = block.view(out.dtype) if block is not None else None
+        b0 = raw_out.data_ptr()
+        dst = out.view(-1) if nbytes % 16 == 0 and b0 % 16 == 0 else None
+        if dst is not None and src is not None:
+            # an output inside the input block is safe only as a whole segment (vector j of every segment is read and
+            # written by one thread); at any other offset a thread would overwrite input another thread still reads
+            a0 = src.data_ptr()
+            if a0 < b0 + nbytes and b0 < a0 + self.world * nbytes and (b0 - a0) % nbytes:
+                dst = None
+        if src is None:                                        # stage every segment at its aligned slot
+            for r, s in enumerate(segs):
+                buf[r * slot:r * slot + nbytes].copy_(s.reshape(-1).view(torch.uint8))
+        self._launch_segments("reducescatter", st, src, dst, seg, variant, max_blocks, code, dt)
+        if dst is None:                                        # the result is at this rank's slot of its buffer
+            raw_out.copy_(buf[self.rank * slot:self.rank * slot + nbytes])
+        return out
+
+    def all_to_all_(self, out: torch.Tensor, inp: torch.Tensor, variant: Optional[int] = None,
+                    max_blocks: Optional[int] = None) -> torch.Tensor:
+        """Equal-segment all-to-all: segment p of ``out`` <- segment ``rank`` of rank p's ``inp`` (any dtype, copied bit for
+        bit; ``out`` and ``inp`` have one size, a multiple of world elements; ``out`` may be ``inp``).  Segments of a
+        multiple of 16 bytes are read from an aligned ``inp`` and written to an aligned ``out`` that does not partly overlap
+        it; anything else goes through the staging buffer, whose first half holds the input segments at 16-byte aligned
+        slots and whose second half receives the output.  The staging size depends on the size alone, and no call
+        allocates device memory."""
+        if not self.supports_raw(out) or not self.supports_raw(inp):
+            raise TypeError("fused all_to_all needs contiguous CUDA tensors on this device")
+        if inp.dtype != out.dtype or inp.numel() != out.numel() or out.numel() % self.world:
+            raise ValueError(f"all_to_all needs an input and an output of one dtype and size, a multiple of world "
+                             f"({self.world}) elements; got {inp.dtype} x {inp.numel()} and {out.dtype} x {out.numel()}")
+        if self.world == 1:
+            out.copy_(inp)
+            return out
+        raw_in, raw_out = inp.view(-1).view(torch.uint8), out.view(-1).view(torch.uint8)
+        total = raw_out.numel()
+        nbytes = total // self.world
+        seg = (nbytes + 15) // 16
+        slot = seg * 16
+        n = self.world * slot
+        st = self._staging_for(torch.float32, 2 * n)
+        buf = st.view(torch.uint8, st.nbytes)
+        a0, b0 = raw_in.data_ptr(), raw_out.data_ptr()
+        overlap = a0 != b0 and a0 < b0 + total and b0 < a0 + total
+        fused = nbytes % 16 == 0
+        src = raw_in if fused and a0 % 16 == 0 else None
+        dst = raw_out if fused and b0 % 16 == 0 and not overlap else buf[n:2 * n]
+        if src is None:                                        # stage every segment at its aligned slot
+            for p in range(self.world):
+                buf[p * slot:p * slot + nbytes].copy_(raw_in[p * nbytes:(p + 1) * nbytes])
+        self._launch_segments("alltoall", st, src, dst, seg, variant, max_blocks)
+        if dst is not raw_out:
+            # contiguous copies (memcpy, no kernel): ranks driven from one process, as on emulated ranks, must not load a
+            # kernel module while a peer's kernel spins, since lazy loading may wait for it
+            for p in range(self.world):
+                raw_out[p * nbytes:(p + 1) * nbytes].copy_(dst[p * slot:p * slot + nbytes])
+        return out
 
     # ------------------------------------------------------------------ point-to-point
     def send_(self, t: torch.Tensor, dst: int) -> None:
