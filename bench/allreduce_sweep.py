@@ -15,11 +15,13 @@ Bandwidth columns:
             reported as link_GBs = link_tx / t against 770 GB/s measured peer copy.
 ``--emit-table`` writes parallel/allreduce_table.json (per-world variant thresholds) from the measured winners.
 
-``--collective {reduce,broadcast,allgather,scatter,gather,reducescatter,alltoall}`` or ``--op {product,max,min}`` time
+``--collective {reduce,broadcast,allgather,scatter,gather,reducescatter,alltoall,alltoallv}`` or ``--op {product,max,min}`` time
 that collective instead: every variant of ours (forced, through the ``SymmWorld`` method ``comm.py`` routes to) against the
 NCCL call on the same tensor, per size (for an all-gather, a scatter, a gather, a reduce-scatter and an all-to-all, the
 size of one rank's segment; the root is rank 0 and its list is one block; reduce-scatter and all-to-all have an LL and a
-pull arm only).  ``--dtype {bf16,fp16,fp64,int8,uint8,int32,int64,bool}`` times the reductions (and the raw moves) on
+pull arm only).  ``alltoallv`` times ``all_to_all_single`` with split sizes: seeded skewed splits of about the size
+per pair, half of every rank's bytes to one hot destination and the rest at random, on the variable-segment kernel
+against NCCL (no speed claim rests on it until it has run on a multi-GPU H100 machine).  ``--dtype {bf16,fp16,fp64,int8,uint8,int32,int64,bool}`` times the reductions (and the raw moves) on
 a tensor of that dtype.  It compares GPUs, so it refuses to run on one.
 """
 import argparse
@@ -83,6 +85,22 @@ DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16, 
           "uint8": torch.uint8, "int32": torch.int32, "int64": torch.int64, "bool": torch.bool}
 
 
+def skewed_splits(size: int, n: int, seed: int) -> list:
+    """``S[s][d]``: elements rank s sends rank d, about ``n`` per pair on average, drawn from ``seed`` (the same on every
+    rank): one hot destination takes half of every rank's elements, the others share the rest at random."""
+    g = torch.Generator().manual_seed(seed)
+    hot = int(torch.randint(0, size, (1,), generator=g))
+    S = []
+    for _ in range(size):
+        share = torch.rand(size, generator=g)
+        share[hot] = 0.0
+        share = share / share.sum() * (size * n - size * n // 2) if size > 1 else share * 0
+        row = [int(x) for x in share]
+        row[hot] += size * n - sum(row)
+        S.append(row)
+    return S
+
+
 def body_collective(rank, size):
     """``--collective`` / ``--op``: ours per forced variant vs NCCL, per size, rows printed and written to ``--out``."""
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -103,7 +121,14 @@ def body_collective(rank, size):
         row = {"bytes": s, "collective": coll, "op": ARGS.op, "dtype": ARGS.dtype}
         arms = []
         segmented = coll in ("reducescatter", "alltoall")     # two kernels only: LL and pull
-        for name, v in ((("ll", 3), ("pull", 0)) if segmented else (("ll", 3), ("oneshot", 0), ("twoshot", 1))):
+        if coll == "alltoallv":                                # one kernel: the variable-segment pull
+            S = skewed_splits(size, n, s)
+            v_in = torch.ones(sum(S[rank]), dtype=dtype, device=dev)
+            v_out = torch.empty(sum(S[p][rank] for p in range(size)), dtype=dtype, device=dev)
+            v_osplit = [S[p][rank] for p in range(size)]
+            arms.append(("pull", lambda: w.all_to_all_v_(v_out, v_in, v_osplit, S[rank])))
+        for name, v in (() if coll == "alltoallv" else (("ll", 3), ("pull", 0)) if segmented else
+                        (("ll", 3), ("oneshot", 0), ("twoshot", 1))):
             if name == "ll" and s > symm.LL_CAP_VEC * 16:
                 continue
             if coll == "reducescatter":
@@ -127,7 +152,8 @@ def body_collective(rank, size):
                 "scatter": lambda: dist.scatter(t, scatter_list=lst, src=0),
                 "gather": lambda: dist.gather(t, gather_list=lst, dst=0),
                 "reducescatter": lambda: dist.reduce_scatter_tensor(t, whole, op=op),
-                "alltoall": lambda: dist.all_to_all_single(outs_whole, whole)}[coll]
+                "alltoall": lambda: dist.all_to_all_single(outs_whole, whole),
+                "alltoallv": lambda: dist.all_to_all_single(v_out, v_in, v_osplit, S[rank])}[coll]
         arms.append(("nccl", nccl))
         best = {}
         for order in (arms, arms[::-1]):
@@ -280,7 +306,7 @@ if __name__ == "__main__":
     ap.add_argument("--out", default=None)
     ap.add_argument("--emit-table", action="store_true", help="write the measured variant thresholds of this world size")
     ap.add_argument("--collective", choices=["allreduce", "reduce", "broadcast", "allgather", "scatter", "gather", "reducescatter",
-                                                 "alltoall"], default="allreduce")
+                                                 "alltoall", "alltoallv"], default="allreduce")
     ap.add_argument("--op", choices=sorted(OPS), default="sum")
     ap.add_argument("--dtype", choices=list(DTYPES), default="fp32", help="tensor dtype of the reductions")
     ARGS = ap.parse_args()

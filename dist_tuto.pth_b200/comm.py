@@ -29,8 +29,10 @@ Design (GPU-first, not a port):
     ``reduce_scatter`` (the ops and dtypes of ``all_reduce``) and the
     equal-segment ``all_to_all_single`` (any dtype) run on peer-memory
     kernels of their own on such a world, and ``all_gather_into_tensor`` on
-    the all-gather's; given split sizes, ``async_op=True``, AVG, other dtypes,
-    CPU tensors and the two-level world go to torch.distributed.
+    the all-gather's; ``all_to_all_single`` with split sizes and the list form
+    ``all_to_all`` (any sizes, any dtype) run on a variable-segment kernel;
+    ``async_op=True``, AVG, other dtypes, CPU tensors and the two-level world
+    go to torch.distributed.
   * on such a world ``send``, ``recv``, ``isend`` and ``irecv`` of a CUDA
     tensor (any dtype, bit for bit) run on our own point-to-point kernels
     (``csrc/p2p.cu``) when the peer is given: messages between a pair are
@@ -52,7 +54,7 @@ __all__ = [
     "reduce_op", "ReduceOp", "send", "recv", "isend", "irecv", "broadcast", "reduce",
     "all_reduce", "scatter", "gather", "gather_to_root", "all_gather", "barrier", "new_group",
     "get_rank", "get_world_size", "is_initialized", "Request", "group_ranks", "reduce_scatter", "reduce_scatter_tensor",
-    "all_to_all_single", "all_gather_into_tensor",
+    "all_to_all_single", "all_gather_into_tensor", "all_to_all",
 ]
 
 
@@ -389,20 +391,52 @@ def reduce_scatter(output: torch.Tensor, input_list: List[torch.Tensor], op=redu
 
 def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes=None,  # noqa: A002
                       input_split_sizes=None, group=None, async_op: bool = False):
-    """Segment p of rank r's ``output`` receives segment r of rank p's ``input`` (torch's ``all_to_all_single``).
+    """Segment p of rank r's ``output`` receives segment r of rank p's ``input`` (torch's ``all_to_all_single``); the split
+    lists cut dim 0 into the ranks' segments (``None``: equal segments).
 
     On a symmetric world the equal-segment form (both split lists ``None``) of a CUDA tensor of any dtype is copied bit for
-    bit by the peer-memory kernels.  Given split sizes always go to torch.distributed, even equal ones: a rank cannot tell
-    from its own arguments whether its peers' segments match, and every rank must enter the same kernel."""
+    bit by the peer-memory kernels.  Given either split list, a blocking call of two CUDA tensors runs on the variable-segment
+    kernel (``SymmWorld.all_to_all_v_``), bit for bit, whatever the splits.  The form of the call picks the kernel, so:
+
+    * every rank must use the same form: a rank that passes split sizes while a peer passes none is a caller error (it waits
+      inside the kernel until its spin limit reports it), although torch.distributed would accept the mix;
+    * ``async_op=True``, CPU tensors and the two-level world of several machines stay on torch.distributed;
+    * splits that disagree between ranks give truncated segments (each receiver takes the shorter of what was sent and what
+      it expects, and leaves the rest of its segment alone), not a hang."""
     _check(output)
     _check(input)
-    if not async_op and output_split_sizes is None and input_split_sizes is None:
+    if not async_op:
         w = _symm_world_for(output, group)
-        if w is not None and hasattr(w, "all_to_all_") and w.supports_raw(output):
-            w.all_to_all_(output, input)
+        if output_split_sizes is None and input_split_sizes is None:
+            if w is not None and hasattr(w, "all_to_all_") and w.supports_raw(output):
+                w.all_to_all_(output, input)
+                return None
+        elif w is not None and hasattr(w, "all_to_all_v_") and w.supports_raw(output) and w.supports_raw(input):
+            w.all_to_all_v_(output, input, output_split_sizes, input_split_sizes)
             return None
     return dist.all_to_all_single(output, input, output_split_sizes=output_split_sizes,
                                   input_split_sizes=input_split_sizes, group=_g(group), async_op=async_op)
+
+
+def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[torch.Tensor], group=None,
+               async_op: bool = False):
+    """``output_tensor_list[p]`` of rank r receives ``input_tensor_list[r]`` of rank p (torch's ``all_to_all``); the
+    tensors may have any sizes.
+
+    On a symmetric world a blocking call whose tensors are all CUDA runs on the variable-segment kernel
+    (``SymmWorld.all_to_all_v_``), bit for bit; a list of the wrong length or of mixed dtypes raises there, on the rank that
+    passed it.  The rules of :func:`all_to_all_single` with split sizes hold: every rank must call the list form,
+    ``async_op=True``, CPU tensors and the two-level world stay on torch.distributed (whose gloo backend has no
+    ``all_to_all``), and sizes that disagree between ranks give truncated segments, not a hang."""
+    outs, ins = list(output_tensor_list), list(input_tensor_list)
+    for t in outs + ins:
+        _check(t)
+    if not async_op and outs + ins:
+        w = _symm_world_for((outs + ins)[0], group)
+        if w is not None and hasattr(w, "all_to_all_v_") and all(w.supports_raw(t) for t in outs + ins):
+            w.all_to_all_v_(outs, ins)
+            return None
+    return dist.all_to_all(outs, ins, group=_g(group), async_op=async_op)
 
 
 def all_gather_into_tensor(output_tensor: torch.Tensor, input_tensor: torch.Tensor, group=None, async_op: bool = False):

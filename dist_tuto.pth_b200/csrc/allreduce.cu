@@ -30,6 +30,8 @@
 // other on one buffer, signal pad and inbox.
 // Reduce-scatter and all-to-all have kernels of their own (segments_pull_kernel, segments_ll_kernel: a pull with barriers
 // and an LL push) on the same lanes, per-block epoch words and inbox, so they too may follow any call on one buffer.
+// The all-to-all with variable segments (alltoallv_kernel: rounds of a fixed chunk through a double-buffered staging window)
+// uses the same signal pads and per-block epoch words and ends with the same final barrier, so it too may follow any call.
 #include <cstdio>
 #include <cstring>
 #include <cuda_fp16.h>
@@ -747,6 +749,145 @@ __global__ void __launch_bounds__(kThreads) segments_ll_kernel(ARArgs a) {
   if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
 }
 
+// ------------------------------------------------------------------------------------------ all-to-allv
+// Variable segments of raw bytes: rank r sends src[d] (src_bytes[d] bytes) to rank d and receives what rank p sends it into
+// dst[p] (dst_bytes[p] bytes).  The staging buffer of every rank is [header | half 0 | half 1]: the header holds this rank's W
+// send lengths, each half W slots of kA2avChunk bytes, slot d for what goes to rank d.  Neither its size nor the grid depends on
+// the lengths, which ranks cannot agree on without communicating: segments move in rounds of at most kA2avChunk bytes per pair.
+//
+//   stage chunk 0 of every send into half 0, publish the header, barrier
+//   every rank reads all W x W lengths: K = max(1, ceil(max / kA2avChunk)), the same on every rank
+//   round k < K: pull chunk k of segment `rank` from every rank's half k & 1 into dst, stage chunk k + 1 into half (k + 1) & 1,
+//                barrier
+//
+// K + 1 barriers in all.  Half h is staged again in round k + 1 only after the barrier that ends round k, the last round whose
+// pulls read it, and the barrier that ends round K - 1 is the one after which no peer reads this buffer (header included), as
+// segments_pull_kernel ends.  Vector j of every slot is staged and pulled by one (block, thread) in every round and on every
+// rank, and every block writes the header itself (identical values), so the per-block barriers order everything a block
+// reads.  The receiver moves min(what the sender published, what it expects) of each pair: splits that disagree between ranks
+// give a truncated segment, never a write outside one or a different number of rounds.
+constexpr size_t kA2avChunk = 128 << 10;     // bytes per (source, destination) pair and round: an unmeasured starting point
+constexpr size_t kA2avHeader = 16 * ((B2_MAX_RANKS * 8 + 15) / 16);   // W 8-byte send lengths, 16-byte aligned
+constexpr size_t kA2avChunkVec = kA2avChunk / 16;
+
+struct A2AVArgs {
+  PeerPtrs bufs;                                   // staging buffer of every rank: header | half 0 | half 1
+  SignalPads sig;
+  const unsigned char* src[B2_MAX_RANKS];          // what this rank sends to rank d ...
+  unsigned long long src_bytes[B2_MAX_RANKS];      // ... and how many bytes
+  unsigned char* dst[B2_MAX_RANKS];                // where what rank p sends lands ...
+  unsigned long long dst_bytes[B2_MAX_RANKS];      // ... and how many bytes this rank expects from it
+  int rank, world;
+};
+
+__device__ __forceinline__ void st_cg_u64(void* p, unsigned long long v) {
+  asm volatile("st.global.cg.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_cg_u64(const void* p) {
+  unsigned long long v;
+  asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// The n (> 0) bytes of a segment at p, at most 16 of them, as one vector: a whole vector with the widest accesses p's alignment
+// allows, a partial one byte by byte, so that no byte outside the segment is read.  The bytes past n are zero.
+__device__ __forceinline__ uint4 a2av_load(const unsigned char* p, size_t n) {
+  const uintptr_t at = reinterpret_cast<uintptr_t>(p);
+  if (n >= 16) {
+    if ((at & 15) == 0) return ld_cg_v4(p);
+    if ((at & 7) == 0) {
+      const uint2 x = reinterpret_cast<const uint2*>(p)[0], y = reinterpret_cast<const uint2*>(p)[1];
+      return make_uint4(x.x, x.y, y.x, y.y);
+    }
+    if ((at & 3) == 0) {
+      const uint32_t* q = reinterpret_cast<const uint32_t*>(p);
+      return make_uint4(q[0], q[1], q[2], q[3]);
+    }
+  }
+  uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+  for (int i = 0; i < 16; ++i)
+    if ((size_t)i < n) w[i >> 2] |= (uint32_t)p[i] << (8 * (i & 3));
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// Store the first n (> 0, at most 16 used) bytes of v at p, never a byte past p + n: a partial vector must not clobber what
+// follows the segment.
+__device__ __forceinline__ void a2av_store(unsigned char* p, size_t n, uint4 v) {
+  const uintptr_t at = reinterpret_cast<uintptr_t>(p);
+  if (n >= 16) {
+    if ((at & 15) == 0) return st_cg_v4(p, v);
+    if ((at & 7) == 0) {
+      reinterpret_cast<uint2*>(p)[0] = make_uint2(v.x, v.y);
+      reinterpret_cast<uint2*>(p)[1] = make_uint2(v.z, v.w);
+      return;
+    }
+    if ((at & 3) == 0) {
+      uint32_t* q = reinterpret_cast<uint32_t*>(p);
+      q[0] = v.x; q[1] = v.y; q[2] = v.z; q[3] = v.w;
+      return;
+    }
+  }
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 16; ++i)
+    if ((size_t)i < n) p[i] = (unsigned char)(w[i >> 2] >> (8 * (i & 3)));
+}
+
+// Stage bytes [off, off + kA2avChunk) of every send into `half` of this rank's buffer (slot d for rank d).
+__device__ __forceinline__ void a2av_stage(const A2AVArgs& a, unsigned char* half, size_t off, size_t first, size_t stride) {
+  for (size_t j = first; j < kA2avChunkVec; j += stride) {
+    const size_t at = off + j * 16;
+#pragma unroll
+    for (int d = 0; d < B2_MAX_RANKS; ++d)
+      if (d < a.world && at < a.src_bytes[d])
+        st_cg_v4(half + (size_t)d * kA2avChunk + j * 16, a2av_load(a.src[d] + at, a.src_bytes[d] - at));
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) alltoallv_kernel(A2AVArgs a) {
+  const int rank = a.rank, world = a.world;
+  uint32_t epoch = barrier_epoch_load(a.sig, rank);
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  const size_t first = (size_t)blockIdx.x * kThreads + threadIdx.x;
+  const size_t half_bytes = (size_t)world * kA2avChunk;
+  unsigned char* mine = reinterpret_cast<unsigned char*>(a.bufs.p[rank]);
+  __shared__ unsigned long long take_s[B2_MAX_RANKS];       // bytes this rank takes from rank s
+  __shared__ unsigned long long longest;                    // the longest send of any rank
+  if (threadIdx.x < (unsigned)world) st_cg_u64(mine + 8 * threadIdx.x, a.src_bytes[threadIdx.x]);
+  if (threadIdx.x == 0) longest = 0;
+  a2av_stage(a, mine + kA2avHeader, 0, first, stride);
+  block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every header and chunk 0 are in place
+  if (threadIdx.x < (unsigned)(world * world)) {
+    const int s = threadIdx.x / world, d = threadIdx.x % world;
+    const unsigned long long n = ld_cg_u64(reinterpret_cast<const unsigned char*>(a.bufs.p[s]) + 8 * d);
+    atomicMax(&longest, n);
+    if (d == rank) take_s[s] = n < a.dst_bytes[s] ? n : a.dst_bytes[s];
+  }
+  __syncthreads();
+  unsigned long long take[B2_MAX_RANKS];
+#pragma unroll
+  for (int s = 0; s < B2_MAX_RANKS; ++s) take[s] = s < world ? take_s[s] : 0ull;
+  const unsigned long long rounds = longest == 0 ? 1ull : (longest + kA2avChunk - 1) / kA2avChunk;
+  for (unsigned long long k = 0; k < rounds; ++k) {
+    const size_t off = (size_t)k * kA2avChunk;
+    const size_t cur = kA2avHeader + (size_t)(k & 1) * half_bytes + (size_t)rank * kA2avChunk;
+    for (size_t j = first; j < kA2avChunkVec; j += stride) {
+      const size_t at = off + j * 16;
+      uint4 raw[B2_MAX_RANKS];
+#pragma unroll
+      for (int s = 0; s < B2_MAX_RANKS; ++s)
+        if (s < world && at < take[s]) raw[s] = ld_cg_v4(reinterpret_cast<const unsigned char*>(a.bufs.p[s]) + cur + j * 16);
+#pragma unroll
+      for (int s = 0; s < B2_MAX_RANKS; ++s)
+        if (s < world && at < take[s]) a2av_store(a.dst[s] + at, take[s] - at, raw[s]);
+    }
+    if (k + 1 < rounds) a2av_stage(a, mine + kA2avHeader + (size_t)((k + 1) & 1) * half_bytes, off + kA2avChunk, first, stride);
+    block_barrier_all_ranks(a.sig, rank, world, ++epoch);        // round k read; after the last, no peer reads this buffer
+  }
+  if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+}
+
 // ------------------------------------------------------------------------------------------ barrier only
 __global__ void __launch_bounds__(32) barrier_kernel(SignalPads sig, int rank, int world) {
   uint32_t epoch = barrier_epoch_load(sig, rank);
@@ -952,6 +1093,39 @@ int b2_alltoall_launch(int variant, const PeerPtrs* bufs, const b2::SignalPads* 
   b2::ARArgs a;
   if (!b2::segments_args(variant, bufs, sig, src, dst, n_vec, rank, world, inbox, ll_cap, &a)) return (int)cudaErrorInvalidValue;
   b2::launch_segments<b2::LaneF32, b2::kSum, true>(variant, b2::segments_grid(variant, n_vec / world, max_blocks), a, stream);
+  return (int)cudaGetLastError();
+}
+
+// The staging layout of the all-to-allv: kA2avChunk bytes per pair and round behind a header of `header` bytes, so a world
+// of W ranks needs header + 2 x W x chunk bytes of symmetric buffer.
+void b2_alltoallv_config(size_t* chunk, size_t* header) {
+  *chunk = b2::kA2avChunk;
+  *header = b2::kA2avHeader;
+}
+
+// All-to-allv of raw bytes (alltoallv_kernel): src[d] / src_bytes[d] is what this rank sends to rank d, dst[p] / dst_bytes[p]
+// where what rank p sends lands; bufs are staging buffers of at least header + 2 x world x chunk bytes (b2_alltoallv_config).
+// The grid is min(chunk / 16 / kThreads, max_blocks) on every rank, whatever the lengths.  Returns cudaError_t as int;
+// cudaErrorInvalidValue, without a launch, for a world outside 1..8, a rank outside [0, world), or a null pointer with a
+// non-zero byte count.
+int b2_alltoallv_launch(const PeerPtrs* bufs, const b2::SignalPads* sig, const void* const* src, const unsigned long long* src_bytes,
+                        void* const* dst, const unsigned long long* dst_bytes, int rank, int world, int max_blocks,
+                        cudaStream_t stream) {
+  if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world || bufs == nullptr || sig == nullptr)
+    return (int)cudaErrorInvalidValue;
+  b2::A2AVArgs a;
+  memset(&a, 0, sizeof(a));
+  a.bufs = *bufs; a.sig = *sig; a.rank = rank; a.world = world;
+  for (int r = 0; r < world; ++r) {
+    if (bufs->p[r] == nullptr || (src_bytes[r] != 0 && src[r] == nullptr) || (dst_bytes[r] != 0 && dst[r] == nullptr))
+      return (int)cudaErrorInvalidValue;
+    a.src[r] = static_cast<const unsigned char*>(src[r]); a.src_bytes[r] = src_bytes[r];
+    a.dst[r] = static_cast<unsigned char*>(dst[r]); a.dst_bytes[r] = dst_bytes[r];
+  }
+  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
+  size_t blocks = (b2::kA2avChunkVec + b2::kThreads - 1) / b2::kThreads;
+  if (blocks > (size_t)max_blocks) blocks = (size_t)max_blocks;
+  b2::alltoallv_kernel<<<dim3((unsigned)blocks), b2::kThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 

@@ -47,6 +47,10 @@ int b2_reduce_scatter_launch(int variant, int dtype, int op, const PeerPtrs* buf
                              size_t ll_cap, cudaStream_t stream);
 int b2_alltoall_launch(int variant, const PeerPtrs* bufs, const SignalPadsH* sig, const void* src, void* dst, size_t n_vec,
                        int rank, int world, int max_blocks, const PeerPtrs* inbox, size_t ll_cap, cudaStream_t stream);
+void b2_alltoallv_config(size_t* chunk, size_t* header);
+int b2_alltoallv_launch(const PeerPtrs* bufs, const SignalPadsH* sig, const void* const* src, const unsigned long long* src_bytes,
+                        void* const* dst, const unsigned long long* dst_bytes, int rank, int world, int max_blocks,
+                        cudaStream_t stream);
 int b2_barrier_launch(const SignalPadsH* sig, int rank, int world, cudaStream_t stream);
 void b2_p2p_config(int* ctas, int* slots, size_t* chunk, int* pad_words);
 int b2_p2p_send_launch(const PeerPtrs* box, const SignalPadsH* sig, const void* src, size_t nbytes, int rank, int peer,
@@ -459,6 +463,41 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                max_blocks, inbox.empty() ? nullptr : &ib, ll_cap, cur_stream()), "alltoall");
   }, py::arg("variant"), py::arg("bufs"), py::arg("sigs"), py::arg("src"), py::arg("dst"), py::arg("n_vec"), py::arg("rank"),
      py::arg("world"), py::arg("max_blocks") = 0, py::arg("inbox") = std::vector<unsigned long long>(), py::arg("ll_cap") = 0);
+  // all-to-allv: srcs[d] (its first src_bytes[d] bytes) goes to rank d; what rank p sends lands in dsts[p], at most
+  // dst_bytes[p] bytes of it.  bufs: staging buffers of header + 2 x world x chunk bytes (alltoallv_config).  Any dtype and
+  // alignment; every rank of one call must run it, whatever its lengths.
+  m.def("alltoallv_config", [] {
+    size_t chunk = 0, header = 0;
+    b2_alltoallv_config(&chunk, &header);
+    return py::make_tuple(chunk, header);
+  }, "(bytes per pair and round, header bytes) of the all-to-allv staging buffer");
+  m.def("alltoallv", [](std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                        std::vector<torch::Tensor> srcs, std::vector<long long> src_bytes, std::vector<torch::Tensor> dsts,
+                        std::vector<long long> dst_bytes, int rank, int world, int max_blocks) {
+    check_world(rank, world, "alltoallv");
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, "alltoallv: one buffer and one signal pad per rank, got ",
+                bufs.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK((int)srcs.size() == world && (int)src_bytes.size() == world && (int)dsts.size() == world &&
+                (int)dst_bytes.size() == world, "alltoallv: one source, one destination and their byte counts per rank, got ",
+                srcs.size(), ", ", src_bytes.size(), ", ", dsts.size(), " and ", dst_bytes.size(), " for world ", world);
+    const void* sp[B2_MAX_RANKS];
+    void* dp[B2_MAX_RANKS];
+    unsigned long long sn[B2_MAX_RANKS], dn[B2_MAX_RANKS];
+    for (int r = 0; r < world; ++r) {
+      check_cuda_contig(srcs[r], "alltoallv: src");
+      check_cuda_contig(dsts[r], "alltoallv: dst");
+      TORCH_CHECK(src_bytes[r] >= 0 && (size_t)src_bytes[r] <= (size_t)srcs[r].nbytes(), "alltoallv: ", src_bytes[r],
+                  " bytes for rank ", r, " from a source of ", srcs[r].nbytes());
+      TORCH_CHECK(dst_bytes[r] >= 0 && (size_t)dst_bytes[r] <= (size_t)dsts[r].nbytes(), "alltoallv: ", dst_bytes[r],
+                  " bytes from rank ", r, " into a destination of ", dsts[r].nbytes());
+      sp[r] = srcs[r].data_ptr(); sn[r] = (unsigned long long)src_bytes[r];
+      dp[r] = dsts[r].data_ptr(); dn[r] = (unsigned long long)dst_bytes[r];
+    }
+    PeerPtrs b = to_ptrs(bufs);
+    SignalPadsH s = to_sig(sigs);
+    ck_cuda(b2_alltoallv_launch(&b, &s, sp, sn, dp, dn, rank, world, max_blocks, cur_stream()), "alltoallv");
+  }, py::arg("bufs"), py::arg("sigs"), py::arg("srcs"), py::arg("src_bytes"), py::arg("dsts"), py::arg("dst_bytes"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
   m.def("barrier", [](std::vector<unsigned long long> sigs, int rank, int world) {
     check_world(rank, world, "barrier");
     TORCH_CHECK((int)sigs.size() == world, "barrier: one signal pad per rank, got ", sigs.size(), " for world ", world);

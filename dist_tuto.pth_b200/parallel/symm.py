@@ -845,6 +845,97 @@ class SymmWorld:
                 raw_out[p * nbytes:(p + 1) * nbytes].copy_(dst[p * slot:p * slot + nbytes])
         return out
 
+    def _splits(self, what: str, splits, t: torch.Tensor) -> List[int]:
+        """Rows of ``t``'s dim 0 per rank: ``splits`` checked against it, or equal ones when it is None."""
+        rows = t.shape[0]
+        if splits is None:
+            if rows % self.world:
+                raise ValueError(f"all_to_all: the {what} has {rows} rows, which do not split equally over world "
+                                 f"{self.world}; give {what}_split_sizes")
+            return [rows // self.world] * self.world
+        s = [int(x) for x in splits]
+        if len(s) != self.world:
+            raise ValueError(f"all_to_all: {what}_split_sizes needs {self.world} entries, got {len(s)}")
+        if any(x < 0 for x in s):
+            raise ValueError(f"all_to_all: {what}_split_sizes has a negative entry: {s}")
+        if sum(s) != rows:
+            raise ValueError(f"all_to_all: {what}_split_sizes sums to {sum(s)}, but the {what} has {rows} rows")
+        return s
+
+    def _segments(self, t: torch.Tensor, splits: List[int]) -> List[torch.Tensor]:
+        """``t``'s rows cut by ``splits``, as uint8 views."""
+        raw = t.reshape(-1).view(torch.uint8)
+        row = raw.numel() // t.shape[0] if t.shape[0] else 0
+        offs = [0]
+        for n in splits:
+            offs.append(offs[-1] + n * row)
+        return [raw[offs[p]:offs[p + 1]] for p in range(self.world)]
+
+    def all_to_all_v_(self, out, inp, output_split_sizes=None, input_split_sizes=None,
+                      max_blocks: Optional[int] = None):
+        """All-to-all with segments of any size, torch's ``all_to_all_single`` with split sizes and its list form
+        ``all_to_all``, copied bit for bit (any dtype).
+
+        Single-tensor form: ``out`` and ``inp`` are tensors of one dtype whose dim 0 is cut by ``output_split_sizes`` /
+        ``input_split_sizes`` (``None``: equal splits); rows p of ``out`` receive rank p's rows for this rank.  List form:
+        ``out`` and ``inp`` are lists of ``world`` tensors of one dtype and any sizes; ``out[p]`` receives rank p's
+        ``inp[rank]``.  Every rank must use the same form.
+
+        Every segment, of any length and alignment, is read and written in place by one kernel that moves fixed chunks per
+        pair in rounds; the round count comes from the lengths every rank publishes, so the staging size and the grid depend on
+        the world size alone.  A receiver takes min(what its peer sends, what it expects): splits that disagree between ranks
+        truncate segments, and bytes beyond are left as they were.  An output that overlaps an input reads from a copy of that
+        input made on the current stream, the only device memory a call allocates.
+
+        A bad argument (a split list of the wrong length, a negative split or one that does not sum to dim 0, a list of the
+        wrong length or of mixed dtypes, or a tensor that is not contiguous, not CUDA or on another device) raises before any
+        launch, on this rank only: its peers are then left inside the kernel until its spin limit reports them
+        (B2_SPIN_LIMIT)."""
+        if isinstance(out, (list, tuple)) or isinstance(inp, (list, tuple)):
+            if not isinstance(out, (list, tuple)) or not isinstance(inp, (list, tuple)):
+                raise TypeError("all_to_all takes two lists of tensors or two tensors")
+            if output_split_sizes is not None or input_split_sizes is not None:
+                raise ValueError("all_to_all: split sizes belong to the single-tensor form")
+            outs, ins = list(out), list(inp)
+            for what, lst in (("output", outs), ("input", ins)):
+                if len(lst) != self.world:
+                    raise ValueError(f"all_to_all needs {self.world} {what} tensors, got {len(lst)}")
+            if not all(isinstance(t, torch.Tensor) and self.supports_raw(t) for t in outs + ins):
+                raise TypeError("fused all_to_all needs contiguous CUDA tensors on this device")
+            if len({t.dtype for t in outs + ins}) != 1:
+                raise ValueError(f"all_to_all needs tensors of one dtype, got {sorted({str(t.dtype) for t in outs + ins})}")
+            dsts = [t.reshape(-1).view(torch.uint8) for t in outs]
+            srcs = [t.reshape(-1).view(torch.uint8) for t in ins]
+        else:
+            if not isinstance(out, torch.Tensor) or not isinstance(inp, torch.Tensor):
+                raise TypeError("all_to_all takes two lists of tensors or two tensors")
+            if not self.supports_raw(out) or not self.supports_raw(inp):
+                raise TypeError("fused all_to_all needs contiguous CUDA tensors on this device")
+            if out.dtype != inp.dtype:
+                raise ValueError(f"all_to_all needs an input and an output of one dtype, got {inp.dtype} and {out.dtype}")
+            if out.dim() == 0 or inp.dim() == 0:
+                raise ValueError("all_to_all with split sizes cuts dim 0, so it needs tensors of at least one dimension")
+            dsts = self._segments(out, self._splits("output", output_split_sizes, out))
+            srcs = self._segments(inp, self._splits("input", input_split_sizes, inp))
+        overlap = lambda a, b: a.numel() and b.numel() and a.data_ptr() < b.data_ptr() + b.numel() and \
+            b.data_ptr() < a.data_ptr() + a.numel()  # noqa: E731
+        if any(overlap(s, d) for s in srcs for d in dsts):
+            if isinstance(inp, torch.Tensor):                  # one copy of the whole input, then its segments
+                srcs = self._segments(inp.clone(), self._splits("input", input_split_sizes, inp))
+            else:
+                srcs = [s.clone() if any(overlap(s, d) for d in dsts) else s for s in srcs]
+        if self.world == 1:
+            n = min(srcs[0].numel(), dsts[0].numel())
+            if n:
+                dsts[0][:n].copy_(srcs[0][:n])
+            return out
+        chunk, header = self.C.alltoallv_config()
+        st = self._staging_for(torch.float32, header + 2 * self.world * chunk)   # the world size alone: allocation is collective
+        mb = self.max_blocks if max_blocks is None else max_blocks
+        self.C.alltoallv(st.ptrs, st.sig_ptrs, srcs, [s.numel() for s in srcs], dsts, [d.numel() for d in dsts], self.rank,
+                         self.world, mb)
+        return out
+
     # ------------------------------------------------------------------ point-to-point
     def send_(self, t: torch.Tensor, dst: int) -> None:
         """Send ``t``'s bytes to global rank ``dst`` (any dtype; copied bit for bit).  Like ``dist.send`` on NCCL it returns
