@@ -777,8 +777,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ------------------------------------------------------------------ wgmma GEMM
   m.def("gemm_available", [] { return b2_gemm_available() != 0; });
-  m.def("gemm_bf16", [](torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor> bias, bool relu, bool out_bf16) {
-    // C[M,N] = A[M,K] @ B[N,K]^T (+bias) (relu) ; A,B bf16 row-major (K contiguous)
+  m.def("gemm_bf16", [](torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor> bias, bool relu, bool out_bf16,
+                        c10::optional<torch::Tensor> out) {
+    // C[M,N] = A[M,K] @ B[N,K]^T (+bias) (relu) ; A,B bf16 row-major (K contiguous).  `out`, if given, receives C in place
+    // (a contiguous [M,N] tensor of the output dtype on A's device, 16-byte aligned), as the batched engine's fixed buffers do.
     check_cuda_contig(a, "a"); check_cuda_contig(b, "b");
     TORCH_CHECK(a.scalar_type() == torch::kBFloat16 && b.scalar_type() == torch::kBFloat16, "bf16 operands");
     TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(1) == b.size(1), "A[M,K], B[N,K]");
@@ -786,12 +788,24 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(K % 8 == 0, "K must be a multiple of 8 (16-byte rows for TMA)");
     const float* bp = nullptr;
     if (bias.has_value()) { TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kFloat32 && bias->numel() == N); bp = bias->data_ptr<float>(); }
-    auto c = torch::empty({M, N}, a.options().dtype(out_bf16 ? torch::kBFloat16 : torch::kFloat32));
+    const auto out_dtype = out_bf16 ? torch::kBFloat16 : torch::kFloat32;
+    torch::Tensor c;
+    if (out.has_value()) {
+      c = *out;
+      TORCH_CHECK(c.is_cuda() && c.device() == a.device(), "gemm_bf16: out must be on the operands' device");
+      TORCH_CHECK(c.scalar_type() == out_dtype, "gemm_bf16: out must be ", out_bf16 ? "bf16" : "fp32");
+      TORCH_CHECK(c.dim() == 2 && c.size(0) == M && c.size(1) == N, "gemm_bf16: out must have shape [M, N]");
+      TORCH_CHECK(c.is_contiguous(), "gemm_bf16: out must be contiguous");
+      TORCH_CHECK((reinterpret_cast<uintptr_t>(c.data_ptr()) & 15) == 0, "gemm_bf16: out must be 16-byte aligned");
+    } else {
+      c = torch::empty({M, N}, a.options().dtype(out_dtype));
+    }
     c10::cuda::CUDAGuard guard(a.device());
     int rc = b2_gemm_bf16_launch(a.data_ptr(), b.data_ptr(), c.data_ptr(), bp, M, N, K, relu, out_bf16, cur_stream());
     if (rc != 0) throw std::runtime_error(std::string("gemm_bf16: ") + b2_gemm_last_error());
     return c;
-  }, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("relu") = false, py::arg("out_bf16") = true);
+  }, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("relu") = false, py::arg("out_bf16") = true,
+     py::arg("out") = py::none());
 
   // ------------------------------------------------------------------ batched tensor-core engine (csrc/convnet_batched.cu)
   // bufs: [P1, P2, H, DH, dP2, DC, W2K, W2R, W3K, W3T, A1, A2, Hrelu, DLOG, G1, B3P] (see ops/convnet_batched.py)

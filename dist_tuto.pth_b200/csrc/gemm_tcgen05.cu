@@ -214,17 +214,40 @@ bool make_map(CUtensorMap* map, const void* ptr, int rows, int k, int box_rows) 
   return true;
 }
 
+// cudaFuncSetAttribute and the SM count belong to one device: both are cached per device, so a process that launches on
+// cuda:1 after cuda:0 configures the kernels there too.
+constexpr int kMaxDevices = 64;
+
+int current_device() {
+  int dev = -1;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { cudaGetLastError(); return -1; }
+  return dev;
+}
+
+int sm_count() {
+  static int sms[kMaxDevices] = {};
+  const int dev = current_device();
+  if (dev < 0) return 132;
+  if (sms[dev] == 0) {
+    cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
+    if (sms[dev] <= 0) sms[dev] = 132;
+  }
+  return sms[dev];
+}
+
 template <int BN>
 int launch(const void* a, const void* b, void* c, const float* bias, int M, int N, int K, int relu, int out_bf16,
            cudaStream_t stream) {
   CUtensorMap ma, mb;
   if (!make_map(&ma, a, M, K, BM) || !make_map(&mb, b, N, K, BN)) return -1;
   const size_t smem = sizeof(SmemLayout<BN, Cfg<BN>::STAGES>) + 1024;
-  static bool configured = false;
-  if (!configured) {
+  static bool configured[kMaxDevices] = {};
+  const int dev = current_device();
+  if (dev < 0) { g_err = "no current CUDA device"; return -2; }
+  if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { g_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e); return -2; }
-    configured = true;
+    configured[dev] = true;
   }
   dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN);
   gemm_bf16_kernel<BN><<<grid, kThreads, smem, stream>>>(ma, mb, c, bias, M, N, K, relu, out_bf16);
@@ -238,32 +261,21 @@ int launch_persistent(const void* a, const void* b, void* c, const float* bias, 
   CUtensorMap ma, mb;
   if (!make_map(&ma, a, M, K, BM) || !make_map(&mb, b, N, K, PBN)) return -1;
   const size_t smem = sizeof(PSmem) + 1024;
-  static int sms = 0;
-  if (sms == 0) {
+  static bool configured[kMaxDevices] = {};
+  const int dev = current_device();
+  if (dev < 0) { g_err = "no current CUDA device"; return -2; }
+  if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { g_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e); return -2; }
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
+    configured[dev] = true;
   }
+  const int sms = sm_count();
   const int tiles = ((M + BM - 1) / BM) * ((N + PBN - 1) / PBN);
   const int grid = tiles < sms ? tiles : sms;
   gemm_bf16_persistent_kernel<<<grid, kThreads, smem, stream>>>(ma, mb, c, bias, M, N, K, relu, out_bf16);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { g_err = std::string("launch: ") + cudaGetErrorString(e); return -3; }
   return 0;
-}
-
-int sm_count() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
-  return sms;
 }
 
 }  // namespace gemm

@@ -56,3 +56,37 @@ def test_tc_linear_is_a_drop_in_linear_on_cpu():
     ref.load_state_dict(m.state_dict())                                   # state-dict compatible
     x = torch.randn(4, 20)
     assert torch.allclose(m(x), ref(x))                                   # CPU tensors take F.linear
+
+
+class _RefusingExt(_FakeExt):
+    """The fake GEMM with the launcher's shape rule: M, N or K = 0 is refused."""
+
+    @staticmethod
+    def gemm_bf16(a, b, bias, relu, out_bf16):
+        if 0 in (a.shape[0], a.shape[1], b.shape[0]):
+            raise RuntimeError("gemm_bf16: bad shape (K must be a multiple of 8)")
+        return _FakeExt.gemm_bf16(a, b, bias, relu, out_bf16)
+
+
+@pytest.mark.parametrize("M,N,K", [(0, 10, 16), (5, 0, 16), (5, 10, 0), (0, 0, 0)])
+@pytest.mark.parametrize("use_bias", [True, False])
+def test_empty_shapes_launch_nothing_and_match_f_linear(monkeypatch, M, N, K, use_bias):
+    monkeypatch.setattr(G._ext, "C", lambda: _RefusingExt)
+    g = torch.Generator().manual_seed(1)
+    x = torch.randn(M, K, generator=g, requires_grad=True)
+    w = torch.randn(N, K, generator=g, requires_grad=True)
+    b = torch.randn(N, generator=g, requires_grad=True) if use_bias else None
+    y = G._LinearTC.apply(x, w, b)
+    yr = torch.nn.functional.linear(x.detach().requires_grad_(), w.detach().requires_grad_(), b)
+    assert y.shape == yr.shape == (M, N) and y.dtype == torch.float32 and torch.equal(y, yr.detach())
+    y.backward(torch.ones_like(y))
+    assert x.grad.shape == x.shape and torch.equal(x.grad, torch.ones(M, N) @ w.detach())
+    assert w.grad.shape == w.shape and torch.equal(w.grad, torch.ones(M, N).t() @ x.detach())
+    if use_bias:
+        assert torch.equal(b.grad, torch.full((N,), float(M)))
+    for relu in (False, True):
+        for dt in (torch.float32, torch.bfloat16):
+            out = G.linear_bf16(x.detach(), w.detach(), b, relu=relu, out_dtype=dt)
+            ref = torch.nn.functional.linear(x.detach(), w.detach(), b)
+            ref = (ref.relu() if relu else ref).to(dt)
+            assert out.shape == (M, N) and out.dtype == dt and torch.equal(out, ref.detach())
