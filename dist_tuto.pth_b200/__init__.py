@@ -5,6 +5,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
 
     init_processes / launch / init_from_env            launch.py
     send recv isend irecv                               comm.py
+    P2POp batch_isend_irecv                             comm.py
     all_reduce reduce broadcast scatter gather gather_to_root all_gather barrier new_group
     reduce_scatter reduce_scatter_tensor all_to_all_single all_to_all all_gather_into_tensor      comm.py
     reduce_op get_rank get_world_size                   comm.py
@@ -20,7 +21,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
 from .comm import (reduce_op, ReduceOp, send, recv, isend, irecv, broadcast, reduce, all_reduce,  # noqa: F401
                    scatter, gather, gather_to_root, all_gather, barrier, new_group, get_rank, get_world_size,
                    is_initialized, group, reduce_scatter, reduce_scatter_tensor, all_to_all_single,
-                   all_gather_into_tensor, all_to_all)
+                   all_gather_into_tensor, all_to_all, P2POp, batch_isend_irecv)
 from .launch import (init_processes, init_process, launch, init_from_env, shutdown, find_free_port,  # noqa: F401
                      LaunchError)
 from .ring import allreduce, allreduce_chunked  # noqa: F401

@@ -38,7 +38,9 @@ Design (GPU-first, not a port):
     (``csrc/p2p.cu``) when the peer is given: messages between a pair are
     matched in issue order and ``tag`` is ignored, as NCCL ignores it.
     ``recv(src=None)``, CPU tensors and the two-level world (no ``send_``)
-    stay on torch.
+    stay on torch.  ``batch_isend_irecv`` gives each op the route ``isend`` /
+    ``irecv`` would, and runs all its peer-memory ops in one launch
+    (``SymmWorld.batch_p2p_``), the rest in one ``dist.batch_isend_irecv``.
   * ``group=0`` (the 2017 spelling of "world", train_dist.py:99, ptp.py:26)
     is accepted and mapped to the default group (fixes defect D2).
 """
@@ -54,7 +56,7 @@ __all__ = [
     "reduce_op", "ReduceOp", "send", "recv", "isend", "irecv", "broadcast", "reduce",
     "all_reduce", "scatter", "gather", "gather_to_root", "all_gather", "barrier", "new_group",
     "get_rank", "get_world_size", "is_initialized", "Request", "group_ranks", "reduce_scatter", "reduce_scatter_tensor",
-    "all_to_all_single", "all_gather_into_tensor", "all_to_all",
+    "all_to_all_single", "all_gather_into_tensor", "all_to_all", "P2POp", "batch_isend_irecv",
 ]
 
 
@@ -203,6 +205,77 @@ def irecv(tensor: torch.Tensor, src: Optional[int] = None, group=None, tag: int 
     if w is not None:
         return Request(w.irecv_(tensor, src), tensor)
     return Request(dist.irecv(tensor, src=src, group=_g(group), tag=tag), tensor)
+
+
+class P2POp:
+    """One send or receive of :func:`batch_isend_irecv` (torch's ``P2POp``): ``op`` is ``isend`` or ``irecv`` of this
+    module or of torch.distributed, ``peer`` a global rank."""
+
+    def __init__(self, op, tensor: torch.Tensor, peer: int, group=None, tag: int = 0):
+        if op not in (isend, irecv, dist.isend, dist.irecv):
+            raise ValueError("P2POp takes isend or irecv (of this module or of torch.distributed) as its op")
+        self.op, self.tensor, self.peer, self.group, self.tag = op, tensor, peer, group, tag
+
+
+def _p2p_op(op):
+    """(send, tensor, peer, group, tag) of a ``P2POp`` of this module or of torch.distributed; the group is None for the
+    default group however it was spelled (torch's P2POp stores the default process group itself)."""
+    if isinstance(op, (P2POp, dist.P2POp)):
+        group = _g(op.group)
+        if group is not None and is_initialized() and group is dist.group.WORLD:
+            group = None
+        return op.op in (isend, dist.isend), op.tensor, op.peer, group, op.tag
+    raise ValueError("batch_isend_irecv takes a list of P2POp (of this module or of torch.distributed), got an element of "
+                     f"type {type(op).__name__}")
+
+
+def batch_isend_irecv(p2p_op_list: List[P2POp]) -> List[Request]:
+    """Issue a list of sends and receives at once (torch's ``batch_isend_irecv``); one :class:`Request` per op, in list
+    order.  Exchanges with several peers (rings, halo exchanges, pipeline stages) may list their sends before their
+    receives: all of a batch's transfers progress together.
+
+    Each op takes the route :func:`isend` / :func:`irecv` would give its tensor and peer, so the two sides of a pair agree
+    whether each uses batches or single calls.  On a symmetric world (``backend="b200"``) all the ops that take the
+    peer-memory kernels go out in one launch (``SymmWorld.batch_p2p_``; their Requests share its completion, as NCCL's
+    coalesced works do, and ``tag`` is ignored); the rest go to one ``dist.batch_isend_irecv``.  Both sides of a pair pass
+    the same byte count, as with :func:`isend`.  Raises ValueError before anything is issued for anything but a non-empty
+    list of P2POp, ops of different groups, a non-contiguous tensor, or an op with this rank as its peer on the peer-memory
+    path."""
+    if not isinstance(p2p_op_list, list) or not p2p_op_list:
+        raise ValueError("batch_isend_irecv takes a non-empty list of P2POp")
+    ops = [_p2p_op(op) for op in p2p_op_list]
+    if any(g != ops[0][3] for _, _, _, g, _ in ops):
+        raise ValueError("All ops need to use the same group.")
+    for _, t, _, _, _ in ops:
+        _check(t)
+    mine, theirs = [], []                                   # (position, op) on the peer-memory kernels / on torch
+    world = None
+    for i, (send, t, peer, group, tag) in enumerate(ops):
+        w = _p2p_world(t, group, peer)
+        if w is None:
+            theirs.append(i)
+            continue
+        if peer == get_rank():
+            raise ValueError(f"batch_isend_irecv: rank {peer} cannot {'send' if send else 'recv'} to itself")
+        world = w
+        mine.append(i)
+    reqs: List[Optional[Request]] = [None] * len(ops)
+    if mine:
+        works = world.batch_p2p_([(ops[i][0], ops[i][1], ops[i][2]) for i in mine])
+        for i, work in zip(mine, works):
+            reqs[i] = Request(work, ops[i][1])
+    if theirs:
+        torch_ops = []
+        for i in theirs:
+            op = p2p_op_list[i]
+            if not isinstance(op, dist.P2POp):
+                send, t, peer, group, tag = ops[i]
+                op = dist.P2POp(dist.isend if send else dist.irecv, t, peer, group=group, tag=tag)
+            torch_ops.append(op)
+        works = dist.batch_isend_irecv(torch_ops)
+        for k, i in enumerate(theirs):                       # NCCL coalesces the batch into one work
+            reqs[i] = Request(works[k] if len(works) == len(theirs) else (works[-1] if works else None), ops[i][1])
+    return reqs
 
 
 # --------------------------------------------------------- collectives -------

@@ -57,6 +57,9 @@ int b2_p2p_send_launch(const PeerPtrs* box, const SignalPadsH* sig, const void* 
                        int world, cudaStream_t stream);
 int b2_p2p_recv_launch(const PeerPtrs* box, const SignalPadsH* sig, void* dst, size_t nbytes, int rank, int peer,
                        int world, cudaStream_t stream);
+int b2_p2p_batch_capacity();
+int b2_p2p_batch_launch(const PeerPtrs* box, const SignalPadsH* sig, const int* send, const int* peer, void* const* msg,
+                        const size_t* nbytes, int n_ops, int rank, int world, cudaStream_t stream);
 int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float* params, float* momentum,
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
@@ -548,6 +551,45 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("p2p_recv", [p2p](std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs, torch::Tensor dst, int peer,
                           int rank, int world) { p2p("p2p_recv", false, bufs, sigs, dst, peer, rank, world); },
         py::arg("bufs"), py::arg("sigs"), py::arg("dst"), py::arg("peer"), py::arg("rank"), py::arg("world"));
+  m.def("p2p_batch_capacity", [] { return b2_p2p_batch_capacity(); }, "the most ops one p2p_batch takes");
+  // ops: [(send, tensor, peer)], all in one launch on the current stream (torch's batch_isend_irecv).  Each pair's messages
+  // match in list order, against batches or single p2p_send / p2p_recv on the peer alike; zero-byte ops are dropped.
+  m.def("p2p_batch", [](std::vector<unsigned long long> bufs, std::vector<unsigned long long> sigs,
+                        std::vector<std::tuple<bool, torch::Tensor, int>> ops, int rank, int world) {
+    const char* what = "p2p_batch";
+    check_world(rank, world, what);
+    TORCH_CHECK(world >= 2, what, ": a point-to-point transfer needs a world of at least 2, got ", world);
+    TORCH_CHECK((int)bufs.size() == world && (int)sigs.size() == world, what, ": one mailbox and one signal pad per rank, got ",
+                bufs.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK((long long)ops.size() <= b2_p2p_batch_capacity(), what, ": at most ", b2_p2p_batch_capacity(),
+                " ops per batch, got ", ops.size());
+    for (const auto& op : ops) {
+      const int p = std::get<2>(op);
+      TORCH_CHECK(p >= 0 && p < world, what, ": peer ", p, " is outside [0, ", world, ")");
+      TORCH_CHECK(p != rank, what, ": rank ", rank, " cannot be its own peer");
+    }
+    std::vector<int> send, peer;
+    std::vector<void*> msg;
+    std::vector<size_t> nbytes;
+    for (const auto& op : ops) {
+      const torch::Tensor& t = std::get<1>(op);
+      const int p = std::get<2>(op);
+      check_cuda_contig(t, "every tensor");
+      TORCH_CHECK(t.device() == std::get<1>(ops[0]).device(), what, ": every tensor must be on one device");
+      TORCH_CHECK((uintptr_t)t.data_ptr() % 16 == 0, what, ": every tensor must be 16-byte aligned");
+      const size_t n = (size_t)t.numel() * t.element_size();
+      if (n == 0) continue;
+      send.push_back(std::get<0>(op) ? 1 : 0);
+      peer.push_back(p);
+      msg.push_back(t.data_ptr());
+      nbytes.push_back(n);
+    }
+    if (msg.empty()) return;
+    PeerPtrs b = to_ptrs(bufs); SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(std::get<1>(ops[0]).device());
+    ck_cuda(b2_p2p_batch_launch(&b, &s, send.data(), peer.data(), msg.data(), nbytes.data(), (int)msg.size(), rank, world,
+                                cur_stream()), what);
+  }, py::arg("bufs"), py::arg("sigs"), py::arg("ops"), py::arg("rank"), py::arg("world"));
   m.def("allreduce_sgd", [](std::vector<unsigned long long> grads, std::vector<unsigned long long> sigs, torch::Tensor params,
                             torch::Tensor momentum, c10::optional<torch::Tensor> step, double lr, double mu, double scale,
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,

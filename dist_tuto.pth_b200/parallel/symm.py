@@ -27,6 +27,8 @@ segment) and never synchronises the host.
 Point-to-point: ``send_``, ``recv_``, ``isend_`` and ``irecv_`` (raw bytes, any dtype) move messages through a mailbox
 every world of more than one rank allocates when it is built (``csrc/p2p.cu``).  Each (peer, direction) pair has its own
 stream, so a receive is never queued behind a send that waits for its peer; like NCCL they never synchronise the host.
+``batch_p2p_`` runs a whole list of sends and receives in one launch (torch's ``batch_isend_irecv``), ordered against the
+single calls through those pair streams.
 """
 from __future__ import annotations
 
@@ -969,10 +971,7 @@ class SymmWorld:
             raise ValueError(f"{what}: rank {peer_rank} cannot {what} to itself")
         if not self.supports_raw(t):
             raise TypeError(f"peer-memory {what} needs a contiguous CUDA tensor on this device")
-        stream = self._p2p_streams.get((peer, send))
-        if stream is None:                                     # a CUDA stream of its own, never one of torch's pooled ones
-            stream = torch.cuda.ExternalStream(self.C.stream_create(self.device.index), device=self.device)
-            self._p2p_streams[(peer, send)] = stream
+        stream = self._p2p_stream((peer, send))
         stream.wait_stream(torch.cuda.current_stream(self.device))
         raw = t.view(-1).view(torch.uint8)
         with torch.cuda.stream(stream):
@@ -987,6 +986,61 @@ class SymmWorld:
         done = torch.cuda.Event()
         done.record(stream)
         return P2PWork(done, self.device)
+
+    def _p2p_stream(self, key) -> torch.cuda.Stream:
+        """The stream of a (peer, direction) pair, or of a batch's set of pairs: a CUDA stream of its own, created on first
+        use, never one of torch's pooled ones (two of those can be one CUDA stream)."""
+        stream = self._p2p_streams.get(key)
+        if stream is None:
+            stream = torch.cuda.ExternalStream(self.C.stream_create(self.device.index), device=self.device)
+            self._p2p_streams[key] = stream
+        return stream
+
+    def batch_p2p_(self, ops) -> List["P2PWork"]:
+        """Every transfer of ``ops`` -- ``[(send, tensor, global peer)]`` -- in one kernel launch (torch's
+        ``batch_isend_irecv``); one :class:`P2PWork` per op, all on the batch's completion event, as NCCL's coalesced works.
+
+        Messages of a pair match in issue order, whether either side uses batches or single ``isend_`` / ``irecv_``: the
+        batch waits for the current stream and for the streams of every (peer, direction) it touches, and those streams
+        wait for the batch before their next transfer.  It runs on a stream of its own per set of pairs, so it is only ever
+        queued behind a batch with exactly its pairs, which it would have to follow anyway.  A list is never split: a batch
+        that sends more than a pair's mailbox holds before it receives completes only because all its transfers run at once.
+        Unaligned tensors go through aligned scratch copies on the batch's stream.  Raises before any launch for a peer
+        equal to this rank, a peer outside the world, a tensor this world cannot take, or more ops than one launch holds."""
+        ops = [(bool(send), t, peer_rank) for send, t, peer_rank in ops]
+        cap = self.C.p2p_batch_capacity()
+        if len(ops) > cap:
+            raise ValueError(f"batch_isend_irecv: at most {cap} peer-memory ops per batch, got {len(ops)}")
+        local = [(send, t, self.local_rank(peer_rank)) for send, t, peer_rank in ops]
+        for (send, t, peer), (_, _, peer_rank) in zip(local, ops):
+            if peer == self.rank:
+                raise ValueError(f"batch_isend_irecv: rank {peer_rank} cannot {'send' if send else 'recv'} to itself")
+        for send, t, _ in local:
+            if not self.supports_raw(t):
+                raise TypeError(f"peer-memory {'send' if send else 'recv'} needs a contiguous CUDA tensor on this device")
+        pairs = sorted({(peer, send) for send, _, peer in local})
+        stream = self._p2p_stream(("batch",) + tuple(pairs))
+        stream.wait_stream(torch.cuda.current_stream(self.device))
+        for key in pairs:
+            stream.wait_stream(self._p2p_stream(key))          # earlier transfers of these pairs come first
+        with torch.cuda.stream(stream):
+            launch, back = [], []
+            for send, t, peer in local:
+                raw = t.view(-1).view(torch.uint8)
+                buf = raw if raw.data_ptr() % 16 == 0 else (raw.clone() if send else torch.empty_like(raw))
+                launch.append((send, buf, peer))
+                if not send and buf is not raw:
+                    back.append((raw, buf))
+            self.C.p2p_batch(self.p2p.ptrs, self.p2p.sig_ptrs, launch, self.rank, self.world)
+            for raw, buf in back:
+                raw.copy_(buf)
+        for _, t, _ in local:
+            t.record_stream(stream)                            # no tensor's memory is reused while the batch runs
+        done = torch.cuda.Event()
+        done.record(stream)
+        for key in pairs:
+            self._p2p_streams[key].wait_event(done)            # later transfers of these pairs come after it
+        return [P2PWork(done, self.device) for _ in local]
 
     def _staging_for(self, dtype, nbytes: int) -> SymmHandle:
         st = self._staging.get(dtype)
