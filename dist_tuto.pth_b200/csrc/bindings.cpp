@@ -64,10 +64,10 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            const b2::LrSchedule* sched, cudaStream_t stream);
+                            const b2::LrSchedule* sched, float wd, int nesterov, cudaStream_t stream);
 int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const long long* steps, float* out, long long n,
                                cudaStream_t stream);
-int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad,
+int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
                        cudaStream_t stream);
 size_t b2_convnet_smem_bytes();
 int b2_convnet_npar();
@@ -78,7 +78,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
                            float* det_partials, float* factors, int input_ready, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
-                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, cudaStream_t stream);
+                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
+                         cudaStream_t stream);
 int b2_convnet_eval_max_ctas(int dev);
 int b2_convnet_eval_samples_per_cta();
 int b2_convnet_eval_launch(const float* params, const void* x, int x_u8, const long long* target, double* result, int* slots,
@@ -149,6 +150,12 @@ void check_cuda_contig(const torch::Tensor& t, const char* name) {
 
 // An lr schedule from its plain-tuple form (ops/optim.LRSchedule.as_tuple):
 //   (kind, warmup, total, start, gamma, min_factor, milestones); None -> no schedule (the lr as given)
+// torch.optim.SGD's rules for weight decay and Nesterov momentum (dampening is always 0 here)
+void check_sgd_options(double weight_decay, bool nesterov, double mu, const char* what) {
+  TORCH_CHECK(weight_decay >= 0.0, what, ": weight_decay must be >= 0, got ", weight_decay);
+  TORCH_CHECK(!nesterov || mu != 0.0, what, ": nesterov needs a nonzero momentum");
+}
+
 b2::LrSchedule to_sched(const py::object& o) {
   b2::LrSchedule s;
   std::memset(&s, 0, sizeof(s));
@@ -220,7 +227,7 @@ struct ExecutorPy {
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
              int max_in_flight, int cluster, torch::Tensor aux, std::vector<unsigned long long> inbox,
              torch::Tensor loss_hist, bool wire_bf16, c10::optional<torch::Tensor> grad_slots, c10::optional<torch::Tensor> factors,
-             py::object lr_schedule)
+             py::object lr_schedule, double weight_decay, bool nesterov)
       : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
@@ -261,6 +268,8 @@ struct ExecutorPy {
     }
     c.wire_bf16 = wire_bf16 ? 1 : 0;
     c.sched = to_sched(lr_schedule);
+    check_sgd_options(weight_decay, nesterov, mu, "StepExecutor");
+    c.wd = (float)weight_decay; c.nesterov = nesterov ? 1 : 0;
     const int cap = std::max(1, l.impl->num_slots() - 2);
     c10::cuda::CUDAGuard guard(params.device());
     c10::cuda::getCurrentCUDAStream().synchronize();     // the executor's streams do not wait for work queued on this one
@@ -594,8 +603,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                             torch::Tensor momentum, c10::optional<torch::Tensor> step, double lr, double mu, double scale,
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,
                             c10::optional<torch::Tensor> aux, std::vector<unsigned long long> inbox, bool wire_bf16,
-                            py::object lr_schedule) {
+                            py::object lr_schedule, double weight_decay, bool nesterov) {
     check_world(rank, world, "allreduce_sgd");
+    check_sgd_options(weight_decay, nesterov, mu, "allreduce_sgd");
     TORCH_CHECK((int)grads.size() == world && (int)sigs.size() == world, "allreduce_sgd: one gradient bucket and one signal pad "
                 "per rank, got ", grads.size(), " and ", sigs.size(), " for world ", world);
     check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
@@ -613,20 +623,24 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_allreduce_sgd_launch(&g, &s, params.data_ptr<float>(), momentum.data_ptr<float>(), st, (size_t)params.numel(),
                                     (float)lr, (float)mu, (float)scale, rank, world, zero_grads, grad_stride, dc, ax,
-                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, &sched, cur_stream()),
+                                    inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, &sched, (float)weight_decay,
+                                    nesterov ? 1 : 0, cur_stream()),
             "allreduce_sgd launch");
   }, py::arg("grads"), py::arg("sigs"), py::arg("params"), py::arg("momentum"), py::arg("step"), py::arg("lr"), py::arg("mu"),
      py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("zero_grads"), py::arg("grad_stride") = 0,
      py::arg("done_counter") = py::none(), py::arg("aux") = py::none(), py::arg("inbox") = std::vector<unsigned long long>(),
-     py::arg("wire_bf16") = false, py::arg("lr_schedule") = py::none());
-  m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad) {
+     py::arg("wire_bf16") = false, py::arg("lr_schedule") = py::none(), py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
+  m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad,
+                       bool nesterov) {
+    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat: nesterov needs a nonzero momentum");
     check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
     TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32);
     TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel());
     TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0, "16-byte aligned buffers");
     ck_cuda(b2_sgd_flat_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), (float)lr,
-                               (float)mu, (float)wd, zero_grad, cur_stream()), "sgd_flat launch");
-  });
+                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, cur_stream()), "sgd_flat launch");
+  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
+     py::arg("nesterov") = false);
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });
@@ -756,7 +770,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("reduce_sgd", [](torch::Tensor slots, int n_slots, torch::Tensor factors, int n_samples, torch::Tensor params,
                          torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,
-                         c10::optional<torch::Tensor> grads, int64_t grad_stride, py::object lr_schedule) {
+                         c10::optional<torch::Tensor> grads, int64_t grad_stride, py::object lr_schedule, double weight_decay,
+                         bool nesterov) {
     // one-GPU optimizer step from convnet_step(..., det_partials=slots, factors=factors): the local gradient is summed from
     // the first n_slots slots and n_samples factor rows in a fixed order, then SGD is applied to it.  The gradient bucket is
     // not read; given `grads`, its other-parity half is re-zeroed like allreduce_sgd does, so a bucket step may follow.
@@ -780,14 +795,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       g = grads->data_ptr<float>();
     }
     const b2::LrSchedule sched = to_sched(lr_schedule);
+    check_sgd_options(weight_decay, nesterov, mu, "reduce_sgd");
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
                                  slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, &sched,
-                                 cur_stream()),
+                                 (float)weight_decay, nesterov ? 1 : 0, cur_stream()),
             "reduce_sgd launch");
   }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
      py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
-     py::arg("grads") = py::none(), py::arg("grad_stride") = 0, py::arg("lr_schedule") = py::none());
+     py::arg("grads") = py::none(), py::arg("grad_stride") = 0, py::arg("lr_schedule") = py::none(),
+     py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
   m.def("lr_schedule_eval", [](py::object schedule, double lr, torch::Tensor steps) {
     // the fp32 lr the optimizer kernels apply at each step-counter value of `steps`, computed by the same device function
     check_cuda_contig(steps, "steps");
@@ -937,7 +954,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
                     int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor,
                     std::vector<unsigned long long>, torch::Tensor, bool, c10::optional<torch::Tensor>,
-                    c10::optional<torch::Tensor>, py::object>(),
+                    c10::optional<torch::Tensor>, py::object, double, bool>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
@@ -945,7 +962,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("max_in_flight") = 3, py::arg("cluster") = 1, py::arg("aux") = torch::Tensor(),
            py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(),
            py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
-           py::arg("factors") = py::none(), py::arg("lr_schedule") = py::none(), py::keep_alive<1, 2>())
+           py::arg("factors") = py::none(), py::arg("lr_schedule") = py::none(), py::arg("weight_decay") = 0.0,
+           py::arg("nesterov") = false, py::keep_alive<1, 2>())
       .def("chunking", [](ExecutorPy&) { return false; })      // read by bench.py: every step is issued on its own
       .def("flag_mode", [](ExecutorPy&) { return false; })     // read by bench.py: the streams are ordered by events
       .def("stats", [](ExecutorPy& e) {

@@ -35,6 +35,8 @@ struct StepConfig {
   float* grad_slots;                 // one GPU, one CTA per sample: per-CTA slots [B][21888] and per-sample fc1 factors [B][384]
   float* factors;                    // of the step kernel, summed by reduce_sgd (sgd.cu) instead of red.add into the bucket
   LrSchedule sched;                  // lr schedule of every step's update (zero: constant lr)
+  float wd;                          // weight decay (0: none) and Nesterov momentum of every step's update (sgd.cu)
+  int nesterov;
 };
 
 class StepExecutor {

@@ -6,8 +6,8 @@
 //   * allreduce_sgd_push_kernel (default for world > 1): every rank stores its locally reduced bucket, flag-in-data,
 //     into every peer's inbox over NVSwitch and reduces out of its own memory -- one NVLink crossing on the critical path;
 //   * allreduce_sgd_kernel: flag barrier, then every rank loads all peers' buckets (one-shot).  Also the world == 1 path.
-// Both apply  buf = mu*buf + g ; p -= lr*buf  (torch.optim.SGD semantics with dampening 0, no nesterov, no weight
-// decay -- train_dist.py:110), re-zero the gradient bucket of the other step parity for the next `red.add` accumulation,
+// Both apply  buf = mu*buf + g ; p -= lr*buf  (torch.optim.SGD semantics with dampening 0 -- train_dist.py:110), or, in their
+// SgdArgsGeneral instances, the same with torch's weight decay and Nesterov momentum (sgd_device.cuh), re-zero the gradient bucket of the other step parity for the next `red.add` accumulation,
 // keep conv2.weight pre-arranged for the step kernels (`aux`) and bump the device step counter used by the dropout RNG.
 #include <cstdio>
 #include <cstdlib>
@@ -18,7 +18,8 @@
 
 namespace b2 {
 
-__global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
+template <class Args>   // SgdArgs or SgdArgsGeneral (weight decay / Nesterov)
+__global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
   const int rank = a.rank, world = a.world;
   // Step parity (which gradient bucket is live) + step bump.  Thread 0 of every block reads the counter and then
   // checks in with an atomic; the LAST block to check in knows every block has read it and bumps it right away, so
@@ -101,8 +102,9 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(SgdArgs a) {
 // kSched: a.sched is a schedule (kind != LRS_NONE).  Thread 0 then also evaluates the step's lr where it waits for the
 // step counter, and the emits read it from shared memory.  Without a schedule the kernel is compiled without that code:
 // the fp64 schedule code costs this latency-bound kernel registers and instruction order even where it does not run.
-template <bool kSched>
-__global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const float* __restrict__ slots, int n_slots,
+// Args: SgdArgs, or SgdArgsGeneral for weight decay / Nesterov, compiled in for the same reason.
+template <bool kSched, class Args>
+__global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(Args a, const float* __restrict__ slots, int n_slots,
                                                                const float* __restrict__ factors, int n_samples, float* loss_acc) {
   __shared__ cn::RedSmem s;
   __shared__ unsigned long long s_step;
@@ -171,7 +173,10 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(SgdArgs a, const 
 // bit-identical and equal to the barrier variant.  epoch = step + 1 (its wrap to 0, the value of a freshly zeroed line,
 // is sent as 1: epoch 1 has the other parity); lines are double-buffered by step parity: a peer can only write parity p
 // again two steps later, which needs my push of the step in between, which I issue after I finished reading parity p.
-__global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_push_kernel(SgdArgs a) {
+// The SgdArgsGeneral instance asks for one CTA per SM: left to itself ptxas aims that instance at three 512-thread CTAs per
+// SM, 40 registers, and spills; the grid (<= 64 CTAs) never needs more than one per SM.  0: the default instance's bounds.
+template <class Args>
+__global__ void __launch_bounds__(kSgdThreads, std::is_same<Args, SgdArgs>::value ? 0 : 1) allreduce_sgd_push_kernel(Args a) {
   __shared__ unsigned long long s_step;
   __shared__ float s_lr;
   pdl_wait();
@@ -219,7 +224,8 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const float* __restrict
   reinterpret_cast<float4*>(grads + (size_t)(st & 1ull) * (size_t)grad_stride)[v] = acc;
 }
 
-// Plain flat momentum SGD (generic models: gradients already averaged in `grad`)
+// Plain flat momentum SGD (generic models: gradients already averaged in `grad`).  kNesterov: step along g + mu*m instead of m.
+template <bool kNesterov>
 __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, float* __restrict__ m,
                                                        const float* __restrict__ g, size_t n, float lr, float mu,
                                                        float wd, int zero_grad, float* gw) {
@@ -231,7 +237,11 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
     float4 mv = reinterpret_cast<float4*>(m)[i];
     gv.x = fmaf(wd, pv.x, gv.x); gv.y = fmaf(wd, pv.y, gv.y); gv.z = fmaf(wd, pv.z, gv.z); gv.w = fmaf(wd, pv.w, gv.w);
     mv.x = fmaf(mu, mv.x, gv.x); mv.y = fmaf(mu, mv.y, gv.y); mv.z = fmaf(mu, mv.z, gv.z); mv.w = fmaf(mu, mv.w, gv.w);
-    pv.x = fmaf(-lr, mv.x, pv.x); pv.y = fmaf(-lr, mv.y, pv.y); pv.z = fmaf(-lr, mv.z, pv.z); pv.w = fmaf(-lr, mv.w, pv.w);
+    float4 dv = mv;
+    if (kNesterov) {
+      dv.x = fmaf(mu, mv.x, gv.x); dv.y = fmaf(mu, mv.y, gv.y); dv.z = fmaf(mu, mv.z, gv.z); dv.w = fmaf(mu, mv.w, gv.w);
+    }
+    pv.x = fmaf(-lr, dv.x, pv.x); pv.y = fmaf(-lr, dv.y, pv.y); pv.z = fmaf(-lr, dv.z, pv.z); pv.w = fmaf(-lr, dv.w, pv.w);
     reinterpret_cast<float4*>(p)[i] = pv;
     reinterpret_cast<float4*>(m)[i] = mv;
     if (zero_grad) reinterpret_cast<float4*>(gw)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -240,7 +250,7 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
     for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
       const float gt = fmaf(wd, p[t], g[t]);
       m[t] = fmaf(mu, m[t], gt);
-      p[t] = fmaf(-lr, m[t], p[t]);
+      p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
       if (zero_grad) gw[t] = 0.f;
     }
   }
@@ -265,9 +275,11 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            const b2::LrSchedule* sched, cudaStream_t stream) {
+                            const b2::LrSchedule* sched, float wd, int nesterov, cudaStream_t stream) {
   if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return (int)cudaErrorInvalidValue;
-  b2::SgdArgs a;
+  if (!(wd >= 0.f)) return (int)cudaErrorInvalidValue;
+  b2::SgdArgsGeneral a;
+  a.wd = wd; a.nesterov = nesterov ? 1 : 0;
   a.phase_ts = g_phase_ts;
   memset(&a.sched, 0, sizeof(a.sched));
   if (sched != nullptr) a.sched = *sched;
@@ -298,16 +310,23 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel, a)
-              : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel, a);
+  const b2::SgdArgs& plain = a;    // the default instances take SgdArgs alone
+  if (wd != 0.f || nesterov)
+    return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgsGeneral>, a)
+                : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgsGeneral>, a);
+  return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgs>, plain)
+              : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgs>, plain);
 }
 
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
-                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, cudaStream_t stream) {
+                         int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
+                         cudaStream_t stream) {
   if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
-  b2::SgdArgs a;
+  if (!(wd >= 0.f)) return (int)cudaErrorInvalidValue;
+  b2::SgdArgsGeneral a;
   memset(&a, 0, sizeof(a));
+  a.wd = wd; a.nesterov = nesterov ? 1 : 0;
   if (sched != nullptr) a.sched = *sched;
   a.params = params; a.momentum = momentum; a.step = step; a.done_counter = done_counter; a.aux = aux;
   a.n_vec = cn::NPAR / 4; a.lr = lr; a.mu = mu; a.scale = 1.f; a.rank = 0; a.world = 1;
@@ -332,9 +351,17 @@ int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* ste
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return a.sched.kind != b2::LRS_NONE
-             ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true>, a, slots, n_slots, factors, n_samples, loss_acc)
-             : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false>, a, slots, n_slots, factors, n_samples, loss_acc);
+  const b2::SgdArgs& plain = a;    // the default instances take SgdArgs alone
+  const bool sch = a.sched.kind != b2::LRS_NONE;
+  if (wd != 0.f || nesterov)
+    return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgsGeneral>, a, slots, n_slots, factors, n_samples,
+                                         loss_acc)
+               : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgsGeneral>, a, slots, n_slots, factors,
+                                         n_samples, loss_acc);
+  return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
+                                       loss_acc)
+             : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
+                                       loss_acc);
 }
 
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
@@ -360,11 +387,14 @@ int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const lo
   return (int)cudaGetLastError();
 }
 
-int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad,
+int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
                        cudaStream_t stream) {
   const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
   const unsigned blocks = (unsigned)((n4 + 255) / 256);
-  b2::sgd_flat_kernel<<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
+  if (nesterov)
+    b2::sgd_flat_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
+  else
+    b2::sgd_flat_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
   return (int)cudaGetLastError();
 }
 

@@ -1,6 +1,7 @@
 // Device-side pieces of the fused [gradient exchange + 1/world + momentum SGD + re-zero] step of the optimizer kernels
 // (sgd.cu), and the phase timestamps the step kernels (convnet.cu) share with them.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "lr_schedule.h"
 
@@ -48,6 +49,16 @@ struct SgdArgs {
   LrSchedule sched;          // lr of the update = lr_schedule_lr(sched, lr, step counter); kind LRS_NONE: lr as it is
 };
 
+// The arguments of the general-update instances of the optimizer kernels: SgdArgs plus torch.optim.SGD's weight decay and
+// Nesterov momentum.  A type of its own rather than two more SgdArgs fields: the default instances keep SgdArgs, so their
+// kernel parameter layout, and with it their code, stays what it was.  The host picks these instances when wd != 0 or
+// nesterov, and sgd_apply_mp then computes
+//   g += wd * p (wd != 0 only);  m = mu * m + g;  p -= lr * (nesterov ? g + mu * m : m)       (one fmaf each)
+struct SgdArgsGeneral : SgdArgs {
+  float wd;                  // >= 0; 0: no decay term at all, as torch skips it
+  int nesterov;
+};
+
 // The lr of the update run at step counter `st`; the kernels evaluate it in thread 0 and share it through shared memory.
 __device__ __forceinline__ float step_lr(const SgdArgs& a, unsigned long long st) { return lr_schedule_lr(a.sched, a.lr, st); }
 
@@ -59,11 +70,24 @@ __device__ __forceinline__ void snapshot_loss(const SgdArgs& a) {
 }
 
 // SGD update of one float4 vector (+ the pre-arranged conv2.weight copies), shared by both exchange variants; sgd_apply_mp
-// takes the vector's momentum and parameters already loaded; `lr` is this step's (step_lr)
-__device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 g, float4 m, float4 p, float lr) {
+// takes the vector's momentum and parameters already loaded; `lr` is this step's (step_lr).  Args: SgdArgs (plain momentum
+// SGD) or SgdArgsGeneral (weight decay / Nesterov).
+template <class Args>
+__device__ __forceinline__ void sgd_apply_mp(const Args& a, size_t v, float4 g, float4 m, float4 p, float lr) {
   g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
+  if constexpr (std::is_same<Args, SgdArgsGeneral>::value) {
+    if (a.wd != 0.f) {
+      g.x = fmaf(a.wd, p.x, g.x); g.y = fmaf(a.wd, p.y, g.y); g.z = fmaf(a.wd, p.z, g.z); g.w = fmaf(a.wd, p.w, g.w);
+    }
+  }
   m.x = fmaf(a.mu, m.x, g.x); m.y = fmaf(a.mu, m.y, g.y); m.z = fmaf(a.mu, m.z, g.z); m.w = fmaf(a.mu, m.w, g.w);
-  p.x = fmaf(-lr, m.x, p.x); p.y = fmaf(-lr, m.y, p.y); p.z = fmaf(-lr, m.z, p.z); p.w = fmaf(-lr, m.w, p.w);
+  if constexpr (std::is_same<Args, SgdArgsGeneral>::value) {
+    const float mun = a.nesterov ? a.mu : 0.f;                          // the step direction d = nesterov ? g + mu*m : m
+    const float4 d = a.nesterov ? make_float4(fmaf(mun, m.x, g.x), fmaf(mun, m.y, g.y), fmaf(mun, m.z, g.z), fmaf(mun, m.w, g.w)) : m;
+    p.x = fmaf(-lr, d.x, p.x); p.y = fmaf(-lr, d.y, p.y); p.z = fmaf(-lr, d.z, p.z); p.w = fmaf(-lr, d.w, p.w);
+  } else {
+    p.x = fmaf(-lr, m.x, p.x); p.y = fmaf(-lr, m.y, p.y); p.z = fmaf(-lr, m.z, p.z); p.w = fmaf(-lr, m.w, p.w);
+  }
   reinterpret_cast<float4*>(a.momentum)[v] = m;
   reinterpret_cast<float4*>(a.params)[v] = p;
   if (a.aux != nullptr && v >= 264 / 4 && v < (264 + 5000) / 4) {      // conv2.weight (flat offset 264, 5000 elements)
@@ -77,7 +101,8 @@ __device__ __forceinline__ void sgd_apply_mp(const SgdArgs& a, size_t v, float4 
     }
   }
 }
-__device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g, float lr) {
+template <class Args>
+__device__ __forceinline__ void sgd_apply(const Args& a, size_t v, float4 g, float lr) {
   sgd_apply_mp(a, v, g, reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v], lr);
 }
 
@@ -86,7 +111,8 @@ __device__ __forceinline__ void sgd_apply(const SgdArgs& a, size_t v, float4 g, 
 //   vector out of MY inbox in fixed rank order (own contribution from registers) => bit-identical replicas; SGD; re-zero the
 //   other-parity bucket.  world == 1: no exchange.  `st` = step index (flag = (uint32)(st + 1), or 1 where that wraps to 0;
 //   parity = st & 1), `lr` = step_lr(a, st).
-__device__ __forceinline__ void exchange_apply_vec(const SgdArgs& a, size_t v, unsigned long long st, float lr) {
+template <class Args>
+__device__ __forceinline__ void exchange_apply_vec(const Args& a, size_t v, unsigned long long st, float lr) {
   const int rank = a.rank, world = a.world;
   const uint32_t epoch = (uint32_t)(st + 1ull);
   const uint32_t flag = epoch == 0u ? 1u : epoch;                       // 0 is "never written"; epoch 1 has the other parity

@@ -19,7 +19,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import Net
 from . import _ext
-from .optim import LRSchedule, schedule_tuple
+from .optim import LRSchedule, check_sgd_options, schedule_tuple
 from .convnet_fused import LAYOUT, NPAR, NPAR_ALLOC, pack_params, unpack_params  # noqa: F401
 
 __all__ = ["BatchedBuffers", "batched_loss_and_grads", "batched_forward", "BatchedTrainer", "STAGES"]
@@ -90,10 +90,13 @@ class BatchedTrainer:
 
     def __init__(self, bsz: int, lr: float = 0.01, momentum: float = 0.5, seed: int = 1234, device=None,
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, use_graph: bool = True,
-                 init_from: Optional[Net] = None, lr_schedule: Optional[LRSchedule] = None):
+                 init_from: Optional[Net] = None, lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0,
+                 nesterov: bool = False):
+        check_sgd_options(momentum, weight_decay, nesterov)
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        self.weight_decay, self.nesterov = float(weight_decay), bool(nesterov)     # torch.optim.SGD's, fixed per trainer
         self._sched = schedule_tuple(lr_schedule)       # computed per update by the optimizer kernel (csrc/lr_schedule.h)
         self.lr_schedule = lr_schedule
         self.group = group
@@ -148,7 +151,7 @@ class BatchedTrainer:
         # zero_grad passes) is what is kept
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
                              self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, 0, self.done_counter, None, [],
-                             lr_schedule=self._sched)
+                             lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov)
         self.C.bt_pack_weights(self.params, self.bufs.as_list())
 
     def step_device(self, x: torch.Tensor, y: torch.Tensor) -> None:
@@ -247,9 +250,12 @@ class BatchedTrainer:
         return {"model": {k: v.detach().cpu().clone() for k, v in p.items()},
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
                 "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
-                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict()}
+                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict(),
+                "weight_decay": self.weight_decay, "nesterov": self.nesterov}
 
     def load_state_dict(self, sd) -> None:
+        """Parameters, momentum and step counter; the lr, its schedule, the weight decay and Nesterov stay the
+        constructor's."""
         self.stream.synchronize()
         model = sd.get("model", sd)
         views = unpack_params(self.params)

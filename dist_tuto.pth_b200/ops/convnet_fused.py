@@ -34,7 +34,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import PARAM_SHAPES, Net
 from . import _ext
-from .optim import LRSchedule, schedule_tuple
+from .optim import LRSchedule, check_sgd_options, schedule_tuple
 
 __all__ = ["LAYOUT", "NPAR", "pack_params", "unpack_params", "convnet_loss_and_grads", "convnet_forward",
            "FusedTrainer"]
@@ -124,10 +124,14 @@ class FusedTrainer:
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, num_slots: int = 4,
                  use_graph: bool = True, init_from: Optional[Net] = None, cluster: Optional[int] = None,
                  deterministic: bool = False, grad_wire: Optional[torch.dtype] = None,
-                 lr_schedule: Optional[LRSchedule] = None):
+                 lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0, nesterov: bool = False):
+        check_sgd_options(momentum, weight_decay, nesterov)
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
+        # torch.optim.SGD's weight_decay (all parameters, biases included) and nesterov, applied by the optimizer kernels'
+        # general-update instances (csrc/sgd_device.cuh); fixed for the trainer's life, so every graph and executor has them
+        self.weight_decay, self.nesterov = float(weight_decay), bool(nesterov)
         # lr_schedule (ops/optim.LRSchedule, step units): the optimizer kernels compute each update's lr from the device step
         # counter (csrc/lr_schedule.h), so graph replays and run_native follow it with fixed launch arguments
         self._sched = schedule_tuple(lr_schedule)
@@ -296,7 +300,7 @@ class FusedTrainer:
             # grads: re-zeroes the other-parity bucket, which a bucket step (the executor's) may use next
             self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
                               self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride,
-                              lr_schedule=self._sched)
+                              lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov)
             return
         if self.deterministic and B * cl <= self.sms:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
@@ -308,7 +312,8 @@ class FusedTrainer:
                                 self.rank * self.bsz, self.training, 1.0 / B, self.p_drop, 0, self.grad_stride, cl, self.aux)
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
                              self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, self.grad_stride,
-                             self.done_counter, self.aux, self._inbox_ptrs, self.wire_bf16, lr_schedule=self._sched)
+                             self.done_counter, self.aux, self._inbox_ptrs, self.wire_bf16, lr_schedule=self._sched,
+                             weight_decay=self.weight_decay, nesterov=self.nesterov)
 
     def _warm(self):
         # forward-only launch: sets the kernel's dynamic-smem attribute outside of graph capture
@@ -426,7 +431,8 @@ class FusedTrainer:
                                       self.training, self.rank, self.world, self.seed, self.rank * self.bsz,
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
                                       self.cluster, self.aux, self._inbox_ptrs, loss_hist, self.wire_bf16,
-                                      *self._native_slots(), lr_schedule=self._sched),
+                                      *self._native_slots(), lr_schedule=self._sched, weight_decay=self.weight_decay,
+                                      nesterov=self.nesterov),
                   self.training)
             self._executors[id(loader)] = ex
         if new_epoch:
@@ -533,12 +539,13 @@ class FusedTrainer:
         return {"model": {k: v.detach().cpu().clone() for k, v in p.items()},
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
                 "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
-                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict()}
+                "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict(),
+                "weight_decay": self.weight_decay, "nesterov": self.nesterov}
 
     def load_state_dict(self, sd):
         """Accepts a trainer checkpoint or a plain ``Net`` state_dict.  Collective when ``steps`` is present (the bucket
-        parity and the exchange epochs derive from the step counter, see :meth:`_reset_exchange`).  The lr and the lr
-        schedule stay the constructor's: ``steps`` is where a schedule continues from."""
+        parity and the exchange epochs derive from the step counter, see :meth:`_reset_exchange`).  The lr, the lr
+        schedule, the weight decay and Nesterov stay the constructor's: ``steps`` is where a schedule continues from."""
         self.sync_lag(0)
         model = sd.get("model", sd)
         views = unpack_params(self.params)

@@ -2,7 +2,8 @@
 
 Parity: ``optim.SGD(model.parameters(), lr=0.01, momentum=0.5)`` + ``optimizer.step()`` + ``optimizer.zero_grad()``
 of the reference's training loop (train_dist.py:110,118,123; tuto.md:283,291,296).  Same update rule as
-``torch.optim.SGD`` (``buf = mu*buf + (g + wd*p)``, ``p -= lr*buf``, dampening 0, no Nesterov).
+``torch.optim.SGD`` (``buf = mu*buf + (g + wd*p)``, ``p -= lr*buf``, or ``p -= lr*(g + wd*p + mu*buf)`` with Nesterov;
+dampening 0).
 
 GPU-first: the gradients of a model already live in flat (symmetric-memory) buckets
 (:class:`~dist_tuto.pth_b200.parallel.ddp.GradBucket`); this optimizer lays the parameters and the momentum out in flat
@@ -19,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "LRSchedule"]
+__all__ = ["FlatSGD", "LRSchedule", "check_sgd_options"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -149,6 +150,14 @@ def schedule_tuple(schedule: Optional[LRSchedule]):
     return schedule.as_tuple()
 
 
+def check_sgd_options(momentum: float, weight_decay: float, nesterov: bool) -> None:
+    """``torch.optim.SGD``'s rules for the options every engine shares (dampening is always 0 here)."""
+    if not float(weight_decay) >= 0.0:
+        raise ValueError(f"weight_decay must be >= 0, got {weight_decay}")
+    if nesterov and float(momentum) == 0.0:
+        raise ValueError("nesterov momentum needs a nonzero momentum")
+
+
 class FlatSGD:
     """``FlatSGD(model)`` where ``model`` is a plain module, a module carrying ``_grad_bucket`` or a
     :class:`DistributedDataParallel` wrapper.
@@ -158,10 +167,12 @@ class FlatSGD:
     ``zero_grad()`` exists for loop compatibility and is then a no-op apart from re-arming the DDP hooks."""
 
     def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
-                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None):
+                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False):
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
+        check_sgd_options(momentum, weight_decay, nesterov)
         self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
+        self.nesterov = bool(nesterov)
         # lr_schedule: update k (k = `steps`, the updates applied so far) uses lr_schedule.lr_at(lr, k), computed on the host
         schedule_tuple(lr_schedule)
         self.lr_schedule, self.steps = lr_schedule, 0
@@ -207,14 +218,15 @@ class FlatSGD:
         for gb, pf, mf in zip(self.buckets, self.param_flats, self.momentum_flats):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
             if pf.is_cuda and g.dtype == torch.float32:
-                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero)
+                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov)
                 continue
-            # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops
+            # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
+            # torch.optim.SGD's order (foreach=False)
             gf = g.to(torch.float32)
             if self.weight_decay:
                 gf = gf.add(pf, alpha=self.weight_decay)
             mf.mul_(self.momentum).add_(gf)
-            pf.add_(mf, alpha=-lr)
+            pf.add_(gf.add(mf, alpha=self.momentum) if self.nesterov else mf, alpha=-lr)
             if self.fused_zero:
                 g.zero_()
         self.steps += 1
@@ -238,7 +250,8 @@ class FlatSGD:
     # ------------------------------------------------------------------ checkpointing
     def state_dict(self) -> dict:
         """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``."""
-        return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "steps": self.steps,
+        return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
+                "steps": self.steps,
                 "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
 
     def named_momentum(self, model: nn.Module) -> dict:
@@ -268,6 +281,7 @@ class FlatSGD:
     def load_state_dict(self, sd: dict) -> None:
         """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
         self.lr, self.momentum, self.weight_decay = float(sd["lr"]), float(sd["momentum"]), float(sd["weight_decay"])
+        self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
         self.steps = int(sd.get("steps", self.steps))
         for m, src in zip(self.momentum_flats, sd["momentum_buffers"]):
             m.copy_(src)

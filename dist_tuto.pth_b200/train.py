@@ -33,7 +33,7 @@ from . import comm
 from .data import default_eval_dataset, partition_dataset
 from .models.convnet import Net
 from .ops.convnet_eval import evaluate
-from .ops.optim import FlatSGD, LRSchedule
+from .ops.optim import FlatSGD, LRSchedule, check_sgd_options
 from .utils import say
 from .utils.checkpoint import load_checkpoint, restore_optimizer, save_checkpoint
 from .utils.trace import NullTracer, Tracer
@@ -52,7 +52,8 @@ class TrainConfig:
                  max_steps: Optional[int] = None, dataset=None, log: Callable[..., None] = say,
                  p_drop: float = 0.5, checkpoint: Optional[str] = None, resume: Optional[str] = None,
                  checkpoint_every: Optional[int] = None, trace: Optional[str] = None, eval_dataset=None,
-                 eval_every: int = 1, lr_schedule: Optional[LRSchedule] = None):
+                 eval_every: int = 1, lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0,
+                 nesterov: bool = False):
         self.epochs, self.lr, self.momentum, self.seed = epochs, lr, momentum, seed
         self.global_batch, self.engine, self.device = global_batch, engine, device
         self.max_steps, self.dataset, self.log, self.p_drop = max_steps, dataset, log, p_drop
@@ -75,6 +76,9 @@ class TrainConfig:
         if lr_schedule is not None and not isinstance(lr_schedule, LRSchedule):
             raise ValueError(f"TrainConfig.lr_schedule must be an LRSchedule or None, got {type(lr_schedule).__name__}")
         self.lr_schedule = lr_schedule
+        # weight_decay / nesterov: torch.optim.SGD's options (dampening 0), the same update on every engine
+        check_sgd_options(momentum, weight_decay, nesterov)
+        self.weight_decay, self.nesterov = float(weight_decay), bool(nesterov)
 
 
 def _spans_machines() -> bool:
@@ -125,7 +129,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     if engine == "fused":
         from .ops.convnet_fused import FusedTrainer
         trainer = FusedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
-                               p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule)
+                               p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule,
+                               weight_decay=cfg.weight_decay, nesterov=cfg.nesterov)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -133,7 +138,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     elif engine == "batched":
         from .ops.convnet_batched import BatchedTrainer
         trainer = BatchedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
-                                 p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule)
+                                 p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule,
+                                 weight_decay=cfg.weight_decay, nesterov=cfg.nesterov)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -159,7 +165,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         broadcast_parameters(model)
         model._grad_bucket = GradBucket(list(model.parameters()))
         # optim.SGD(lr=0.01, momentum=0.5) of train_dist.py:110, over flat buffers: update + zero_grad in one pass
-        optimizer = FlatSGD(model, lr=cfg.lr, momentum=cfg.momentum, lr_schedule=schedule)
+        optimizer = FlatSGD(model, lr=cfg.lr, momentum=cfg.momentum, lr_schedule=schedule, weight_decay=cfg.weight_decay,
+                            nesterov=cfg.nesterov)
         if cfg.resume:
             restore_optimizer(optimizer, model, resume_blob)         # momentum: FlatSGD layout or per-name (fused engine's)
             optimizer.steps = start_steps                            # the schedule continues where the checkpoint stopped
