@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -64,11 +65,15 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            const b2::LrSchedule* sched, float wd, int nesterov, cudaStream_t stream);
+                            const b2::LrSchedule* sched, float wd, int nesterov, float max_norm, float* clip_ws,
+                            float* grad_norm_out, cudaStream_t stream);
 int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const long long* steps, float* out, long long n,
                                cudaStream_t stream);
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
-                       cudaStream_t stream);
+                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream);
+int b2_grad_sqnorm_ws_floats();
+int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
+size_t b2_clip_ws_floats(size_t n_elems);
 size_t b2_convnet_smem_bytes();
 int b2_convnet_npar();
 int b2_convnet_step_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
@@ -79,7 +84,7 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         cudaStream_t stream);
+                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream);
 int b2_convnet_eval_max_ctas(int dev);
 int b2_convnet_eval_samples_per_cta();
 int b2_convnet_eval_launch(const float* params, const void* x, int x_u8, const long long* target, double* result, int* slots,
@@ -156,6 +161,31 @@ void check_sgd_options(double weight_decay, bool nesterov, double mu, const char
   TORCH_CHECK(!nesterov || mu != 0.0, what, ": nesterov needs a nonzero momentum");
 }
 
+// torch.nn.utils.clip_grad_norm_'s max_norm (norm type 2): None (no clipping) or a finite value > 0.  Returns the value the
+// launchers take, 0 for None.
+float check_max_grad_norm(const py::object& o, const char* what) {
+  if (o.is_none()) return 0.f;
+  const double c = o.cast<double>();
+  TORCH_CHECK(std::isfinite(c) && c > 0.0 && (float)c > 0.f && std::isfinite((float)c), what,
+              ": max_grad_norm must be None or a finite value > 0, got ", c);
+  return (float)c;
+}
+
+// The clip instances' workspace for `n` flat elements: fp32 CUDA, b2_clip_ws_floats(n) floats, zero before its first use.
+float* clip_ws_ptr(float max_norm, const c10::optional<torch::Tensor>& ws, int64_t n, const char* what) {
+  if (max_norm == 0.f) return nullptr;
+  TORCH_CHECK(ws.has_value() && ws->is_cuda() && ws->is_contiguous() && ws->scalar_type() == torch::kFloat32 &&
+              ws->numel() >= (int64_t)b2_clip_ws_floats((size_t)n) && (uintptr_t)ws->data_ptr() % 16 == 0, what,
+              ": max_grad_norm needs clip_workspace, a 16-byte aligned fp32 CUDA tensor of clip_workspace_numel(", n, ") = ",
+              b2_clip_ws_floats((size_t)n), " elements");
+  return ws->data_ptr<float>();
+}
+float* grad_norm_ptr(const c10::optional<torch::Tensor>& t, const char* what) {
+  if (!t.has_value()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->numel() >= 1, what, ": grad_norm_out: fp32 CUDA [1]");
+  return t->data_ptr<float>();
+}
+
 b2::LrSchedule to_sched(const py::object& o) {
   b2::LrSchedule s;
   std::memset(&s, 0, sizeof(s));
@@ -227,7 +257,8 @@ struct ExecutorPy {
              int world, uint64_t seed, int64_t sample_base, int64_t grad_stride, double lr, double mu, double p_drop,
              int max_in_flight, int cluster, torch::Tensor aux, std::vector<unsigned long long> inbox,
              torch::Tensor loss_hist, bool wire_bf16, c10::optional<torch::Tensor> grad_slots, c10::optional<torch::Tensor> factors,
-             py::object lr_schedule, double weight_decay, bool nesterov)
+             py::object lr_schedule, double weight_decay, bool nesterov, py::object max_grad_norm,
+             c10::optional<torch::Tensor> clip_workspace, c10::optional<torch::Tensor> grad_norm_out)
       : loader(&l), keep{params, momentum, grads, step, done_counter, loss_acc, in_dev, aux, loss_hist} {
     TORCH_CHECK(l.impl->pinned(), "the native executor needs a pinned loader");
     TORCH_CHECK(raw_u8 == l.impl->raw(), "loader / trainer input dtype mismatch");
@@ -270,6 +301,11 @@ struct ExecutorPy {
     c.sched = to_sched(lr_schedule);
     check_sgd_options(weight_decay, nesterov, mu, "StepExecutor");
     c.wd = (float)weight_decay; c.nesterov = nesterov ? 1 : 0;
+    c.max_norm = check_max_grad_norm(max_grad_norm, "StepExecutor");
+    c.clip_ws = clip_ws_ptr(c.max_norm, clip_workspace, params.numel(), "StepExecutor");
+    c.grad_norm = grad_norm_ptr(grad_norm_out, "StepExecutor");
+    if (c.clip_ws != nullptr) keep.push_back(*clip_workspace);
+    if (c.grad_norm != nullptr) keep.push_back(*grad_norm_out);
     const int cap = std::max(1, l.impl->num_slots() - 2);
     c10::cuda::CUDAGuard guard(params.device());
     c10::cuda::getCurrentCUDAStream().synchronize();     // the executor's streams do not wait for work queued on this one
@@ -603,9 +639,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                             torch::Tensor momentum, c10::optional<torch::Tensor> step, double lr, double mu, double scale,
                             int rank, int world, bool zero_grads, int64_t grad_stride, c10::optional<torch::Tensor> done_counter,
                             c10::optional<torch::Tensor> aux, std::vector<unsigned long long> inbox, bool wire_bf16,
-                            py::object lr_schedule, double weight_decay, bool nesterov) {
+                            py::object lr_schedule, double weight_decay, bool nesterov, py::object max_grad_norm,
+                            c10::optional<torch::Tensor> clip_workspace, c10::optional<torch::Tensor> grad_norm_out) {
     check_world(rank, world, "allreduce_sgd");
     check_sgd_options(weight_decay, nesterov, mu, "allreduce_sgd");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "allreduce_sgd");
     TORCH_CHECK((int)grads.size() == world && (int)sigs.size() == world, "allreduce_sgd: one gradient bucket and one signal pad "
                 "per rank, got ", grads.size(), " and ", sigs.size(), " for world ", world);
     check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
@@ -620,27 +658,57 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(st == nullptr || dc != nullptr, "a step counter needs a done_counter scratch word");
     float* ax = nullptr;
     if (aux.has_value()) { TORCH_CHECK(aux->is_cuda() && aux->scalar_type() == torch::kFloat32 && aux->numel() >= 13000); ax = aux->data_ptr<float>(); }
+    float* ws = clip_ws_ptr(max_norm, clip_workspace, params.numel(), "allreduce_sgd");
+    float* gn = grad_norm_ptr(grad_norm_out, "allreduce_sgd");
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_allreduce_sgd_launch(&g, &s, params.data_ptr<float>(), momentum.data_ptr<float>(), st, (size_t)params.numel(),
                                     (float)lr, (float)mu, (float)scale, rank, world, zero_grads, grad_stride, dc, ax,
                                     inbox.empty() ? nullptr : &ib, nullptr, nullptr, wire_bf16 ? 1 : 0, &sched, (float)weight_decay,
-                                    nesterov ? 1 : 0, cur_stream()),
+                                    nesterov ? 1 : 0, max_norm, ws, gn, cur_stream()),
             "allreduce_sgd launch");
   }, py::arg("grads"), py::arg("sigs"), py::arg("params"), py::arg("momentum"), py::arg("step"), py::arg("lr"), py::arg("mu"),
      py::arg("scale"), py::arg("rank"), py::arg("world"), py::arg("zero_grads"), py::arg("grad_stride") = 0,
      py::arg("done_counter") = py::none(), py::arg("aux") = py::none(), py::arg("inbox") = std::vector<unsigned long long>(),
-     py::arg("wire_bf16") = false, py::arg("lr_schedule") = py::none(), py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
+     py::arg("wire_bf16") = false, py::arg("lr_schedule") = py::none(), py::arg("weight_decay") = 0.0, py::arg("nesterov") = false,
+     py::arg("max_grad_norm") = py::none(), py::arg("clip_workspace") = py::none(), py::arg("grad_norm_out") = py::none());
+  m.def("clip_workspace_numel", [](int64_t n) { return (int64_t)b2_clip_ws_floats((size_t)n); },
+        "elements of the fp32 clip_workspace the optimizer kernels need for n flat parameters with max_grad_norm set");
+  m.def("grad_sqnorm_workspace_numel", [] { return b2_grad_sqnorm_ws_floats(); });
+  m.def("grad_sqnorm", [](torch::Tensor g, torch::Tensor sqnorms, int k, torch::Tensor workspace) {
+    // sqnorms[k] = the sum of squares of g (fp32 per thread and CTA, fp64 across the CTAs in CTA order), for sgd_flat's clipping
+    check_cuda_contig(g, "g"); check_cuda_contig(sqnorms, "sqnorms"); check_cuda_contig(workspace, "workspace");
+    TORCH_CHECK(g.scalar_type() == torch::kFloat32 && (uintptr_t)g.data_ptr() % 16 == 0, "grad_sqnorm: g: 16-byte aligned fp32");
+    TORCH_CHECK(sqnorms.scalar_type() == torch::kFloat64 && k >= 0 && k < sqnorms.numel(), "grad_sqnorm: sqnorms: fp64 with slot k");
+    TORCH_CHECK(workspace.scalar_type() == torch::kFloat32 && workspace.numel() >= b2_grad_sqnorm_ws_floats(),
+                "grad_sqnorm: workspace: fp32 [grad_sqnorm_workspace_numel()], zero before its first use");
+    c10::cuda::CUDAGuard guard(g.device());
+    ck_cuda(b2_grad_sqnorm_launch(g.data_ptr<float>(), (size_t)g.numel(), workspace.data_ptr<float>(), sqnorms.data_ptr<double>(), k,
+                                  cur_stream()), "grad_sqnorm launch");
+  }, py::arg("g"), py::arg("sqnorms"), py::arg("k"), py::arg("workspace"));
   m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad,
-                       bool nesterov) {
+                       bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                       c10::optional<torch::Tensor> grad_norm_out) {
     TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat: nesterov needs a nonzero momentum");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "sgd_flat: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat");
     check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
     TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32);
     TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel());
     TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0, "16-byte aligned buffers");
     ck_cuda(b2_sgd_flat_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), (float)lr,
-                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, cur_stream()), "sgd_flat launch");
+                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+            "sgd_flat launch");
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
-     py::arg("nesterov") = false);
+     py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none());
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });
@@ -771,7 +839,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          torch::Tensor momentum, c10::optional<torch::Tensor> step, c10::optional<torch::Tensor> done_counter,
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,
                          c10::optional<torch::Tensor> grads, int64_t grad_stride, py::object lr_schedule, double weight_decay,
-                         bool nesterov) {
+                         bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> clip_workspace,
+                         c10::optional<torch::Tensor> grad_norm_out) {
     // one-GPU optimizer step from convnet_step(..., det_partials=slots, factors=factors): the local gradient is summed from
     // the first n_slots slots and n_samples factor rows in a fixed order, then SGD is applied to it.  The gradient bucket is
     // not read; given `grads`, its other-parity half is re-zeroed like allreduce_sgd does, so a bucket step may follow.
@@ -796,15 +865,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     const b2::LrSchedule sched = to_sched(lr_schedule);
     check_sgd_options(weight_decay, nesterov, mu, "reduce_sgd");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "reduce_sgd");
+    float* ws = clip_ws_ptr(max_norm, clip_workspace, params.numel(), "reduce_sgd");
+    float* gn = grad_norm_ptr(grad_norm_out, "reduce_sgd");
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
                                  slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, &sched,
-                                 (float)weight_decay, nesterov ? 1 : 0, cur_stream()),
+                                 (float)weight_decay, nesterov ? 1 : 0, max_norm, ws, gn, cur_stream()),
             "reduce_sgd launch");
   }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
      py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
      py::arg("grads") = py::none(), py::arg("grad_stride") = 0, py::arg("lr_schedule") = py::none(),
-     py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
+     py::arg("weight_decay") = 0.0, py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(),
+     py::arg("clip_workspace") = py::none(), py::arg("grad_norm_out") = py::none());
   m.def("lr_schedule_eval", [](py::object schedule, double lr, torch::Tensor steps) {
     // the fp32 lr the optimizer kernels apply at each step-counter value of `steps`, computed by the same device function
     check_cuda_contig(steps, "steps");
@@ -954,7 +1027,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     std::vector<unsigned long long>, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, bool, bool,
                     int, int, uint64_t, int64_t, int64_t, double, double, double, int, int, torch::Tensor,
                     std::vector<unsigned long long>, torch::Tensor, bool, c10::optional<torch::Tensor>,
-                    c10::optional<torch::Tensor>, py::object, double, bool>(),
+                    c10::optional<torch::Tensor>, py::object, double, bool, py::object, c10::optional<torch::Tensor>,
+                    c10::optional<torch::Tensor>>(),
            py::arg("loader"), py::arg("params"), py::arg("momentum"), py::arg("grads"), py::arg("grad_ptrs"),
            py::arg("sig_ptrs"), py::arg("step"), py::arg("done_counter"), py::arg("loss_acc"), py::arg("in_dev"),
            py::arg("raw_u8"), py::arg("training"), py::arg("rank"), py::arg("world"), py::arg("seed"),
@@ -963,7 +1037,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("inbox") = std::vector<unsigned long long>(), py::arg("loss_hist") = torch::Tensor(),
            py::arg("wire_bf16") = false, py::arg("grad_slots") = py::none(),
            py::arg("factors") = py::none(), py::arg("lr_schedule") = py::none(), py::arg("weight_decay") = 0.0,
-           py::arg("nesterov") = false, py::keep_alive<1, 2>())
+           py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("clip_workspace") = py::none(),
+           py::arg("grad_norm_out") = py::none(), py::keep_alive<1, 2>())
       .def("chunking", [](ExecutorPy&) { return false; })      // read by bench.py: every step is issued on its own
       .def("flag_mode", [](ExecutorPy&) { return false; })     // read by bench.py: the streams are ordered by events
       .def("stats", [](ExecutorPy& e) {

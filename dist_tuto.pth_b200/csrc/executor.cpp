@@ -31,11 +31,12 @@ int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, floa
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrsC* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            const b2::LrSchedule* sched, float wd, int nesterov, cudaStream_t stream);
+                            const b2::LrSchedule* sched, float wd, int nesterov, float max_norm, float* clip_ws,
+                            float* grad_norm_out, cudaStream_t stream);
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         cudaStream_t stream);
+                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream);
 int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
@@ -99,7 +100,8 @@ void StepExecutor::record_step(const void* x, const long long* y, float* loss_sn
   if (slots) {
     rc2 = b2_reduce_sgd_launch(cfg_.params, cfg_.momentum, cfg_.step_counter, cfg_.done_counter, cfg_.lr, cfg_.mu, cfg_.aux,
                                cfg_.loss_acc, loss_snapshot, cfg_.grad_slots, cfg_.B, cfg_.factors, cfg_.B, cfg_.grads_local,
-                               cfg_.grad_stride, &cfg_.sched, cfg_.wd, cfg_.nesterov, compute_);
+                               cfg_.grad_stride, &cfg_.sched, cfg_.wd, cfg_.nesterov, cfg_.max_norm, cfg_.clip_ws, cfg_.grad_norm,
+                               compute_);
   } else {
     PeerPtrsC g;
     SignalPadsC sg;
@@ -110,7 +112,7 @@ void StepExecutor::record_step(const void* x, const long long* y, float* loss_sn
     rc2 = b2_allreduce_sgd_launch(&g, &sg, cfg_.params, cfg_.momentum, cfg_.step_counter, (size_t)b2_convnet_npar(),
                                   cfg_.lr, cfg_.mu, 1.f / cfg_.world, cfg_.rank, cfg_.world, 1, cfg_.grad_stride,
                                   cfg_.done_counter, cfg_.aux, cfg_.push ? &ib : nullptr, cfg_.loss_acc, loss_snapshot, cfg_.wire_bf16,
-                                  &cfg_.sched, cfg_.wd, cfg_.nesterov, compute_);
+                                  &cfg_.sched, cfg_.wd, cfg_.nesterov, cfg_.max_norm, cfg_.clip_ws, cfg_.grad_norm, compute_);
   }
   if ((rc != 0 || rc2 != 0) && err_.empty())
     err_ = std::string("kernel launch failed: ") + cudaGetErrorString((cudaError_t)(rc ? rc : rc2));

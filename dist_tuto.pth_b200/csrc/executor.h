@@ -37,6 +37,9 @@ struct StepConfig {
   LrSchedule sched;                  // lr schedule of every step's update (zero: constant lr)
   float wd;                          // weight decay (0: none) and Nesterov momentum of every step's update (sgd.cu)
   int nesterov;
+  float max_norm;                    // gradient-norm clipping of every update (0: none): the clip instances' scratch
+  float* clip_ws;                    // (b2_clip_ws_floats) and where they write the pre-clip norm (optional)
+  float* grad_norm;
 };
 
 class StepExecutor {

@@ -18,8 +18,10 @@
 
 namespace b2 {
 
-template <class Args>   // SgdArgs or SgdArgsGeneral (weight decay / Nesterov)
-__global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
+// Args: SgdArgs, SgdArgsGeneral (weight decay / Nesterov) or SgdArgsClip (+ gradient-norm clipping).  The clip instance asks
+// for one CTA per SM (its grid is at most 64 CTAs): aimed at two, ptxas gives it 64 registers and it spills.
+template <class Args>
+__global__ void __launch_bounds__(kSgdThreads, kClipArgs<Args> ? 1 : 0) allreduce_sgd_kernel(Args a) {
   const int rank = a.rank, world = a.world;
   // Step parity (which gradient bucket is live) + step bump.  Thread 0 of every block reads the counter and then
   // checks in with an atomic; the LAST block to check in knows every block has read it and bumps it right away, so
@@ -52,6 +54,7 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
   const size_t par = dbuf ? (size_t)s_par : 0;
   const size_t cur_off = par * (size_t)a.grad_stride * sizeof(float);
   const size_t oth_off = (par ^ 1) * (size_t)a.grad_stride * sizeof(float);
+  float sq = 0.f;                     // clip instance: this thread's sum of squares of the averaged gradient
   // block-uniform trip count (barrier inside the loop)
   for (size_t base = (size_t)blockIdx.x * kSgdThreads; base < a.n_vec; base += stride) {
     const size_t v = base + threadIdx.x;
@@ -68,7 +71,8 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
           g.x += __uint_as_float(raw[r].x); g.y += __uint_as_float(raw[r].y);
           g.z += __uint_as_float(raw[r].z); g.w += __uint_as_float(raw[r].w);
         }
-      sgd_apply(a, v, g, lr);
+      if constexpr (kClipArgs<Args>) clip_stash(a, v, g, sq);
+      else sgd_apply(a, v, g, lr);
     }
     if (a.zero_grads) {
       if (dbuf) {
@@ -80,6 +84,10 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
     }
   }
   if (world > 1 && threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+  if constexpr (kClipArgs<Args>) {   // phase B: every thread applies the vectors it stashed, clipped by the grid's norm
+    const float coef = clip_grid_coef(a, sq);
+    for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) clip_apply(a, v, coef, lr);
+  }
   if (a.phase_ts != nullptr) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -102,7 +110,9 @@ __global__ void __launch_bounds__(kSgdThreads) allreduce_sgd_kernel(Args a) {
 // kSched: a.sched is a schedule (kind != LRS_NONE).  Thread 0 then also evaluates the step's lr where it waits for the
 // step counter, and the emits read it from shared memory.  Without a schedule the kernel is compiled without that code:
 // the fp64 schedule code costs this latency-bound kernel registers and instruction order even where it does not run.
-// Args: SgdArgs, or SgdArgsGeneral for weight decay / Nesterov, compiled in for the same reason.
+// Args: SgdArgs, or SgdArgsGeneral for weight decay / Nesterov, compiled in for the same reason.  SgdArgsClip: phase A
+// reduces every unit into the clip scratch (a CTA runs several units where the card has fewer than RED_UNITS SMs), and
+// phase B applies the clipped gradient grid-stride after the grid barrier.
 template <bool kSched, class Args>
 __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(Args a, const float* __restrict__ slots, int n_slots,
                                                                const float* __restrict__ factors, int n_samples, float* loss_acc) {
@@ -128,14 +138,21 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(Args a, const flo
     }
   }
   // momentum and parameters of the vectors a thread will update are loaded together with the unit's gradient terms
+  // (clip instance: they are loaded in phase B)
   struct MP { float4 m, p; };
+  struct NoMP {};
   unsigned long long t_mark[3] = {0ull, 0ull, 0ull};
   int last_unit = 0;
+  float sq = 0.f;                    // clip instance: this thread's sum of squares of the local gradient
   cn::reduce_local_grad(
       slots, n_slots, factors, n_samples, (int)blockIdx.x, (int)gridDim.x, s,
-      [&](int v) { return MP{reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]}; },
-      [&](int v, float4 g, const MP& h) {
-        sgd_apply_mp(a, (size_t)v, g, h.m, h.p, kSched ? s_lr : a.lr);   // s_lr, s_step: written before the first barrier
+      [&](int v) {
+        if constexpr (kClipArgs<Args>) return NoMP{};
+        else return MP{reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v]};
+      },
+      [&](int v, float4 g, const auto& h) {
+        if constexpr (kClipArgs<Args>) clip_stash(a, (size_t)v, g, sq);
+        else sgd_apply_mp(a, (size_t)v, g, h.m, h.p, kSched ? s_lr : a.lr);   // s_lr, s_step: written before the first barrier
         if (a.grads.p[0] != nullptr) {
           const size_t z = a.grad_stride > 0 ? (size_t)((s_step & 1ull) ^ 1ull) * (size_t)a.grad_stride : 0;
           st_cg_v4(reinterpret_cast<float*>(a.grads.p[0]) + z + (size_t)v * 4, make_uint4(0u, 0u, 0u, 0u));
@@ -151,6 +168,12 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(Args a, const flo
       });
   __syncthreads();                   // s_step is visible to every thread
   const unsigned long long st = s_step;
+  if constexpr (kClipArgs<Args>) {   // phase B
+    const float coef = clip_grid_coef(a, sq);
+    const float lr = kSched ? s_lr : a.lr;
+    for (size_t v = (size_t)blockIdx.x * cn::RED_T + threadIdx.x; v < a.n_vec; v += (size_t)gridDim.x * cn::RED_T)
+      clip_apply(a, v, coef, lr);
+  }
   if (a.phase_ts != nullptr) {
     if (threadIdx.x == 0) {
       ts_put(a.phase_ts, st, (int)blockIdx.x, TS_OPT_UNIT, last_unit < cn::RED_FC1_TILES ? 1ull : 2ull);
@@ -175,6 +198,7 @@ __global__ void __launch_bounds__(cn::RED_T) reduce_sgd_kernel(Args a, const flo
 // again two steps later, which needs my push of the step in between, which I issue after I finished reading parity p.
 // The SgdArgsGeneral instance asks for one CTA per SM: left to itself ptxas aims that instance at three 512-thread CTAs per
 // SM, 40 registers, and spills; the grid (<= 64 CTAs) never needs more than one per SM.  0: the default instance's bounds.
+// The SgdArgsClip instance (the same bounds) stashes the vectors in phase A and applies them after the grid barrier.
 template <class Args>
 __global__ void __launch_bounds__(kSgdThreads, std::is_same<Args, SgdArgs>::value ? 0 : 1) allreduce_sgd_push_kernel(Args a) {
   __shared__ unsigned long long s_step;
@@ -192,7 +216,14 @@ __global__ void __launch_bounds__(kSgdThreads, std::is_same<Args, SgdArgs>::valu
   const unsigned long long st = s_step;
   const float lr = s_lr;
   const size_t stride = (size_t)gridDim.x * kSgdThreads;
-  for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st, lr);
+  if constexpr (kClipArgs<Args>) {
+    float sq = 0.f;
+    for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st, lr, &sq);
+    const float coef = clip_grid_coef(a, sq);
+    for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) clip_apply(a, v, coef, lr);
+  } else {
+    for (size_t v = (size_t)blockIdx.x * kSgdThreads + threadIdx.x; v < a.n_vec; v += stride) exchange_apply_vec(a, v, st, lr);
+  }
   if (threadIdx.x == 0 && seen == gridDim.x - 1) { *a.done_counter = 0u; *a.step = st + 1ull; }
 }
 
@@ -256,6 +287,93 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
   }
 }
 
+// FlatSGD's clipping, part 1: the sum of squares of one bucket's gradient g[0, n) into sqnorms[k] (fp64).  Each thread sums
+// its squares in fp32 (its float4 vectors in order; thread 0 of CTA 0 also the < 4 tail elements), each CTA in a fixed
+// tree, and the last CTA to finish adds the CTA partials in CTA order in fp64.  ws: [kClipMaxCtas partials | ticket], the
+// ticket zero between calls (the last CTA resets it).
+constexpr int kSqnormThreads = 256;
+__global__ void __launch_bounds__(kSqnormThreads) grad_sqnorm_kernel(const float* __restrict__ g, size_t n, float* ws,
+                                                                      double* __restrict__ sqnorms, int k) {
+  __shared__ float s_part[kClipMaxCtas];
+  __shared__ int s_last;
+  const size_t n4 = n / 4;
+  float sq = 0.f;
+  for (size_t i = (size_t)blockIdx.x * kSqnormThreads + threadIdx.x; i < n4; i += (size_t)gridDim.x * kSqnormThreads) {
+    const float4 v = reinterpret_cast<const float4*>(g)[i];
+    sq = fmaf(v.x, v.x, sq); sq = fmaf(v.y, v.y, sq); sq = fmaf(v.z, v.z, sq); sq = fmaf(v.w, v.w, sq);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0)
+    for (size_t t = n4 * 4; t < n; ++t) sq = fmaf(g[t], g[t], sq);
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, d);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = sq;
+  __syncthreads();
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(ws + kClipMaxCtas);
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < kSqnormThreads / 32; ++w) t += s_part[w];
+    __stcg(ws + blockIdx.x, t);
+    __threadfence();
+    s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    if (s_last) __threadfence();
+  }
+  __syncthreads();
+  if (!s_last) return;
+  if (threadIdx.x < gridDim.x) s_part[threadIdx.x] = __ldcg(ws + threadIdx.x);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int i = 0; i < (int)gridDim.x; ++i) s += (double)s_part[i];
+    sqnorms[k] = s;
+    *ticket = 0u;
+  }
+}
+
+// FlatSGD's clipping, part 2: sgd_flat_kernel's update of one bucket after g *= coef, where coef comes from the total norm
+// sqrt(sum of sqnorms[0, n_buckets) in bucket order), taken in fp64 and rounded once to fp32 (grad_norm_out, optional).
+template <bool kNesterov>
+__global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ p, float* __restrict__ m,
+                                                            const float* __restrict__ g, size_t n, float lr, float mu,
+                                                            float wd, int zero_grad, float* gw, const double* __restrict__ sqnorms,
+                                                            int n_buckets, float max_norm, float* grad_norm_out) {
+  __shared__ float s_coef;
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int k = 0; k < n_buckets; ++k) s += sqnorms[k];
+    const float nrm = __double2float_rn(__dsqrt_rn(s));
+    s_coef = clip_coef(nrm, max_norm);
+    if (blockIdx.x == 0 && grad_norm_out != nullptr) *grad_norm_out = nrm;
+  }
+  __syncthreads();
+  const float c = s_coef;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 pv = reinterpret_cast<float4*>(p)[i];
+    float4 mv = reinterpret_cast<float4*>(m)[i];
+    gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
+    gv.x = fmaf(wd, pv.x, gv.x); gv.y = fmaf(wd, pv.y, gv.y); gv.z = fmaf(wd, pv.z, gv.z); gv.w = fmaf(wd, pv.w, gv.w);
+    mv.x = fmaf(mu, mv.x, gv.x); mv.y = fmaf(mu, mv.y, gv.y); mv.z = fmaf(mu, mv.z, gv.z); mv.w = fmaf(mu, mv.w, gv.w);
+    float4 dv = mv;
+    if (kNesterov) {
+      dv.x = fmaf(mu, mv.x, gv.x); dv.y = fmaf(mu, mv.y, gv.y); dv.z = fmaf(mu, mv.z, gv.z); dv.w = fmaf(mu, mv.w, gv.w);
+    }
+    pv.x = fmaf(-lr, dv.x, pv.x); pv.y = fmaf(-lr, dv.y, pv.y); pv.z = fmaf(-lr, dv.z, pv.z); pv.w = fmaf(-lr, dv.w, pv.w);
+    reinterpret_cast<float4*>(p)[i] = pv;
+    reinterpret_cast<float4*>(m)[i] = mv;
+    if (zero_grad) reinterpret_cast<float4*>(gw)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (i == 0) {
+    for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
+      const float gt = fmaf(wd, p[t], __fmul_rn(g[t], c));
+      m[t] = fmaf(mu, m[t], gt);
+      p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
+      if (zero_grad) gw[t] = 0.f;
+    }
+  }
+}
+
 // out[i] = the lr the optimizer kernels apply when the step counter reads steps[i] (tests tie it to ops/optim.LRSchedule)
 __global__ void __launch_bounds__(256) lr_schedule_eval_kernel(LrSchedule s, float base, const long long* __restrict__ steps,
                                                                float* __restrict__ out, long long n) {
@@ -267,6 +385,20 @@ __global__ void __launch_bounds__(256) lr_schedule_eval_kernel(LrSchedule s, flo
 
 extern "C" {
 
+// A clip instance waits for every CTA of its grid at the grid barrier, so the whole grid must be resident at once: refuse a
+// grid the device cannot hold (`resident`: that kernel's resident-CTA capacity, computed once).
+static int clip_grid_fits(const void* kernel, int threads, unsigned blocks, int* resident) {
+  if (*resident == 0) {
+    int dev = 0, sms = 0, per = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, threads, 0);
+    if (e != cudaSuccess) return (int)e;
+    *resident = per * sms;
+  }
+  return blocks <= (unsigned)b2::kClipMaxCtas && (int)blocks <= *resident ? 0 : (int)cudaErrorCooperativeLaunchTooLarge;
+}
+
 static unsigned long long* g_phase_ts = nullptr;   // opt-in phase timestamps (sgd_device.cuh: TS_STEPS); read at launch
 void b2_set_phase_ts(unsigned long long* p) { g_phase_ts = p; }
 unsigned long long* b2_phase_ts() { return g_phase_ts; }
@@ -275,11 +407,15 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
                             unsigned long long* step, size_t n_elems, float lr, float mu, float scale, int rank,
                             int world, int zero_grads, long long grad_stride, unsigned int* done_counter, float* aux,
                             const PeerPtrs* inbox, const float* loss_acc, float* loss_snapshot, int wire_bf16,
-                            const b2::LrSchedule* sched, float wd, int nesterov, cudaStream_t stream) {
+                            const b2::LrSchedule* sched, float wd, int nesterov, float max_norm, float* clip_ws,
+                            float* grad_norm_out, cudaStream_t stream) {
   if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return (int)cudaErrorInvalidValue;
   if (!(wd >= 0.f)) return (int)cudaErrorInvalidValue;
-  b2::SgdArgsGeneral a;
+  const bool clip = max_norm > 0.f;     // max_norm 0: no clipping
+  if (clip && (clip_ws == nullptr || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
+  b2::SgdArgsClip a;
   a.wd = wd; a.nesterov = nesterov ? 1 : 0;
+  a.max_norm = max_norm; a.clip_ws = clip_ws; a.grad_norm_out = grad_norm_out;
   a.phase_ts = g_phase_ts;
   memset(&a.sched, 0, sizeof(a.sched));
   if (sched != nullptr) a.sched = *sched;
@@ -311,22 +447,36 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
   const b2::SgdArgs& plain = a;    // the default instances take SgdArgs alone
-  if (wd != 0.f || nesterov)
-    return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgsGeneral>, a)
-                : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgsGeneral>, a);
-  return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgs>, plain)
-              : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgs>, plain);
+  const b2::SgdArgsGeneral& general = a;
+  if (!clip) {
+    if (wd != 0.f || nesterov)
+      return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgsGeneral>, general)
+                  : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgsGeneral>, general);
+    return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgs>, plain)
+                : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgs>, plain);
+  }
+  static int resident_push = 0, resident_pull = 0;
+  const int rc = push ? clip_grid_fits((const void*)b2::allreduce_sgd_push_kernel<b2::SgdArgsClip>, b2::kSgdThreads,
+                                       (unsigned)blocks, &resident_push)
+                      : clip_grid_fits((const void*)b2::allreduce_sgd_kernel<b2::SgdArgsClip>, b2::kSgdThreads,
+                                       (unsigned)blocks, &resident_pull);
+  if (rc != 0) return rc;
+  return push ? (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_push_kernel<b2::SgdArgsClip>, a)
+              : (int)cudaLaunchKernelEx(&cfg, b2::allreduce_sgd_kernel<b2::SgdArgsClip>, a);
 }
 
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         cudaStream_t stream) {
+                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream) {
   if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
   if (!(wd >= 0.f)) return (int)cudaErrorInvalidValue;
-  b2::SgdArgsGeneral a;
+  const bool clip = max_norm > 0.f;     // max_norm 0: no clipping
+  if (clip && (clip_ws == nullptr || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
+  b2::SgdArgsClip a;
   memset(&a, 0, sizeof(a));
   a.wd = wd; a.nesterov = nesterov ? 1 : 0;
+  a.max_norm = max_norm; a.clip_ws = clip_ws; a.grad_norm_out = grad_norm_out;
   if (sched != nullptr) a.sched = *sched;
   a.params = params; a.momentum = momentum; a.step = step; a.done_counter = done_counter; a.aux = aux;
   a.n_vec = cn::NPAR / 4; a.lr = lr; a.mu = mu; a.scale = 1.f; a.rank = 0; a.world = 1;
@@ -352,16 +502,23 @@ int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* ste
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
   const b2::SgdArgs& plain = a;    // the default instances take SgdArgs alone
+  const b2::SgdArgsGeneral& general = a;
   const bool sch = a.sched.kind != b2::LRS_NONE;
-  if (wd != 0.f || nesterov)
-    return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgsGeneral>, a, slots, n_slots, factors, n_samples,
+  if (!clip) {
+    if (wd != 0.f || nesterov)
+      return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgsGeneral>, general, slots, n_slots, factors,
+                                           n_samples, loss_acc)
+                 : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgsGeneral>, general, slots, n_slots, factors,
+                                           n_samples, loss_acc);
+    return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
                                          loss_acc)
-               : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgsGeneral>, a, slots, n_slots, factors,
-                                         n_samples, loss_acc);
-  return sch ? (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
-                                       loss_acc)
-             : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
-                                       loss_acc);
+               : (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<false, b2::SgdArgs>, plain, slots, n_slots, factors, n_samples,
+                                         loss_acc);
+  }
+  static int resident = 0;         // one clip instance: a zero schedule gives the lr as it is
+  const int rc = clip_grid_fits((const void*)b2::reduce_sgd_kernel<true, b2::SgdArgsClip>, cn::RED_T, (unsigned)blocks, &resident);
+  if (rc != 0) return rc;
+  return (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgsClip>, a, slots, n_slots, factors, n_samples, loss_acc);
 }
 
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
@@ -388,14 +545,36 @@ int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const lo
 }
 
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
-                       cudaStream_t stream) {
+                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream) {
   const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
   const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  if (max_norm > 0.f) {            // clipped by the norm of grad_sqnorm's n_buckets sums (0: no clipping)
+    if (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY)) return (int)cudaErrorInvalidValue;
+    if (nesterov)
+      b2::sgd_flat_clip_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g), sqnorms,
+                                                                 n_buckets, max_norm, grad_norm_out);
+    else
+      b2::sgd_flat_clip_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g), sqnorms,
+                                                                  n_buckets, max_norm, grad_norm_out);
+    return (int)cudaGetLastError();
+  }
   if (nesterov)
     b2::sgd_flat_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
   else
     b2::sgd_flat_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
   return (int)cudaGetLastError();
 }
+
+// ws: b2_grad_sqnorm_ws_floats() floats, zero before the first call
+int b2_grad_sqnorm_ws_floats() { return b2::kClipMaxCtas + 4; }
+int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream) {
+  size_t blocks = (n / 4 + b2::kSqnormThreads - 1) / b2::kSqnormThreads;
+  if (blocks < 1) blocks = 1;
+  if (blocks > (size_t)b2::kClipMaxCtas) blocks = b2::kClipMaxCtas;
+  b2::grad_sqnorm_kernel<<<(unsigned)blocks, b2::kSqnormThreads, 0, stream>>>(g, n, ws, sqnorms, k);
+  return (int)cudaGetLastError();
+}
+
+size_t b2_clip_ws_floats(size_t n_elems) { return b2::clip_ws_floats(n_elems / 4); }
 
 }  // extern "C"

@@ -59,6 +59,23 @@ struct SgdArgsGeneral : SgdArgs {
   int nesterov;
 };
 
+// The arguments of the clip instances: the general update after torch.nn.utils.clip_grad_norm_ (norm type 2).  Those
+// instances run in two phases around one grid-wide barrier (clip_grid_coef): phase A runs the exchange or reduction as the
+// other instances do but stores each averaged vector (times 1/world) to the scratch and sums its squares; phase B takes
+// the total norm n, coef = min(c / (n + 1e-6), 1) rounded as torch does, and applies g * coef through sgd_apply_mp.
+// The barrier needs every CTA of the grid resident at once; the launchers check that before they launch.
+constexpr int kClipMaxCtas = 256;
+struct SgdArgsClip : SgdArgsGeneral {
+  float max_norm;            // c: finite, > 0
+  float* clip_ws;            // [arrival count, generation, 2 unused | kClipMaxCtas CTA partials | n_vec * 4 averaged gradient]
+  float* grad_norm_out;      // optional: the pre-clip total norm, written by CTA 0
+};
+template <class Args> constexpr bool kClipArgs = std::is_same<Args, SgdArgsClip>::value;
+template <class Args> constexpr bool kGeneralArgs = std::is_base_of<SgdArgsGeneral, Args>::value;
+// The barrier words and partials lead the workspace, so a trainer can share one workspace between kernels of any n_vec.
+constexpr int kClipWsHead = 4 + kClipMaxCtas;
+__host__ __device__ constexpr size_t clip_ws_floats(size_t n_vec) { return kClipWsHead + n_vec * 4; }
+
 // The lr of the update run at step counter `st`; the kernels evaluate it in thread 0 and share it through shared memory.
 __device__ __forceinline__ float step_lr(const SgdArgs& a, unsigned long long st) { return lr_schedule_lr(a.sched, a.lr, st); }
 
@@ -71,17 +88,19 @@ __device__ __forceinline__ void snapshot_loss(const SgdArgs& a) {
 
 // SGD update of one float4 vector (+ the pre-arranged conv2.weight copies), shared by both exchange variants; sgd_apply_mp
 // takes the vector's momentum and parameters already loaded; `lr` is this step's (step_lr).  Args: SgdArgs (plain momentum
-// SGD) or SgdArgsGeneral (weight decay / Nesterov).
+// SGD), SgdArgsGeneral (weight decay / Nesterov) or SgdArgsClip, whose `g` is already averaged and clipped (clip_apply).
 template <class Args>
 __device__ __forceinline__ void sgd_apply_mp(const Args& a, size_t v, float4 g, float4 m, float4 p, float lr) {
-  g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
-  if constexpr (std::is_same<Args, SgdArgsGeneral>::value) {
+  if constexpr (!kClipArgs<Args>) {
+    g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
+  }
+  if constexpr (kGeneralArgs<Args>) {
     if (a.wd != 0.f) {
       g.x = fmaf(a.wd, p.x, g.x); g.y = fmaf(a.wd, p.y, g.y); g.z = fmaf(a.wd, p.z, g.z); g.w = fmaf(a.wd, p.w, g.w);
     }
   }
   m.x = fmaf(a.mu, m.x, g.x); m.y = fmaf(a.mu, m.y, g.y); m.z = fmaf(a.mu, m.z, g.z); m.w = fmaf(a.mu, m.w, g.w);
-  if constexpr (std::is_same<Args, SgdArgsGeneral>::value) {
+  if constexpr (kGeneralArgs<Args>) {
     const float mun = a.nesterov ? a.mu : 0.f;                          // the step direction d = nesterov ? g + mu*m : m
     const float4 d = a.nesterov ? make_float4(fmaf(mun, m.x, g.x), fmaf(mun, m.y, g.y), fmaf(mun, m.z, g.z), fmaf(mun, m.w, g.w)) : m;
     p.x = fmaf(-lr, d.x, p.x); p.y = fmaf(-lr, d.y, p.y); p.z = fmaf(-lr, d.z, p.z); p.w = fmaf(-lr, d.w, p.w);
@@ -106,13 +125,22 @@ __device__ __forceinline__ void sgd_apply(const Args& a, size_t v, float4 g, flo
   sgd_apply_mp(a, v, g, reinterpret_cast<const float4*>(a.momentum)[v], reinterpret_cast<const float4*>(a.params)[v], lr);
 }
 
+// Phase A of the clip instances (SgdArgsClip): vector v of the summed gradient, times 1/world as sgd_apply_mp scales it, goes to the scratch; its squares are
+// added to the thread's fp32 sum.
+__device__ __forceinline__ void clip_stash(const SgdArgsClip& a, size_t v, float4 g, float& sq) {
+  g.x *= a.scale; g.y *= a.scale; g.z *= a.scale; g.w *= a.scale;
+  __stcg(reinterpret_cast<float4*>(a.clip_ws + kClipWsHead) + v, g);
+  sq = fmaf(g.x, g.x, sq); sq = fmaf(g.y, g.y, sq); sq = fmaf(g.z, g.z, sq); sq = fmaf(g.w, g.w, sq);
+}
+
 // One float4 vector `v` of the flat bucket through the push ("LL") exchange and the optimizer:
 //   store my value, flag-in-data, into every peer's inbox (16-byte lines {v0, epoch, v1, epoch}); sum the world lines of this
 //   vector out of MY inbox in fixed rank order (own contribution from registers) => bit-identical replicas; SGD; re-zero the
 //   other-parity bucket.  world == 1: no exchange.  `st` = step index (flag = (uint32)(st + 1), or 1 where that wraps to 0;
-//   parity = st & 1), `lr` = step_lr(a, st).
+//   parity = st & 1), `lr` = step_lr(a, st).  SgdArgsClip: the vector goes to the scratch instead (clip_stash, squares into
+//   *sq) and is applied in phase B.
 template <class Args>
-__device__ __forceinline__ void exchange_apply_vec(const Args& a, size_t v, unsigned long long st, float lr) {
+__device__ __forceinline__ void exchange_apply_vec(const Args& a, size_t v, unsigned long long st, float lr, float* sq = nullptr) {
   const int rank = a.rank, world = a.world;
   const uint32_t epoch = (uint32_t)(st + 1ull);
   const uint32_t flag = epoch == 0u ? 1u : epoch;                       // 0 is "never written"; epoch 1 has the other parity
@@ -199,11 +227,78 @@ __device__ __forceinline__ void exchange_apply_vec(const Args& a, size_t v, unsi
   } else {
     g = make_float4(__uint_as_float(mine.x), __uint_as_float(mine.y), __uint_as_float(mine.z), __uint_as_float(mine.w));
   }
-  sgd_apply(a, v, g, lr);
+  if constexpr (kClipArgs<Args>) clip_stash(a, v, g, *sq);
+  else sgd_apply(a, v, g, lr);
   if (a.zero_grads) {
     const size_t z_off = a.grad_stride > 0 ? (par ^ 1) * (size_t)a.grad_stride * sizeof(float) : 0;
     st_cg_v4(reinterpret_cast<uint4*>(reinterpret_cast<char*>(a.grads.p[rank]) + z_off) + v, make_uint4(0u, 0u, 0u, 0u));
   }
+}
+
+// ----------------------------------------------------------------- gradient-norm clipping: the grid barrier and phase B
+// torch's coefficient for total norm n and max_norm c: clamp(c / (n + 1e-6), max=1), where torch computes the division as
+// reciprocal() * c.  Every step is rounded to nearest whatever the fast-math flags; a NaN passes the clamp, as in torch.
+__device__ __forceinline__ float clip_coef(float n, float c) {
+  const float k = __fmul_rn(__frcp_rn(__fadd_rn(n, 1e-6f)), c);
+  return k > 1.f ? 1.f : k;
+}
+
+// The grid-wide step between the phases: the CTA's sum of squares (warp butterflies, then the warps in order, fp32) goes to
+// its partial; once every CTA of the grid has arrived, every CTA sums the partials in CTA order in fp64, takes the root in
+// fp64 and rounds it once to fp32.  Returns the clip coefficient to every thread; CTA 0 writes the norm.  The arrival count
+// is reset by the last CTA to arrive before it releases the next generation, so the barrier holds for any grid size.
+// Called by every thread of the CTA.
+__device__ __forceinline__ float clip_grid_coef(const SgdArgsClip& a, float sq) {
+  __shared__ float s_part[kClipMaxCtas];
+  __shared__ float s_coef;
+  uint32_t* count = reinterpret_cast<uint32_t*>(a.clip_ws);
+  uint32_t* gen = count + 1;
+  float* part = a.clip_ws + 4;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, d);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = sq;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_part[w];
+    const uint32_t g0 = ld_acquire_sys(gen);
+    __stcg(part + blockIdx.x, t);
+    __threadfence();
+    if (atomicAdd(count, 1u) == gridDim.x - 1) {
+      __threadfence();
+      *reinterpret_cast<volatile uint32_t*>(count) = 0u;
+      st_release_sys(gen, g0 + 1u);
+    } else {
+      unsigned long long spins = 0;
+      while (ld_acquire_sys(gen) == g0) {
+        if (++spins > B2_SPIN_LIMIT) {
+          printf("[b200dist] gradient clipping: CTA %d of %d timed out at the grid barrier (%u arrived)\n", (int)blockIdx.x,
+                 (int)gridDim.x, *reinterpret_cast<volatile uint32_t*>(count));
+          __trap();
+        }
+      }
+    }
+    __threadfence();
+  }
+  __syncthreads();
+  if (threadIdx.x < gridDim.x) s_part[threadIdx.x] = __ldcg(part + threadIdx.x);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int i = 0; i < (int)gridDim.x; ++i) s += (double)s_part[i];
+    const float n = __double2float_rn(__dsqrt_rn(s));
+    s_coef = clip_coef(n, a.max_norm);
+    if (blockIdx.x == 0 && a.grad_norm_out != nullptr) *a.grad_norm_out = n;
+  }
+  __syncthreads();
+  return s_coef;
+}
+
+// Phase B: vector v from the scratch, times the coefficient, through the update.
+__device__ __forceinline__ void clip_apply(const SgdArgsClip& a, size_t v, float coef, float lr) {
+  float4 g = __ldcg(reinterpret_cast<const float4*>(a.clip_ws + kClipWsHead) + v);
+  g.x = __fmul_rn(g.x, coef); g.y = __fmul_rn(g.y, coef); g.z = __fmul_rn(g.z, coef); g.w = __fmul_rn(g.w, coef);
+  sgd_apply(a, v, g, lr);
 }
 
 }  // namespace b2

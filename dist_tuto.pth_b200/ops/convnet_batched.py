@@ -19,7 +19,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import Net
 from . import _ext
-from .optim import LRSchedule, check_sgd_options, schedule_tuple
+from .optim import LRSchedule, check_max_grad_norm, check_sgd_options, schedule_tuple
 from .convnet_fused import LAYOUT, NPAR, NPAR_ALLOC, pack_params, unpack_params  # noqa: F401
 
 __all__ = ["BatchedBuffers", "batched_loss_and_grads", "batched_forward", "BatchedTrainer", "STAGES"]
@@ -91,8 +91,9 @@ class BatchedTrainer:
     def __init__(self, bsz: int, lr: float = 0.01, momentum: float = 0.5, seed: int = 1234, device=None,
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, use_graph: bool = True,
                  init_from: Optional[Net] = None, lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0,
-                 nesterov: bool = False):
+                 nesterov: bool = False, max_grad_norm: Optional[float] = None):
         check_sgd_options(momentum, weight_decay, nesterov)
+        max_grad_norm = check_max_grad_norm(max_grad_norm)
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
@@ -127,6 +128,14 @@ class BatchedTrainer:
         self.bufs = BatchedBuffers(self.bsz, self.device)
         self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.done_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
+        # max_grad_norm: clip_grad_norm_ of every update in allreduce_sgd's clip instance (see FusedTrainer)
+        self.max_grad_norm = max_grad_norm
+        self._clip_kw = {}
+        if max_grad_norm is not None:
+            self._grad_norm = torch.zeros(1, dtype=torch.float32, device=self.device)
+            self._clip_kw = dict(max_grad_norm=max_grad_norm, grad_norm_out=self._grad_norm,
+                                 clip_workspace=torch.zeros(self.C.clip_workspace_numel(NPAR_ALLOC), dtype=torch.float32,
+                                                            device=self.device))
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=self.device)
         xdt = torch.uint8 if raw_uint8 else torch.float32
         self.x_dev = torch.zeros(self.bsz, 1, 28, 28, dtype=xdt, device=self.device)
@@ -151,7 +160,7 @@ class BatchedTrainer:
         # zero_grad passes) is what is kept
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
                              self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, 0, self.done_counter, None, [],
-                             lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov)
+                             lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov, **self._clip_kw)
         self.C.bt_pack_weights(self.params, self.bufs.as_list())
 
     def step_device(self, x: torch.Tensor, y: torch.Tensor) -> None:
@@ -215,6 +224,14 @@ class BatchedTrainer:
             step = int(self.step_counter.item())
         return self._lr if self.lr_schedule is None else self.lr_schedule.lr_at(self._lr, step)
 
+    def grad_norm(self) -> Optional[float]:
+        """The pre-clip total L2 norm of the averaged gradient of the last update; ``None`` without ``max_grad_norm``.
+        Synchronises like :meth:`lr_at`."""
+        if self.max_grad_norm is None:
+            return None
+        self.stream.synchronize()
+        return float(self._grad_norm.item())
+
     # ------------------------------------------------------------------ nn.Module-like surface
     def train(self, mode: bool = True):
         if mode != self.training:
@@ -251,11 +268,11 @@ class BatchedTrainer:
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
                 "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
                 "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict(),
-                "weight_decay": self.weight_decay, "nesterov": self.nesterov}
+                "weight_decay": self.weight_decay, "nesterov": self.nesterov, "max_grad_norm": self.max_grad_norm}
 
     def load_state_dict(self, sd) -> None:
-        """Parameters, momentum and step counter; the lr, its schedule, the weight decay and Nesterov stay the
-        constructor's."""
+        """Parameters, momentum and step counter; the lr, its schedule, the weight decay, Nesterov and max_grad_norm stay
+        the constructor's."""
         self.stream.synchronize()
         model = sd.get("model", sd)
         views = unpack_params(self.params)

@@ -34,7 +34,7 @@ import torch.distributed as dist
 from .. import comm
 from ..models.convnet import PARAM_SHAPES, Net
 from . import _ext
-from .optim import LRSchedule, check_sgd_options, schedule_tuple
+from .optim import LRSchedule, check_max_grad_norm, check_sgd_options, schedule_tuple
 
 __all__ = ["LAYOUT", "NPAR", "pack_params", "unpack_params", "convnet_loss_and_grads", "convnet_forward",
            "FusedTrainer"]
@@ -124,8 +124,10 @@ class FusedTrainer:
                  p_drop: float = 0.5, group=None, raw_uint8: bool = False, num_slots: int = 4,
                  use_graph: bool = True, init_from: Optional[Net] = None, cluster: Optional[int] = None,
                  deterministic: bool = False, grad_wire: Optional[torch.dtype] = None,
-                 lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0, nesterov: bool = False):
+                 lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0, nesterov: bool = False,
+                 max_grad_norm: Optional[float] = None):
         check_sgd_options(momentum, weight_decay, nesterov)
+        max_grad_norm = check_max_grad_norm(max_grad_norm)
         self.C = _ext.C()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.bsz, self._lr, self.mu, self.seed, self.p_drop = int(bsz), float(lr), float(momentum), int(seed), p_drop
@@ -194,6 +196,16 @@ class FusedTrainer:
         self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.done_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.loss_acc = torch.zeros(2, dtype=torch.float32, device=self.device)   # [sum of batch-mean nll, #correct]
+        # max_grad_norm: torch.nn.utils.clip_grad_norm_ of every update, in the optimizer kernels' clip instances (a grid
+        # barrier between the exchange and the update, csrc/sgd_device.cuh); fixed for the trainer's life like the options
+        # above.  The trainer owns their workspace and the device word of the last pre-clip norm (grad_norm()).
+        self.max_grad_norm = max_grad_norm
+        self._clip_kw = {}
+        if max_grad_norm is not None:
+            self._grad_norm = torch.zeros(1, dtype=torch.float32, device=self.device)
+            self._clip_kw = dict(max_grad_norm=max_grad_norm, grad_norm_out=self._grad_norm,
+                                 clip_workspace=torch.zeros(self.C.clip_workspace_numel(NPAR_ALLOC), dtype=torch.float32,
+                                                            device=self.device))
         xdt = torch.uint8 if raw_uint8 else torch.float32
         self.x_dev = torch.zeros(self.bsz, 1, 28, 28, dtype=xdt, device=self.device)
         self.y_dev = torch.zeros(self.bsz, dtype=torch.int64, device=self.device)
@@ -300,7 +312,7 @@ class FusedTrainer:
             # grads: re-zeroes the other-parity bucket, which a bucket step (the executor's) may use next
             self.C.reduce_sgd(self.grad_slots, n, self.factors, B, self.params, self.momentum, self.step_counter,
                               self.done_counter, self.lr, self.mu, self.aux, self.loss_acc, self.grads, self.grad_stride,
-                              lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov)
+                              lr_schedule=self._sched, weight_decay=self.weight_decay, nesterov=self.nesterov, **self._clip_kw)
             return
         if self.deterministic and B * cl <= self.sms:
             self.C.convnet_step(self.params, self.grads, x, y, self.loss_acc, None, None, self.step_counter, self.seed,
@@ -313,7 +325,7 @@ class FusedTrainer:
         self.C.allreduce_sgd(self._grad_ptrs, self._sig_ptrs, self.params, self.momentum, self.step_counter,
                              self.lr, self.mu, 1.0 / self.world, self.rank, self.world, True, self.grad_stride,
                              self.done_counter, self.aux, self._inbox_ptrs, self.wire_bf16, lr_schedule=self._sched,
-                             weight_decay=self.weight_decay, nesterov=self.nesterov)
+                             weight_decay=self.weight_decay, nesterov=self.nesterov, **self._clip_kw)
 
     def _warm(self):
         # forward-only launch: sets the kernel's dynamic-smem attribute outside of graph capture
@@ -432,7 +444,7 @@ class FusedTrainer:
                                       self.grad_stride, self.lr, self.mu, self.p_drop, max(1, loader.num_buffers - 2),
                                       self.cluster, self.aux, self._inbox_ptrs, loss_hist, self.wire_bf16,
                                       *self._native_slots(), lr_schedule=self._sched, weight_decay=self.weight_decay,
-                                      nesterov=self.nesterov),
+                                      nesterov=self.nesterov, **self._clip_kw),
                   self.training)
             self._executors[id(loader)] = ex
         if new_epoch:
@@ -495,6 +507,15 @@ class FusedTrainer:
             step = int(self.step_counter.item())
         return self._lr if self.lr_schedule is None else self.lr_schedule.lr_at(self._lr, step)
 
+    def grad_norm(self) -> Optional[float]:
+        """The pre-clip total L2 norm of the averaged gradient of the last update (what ``clip_grad_norm_`` returns);
+        ``None`` without ``max_grad_norm``.  Synchronises like :meth:`lr_at`."""
+        if self.max_grad_norm is None:
+            return None
+        self.sync_lag(0)
+        self.stream.synchronize()
+        return float(self._grad_norm.item())
+
     # ------------------------------------------------------------------ nn.Module-like surface
     def train(self, mode: bool = True):
         """``model.train()`` / ``model.eval()``: dropout on/off (captured graphs are dropped, the flag is baked in)."""
@@ -540,12 +561,13 @@ class FusedTrainer:
                 "momentum": {k: v.detach().cpu().clone() for k, v in m.items()},
                 "steps": int(self.step_counter.item()), "lr": self.lr, "mu": self.mu,
                 "lr_schedule": None if self.lr_schedule is None else self.lr_schedule.to_dict(),
-                "weight_decay": self.weight_decay, "nesterov": self.nesterov}
+                "weight_decay": self.weight_decay, "nesterov": self.nesterov, "max_grad_norm": self.max_grad_norm}
 
     def load_state_dict(self, sd):
         """Accepts a trainer checkpoint or a plain ``Net`` state_dict.  Collective when ``steps`` is present (the bucket
         parity and the exchange epochs derive from the step counter, see :meth:`_reset_exchange`).  The lr, the lr
-        schedule, the weight decay and Nesterov stay the constructor's: ``steps`` is where a schedule continues from."""
+        schedule, the weight decay, Nesterov and max_grad_norm stay the constructor's: ``steps`` is where a schedule
+        continues from."""
         self.sync_lag(0)
         model = sd.get("model", sd)
         views = unpack_params(self.params)

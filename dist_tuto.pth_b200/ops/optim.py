@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "LRSchedule", "check_sgd_options"]
+__all__ = ["FlatSGD", "LRSchedule", "check_sgd_options", "check_max_grad_norm"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -158,21 +158,44 @@ def check_sgd_options(momentum: float, weight_decay: float, nesterov: bool) -> N
         raise ValueError("nesterov momentum needs a nonzero momentum")
 
 
+def check_max_grad_norm(max_grad_norm) -> Optional[float]:
+    """``torch.nn.utils.clip_grad_norm_``'s ``max_norm`` for every engine (the L2 norm only): ``None`` (no clipping) or a
+    finite value > 0 that stays > 0 in fp32.  Returns it as a float (or ``None``)."""
+    if max_grad_norm is None:
+        return None
+    if isinstance(max_grad_norm, bool) or not isinstance(max_grad_norm, (int, float)):
+        raise ValueError(f"max_grad_norm must be None or a finite number > 0, got {max_grad_norm!r}")
+    c = float(max_grad_norm)
+    c32 = float(torch.tensor(c, dtype=torch.float32))
+    if not (math.isfinite(c) and c > 0.0 and math.isfinite(c32) and c32 > 0.0):
+        raise ValueError(f"max_grad_norm must be None or a finite number > 0, got {max_grad_norm!r}")
+    return c
+
+
 class FlatSGD:
     """``FlatSGD(model)`` where ``model`` is a plain module, a module carrying ``_grad_bucket`` or a
     :class:`DistributedDataParallel` wrapper.
 
     ``step()`` expects averaged gradients (call ``average_gradients(model)`` first, as the tutorial loop does) and,
     with ``zero_grad=True`` (default), leaves the buckets zeroed so no separate ``zero_grad()`` pass is needed;
-    ``zero_grad()`` exists for loop compatibility and is then a no-op apart from re-arming the DDP hooks."""
+    ``zero_grad()`` exists for loop compatibility and is then a no-op apart from re-arming the DDP hooks.
+
+    ``max_grad_norm=c`` clips the averaged gradient first, as ``torch.nn.utils.clip_grad_norm_(params, c)`` would: on CUDA
+    fp32 buckets ``grad_sqnorm`` sums each bucket's squares on the device and ``sgd_flat`` takes the norm and the
+    coefficient there (no host synchronisation); elsewhere ``clip_grad_norm_(..., foreach=False)`` itself runs.
+    :meth:`grad_norm` returns the last update's pre-clip norm."""
 
     def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
-                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False):
+                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
+                 max_grad_norm: Optional[float] = None):
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
         check_sgd_options(momentum, weight_decay, nesterov)
         self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
         self.nesterov = bool(nesterov)
+        self.max_grad_norm = check_max_grad_norm(max_grad_norm)
+        self._grad_norm = None           # the last update's pre-clip norm (a 0-dim / [1] tensor), see grad_norm()
+        self._clip_bufs = None           # kernel path: (fp64 [buckets] squares, grad_sqnorm workspace, fp32 [1] norm)
         # lr_schedule: update k (k = `steps`, the updates applied so far) uses lr_schedule.lr_at(lr, k), computed on the host
         schedule_tuple(lr_schedule)
         self.lr_schedule, self.steps = lr_schedule, 0
@@ -215,10 +238,23 @@ class FlatSGD:
         """``optimizer.step()`` (train_dist.py:124) for every bucket, and -- with ``zero_grad=True`` -- the
         ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass."""
         lr = self.lr_at()
-        for gb, pf, mf in zip(self.buckets, self.param_flats, self.momentum_flats):
+        kernel = [pf.is_cuda and gb.flat.dtype == torch.float32 for gb, pf in zip(self.buckets, self.param_flats)]
+        clip = {}
+        if self.max_grad_norm is not None:
+            if all(kernel):
+                clip = self._clip_on_device()
+            else:                        # every bucket by torch itself, before any update
+                params = []
+                for gb in self.buckets:
+                    gb.attach()          # p.grad is the bucket's view, so the clip scales the bucket in place
+                    params += gb.params
+                self._grad_norm = torch.nn.utils.clip_grad_norm_(params, self.max_grad_norm, foreach=False)
+                kernel = [False] * len(kernel)
+        for gb, pf, mf, kern in zip(self.buckets, self.param_flats, self.momentum_flats, kernel):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
-            if pf.is_cuda and g.dtype == torch.float32:
-                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov)
+            if kern:
+                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov,
+                                        **clip)
                 continue
             # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
             # torch.optim.SGD's order (foreach=False)
@@ -232,6 +268,26 @@ class FlatSGD:
         self.steps += 1
         if self.fused_zero and self._engine is not None:
             self._engine._reset()
+
+    def _clip_on_device(self) -> dict:
+        """Every bucket's sum of squares into the fp64 device array (grad_sqnorm, one launch per bucket); the sgd_flat
+        arguments that take the norm and the coefficient from it."""
+        C = self._kernel()
+        if self._clip_bufs is None:
+            dev = self.param_flats[0].device
+            self._clip_bufs = (torch.zeros(len(self.buckets), dtype=torch.float64, device=dev),
+                               torch.zeros(C.grad_sqnorm_workspace_numel(), dtype=torch.float32, device=dev),
+                               torch.zeros(1, dtype=torch.float32, device=dev))
+        sq, ws, norm = self._clip_bufs
+        for k, gb in enumerate(self.buckets):
+            C.grad_sqnorm(gb.flat[:gb.numel], sq, k, ws)
+        self._grad_norm = norm
+        return dict(max_grad_norm=self.max_grad_norm, sqnorms=sq, grad_norm_out=norm)
+
+    def grad_norm(self) -> Optional[float]:
+        """The pre-clip total L2 norm of the gradient of the last update (what ``clip_grad_norm_`` returns); ``None``
+        without clipping or before the first update.  Synchronises with the device."""
+        return None if self._grad_norm is None else float(self._grad_norm.reshape(-1)[0].item())
 
     def lr_at(self, step: Optional[int] = None) -> float:
         """The lr of the update applied after ``step`` updates (default: the next one, ``steps``)."""
@@ -251,7 +307,7 @@ class FlatSGD:
     def state_dict(self) -> dict:
         """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``."""
         return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
-                "steps": self.steps,
+                "max_grad_norm": self.max_grad_norm, "steps": self.steps,
                 "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
 
     def named_momentum(self, model: nn.Module) -> dict:
@@ -282,6 +338,7 @@ class FlatSGD:
         """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
         self.lr, self.momentum, self.weight_decay = float(sd["lr"]), float(sd["momentum"]), float(sd["weight_decay"])
         self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
+        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))   # ... and before clipping: none
         self.steps = int(sd.get("steps", self.steps))
         for m, src in zip(self.momentum_flats, sd["momentum_buffers"]):
             m.copy_(src)

@@ -33,7 +33,7 @@ from . import comm
 from .data import default_eval_dataset, partition_dataset
 from .models.convnet import Net
 from .ops.convnet_eval import evaluate
-from .ops.optim import FlatSGD, LRSchedule, check_sgd_options
+from .ops.optim import FlatSGD, LRSchedule, check_max_grad_norm, check_sgd_options
 from .utils import say
 from .utils.checkpoint import load_checkpoint, restore_optimizer, save_checkpoint
 from .utils.trace import NullTracer, Tracer
@@ -53,7 +53,7 @@ class TrainConfig:
                  p_drop: float = 0.5, checkpoint: Optional[str] = None, resume: Optional[str] = None,
                  checkpoint_every: Optional[int] = None, trace: Optional[str] = None, eval_dataset=None,
                  eval_every: int = 1, lr_schedule: Optional[LRSchedule] = None, weight_decay: float = 0.0,
-                 nesterov: bool = False):
+                 nesterov: bool = False, max_grad_norm: Optional[float] = None):
         self.epochs, self.lr, self.momentum, self.seed = epochs, lr, momentum, seed
         self.global_batch, self.engine, self.device = global_batch, engine, device
         self.max_steps, self.dataset, self.log, self.p_drop = max_steps, dataset, log, p_drop
@@ -79,6 +79,8 @@ class TrainConfig:
         # weight_decay / nesterov: torch.optim.SGD's options (dampening 0), the same update on every engine
         check_sgd_options(momentum, weight_decay, nesterov)
         self.weight_decay, self.nesterov = float(weight_decay), bool(nesterov)
+        # max_grad_norm: torch.nn.utils.clip_grad_norm_ (L2) of every update on every engine; None: no clipping
+        self.max_grad_norm = check_max_grad_norm(max_grad_norm)
 
 
 def _spans_machines() -> bool:
@@ -130,7 +132,7 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         from .ops.convnet_fused import FusedTrainer
         trainer = FusedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
                                p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule,
-                               weight_decay=cfg.weight_decay, nesterov=cfg.nesterov)
+                               weight_decay=cfg.weight_decay, nesterov=cfg.nesterov, max_grad_norm=cfg.max_grad_norm)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -139,7 +141,7 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         from .ops.convnet_batched import BatchedTrainer
         trainer = BatchedTrainer(bsz, lr=cfg.lr, momentum=cfg.momentum, seed=cfg.seed, device=device,
                                  p_drop=cfg.p_drop, raw_uint8=fused_raw, lr_schedule=schedule,
-                                 weight_decay=cfg.weight_decay, nesterov=cfg.nesterov)
+                                 weight_decay=cfg.weight_decay, nesterov=cfg.nesterov, max_grad_norm=cfg.max_grad_norm)
         if cfg.resume:
             resume_blob = load_checkpoint(cfg.resume, trainer)
             start_steps = int(resume_blob.get("steps", 0))
@@ -166,10 +168,11 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         model._grad_bucket = GradBucket(list(model.parameters()))
         # optim.SGD(lr=0.01, momentum=0.5) of train_dist.py:110, over flat buffers: update + zero_grad in one pass
         optimizer = FlatSGD(model, lr=cfg.lr, momentum=cfg.momentum, lr_schedule=schedule, weight_decay=cfg.weight_decay,
-                            nesterov=cfg.nesterov)
+                            nesterov=cfg.nesterov, max_grad_norm=cfg.max_grad_norm)
         if cfg.resume:
             restore_optimizer(optimizer, model, resume_blob)         # momentum: FlatSGD layout or per-name (fused engine's)
             optimizer.steps = start_steps                            # the schedule continues where the checkpoint stopped
+            optimizer.max_grad_norm = cfg.max_grad_norm              # the run's clipping, as on the other engines
         acc = torch.zeros((), device=device)
 
         # The native loader recycles its pinned staging buffers; the async H2D copies below must have left a buffer
@@ -209,7 +212,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
     eval_set = None
     if cfg.eval_dataset is not None:
         eval_set = default_eval_dataset() if isinstance(cfg.eval_dataset, str) else cfg.eval_dataset
-    evals, eval_seconds, epoch_lrs = [], 0.0, []
+    evals, eval_seconds, epoch_lrs, epoch_norms = [], 0.0, [], []
+    norm_of = (optimizer if engine == "torch" else trainer).grad_norm if cfg.max_grad_norm is not None else None
     history, steps, t0 = [], 0, time.perf_counter()
     start_epoch = 0
     if resume_blob.get("in_progress"):            # a periodic checkpoint of an unfinished run: do the REMAINING epochs
@@ -252,6 +256,8 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         history.append(mean_loss)
         last = start_steps + steps - 1                             # step counter of the epoch's last update
         epoch_lrs.append(cfg.lr if schedule is None else schedule.lr_at(cfg.lr, max(last, 0)))
+        if norm_of is not None:
+            epoch_norms.append(norm_of())                          # pre-clip norm of the epoch's last update
         cfg.log("Rank ", comm.get_rank(), ", epoch ", epoch, ": ", mean_loss)
         if eval_set is not None and (done or (epoch + 1) % cfg.eval_every == 0 or epoch + 1 == cfg.epochs):
             te = time.perf_counter()
@@ -274,9 +280,12 @@ def train(rank: int, size: int, cfg: Optional[TrainConfig] = None):
         save_checkpoint(cfg.checkpoint, model, optimizer=optimizer, steps=start_steps + steps, history=history,
                         epoch=max(0, len(history) - (1 if done else 0)), in_progress=False)
     trace_file = tracer.save(cfg.trace) if cfg.trace else None          # collective: rank 0 writes every rank's rows
-    return {"loss": history, "steps": steps, "seconds": elapsed, "bsz": bsz,
-            "samples_per_s": steps * bsz * size / max(elapsed, 1e-9), "model": model, "trace": trace_file,
-            "eval": evals, "eval_seconds": eval_seconds, "lr": epoch_lrs}
+    out = {"loss": history, "steps": steps, "seconds": elapsed, "bsz": bsz,
+           "samples_per_s": steps * bsz * size / max(elapsed, 1e-9), "model": model, "trace": trace_file,
+           "eval": evals, "eval_seconds": eval_seconds, "lr": epoch_lrs}
+    if norm_of is not None:
+        out["grad_norm"] = epoch_norms
+    return out
 
 
 def run(rank: int, size: int):

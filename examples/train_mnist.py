@@ -6,6 +6,7 @@
     python examples/train_mnist.py --backend b200 --size 8 --global-batch 32768   # large batch: wgmma batched engine
     python examples/train_mnist.py --backend b200 --size 8 --eval   # + test loss / accuracy after every epoch
     python examples/train_mnist.py --backend b200 --size 8 --weight-decay 5e-4 --nesterov   # torch.optim.SGD's options
+    python examples/train_mnist.py --backend b200 --size 1 --global-batch 4096 --lr 0.32 --max-grad-norm 1.0   # clip_grad_norm_
     python examples/train_mnist.py --backend b200 --size 1 --global-batch 4096 --lr 0.32 --warmup-epochs 1 \
         --lr-decay cosine --eval                       # large batch: linearly scaled lr, 1 epoch of warmup, cosine decay
     python -m dist_tuto.pth_b200.spawn --size 8 --max-restarts 2 examples/train_mnist.py --external --backend b200 \
@@ -45,7 +46,8 @@ def run(rank, size):
                            checkpoint_every=CFG["ckpt_every"], resume=resume, global_batch=CFG["global_batch"],
                            engine=CFG["engine"], trace=CFG["trace"],
                            eval_dataset="default" if CFG["eval"] else None, eval_every=CFG["eval_every"],
-                           lr_schedule=schedule_from(CFG), weight_decay=CFG["weight_decay"], nesterov=CFG["nesterov"])
+                           lr_schedule=schedule_from(CFG), weight_decay=CFG["weight_decay"], nesterov=CFG["nesterov"],
+                           max_grad_norm=CFG.get("max_grad_norm"))
     out = dist.train(rank, size, cfg)
     if rank == 0:
         print(f"{out['steps']} steps, {out['samples_per_s']:.0f} samples/s (wall clock, whole job)")
@@ -78,6 +80,8 @@ if __name__ == "__main__":
     ap.add_argument("--lr-min-factor", type=float, default=0.0, help="cosine: final lr factor (default 0)")
     ap.add_argument("--weight-decay", type=float, default=0.0, help="L2 weight decay on every parameter (default 0)")
     ap.add_argument("--nesterov", action="store_true", help="Nesterov momentum")
+    ap.add_argument("--max-grad-norm", type=float, default=None,
+                    help="clip the averaged gradient to this L2 norm before every update (default: no clipping)")
     a = ap.parse_args()
     os.environ["B2_TRAIN_CFG"] = json.dumps(dict(epochs=a.epochs, lr=a.lr, max_steps=a.max_steps, ckpt=a.checkpoint, ckpt_every=a.checkpoint_every, resume=a.resume, trace=a.trace,
                                                  global_batch=a.global_batch, engine=a.engine, eval=a.eval,
@@ -85,7 +89,7 @@ if __name__ == "__main__":
                                                  warmup_start=a.warmup_start, lr_decay=a.lr_decay,
                                                  lr_milestones=a.lr_milestones, lr_gamma=a.lr_gamma,
                                                  lr_min_factor=a.lr_min_factor, weight_decay=a.weight_decay,
-                                                 nesterov=a.nesterov))
+                                                 nesterov=a.nesterov, max_grad_norm=a.max_grad_norm))
     if a.external:
         dist.init_from_env(run, backend=a.backend)
     else:
