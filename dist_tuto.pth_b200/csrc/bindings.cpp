@@ -71,6 +71,9 @@ int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const lo
                                cudaStream_t stream);
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
                        float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream);
+int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* momentum,
+                          size_t n_vec, float lr, float mu, float wd, int nesterov, float scale, int zero_grad, int rank,
+                          int world, int max_blocks, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
@@ -709,6 +712,35 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
      py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
      py::arg("grad_norm_out") = py::none());
+  // Sharded optimizer step of one bucket (csrc/sharded_sgd.cu): reduce-scatter of the gradient buckets `grads`, momentum SGD on
+  // this rank's slice with its momentum shard, and the new parameters stored into every rank's flat in `params`.  n_vec counts
+  // the 16-byte vectors of one gradient bucket; raw per-rank pointers, like `allreduce`.
+  m.def("sharded_sgd", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                          std::vector<unsigned long long> sigs, torch::Tensor momentum, size_t n_vec, double lr, double mu,
+                          double wd, bool nesterov, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    check_world(rank, world, "sharded_sgd");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_sgd: one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ",
+                params.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd: every rank owns n_vec / world vectors, so n_vec must be a multiple of "
+                "world (pad the buffers), got n_vec ", n_vec, " for world ", world);
+    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd: nesterov needs a nonzero momentum");
+    check_cuda_contig(momentum, "momentum");
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
+                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd: momentum: 16-byte aligned fp32 of at least ", shard,
+                " elements (this rank's slice)");
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd: null or misaligned per-rank pointer");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(momentum.device());
+    ck_cuda(b2_sharded_sgd_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), n_vec, (float)lr, (float)mu, (float)wd,
+                                  nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+            "sharded_sgd launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("n_vec"), py::arg("lr"),
+     py::arg("mu"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0);
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });

@@ -1,0 +1,169 @@
+// Sharded optimizer step for generic models on sm_90a: reduce-scatter of one gradient bucket, momentum SGD on the slice this
+// rank owns and all-gather of the updated PARAMETERS, in one launch per bucket.
+//
+// The two-shot all-reduce (allreduce.cu) has rank r reduce slice r and push the averaged gradient slice to every rank, where a
+// second kernel (sgd_flat_kernel, sgd.cu) then applies the same update W times over.  Here the owner of slice r applies the
+// update itself and pushes the new parameters instead: the NVLink bytes are the same, the second kernel is gone, and the
+// momentum exists for the owned slice only (optimizer state is 1/W per GPU).
+//
+// Same grid and slice mapping as allreduce_twoshot_kernel: slice = n_vec / world, rank r owns vectors [r*slice, (r+1)*slice)
+// of the gradient bucket, and vector j of a slice belongs to the same (block, thread) on every rank and in every phase, so
+// the per-block barriers order everything a block touches.
+//
+//   barrier                      every rank's gradients of this bucket are complete
+//   owned slice, per vector      g = (((0 + g_0) + g_1) + ...) * scale in fp32, in rank order (bit for bit what the one-shot and
+//                                two-shot all-reduce store for an fp32 bucket); sgd_flat_kernel's fmaf sequence on the own
+//                                parameter and momentum vectors; momentum stored locally; the new parameter vector stored
+//                                into EVERY rank's parameter flat
+//   barrier                      every parameter slice has landed everywhere, and every peer has finished reading this rank's
+//                                gradients
+//   zero the local bucket        only now: before that barrier the peers are still loading this bucket's slices
+//
+// A bf16 bucket (8 gradients per vector) updates two fp32 parameter vectors per gradient vector.  The fp32 sum x scale feeds
+// the update unrounded: the averaged gradient never takes a bf16 round trip.
+#include <cstring>
+#include "common.cuh"
+
+namespace b2 {
+
+constexpr int kShardThreads = 512;   // as the all-reduce kernels (kThreads)
+constexpr int kShardUnroll = 2;      // gradient vectors per thread and pass: 2 x world 16-byte peer loads in flight
+
+struct ShardedSgdArgs {
+  PeerPtrs grads;         // symmetric gradient bucket of every rank
+  PeerPtrs params;        // symmetric fp32 parameter flat of every rank
+  SignalPads sig;         // signal pad of the gradient bucket
+  float* momentum;        // this rank's shard: the fp32 momentum of its slice only
+  size_t n_vec;           // 16-byte vectors of the gradient bucket, a multiple of world
+  float lr, mu, wd, scale;
+  int rank, world, zero_grad;
+};
+
+// momentum SGD on four elements, the fmaf sequence of sgd_flat_kernel
+template <bool kNesterov>
+__device__ __forceinline__ void sgd4(float4& p, float4& m, float4 g, float lr, float mu, float wd) {
+  g.x = fmaf(wd, p.x, g.x); g.y = fmaf(wd, p.y, g.y); g.z = fmaf(wd, p.z, g.z); g.w = fmaf(wd, p.w, g.w);
+  m.x = fmaf(mu, m.x, g.x); m.y = fmaf(mu, m.y, g.y); m.z = fmaf(mu, m.z, g.z); m.w = fmaf(mu, m.w, g.w);
+  float4 d = m;
+  if (kNesterov) {
+    d.x = fmaf(mu, m.x, g.x); d.y = fmaf(mu, m.y, g.y); d.z = fmaf(mu, m.z, g.z); d.w = fmaf(mu, m.w, g.w);
+  }
+  p.x = fmaf(-lr, d.x, p.x); p.y = fmaf(-lr, d.y, p.y); p.z = fmaf(-lr, d.z, p.z); p.w = fmaf(-lr, d.w, p.w);
+}
+
+__device__ __forceinline__ float4 as_f4(uint4 v) {
+  return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
+}
+__device__ __forceinline__ uint4 as_u4(float4 v) {
+  return make_uint4(__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w));
+}
+
+// kBf16: the gradient bucket is bf16 (8 elements per vector), else fp32 (4).  Parameters and momentum are fp32 in both.
+template <bool kBf16, bool kNesterov>
+__global__ void __launch_bounds__(kShardThreads) sharded_sgd_kernel(ShardedSgdArgs a) {
+  constexpr int kP = kBf16 ? 2 : 1;                     // fp32 parameter vectors per gradient vector
+  const int rank = a.rank, world = a.world;
+  uint32_t epoch = barrier_epoch_load(a.sig, rank);
+  const size_t slice = a.n_vec / world;
+  const size_t stride = (size_t)gridDim.x * kShardThreads;
+  const size_t first = (size_t)blockIdx.x * kShardThreads + threadIdx.x;
+  const size_t off = (size_t)rank * slice;
+  const uint4* own = reinterpret_cast<const uint4*>(a.params.p[rank]) + kP * off;
+  block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's gradients are complete
+  for (size_t base = first; base < slice; base += stride * kShardUnroll) {
+    uint4 raw[kShardUnroll][B2_MAX_RANKS];
+#pragma unroll
+    for (int u = 0; u < kShardUnroll; ++u) {
+      const size_t j = base + (size_t)u * stride;
+#pragma unroll
+      for (int r = 0; r < B2_MAX_RANKS; ++r)
+        if (r < world && j < slice) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.grads.p[r]) + off + j);
+    }
+#pragma unroll
+    for (int u = 0; u < kShardUnroll; ++u) {
+      const size_t j = base + (size_t)u * stride;
+      if (j >= slice) continue;
+      float4 p[kP], m[kP], g[kP];
+      float4* mom = reinterpret_cast<float4*>(a.momentum) + kP * j;
+#pragma unroll
+      for (int h = 0; h < kP; ++h) {
+        p[h] = as_f4(ld_cg_v4(own + kP * j + h));
+        m[h] = mom[h];
+        g[h] = make_float4(0.f, 0.f, 0.f, 0.f);                  // the all-reduce's accumulator starts at +0 too
+      }
+#pragma unroll
+      for (int r = 0; r < B2_MAX_RANKS; ++r) {
+        if (r < world) {
+          const uint4 v = raw[u][r];
+          if constexpr (kBf16) {
+            g[0].x += bf16lo(v.x); g[0].y += bf16hi(v.x); g[0].z += bf16lo(v.y); g[0].w += bf16hi(v.y);
+            g[1].x += bf16lo(v.z); g[1].y += bf16hi(v.z); g[1].z += bf16lo(v.w); g[1].w += bf16hi(v.w);
+          } else {
+            g[0].x += __uint_as_float(v.x); g[0].y += __uint_as_float(v.y);
+            g[0].z += __uint_as_float(v.z); g[0].w += __uint_as_float(v.w);
+          }
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < kP; ++h) {
+        g[h].x *= a.scale; g[h].y *= a.scale; g[h].z *= a.scale; g[h].w *= a.scale;
+        sgd4<kNesterov>(p[h], m[h], g[h], a.lr, a.mu, a.wd);
+        mom[h] = m[h];
+      }
+#pragma unroll
+      for (int r = 0; r < B2_MAX_RANKS; ++r) {
+        if (r < world) {
+#pragma unroll
+          for (int h = 0; h < kP; ++h) st_cg_v4(reinterpret_cast<uint4*>(a.params.p[r]) + kP * (off + j) + h, as_u4(p[h]));
+        }
+      }
+    }
+  }
+  // every parameter slice has landed everywhere; no peer reads this rank's gradients any more
+  block_barrier_all_ranks(a.sig, rank, world, ++epoch);
+  if (a.zero_grad) {
+    uint4* mine = reinterpret_cast<uint4*>(a.grads.p[rank]);
+    for (int s = 0; s < world; ++s)                               // vector j of every slice: the peers' block of the same index read it
+      for (size_t j = first; j < slice; j += stride) mine[(size_t)s * slice + j] = make_uint4(0u, 0u, 0u, 0u);
+  }
+  if (threadIdx.x == 0) barrier_epoch_store(a.sig, rank, epoch);
+}
+
+}  // namespace b2
+
+extern "C" {
+
+// One sharded optimizer step of one bucket on `stream`.  n_vec: 16-byte vectors of the gradient bucket (4 fp32 or, with bf16,
+// 8 bf16 gradients each); the parameter flats hold n_vec x 4 (x 8) floats and `momentum` n_vec / world x 4 (x 8).  The grid is
+// the two-shot all-reduce's: ceil(ceil(slice / 512) / 2) CTAs, at most max_blocks.  Returns cudaError_t as int;
+// cudaErrorInvalidValue, without a launch, for a world outside 1..8, a rank outside [0, world), an n_vec that is not a
+// multiple of world (the remainder would be left out) or a null pointer.
+int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* momentum,
+                          size_t n_vec, float lr, float mu, float wd, int nesterov, float scale, int zero_grad, int rank,
+                          int world, int max_blocks, cudaStream_t stream) {
+  if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return (int)cudaErrorInvalidValue;
+  if (grads == nullptr || params == nullptr || sig == nullptr || momentum == nullptr) return (int)cudaErrorInvalidValue;
+  if (n_vec % (size_t)world != 0) return (int)cudaErrorInvalidValue;
+  for (int r = 0; r < world; ++r)
+    if (grads->p[r] == nullptr || params->p[r] == nullptr || sig->pad[r] == nullptr) return (int)cudaErrorInvalidValue;
+  b2::ShardedSgdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.momentum = momentum; a.n_vec = n_vec;
+  a.lr = lr; a.mu = mu; a.wd = wd; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad;
+  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
+  size_t blocks = (n_vec / world + b2::kShardThreads - 1) / b2::kShardThreads;
+  blocks = (blocks + 1) / 2;
+  if (blocks < 1) blocks = 1;
+  if (blocks > (size_t)max_blocks) blocks = (size_t)max_blocks;
+  const dim3 grid((unsigned)blocks);
+  if (bf16) {
+    if (nesterov) b2::sharded_sgd_kernel<true, true><<<grid, b2::kShardThreads, 0, stream>>>(a);
+    else b2::sharded_sgd_kernel<true, false><<<grid, b2::kShardThreads, 0, stream>>>(a);
+  } else {
+    if (nesterov) b2::sharded_sgd_kernel<false, true><<<grid, b2::kShardThreads, 0, stream>>>(a);
+    else b2::sharded_sgd_kernel<false, false><<<grid, b2::kShardThreads, 0, stream>>>(a);
+  }
+  return (int)cudaGetLastError();
+}
+
+}  // extern "C"

@@ -10,6 +10,11 @@ GPU-first: the gradients of a model already live in flat (symmetric-memory) buck
 buffers with the *same* offsets and strides (``p.data`` becomes a view), so a whole bucket is updated -- and its
 gradients re-zeroed for the next backward -- by ONE ``sgd_flat_kernel`` launch (csrc/sgd.cu) that streams the three
 arrays once.  (The ConvNet goes further and fuses the all-reduce into the same kernel: ``allreduce_sgd_kernel``.)
+
+``FlatSGD(..., sharded=True)`` does the same for generic models: per bucket ONE ``sharded_sgd_kernel`` launch
+(csrc/sharded_sgd.cu) reduce-scatters the gradients, updates the slice of the parameters this rank owns and stores the new
+parameters into every rank's flat, so the momentum exists for the owned slice only (optimizer state is 1/W per GPU) and no
+separate update kernel runs.
 """
 from __future__ import annotations
 
@@ -172,6 +177,16 @@ def check_max_grad_norm(max_grad_norm) -> Optional[float]:
     return c
 
 
+def _peer_world(gb) -> bool:
+    """Does this gradient bucket live in the symmetric memory of ONE peer-memory world (not the two-level world of several
+    machines), in a dtype ``sharded_sgd_kernel`` reduces?"""
+    if gb.symm_handle is None or not gb.flat.is_cuda or gb.flat.dtype not in (torch.float32, torch.bfloat16):
+        return False
+    from ..parallel import symm
+
+    return isinstance(gb.world, symm.SymmWorld)
+
+
 class FlatSGD:
     """``FlatSGD(model)`` where ``model`` is a plain module, a module carrying ``_grad_bucket`` or a
     :class:`DistributedDataParallel` wrapper.
@@ -183,14 +198,35 @@ class FlatSGD:
     ``max_grad_norm=c`` clips the averaged gradient first, as ``torch.nn.utils.clip_grad_norm_(params, c)`` would: on CUDA
     fp32 buckets ``grad_sqnorm`` sums each bucket's squares on the device and ``sgd_flat`` takes the norm and the
     coefficient there (no host synchronisation); elsewhere ``clip_grad_norm_(..., foreach=False)`` itself runs.
-    :meth:`grad_norm` returns the last update's pre-clip norm."""
+    :meth:`grad_norm` returns the last update's pre-clip norm.
+
+    ``sharded=True`` shards the optimizer over the ranks (ZeRO stage 1): every bucket is cut into W equal slices, rank r keeps
+    the momentum of slice r only (``momentum_flats[k]`` is that shard, :meth:`shard_range` its element range) and updates
+    only that slice of the parameters, which then reach every rank.  The update runs where the gradient exchange runs, not in
+    ``step()``: the DDP hooks (or ``average_gradients(model)``) launch, per bucket, either ONE ``sharded_sgd`` kernel on a
+    symmetric CUDA world (reduce-scatter in fp32 in rank order, update, parameter all-gather through peer stores; a bf16
+    bucket's fp32 sum feeds the update unrounded) or, elsewhere (gloo, several machines, no symmetric world), the bucket's
+    all-reduce, the update of the owned slice and an ``all_gather_into_tensor`` of the parameters.  So **after
+    ``average_gradients(model)`` the parameters are already updated** and ``p.grad`` is zero (with ``zero_grad=False`` it
+    holds this rank's local, unaveraged gradient on the kernel path and the averaged one elsewhere); ``step()`` launches
+    nothing: it advances ``steps``, re-arms the hooks, and raises if the step's buckets were not exchanged.  One
+    ``average_gradients`` goes with one ``step``.  With fp32 buckets the parameters are bit for bit those of
+    ``sharded=False`` (given the all-reduce's fixed rank order).  ``max_grad_norm`` cannot be combined with it (the total
+    norm needs every bucket reduced before any update) and raises ``ValueError``.  :meth:`named_momentum` is then collective
+    (every rank calls it; it gathers the shards) and returns the same per-name tensors as an unsharded optimizer, so
+    checkpoints stay engine-independent.  At world size 1 the flag changes nothing."""
 
     def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
                  zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
-                 max_grad_norm: Optional[float] = None):
+                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+        from .. import comm
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
         check_sgd_options(momentum, weight_decay, nesterov)
+        self.sharded = bool(sharded)
+        if self.sharded and max_grad_norm is not None:
+            raise ValueError("FlatSGD(sharded=True) cannot clip: the total norm needs every bucket reduced before any update, "
+                             "and the sharded update runs bucket by bucket during backward; use sharded=False with max_grad_norm")
         self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
         self.nesterov = bool(nesterov)
         self.max_grad_norm = check_max_grad_norm(max_grad_norm)
@@ -211,18 +247,45 @@ class FlatSGD:
             self.buckets = [gb]
         self.param_flats: List[torch.Tensor] = []
         self.momentum_flats: List[torch.Tensor] = []
+        # sharded over more than one rank: "kernel" (sharded_sgd on a symmetric CUDA world) or "torch"; None: every rank
+        # holds and updates everything
+        self._group = self._engine.group if self._engine is not None else self.buckets[0].group
+        self._world, self._rank = comm.get_world_size(self._group), comm.get_rank(self._group)
+        self._shard_mode = None
+        if self.sharded and self._world > 1:
+            self._shard_mode = "kernel" if all(_peer_world(gb) for gb in self.buckets) else "torch"
+        self._shards: List[tuple] = []   # per bucket: (gradient vectors, padded elements, elements per rank, whole parameter flat, its handle)
+        self._done = [False] * len(self.buckets)
         for gb in self.buckets:
             p0 = gb.params[0]
             if any(p.dtype != torch.float32 for p in gb.params):
                 raise TypeError("FlatSGD keeps fp32 master parameters; cast activations (autocast), not the parameters")
-            pf = torch.zeros(gb.numel, dtype=torch.float32, device=p0.device)
+            if self._shard_mode is None:
+                pf = torch.zeros(gb.numel, dtype=torch.float32, device=p0.device)
+            else:
+                # padded like the gradient bucket to W equal slices of whole 16-byte gradient vectors
+                es = gb.flat.element_size()
+                n_vec = ((gb.flat.numel() * es + 15) // 16 + self._world - 1) // self._world * self._world
+                n_pad = n_vec * (16 // es)
+                handle = None
+                if self._shard_mode == "kernel":     # symmetric, so that the owners of the other slices can store into it
+                    handle = gb.world.alloc_bytes(n_pad * 4, ll=False)
+                    full = handle.view(torch.float32, n_pad)
+                else:
+                    full = torch.zeros(n_pad, dtype=torch.float32, device=p0.device)
+                self._shards.append((n_vec, n_pad, n_pad // self._world, full, handle))
+                pf = full[:gb.numel]
             with torch.no_grad():
                 for p, o, gv in zip(gb.params, gb.offsets, gb.views):
                     pv = pf[o:o + p.numel()].as_strided(gv.shape, gv.stride())   # same layout as the gradient view
                     pv.copy_(p.data)
                     p.data = pv
             self.param_flats.append(pf)
-            self.momentum_flats.append(torch.zeros_like(pf))
+            if self._shard_mode is None:
+                self.momentum_flats.append(torch.zeros_like(pf))
+            else:
+                self.momentum_flats.append(torch.zeros(self._shards[-1][2], dtype=torch.float32, device=p0.device))
+                gb.sharded_step = lambda max_blocks=None, k=len(self.param_flats) - 1: self._sharded_step(k, max_blocks)
         self._native = None
 
     # ------------------------------------------------------------------ update
@@ -237,6 +300,15 @@ class FlatSGD:
     def step(self) -> None:
         """``optimizer.step()`` (train_dist.py:124) for every bucket, and -- with ``zero_grad=True`` -- the
         ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass."""
+        if self._shard_mode is not None:      # the buckets' exchanges applied the update already
+            if not all(self._done):
+                raise RuntimeError("FlatSGD(sharded=True).step(): this step's gradient buckets were not exchanged; call "
+                                   "average_gradients(model) after backward() (one average_gradients per step)")
+            self._done = [False] * len(self.buckets)
+            self.steps += 1
+            if self._engine is not None:
+                self._engine._reset()
+            return
         lr = self.lr_at()
         kernel = [pf.is_cuda and gb.flat.dtype == torch.float32 for gb, pf in zip(self.buckets, self.param_flats)]
         clip = {}
@@ -268,6 +340,58 @@ class FlatSGD:
         self.steps += 1
         if self.fused_zero and self._engine is not None:
             self._engine._reset()
+
+    @torch.no_grad()
+    def _sharded_step(self, k: int, max_blocks: Optional[int] = None) -> None:
+        """Bucket ``k``'s gradient exchange and update in sharded mode (``GradBucket.exchange_`` calls it on the stream the
+        all-reduce would run on): afterwards every rank holds the updated parameters of the whole bucket."""
+        from .. import comm
+
+        if self._done[k]:
+            raise RuntimeError("FlatSGD(sharded=True): a gradient bucket was exchanged twice in one step, which would apply "
+                               "its update twice; one average_gradients(model) goes with one step()")
+        gb, mf = self.buckets[k], self.momentum_flats[k]
+        n_vec, _, per, full, handle = self._shards[k]
+        lr, W, rank = self.lr_at(), self._world, self._rank
+        if self._shard_mode == "kernel":
+            gh = gb.symm_handle
+            self._kernel().sharded_sgd(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, n_vec, lr,
+                                       self.momentum, self.weight_decay, self.nesterov, 1.0 / W, self.fused_zero,
+                                       gb.world.rank, W, gb.world.max_blocks if max_blocks is None else max_blocks)
+        else:
+            gb.all_reduce_average_(max_blocks)
+            lo = rank * per
+            n = min(lo + per, gb.flat.numel()) - lo          # the rest of the slice is padding no gradient exists for
+            if n > 0:                                        # the unsharded update (step()), on the owned slice
+                pv, mv = full[lo:lo + n], mf[:n]
+                gf = gb.flat[lo:lo + n].to(torch.float32)
+                if self.weight_decay:
+                    gf = gf.add(pv, alpha=self.weight_decay)
+                mv.mul_(self.momentum).add_(gf)
+                pv.add_(gf.add(mv, alpha=self.momentum) if self.nesterov else mv, alpha=-lr)
+            comm.all_gather_into_tensor(full, full[lo:lo + per].clone(), group=self._group)
+            if self.fused_zero:
+                gb.flat.zero_()
+        self._done[k] = True
+
+    def shard_range(self, k: int) -> tuple:
+        """``(lo, hi)``: the elements of bucket ``k``'s flat this rank owns (updates, and holds the momentum of); everything
+        when the optimizer is not sharded over several ranks."""
+        numel = self.buckets[k].numel
+        if self._shard_mode is None:
+            return 0, numel
+        per = self._shards[k][2]
+        return min(self._rank * per, numel), min((self._rank + 1) * per, numel)
+
+    def _full_momentum(self, k: int) -> torch.Tensor:
+        """Bucket ``k``'s whole momentum flat; collective in sharded mode (gathers the shards)."""
+        from .. import comm
+
+        if self._shard_mode is None:
+            return self.momentum_flats[k]
+        full = torch.empty_like(self._shards[k][3])
+        comm.all_gather_into_tensor(full, self.momentum_flats[k], group=self._group)
+        return full
 
     def _clip_on_device(self) -> dict:
         """Every bucket's sum of squares into the fp64 device array (grad_sqnorm, one launch per bucket); the sgd_flat
@@ -305,17 +429,25 @@ class FlatSGD:
 
     # ------------------------------------------------------------------ checkpointing
     def state_dict(self) -> dict:
-        """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``."""
-        return {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
-                "max_grad_norm": self.max_grad_norm, "steps": self.steps,
-                "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
+        """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``.  Sharded over
+        several ranks, the buffers are this rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that
+        crosses world sizes and engines is :meth:`named_momentum`."""
+        sd = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
+              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
+              "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
+        if self._shard_mode is not None:
+            sd.update(sharded=True, world=self._world, rank=self._rank)
+        return sd
 
     def named_momentum(self, model: nn.Module) -> dict:
         """Momentum per parameter NAME (CPU copies) -- the canonical, engine-independent form written to checkpoints: the
-        fused trainer stores exactly this (``state_dict()['momentum']``), so checkpoints cross engines with momentum."""
+        fused trainer stores exactly this (``state_dict()['momentum']``), so checkpoints cross engines with momentum.
+        Sharded over several ranks this is collective: every rank calls it, the shards are gathered, and every rank gets the
+        full tensors an unsharded optimizer would return."""
         names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
         out = {}
-        for gb, mf in zip(self.buckets, self.momentum_flats):
+        for k, gb in enumerate(self.buckets):
+            mf = self._full_momentum(k)
             for p, o, gv in zip(gb.params, gb.offsets, gb.views):
                 if id(p) in names:
                     out[names[id(p)]] = mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).detach().cpu().clone()
@@ -323,15 +455,25 @@ class FlatSGD:
 
     @torch.no_grad()
     def load_named_momentum(self, model: nn.Module, named: dict) -> int:
-        """Inverse of :meth:`named_momentum`; returns how many tensors were restored."""
+        """Inverse of :meth:`named_momentum`; returns how many tensors were restored.  Sharded over several ranks, each rank
+        keeps its slice of the full tensors (not collective)."""
         names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
         done = 0
-        for gb, mf in zip(self.buckets, self.momentum_flats):
+        for k, (gb, mf) in enumerate(zip(self.buckets, self.momentum_flats)):
+            if self._shard_mode is not None:       # lay the tensors out in a whole flat, then cut this rank's slice out
+                shard = mf
+                mf = torch.zeros_like(self._shards[k][3])
+                given = torch.zeros_like(mf, dtype=torch.bool)
             for p, o, gv in zip(gb.params, gb.offsets, gb.views):
                 src = named.get(names.get(id(p)))
                 if src is not None:
                     mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).copy_(src)
+                    if self._shard_mode is not None:
+                        given[o:o + p.numel()] = True
                     done += 1
+            if self._shard_mode is not None:
+                lo, per = self._rank * self._shards[k][2], self._shards[k][2]
+                shard.copy_(torch.where(given[lo:lo + per], mf[lo:lo + per], shard))
         return done
 
     def load_state_dict(self, sd: dict) -> None:
@@ -340,5 +482,17 @@ class FlatSGD:
         self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
         self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))   # ... and before clipping: none
         self.steps = int(sd.get("steps", self.steps))
+        if sd.get("sharded"):                                    # the buffers are the shards of one rank of one world size
+            if self._shard_mode is None or (sd["world"], sd["rank"]) != (self._world, self._rank):
+                raise ValueError(f"this state_dict holds the momentum shard of rank {sd['rank']} of {sd['world']}; it loads "
+                                 f"into a sharded FlatSGD on that rank of a world of that size only.  To change the world size "
+                                 f"or the engine, carry the momentum with named_momentum() / load_named_momentum()")
+        elif self._shard_mode is not None:                       # whole buffers of an unsharded optimizer: take the slice
+            for k, (m, src) in enumerate(zip(self.momentum_flats, sd["momentum_buffers"])):
+                per = self._shards[k][2]
+                whole = torch.zeros(self._shards[k][1], dtype=torch.float32)
+                whole[:src.numel()].copy_(src)
+                m.copy_(whole[self._rank * per:(self._rank + 1) * per])
+            return
         for m, src in zip(self.momentum_flats, sd["momentum_buffers"]):
             m.copy_(src)

@@ -69,6 +69,7 @@ class GradBucket:
         self.numel = n
         self.world = _symm_world(group, dev) if symmetric else None
         self.symm_handle = None
+        self.sharded_step = None         # FlatSGD(sharded=True) registers its per-bucket exchange + update here
         if self.world is not None:
             self.symm_handle = self.world.alloc(n, self.dtype)
             self.flat = self.symm_handle.local
@@ -125,6 +126,14 @@ class GradBucket:
             dist.all_reduce(self.flat, op=dist.ReduceOp.SUM, group=comm._g(self.group))
             self.flat.div_(size)
 
+    def exchange_(self, max_blocks: Optional[int] = None) -> None:
+        """What a step does with the bucket once its gradients are complete: the all-reduce, or -- when a sharded optimizer
+        registered itself -- that optimizer's reduce-scatter + update + parameter all-gather."""
+        if self.sharded_step is not None:
+            self.sharded_step(max_blocks)
+        else:
+            self.all_reduce_average_(max_blocks)
+
 
 def flatten_params(model: nn.Module) -> List[nn.Parameter]:
     """The trainable parameters in definition order (what ``model.parameters()`` of train_dist.py:97 iterates)."""
@@ -149,7 +158,7 @@ def average_gradients(model: nn.Module, group=None) -> None:
     bucket = getattr(model, "_grad_bucket", None)
     if bucket is not None:
         bucket.attach()
-        bucket.all_reduce_average_()
+        bucket.exchange_()
         return
     size = comm.get_world_size(group)
     if size == 1:
@@ -284,9 +293,9 @@ class DistributedDataParallel(nn.Module):
             ev.record(cur)
             self.comm_stream.wait_event(ev)
             with torch.cuda.stream(self.comm_stream):
-                b.gb.all_reduce_average_(self.comm_blocks)
+                b.gb.exchange_(self.comm_blocks)
         else:
-            b.gb.all_reduce_average_()
+            b.gb.exchange_()
 
     def _on_grad(self, p: nn.Parameter):
         b = self._bucket_of[p]

@@ -1,0 +1,70 @@
+#!/usr/bin/env python
+"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` in the tutorial's loop, on synthetic data.
+
+    python examples/train_ddp.py                                  # CPU, gloo, world 2
+    python examples/train_ddp.py --sharded-optimizer              # momentum sharded over the ranks (ZeRO stage 1)
+    python examples/train_ddp.py --backend b200 --size 8 --sharded-optimizer   # one process per GPU: per bucket ONE kernel
+                                                                  # reduces, updates the owned slice and gathers the parameters
+
+The loop is ``backward(); average_gradients(model); optimizer.step()`` either way.  With ``--sharded-optimizer`` the update
+happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
+gradient buckets the parameters are bit for bit the same.  Prints ``Rank r, step s: loss`` for the last step."""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch  # noqa: E402
+import torch.nn as nn  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+import dist_tuto.pth_b200 as dist  # noqa: E402
+
+
+class SmallConvNet(nn.Module):
+    """A generic model (not the library's fused MNIST Net): two convolutions and two linear layers."""
+
+    def __init__(self):
+        super().__init__()
+        self.conv1, self.conv2 = nn.Conv2d(3, 16, 3, padding=1), nn.Conv2d(16, 32, 3, padding=1)
+        self.fc1, self.fc2 = nn.Linear(32 * 4 * 4, 64), nn.Linear(64, 10)
+
+    def forward(self, x):
+        x = F.max_pool2d(F.relu(self.conv1(x)), 2)
+        x = F.max_pool2d(F.relu(self.conv2(x)), 2)
+        return self.fc2(F.relu(self.fc1(x.flatten(1))))
+
+
+def run(rank, size):
+    CFG = json.loads(os.environ["B2_DDP_CFG"])            # spawned ranks re-import this file: pass the CLI through the env
+    dev = torch.device("cuda", torch.cuda.current_device()) if CFG["backend"] != "gloo" and torch.cuda.is_available() \
+        else torch.device("cpu")
+    torch.manual_seed(1234)
+    model = dist.DistributedDataParallel(SmallConvNet().to(dev), bucket_cap_bytes=64 << 10)
+    optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"])
+    loss = None
+    for step in range(CFG["steps"]):
+        g = torch.Generator().manual_seed(1000 * step + rank)        # every rank its own part of the global batch
+        x, y = torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
+        optimizer.zero_grad()
+        loss = F.cross_entropy(model(x), y)
+        loss.backward()
+        dist.average_gradients(model)       # --sharded-optimizer: the parameters are updated when this returns
+        optimizer.step()
+    total = loss.detach().clone()
+    dist.all_reduce(total)
+    print(f"Rank {rank}, step {CFG['steps']}: loss {float(loss.detach()):.6f} (mean over ranks {float(total) / size:.9f}), "
+          f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}")
+
+
+if __name__ == "__main__":
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--size", type=int, default=2)
+    ap.add_argument("--backend", default="gloo")
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--sharded-optimizer", action="store_true",
+                    help="FlatSGD(sharded=True): each rank keeps the momentum of, and updates, 1/size of every bucket")
+    a = ap.parse_args()
+    os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer))
+    dist.launch(run, size=a.size, backend=a.backend)
