@@ -13,6 +13,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
     Partition DataPartitioner partition_dataset         data.py
     Net                                                 models/convnet.py
     average_gradients GradBucket DistributedDataParallel parallel/ddp.py
+    SyncBatchNorm (global-batch statistics)            parallel/sync_bn.py
     FlatSGD (one-launch momentum SGD over flat buffers) ops/optim.py
     run / train / TrainConfig                           train.py
     evaluate (test loss / accuracy, sharded over ranks) ops/convnet_eval.py
@@ -30,6 +31,7 @@ from .data import (Partition, DataPartitioner, partition_dataset, SyntheticMNIST
 from .models.convnet import Net  # noqa: F401
 from .parallel.ddp import (average_gradients, GradBucket, DistributedDataParallel,  # noqa: F401
                            broadcast_parameters)
+from .parallel.sync_bn import SyncBatchNorm  # noqa: F401
 from .ops.optim import FlatSGD, LRSchedule  # noqa: F401
 from .ops.convnet_eval import evaluate  # noqa: F401
 from .train import run, train, TrainConfig  # noqa: F401

@@ -25,9 +25,10 @@ OBJ = os.path.join(CSRC, "build")
 TARGET = os.path.join(HERE, "_C.so")
 
 CU_SOURCES = ["allreduce.cu", "convnet.cu", "convnet_cluster.cu", "sgd.cu", "gemm_tcgen05.cu", "tc_probe.cu", "convnet_batched.cu",
-              "convnet_eval.cu", "p2p.cu", "sharded_sgd.cu"]
+              "convnet_eval.cu", "p2p.cu", "sharded_sgd.cu", "batchnorm.cu"]
 CPP_SOURCES = ["symm_mem.cpp", "loader.cpp", "executor.cpp", "bindings.cpp"]
-HEADERS = ["common.cuh", "tc_common.cuh", "convnet_args.cuh", "convnet_reduce.cuh", "sgd_device.cuh", "lr_schedule.h", "loader.h", "executor.h"]
+HEADERS = ["common.cuh", "tc_common.cuh", "convnet_args.cuh", "convnet_reduce.cuh", "sgd_device.cuh", "lr_schedule.h", "loader.h", "executor.h",
+           "batchnorm.h"]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]

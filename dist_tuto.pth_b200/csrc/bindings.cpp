@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "executor.h"
+#include "batchnorm.h"
 #include "loader.h"
 
 #define B2_MAX_RANKS 8
@@ -77,6 +78,8 @@ int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* param
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
+int b2_bn_launch(int kind, int dtype, int vec, int cl, long long M, long long L, int max_blocks, const b2::bn::Args* args,
+                 unsigned int* grid_out, cudaStream_t stream);
 size_t b2_convnet_smem_bytes();
 int b2_convnet_npar();
 int b2_convnet_step_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
@@ -327,6 +330,110 @@ struct ExecutorPy {
     return py::make_tuple(done, tail, epoch_done != 0);
   }
 };
+
+// ---- SyncBatchNorm (csrc/batchnorm.cu)
+int bn_dtype(const torch::Tensor& t, const char* what) {
+  switch (t.scalar_type()) {
+    case torch::kFloat32: return 0;
+    case torch::kBFloat16: return 1;
+    case torch::kHalf: return 2;
+    default: TORCH_CHECK(false, "sync_batch_norm: ", what, " must be fp32, bf16 or fp16, got ", t.scalar_type());
+  }
+  return 0;
+}
+
+// One SyncBatchNorm kernel.  kind 0: statistics of x into ex; 1: y from ex (+ stats, running stats); 2: backward sums of
+// dy, x into ex (+ grad_weight / grad_bias); 3: dx from ex and stats.  x is [N, C, ...], plain contiguous or channels-last
+// (dy, y and dx share its strides); an [N, C] input (or any input with one element per (n, c)) is channels-last.
+void bn_launch(int kind, torch::Tensor x, c10::optional<torch::Tensor> dy, c10::optional<torch::Tensor> out, torch::Tensor ex,
+               torch::Tensor stats, c10::optional<torch::Tensor> tickets, c10::optional<torch::Tensor> weight,
+               c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> running_mean,
+               c10::optional<torch::Tensor> running_var, c10::optional<torch::Tensor> num_batches_tracked,
+               c10::optional<torch::Tensor> grad_weight, c10::optional<torch::Tensor> grad_bias, double momentum, double eps,
+               int max_blocks) {
+  TORCH_CHECK(kind >= 0 && kind <= 3, "bn_launch: kind 0..3");
+  TORCH_CHECK(x.is_cuda() && x.dim() >= 2, "sync_batch_norm: x must be a CUDA tensor of rank >= 2");
+  const int dt = bn_dtype(x, "the input");
+  const int64_t N = x.size(0), C = x.size(1);
+  TORCH_CHECK(C >= 1 && C < (1ll << 30), "sync_batch_norm: channel count out of range");
+  int64_t L = 1;
+  for (int d = 2; d < x.dim(); ++d) L *= x.size(d);
+  bool cl = false;
+  if (L == 1 && x.is_contiguous()) cl = true;
+  else if (x.is_contiguous()) cl = false;
+  else if ((x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast)) ||
+           (x.dim() == 5 && x.is_contiguous(at::MemoryFormat::ChannelsLast3d))) cl = true;
+  else TORCH_CHECK(false, "sync_batch_norm: x must be contiguous, channels_last or channels_last_3d");
+  const int64_t M = cl ? N * L : N;
+  std::vector<const torch::Tensor*> same;          // tensors laid out as x
+  if (dy.has_value()) same.push_back(&*dy);
+  if (out.has_value()) same.push_back(&*out);
+  for (auto* t : same) {
+    bool ok = t->is_cuda() && t->device() == x.device() && t->scalar_type() == x.scalar_type() && t->sizes() == x.sizes();
+    for (int d = 0; ok && d < x.dim(); ++d) ok = x.size(d) == 1 || t->stride(d) == x.stride(d);   // size-1 strides are free
+    TORCH_CHECK(ok, "sync_batch_norm: dy / y / dx must have the input's dtype, shape and strides");
+  }
+  TORCH_CHECK((kind == 0 || kind == 2 || out.has_value()) && (kind < 2 || dy.has_value()), "bn_launch: missing tensor");
+  const int64_t es = x.element_size(), vw = 16 / es;
+  bool vec = cl ? (C % vw == 0) : (L % vw == 0);
+  vec = vec && (uintptr_t)x.data_ptr() % 16 == 0;
+  for (auto* t : same) vec = vec && (uintptr_t)t->data_ptr() % 16 == 0;
+  const int64_t n_ex = kind < 2 ? 1 + 2 * C : 2 * C;
+  TORCH_CHECK(ex.is_cuda() && ex.is_contiguous() && ex.scalar_type() == torch::kFloat64 && ex.numel() >= n_ex,
+              "sync_batch_norm: the exchange buffer must be contiguous fp64 CUDA of at least ", n_ex, " elements");
+  TORCH_CHECK(stats.is_cuda() && stats.is_contiguous() && stats.scalar_type() == torch::kFloat64 && stats.numel() >= 2 * C + 1,
+              "sync_batch_norm: stats must be contiguous fp64 CUDA [2C + 1]");
+  auto param = [&](const c10::optional<torch::Tensor>& t, const char* what, int* code) -> void* {
+    if (!t.has_value()) return nullptr;
+    TORCH_CHECK(t->is_cuda() && t->device() == x.device() && t->is_contiguous() && t->numel() == C, "sync_batch_norm: ", what,
+                " must be a contiguous CUDA tensor of C elements");
+    const int c = bn_dtype(*t, what);
+    TORCH_CHECK(c == 0 || c == dt, "sync_batch_norm: ", what, " must be fp32 or the input's dtype");
+    TORCH_CHECK(*code < 0 || *code == c, "sync_batch_norm: weight, bias and their gradients (and the running stats) share a dtype");
+    *code = c;
+    return t->data_ptr();
+  };
+  b2::bn::Args a{};
+  int pw = -1, pr = -1;
+  a.x = x.data_ptr();
+  if (kind == 1) a.y = out->data_ptr();
+  if (kind == 3) a.dx = out->data_ptr();
+  if (kind >= 2) a.dy = dy->data_ptr();
+  a.w = param(weight, "weight", &pw);
+  a.b = param(bias, "bias", &pw);
+  a.gw = param(grad_weight, "grad_weight", &pw);
+  a.gb = param(grad_bias, "grad_bias", &pw);
+  a.rmean = param(running_mean, "running_mean", &pr);
+  a.rvar = param(running_var, "running_var", &pr);
+  TORCH_CHECK((a.rmean == nullptr) == (a.rvar == nullptr), "sync_batch_norm: running_mean and running_var go together");
+  a.pw = pw < 0 ? 0 : pw;
+  a.pr = pr < 0 ? 0 : pr;
+  if (num_batches_tracked.has_value()) {
+    TORCH_CHECK(num_batches_tracked->is_cuda() && num_batches_tracked->scalar_type() == torch::kInt64 &&
+                num_batches_tracked->numel() == 1, "sync_batch_norm: num_batches_tracked must be a CUDA int64 scalar");
+    a.nbt = reinterpret_cast<const long long*>(num_batches_tracked->data_ptr());
+  }
+  a.momentum = momentum;
+  a.eps = eps;
+  a.ex = ex.data_ptr<double>();
+  a.n_ex = (int)ex.numel();
+  a.stats = stats.data_ptr<double>();
+  a.count = (long long)(N * L);
+  a.C = (int)C;
+  c10::cuda::CUDAGuard guard(x.device());
+  torch::Tensor part;
+  if (kind == 0 || kind == 2) {
+    TORCH_CHECK(tickets.has_value() && tickets->is_cuda() && tickets->is_contiguous() && tickets->scalar_type() == torch::kInt32 &&
+                tickets->numel() >= C, "sync_batch_norm: tickets must be a contiguous int32 CUDA tensor of at least C elements, "
+                "zero before its first use");
+    unsigned int g[2];
+    ck_cuda(b2_bn_launch(kind, dt, vec, cl, M, L, max_blocks, &a, g, cur_stream()), "bn geometry");
+    part = torch::empty({(int64_t)g[1] * 2 * C}, x.options().dtype(torch::kFloat64));
+    a.part = part.data_ptr<double>();
+    a.tickets = reinterpret_cast<unsigned int*>(tickets->data_ptr());
+  }
+  ck_cuda(b2_bn_launch(kind, dt, vec, cl, M, L, max_blocks, &a, nullptr, cur_stream()), "sync_batch_norm launch");
+}
 
 }  // namespace
 
@@ -676,6 +783,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("max_grad_norm") = py::none(), py::arg("clip_workspace") = py::none(), py::arg("grad_norm_out") = py::none());
   m.def("clip_workspace_numel", [](int64_t n) { return (int64_t)b2_clip_ws_floats((size_t)n); },
         "elements of the fp32 clip_workspace the optimizer kernels need for n flat parameters with max_grad_norm set");
+  m.def("bn_launch", &bn_launch, py::arg("kind"), py::arg("x"), py::arg("dy"), py::arg("out"), py::arg("ex"), py::arg("stats"),
+        py::arg("tickets"), py::arg("weight"), py::arg("bias"), py::arg("running_mean"), py::arg("running_var"),
+        py::arg("num_batches_tracked"), py::arg("grad_weight"), py::arg("grad_bias"), py::arg("momentum"), py::arg("eps"),
+        py::arg("max_blocks"), "one SyncBatchNorm kernel (csrc/batchnorm.cu); parallel/sync_bn.py drives them");
   m.def("grad_sqnorm_workspace_numel", [] { return b2_grad_sqnorm_ws_floats(); });
   m.def("grad_sqnorm", [](torch::Tensor g, torch::Tensor sqnorms, int k, torch::Tensor workspace) {
     // sqnorms[k] = the sum of squares of g (fp32 per thread and CTA, fp64 across the CTAs in CTA order), for sgd_flat's clipping
