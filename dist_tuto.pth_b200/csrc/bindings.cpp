@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "adamw.h"
 #include "executor.h"
 #include "batchnorm.h"
 #include "loader.h"
@@ -75,6 +76,11 @@ int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, f
 int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* momentum,
                           size_t n_vec, float lr, float mu, float wd, int nesterov, float scale, int zero_grad, int rank,
                           int world, int max_blocks, cudaStream_t stream);
+int b2_adamw_flat_launch(float* p, float* m, float* v, float* g, size_t n, const b2::AdamwScalars* s, int zero_grad,
+                         float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream);
+int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
+                            float* exp_avg_sq, size_t n_vec, const b2::AdamwScalars* s, float scale, int zero_grad, int rank,
+                            int world, int max_blocks, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
@@ -190,6 +196,19 @@ float* grad_norm_ptr(const c10::optional<torch::Tensor>& t, const char* what) {
   if (!t.has_value()) return nullptr;
   TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->numel() >= 1, what, ": grad_norm_out: fp32 CUDA [1]");
   return t->data_ptr<float>();
+}
+
+// One AdamW update's scalars (csrc/adamw.h), computed by the host in fp64 (ops/optim.py adamw_scalars): (1 - lr*wd,
+// 1 - beta1, beta2, 1 - beta2, lr / bc1, sqrt(bc2), eps), each rounded once to fp32 here.
+b2::AdamwScalars to_adamw(const std::vector<double>& v, const char* what) {
+  TORCH_CHECK(v.size() == 7, what, ": scalars: (decay, 1 - beta1, beta2, 1 - beta2, step_size, sqrt(bc2), eps), got ", v.size(),
+              " values");
+  for (double x : v) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), what, ": scalars must be finite in fp32");
+  TORCH_CHECK((float)v[5] > 0.f && v[6] >= 0.0, what, ": sqrt(bc2) must be > 0 (update t >= 1) and eps >= 0");
+  b2::AdamwScalars a;
+  a.decay = (float)v[0]; a.w1 = (float)v[1]; a.beta2 = (float)v[2]; a.c2 = (float)v[3];
+  a.step_size = (float)v[4]; a.sbc2 = (float)v[5]; a.eps = (float)v[6];
+  return a;
 }
 
 b2::LrSchedule to_sched(const py::object& o) {
@@ -823,6 +842,64 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
      py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
      py::arg("grad_norm_out") = py::none());
+  m.def("adamw_flat", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                         std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
+                         c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    // FlatAdamW's update of one fp32 bucket (csrc/adamw.cu); with max_grad_norm, g is first scaled by the clip coefficient of
+    // the norm of grad_sqnorm's per-bucket sums
+    const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "adamw_flat: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat");
+    check_cuda_contig(p, "p"); check_cuda_contig(exp_avg, "exp_avg"); check_cuda_contig(exp_avg_sq, "exp_avg_sq");
+    check_cuda_contig(g, "g");
+    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel(), "adamw_flat: p, exp_avg, exp_avg_sq and g: fp32 of ",
+                  "one size");
+      TORCH_CHECK((uintptr_t)t->data_ptr() % 16 == 0, "adamw_flat: 16-byte aligned buffers");
+    }
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_adamw_flat_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
+                                 (size_t)p.numel(), &sc, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+            "adamw_flat launch");
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+  // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instance): as sharded_sgd, with this rank's
+  // exp_avg / exp_avg_sq shards in place of the momentum shard.
+  m.def("sharded_adamw", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                            std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, size_t n_vec,
+                            std::vector<double> scalars, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    check_world(rank, world, "sharded_adamw");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_adamw: one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ",
+                params.size(), " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw: every rank owns n_vec / world vectors, so n_vec must be a multiple of "
+                "world (pad the buffers), got n_vec ", n_vec, " for world ", world);
+    const b2::AdamwScalars sc = to_adamw(scalars, "sharded_adamw");
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
+      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "sharded_adamw: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements (this rank's slice)");
+    }
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw: null or misaligned per-rank pointer");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(exp_avg.device());
+    ck_cuda(b2_sharded_adamw_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), n_vec, &sc,
+                                    (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+            "sharded_adamw launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+     py::arg("n_vec"), py::arg("scalars"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"),
+     py::arg("max_blocks") = 0);
   // Sharded optimizer step of one bucket (csrc/sharded_sgd.cu): reduce-scatter of the gradient buckets `grads`, momentum SGD on
   // this rank's slice with its momentum shard, and the new parameters stored into every rank's flat in `params`.  n_vec counts
   // the 16-byte vectors of one gradient bucket; raw per-rank pointers, like `allreduce`.

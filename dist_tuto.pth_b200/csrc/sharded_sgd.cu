@@ -21,7 +21,13 @@
 //
 // A bf16 bucket (8 gradients per vector) updates two fp32 parameter vectors per gradient vector.  The fp32 sum x scale feeds
 // the update unrounded: the averaged gradient never takes a bf16 round trip.
+//
+// The update is a template parameter of the one kernel (sharded_step_kernel): ShardedSgdUpdate (momentum SGD, FlatSGD) and
+// ShardedAdamwUpdate (AdamW, FlatAdamW: adamw_elem of adamw_device.cuh on the slice's first and second moment shards).  An
+// update type names its argument struct, which carries the fields the skeleton reads (grads, params, sig, n_vec, scale, rank,
+// world, zero_grad), loads its optimizer state for a parameter vector, applies the update and stores the state back.
 #include <cstring>
+#include "adamw_device.cuh"
 #include "common.cuh"
 
 namespace b2 {
@@ -39,6 +45,18 @@ struct ShardedSgdArgs {
   int rank, world, zero_grad;
 };
 
+struct ShardedAdamwArgs {
+  PeerPtrs grads;         // as ShardedSgdArgs
+  PeerPtrs params;
+  SignalPads sig;
+  float* exp_avg;         // this rank's shards of the first and second moments (its slice only)
+  float* exp_avg_sq;
+  size_t n_vec;
+  AdamwScalars s;
+  float scale;
+  int rank, world, zero_grad;
+};
+
 // momentum SGD on four elements, the fmaf sequence of sgd_flat_kernel
 template <bool kNesterov>
 __device__ __forceinline__ void sgd4(float4& p, float4& m, float4 g, float lr, float mu, float wd) {
@@ -51,6 +69,32 @@ __device__ __forceinline__ void sgd4(float4& p, float4& m, float4 g, float lr, f
   p.x = fmaf(-lr, d.x, p.x); p.y = fmaf(-lr, d.y, p.y); p.z = fmaf(-lr, d.z, p.z); p.w = fmaf(-lr, d.w, p.w);
 }
 
+// The per-vector updates of sharded_step_kernel.  q indexes the fp32 state vector within this rank's shard.
+template <bool kNesterov>
+struct ShardedSgdUpdate {
+  using Args = ShardedSgdArgs;
+  static constexpr int kUnroll = kShardUnroll;
+  float4 m;
+  __device__ __forceinline__ void load(const Args& a, size_t q) { m = reinterpret_cast<float4*>(a.momentum)[q]; }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) { sgd4<kNesterov>(p, m, g, a.lr, a.mu, a.wd); }
+  __device__ __forceinline__ void store(const Args& a, size_t q) { reinterpret_cast<float4*>(a.momentum)[q] = m; }
+};
+
+struct ShardedAdamwUpdate {
+  using Args = ShardedAdamwArgs;
+  static constexpr int kUnroll = 1;       // two moment vectors per parameter vector: unroll 2 would not fit in 128 registers
+  float4 m, v;
+  __device__ __forceinline__ void load(const Args& a, size_t q) {
+    m = reinterpret_cast<float4*>(a.exp_avg)[q];
+    v = reinterpret_cast<float4*>(a.exp_avg_sq)[q];
+  }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) { adamw4(p, m, v, g, a.s); }
+  __device__ __forceinline__ void store(const Args& a, size_t q) {
+    reinterpret_cast<float4*>(a.exp_avg)[q] = m;
+    reinterpret_cast<float4*>(a.exp_avg_sq)[q] = v;
+  }
+};
+
 __device__ __forceinline__ float4 as_f4(uint4 v) {
   return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
 }
@@ -58,10 +102,11 @@ __device__ __forceinline__ uint4 as_u4(float4 v) {
   return make_uint4(__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w));
 }
 
-// kBf16: the gradient bucket is bf16 (8 elements per vector), else fp32 (4).  Parameters and momentum are fp32 in both.
-template <bool kBf16, bool kNesterov>
-__global__ void __launch_bounds__(kShardThreads) sharded_sgd_kernel(ShardedSgdArgs a) {
+// kBf16: the gradient bucket is bf16 (8 elements per vector), else fp32 (4).  Parameters and optimizer state are fp32 in both.
+template <bool kBf16, class Update>
+__global__ void __launch_bounds__(kShardThreads) sharded_step_kernel(typename Update::Args a) {
   constexpr int kP = kBf16 ? 2 : 1;                     // fp32 parameter vectors per gradient vector
+  constexpr int kUnroll = Update::kUnroll;           // gradient vectors per thread and pass
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
   const size_t slice = a.n_vec / world;
@@ -70,25 +115,25 @@ __global__ void __launch_bounds__(kShardThreads) sharded_sgd_kernel(ShardedSgdAr
   const size_t off = (size_t)rank * slice;
   const uint4* own = reinterpret_cast<const uint4*>(a.params.p[rank]) + kP * off;
   block_barrier_all_ranks(a.sig, rank, world, ++epoch);          // every rank's gradients are complete
-  for (size_t base = first; base < slice; base += stride * kShardUnroll) {
-    uint4 raw[kShardUnroll][B2_MAX_RANKS];
+  for (size_t base = first; base < slice; base += stride * kUnroll) {
+    uint4 raw[kUnroll][B2_MAX_RANKS];
 #pragma unroll
-    for (int u = 0; u < kShardUnroll; ++u) {
+    for (int u = 0; u < kUnroll; ++u) {
       const size_t j = base + (size_t)u * stride;
 #pragma unroll
       for (int r = 0; r < B2_MAX_RANKS; ++r)
         if (r < world && j < slice) raw[u][r] = ld_cg_v4(reinterpret_cast<const uint4*>(a.grads.p[r]) + off + j);
     }
 #pragma unroll
-    for (int u = 0; u < kShardUnroll; ++u) {
+    for (int u = 0; u < kUnroll; ++u) {
       const size_t j = base + (size_t)u * stride;
       if (j >= slice) continue;
-      float4 p[kP], m[kP], g[kP];
-      float4* mom = reinterpret_cast<float4*>(a.momentum) + kP * j;
+      float4 p[kP], g[kP];
+      Update st[kP];
 #pragma unroll
       for (int h = 0; h < kP; ++h) {
         p[h] = as_f4(ld_cg_v4(own + kP * j + h));
-        m[h] = mom[h];
+        st[h].load(a, kP * j + h);
         g[h] = make_float4(0.f, 0.f, 0.f, 0.f);                  // the all-reduce's accumulator starts at +0 too
       }
 #pragma unroll
@@ -107,8 +152,8 @@ __global__ void __launch_bounds__(kShardThreads) sharded_sgd_kernel(ShardedSgdAr
 #pragma unroll
       for (int h = 0; h < kP; ++h) {
         g[h].x *= a.scale; g[h].y *= a.scale; g[h].z *= a.scale; g[h].w *= a.scale;
-        sgd4<kNesterov>(p[h], m[h], g[h], a.lr, a.mu, a.wd);
-        mom[h] = m[h];
+        st[h].apply(a, p[h], g[h]);
+        st[h].store(a, kP * j + h);
       }
 #pragma unroll
       for (int r = 0; r < B2_MAX_RANKS; ++r) {
@@ -131,6 +176,31 @@ __global__ void __launch_bounds__(kShardThreads) sharded_sgd_kernel(ShardedSgdAr
 
 }  // namespace b2
 
+namespace {
+
+// The checks of both launchers: cudaErrorInvalidValue (and no launch) for a world outside 1..8, a rank outside [0, world), an
+// n_vec that is not a multiple of world (the remainder would be left out) or a null pointer.
+bool shard_args_ok(const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, size_t n_vec, int rank, int world) {
+  if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return false;
+  if (grads == nullptr || params == nullptr || sig == nullptr) return false;
+  if (n_vec % (size_t)world != 0) return false;
+  for (int r = 0; r < world; ++r)
+    if (grads->p[r] == nullptr || params->p[r] == nullptr || sig->pad[r] == nullptr) return false;
+  return true;
+}
+
+// The two-shot all-reduce's grid: ceil(ceil(slice / 512) / 2) CTAs, at most max_blocks.
+dim3 shard_grid(size_t n_vec, int world, int max_blocks) {
+  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
+  size_t blocks = (n_vec / world + b2::kShardThreads - 1) / b2::kShardThreads;
+  blocks = (blocks + 1) / 2;
+  if (blocks < 1) blocks = 1;
+  if (blocks > (size_t)max_blocks) blocks = (size_t)max_blocks;
+  return dim3((unsigned)blocks);
+}
+
+}  // namespace
+
 extern "C" {
 
 // One sharded optimizer step of one bucket on `stream`.  n_vec: 16-byte vectors of the gradient bucket (4 fp32 or, with bf16,
@@ -141,28 +211,38 @@ extern "C" {
 int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* momentum,
                           size_t n_vec, float lr, float mu, float wd, int nesterov, float scale, int zero_grad, int rank,
                           int world, int max_blocks, cudaStream_t stream) {
-  if (world < 1 || world > B2_MAX_RANKS || rank < 0 || rank >= world) return (int)cudaErrorInvalidValue;
-  if (grads == nullptr || params == nullptr || sig == nullptr || momentum == nullptr) return (int)cudaErrorInvalidValue;
-  if (n_vec % (size_t)world != 0) return (int)cudaErrorInvalidValue;
-  for (int r = 0; r < world; ++r)
-    if (grads->p[r] == nullptr || params->p[r] == nullptr || sig->pad[r] == nullptr) return (int)cudaErrorInvalidValue;
+  if (momentum == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world)) return (int)cudaErrorInvalidValue;
   b2::ShardedSgdArgs a;
   memset(&a, 0, sizeof(a));
   a.grads = *grads; a.params = *params; a.sig = *sig; a.momentum = momentum; a.n_vec = n_vec;
   a.lr = lr; a.mu = mu; a.wd = wd; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad;
-  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
-  size_t blocks = (n_vec / world + b2::kShardThreads - 1) / b2::kShardThreads;
-  blocks = (blocks + 1) / 2;
-  if (blocks < 1) blocks = 1;
-  if (blocks > (size_t)max_blocks) blocks = (size_t)max_blocks;
-  const dim3 grid((unsigned)blocks);
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  using namespace b2;
   if (bf16) {
-    if (nesterov) b2::sharded_sgd_kernel<true, true><<<grid, b2::kShardThreads, 0, stream>>>(a);
-    else b2::sharded_sgd_kernel<true, false><<<grid, b2::kShardThreads, 0, stream>>>(a);
+    if (nesterov) sharded_step_kernel<true, ShardedSgdUpdate<true>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<true, ShardedSgdUpdate<false>><<<grid, kShardThreads, 0, stream>>>(a);
   } else {
-    if (nesterov) b2::sharded_sgd_kernel<false, true><<<grid, b2::kShardThreads, 0, stream>>>(a);
-    else b2::sharded_sgd_kernel<false, false><<<grid, b2::kShardThreads, 0, stream>>>(a);
+    if (nesterov) sharded_step_kernel<false, ShardedSgdUpdate<true>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, ShardedSgdUpdate<false>><<<grid, kShardThreads, 0, stream>>>(a);
   }
+  return (int)cudaGetLastError();
+}
+
+// The same step with AdamW (FlatAdamW): `exp_avg` and `exp_avg_sq` are this rank's moment shards, n_vec / world x 4 (x 8)
+// floats each, and `s` the update's scalars (adamw_device.cuh).  Same grid, same refusals.
+int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* exp_avg,
+                            float* exp_avg_sq, size_t n_vec, const b2::AdamwScalars* s, float scale, int zero_grad, int rank,
+                            int world, int max_blocks, cudaStream_t stream) {
+  if (exp_avg == nullptr || exp_avg_sq == nullptr || s == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  b2::ShardedAdamwArgs a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.n_vec = n_vec;
+  a.s = *s; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  using namespace b2;
+  if (bf16) sharded_step_kernel<true, ShardedAdamwUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  else sharded_step_kernel<false, ShardedAdamwUpdate><<<grid, kShardThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 

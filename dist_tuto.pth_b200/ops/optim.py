@@ -15,6 +15,10 @@ arrays once.  (The ConvNet goes further and fuses the all-reduce into the same k
 (csrc/sharded_sgd.cu) reduce-scatters the gradients, updates the slice of the parameters this rank owns and stores the new
 parameters into every rank's flat, so the momentum exists for the owned slice only (optimizer state is 1/W per GPU) and no
 separate update kernel runs.
+
+``FlatAdamW`` is ``torch.optim.AdamW`` on the same flat layout: one ``adamw_flat_kernel`` launch per bucket (csrc/adamw.cu),
+and with ``sharded=True`` the AdamW instance of the same sharded kernel, with both moments sharded.  Both optimizers share
+the layout, the sharding, the exchange hooks and the step bookkeeping (``_FlatOptimizer``).
 """
 from __future__ import annotations
 
@@ -25,7 +29,7 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "LRSchedule", "check_sgd_options", "check_max_grad_norm"]
+__all__ = ["FlatSGD", "FlatAdamW", "LRSchedule", "adamw_scalars", "check_sgd_options", "check_max_grad_norm"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -187,48 +191,24 @@ def _peer_world(gb) -> bool:
     return isinstance(gb.world, symm.SymmWorld)
 
 
-class FlatSGD:
-    """``FlatSGD(model)`` where ``model`` is a plain module, a module carrying ``_grad_bucket`` or a
-    :class:`DistributedDataParallel` wrapper.
+class _FlatOptimizer:
+    """What :class:`FlatSGD` and :class:`FlatAdamW` share: the flat fp32 parameter layout over the gradient buckets (``p.data``
+    becomes a view with the gradient view's offset and strides), the shard padding and the symmetric parameter flats of
+    ``sharded=True``, the registration of the sharded update with the buckets' exchange, the ``step()`` bookkeeping, the lr
+    schedule, on-device gradient-norm clipping, and the gathering and slicing of per-bucket optimizer state.  A subclass
+    allocates its state flats (:meth:`_state_flat`) and updates a whole bucket (``_update``), a bucket in one peer-memory
+    kernel (``_sharded_kernel``) or the owned slice of a bucket with torch ops (``_update_slice``)."""
 
-    ``step()`` expects averaged gradients (call ``average_gradients(model)`` first, as the tutorial loop does) and,
-    with ``zero_grad=True`` (default), leaves the buckets zeroed so no separate ``zero_grad()`` pass is needed;
-    ``zero_grad()`` exists for loop compatibility and is then a no-op apart from re-arming the DDP hooks.
-
-    ``max_grad_norm=c`` clips the averaged gradient first, as ``torch.nn.utils.clip_grad_norm_(params, c)`` would: on CUDA
-    fp32 buckets ``grad_sqnorm`` sums each bucket's squares on the device and ``sgd_flat`` takes the norm and the
-    coefficient there (no host synchronisation); elsewhere ``clip_grad_norm_(..., foreach=False)`` itself runs.
-    :meth:`grad_norm` returns the last update's pre-clip norm.
-
-    ``sharded=True`` shards the optimizer over the ranks (ZeRO stage 1): every bucket is cut into W equal slices, rank r keeps
-    the momentum of slice r only (``momentum_flats[k]`` is that shard, :meth:`shard_range` its element range) and updates
-    only that slice of the parameters, which then reach every rank.  The update runs where the gradient exchange runs, not in
-    ``step()``: the DDP hooks (or ``average_gradients(model)``) launch, per bucket, either ONE ``sharded_sgd`` kernel on a
-    symmetric CUDA world (reduce-scatter in fp32 in rank order, update, parameter all-gather through peer stores; a bf16
-    bucket's fp32 sum feeds the update unrounded) or, elsewhere (gloo, several machines, no symmetric world), the bucket's
-    all-reduce, the update of the owned slice and an ``all_gather_into_tensor`` of the parameters.  So **after
-    ``average_gradients(model)`` the parameters are already updated** and ``p.grad`` is zero (with ``zero_grad=False`` it
-    holds this rank's local, unaveraged gradient on the kernel path and the averaged one elsewhere); ``step()`` launches
-    nothing: it advances ``steps``, re-arms the hooks, and raises if the step's buckets were not exchanged.  One
-    ``average_gradients`` goes with one ``step``.  With fp32 buckets the parameters are bit for bit those of
-    ``sharded=False`` (given the all-reduce's fixed rank order).  ``max_grad_norm`` cannot be combined with it (the total
-    norm needs every bucket reduced before any update) and raises ``ValueError``.  :meth:`named_momentum` is then collective
-    (every rank calls it; it gathers the shards) and returns the same per-name tensors as an unsharded optimizer, so
-    checkpoints stay engine-independent.  At world size 1 the flag changes nothing."""
-
-    def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
-                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
-                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+    def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
+                 max_grad_norm: Optional[float], sharded: bool):
         from .. import comm
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
-        check_sgd_options(momentum, weight_decay, nesterov)
+        name = type(self).__name__
         self.sharded = bool(sharded)
         if self.sharded and max_grad_norm is not None:
-            raise ValueError("FlatSGD(sharded=True) cannot clip: the total norm needs every bucket reduced before any update, "
+            raise ValueError(f"{name}(sharded=True) cannot clip: the total norm needs every bucket reduced before any update, "
                              "and the sharded update runs bucket by bucket during backward; use sharded=False with max_grad_norm")
-        self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
-        self.nesterov = bool(nesterov)
         self.max_grad_norm = check_max_grad_norm(max_grad_norm)
         self._grad_norm = None           # the last update's pre-clip norm (a 0-dim / [1] tensor), see grad_norm()
         self._clip_bufs = None           # kernel path: (fp64 [buckets] squares, grad_sqnorm workspace, fp32 [1] norm)
@@ -246,9 +226,8 @@ class FlatSGD:
                 object.__setattr__(model, "_grad_bucket", gb)
             self.buckets = [gb]
         self.param_flats: List[torch.Tensor] = []
-        self.momentum_flats: List[torch.Tensor] = []
-        # sharded over more than one rank: "kernel" (sharded_sgd on a symmetric CUDA world) or "torch"; None: every rank
-        # holds and updates everything
+        # sharded over more than one rank: "kernel" (one peer-memory kernel per bucket on a symmetric CUDA world) or "torch";
+        # None: every rank holds and updates everything
         self._group = self._engine.group if self._engine is not None else self.buckets[0].group
         self._world, self._rank = comm.get_world_size(self._group), comm.get_rank(self._group)
         self._shard_mode = None
@@ -259,7 +238,7 @@ class FlatSGD:
         for gb in self.buckets:
             p0 = gb.params[0]
             if any(p.dtype != torch.float32 for p in gb.params):
-                raise TypeError("FlatSGD keeps fp32 master parameters; cast activations (autocast), not the parameters")
+                raise TypeError(f"{name} keeps fp32 master parameters; cast activations (autocast), not the parameters")
             if self._shard_mode is None:
                 pf = torch.zeros(gb.numel, dtype=torch.float32, device=p0.device)
             else:
@@ -281,12 +260,16 @@ class FlatSGD:
                     pv.copy_(p.data)
                     p.data = pv
             self.param_flats.append(pf)
-            if self._shard_mode is None:
-                self.momentum_flats.append(torch.zeros_like(pf))
-            else:
-                self.momentum_flats.append(torch.zeros(self._shards[-1][2], dtype=torch.float32, device=p0.device))
+            if self._shard_mode is not None:
                 gb.sharded_step = lambda max_blocks=None, k=len(self.param_flats) - 1: self._sharded_step(k, max_blocks)
         self._native = None
+
+    def _state_flat(self, k: int) -> torch.Tensor:
+        """A zero fp32 state flat for bucket ``k``: the whole flat, or this rank's shard of it when sharded."""
+        pf = self.param_flats[k]
+        if self._shard_mode is None:
+            return torch.zeros_like(pf)
+        return torch.zeros(self._shards[k][2], dtype=torch.float32, device=pf.device)
 
     # ------------------------------------------------------------------ update
     def _kernel(self):
@@ -302,14 +285,13 @@ class FlatSGD:
         ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass."""
         if self._shard_mode is not None:      # the buckets' exchanges applied the update already
             if not all(self._done):
-                raise RuntimeError("FlatSGD(sharded=True).step(): this step's gradient buckets were not exchanged; call "
-                                   "average_gradients(model) after backward() (one average_gradients per step)")
+                raise RuntimeError(f"{type(self).__name__}(sharded=True).step(): this step's gradient buckets were not "
+                                   "exchanged; call average_gradients(model) after backward() (one average_gradients per step)")
             self._done = [False] * len(self.buckets)
             self.steps += 1
             if self._engine is not None:
                 self._engine._reset()
             return
-        lr = self.lr_at()
         kernel = [pf.is_cuda and gb.flat.dtype == torch.float32 for gb, pf in zip(self.buckets, self.param_flats)]
         clip = {}
         if self.max_grad_norm is not None:
@@ -322,21 +304,7 @@ class FlatSGD:
                     params += gb.params
                 self._grad_norm = torch.nn.utils.clip_grad_norm_(params, self.max_grad_norm, foreach=False)
                 kernel = [False] * len(kernel)
-        for gb, pf, mf, kern in zip(self.buckets, self.param_flats, self.momentum_flats, kernel):
-            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
-            if kern:
-                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov,
-                                        **clip)
-                continue
-            # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
-            # torch.optim.SGD's order (foreach=False)
-            gf = g.to(torch.float32)
-            if self.weight_decay:
-                gf = gf.add(pf, alpha=self.weight_decay)
-            mf.mul_(self.momentum).add_(gf)
-            pf.add_(gf.add(mf, alpha=self.momentum) if self.nesterov else mf, alpha=-lr)
-            if self.fused_zero:
-                g.zero_()
+        self._update(kernel, clip)
         self.steps += 1
         if self.fused_zero and self._engine is not None:
             self._engine._reset()
@@ -348,53 +316,104 @@ class FlatSGD:
         from .. import comm
 
         if self._done[k]:
-            raise RuntimeError("FlatSGD(sharded=True): a gradient bucket was exchanged twice in one step, which would apply "
-                               "its update twice; one average_gradients(model) goes with one step()")
-        gb, mf = self.buckets[k], self.momentum_flats[k]
-        n_vec, _, per, full, handle = self._shards[k]
-        lr, W, rank = self.lr_at(), self._world, self._rank
+            raise RuntimeError(f"{type(self).__name__}(sharded=True): a gradient bucket was exchanged twice in one step, which "
+                               "would apply its update twice; one average_gradients(model) goes with one step()")
+        gb = self.buckets[k]
+        per, full = self._shards[k][2], self._shards[k][3]
         if self._shard_mode == "kernel":
-            gh = gb.symm_handle
-            self._kernel().sharded_sgd(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, n_vec, lr,
-                                       self.momentum, self.weight_decay, self.nesterov, 1.0 / W, self.fused_zero,
-                                       gb.world.rank, W, gb.world.max_blocks if max_blocks is None else max_blocks)
+            self._sharded_kernel(k, gb.world.max_blocks if max_blocks is None else max_blocks)
         else:
             gb.all_reduce_average_(max_blocks)
-            lo = rank * per
+            lo = self._rank * per
             n = min(lo + per, gb.flat.numel()) - lo          # the rest of the slice is padding no gradient exists for
             if n > 0:                                        # the unsharded update (step()), on the owned slice
-                pv, mv = full[lo:lo + n], mf[:n]
-                gf = gb.flat[lo:lo + n].to(torch.float32)
-                if self.weight_decay:
-                    gf = gf.add(pv, alpha=self.weight_decay)
-                mv.mul_(self.momentum).add_(gf)
-                pv.add_(gf.add(mv, alpha=self.momentum) if self.nesterov else mv, alpha=-lr)
+                self._update_slice(k, lo, n)
             comm.all_gather_into_tensor(full, full[lo:lo + per].clone(), group=self._group)
             if self.fused_zero:
                 gb.flat.zero_()
         self._done[k] = True
 
     def shard_range(self, k: int) -> tuple:
-        """``(lo, hi)``: the elements of bucket ``k``'s flat this rank owns (updates, and holds the momentum of); everything
-        when the optimizer is not sharded over several ranks."""
+        """``(lo, hi)``: the elements of bucket ``k``'s flat this rank owns (updates, and holds the optimizer state of);
+        everything when the optimizer is not sharded over several ranks."""
         numel = self.buckets[k].numel
         if self._shard_mode is None:
             return 0, numel
         per = self._shards[k][2]
         return min(self._rank * per, numel), min((self._rank + 1) * per, numel)
 
-    def _full_momentum(self, k: int) -> torch.Tensor:
-        """Bucket ``k``'s whole momentum flat; collective in sharded mode (gathers the shards)."""
+    def _full_flat(self, k: int, flat: torch.Tensor) -> torch.Tensor:
+        """Bucket ``k``'s whole state flat of which ``flat`` is this rank's part; collective in sharded mode (gathers)."""
         from .. import comm
 
         if self._shard_mode is None:
-            return self.momentum_flats[k]
+            return flat
         full = torch.empty_like(self._shards[k][3])
-        comm.all_gather_into_tensor(full, self.momentum_flats[k], group=self._group)
+        comm.all_gather_into_tensor(full, flat, group=self._group)
         return full
 
+    def _named(self, model: nn.Module, flats: List[torch.Tensor]) -> dict:
+        """``{parameter name: its part of the state flats}`` (CPU copies); collective in sharded mode."""
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        out = {}
+        for k, gb in enumerate(self.buckets):
+            f = self._full_flat(k, flats[k])
+            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
+                if id(p) in names:
+                    out[names[id(p)]] = f[o:o + p.numel()].as_strided(gv.shape, gv.stride()).detach().cpu().clone()
+        return out
+
+    @torch.no_grad()
+    def _load_named(self, model: nn.Module, named: dict, flats: List[torch.Tensor]) -> int:
+        """Inverse of :meth:`_named`; returns how many tensors were restored.  Sharded over several ranks, each rank keeps its
+        slice of the full tensors (not collective)."""
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        done = 0
+        for k, (gb, mf) in enumerate(zip(self.buckets, flats)):
+            if self._shard_mode is not None:       # lay the tensors out in a whole flat, then cut this rank's slice out
+                shard = mf
+                mf = torch.zeros_like(self._shards[k][3])
+                given = torch.zeros_like(mf, dtype=torch.bool)
+            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
+                src = named.get(names.get(id(p)))
+                if src is not None:
+                    mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).copy_(src)
+                    if self._shard_mode is not None:
+                        given[o:o + p.numel()] = True
+                    done += 1
+            if self._shard_mode is not None:
+                lo, per = self._rank * self._shards[k][2], self._shards[k][2]
+                shard.copy_(torch.where(given[lo:lo + per], mf[lo:lo + per], shard))
+        return done
+
+    def _shard_tags(self) -> dict:
+        """What a state_dict records when its buffers are one rank's shards."""
+        return dict(sharded=True, world=self._world, rank=self._rank) if self._shard_mode is not None else {}
+
+    @torch.no_grad()
+    def _load_flats(self, sd: dict, pairs: list, noun: str, carry: str) -> None:
+        """The buffers of ``sd`` into the state flats, ``pairs`` = [(flats, saved buffers)]: shards load on their own rank of
+        their own world size only; whole buffers of an unsharded optimizer load into a sharded one as this rank's slice.
+        ``noun`` names the state and ``carry`` the per-name methods that cross world sizes."""
+        if sd.get("sharded"):                                    # the buffers are the shards of one rank of one world size
+            if self._shard_mode is None or (sd["world"], sd["rank"]) != (self._world, self._rank):
+                raise ValueError(f"this state_dict holds the {noun} shard of rank {sd['rank']} of {sd['world']}; it loads "
+                                 f"into a sharded {type(self).__name__} on that rank of a world of that size only.  To change "
+                                 f"the world size or the engine, carry the {noun} with {carry}")
+        elif self._shard_mode is not None:                       # whole buffers of an unsharded optimizer: take the slice
+            for flats, saved in pairs:
+                for k, (m, src) in enumerate(zip(flats, saved)):
+                    per = self._shards[k][2]
+                    whole = torch.zeros(self._shards[k][1], dtype=torch.float32)
+                    whole[:src.numel()].copy_(src)
+                    m.copy_(whole[self._rank * per:(self._rank + 1) * per])
+            return
+        for flats, saved in pairs:
+            for m, src in zip(flats, saved):
+                m.copy_(src)
+
     def _clip_on_device(self) -> dict:
-        """Every bucket's sum of squares into the fp64 device array (grad_sqnorm, one launch per bucket); the sgd_flat
+        """Every bucket's sum of squares into the fp64 device array (grad_sqnorm, one launch per bucket); the update kernel's
         arguments that take the norm and the coefficient from it."""
         C = self._kernel()
         if self._clip_bufs is None:
@@ -427,6 +446,83 @@ class FlatSGD:
             for gb in self.buckets:
                 gb.zero_()
 
+
+class FlatSGD(_FlatOptimizer):
+    """``FlatSGD(model)`` where ``model`` is a plain module, a module carrying ``_grad_bucket`` or a
+    :class:`DistributedDataParallel` wrapper.
+
+    ``step()`` expects averaged gradients (call ``average_gradients(model)`` first, as the tutorial loop does) and,
+    with ``zero_grad=True`` (default), leaves the buckets zeroed so no separate ``zero_grad()`` pass is needed;
+    ``zero_grad()`` exists for loop compatibility and is then a no-op apart from re-arming the DDP hooks.
+
+    ``max_grad_norm=c`` clips the averaged gradient first, as ``torch.nn.utils.clip_grad_norm_(params, c)`` would: on CUDA
+    fp32 buckets ``grad_sqnorm`` sums each bucket's squares on the device and ``sgd_flat`` takes the norm and the
+    coefficient there (no host synchronisation); elsewhere ``clip_grad_norm_(..., foreach=False)`` itself runs.
+    :meth:`grad_norm` returns the last update's pre-clip norm.
+
+    ``sharded=True`` shards the optimizer over the ranks (ZeRO stage 1): every bucket is cut into W equal slices, rank r keeps
+    the momentum of slice r only (``momentum_flats[k]`` is that shard, :meth:`shard_range` its element range) and updates
+    only that slice of the parameters, which then reach every rank.  The update runs where the gradient exchange runs, not in
+    ``step()``: the DDP hooks (or ``average_gradients(model)``) launch, per bucket, either ONE ``sharded_sgd`` kernel on a
+    symmetric CUDA world (reduce-scatter in fp32 in rank order, update, parameter all-gather through peer stores; a bf16
+    bucket's fp32 sum feeds the update unrounded) or, elsewhere (gloo, several machines, no symmetric world), the bucket's
+    all-reduce, the update of the owned slice and an ``all_gather_into_tensor`` of the parameters.  So **after
+    ``average_gradients(model)`` the parameters are already updated** and ``p.grad`` is zero (with ``zero_grad=False`` it
+    holds this rank's local, unaveraged gradient on the kernel path and the averaged one elsewhere); ``step()`` launches
+    nothing: it advances ``steps``, re-arms the hooks, and raises if the step's buckets were not exchanged.  One
+    ``average_gradients`` goes with one ``step``.  With fp32 buckets the parameters are bit for bit those of
+    ``sharded=False`` (given the all-reduce's fixed rank order).  ``max_grad_norm`` cannot be combined with it (the total
+    norm needs every bucket reduced before any update) and raises ``ValueError``.  :meth:`named_momentum` is then collective
+    (every rank calls it; it gathers the shards) and returns the same per-name tensors as an unsharded optimizer, so
+    checkpoints stay engine-independent.  At world size 1 the flag changes nothing."""
+
+    def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
+                 zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
+                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+        check_sgd_options(momentum, weight_decay, nesterov)
+        self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
+        self.nesterov = bool(nesterov)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded)
+        self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        lr = self.lr_at()
+        for gb, pf, mf, kern in zip(self.buckets, self.param_flats, self.momentum_flats, kernel):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern:
+                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov,
+                                        **clip)
+                continue
+            # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
+            # torch.optim.SGD's order (foreach=False)
+            gf = g.to(torch.float32)
+            if self.weight_decay:
+                gf = gf.add(pf, alpha=self.weight_decay)
+            mf.mul_(self.momentum).add_(gf)
+            pf.add_(gf.add(mf, alpha=self.momentum) if self.nesterov else mf, alpha=-lr)
+            if self.fused_zero:
+                g.zero_()
+
+    def _sharded_kernel(self, k: int, max_blocks: int) -> None:
+        gb, mf = self.buckets[k], self.momentum_flats[k]
+        n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        self._kernel().sharded_sgd(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, n_vec, self.lr_at(),
+                                   self.momentum, self.weight_decay, self.nesterov, 1.0 / W, self.fused_zero, gb.world.rank, W,
+                                   max_blocks)
+
+    def _update_slice(self, k: int, lo: int, n: int) -> None:
+        lr = self.lr_at()
+        pv, mv = self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n]
+        gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
+        if self.weight_decay:
+            gf = gf.add(pv, alpha=self.weight_decay)
+        mv.mul_(self.momentum).add_(gf)
+        pv.add_(gf.add(mv, alpha=self.momentum) if self.nesterov else mv, alpha=-lr)
+
+    def _full_momentum(self, k: int) -> torch.Tensor:
+        """Bucket ``k``'s whole momentum flat; collective in sharded mode (gathers the shards)."""
+        return self._full_flat(k, self.momentum_flats[k])
+
     # ------------------------------------------------------------------ checkpointing
     def state_dict(self) -> dict:
         """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``.  Sharded over
@@ -435,8 +531,7 @@ class FlatSGD:
         sd = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
               "max_grad_norm": self.max_grad_norm, "steps": self.steps,
               "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
-        if self._shard_mode is not None:
-            sd.update(sharded=True, world=self._world, rank=self._rank)
+        sd.update(self._shard_tags())
         return sd
 
     def named_momentum(self, model: nn.Module) -> dict:
@@ -444,37 +539,12 @@ class FlatSGD:
         fused trainer stores exactly this (``state_dict()['momentum']``), so checkpoints cross engines with momentum.
         Sharded over several ranks this is collective: every rank calls it, the shards are gathered, and every rank gets the
         full tensors an unsharded optimizer would return."""
-        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
-        out = {}
-        for k, gb in enumerate(self.buckets):
-            mf = self._full_momentum(k)
-            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
-                if id(p) in names:
-                    out[names[id(p)]] = mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).detach().cpu().clone()
-        return out
+        return self._named(model, self.momentum_flats)
 
-    @torch.no_grad()
     def load_named_momentum(self, model: nn.Module, named: dict) -> int:
         """Inverse of :meth:`named_momentum`; returns how many tensors were restored.  Sharded over several ranks, each rank
         keeps its slice of the full tensors (not collective)."""
-        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
-        done = 0
-        for k, (gb, mf) in enumerate(zip(self.buckets, self.momentum_flats)):
-            if self._shard_mode is not None:       # lay the tensors out in a whole flat, then cut this rank's slice out
-                shard = mf
-                mf = torch.zeros_like(self._shards[k][3])
-                given = torch.zeros_like(mf, dtype=torch.bool)
-            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
-                src = named.get(names.get(id(p)))
-                if src is not None:
-                    mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).copy_(src)
-                    if self._shard_mode is not None:
-                        given[o:o + p.numel()] = True
-                    done += 1
-            if self._shard_mode is not None:
-                lo, per = self._rank * self._shards[k][2], self._shards[k][2]
-                shard.copy_(torch.where(given[lo:lo + per], mf[lo:lo + per], shard))
-        return done
+        return self._load_named(model, named, self.momentum_flats)
 
     def load_state_dict(self, sd: dict) -> None:
         """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
@@ -482,17 +552,137 @@ class FlatSGD:
         self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
         self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))   # ... and before clipping: none
         self.steps = int(sd.get("steps", self.steps))
-        if sd.get("sharded"):                                    # the buffers are the shards of one rank of one world size
-            if self._shard_mode is None or (sd["world"], sd["rank"]) != (self._world, self._rank):
-                raise ValueError(f"this state_dict holds the momentum shard of rank {sd['rank']} of {sd['world']}; it loads "
-                                 f"into a sharded FlatSGD on that rank of a world of that size only.  To change the world size "
-                                 f"or the engine, carry the momentum with named_momentum() / load_named_momentum()")
-        elif self._shard_mode is not None:                       # whole buffers of an unsharded optimizer: take the slice
-            for k, (m, src) in enumerate(zip(self.momentum_flats, sd["momentum_buffers"])):
-                per = self._shards[k][2]
-                whole = torch.zeros(self._shards[k][1], dtype=torch.float32)
-                whole[:src.numel()].copy_(src)
-                m.copy_(whole[self._rank * per:(self._rank + 1) * per])
-            return
-        for m, src in zip(self.momentum_flats, sd["momentum_buffers"]):
-            m.copy_(src)
+        self._load_flats(sd, [(self.momentum_flats, sd["momentum_buffers"])], "momentum",
+                         "named_momentum() / load_named_momentum()")
+
+
+def check_adamw_options(lr: float, betas, eps: float, weight_decay: float) -> tuple:
+    """``torch.optim.AdamW``'s rules for the hyper-parameters; returns ``(beta1, beta2)`` as floats."""
+    if not float(lr) >= 0.0:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if not float(eps) >= 0.0:
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    b1, b2 = (float(b) for b in betas)
+    if not 0.0 <= b1 < 1.0:
+        raise ValueError(f"Invalid beta parameter at index 0: {b1}")
+    if not 0.0 <= b2 < 1.0:
+        raise ValueError(f"Invalid beta parameter at index 1: {b2}")
+    if not float(weight_decay) >= 0.0:
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+    return b1, b2
+
+
+def adamw_scalars(lr: float, betas: tuple, eps: float, weight_decay: float, t: int) -> list:
+    """The scalars of AdamW update ``t`` (1-based) that the kernels take (csrc/adamw.h), in fp64 as torch's non-capturable
+    single-tensor path computes them: ``[1 - lr*wd, 1 - beta1, beta2, 1 - beta2, lr / (1 - beta1^t), sqrt(1 - beta2^t), eps]``.
+    The bindings round each once to fp32."""
+    b1, b2 = betas
+    return [1.0 - lr * weight_decay, 1.0 - b1, b2, 1.0 - b2, lr / (1.0 - b1 ** t), (1.0 - b2 ** t) ** 0.5, eps]
+
+
+class FlatAdamW(_FlatOptimizer):
+    """``torch.optim.AdamW`` (``amsgrad=False``, ``maximize=False``) over flat buffers: ``FlatAdamW(model)`` where ``model``
+    is a plain module, a module carrying ``_grad_bucket`` or a :class:`DistributedDataParallel` wrapper, in the same loop as
+    :class:`FlatSGD` (``backward(); average_gradients(model); opt.step()``).
+
+    The first and second moments (``exp_avg_flats``, ``exp_avg_sq_flats``) have the parameter flats' layout, so on CUDA fp32
+    buckets ONE ``adamw_flat`` launch per bucket (csrc/adamw.cu) streams the parameters, gradients and both moments once,
+    and with ``zero_grad=True`` (default) re-zeroes the gradients in the same pass.  Update k (``steps`` before it) uses
+    t = k + 1; ``1 - lr*wd``, ``lr / (1 - beta1^t)`` and ``sqrt(1 - beta2^t)`` are computed on the host in fp64, as torch
+    does, with ``lr = lr_at()`` (:class:`LRSchedule`).  Elsewhere (CPU tensors, bf16 buckets) torch's own single-tensor
+    AdamW runs on each parameter's views of the flats, so a CPU run is bit for bit ``torch.optim.AdamW(foreach=False)``.
+
+    ``max_grad_norm=c`` clips first, as :class:`FlatSGD` does (``grad_sqnorm`` and the clip coefficient on the device, no
+    host synchronisation; :meth:`grad_norm`).  ``sharded=True`` is :class:`FlatSGD`'s ZeRO stage 1 with both moments
+    sharded (8/W bytes of state per parameter): per bucket ONE ``sharded_adamw`` kernel reduce-scatters the gradients in
+    fp32 in rank order, applies AdamW to the owned slice and stores the new parameters into every rank's flat, inside
+    ``average_gradients`` / the DDP hooks; ``step()`` only counts the step.  Without one peer-memory world torch ops run the
+    same semantics; at world size 1 the flag changes nothing; with ``max_grad_norm`` it raises ``ValueError``.
+    :meth:`named_state` (collective when sharded) is ``torch.optim.AdamW``'s per-parameter state by parameter name."""
+
+    def __init__(self, model: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
+                 weight_decay: float = 1e-2, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
+                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+        self.betas = check_adamw_options(lr, betas, eps, weight_decay)
+        self.lr, self.eps, self.weight_decay = float(lr), float(eps), float(weight_decay)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded)
+        self.exp_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+        self.exp_avg_sq_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+
+    def scalars(self) -> list:
+        """:func:`adamw_scalars` of the next update (t = ``steps`` + 1, lr = :meth:`lr_at`)."""
+        return adamw_scalars(self.lr_at(), self.betas, self.eps, self.weight_decay, self.steps + 1)
+
+    def _torch_adamw(self, p: list, g: list, m: list, v: list) -> None:
+        """torch's single-tensor AdamW on the given views (update t = steps + 1)."""
+        from torch.optim.adamw import adamw
+
+        steps = [torch.tensor(float(self.steps)) for _ in p]
+        adamw(p, g, m, v, [], steps, foreach=False, capturable=False, differentiable=False, fused=None, amsgrad=False,
+              beta1=self.betas[0], beta2=self.betas[1], lr=self.lr_at(), weight_decay=self.weight_decay, eps=self.eps,
+              maximize=False)
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        sc = self.scalars() if any(kernel) else None
+        for gb, pf, mf, vf, kern in zip(self.buckets, self.param_flats, self.exp_avg_flats, self.exp_avg_sq_flats, kernel):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern:
+                self._kernel().adamw_flat(pf, mf, vf, g, sc, self.fused_zero, **clip)
+                continue
+            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
+                     for f in (pf, gf, mf, vf)]
+            self._torch_adamw(*views)
+            if self.fused_zero:
+                g.zero_()
+
+    def _sharded_kernel(self, k: int, max_blocks: int) -> None:
+        gb = self.buckets[k]
+        n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        self._kernel().sharded_adamw(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, self.exp_avg_flats[k],
+                                     self.exp_avg_sq_flats[k], n_vec, self.scalars(), 1.0 / W, self.fused_zero, gb.world.rank,
+                                     W, max_blocks)
+
+    def _update_slice(self, k: int, lo: int, n: int) -> None:
+        gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
+        self._torch_adamw([self._shards[k][3][lo:lo + n]], [gf], [self.exp_avg_flats[k][:n]], [self.exp_avg_sq_flats[k][:n]])
+
+    # ------------------------------------------------------------------ checkpointing
+    def state_dict(self) -> dict:
+        """Hyper-parameters, ``steps`` and the flat moment buffers (CPU copies).  Sharded over several ranks, the buffers are
+        this rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that crosses world sizes and modes is
+        :meth:`named_state`."""
+        sd = {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
+              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
+              "exp_avg": [m.detach().cpu().clone() for m in self.exp_avg_flats],
+              "exp_avg_sq": [v.detach().cpu().clone() for v in self.exp_avg_sq_flats]}
+        sd.update(self._shard_tags())
+        return sd
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
+        self._load_flats(sd, [(self.exp_avg_flats, sd["exp_avg"]), (self.exp_avg_sq_flats, sd["exp_avg_sq"])],
+                         "AdamW state", "named_state() / load_named_state()")
+        self.betas = check_adamw_options(sd["lr"], sd["betas"], sd["eps"], sd["weight_decay"])
+        self.lr, self.eps, self.weight_decay = float(sd["lr"]), float(sd["eps"]), float(sd["weight_decay"])
+        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
+        self.steps = int(sd["steps"])
+
+    def named_state(self, model: nn.Module) -> dict:
+        """``{name: {"step", "exp_avg", "exp_avg_sq"}}`` (CPU copies), ``torch.optim.AdamW``'s per-parameter state by
+        parameter name, the form that crosses world sizes, sharded and unsharded runs and ``torch.optim.AdamW``.  Sharded
+        over several ranks this is collective: every rank calls it and gets the full tensors."""
+        m, v = self._named(model, self.exp_avg_flats), self._named(model, self.exp_avg_sq_flats)
+        return {n: {"step": torch.tensor(float(self.steps)), "exp_avg": m[n], "exp_avg_sq": v[n]} for n in m}
+
+    def load_named_state(self, model: nn.Module, named: dict) -> int:
+        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
+        (common) ``step``.  Sharded over several ranks, each rank keeps its slice (not collective)."""
+        steps = {int(s["step"]) for s in named.values()}
+        if len(steps) > 1:
+            raise ValueError(f"FlatAdamW keeps one step count for all parameters; this state has steps {sorted(steps)}")
+        done = self._load_named(model, {n: s["exp_avg"] for n, s in named.items()}, self.exp_avg_flats)
+        self._load_named(model, {n: s["exp_avg_sq"] for n, s in named.items()}, self.exp_avg_sq_flats)
+        if done and steps:
+            self.steps = steps.pop()
+        return done

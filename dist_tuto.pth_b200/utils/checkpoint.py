@@ -7,7 +7,11 @@ using the reference's parameter names).  Momentum is always ALSO stored per
 parameter name under ``"momentum"`` -- the one form both engines read -- so a
 checkpoint written by the fused engine resumes on the torch engine (and vice
 versa) with its momentum; a checkpoint whose momentum the loading side cannot
-use raises a warning instead of silently training from zero momentum."""
+use raises a warning instead of silently training from zero momentum.
+
+``FlatAdamW`` state is stored the same way, per parameter name under
+``"optim_state"`` (``named_state()``: ``torch.optim.AdamW``'s per-parameter
+form), so an AdamW checkpoint crosses world sizes and sharded / unsharded runs."""
 from __future__ import annotations
 
 import os
@@ -29,6 +33,8 @@ def save_checkpoint(path: str, model, optimizer=None, **extra: Any) -> str:
         blob["optim"] = optimizer.state_dict()
         if "momentum" not in blob and hasattr(optimizer, "named_momentum"):
             blob["momentum"] = optimizer.named_momentum(model)        # canonical per-name form (see module docstring)
+        if hasattr(optimizer, "named_state"):
+            blob["optim_state"] = optimizer.named_state(model)        # FlatAdamW's per-name form
     blob.update(extra)
     tmp = f"{path}.tmp.{os.getpid()}"
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
@@ -39,7 +45,7 @@ def save_checkpoint(path: str, model, optimizer=None, **extra: Any) -> str:
 
 def load_checkpoint(path: str, model=None, optimizer=None, map_location="cpu") -> Dict[str, Any]:
     """Restore ``model`` (an ``nn.Module`` or a fused trainer) and, when given, ``optimizer`` (``torch.optim`` or
-    ``FlatSGD``) from ``path``; returns the whole blob (``steps``, ``history``, ...)."""
+    ``FlatSGD`` / ``FlatAdamW``) from ``path``; returns the whole blob (``steps``, ``history``, ...)."""
     blob = torch.load(path, map_location=map_location)
     if model is not None:
         if isinstance(model, torch.nn.Module):
@@ -63,8 +69,12 @@ def restore_optimizer(optimizer, model, blob: Dict[str, Any]) -> None:
         except Exception as e:                     # different bucket layout / optimizer class: fall through to names
             warnings.warn(f"checkpoint optimizer state does not fit this optimizer ({e!r}); trying per-name momentum")
     named = blob.get("momentum")
-    if named and hasattr(optimizer, "load_named_momentum") and model is not None:
+    state = blob.get("optim_state")
+    if state and hasattr(optimizer, "load_named_state") and model is not None:
+        if optimizer.load_named_state(model, state) == 0:
+            warnings.warn("checkpoint optimizer-state names match no parameter of this model: the state restarts at zero")
+    elif named and hasattr(optimizer, "load_named_momentum") and model is not None:
         if optimizer.load_named_momentum(model, named) == 0:
             warnings.warn("checkpoint momentum names match no parameter of this model: momentum restarts at zero")
-    elif named or optim is not None:
+    elif named or state or optim is not None:
         warnings.warn("checkpoint carries momentum this optimizer cannot read: momentum restarts at zero")

@@ -1,10 +1,12 @@
 #!/usr/bin/env python
-"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` in the tutorial's loop, on synthetic data.
+"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` (or ``FlatAdamW``) in the tutorial's loop, on
+synthetic data.
 
     python examples/train_ddp.py                                  # CPU, gloo, world 2
     python examples/train_ddp.py --sharded-optimizer              # momentum sharded over the ranks (ZeRO stage 1)
     python examples/train_ddp.py --backend b200 --size 8 --sharded-optimizer   # one process per GPU: per bucket ONE kernel
                                                                   # reduces, updates the owned slice and gathers the parameters
+    python examples/train_ddp.py --optimizer adamw [--sharded-optimizer]   # FlatAdamW; sharded: both moments 1/size per rank
 
 The loop is ``backward(); average_gradients(model); optimizer.step()`` either way.  With ``--sharded-optimizer`` the update
 happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
@@ -42,7 +44,10 @@ def run(rank, size):
         else torch.device("cpu")
     torch.manual_seed(1234)
     model = dist.DistributedDataParallel(SmallConvNet().to(dev), bucket_cap_bytes=64 << 10)
-    optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"])
+    if CFG["optimizer"] == "adamw":
+        optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"])
+    else:
+        optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"])
     loss = None
     for step in range(CFG["steps"]):
         g = torch.Generator().manual_seed(1000 * step + rank)        # every rank its own part of the global batch
@@ -54,8 +59,12 @@ def run(rank, size):
         optimizer.step()
     total = loss.detach().clone()
     dist.all_reduce(total)
+    if CFG["optimizer"] == "adamw":
+        state = f"AdamW moment elements on this rank {sum(m.numel() for m in optimizer.exp_avg_flats + optimizer.exp_avg_sq_flats)}"
+    else:
+        state = f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}"
     print(f"Rank {rank}, step {CFG['steps']}: loss {float(loss.detach()):.6f} (mean over ranks {float(total) / size:.9f}), "
-          f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}")
+          + state)
 
 
 if __name__ == "__main__":
@@ -64,7 +73,10 @@ if __name__ == "__main__":
     ap.add_argument("--backend", default="gloo")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--sharded-optimizer", action="store_true",
-                    help="FlatSGD(sharded=True): each rank keeps the momentum of, and updates, 1/size of every bucket")
+                    help="sharded=True: each rank keeps the optimizer state of, and updates, 1/size of every bucket")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
+                    help="FlatSGD (momentum SGD, the default) or FlatAdamW")
     a = ap.parse_args()
-    os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer))
+    os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
+                                                optimizer=a.optimizer))
     dist.launch(run, size=a.size, backend=a.backend)
