@@ -17,11 +17,18 @@
 
 namespace b2 {
 
-__device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g, const AdamwScalars& s) {
-  p = __fmul_rn(p, s.decay);
+// The moment lines of the sequence above, shared with LAMB (layerwise_device.cuh).  S: any type with the fields w1 (1 - beta1),
+// beta2 and c2 (1 - beta2): AdamwScalars or LwArgs.
+template <class S>
+__device__ __forceinline__ void adam_moments(float& m, float& v, float g, const S& s) {
   const float d = __fsub_rn(g, m);
   m = s.w1 < 0.5f ? fmaf(s.w1, d, m) : fmaf(-d, __fsub_rn(1.f, s.w1), g);
   v = fmaf(__fmul_rn(s.c2, g), g, __fmul_rn(v, s.beta2));
+}
+
+__device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g, const AdamwScalars& s) {
+  p = __fmul_rn(p, s.decay);
+  adam_moments(m, v, g, s);
   const float den = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), s.sbc2), s.eps);
   p = fmaf(-s.step_size, __fdiv_rn(m, den), p);
 }

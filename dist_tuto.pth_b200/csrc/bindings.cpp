@@ -15,6 +15,7 @@
 #include "adamw.h"
 #include "executor.h"
 #include "batchnorm.h"
+#include "layerwise.h"
 #include "loader.h"
 
 #define B2_MAX_RANKS 8
@@ -81,6 +82,7 @@ int b2_adamw_flat_launch(float* p, float* m, float* v, float* g, size_t n, const
 int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
                             float* exp_avg_sq, size_t n_vec, const b2::AdamwScalars* s, float scale, int zero_grad, int rank,
                             int world, int max_blocks, cudaStream_t stream);
+int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
@@ -208,6 +210,84 @@ b2::AdamwScalars to_adamw(const std::vector<double>& v, const char* what) {
   b2::AdamwScalars a;
   a.decay = (float)v[0]; a.w1 = (float)v[1]; a.beta2 = (float)v[2]; a.c2 = (float)v[3];
   a.step_size = (float)v[4]; a.sbc2 = (float)v[5]; a.eps = (float)v[6];
+  return a;
+}
+
+// FlatLAMB / FlatLARS (csrc/layerwise.cu): the chunk table of one bucket from its tensors' offsets, sizes and adapt flags,
+// checked on the host and uploaded to `device`; returns (table, number of chunks).
+py::tuple layerwise_table(const std::vector<int64_t>& offsets, const std::vector<int64_t>& numels, const std::vector<bool>& adapt,
+                          int64_t n, torch::Device device) {
+  TORCH_CHECK(!offsets.empty() && offsets.size() == numels.size() && offsets.size() == adapt.size(),
+              "layerwise_table: one offset, size and adapt flag per tensor, at least one tensor");
+  TORCH_CHECK(offsets.size() < (size_t)INT32_MAX, "layerwise_table: too many tensors");
+  std::vector<int64_t> chunks, tens;
+  int64_t end = 0;
+  for (size_t t = 0; t < offsets.size(); ++t) {
+    const int64_t o = offsets[t], k = numels[t];
+    TORCH_CHECK(o % 4 == 0 && k >= 0 && o >= end && o + k <= n, "layerwise_table: tensor ", t, " at [", o, ", ", o + k,
+                ") must start at a multiple of 4 elements, after the previous tensor, inside the flat of ", n, " elements");
+    end = o + k;
+    tens.push_back((int64_t)chunks.size() / b2::kLwRow);
+    int64_t c = 0;
+    for (int64_t s = 0; s < k; s += b2::kLwChunk, ++c) {
+      chunks.push_back(o + s);
+      chunks.push_back(std::min<int64_t>(b2::kLwChunk, k - s));
+      chunks.push_back((int64_t)t);
+    }
+    tens.push_back(c);
+    tens.push_back(adapt[t] ? 1 : 0);
+  }
+  const int64_t n_chunks = (int64_t)chunks.size() / b2::kLwRow;
+  TORCH_CHECK(n_chunks >= 1 && n_chunks < INT32_MAX, "layerwise_table: the tensors hold no element, or too many chunks");
+  chunks.insert(chunks.end(), tens.begin(), tens.end());
+  auto host = torch::tensor(chunks, torch::dtype(torch::kInt64));
+  return py::make_tuple(host.to(device), n_chunks);
+}
+
+// The arguments every layer-wise launch shares: the table, the workspaces and clipping.  `states` are the state flats.
+b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, const std::vector<torch::Tensor*>& states,
+                          const torch::Tensor& table, int64_t n_chunks, torch::Tensor& partials, torch::Tensor& tickets,
+                          torch::Tensor& sums, torch::Tensor& ratios, bool zero_grad, const py::object& max_grad_norm,
+                          const c10::optional<torch::Tensor>& sqnorms, const c10::optional<torch::Tensor>& grad_norm_out) {
+  std::vector<const torch::Tensor*> flats = {&p, &g};
+  for (torch::Tensor* t : states) flats.push_back(t);
+  for (const torch::Tensor* t : flats) {
+    check_cuda_contig(*t, what);
+    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && t->device() == p.device() &&
+                (uintptr_t)t->data_ptr() % 16 == 0, what, ": parameters, gradients and state: 16-byte aligned fp32 of one size on one device");
+  }
+  for (const torch::Tensor* t : {&table, (const torch::Tensor*)&partials, (const torch::Tensor*)&tickets,
+                                 (const torch::Tensor*)&sums, (const torch::Tensor*)&ratios}) {
+    check_cuda_contig(*t, what);
+    TORCH_CHECK(t->device() == p.device(), what, ": the table and the workspaces live on the parameters' device");
+  }
+  const int64_t n_tensors = tickets.numel();
+  TORCH_CHECK(n_chunks >= 1 && n_chunks <= p.numel() && n_tensors >= 1 && table.scalar_type() == torch::kInt64 &&
+              table.numel() == (n_chunks + n_tensors) * b2::kLwRow, what, ": table: int64 of (chunks + tensors) * ", b2::kLwRow,
+              " entries from layerwise_table, tickets: one per tensor");
+  TORCH_CHECK(tickets.scalar_type() == torch::kInt32, what, ": tickets: int32 [tensors], zero before the first call");
+  TORCH_CHECK(partials.scalar_type() == torch::kFloat32 && partials.numel() == 2 * n_chunks && (uintptr_t)partials.data_ptr() % 8 == 0,
+              what, ": partials: fp32 [2 * chunks]");
+  TORCH_CHECK(sums.scalar_type() == torch::kFloat64 && sums.numel() == 2 * n_tensors, what, ": sums: fp64 [2 * tensors]");
+  TORCH_CHECK(ratios.scalar_type() == torch::kFloat32 && ratios.numel() == n_tensors, what, ": ratios: fp32 [tensors]");
+  b2::LwArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.p = p.data_ptr<float>(); a.g = g.data_ptr<float>();
+  a.m = states[0]->data_ptr<float>(); a.v = states.size() > 1 ? states[1]->data_ptr<float>() : nullptr;
+  a.n = (size_t)p.numel();
+  a.table = reinterpret_cast<const long long*>(table.data_ptr<int64_t>());
+  a.n_chunks = (int)n_chunks; a.n_tensors = (int)n_tensors;
+  a.partials = partials.data_ptr<float>(); a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int32_t>());
+  a.sums = sums.data_ptr<double>(); a.ratios = ratios.data_ptr<float>();
+  a.zero_grad = zero_grad ? 1 : 0;
+  a.max_norm = check_max_grad_norm(max_grad_norm, what);
+  if (a.max_norm > 0.f) {
+    TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+    a.sqnorms = sqnorms->data_ptr<double>();
+    a.n_buckets = (int)sqnorms->numel();
+  }
+  a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
   return a;
 }
 
@@ -870,6 +950,47 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                  (size_t)p.numel(), &sc, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
             "adamw_flat launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+  m.def("layerwise_chunk_elems", [] { return (int64_t)b2::kLwChunk; }, "the largest chunk of a layer-wise chunk table");
+  m.def("layerwise_table", &layerwise_table, py::arg("offsets"), py::arg("numels"), py::arg("adapt"), py::arg("n"),
+        py::arg("device"), "FlatLAMB / FlatLARS: (the chunk table of one bucket on `device`, its number of chunks)");
+  m.def("lamb_flat", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g, torch::Tensor table,
+                        int64_t n_chunks, torch::Tensor partials, torch::Tensor tickets, torch::Tensor sums, torch::Tensor ratios,
+                        std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
+                        c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    // FlatLAMB's update of one fp32 bucket (csrc/layerwise.cu).  scalars (fp64, each rounded once to fp32 here):
+    // (1 - beta1, beta2, 1 - beta2, sqrt(1 - beta2^t), eps, 1 / (1 - beta1^t), lr, weight_decay)
+    TORCH_CHECK(scalars.size() == 8, "lamb_flat: scalars: (1 - beta1, beta2, 1 - beta2, sqrt(bc2), eps, 1 / bc1, lr, "
+                "weight_decay), got ", scalars.size(), " values");
+    for (double x : scalars) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), "lamb_flat: scalars must be finite in fp32");
+    TORCH_CHECK((float)scalars[3] > 0.f && scalars[4] >= 0.0, "lamb_flat: sqrt(bc2) must be > 0 (update t >= 1) and eps >= 0");
+    b2::LwArgs a = layerwise_args("lamb_flat", p, g, {&exp_avg, &exp_avg_sq}, table, n_chunks, partials, tickets, sums, ratios,
+                                  zero_grad, max_grad_norm, sqnorms, grad_norm_out);
+    a.w1 = (float)scalars[0]; a.beta2 = (float)scalars[1]; a.c2 = (float)scalars[2]; a.sbc2 = (float)scalars[3];
+    a.eps = (float)scalars[4]; a.rbc1 = (float)scalars[5]; a.lr = (float)scalars[6]; a.wd = (float)scalars[7];
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_layerwise_launch(1, &a, cur_stream()), "lamb_flat launch");
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("table"), py::arg("n_chunks"),
+     py::arg("partials"), py::arg("tickets"), py::arg("sums"), py::arg("ratios"), py::arg("scalars"), py::arg("zero_grad"),
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+  m.def("lars_flat", [](torch::Tensor p, torch::Tensor momentum_buf, torch::Tensor g, torch::Tensor table, int64_t n_chunks,
+                        torch::Tensor partials, torch::Tensor tickets, torch::Tensor sums, torch::Tensor ratios, double lr,
+                        double momentum, double weight_decay, double trust_coefficient, double eps, bool nesterov, bool zero_grad,
+                        py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    // FlatLARS's update of one fp32 bucket (csrc/layerwise.cu)
+    check_sgd_options(weight_decay, nesterov, momentum, "lars_flat");
+    TORCH_CHECK(std::isfinite(lr) && std::isfinite(momentum) && std::isfinite(weight_decay) && trust_coefficient > 0.0 &&
+                std::isfinite(trust_coefficient) && eps >= 0.0 && std::isfinite(eps),
+                "lars_flat: lr, momentum and weight_decay finite, trust_coefficient > 0 and eps >= 0 finite");
+    b2::LwArgs a = layerwise_args("lars_flat", p, g, {&momentum_buf}, table, n_chunks, partials, tickets, sums, ratios, zero_grad,
+                                  max_grad_norm, sqnorms, grad_norm_out);
+    a.lr = (float)lr; a.mu = (float)momentum; a.wd = (float)weight_decay; a.nesterov = nesterov ? 1 : 0;
+    a.eta64 = trust_coefficient; a.wd64 = weight_decay; a.eps64 = eps;
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_layerwise_launch(0, &a, cur_stream()), "lars_flat launch");
+  }, py::arg("p"), py::arg("momentum_buffer"), py::arg("g"), py::arg("table"), py::arg("n_chunks"), py::arg("partials"),
+     py::arg("tickets"), py::arg("sums"), py::arg("ratios"), py::arg("lr"), py::arg("momentum"), py::arg("weight_decay"),
+     py::arg("trust_coefficient"), py::arg("eps"), py::arg("nesterov"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
   // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instance): as sharded_sgd, with this rank's
   // exp_avg / exp_avg_sq shards in place of the momentum shard.

@@ -19,6 +19,9 @@ separate update kernel runs.
 ``FlatAdamW`` is ``torch.optim.AdamW`` on the same flat layout: one ``adamw_flat_kernel`` launch per bucket (csrc/adamw.cu),
 and with ``sharded=True`` the AdamW instance of the same sharded kernel, with both moments sharded.  Both optimizers share
 the layout, the sharding, the exchange hooks and the step bookkeeping (``_FlatOptimizer``).
+
+``FlatLAMB`` and ``FlatLARS`` are the large-batch optimizers with a trust ratio per parameter tensor: per bucket two kernels
+(csrc/layerwise.cu) form every tensor's norms in a fixed order over a chunk table of the flat layout, then apply the update.
 """
 from __future__ import annotations
 
@@ -29,7 +32,8 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "FlatAdamW", "LRSchedule", "adamw_scalars", "check_sgd_options", "check_max_grad_norm"]
+__all__ = ["FlatSGD", "FlatAdamW", "FlatLAMB", "FlatLARS", "LRSchedule", "adamw_scalars", "lamb_scalars", "exclude_1d",
+           "check_sgd_options", "check_max_grad_norm"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -686,3 +690,215 @@ class FlatAdamW(_FlatOptimizer):
         if done and steps:
             self.steps = steps.pop()
         return done
+
+
+def exclude_1d(name: str, param: torch.Tensor) -> bool:      # noqa: ARG001 - the name is there for custom rules
+    """The default ``exclude_from_adaptation`` of :class:`FlatLAMB` and :class:`FlatLARS`: biases and norm weights
+    (``param.ndim <= 1``) get no weight decay and a trust ratio of 1, as in the usual LARS and BERT-LAMB recipes."""
+    return param.ndim <= 1
+
+
+def lamb_scalars(lr: float, betas: tuple, eps: float, weight_decay: float, t: int) -> list:
+    """The scalars of LAMB update ``t`` (1-based) that ``lamb_flat`` takes (csrc/layerwise.h), in fp64:
+    ``[1 - beta1, beta2, 1 - beta2, sqrt(1 - beta2^t), eps, 1 / (1 - beta1^t), lr, weight_decay]``.  The binding rounds
+    each once to fp32."""
+    b1, b2 = betas
+    return [1.0 - b1, b2, 1.0 - b2, (1.0 - b2 ** t) ** 0.5, eps, 1.0 / (1.0 - b1 ** t), lr, weight_decay]
+
+
+class _LayerwiseOptimizer(_FlatOptimizer):
+    """What :class:`FlatLAMB` and :class:`FlatLARS` share: the per-tensor adaptation flags, the trust ratios of the last
+    update, and on CUDA fp32 buckets the chunk table and the workspaces of the layer-wise kernels (csrc/layerwise.cu)."""
+
+    def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
+                 max_grad_norm: Optional[float], sharded: bool, exclude_from_adaptation):
+        if sharded:
+            raise ValueError(f"{type(self).__name__} cannot be sharded: the norms of the tensors that straddle shard boundaries "
+                             "would need an exchange between the ranks before any update; use sharded=False")
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, False)
+        exclude = exclude_1d if exclude_from_adaptation is None else exclude_from_adaptation
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        self.adapt: List[List[bool]] = [[not bool(exclude(names.get(id(p), ""), p)) for p in gb.params] for gb in self.buckets]
+        # the trust ratio of every tensor of a bucket (bucket order) in the last update; 1 before the first
+        self.ratio_flats = [torch.ones(len(gb.params), dtype=torch.float32, device=pf.device)
+                            for gb, pf in zip(self.buckets, self.param_flats)]
+        self._lw = []                    # per bucket on the kernel path: (table, chunks, partials, tickets, sums), else None
+        for gb, pf, adapt in zip(self.buckets, self.param_flats, self.adapt):
+            if not (pf.is_cuda and gb.flat.dtype == torch.float32):
+                self._lw.append(None)
+                continue
+            table, n_chunks = self._kernel().layerwise_table(gb.offsets, [p.numel() for p in gb.params], adapt, gb.numel,
+                                                             pf.device)
+            n_t = len(gb.params)
+            self._lw.append((table, n_chunks, torch.zeros(2 * n_chunks, dtype=torch.float32, device=pf.device),
+                             torch.zeros(n_t, dtype=torch.int32, device=pf.device),
+                             torch.zeros(2 * n_t, dtype=torch.float64, device=pf.device)))
+
+    def _tensors(self, k: int, flats: list):
+        """Per tensor of bucket ``k``: (index, adapted?, its 1-D slice of each flat in ``flats``)."""
+        gb = self.buckets[k]
+        for i, (p, o) in enumerate(zip(gb.params, gb.offsets)):
+            yield i, self.adapt[k][i], [f[o:o + p.numel()] for f in flats]
+
+    def trust_ratios(self, model: nn.Module) -> dict:
+        """``{parameter name: trust ratio of the last update}`` (1.0 before the first update and for excluded tensors).
+        Synchronises with the device."""
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        out = {}
+        for gb, r in zip(self.buckets, self.ratio_flats):
+            for p, x in zip(gb.params, r.tolist()):
+                if id(p) in names:
+                    out[names[id(p)]] = x
+        return out
+
+
+def _norm64(x: torch.Tensor) -> float:
+    return float(torch.linalg.vector_norm(x, dtype=torch.float64))
+
+
+class FlatLAMB(_LayerwiseOptimizer):
+    """LAMB (You et al. 2020, as Apex ``FusedLAMB`` with ``use_nvlamb=False``) over flat buffers, in the loop of
+    :class:`FlatSGD` (``backward(); average_gradients(model); opt.step()``).  Update t = ``steps + 1``:
+
+    * ``m``, ``v``: AdamW's moments;  ``u = (m / (sqrt(v) / sqrt(1 - beta2^t) + eps)) / (1 - beta1^t) + wd_l * p``;
+    * ``r_l = ||p_l|| / ||u_l||`` per parameter tensor (1 if the tensor is excluded or a norm is 0);  ``p -= (lr * r_l) * u``.
+
+    ``exclude_from_adaptation(name, param) -> bool`` picks the tensors with ``wd_l = 0`` and ``r_l = 1`` (default
+    :func:`exclude_1d`: biases and norm weights).  On CUDA fp32 buckets two kernels per bucket (csrc/layerwise.cu) form the
+    per-tensor norms in a fixed order (fp32 per thread and CTA, fp64 over the chunks of a tensor) and apply the update with
+    no host synchronisation; elsewhere (CPU tensors, bf16 buckets) torch ops run the same semantics on each tensor.
+    ``max_grad_norm`` clips first, as in :class:`FlatAdamW`.  :meth:`trust_ratios` gives the last update's ratios.  The
+    checkpoint forms are :class:`FlatAdamW`'s, so LAMB state loads into ``FlatAdamW`` and back.  ``sharded=True`` raises
+    ``ValueError``."""
+
+    def __init__(self, model: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6,
+                 weight_decay: float = 0.01, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, exclude_from_adaptation=None):
+        self.betas = check_adamw_options(lr, betas, eps, weight_decay)
+        self.lr, self.eps, self.weight_decay = float(lr), float(eps), float(weight_decay)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, exclude_from_adaptation)
+        self.exp_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+        self.exp_avg_sq_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+
+    def scalars(self) -> list:
+        """:func:`lamb_scalars` of the next update (t = ``steps`` + 1, lr = :meth:`lr_at`)."""
+        return lamb_scalars(self.lr_at(), self.betas, self.eps, self.weight_decay, self.steps + 1)
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        sc = self.scalars()
+        w1, b2, c2, sbc2, eps, rbc1, lr, wd = sc
+        for k, (gb, pf, mf, vf, kern) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats,
+                                                        self.exp_avg_sq_flats, kernel)):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern:
+                self._kernel().lamb_flat(pf, mf, vf, g, *self._lw[k], self.ratio_flats[k], sc, self.fused_zero, **clip)
+                continue
+            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            ratios = []
+            for _, adapt, (p, gt, m, v) in self._tensors(k, [pf, gf, mf, vf]):
+                m.lerp_(gt, w1)
+                v.mul_(b2).addcmul_(gt, gt, value=c2)
+                u = (m / (v.sqrt() / sbc2).add_(eps)).mul_(rbc1)
+                if adapt and wd != 0.0:
+                    u.add_(p, alpha=wd)
+                r = 1.0
+                if adapt:
+                    wn, un = _norm64(p), _norm64(u)
+                    if wn > 0.0 and un > 0.0:
+                        r = _f32(wn / un)
+                p.add_(u, alpha=-_f32(_f32(lr) * r))
+                ratios.append(r)
+            self.ratio_flats[k].copy_(torch.tensor(ratios, dtype=torch.float32))
+            if self.fused_zero:
+                g.zero_()
+
+    # ------------------------------------------------------------------ checkpointing: FlatAdamW's forms
+    state_dict = FlatAdamW.state_dict
+    load_state_dict = FlatAdamW.load_state_dict
+    named_state = FlatAdamW.named_state
+    load_named_state = FlatAdamW.load_named_state
+
+
+def check_lars_options(lr: float, momentum: float, weight_decay: float, trust_coefficient: float, eps: float,
+                       nesterov: bool) -> None:
+    """The hyper-parameter rules of :class:`FlatLARS`."""
+    if not float(lr) >= 0.0:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if not float(momentum) >= 0.0:
+        raise ValueError(f"Invalid momentum value: {momentum}")
+    if not (math.isfinite(float(trust_coefficient)) and float(trust_coefficient) > 0.0):
+        raise ValueError(f"trust_coefficient must be a finite value > 0, got {trust_coefficient}")
+    if not float(eps) >= 0.0:
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    check_sgd_options(momentum, weight_decay, nesterov)
+
+
+class FlatLARS(_LayerwiseOptimizer):
+    """LARS (You, Gitman, Ginsburg 2017) over flat buffers, in the loop of :class:`FlatSGD`:
+
+    * ``r_l = trust_coefficient * ||p_l|| / (||g_l|| + wd_l * ||p_l|| + eps)`` per parameter tensor (1 if the tensor is
+      excluded or a norm is 0);
+    * ``d = r_l * (g + wd_l * p)``, then ``torch.optim.SGD(momentum, dampening=0, nesterov, weight_decay=0)`` on ``d``.
+
+    ``exclude_from_adaptation(name, param) -> bool`` picks the tensors with ``wd_l = 0`` and ``r_l = 1`` (default
+    :func:`exclude_1d`).  On CUDA fp32 buckets two kernels per bucket (csrc/layerwise.cu) form the norms and apply
+    :class:`FlatSGD`'s fmaf sequence to ``d``; elsewhere the ratio is formed with torch ops and
+    ``torch.optim.SGD(foreach=False)``'s update runs on ``d``.  ``max_grad_norm`` clips ``g`` first.  The checkpoint forms
+    are :class:`FlatSGD`'s (``named_momentum``), so LARS momentum loads into ``FlatSGD`` and back.  ``sharded=True``
+    raises ``ValueError``."""
+
+    def __init__(self, model: nn.Module, lr: float = 0.1, momentum: float = 0.9, weight_decay: float = 1e-4,
+                 trust_coefficient: float = 1e-3, eps: float = 1e-8, nesterov: bool = False, zero_grad: bool = True,
+                 group=None, lr_schedule: Optional[LRSchedule] = None, max_grad_norm: Optional[float] = None,
+                 sharded: bool = False, exclude_from_adaptation=None):
+        check_lars_options(lr, momentum, weight_decay, trust_coefficient, eps, nesterov)
+        self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
+        self.trust_coefficient, self.eps, self.nesterov = float(trust_coefficient), float(eps), bool(nesterov)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, exclude_from_adaptation)
+        self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        from torch.optim.sgd import sgd
+
+        lr, wd, eta, eps = self.lr_at(), self.weight_decay, self.trust_coefficient, self.eps
+        for k, (gb, pf, mf, kern) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats, kernel)):
+            g = gb.flat[:gb.numel]
+            if kern:
+                self._kernel().lars_flat(pf, mf, g, *self._lw[k], self.ratio_flats[k], lr, self.momentum, wd, eta, eps,
+                                         self.nesterov, self.fused_zero, **clip)
+                continue
+            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            ratios = []
+            for _, adapt, (p, gt, m) in self._tensors(k, [pf, gf, mf]):
+                r = 1.0
+                if adapt:
+                    wn, gn = _norm64(p), _norm64(gt)
+                    if wn > 0.0 and gn > 0.0:
+                        r = _f32(eta * wn / (gn + wd * wn + eps))
+                d = gt.add(p, alpha=wd) if adapt and wd != 0.0 else gt.clone()
+                if r != 1.0:
+                    d.mul_(r)
+                sgd([p], [d], [m], foreach=False, weight_decay=0.0, momentum=self.momentum, lr=lr, dampening=0.0,
+                    nesterov=self.nesterov, maximize=False)
+                ratios.append(r)
+            self.ratio_flats[k].copy_(torch.tensor(ratios, dtype=torch.float32))
+            if self.fused_zero:
+                g.zero_()
+
+    # ------------------------------------------------------------------ checkpointing: FlatSGD's forms
+    def state_dict(self) -> dict:
+        """:meth:`FlatSGD.state_dict` plus ``trust_coefficient`` and ``eps``; loads into ``FlatSGD`` as well."""
+        sd = FlatSGD.state_dict(self)
+        sd.update(trust_coefficient=self.trust_coefficient, eps=self.eps)
+        return sd
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict`; a ``FlatSGD`` state_dict loads too (the LARS hyper-parameters stay)."""
+        check_lars_options(sd["lr"], sd["momentum"], sd["weight_decay"], sd.get("trust_coefficient", self.trust_coefficient),
+                           sd.get("eps", self.eps), bool(sd.get("nesterov", False)))
+        FlatSGD.load_state_dict(self, sd)
+        self.trust_coefficient = float(sd.get("trust_coefficient", self.trust_coefficient))
+        self.eps = float(sd.get("eps", self.eps))
+
+    named_momentum = FlatSGD.named_momentum
+    load_named_momentum = FlatSGD.load_named_momentum

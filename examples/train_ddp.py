@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` (or ``FlatAdamW``) in the tutorial's loop, on
-synthetic data.
+"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` (or ``FlatAdamW``, ``FlatLAMB``, ``FlatLARS``) in
+the tutorial's loop, on synthetic data.
 
     python examples/train_ddp.py                                  # CPU, gloo, world 2
     python examples/train_ddp.py --sharded-optimizer              # momentum sharded over the ranks (ZeRO stage 1)
     python examples/train_ddp.py --backend b200 --size 8 --sharded-optimizer   # one process per GPU: per bucket ONE kernel
                                                                   # reduces, updates the owned slice and gathers the parameters
     python examples/train_ddp.py --optimizer adamw [--sharded-optimizer]   # FlatAdamW; sharded: both moments 1/size per rank
+    python examples/train_ddp.py --optimizer lamb                 # FlatLAMB / FlatLARS (--optimizer lars): per-tensor trust
+                                                                  # ratios for large global batches
 
 The loop is ``backward(); average_gradients(model); optimizer.step()`` either way.  With ``--sharded-optimizer`` the update
 happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
@@ -46,6 +48,10 @@ def run(rank, size):
     model = dist.DistributedDataParallel(SmallConvNet().to(dev), bucket_cap_bytes=64 << 10)
     if CFG["optimizer"] == "adamw":
         optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"])
+    elif CFG["optimizer"] == "lamb":
+        optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2)
+    elif CFG["optimizer"] == "lars":
+        optimizer = dist.FlatLARS(model, lr=2.0, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-2)
     else:
         optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"])
     loss = None
@@ -59,7 +65,7 @@ def run(rank, size):
         optimizer.step()
     total = loss.detach().clone()
     dist.all_reduce(total)
-    if CFG["optimizer"] == "adamw":
+    if CFG["optimizer"] in ("adamw", "lamb"):
         state = f"AdamW moment elements on this rank {sum(m.numel() for m in optimizer.exp_avg_flats + optimizer.exp_avg_sq_flats)}"
     else:
         state = f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}"
@@ -74,8 +80,8 @@ if __name__ == "__main__":
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--sharded-optimizer", action="store_true",
                     help="sharded=True: each rank keeps the optimizer state of, and updates, 1/size of every bucket")
-    ap.add_argument("--optimizer", choices=("sgd", "adamw"), default="sgd",
-                    help="FlatSGD (momentum SGD, the default) or FlatAdamW")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb", "lars"), default="sgd",
+                    help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatLAMB or FlatLARS (the last two unsharded)")
     a = ap.parse_args()
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
                                                 optimizer=a.optimizer))
