@@ -2,6 +2,7 @@
 // moments and averaged gradients, one launch per bucket, streaming the four arrays once and re-zeroing the gradients in the
 // same pass.  The per-element sequence is adamw_elem (adamw_device.cuh).
 #include "adamw_device.cuh"
+#include "param_groups.cuh"
 #include "sgd_device.cuh"
 
 namespace b2 {
@@ -50,6 +51,59 @@ __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, 
   }
 }
 
+// adamw_flat_kernel with parameter groups: parameter vector i takes decay and step_size of group map[i] (param_groups.cuh),
+// the other five scalars are shared; the tail (< 4 elements) shares the map entry of its vector.
+template <bool kClip>
+__global__ void __launch_bounds__(256) adamw_flat_grouped_kernel(float* __restrict__ p, float* __restrict__ m,
+                                                                 float* __restrict__ v, float* __restrict__ g, size_t n,
+                                                                 const uint8_t* __restrict__ map, AdamwScalars s, AdamwGroups gs,
+                                                                 int zero_grad, const double* __restrict__ sqnorms, int n_buckets,
+                                                                 float max_norm, float* grad_norm_out) {
+  float c = 1.f;
+  if constexpr (kClip) {
+    __shared__ float s_coef;
+    if (threadIdx.x == 0) {
+      double q = 0.0;
+      for (int k = 0; k < n_buckets; ++k) q += sqnorms[k];
+      const float nrm = __double2float_rn(__dsqrt_rn(q));
+      s_coef = clip_coef(nrm, max_norm);
+      if (blockIdx.x == 0 && grad_norm_out != nullptr) *grad_norm_out = nrm;
+    }
+    __syncthreads();
+    c = s_coef;
+  }
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    const int gid = map[i];
+    AdamwScalars sg = s;
+    sg.decay = gs.decay[gid];
+    sg.step_size = gs.step_size[gid];
+    float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 pv = reinterpret_cast<float4*>(p)[i];
+    float4 mv = reinterpret_cast<float4*>(m)[i];
+    float4 vv = reinterpret_cast<float4*>(v)[i];
+    if constexpr (kClip) {
+      gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
+    }
+    adamw4(pv, mv, vv, gv, sg);
+    reinterpret_cast<float4*>(p)[i] = pv;
+    reinterpret_cast<float4*>(m)[i] = mv;
+    reinterpret_cast<float4*>(v)[i] = vv;
+    if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (i < n - n4 * 4) {                        // tail (< 4 elements): threads 0..2 of CTA 0, one element each
+    const size_t t = n4 * 4 + i;
+    const int gid = map[n4];
+    AdamwScalars sg = s;
+    sg.decay = gs.decay[gid];
+    sg.step_size = gs.step_size[gid];
+    const float gt = kClip ? __fmul_rn(g[t], c) : g[t];
+    adamw_elem(p[t], m[t], v[t], gt, sg);
+    if (zero_grad) g[t] = 0.f;
+  }
+}
+
 }  // namespace b2
 
 extern "C" {
@@ -67,6 +121,28 @@ int b2_adamw_flat_launch(float* p, float* m, float* v, float* g, size_t n, const
                                                              grad_norm_out);
   } else {
     b2::adamw_flat_kernel<false><<<blocks, 256, 0, stream>>>(p, m, v, g, n, *s, zero_grad, nullptr, 0, 0.f, nullptr);
+  }
+  return (int)cudaGetLastError();
+}
+
+// The same update with parameter groups: `map` holds one group id per parameter vector (ceil(n / 4) ids), `gs` the per-group
+// scalars of n_groups groups.  Also cudaErrorInvalidValue, without a launch, for a null map or n_groups outside 1..64; the ids
+// themselves are checked on the host where the map is built.
+int b2_adamw_flat_grouped_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::AdamwScalars* s,
+                                 const b2::AdamwGroups* gs, int n_groups, int zero_grad, float max_norm, const double* sqnorms,
+                                 int n_buckets, float* grad_norm_out, cudaStream_t stream) {
+  if (p == nullptr || m == nullptr || v == nullptr || g == nullptr || s == nullptr || map == nullptr || gs == nullptr ||
+      n_groups < 1 || n_groups > b2::kMaxGroups)
+    return (int)cudaErrorInvalidValue;
+  const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
+  const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  if (max_norm > 0.f) {
+    if (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY)) return (int)cudaErrorInvalidValue;
+    b2::adamw_flat_grouped_kernel<true><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, *s, *gs, zero_grad, sqnorms, n_buckets,
+                                                                     max_norm, grad_norm_out);
+  } else {
+    b2::adamw_flat_grouped_kernel<false><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, *s, *gs, zero_grad, nullptr, 0, 0.f,
+                                                                      nullptr);
   }
   return (int)cudaGetLastError();
 }

@@ -17,6 +17,7 @@
 #include "batchnorm.h"
 #include "layerwise.h"
 #include "loader.h"
+#include "param_groups.h"
 
 #define B2_MAX_RANKS 8
 struct PeerPtrs { void* p[B2_MAX_RANKS]; };
@@ -82,6 +83,20 @@ int b2_adamw_flat_launch(float* p, float* m, float* v, float* g, size_t n, const
 int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
                             float* exp_avg_sq, size_t n_vec, const b2::AdamwScalars* s, float scale, int zero_grad, int rank,
                             int world, int max_blocks, cudaStream_t stream);
+int b2_sgd_flat_grouped_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::SgdGroups* gs,
+                               int n_groups, float mu, int zero_grad, int nesterov, float max_norm, const double* sqnorms,
+                               int n_buckets, float* grad_norm_out, cudaStream_t stream);
+int b2_adamw_flat_grouped_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::AdamwScalars* s,
+                                 const b2::AdamwGroups* gs, int n_groups, int zero_grad, float max_norm, const double* sqnorms,
+                                 int n_buckets, float* grad_norm_out, cudaStream_t stream);
+int b2_sharded_sgd_grouped_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig,
+                                  float* momentum, const uint8_t* map, const b2::SgdGroups* gs, int n_groups, size_t n_vec, float mu,
+                                  int nesterov, float scale, int zero_grad, int rank, int world, int max_blocks,
+                                  cudaStream_t stream);
+int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig,
+                                    float* exp_avg, float* exp_avg_sq, const uint8_t* map, const b2::AdamwScalars* s,
+                                    const b2::AdamwGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank,
+                                    int world, int max_blocks, cudaStream_t stream);
 int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
@@ -211,6 +226,22 @@ b2::AdamwScalars to_adamw(const std::vector<double>& v, const char* what) {
   a.decay = (float)v[0]; a.w1 = (float)v[1]; a.beta2 = (float)v[2]; a.c2 = (float)v[3];
   a.step_size = (float)v[4]; a.sbc2 = (float)v[5]; a.eps = (float)v[6];
   return a;
+}
+
+// Parameter groups (csrc/param_groups.h): the group map of `n_ids` parameter vectors (uint8 CUDA, 1..64 groups) and two
+// per-group scalar lists of one length, rounded once to fp32.  Returns the number of groups.
+int check_groups(const torch::Tensor& map, int64_t n_ids, const std::vector<double>& a, const std::vector<double>& b,
+                 float* out_a, float* out_b, const char* what) {
+  TORCH_CHECK(map.is_cuda() && map.is_contiguous() && map.scalar_type() == torch::kUInt8 && map.numel() >= n_ids, what,
+              ": group_map: contiguous uint8 CUDA of at least ", n_ids, " ids (one per fp32 parameter vector)");
+  TORCH_CHECK(!a.empty() && a.size() <= (size_t)b2::kMaxGroups && a.size() == b.size(), what, ": 1..", b2::kMaxGroups,
+              " groups with one value of each per-group scalar, got ", a.size(), " and ", b.size());
+  for (size_t i = 0; i < a.size(); ++i) {
+    TORCH_CHECK(std::isfinite((float)a[i]) && std::isfinite((float)b[i]), what, ": per-group scalars must be finite in fp32");
+    out_a[i] = (float)a[i];
+    out_b[i] = (float)b[i];
+  }
+  return (int)a.size();
 }
 
 // FlatLAMB / FlatLARS (csrc/layerwise.cu): the chunk table of one bucket from its tensors' offsets, sizes and adapt flags,
@@ -951,6 +982,74 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
             "adamw_flat launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+  m.def("max_param_groups", [] { return b2::kMaxGroups; }, "the most parameter groups the grouped optimizer kernels take");
+  m.def("sgd_flat_grouped", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, torch::Tensor group_map, std::vector<double> lrs,
+                               std::vector<double> weight_decays, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
+                               c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    // sgd_flat with parameter groups (csrc/sgd.cu): parameter vector i takes lrs / weight_decays of group group_map[i]
+    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_grouped: nesterov needs a nonzero momentum");
+    for (double wd : weight_decays) TORCH_CHECK(wd >= 0.0, "sgd_flat_grouped: weight_decay must be >= 0, got ", wd);
+    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat_grouped");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "sgd_flat_grouped: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat_grouped");
+    check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
+    TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32,
+                "sgd_flat_grouped: p, m and g: fp32");
+    TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel(), "sgd_flat_grouped: p, m and g: one size");
+    TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0,
+                "sgd_flat_grouped: 16-byte aligned buffers");
+    b2::SgdGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    const int n_groups = check_groups(group_map, (p.numel() + 3) / 4, lrs, weight_decays, gs.lr, gs.wd, "sgd_flat_grouped");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_sgd_flat_grouped_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(),
+                                       group_map.data_ptr<uint8_t>(), &gs, n_groups, (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0,
+                                       max_norm, sq, n_buckets, gn, cur_stream()),
+            "sgd_flat_grouped launch");
+  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"),
+     py::arg("zero_grad"), py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none());
+  m.def("adamw_flat_grouped", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                                 torch::Tensor group_map, std::vector<double> scalars, std::vector<double> decays,
+                                 std::vector<double> step_sizes, bool zero_grad, py::object max_grad_norm,
+                                 c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    // adamw_flat with parameter groups (csrc/adamw.cu): `scalars` as adamw_flat's (their decay and step_size are not used),
+    // decays / step_sizes: 1 - lr_g*wd_g and lr_g / (1 - beta1^t) of every group, fp64, each rounded once to fp32 here
+    const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat_grouped");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat_grouped");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "adamw_flat_grouped: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat_grouped");
+    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
+      check_cuda_contig(*t, "adamw_flat_grouped: p, exp_avg, exp_avg_sq and g");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "adamw_flat_grouped: p, exp_avg, exp_avg_sq and g: 16-byte aligned fp32 of one size");
+    }
+    b2::AdamwGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    const int n_groups = check_groups(group_map, (p.numel() + 3) / 4, decays, step_sizes, gs.decay, gs.step_size,
+                                      "adamw_flat_grouped");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_adamw_flat_grouped_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
+                                         g.data_ptr<float>(), (size_t)p.numel(), group_map.data_ptr<uint8_t>(), &sc, &gs, n_groups,
+                                         zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+            "adamw_flat_grouped launch");
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("scalars"),
+     py::arg("decays"), py::arg("step_sizes"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
+     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
   m.def("layerwise_chunk_elems", [] { return (int64_t)b2::kLwChunk; }, "the largest chunk of a layer-wise chunk table");
   m.def("layerwise_table", &layerwise_table, py::arg("offsets"), py::arg("numels"), py::arg("adapt"), py::arg("n"),
         py::arg("device"), "FlatLAMB / FlatLARS: (the chunk table of one bucket on `device`, its number of chunks)");
@@ -1050,6 +1149,69 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("n_vec"), py::arg("lr"),
      py::arg("mu"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
      py::arg("world"), py::arg("max_blocks") = 0);
+  // sharded_sgd / sharded_adamw with parameter groups: group_map holds this rank's ids, one per fp32 parameter vector of its
+  // slice (n_vec / world x 1, x 2 with bf16)
+  m.def("sharded_sgd_grouped", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                  std::vector<unsigned long long> sigs, torch::Tensor momentum, torch::Tensor group_map, size_t n_vec,
+                                  std::vector<double> lrs, std::vector<double> weight_decays, double mu, bool nesterov, double scale,
+                                  bool zero_grad, int rank, int world, int max_blocks) {
+    check_world(rank, world, "sharded_sgd_grouped");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_sgd_grouped: one gradient bucket, one parameter flat and one signal pad per rank");
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd_grouped: n_vec must be a multiple of world, got ", n_vec, " for ", world);
+    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd_grouped: nesterov needs a nonzero momentum");
+    for (double wd : weight_decays) TORCH_CHECK(wd >= 0.0, "sharded_sgd_grouped: weight_decay must be >= 0, got ", wd);
+    check_cuda_contig(momentum, "momentum");
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
+                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd_grouped: momentum: 16-byte aligned fp32 of at least ", shard,
+                " elements (this rank's slice)");
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd_grouped: null or misaligned per-rank pointer");
+    b2::SgdGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    const int n_groups = check_groups(group_map, (int64_t)(shard / 4), lrs, weight_decays, gs.lr, gs.wd, "sharded_sgd_grouped");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(momentum.device());
+    ck_cuda(b2_sharded_sgd_grouped_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), group_map.data_ptr<uint8_t>(), &gs,
+                                          n_groups, n_vec, (float)mu, nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world,
+                                          max_blocks, cur_stream()),
+            "sharded_sgd_grouped launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("group_map"),
+     py::arg("n_vec"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"), py::arg("nesterov"), py::arg("scale"),
+     py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  m.def("sharded_adamw_grouped", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                    std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
+                                    torch::Tensor group_map, size_t n_vec, std::vector<double> scalars, std::vector<double> decays,
+                                    std::vector<double> step_sizes, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    check_world(rank, world, "sharded_adamw_grouped");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_adamw_grouped: one gradient bucket, one parameter flat and one signal pad per rank");
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw_grouped: n_vec must be a multiple of world, got ", n_vec, " for ", world);
+    const b2::AdamwScalars sc = to_adamw(scalars, "sharded_adamw_grouped");
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
+      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "sharded_adamw_grouped: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements");
+    }
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw_grouped: null or misaligned per-rank pointer");
+    b2::AdamwGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    const int n_groups = check_groups(group_map, (int64_t)(shard / 4), decays, step_sizes, gs.decay, gs.step_size,
+                                      "sharded_adamw_grouped");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(exp_avg.device());
+    ck_cuda(b2_sharded_adamw_grouped_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
+                                            group_map.data_ptr<uint8_t>(), &sc, &gs, n_groups, n_vec, (float)scale, zero_grad ? 1 : 0,
+                                            rank, world, max_blocks, cur_stream()),
+            "sharded_adamw_grouped launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+     py::arg("group_map"), py::arg("n_vec"), py::arg("scalars"), py::arg("decays"), py::arg("step_sizes"), py::arg("scale"),
+     py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });

@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "sgd_device.cuh"
 #include "convnet_reduce.cuh"
+#include "param_groups.cuh"
 
 namespace b2 {
 
@@ -374,6 +375,55 @@ __global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ 
   }
 }
 
+// sgd_flat_kernel / sgd_flat_clip_kernel with parameter groups: parameter vector i takes the lr and weight decay of group
+// map[i] (param_groups.cuh); the tail (< 4 elements) shares the map entry of its vector.  The per-element sequence is the
+// ungrouped kernels' (sgd4), so running those on each tensor's segment with its group's scalars gives the same bits.
+template <bool kNesterov, bool kClip>
+__global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict__ p, float* __restrict__ m,
+                                                               const float* __restrict__ g, size_t n,
+                                                               const uint8_t* __restrict__ map, SgdGroups gs, float mu,
+                                                               int zero_grad, float* gw, const double* __restrict__ sqnorms,
+                                                               int n_buckets, float max_norm, float* grad_norm_out) {
+  float c = 1.f;
+  if constexpr (kClip) {
+    __shared__ float s_coef;
+    if (threadIdx.x == 0) {
+      double s = 0.0;
+      for (int k = 0; k < n_buckets; ++k) s += sqnorms[k];
+      const float nrm = __double2float_rn(__dsqrt_rn(s));
+      s_coef = clip_coef(nrm, max_norm);
+      if (blockIdx.x == 0 && grad_norm_out != nullptr) *grad_norm_out = nrm;
+    }
+    __syncthreads();
+    c = s_coef;
+  }
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    const int gid = map[i];
+    float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 pv = reinterpret_cast<float4*>(p)[i];
+    float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kClip) {
+      gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
+    }
+    sgd4<kNesterov>(pv, mv, gv, gs.lr[gid], mu, gs.wd[gid]);
+    reinterpret_cast<float4*>(p)[i] = pv;
+    reinterpret_cast<float4*>(m)[i] = mv;
+    if (zero_grad) reinterpret_cast<float4*>(gw)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (i == 0 && n4 * 4 < n) {
+    const int gid = map[n4];
+    const float lr = gs.lr[gid], wd = gs.wd[gid];
+    for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
+      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(g[t], c) : g[t]);
+      m[t] = fmaf(mu, m[t], gt);
+      p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
+      if (zero_grad) gw[t] = 0.f;
+    }
+  }
+}
+
 // out[i] = the lr the optimizer kernels apply when the step counter reads steps[i] (tests tie it to ops/optim.LRSchedule)
 __global__ void __launch_bounds__(256) lr_schedule_eval_kernel(LrSchedule s, float base, const long long* __restrict__ steps,
                                                                float* __restrict__ out, long long n) {
@@ -562,6 +612,36 @@ int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, f
     b2::sgd_flat_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
   else
     b2::sgd_flat_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
+  return (int)cudaGetLastError();
+}
+
+// sgd_flat with parameter groups: `map` holds one group id per parameter vector (ceil(n / 4) ids) and `gs` the scalars of
+// n_groups groups.  cudaErrorInvalidValue, without a launch, for a null pointer, n_groups outside 1..64 or clipping without
+// sqnorms; the ids themselves are checked on the host where the map is built.
+int b2_sgd_flat_grouped_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::SgdGroups* gs,
+                               int n_groups, float mu, int zero_grad, int nesterov, float max_norm, const double* sqnorms,
+                               int n_buckets, float* grad_norm_out, cudaStream_t stream) {
+  if (p == nullptr || m == nullptr || g == nullptr || map == nullptr || gs == nullptr || n_groups < 1 ||
+      n_groups > b2::kMaxGroups)
+    return (int)cudaErrorInvalidValue;
+  const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
+  const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  float* gw = const_cast<float*>(g);
+  if (max_norm > 0.f) {
+    if (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY)) return (int)cudaErrorInvalidValue;
+    if (nesterov)
+      b2::sgd_flat_grouped_kernel<true, true><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, sqnorms,
+                                                                          n_buckets, max_norm, grad_norm_out);
+    else
+      b2::sgd_flat_grouped_kernel<false, true><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, sqnorms,
+                                                                           n_buckets, max_norm, grad_norm_out);
+  } else if (nesterov) {
+    b2::sgd_flat_grouped_kernel<true, false><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, nullptr, 0,
+                                                                         0.f, nullptr);
+  } else {
+    b2::sgd_flat_grouped_kernel<false, false><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, nullptr, 0,
+                                                                          0.f, nullptr);
+  }
   return (int)cudaGetLastError();
 }
 

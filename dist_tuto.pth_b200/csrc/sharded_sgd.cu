@@ -26,9 +26,13 @@
 // ShardedAdamwUpdate (AdamW, FlatAdamW: adamw_elem of adamw_device.cuh on the slice's first and second moment shards).  An
 // update type names its argument struct, which carries the fields the skeleton reads (grads, params, sig, n_vec, scale, rank,
 // world, zero_grad), loads its optimizer state for a parameter vector, applies the update and stores the state back.
+//
+// With parameter groups, ShardedSgdGroupedUpdate and ShardedAdamwGroupedUpdate load a group id next to the state of each
+// parameter vector and take that group's scalars; the skeleton and the other instances are unchanged.
 #include <cstring>
 #include "adamw_device.cuh"
 #include "common.cuh"
+#include "param_groups.cuh"
 
 namespace b2 {
 
@@ -57,17 +61,33 @@ struct ShardedAdamwArgs {
   int rank, world, zero_grad;
 };
 
-// momentum SGD on four elements, the fmaf sequence of sgd_flat_kernel
-template <bool kNesterov>
-__device__ __forceinline__ void sgd4(float4& p, float4& m, float4 g, float lr, float mu, float wd) {
-  g.x = fmaf(wd, p.x, g.x); g.y = fmaf(wd, p.y, g.y); g.z = fmaf(wd, p.z, g.z); g.w = fmaf(wd, p.w, g.w);
-  m.x = fmaf(mu, m.x, g.x); m.y = fmaf(mu, m.y, g.y); m.z = fmaf(mu, m.z, g.z); m.w = fmaf(mu, m.w, g.w);
-  float4 d = m;
-  if (kNesterov) {
-    d.x = fmaf(mu, m.x, g.x); d.y = fmaf(mu, m.y, g.y); d.z = fmaf(mu, m.z, g.z); d.w = fmaf(mu, m.w, g.w);
-  }
-  p.x = fmaf(-lr, d.x, p.x); p.y = fmaf(-lr, d.y, p.y); p.z = fmaf(-lr, d.z, p.z); p.w = fmaf(-lr, d.w, p.w);
-}
+// With parameter groups (FlatSGD / FlatAdamW param_groups): the same fields, plus this rank's group map (one uint8 id per
+// fp32 parameter vector of its slice, kP x slice ids) and the per-group scalars (param_groups.cuh).
+struct ShardedSgdGroupedArgs {
+  PeerPtrs grads;
+  PeerPtrs params;
+  SignalPads sig;
+  float* momentum;
+  const uint8_t* map;
+  size_t n_vec;
+  float mu, scale;
+  int rank, world, zero_grad;
+  SgdGroups gs;
+};
+
+struct ShardedAdamwGroupedArgs {
+  PeerPtrs grads;
+  PeerPtrs params;
+  SignalPads sig;
+  float* exp_avg;
+  float* exp_avg_sq;
+  const uint8_t* map;
+  size_t n_vec;
+  AdamwScalars s;         // decay and step_size unused: they come from the vector's group
+  float scale;
+  int rank, world, zero_grad;
+  AdamwGroups gs;
+};
 
 // The per-vector updates of sharded_step_kernel.  q indexes the fp32 state vector within this rank's shard.
 template <bool kNesterov>
@@ -89,6 +109,45 @@ struct ShardedAdamwUpdate {
     v = reinterpret_cast<float4*>(a.exp_avg_sq)[q];
   }
   __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) { adamw4(p, m, v, g, a.s); }
+  __device__ __forceinline__ void store(const Args& a, size_t q) {
+    reinterpret_cast<float4*>(a.exp_avg)[q] = m;
+    reinterpret_cast<float4*>(a.exp_avg_sq)[q] = v;
+  }
+};
+
+// Grouped instances: the group id of the vector is loaded next to its state, and the update takes that group's scalars.
+template <bool kNesterov>
+struct ShardedSgdGroupedUpdate {
+  using Args = ShardedSgdGroupedArgs;
+  static constexpr int kUnroll = kShardUnroll;
+  float4 m;
+  int gid;
+  __device__ __forceinline__ void load(const Args& a, size_t q) {
+    m = reinterpret_cast<float4*>(a.momentum)[q];
+    gid = a.map[q];
+  }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) {
+    sgd4<kNesterov>(p, m, g, a.gs.lr[gid], a.mu, a.gs.wd[gid]);
+  }
+  __device__ __forceinline__ void store(const Args& a, size_t q) { reinterpret_cast<float4*>(a.momentum)[q] = m; }
+};
+
+struct ShardedAdamwGroupedUpdate {
+  using Args = ShardedAdamwGroupedArgs;
+  static constexpr int kUnroll = 1;
+  float4 m, v;
+  int gid;
+  __device__ __forceinline__ void load(const Args& a, size_t q) {
+    m = reinterpret_cast<float4*>(a.exp_avg)[q];
+    v = reinterpret_cast<float4*>(a.exp_avg_sq)[q];
+    gid = a.map[q];
+  }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) {
+    AdamwScalars s = a.s;
+    s.decay = a.gs.decay[gid];
+    s.step_size = a.gs.step_size[gid];
+    adamw4(p, m, v, g, s);
+  }
   __device__ __forceinline__ void store(const Args& a, size_t q) {
     reinterpret_cast<float4*>(a.exp_avg)[q] = m;
     reinterpret_cast<float4*>(a.exp_avg_sq)[q] = v;
@@ -243,6 +302,50 @@ int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* par
   using namespace b2;
   if (bf16) sharded_step_kernel<true, ShardedAdamwUpdate><<<grid, kShardThreads, 0, stream>>>(a);
   else sharded_step_kernel<false, ShardedAdamwUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// The grouped steps: `map` holds this rank's group ids, one per fp32 parameter vector of its slice (n_vec / world x 1 (x 2)),
+// and `gs` the scalars of n_groups groups.  Also cudaErrorInvalidValue, without a launch, for a null map or n_groups outside
+// 1..64; the ids themselves are checked on the host where the map is built.
+int b2_sharded_sgd_grouped_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig,
+                                  float* momentum, const uint8_t* map, const b2::SgdGroups* gs, int n_groups, size_t n_vec, float mu,
+                                  int nesterov, float scale, int zero_grad, int rank, int world, int max_blocks,
+                                  cudaStream_t stream) {
+  if (momentum == nullptr || map == nullptr || gs == nullptr || n_groups < 1 || n_groups > b2::kMaxGroups ||
+      !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  b2::ShardedSgdGroupedArgs a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.momentum = momentum; a.map = map; a.n_vec = n_vec;
+  a.mu = mu; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.gs = *gs;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  using namespace b2;
+  if (bf16) {
+    if (nesterov) sharded_step_kernel<true, ShardedSgdGroupedUpdate<true>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<true, ShardedSgdGroupedUpdate<false>><<<grid, kShardThreads, 0, stream>>>(a);
+  } else {
+    if (nesterov) sharded_step_kernel<false, ShardedSgdGroupedUpdate<true>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, ShardedSgdGroupedUpdate<false>><<<grid, kShardThreads, 0, stream>>>(a);
+  }
+  return (int)cudaGetLastError();
+}
+
+int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig,
+                                    float* exp_avg, float* exp_avg_sq, const uint8_t* map, const b2::AdamwScalars* s,
+                                    const b2::AdamwGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank,
+                                    int world, int max_blocks, cudaStream_t stream) {
+  if (exp_avg == nullptr || exp_avg_sq == nullptr || map == nullptr || s == nullptr || gs == nullptr || n_groups < 1 ||
+      n_groups > b2::kMaxGroups || !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  b2::ShardedAdamwGroupedArgs a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.map = map;
+  a.n_vec = n_vec; a.s = *s; a.gs = *gs; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  using namespace b2;
+  if (bf16) sharded_step_kernel<true, ShardedAdamwGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  else sharded_step_kernel<false, ShardedAdamwGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 

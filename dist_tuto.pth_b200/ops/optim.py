@@ -20,6 +20,9 @@ separate update kernel runs.
 and with ``sharded=True`` the AdamW instance of the same sharded kernel, with both moments sharded.  Both optimizers share
 the layout, the sharding, the exchange hooks and the step bookkeeping (``_FlatOptimizer``).
 
+``FlatSGD`` and ``FlatAdamW`` take torch-style ``param_groups`` (per-group lr and weight decay): the same launches with a
+per-vector group map and the groups' scalars in the kernel arguments.
+
 ``FlatLAMB`` and ``FlatLARS`` are the large-batch optimizers with a trust ratio per parameter tensor: per bucket two kernels
 (csrc/layerwise.cu) form every tensor's norms in a fixed order over a chunk table of the flat layout, then apply the update.
 """
@@ -33,7 +36,7 @@ import torch
 import torch.nn as nn
 
 __all__ = ["FlatSGD", "FlatAdamW", "FlatLAMB", "FlatLARS", "LRSchedule", "adamw_scalars", "lamb_scalars", "exclude_1d",
-           "check_sgd_options", "check_max_grad_norm"]
+           "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -185,6 +188,62 @@ def check_max_grad_norm(max_grad_norm) -> Optional[float]:
     return c
 
 
+MAX_PARAM_GROUPS = 64                                        # csrc/param_groups.h: kMaxGroups
+_GROUP_KEYS = ("params", "lr", "weight_decay")
+
+
+def _check_param_groups(name: str, model: nn.Module, param_groups, lr: float, weight_decay: float, check) -> list:
+    """``param_groups`` of :class:`FlatSGD` / :class:`FlatAdamW` checked before anything is allocated or laid out: a list of
+    ``{"params", "lr", "weight_decay"}`` dicts, absent keys taking the constructor's values and ``check(lr, weight_decay)``
+    applied to every group.  Raises ``ValueError`` for a parameter that is in no bucket of ``model`` or in two groups, an
+    empty ``"params"``, any other key, a bad value, more than :data:`MAX_PARAM_GROUPS` groups (the default group of the
+    parameters named in no group included), or a CUDA bucket with a tensor at an offset that is not a multiple of 4."""
+    from ..parallel.ddp import DistributedDataParallel, flatten_params
+
+    if isinstance(param_groups, dict) or not isinstance(param_groups, (list, tuple)):
+        raise ValueError(f"{name}: param_groups must be a list of dicts, got {type(param_groups).__name__}")
+    engine = model if isinstance(model, DistributedDataParallel) else getattr(model, "_ddp_engine", None)
+    buckets = engine.buckets if engine is not None else [gb for gb in [getattr(model, "_grad_bucket", None)] if gb is not None]
+    laid = [p for gb in buckets for p in gb.params] if buckets else flatten_params(model)
+    known = {id(p) for p in laid}
+    seen, out = set(), []
+    for i, g in enumerate(param_groups):
+        if not isinstance(g, dict):
+            raise ValueError(f"{name}: param_groups[{i}] must be a dict, got {type(g).__name__}")
+        for key in g:
+            if key not in _GROUP_KEYS:
+                raise ValueError(f"{name}: param_groups[{i}] has the key {key!r}; a group sets only 'lr' and 'weight_decay' "
+                                 "(every other hyper-parameter is the optimizer's)")
+        if "params" not in g:
+            raise ValueError(f"{name}: param_groups[{i}] has no 'params'")
+        params = [g["params"]] if isinstance(g["params"], torch.Tensor) else list(g["params"])
+        if not params:
+            raise ValueError(f"{name}: param_groups[{i}]['params'] is empty")
+        for p in params:
+            if id(p) not in known:
+                raise ValueError(f"{name}: param_groups[{i}] names a parameter that is in no gradient bucket of the model")
+            if id(p) in seen:
+                raise ValueError(f"{name}: a parameter appears twice in param_groups (again in group {i})")
+            seen.add(id(p))
+        glr, gwd = float(g.get("lr", lr)), float(g.get("weight_decay", weight_decay))
+        check(glr, gwd)
+        out.append({"params": params, "lr": glr, "weight_decay": gwd})
+    n = len(out) + (1 if len(seen) < len(known) else 0)
+    if n > MAX_PARAM_GROUPS:
+        raise ValueError(f"{name}: at most {MAX_PARAM_GROUPS} parameter groups, the default group of the parameters named in "
+                         f"no group included; got {n}")
+    for gb in buckets:
+        if gb.flat.is_cuda and any(o % 4 for o in gb.offsets):
+            raise ValueError(f"{name}: param_groups on CUDA need every tensor of a bucket at a multiple of 4 elements (the "
+                             "group map has one id per 16-byte parameter vector); build the buckets with align=4")
+    return out
+
+
+def _group_attr(key: str):
+    """``lr`` / ``weight_decay`` of FlatSGD and FlatAdamW: the default group's values (``param_groups[-1]``)."""
+    return property(lambda self: self._default_group[key], lambda self, v: self._default_group.__setitem__(key, float(v)))
+
+
 def _peer_world(gb) -> bool:
     """Does this gradient bucket live in the symmetric memory of ONE peer-memory world (not the two-level world of several
     machines), in a dtype ``sharded_sgd_kernel`` reduces?"""
@@ -204,7 +263,7 @@ class _FlatOptimizer:
     kernel (``_sharded_kernel``) or the owned slice of a bucket with torch ops (``_update_slice``)."""
 
     def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
-                 max_grad_norm: Optional[float], sharded: bool):
+                 max_grad_norm: Optional[float], sharded: bool, param_groups: Optional[list] = None):
         from .. import comm
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
@@ -267,6 +326,111 @@ class _FlatOptimizer:
             if self._shard_mode is not None:
                 gb.sharded_step = lambda max_blocks=None, k=len(self.param_flats) - 1: self._sharded_step(k, max_blocks)
         self._native = None
+        self._names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        self._set_groups(param_groups)
+
+    # ------------------------------------------------------------------ parameter groups
+    def _set_groups(self, given: Optional[list]) -> None:
+        """The group layout of ``given`` (checked groups, or None: no groups).  ``_group_list`` holds the groups the updates
+        read -- the given ones in order, then the default group if any parameter is in none -- and per bucket ``_runs[k]``
+        cuts ``[0, numel)`` into ``(lo, hi, group)`` runs: each tensor's padded segment takes its tensor's group, and adjacent
+        segments of one group merge.  The kernel paths also get a uint8 group map with one id per fp32 parameter vector: the
+        whole bucket, or this rank's slice of the padded flat (padding in the last group)."""
+        self._grouped = given is not None
+        self._group_list, self._runs, self._maps = None, [], []
+        laid = [p for gb in self.buckets for p in gb.params]
+        default = getattr(self, "_default_group", None)
+        if not self._grouped:
+            if default is not None:
+                default["params"] = laid
+            return
+        gid = {}
+        for i, g in enumerate(given):
+            for p in g["params"]:
+                gid[id(p)] = i
+        rest = [p for p in laid if id(p) not in gid]
+        default["params"] = rest
+        self._group_list = list(given) + ([default] if rest else [])
+        for p in rest:
+            gid[id(p)] = len(given)
+        n_groups = len(self._group_list)
+        for k, (gb, pf) in enumerate(zip(self.buckets, self.param_flats)):
+            runs = []
+            for i, (p, o) in enumerate(zip(gb.params, gb.offsets)):
+                lo, hi = (0 if i == 0 else o), (gb.offsets[i + 1] if i + 1 < len(gb.params) else gb.numel)
+                if runs and runs[-1][2] == gid[id(p)]:
+                    runs[-1][1] = hi
+                else:
+                    runs.append([lo, hi, gid[id(p)]])
+            self._runs.append([tuple(r) for r in runs])
+            if self._shard_mode == "kernel":
+                n_pad, per = self._shards[k][1], self._shards[k][2]
+                whole = self._group_map(runs + [[gb.numel, n_pad, n_groups - 1]], n_pad // 4, n_groups)
+                self._maps.append(whole[self._rank * per // 4:(self._rank + 1) * per // 4].to(pf.device))
+            elif self._shard_mode is None and pf.is_cuda and gb.flat.dtype == torch.float32:
+                self._maps.append(self._group_map(runs, (gb.numel + 3) // 4, n_groups).to(pf.device))
+            else:
+                self._maps.append(None)
+
+    @staticmethod
+    def _group_map(runs: list, n_vec: int, n_groups: int) -> torch.Tensor:
+        """One uint8 group id per 16-byte fp32 vector of ``runs`` (element runs at multiples of 4), checked against the
+        number of groups before it is used."""
+        ids = torch.tensor([r[2] for r in runs if r[1] > r[0]], dtype=torch.int64)
+        lens = torch.tensor([(min(r[1], 4 * n_vec) + 3) // 4 - r[0] // 4 for r in runs if r[1] > r[0]], dtype=torch.int64)
+        m = torch.repeat_interleave(ids, lens)
+        if m.numel() != n_vec or (m.numel() and not (0 <= int(m.min()) and int(m.max()) < n_groups <= MAX_PARAM_GROUPS)):
+            raise ValueError(f"group map of {m.numel()} ids for {n_vec} vectors, or an id outside [0, {n_groups})")
+        return m.to(torch.uint8)
+
+    def _group_values(self) -> list:
+        """``(lr, weight_decay)`` of every group for the next update: ``lr_schedule.lr_at(group lr, steps)`` with a schedule."""
+        s = self.lr_schedule
+        return [(s.lr_at(g["lr"], self.steps) if s is not None else float(g["lr"]), float(g["weight_decay"]))
+                for g in self._group_list]
+
+    def _slice_runs(self, k: int, lo: int, n: int) -> list:
+        """Bucket ``k``'s runs cut to ``[lo, lo + n)``, as ``(start, end, group)`` relative to ``lo``."""
+        out = []
+        for a, b, g in self._runs[k]:
+            a, b = max(a, lo), min(b, lo + n)
+            if a < b:
+                out.append((a - lo, b - lo, g))
+        return out
+
+    @property
+    def param_groups(self) -> list:
+        """The parameter groups, as torch's optimizers list them: the ``param_groups`` given to the constructor in order,
+        then the default group of the parameters named in none (``lr`` / ``weight_decay`` are the optimizer's ``lr`` /
+        ``weight_decay``).  Each is a dict with ``"params"``, ``"lr"`` and ``"weight_decay"``; every update reads the values,
+        so assigning to them works as in torch.  Without ``param_groups`` it is the one default group."""
+        return list(self._group_list) if self._grouped else [self._default_group]
+
+    def _group_state(self) -> dict:
+        """What a state_dict records of the groups: ``{"param_groups": [{"params": [names], "lr", "weight_decay"}]}``."""
+        if not self._grouped:
+            return {}
+        return {"param_groups": [{"params": [self._names.get(id(p), "") for p in g["params"]], "lr": float(g["lr"]),
+                                  "weight_decay": float(g["weight_decay"])} for g in self._group_list]}
+
+    def _load_group_state(self, sd: dict, apply: bool = True) -> None:
+        """The groups' lr / weight_decay from ``sd["param_groups"]``; ``ValueError`` if its membership is not this optimizer's
+        (``apply=False``: only that check).  A state_dict without the key (written without groups) leaves the groups as built."""
+        saved = sd.get("param_groups")
+        if saved is None:
+            return
+        mine = self.param_groups if hasattr(self, "_default_group") else [{"params": [p for gb in self.buckets for p in gb.params]}]
+        names = [sorted(self._names.get(id(p), "") for p in g["params"]) for g in mine]
+        if names != [sorted(g["params"]) for g in saved]:
+            raise ValueError(f"{type(self).__name__}.load_state_dict: the state_dict's parameter groups hold other parameters "
+                             f"than this optimizer's ({len(saved)} saved groups, {len(mine)} here)")
+        if not apply:
+            return
+        if not self._grouped:                  # one group with every parameter: the optimizer's own lr / weight_decay
+            self.lr, self.weight_decay = float(saved[0]["lr"]), float(saved[0]["weight_decay"])
+            return
+        for g, s in zip(self._group_list, saved):
+            g["lr"], g["weight_decay"] = float(s["lr"]), float(s["weight_decay"])
 
     def _state_flat(self, k: int) -> torch.Tensor:
         """A zero fp32 state flat for bucket ``k``: the whole flat, or this rank's shard of it when sharded."""
@@ -478,18 +642,56 @@ class FlatSGD(_FlatOptimizer):
     ``sharded=False`` (given the all-reduce's fixed rank order).  ``max_grad_norm`` cannot be combined with it (the total
     norm needs every bucket reduced before any update) and raises ``ValueError``.  :meth:`named_momentum` is then collective
     (every rank calls it; it gathers the shards) and returns the same per-name tensors as an unsharded optimizer, so
-    checkpoints stay engine-independent.  At world size 1 the flag changes nothing."""
+    checkpoints stay engine-independent.  At world size 1 the flag changes nothing.
+
+    ``param_groups=[{"params": [...], "lr": ..., "weight_decay": ...}, ...]`` gives groups of parameters their own lr and /
+    or weight decay, as torch's parameter groups do (absent keys take the constructor's values; other keys raise
+    ``ValueError``; at most 64 groups).  The parameters named in no group form the default group, last in
+    :attr:`param_groups`, whose values are ``lr`` / ``weight_decay``.  Every update reads the groups' values, and
+    ``lr_schedule`` scales each group's lr.  On CUDA the update stays one launch per bucket (``sgd_flat_grouped``,
+    ``sharded_sgd_grouped``): a uint8 group map, one id per 16-byte parameter vector, picks each element's scalars.
+    ``state_dict()`` records the groups by parameter name and ``load_state_dict`` restores their values."""
+
+    lr = _group_attr("lr")
+    weight_decay = _group_attr("weight_decay")
 
     def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
                  zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
-                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None):
         check_sgd_options(momentum, weight_decay, nesterov)
-        self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
+        if param_groups is not None:
+            param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
+                                               lambda glr, gwd: check_sgd_options(momentum, gwd, nesterov))
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.momentum = float(momentum)
         self.nesterov = bool(nesterov)
-        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups)
         self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
 
+    def _sgd_runs(self, runs: list, pv: torch.Tensor, mv: torch.Tensor, g: torch.Tensor) -> None:
+        """The torch-op update of ``_update`` on each ``(lo, hi, group)`` run of the views, with the group's lr and decay."""
+        vals = self._group_values()
+        for lo, hi, gi in runs:
+            lr, wd = vals[gi]
+            p, m, gf = pv[lo:hi], mv[lo:hi], g[lo:hi].to(torch.float32)
+            if wd:
+                gf = gf.add(p, alpha=wd)
+            m.mul_(self.momentum).add_(gf)
+            p.add_(gf.add(m, alpha=self.momentum) if self.nesterov else m, alpha=-lr)
+
     def _update(self, kernel: List[bool], clip: dict) -> None:
+        if self._grouped:
+            vals = self._group_values()
+            for k, (gb, pf, mf, kern) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats, kernel)):
+                g = gb.flat[:gb.numel]
+                if kern:
+                    self._kernel().sgd_flat_grouped(pf, mf, g, self._maps[k], [v[0] for v in vals], [v[1] for v in vals],
+                                                    self.momentum, self.fused_zero, self.nesterov, **clip)
+                    continue
+                self._sgd_runs(self._runs[k], pf, mf, g)
+                if self.fused_zero:
+                    g.zero_()
+            return
         lr = self.lr_at()
         for gb, pf, mf, kern in zip(self.buckets, self.param_flats, self.momentum_flats, kernel):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
@@ -510,11 +712,21 @@ class FlatSGD(_FlatOptimizer):
     def _sharded_kernel(self, k: int, max_blocks: int) -> None:
         gb, mf = self.buckets[k], self.momentum_flats[k]
         n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        if self._grouped:
+            vals = self._group_values()
+            self._kernel().sharded_sgd_grouped(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, self._maps[k],
+                                               n_vec, [v[0] for v in vals], [v[1] for v in vals], self.momentum, self.nesterov,
+                                               1.0 / W, self.fused_zero, gb.world.rank, W, max_blocks)
+            return
         self._kernel().sharded_sgd(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, n_vec, self.lr_at(),
                                    self.momentum, self.weight_decay, self.nesterov, 1.0 / W, self.fused_zero, gb.world.rank, W,
                                    max_blocks)
 
     def _update_slice(self, k: int, lo: int, n: int) -> None:
+        if self._grouped:
+            self._sgd_runs(self._slice_runs(k, lo, n), self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n],
+                           self.buckets[k].flat[lo:lo + n])
+            return
         lr = self.lr_at()
         pv, mv = self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n]
         gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
@@ -536,6 +748,7 @@ class FlatSGD(_FlatOptimizer):
               "max_grad_norm": self.max_grad_norm, "steps": self.steps,
               "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
         sd.update(self._shard_tags())
+        sd.update(self._group_state())
         return sd
 
     def named_momentum(self, model: nn.Module) -> dict:
@@ -551,13 +764,16 @@ class FlatSGD(_FlatOptimizer):
         return self._load_named(model, named, self.momentum_flats)
 
     def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
+        """Inverse of :meth:`state_dict` (same model => same bucket layout).  A state_dict with ``param_groups`` restores each
+        group's lr / weight_decay and raises ``ValueError`` if its groups hold other parameters than this optimizer's."""
+        self._load_group_state(sd, apply=False)
         self.lr, self.momentum, self.weight_decay = float(sd["lr"]), float(sd["momentum"]), float(sd["weight_decay"])
         self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
         self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))   # ... and before clipping: none
         self.steps = int(sd.get("steps", self.steps))
         self._load_flats(sd, [(self.momentum_flats, sd["momentum_buffers"])], "momentum",
                          "named_momentum() / load_named_momentum()")
+        self._load_group_state(sd)
 
 
 def check_adamw_options(lr: float, betas, eps: float, weight_decay: float) -> tuple:
@@ -602,14 +818,25 @@ class FlatAdamW(_FlatOptimizer):
     fp32 in rank order, applies AdamW to the owned slice and stores the new parameters into every rank's flat, inside
     ``average_gradients`` / the DDP hooks; ``step()`` only counts the step.  Without one peer-memory world torch ops run the
     same semantics; at world size 1 the flag changes nothing; with ``max_grad_norm`` it raises ``ValueError``.
-    :meth:`named_state` (collective when sharded) is ``torch.optim.AdamW``'s per-parameter state by parameter name."""
+    :meth:`named_state` (collective when sharded) is ``torch.optim.AdamW``'s per-parameter state by parameter name.
+
+    ``param_groups`` are :class:`FlatSGD`'s (per-group ``lr`` / ``weight_decay``; e.g. no decay on biases and norm weights).
+    The grouped kernels (``adamw_flat_grouped``, ``sharded_adamw_grouped``) take ``1 - lr_g*wd_g`` and ``lr_g / (1 - beta1^t)``
+    per group (:meth:`group_scalars`); elsewhere torch's AdamW runs once per group, as ``torch.optim.AdamW`` does."""
+
+    lr = _group_attr("lr")
+    weight_decay = _group_attr("weight_decay")
 
     def __init__(self, model: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 1e-2, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
-                 max_grad_norm: Optional[float] = None, sharded: bool = False):
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None):
         self.betas = check_adamw_options(lr, betas, eps, weight_decay)
-        self.lr, self.eps, self.weight_decay = float(lr), float(eps), float(weight_decay)
-        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded)
+        if param_groups is not None:
+            param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
+                                               lambda glr, gwd: check_adamw_options(glr, betas, eps, gwd))
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.eps = float(eps)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups)
         self.exp_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
         self.exp_avg_sq_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
 
@@ -617,16 +844,54 @@ class FlatAdamW(_FlatOptimizer):
         """:func:`adamw_scalars` of the next update (t = ``steps`` + 1, lr = :meth:`lr_at`)."""
         return adamw_scalars(self.lr_at(), self.betas, self.eps, self.weight_decay, self.steps + 1)
 
-    def _torch_adamw(self, p: list, g: list, m: list, v: list) -> None:
-        """torch's single-tensor AdamW on the given views (update t = steps + 1)."""
+    def group_scalars(self) -> tuple:
+        """With parameter groups: ``(shared, decays, step_sizes)`` of the next update -- :meth:`scalars` (whose decay and
+        step size the grouped kernels do not use), then ``1 - lr_g*wd_g`` and ``lr_g / (1 - beta1^t)`` of every group, each
+        computed in fp64 by :func:`adamw_scalars` from the group's scheduled lr."""
+        per = [adamw_scalars(lr, self.betas, self.eps, wd, self.steps + 1) for lr, wd in self._group_values()]
+        return self.scalars(), [s[0] for s in per], [s[4] for s in per]
+
+    def _torch_adamw(self, p: list, g: list, m: list, v: list, lr: Optional[float] = None,
+                     weight_decay: Optional[float] = None) -> None:
+        """torch's single-tensor AdamW on the given views (update t = steps + 1), with the optimizer's lr and weight decay
+        unless a group's are given."""
         from torch.optim.adamw import adamw
 
         steps = [torch.tensor(float(self.steps)) for _ in p]
         adamw(p, g, m, v, [], steps, foreach=False, capturable=False, differentiable=False, fused=None, amsgrad=False,
-              beta1=self.betas[0], beta2=self.betas[1], lr=self.lr_at(), weight_decay=self.weight_decay, eps=self.eps,
-              maximize=False)
+              beta1=self.betas[0], beta2=self.betas[1], lr=self.lr_at() if lr is None else lr,
+              weight_decay=self.weight_decay if weight_decay is None else weight_decay, eps=self.eps, maximize=False)
+
+    def _adamw_runs(self, runs: list, flats: list) -> None:
+        """torch's AdamW once per group (as torch.optim.AdamW steps its groups), on the group's ``(lo, hi, group)`` runs of the
+        views ``flats`` = [p, g (fp32), m, v]."""
+        vals = self._group_values()
+        for gi, (lr, wd) in enumerate(vals):
+            mine = [(lo, hi) for lo, hi, g in runs if g == gi]
+            if mine:
+                self._torch_adamw(*[[f[lo:hi] for lo, hi in mine] for f in flats], lr=lr, weight_decay=wd)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
+        if self._grouped:
+            sc = self.group_scalars() if any(kernel) else None
+            for k, (gb, pf, mf, vf, kern) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats,
+                                                            self.exp_avg_sq_flats, kernel)):
+                g = gb.flat[:gb.numel]
+                if kern:
+                    self._kernel().adamw_flat_grouped(pf, mf, vf, g, self._maps[k], *sc, self.fused_zero, **clip)
+                    continue
+                gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+                # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.AdamW sees it
+                views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
+                         for f in (pf, gf, mf, vf)]
+                gid = [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
+                for gi, (lr, wd) in enumerate(self._group_values()):
+                    idx = [i for i, x in enumerate(gid) if x == gi]
+                    if idx:
+                        self._torch_adamw(*[[vs[i] for i in idx] for vs in views], lr=lr, weight_decay=wd)
+                if self.fused_zero:
+                    g.zero_()
+            return
         sc = self.scalars() if any(kernel) else None
         for gb, pf, mf, vf, kern in zip(self.buckets, self.param_flats, self.exp_avg_flats, self.exp_avg_sq_flats, kernel):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
@@ -643,12 +908,21 @@ class FlatAdamW(_FlatOptimizer):
     def _sharded_kernel(self, k: int, max_blocks: int) -> None:
         gb = self.buckets[k]
         n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        if self._grouped:
+            self._kernel().sharded_adamw_grouped(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs,
+                                                 self.exp_avg_flats[k], self.exp_avg_sq_flats[k], self._maps[k], n_vec,
+                                                 *self.group_scalars(), 1.0 / W, self.fused_zero, gb.world.rank, W, max_blocks)
+            return
         self._kernel().sharded_adamw(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, self.exp_avg_flats[k],
                                      self.exp_avg_sq_flats[k], n_vec, self.scalars(), 1.0 / W, self.fused_zero, gb.world.rank,
                                      W, max_blocks)
 
     def _update_slice(self, k: int, lo: int, n: int) -> None:
         gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
+        if self._grouped:
+            self._adamw_runs(self._slice_runs(k, lo, n), [self._shards[k][3][lo:lo + n], gf, self.exp_avg_flats[k][:n],
+                                                          self.exp_avg_sq_flats[k][:n]])
+            return
         self._torch_adamw([self._shards[k][3][lo:lo + n]], [gf], [self.exp_avg_flats[k][:n]], [self.exp_avg_sq_flats[k][:n]])
 
     # ------------------------------------------------------------------ checkpointing
@@ -661,16 +935,20 @@ class FlatAdamW(_FlatOptimizer):
               "exp_avg": [m.detach().cpu().clone() for m in self.exp_avg_flats],
               "exp_avg_sq": [v.detach().cpu().clone() for v in self.exp_avg_sq_flats]}
         sd.update(self._shard_tags())
+        sd.update(self._group_state())
         return sd
 
     def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout)."""
+        """Inverse of :meth:`state_dict` (same model => same bucket layout).  A state_dict with ``param_groups`` restores each
+        group's lr / weight_decay and raises ``ValueError`` if its groups hold other parameters than this optimizer's."""
+        self._load_group_state(sd, apply=False)
         self._load_flats(sd, [(self.exp_avg_flats, sd["exp_avg"]), (self.exp_avg_sq_flats, sd["exp_avg_sq"])],
                          "AdamW state", "named_state() / load_named_state()")
         self.betas = check_adamw_options(sd["lr"], sd["betas"], sd["eps"], sd["weight_decay"])
         self.lr, self.eps, self.weight_decay = float(sd["lr"]), float(sd["eps"]), float(sd["weight_decay"])
         self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
         self.steps = int(sd["steps"])
+        self._load_group_state(sd)
 
     def named_state(self, model: nn.Module) -> dict:
         """``{name: {"step", "exp_avg", "exp_avg_sq"}}`` (CPU copies), ``torch.optim.AdamW``'s per-parameter state by

@@ -46,14 +46,16 @@ def run(rank, size):
         else torch.device("cpu")
     torch.manual_seed(1234)
     model = dist.DistributedDataParallel(SmallConvNet().to(dev), bucket_cap_bytes=64 << 10)
+    # --no-decay-bias-norm: biases and norm weights (ndim <= 1) in a group without weight decay, the usual recipe
+    groups = [{"params": [p for p in model.parameters() if p.ndim <= 1], "weight_decay": 0.0}] if CFG["no_decay"] else None
     if CFG["optimizer"] == "adamw":
-        optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"])
+        optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"], param_groups=groups)
     elif CFG["optimizer"] == "lamb":
         optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2)
     elif CFG["optimizer"] == "lars":
         optimizer = dist.FlatLARS(model, lr=2.0, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-2)
     else:
-        optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"])
+        optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"], param_groups=groups)
     loss = None
     for step in range(CFG["steps"]):
         g = torch.Generator().manual_seed(1000 * step + rank)        # every rank its own part of the global batch
@@ -82,7 +84,11 @@ if __name__ == "__main__":
                     help="sharded=True: each rank keeps the optimizer state of, and updates, 1/size of every bucket")
     ap.add_argument("--optimizer", choices=("sgd", "adamw", "lamb", "lars"), default="sgd",
                     help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatLAMB or FlatLARS (the last two unsharded)")
+    ap.add_argument("--no-decay-bias-norm", action="store_true",
+                    help="sgd / adamw: no weight decay on biases and norm weights (a param_groups entry with weight_decay=0)")
     a = ap.parse_args()
+    if a.no_decay_bias_norm and a.optimizer not in ("sgd", "adamw"):
+        ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw; FlatLAMB and FlatLARS exclude them already")
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
-                                                optimizer=a.optimizer))
+                                                optimizer=a.optimizer, no_decay=a.no_decay_bias_norm))
     dist.launch(run, size=a.size, backend=a.backend)
