@@ -4,6 +4,7 @@
 #include "adamw_device.cuh"
 #include "param_groups.cuh"
 #include "sgd_device.cuh"
+#include "flat_scalars.cuh"
 
 namespace b2 {
 
@@ -104,9 +105,86 @@ __global__ void __launch_bounds__(256) adamw_flat_grouped_kernel(float* __restri
   }
 }
 
+// Capturable instances of adamw_flat_kernel and adamw_flat_grouped_kernel (flat_scalars.cuh): the AdamwScalars (kGrouped:
+// also every group's decay and step_size) come from the scalar block `blk`, loaded once per CTA through shared memory.  The
+// per-element sequence is adamw_elem, so the same scalars give the same bits.
+template <bool kClip, bool kGrouped>
+__global__ void __launch_bounds__(256) adamw_flat_cap_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
+                                                             float* __restrict__ g, size_t n, const uint8_t* __restrict__ map,
+                                                             const FlatScalars* __restrict__ blk, int zero_grad,
+                                                             const double* __restrict__ sqnorms, int n_buckets, float max_norm,
+                                                             float* grad_norm_out) {
+  __shared__ float s_coef;
+  __shared__ AdamwScalars s_s;
+  __shared__ AdamwGroups s_gs;
+  flat_block_load(s_s, blk->adamw);
+  if constexpr (kGrouped) flat_block_load(s_gs, blk->adamw_groups);
+  if constexpr (kClip) {
+    if (threadIdx.x == 0) s_coef = flat_clip_coef(sqnorms, n_buckets, max_norm, grad_norm_out);
+  }
+  __syncthreads();
+  const float c = kClip ? s_coef : 1.f;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    AdamwScalars sg = s_s;
+    if constexpr (kGrouped) {
+      const int gid = map[i];
+      sg.decay = s_gs.decay[gid];
+      sg.step_size = s_gs.step_size[gid];
+    }
+    float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 pv = reinterpret_cast<float4*>(p)[i];
+    float4 mv = reinterpret_cast<float4*>(m)[i];
+    float4 vv = reinterpret_cast<float4*>(v)[i];
+    if constexpr (kClip) {
+      gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
+    }
+    adamw4(pv, mv, vv, gv, sg);
+    reinterpret_cast<float4*>(p)[i] = pv;
+    reinterpret_cast<float4*>(m)[i] = mv;
+    reinterpret_cast<float4*>(v)[i] = vv;
+    if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (i < n - n4 * 4) {                        // tail (< 4 elements): threads 0..2 of CTA 0, one element each
+    const size_t t = n4 * 4 + i;
+    AdamwScalars sg = s_s;
+    if constexpr (kGrouped) {
+      const int gid = map[n4];
+      sg.decay = s_gs.decay[gid];
+      sg.step_size = s_gs.step_size[gid];
+    }
+    const float gt = kClip ? __fmul_rn(g[t], c) : g[t];
+    adamw_elem(p[t], m[t], v[t], gt, sg);
+    if (zero_grad) g[t] = 0.f;
+  }
+}
+
 }  // namespace b2
 
 extern "C" {
+
+// The capturable adamw_flat / adamw_flat_grouped (flat_scalars.cuh): the scalars come from the block `blk` on the device.
+// `map`: null without groups, else one group id per parameter vector.  cudaErrorInvalidValue, without a launch, for a null
+// pointer or clipping without sqnorms.
+int b2_adamw_flat_cap_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk,
+                             int zero_grad, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
+                             cudaStream_t stream) {
+  if (p == nullptr || m == nullptr || v == nullptr || g == nullptr || blk == nullptr) return (int)cudaErrorInvalidValue;
+  const bool clip = max_norm > 0.f;
+  if (clip && (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
+  const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
+  const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  using namespace b2;
+  if (clip) {
+    if (map != nullptr) adamw_flat_cap_kernel<true, true><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, blk, zero_grad, sqnorms, n_buckets, max_norm, grad_norm_out);
+    else adamw_flat_cap_kernel<true, false><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, blk, zero_grad, sqnorms, n_buckets, max_norm, grad_norm_out);
+  } else {
+    if (map != nullptr) adamw_flat_cap_kernel<false, true><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, blk, zero_grad, nullptr, 0, 0.f, nullptr);
+    else adamw_flat_cap_kernel<false, false><<<blocks, 256, 0, stream>>>(p, m, v, g, n, map, blk, zero_grad, nullptr, 0, 0.f, nullptr);
+  }
+  return (int)cudaGetLastError();
+}
 
 // One AdamW update of a flat bucket of n elements on `stream`.  max_norm > 0: clipped by the norm of grad_sqnorm's n_buckets
 // sums.  cudaErrorInvalidValue, without a launch, for a null pointer or clipping without sqnorms.

@@ -14,6 +14,7 @@
 
 #include "adamw.h"
 #include "executor.h"
+#include "flat_scalars.h"
 #include "batchnorm.h"
 #include "layerwise.h"
 #include "loader.h"
@@ -98,6 +99,20 @@ int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerP
                                     const b2::AdamwGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank,
                                     int world, int max_blocks, cudaStream_t stream);
 int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
+int b2_flat_scalars_launch(const b2::FlatHyper* table, unsigned long long* counter, b2::FlatScalars* block, int advance,
+                           cudaStream_t stream);
+int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk, float mu,
+                           int zero_grad, int nesterov, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
+                           cudaStream_t stream);
+int b2_adamw_flat_cap_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk,
+                             int zero_grad, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
+                             cudaStream_t stream);
+int b2_sharded_sgd_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* momentum,
+                              const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float mu, int nesterov, float scale,
+                              int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream);
+int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
+                                float* exp_avg_sq, const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float scale,
+                                int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
@@ -338,6 +353,39 @@ b2::LrSchedule to_sched(const py::object& o) {
   s.n_milestones = (int)ms.size();
   for (size_t i = 0; i < ms.size(); ++i) s.milestones[i] = ms[i];
   return s;
+}
+
+// A capturable optimizer's device state (csrc/flat_scalars.h): the step counter (int64 CUDA [1], read as uint64), the table
+// and the scalar block (uint8 CUDA, 16-byte aligned, at least flat_scalars_layout()'s bytes, on one device).
+struct FlatState {
+  b2::FlatHyper* table;
+  unsigned long long* counter;
+  b2::FlatScalars* block;
+};
+FlatState flat_state(const torch::Tensor& table, const torch::Tensor& counter, const torch::Tensor& block, const char* what) {
+  TORCH_CHECK(counter.is_cuda() && counter.scalar_type() == torch::kInt64 && counter.numel() == 1, what,
+              ": counter: int64 CUDA [1]");
+  for (const torch::Tensor* t : {&table, &block})
+    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kUInt8 && t->device() == counter.device() &&
+                (uintptr_t)t->data_ptr() % 16 == 0, what, ": table / block: 16-byte aligned uint8 CUDA on the counter's device");
+  TORCH_CHECK((size_t)table.numel() >= sizeof(b2::FlatHyper) && (size_t)block.numel() >= sizeof(b2::FlatScalars), what,
+              ": table / block: at least ", sizeof(b2::FlatHyper), " / ", sizeof(b2::FlatScalars), " bytes");
+  return {reinterpret_cast<b2::FlatHyper*>(table.data_ptr()), reinterpret_cast<unsigned long long*>(counter.data_ptr()),
+          reinterpret_cast<b2::FlatScalars*>(block.data_ptr())};
+}
+// The block argument of a capturable update launch (see flat_state)
+const b2::FlatScalars* flat_block(const torch::Tensor& block, const torch::Tensor& like, const char* what) {
+  TORCH_CHECK(block.is_cuda() && block.is_contiguous() && block.scalar_type() == torch::kUInt8 && block.device() == like.device() &&
+              (size_t)block.numel() >= sizeof(b2::FlatScalars) && (uintptr_t)block.data_ptr() % 16 == 0, what,
+              ": block: 16-byte aligned uint8 CUDA of at least ", sizeof(b2::FlatScalars), " bytes on the parameters' device");
+  return reinterpret_cast<const b2::FlatScalars*>(block.data_ptr());
+}
+// An optional group map of `n_ids` ids (null without groups)
+const uint8_t* flat_map(const c10::optional<torch::Tensor>& map, int64_t n_ids, const char* what) {
+  if (!map.has_value()) return nullptr;
+  TORCH_CHECK(map->is_cuda() && map->is_contiguous() && map->scalar_type() == torch::kUInt8 && map->numel() >= n_ids, what,
+              ": group_map: contiguous uint8 CUDA of at least ", n_ids, " ids (one per fp32 parameter vector)");
+  return map->data_ptr<uint8_t>();
 }
 
 torch::Tensor tensor_from_ptr(unsigned long long ptr, int64_t numel, py::object dtype, int device) {
@@ -983,6 +1031,180 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
   m.def("max_param_groups", [] { return b2::kMaxGroups; }, "the most parameter groups the grouped optimizer kernels take");
+  // Capturable FlatSGD / FlatAdamW (csrc/flat_scalars.cuh): the layout of the scalar block in fp32 words and the byte sizes
+  // of the block and the table
+  m.def("flat_scalars_layout", [] {
+    py::dict d;
+    d["lr"] = offsetof(b2::FlatScalars, lr) / 4;
+    d["wd"] = offsetof(b2::FlatScalars, wd) / 4;
+    d["adamw"] = offsetof(b2::FlatScalars, adamw) / 4;
+    d["sgd_lr"] = (offsetof(b2::FlatScalars, sgd) + offsetof(b2::SgdGroups, lr)) / 4;
+    d["sgd_wd"] = (offsetof(b2::FlatScalars, sgd) + offsetof(b2::SgdGroups, wd)) / 4;
+    d["decay"] = (offsetof(b2::FlatScalars, adamw_groups) + offsetof(b2::AdamwGroups, decay)) / 4;
+    d["step_size"] = (offsetof(b2::FlatScalars, adamw_groups) + offsetof(b2::AdamwGroups, step_size)) / 4;
+    d["block_bytes"] = sizeof(b2::FlatScalars);
+    d["table_bytes"] = sizeof(b2::FlatHyper);
+    return d;
+  });
+  // Upload the hyper-parameters (every group's base lr and weight decay in fp64, the AdamW constants, the schedule) and, with
+  // `steps`, the step counter, then fill the block of the update run at the counter's value.  The values are staged in a
+  // pinned buffer of torch's caching host allocator and copied with non_blocking copies (the allocator keeps the buffer until
+  // the copy has run), so the call does not wait for the device.  Refused while the current stream is being captured: a
+  // graph would replay this call's values.
+  m.def("flat_scalars_sync", [](torch::Tensor table, torch::Tensor counter, torch::Tensor block, std::vector<double> lrs,
+                                std::vector<double> weight_decays, double beta1, double beta2, double eps, py::object schedule,
+                                c10::optional<int64_t> steps) {
+    const FlatState st = flat_state(table, counter, block, "flat_scalars_sync");
+    TORCH_CHECK(!lrs.empty() && lrs.size() <= (size_t)b2::kMaxGroups && lrs.size() == weight_decays.size(),
+                "flat_scalars_sync: 1..", b2::kMaxGroups, " groups with one lr and one weight_decay each");
+    TORCH_CHECK(!steps.has_value() || *steps >= 0, "flat_scalars_sync: steps must be >= 0");
+    b2::FlatHyper h;
+    std::memset(&h, 0, sizeof(h));
+    h.sched = to_sched(schedule);
+    h.beta1 = beta1; h.beta2 = beta2; h.eps = eps;
+    h.n_groups = (int)lrs.size();
+    for (size_t i = 0; i < lrs.size(); ++i) {
+      TORCH_CHECK(std::isfinite((float)lrs[i]) && weight_decays[i] >= 0.0 && std::isfinite(weight_decays[i]),
+                  "flat_scalars_sync: lr must be finite in fp32 and weight_decay finite and >= 0");
+      h.lr[i] = lrs[i];
+      h.wd[i] = weight_decays[i];
+    }
+    c10::cuda::CUDAGuard guard(counter.device());
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    ck_cuda((int)cudaStreamIsCapturing(cur_stream(), &cap), "flat_scalars_sync");
+    TORCH_CHECK(cap == cudaStreamCaptureStatusNone, "flat_scalars_sync: the current stream is being captured; upload the "
+                "hyper-parameters or set the step counter outside the capture");
+    const int64_t nh = (int64_t)sizeof(b2::FlatHyper);
+    auto staged = torch::empty({nh + 8}, torch::TensorOptions().dtype(torch::kUInt8).pinned_memory(true));
+    std::memcpy(staged.data_ptr(), &h, sizeof(h));
+    table.narrow(0, 0, nh).copy_(staged.narrow(0, 0, nh), /*non_blocking=*/true);
+    if (steps.has_value()) {
+      const unsigned long long s = (unsigned long long)*steps;
+      std::memcpy(staged.data_ptr<uint8_t>() + nh, &s, sizeof(s));
+      counter.view(torch::kUInt8).copy_(staged.narrow(0, nh, 8), /*non_blocking=*/true);
+    }
+    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, 0, cur_stream()), "flat_scalars_sync launch");
+  }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("lrs"), py::arg("weight_decays"), py::arg("beta1") = 0.0,
+     py::arg("beta2") = 0.0, py::arg("eps") = 0.0, py::arg("schedule") = py::none(), py::arg("steps") = py::none());
+  // counter += 1 and the block of the next update, in one single-CTA launch (advance = false: the block only)
+  m.def("flat_scalars_advance", [](torch::Tensor table, torch::Tensor counter, torch::Tensor block, bool advance) {
+    const FlatState st = flat_state(table, counter, block, "flat_scalars_advance");
+    c10::cuda::CUDAGuard guard(counter.device());
+    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, advance ? 1 : 0, cur_stream()), "flat_scalars_advance launch");
+  }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("advance") = true);
+  // sgd_flat / sgd_flat_grouped (with group_map) with the scalars from the block: arguments as theirs otherwise
+  m.def("sgd_flat_cap", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, c10::optional<torch::Tensor> group_map,
+                           torch::Tensor block, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
+                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_cap: nesterov needs a nonzero momentum");
+    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat_cap");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "sgd_flat_cap: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat_cap");
+    for (const auto* t : {&p, &mom, &g}) {
+      check_cuda_contig(*t, "sgd_flat_cap: p, m and g");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "sgd_flat_cap: p, m and g: 16-byte aligned fp32 of one size");
+    }
+    const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "sgd_flat_cap");
+    const b2::FlatScalars* blk = flat_block(block, p, "sgd_flat_cap");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_sgd_flat_cap_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), map, blk,
+                                   (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+            "sgd_flat_cap launch");
+  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("block"), py::arg("mu"), py::arg("zero_grad"),
+     py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none());
+  // adamw_flat / adamw_flat_grouped (with group_map) with the scalars from the block
+  m.def("adamw_flat_cap", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                             c10::optional<torch::Tensor> group_map, torch::Tensor block, bool zero_grad, py::object max_grad_norm,
+                             c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat_cap");
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, "adamw_flat_cap: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat_cap");
+    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
+      check_cuda_contig(*t, "adamw_flat_cap: p, exp_avg, exp_avg_sq and g");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "adamw_flat_cap: p, exp_avg, exp_avg_sq and g: 16-byte aligned fp32 of one size");
+    }
+    const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "adamw_flat_cap");
+    const b2::FlatScalars* blk = flat_block(block, p, "adamw_flat_cap");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_adamw_flat_cap_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
+                                     (size_t)p.numel(), map, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+            "adamw_flat_cap launch");
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("block"),
+     py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none());
+  // sharded_sgd / sharded_sgd_grouped (with group_map: this rank's ids) with the scalars from the block
+  m.def("sharded_sgd_cap", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                              std::vector<unsigned long long> sigs, torch::Tensor momentum, c10::optional<torch::Tensor> group_map,
+                              torch::Tensor block, size_t n_vec, double mu, bool nesterov, double scale, bool zero_grad, int rank,
+                              int world, int max_blocks) {
+    check_world(rank, world, "sharded_sgd_cap");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_sgd_cap: one gradient bucket, one parameter flat and one signal pad per rank");
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd_cap: n_vec must be a multiple of world, got ", n_vec, " for ", world);
+    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd_cap: nesterov needs a nonzero momentum");
+    check_cuda_contig(momentum, "momentum");
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
+                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd_cap: momentum: 16-byte aligned fp32 of at least ", shard,
+                " elements (this rank's slice)");
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd_cap: null or misaligned per-rank pointer");
+    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), "sharded_sgd_cap");
+    const b2::FlatScalars* blk = flat_block(block, momentum, "sharded_sgd_cap");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(momentum.device());
+    ck_cuda(b2_sharded_sgd_cap_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), map, blk, n_vec, (float)mu,
+                                      nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+            "sharded_sgd_cap launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("group_map"),
+     py::arg("block"), py::arg("n_vec"), py::arg("mu"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  // sharded_adamw / sharded_adamw_grouped (with group_map: this rank's ids) with the scalars from the block
+  m.def("sharded_adamw_cap", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
+                                c10::optional<torch::Tensor> group_map, torch::Tensor block, size_t n_vec, double scale,
+                                bool zero_grad, int rank, int world, int max_blocks) {
+    check_world(rank, world, "sharded_adamw_cap");
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
+                "sharded_adamw_cap: one gradient bucket, one parameter flat and one signal pad per rank");
+    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw_cap: n_vec must be a multiple of world, got ", n_vec, " for ", world);
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
+      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
+                  "sharded_adamw_cap: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements");
+    }
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw_cap: null or misaligned per-rank pointer");
+    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), "sharded_adamw_cap");
+    const b2::FlatScalars* blk = flat_block(block, exp_avg, "sharded_adamw_cap");
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(exp_avg.device());
+    ck_cuda(b2_sharded_adamw_cap_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), map, blk,
+                                        n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+            "sharded_adamw_cap launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+     py::arg("group_map"), py::arg("block"), py::arg("n_vec"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0);
   m.def("sgd_flat_grouped", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, torch::Tensor group_map, std::vector<double> lrs,
                                std::vector<double> weight_decays, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
                                c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {

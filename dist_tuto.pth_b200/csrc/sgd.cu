@@ -16,6 +16,7 @@
 #include "sgd_device.cuh"
 #include "convnet_reduce.cuh"
 #include "param_groups.cuh"
+#include "flat_scalars.cuh"
 
 namespace b2 {
 
@@ -424,6 +425,52 @@ __global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict
   }
 }
 
+// Capturable instances of sgd_flat_kernel, sgd_flat_clip_kernel and sgd_flat_grouped_kernel (flat_scalars.cuh): the lr and
+// weight decay (kGrouped: every group's) come from the scalar block `blk`, loaded once per CTA through shared memory, instead
+// of the kernel arguments.  The per-element sequence is sgd4, the fmaf sequence of those kernels, so the same scalars give
+// the same bits.
+template <bool kNesterov, bool kClip, bool kGrouped>
+__global__ void __launch_bounds__(256) sgd_flat_cap_kernel(float* __restrict__ p, float* __restrict__ m,
+                                                           const float* __restrict__ g, size_t n, const uint8_t* __restrict__ map,
+                                                           const FlatScalars* __restrict__ blk, float mu, int zero_grad, float* gw,
+                                                           const double* __restrict__ sqnorms, int n_buckets, float max_norm,
+                                                           float* grad_norm_out) {
+  __shared__ float s_coef, s_lr, s_wd;
+  __shared__ SgdGroups s_gs;
+  if constexpr (kGrouped) flat_block_load(s_gs, blk->sgd);
+  if (threadIdx.x == 0) {
+    if constexpr (!kGrouped) { s_lr = blk->lr; s_wd = blk->wd; }
+    if constexpr (kClip) s_coef = flat_clip_coef(sqnorms, n_buckets, max_norm, grad_norm_out);
+  }
+  __syncthreads();
+  const float c = kClip ? s_coef : 1.f;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (i < n4) {
+    const int gid = kGrouped ? map[i] : 0;
+    float4 gv = reinterpret_cast<const float4*>(g)[i];
+    float4 pv = reinterpret_cast<float4*>(p)[i];
+    float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kClip) {
+      gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
+    }
+    sgd4<kNesterov>(pv, mv, gv, kGrouped ? s_gs.lr[gid] : s_lr, mu, kGrouped ? s_gs.wd[gid] : s_wd);
+    reinterpret_cast<float4*>(p)[i] = pv;
+    reinterpret_cast<float4*>(m)[i] = mv;
+    if (zero_grad) reinterpret_cast<float4*>(gw)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (i == 0 && n4 * 4 < n) {
+    const int gid = kGrouped ? map[n4] : 0;
+    const float lr = kGrouped ? s_gs.lr[gid] : s_lr, wd = kGrouped ? s_gs.wd[gid] : s_wd;
+    for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
+      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(g[t], c) : g[t]);
+      m[t] = fmaf(mu, m[t], gt);
+      p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
+      if (zero_grad) gw[t] = 0.f;
+    }
+  }
+}
+
 // out[i] = the lr the optimizer kernels apply when the step counter reads steps[i] (tests tie it to ops/optim.LRSchedule)
 __global__ void __launch_bounds__(256) lr_schedule_eval_kernel(LrSchedule s, float base, const long long* __restrict__ steps,
                                                                float* __restrict__ out, long long n) {
@@ -642,6 +689,36 @@ int b2_sgd_flat_grouped_launch(float* p, float* m, const float* g, size_t n, con
     b2::sgd_flat_grouped_kernel<false, false><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, nullptr, 0,
                                                                           0.f, nullptr);
   }
+  return (int)cudaGetLastError();
+}
+
+// The capturable sgd_flat / sgd_flat_grouped (flat_scalars.cuh): the scalars come from the block `blk` on the device.  `map`:
+// null without groups, else one group id per parameter vector.  cudaErrorInvalidValue, without a launch, for a null pointer
+// or clipping without sqnorms.
+int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk, float mu,
+                           int zero_grad, int nesterov, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
+                           cudaStream_t stream) {
+  if (p == nullptr || m == nullptr || g == nullptr || blk == nullptr) return (int)cudaErrorInvalidValue;
+  const bool clip = max_norm > 0.f;
+  if (clip && (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
+  const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
+  const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  float* gw = const_cast<float*>(g);
+  using namespace b2;
+#define B2_SGD_CAP(N, C, G) sgd_flat_cap_kernel<N, C, G><<<blocks, 256, 0, stream>>>(p, m, g, n, map, blk, mu, zero_grad, gw, \
+                                                                                   sqnorms, n_buckets, max_norm, grad_norm_out)
+  const int k = (nesterov ? 4 : 0) | (clip ? 2 : 0) | (map != nullptr ? 1 : 0);
+  switch (k) {
+    case 0: B2_SGD_CAP(false, false, false); break;
+    case 1: B2_SGD_CAP(false, false, true); break;
+    case 2: B2_SGD_CAP(false, true, false); break;
+    case 3: B2_SGD_CAP(false, true, true); break;
+    case 4: B2_SGD_CAP(true, false, false); break;
+    case 5: B2_SGD_CAP(true, false, true); break;
+    case 6: B2_SGD_CAP(true, true, false); break;
+    default: B2_SGD_CAP(true, true, true); break;
+  }
+#undef B2_SGD_CAP
   return (int)cudaGetLastError();
 }
 

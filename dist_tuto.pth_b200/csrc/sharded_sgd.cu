@@ -29,9 +29,15 @@
 //
 // With parameter groups, ShardedSgdGroupedUpdate and ShardedAdamwGroupedUpdate load a group id next to the state of each
 // parameter vector and take that group's scalars; the skeleton and the other instances are unchanged.
+//
+// Capturable<U> (FlatSGD / FlatAdamW capturable=True, flat_scalars.cuh) is U with its scalars read from the device scalar
+// block: the skeleton calls its begin() once per CTA, which copies them to shared memory; the other instances compile
+// without that call.
 #include <cstring>
+#include <type_traits>
 #include "adamw_device.cuh"
 #include "common.cuh"
+#include "flat_scalars.cuh"
 #include "param_groups.cuh"
 
 namespace b2 {
@@ -154,6 +160,53 @@ struct ShardedAdamwGroupedUpdate {
   }
 };
 
+// Capturable instances (flat_scalars.cuh): Capturable<U> is the update U with the scalars its apply() reads taken from the
+// scalar block on the device instead of the kernel arguments.  Its begin(), which the skeleton calls once per CTA, copies them
+// into a shared copy of U's arguments; load(), apply() and store() are U's, apply() reading that copy.
+__device__ __forceinline__ void cap_fill(ShardedSgdArgs& s, const ShardedSgdArgs& a, const FlatScalars& b) {
+  if (threadIdx.x == 0) { s.lr = b.lr; s.wd = b.wd; s.mu = a.mu; }
+}
+__device__ __forceinline__ void cap_fill(ShardedAdamwArgs& s, const ShardedAdamwArgs&, const FlatScalars& b) {
+  flat_block_load(s.s, b.adamw);
+}
+__device__ __forceinline__ void cap_fill(ShardedSgdGroupedArgs& s, const ShardedSgdGroupedArgs& a, const FlatScalars& b) {
+  flat_block_load(s.gs, b.sgd);
+  if (threadIdx.x == 0) s.mu = a.mu;
+}
+__device__ __forceinline__ void cap_fill(ShardedAdamwGroupedArgs& s, const ShardedAdamwGroupedArgs&, const FlatScalars& b) {
+  flat_block_load(s.s, b.adamw);
+  flat_block_load(s.gs, b.adamw_groups);
+}
+
+template <class A>
+struct CapArgs : A {
+  const FlatScalars* blk;
+};
+
+template <class U>
+struct Capturable {
+  using Args = CapArgs<typename U::Args>;
+  static constexpr int kUnroll = U::kUnroll;
+  U u;
+  static __device__ __forceinline__ typename U::Args& scalars() {
+    __shared__ typename U::Args s;
+    return s;
+  }
+  static __device__ __forceinline__ void begin(const Args& a) {
+    cap_fill(scalars(), a, *a.blk);
+    __syncthreads();
+  }
+  __device__ __forceinline__ void load(const Args& a, size_t q) { u.load(a, q); }
+  __device__ __forceinline__ void apply(const Args&, float4& p, float4 g) { u.apply(scalars(), p, g); }
+  __device__ __forceinline__ void store(const Args& a, size_t q) { u.store(a, q); }
+};
+
+// Does the update have a per-CTA begin() (the capturable ones)?  The other instances compile without the call.
+template <class U, class = void>
+struct HasBegin : std::false_type {};
+template <class U>
+struct HasBegin<U, std::void_t<decltype(&U::begin)>> : std::true_type {};
+
 __device__ __forceinline__ float4 as_f4(uint4 v) {
   return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
 }
@@ -166,6 +219,7 @@ template <bool kBf16, class Update>
 __global__ void __launch_bounds__(kShardThreads) sharded_step_kernel(typename Update::Args a) {
   constexpr int kP = kBf16 ? 2 : 1;                     // fp32 parameter vectors per gradient vector
   constexpr int kUnroll = Update::kUnroll;           // gradient vectors per thread and pass
+  if constexpr (HasBegin<Update>::value) Update::begin(a);
   const int rank = a.rank, world = a.world;
   uint32_t epoch = barrier_epoch_load(a.sig, rank);
   const size_t slice = a.n_vec / world;
@@ -346,6 +400,68 @@ int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerP
   using namespace b2;
   if (bf16) sharded_step_kernel<true, ShardedAdamwGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
   else sharded_step_kernel<false, ShardedAdamwGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// The capturable steps (Capturable<U>): as the launchers above, with the scalars taken from the block `blk` on the device.
+// `map`: null without groups, else this rank's group ids.  Same grid, same refusals, and a null block is refused too.
+int b2_sharded_sgd_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* momentum,
+                              const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float mu, int nesterov, float scale,
+                              int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream) {
+  if (momentum == nullptr || blk == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  using namespace b2;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  if (map != nullptr) {
+    CapArgs<ShardedSgdGroupedArgs> a;
+    memset(&a, 0, sizeof(a));
+    a.grads = *grads; a.params = *params; a.sig = *sig; a.momentum = momentum; a.map = map; a.n_vec = n_vec;
+    a.mu = mu; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.blk = blk;
+    if (bf16) {
+      if (nesterov) sharded_step_kernel<true, Capturable<ShardedSgdGroupedUpdate<true>>><<<grid, kShardThreads, 0, stream>>>(a);
+      else sharded_step_kernel<true, Capturable<ShardedSgdGroupedUpdate<false>>><<<grid, kShardThreads, 0, stream>>>(a);
+    } else {
+      if (nesterov) sharded_step_kernel<false, Capturable<ShardedSgdGroupedUpdate<true>>><<<grid, kShardThreads, 0, stream>>>(a);
+      else sharded_step_kernel<false, Capturable<ShardedSgdGroupedUpdate<false>>><<<grid, kShardThreads, 0, stream>>>(a);
+    }
+    return (int)cudaGetLastError();
+  }
+  CapArgs<ShardedSgdArgs> a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.momentum = momentum; a.n_vec = n_vec;
+  a.mu = mu; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.blk = blk;
+  if (bf16) {
+    if (nesterov) sharded_step_kernel<true, Capturable<ShardedSgdUpdate<true>>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<true, Capturable<ShardedSgdUpdate<false>>><<<grid, kShardThreads, 0, stream>>>(a);
+  } else {
+    if (nesterov) sharded_step_kernel<false, Capturable<ShardedSgdUpdate<true>>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, Capturable<ShardedSgdUpdate<false>>><<<grid, kShardThreads, 0, stream>>>(a);
+  }
+  return (int)cudaGetLastError();
+}
+
+int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* exp_avg,
+                                float* exp_avg_sq, const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float scale,
+                                int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream) {
+  if (exp_avg == nullptr || exp_avg_sq == nullptr || blk == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  using namespace b2;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  if (map != nullptr) {
+    CapArgs<ShardedAdamwGroupedArgs> a;
+    memset(&a, 0, sizeof(a));
+    a.grads = *grads; a.params = *params; a.sig = *sig; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.map = map;
+    a.n_vec = n_vec; a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.blk = blk;
+    if (bf16) sharded_step_kernel<true, Capturable<ShardedAdamwGroupedUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, Capturable<ShardedAdamwGroupedUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+    return (int)cudaGetLastError();
+  }
+  CapArgs<ShardedAdamwArgs> a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.n_vec = n_vec;
+  a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.blk = blk;
+  if (bf16) sharded_step_kernel<true, Capturable<ShardedAdamwUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+  else sharded_step_kernel<false, Capturable<ShardedAdamwUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 

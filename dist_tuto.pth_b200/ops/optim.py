@@ -23,6 +23,9 @@ the layout, the sharding, the exchange hooks and the step bookkeeping (``_FlatOp
 ``FlatSGD`` and ``FlatAdamW`` take torch-style ``param_groups`` (per-group lr and weight decay): the same launches with a
 per-vector group map and the groups' scalars in the kernel arguments.
 
+``FlatSGD(..., capturable=True)`` and ``FlatAdamW(..., capturable=True)`` keep the step counter, the lr schedule and AdamW's bias
+corrections on the device (csrc/flat_scalars.cuh), so a whole DDP step can be captured in a CUDA graph and replayed.
+
 ``FlatLAMB`` and ``FlatLARS`` are the large-batch optimizers with a trust ratio per parameter tensor: per bucket two kernels
 (csrc/layerwise.cu) form every tensor's norms in a fixed order over a chunk table of the flat layout, then apply the update.
 """
@@ -263,11 +266,13 @@ class _FlatOptimizer:
     kernel (``_sharded_kernel``) or the owned slice of a bucket with torch ops (``_update_slice``)."""
 
     def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
-                 max_grad_norm: Optional[float], sharded: bool, param_groups: Optional[list] = None):
+                 max_grad_norm: Optional[float], sharded: bool, param_groups: Optional[list] = None,
+                 capturable: bool = False):
         from .. import comm
         from ..parallel.ddp import DistributedDataParallel, GradBucket, flatten_params
 
         name = type(self).__name__
+        self.capturable = bool(capturable)
         self.sharded = bool(sharded)
         if self.sharded and max_grad_norm is not None:
             raise ValueError(f"{name}(sharded=True) cannot clip: the total norm needs every bucket reduced before any update, "
@@ -328,6 +333,75 @@ class _FlatOptimizer:
         self._native = None
         self._names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
         self._set_groups(param_groups)
+        if self.capturable:
+            self._init_capturable(name)
+
+    # ------------------------------------------------------------------ capturable: step counter and scalars on the device
+    def _init_capturable(self, name: str) -> None:
+        """``capturable=True``: refuse every bucket a torch-op path would update (its host scalars would be frozen by a graph),
+        then allocate the extension, the clip buffers, the device step counter, the hyper-parameter table and the scalar
+        block (csrc/flat_scalars.h), and fill the block of the first update."""
+        for gb, pf in zip(self.buckets, self.param_flats):
+            if not pf.is_cuda:
+                raise ValueError(f"{name}(capturable=True) needs CUDA parameters; CPU (gloo) updates run torch ops on the host")
+            if self._shard_mode is None and gb.flat.dtype != torch.float32:
+                raise ValueError(f"{name}(capturable=True) needs fp32 gradient buckets unless sharded=True: a {gb.flat.dtype} "
+                                 "bucket is updated by torch ops whose scalars a CUDA graph would freeze")
+        if self._shard_mode == "torch":
+            raise ValueError(f"{name}(capturable=True, sharded=True) needs one peer-memory world (backend 'b200' on one "
+                             "machine): elsewhere the sharded update runs torch ops whose scalars a CUDA graph would freeze")
+        C = self._kernel()
+        lay = C.flat_scalars_layout()
+        dev = self.param_flats[0].device
+        if self.max_grad_norm is not None:
+            self._clip_bufs = (torch.zeros(len(self.buckets), dtype=torch.float64, device=dev),
+                               torch.zeros(C.grad_sqnorm_workspace_numel(), dtype=torch.float32, device=dev),
+                               torch.zeros(1, dtype=torch.float32, device=dev))
+        self._cap_counter = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._cap_table = torch.zeros(lay["table_bytes"], dtype=torch.uint8, device=dev)
+        self._cap_block = torch.zeros(lay["block_bytes"], dtype=torch.uint8, device=dev)
+        self._cap_synced = None
+        self._sync_device(steps=self._steps)
+
+    def _hyper(self) -> tuple:
+        """What the device table holds: every group's base lr and weight decay, the AdamW constants and the schedule."""
+        groups = self._group_list if self._grouped else [self._default_group]
+        b1, b2 = getattr(self, "betas", (0.0, 0.0))
+        return ([float(g["lr"]) for g in groups], [float(g["weight_decay"]) for g in groups], float(b1), float(b2),
+                float(getattr(self, "eps", 0.0)), schedule_tuple(self.lr_schedule))
+
+    def _sync_device(self, steps: Optional[int] = None) -> None:
+        """Upload the table (and with ``steps`` the counter) and refill the block; refused inside a capture, which would
+        replay this call's values."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError(f"{type(self).__name__}: the hyper-parameters and the step counter of a capturable optimizer are "
+                               "uploaded outside a CUDA-graph capture (call sync_hyperparameters() or set steps before "
+                               "capturing or between replays)")
+        h = self._hyper()
+        self._kernel().flat_scalars_sync(self._cap_table, self._cap_counter, self._cap_block, *h, steps=steps)
+        self._cap_synced = h
+
+    def _cap_refresh(self) -> None:
+        """Before an eager capturable update: upload the hyper-parameters if one changed since the last upload.  Inside a
+        capture nothing is uploaded (the replays use the table as it stands)."""
+        if not torch.cuda.is_current_stream_capturing() and self._hyper() != self._cap_synced:
+            self._sync_device()
+
+    @property
+    def steps(self) -> int:
+        """Updates applied so far.  With ``capturable=True`` it is the device counter (reading it synchronises; assigning it
+        writes the counter and recomputes the next update's scalars, and raises ``RuntimeError`` inside a capture), so it
+        counts graph replays too."""
+        if getattr(self, "_cap_counter", None) is not None:
+            return int(self._cap_counter.item())
+        return self._steps
+
+    @steps.setter
+    def steps(self, value: int) -> None:
+        if getattr(self, "_cap_counter", None) is not None:
+            self._sync_device(steps=int(value))
+        else:
+            self._steps = int(value)
 
     # ------------------------------------------------------------------ parameter groups
     def _set_groups(self, given: Optional[list]) -> None:
@@ -456,8 +530,18 @@ class _FlatOptimizer:
                 raise RuntimeError(f"{type(self).__name__}(sharded=True).step(): this step's gradient buckets were not "
                                    "exchanged; call average_gradients(model) after backward() (one average_gradients per step)")
             self._done = [False] * len(self.buckets)
-            self.steps += 1
+            if self.capturable:
+                self._advance()
+            else:
+                self.steps += 1
             if self._engine is not None:
+                self._engine._reset()
+            return
+        if self.capturable:
+            self._cap_refresh()
+            self._update_capturable(self._clip_on_device() if self.max_grad_norm is not None else {})
+            self._advance()
+            if self.fused_zero and self._engine is not None:
                 self._engine._reset()
             return
         kernel = [pf.is_cuda and gb.flat.dtype == torch.float32 for gb, pf in zip(self.buckets, self.param_flats)]
@@ -489,6 +573,8 @@ class _FlatOptimizer:
         gb = self.buckets[k]
         per, full = self._shards[k][2], self._shards[k][3]
         if self._shard_mode == "kernel":
+            if self.capturable:                 # the scalars the previous step() computed, with any new group values
+                self._cap_refresh()
             self._sharded_kernel(k, gb.world.max_blocks if max_blocks is None else max_blocks)
         else:
             gb.all_reduce_average_(max_blocks)
@@ -500,6 +586,23 @@ class _FlatOptimizer:
             if self.fused_zero:
                 gb.flat.zero_()
         self._done[k] = True
+
+    def _sync_hyperparameters(self) -> None:
+        """``capturable=True``: upload the groups' ``lr`` / ``weight_decay`` (and ``lr_schedule``) to the device table and
+        recompute the next update's scalars from it: two non-blocking copies from pinned memory and one launch on the current
+        stream.  An eager ``step()`` does this by itself when a value changed; a CUDA graph replays the table as it stands, so
+        after assigning a new lr between replays call this outside the capture (as with torch's capturable optimizers, whose
+        lr must be a tensor to change under a graph).  ``RuntimeError`` inside a capture.  Without ``capturable`` it does
+        nothing."""
+        if self.capturable:
+            self._sync_device()
+
+    def _advance(self) -> None:
+        """capturable: counter += 1 and the scalars of the next update, one single-CTA launch after this step's updates."""
+        self._kernel().flat_scalars_advance(self._cap_table, self._cap_counter, self._cap_block)
+
+    def _cap_map(self, k: int) -> Optional[torch.Tensor]:
+        return self._maps[k] if self._grouped else None
 
     def shard_range(self, k: int) -> tuple:
         """``(lo, hi)``: the elements of bucket ``k``'s flat this rank owns (updates, and holds the optimizer state of);
@@ -650,14 +753,26 @@ class FlatSGD(_FlatOptimizer):
     :attr:`param_groups`, whose values are ``lr`` / ``weight_decay``.  Every update reads the groups' values, and
     ``lr_schedule`` scales each group's lr.  On CUDA the update stays one launch per bucket (``sgd_flat_grouped``,
     ``sharded_sgd_grouped``): a uint8 group map, one id per 16-byte parameter vector, picks each element's scalars.
-    ``state_dict()`` records the groups by parameter name and ``load_state_dict`` restores their values."""
+    ``state_dict()`` records the groups by parameter name and ``load_state_dict`` restores their values.
+
+    ``capturable=True`` lets a CUDA graph capture the whole step (forward, backward with the bucket exchanges, ``step()``),
+    as ``torch.optim.SGD(capturable=True)`` does: the step counter lives on the device, and the update kernels read their
+    scalars (the scheduled lr of every group and its weight decay) from a block on the device that a one-CTA kernel advances after every
+    update, so replays follow the schedule.  ``step()`` then does no host synchronisation, allocation or host-to-device
+    copy, apart from uploading group ``lr`` / ``weight_decay`` values that changed since the last eager step;
+    :meth:`sync_hyperparameters` does that upload outside a capture (replays read the device table as it stands, so a
+    value assigned between replays takes effect with that call).  ``steps``, :meth:`lr_at` and the checkpoints read or write the device counter.  Warm up with eager steps
+    on a side stream before capturing, as torch requires.  Refused (``ValueError``) where a bucket would take a torch-op
+    path: CPU (gloo), reduced-precision unsharded gradient buckets, and ``sharded=True`` without one peer-memory world."""
 
     lr = _group_attr("lr")
     weight_decay = _group_attr("weight_decay")
+    sync_hyperparameters = _FlatOptimizer._sync_hyperparameters
 
     def __init__(self, model: nn.Module, lr: float = 0.01, momentum: float = 0.5, weight_decay: float = 0.0,
                  zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None, nesterov: bool = False,
-                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None):
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None,
+                 capturable: bool = False):
         check_sgd_options(momentum, weight_decay, nesterov)
         if param_groups is not None:
             param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
@@ -665,7 +780,7 @@ class FlatSGD(_FlatOptimizer):
         self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
         self.momentum = float(momentum)
         self.nesterov = bool(nesterov)
-        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups, capturable)
         self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
 
     def _sgd_runs(self, runs: list, pv: torch.Tensor, mv: torch.Tensor, g: torch.Tensor) -> None:
@@ -709,9 +824,19 @@ class FlatSGD(_FlatOptimizer):
             if self.fused_zero:
                 g.zero_()
 
+    def _update_capturable(self, clip: dict) -> None:
+        for k, (gb, pf, mf) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats)):
+            self._kernel().sgd_flat_cap(pf, mf, gb.flat[:gb.numel], self._cap_map(k), self._cap_block, self.momentum,
+                                        self.fused_zero, self.nesterov, **clip)
+
     def _sharded_kernel(self, k: int, max_blocks: int) -> None:
         gb, mf = self.buckets[k], self.momentum_flats[k]
         n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        if self.capturable:
+            self._kernel().sharded_sgd_cap(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, self._cap_map(k),
+                                           self._cap_block, n_vec, self.momentum, self.nesterov, 1.0 / W, self.fused_zero,
+                                           gb.world.rank, W, max_blocks)
+            return
         if self._grouped:
             vals = self._group_values()
             self._kernel().sharded_sgd_grouped(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs, mf, self._maps[k],
@@ -774,6 +899,7 @@ class FlatSGD(_FlatOptimizer):
         self._load_flats(sd, [(self.momentum_flats, sd["momentum_buffers"])], "momentum",
                          "named_momentum() / load_named_momentum()")
         self._load_group_state(sd)
+        self._sync_hyperparameters()
 
 
 def check_adamw_options(lr: float, betas, eps: float, weight_decay: float) -> tuple:
@@ -822,21 +948,33 @@ class FlatAdamW(_FlatOptimizer):
 
     ``param_groups`` are :class:`FlatSGD`'s (per-group ``lr`` / ``weight_decay``; e.g. no decay on biases and norm weights).
     The grouped kernels (``adamw_flat_grouped``, ``sharded_adamw_grouped``) take ``1 - lr_g*wd_g`` and ``lr_g / (1 - beta1^t)``
-    per group (:meth:`group_scalars`); elsewhere torch's AdamW runs once per group, as ``torch.optim.AdamW`` does."""
+    per group (:meth:`group_scalars`); elsewhere torch's AdamW runs once per group, as ``torch.optim.AdamW`` does.
+
+    ``capturable=True`` lets a CUDA graph capture the whole step (forward, backward with the bucket exchanges, ``step()``),
+    as ``torch.optim.AdamW(capturable=True)`` does: the step counter lives on the device, and the update kernels read their
+    scalars (the scheduled lr of every group, ``1 - lr*wd``, ``lr / (1 - beta1^t)`` and ``sqrt(1 - beta2^t)``) from a block
+    on the device that a one-CTA kernel advances after every update, so replays follow the schedule.  ``step()`` then does no host synchronisation, allocation or host-to-device
+    copy, apart from uploading group ``lr`` / ``weight_decay`` values that changed since the last eager step;
+    :meth:`sync_hyperparameters` does that upload outside a capture (replays read the device table as it stands, so a
+    value assigned between replays takes effect with that call).  ``steps``, :meth:`lr_at` and the checkpoints read or write the device counter.  Warm up with eager steps
+    on a side stream before capturing, as torch requires.  Refused (``ValueError``) where a bucket would take a torch-op
+    path: CPU (gloo), reduced-precision unsharded gradient buckets, and ``sharded=True`` without one peer-memory world."""
 
     lr = _group_attr("lr")
     weight_decay = _group_attr("weight_decay")
+    sync_hyperparameters = _FlatOptimizer._sync_hyperparameters
 
     def __init__(self, model: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 1e-2, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
-                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None):
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None,
+                 capturable: bool = False):
         self.betas = check_adamw_options(lr, betas, eps, weight_decay)
         if param_groups is not None:
             param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
                                                lambda glr, gwd: check_adamw_options(glr, betas, eps, gwd))
         self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
         self.eps = float(eps)
-        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups, capturable)
         self.exp_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
         self.exp_avg_sq_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
 
@@ -905,9 +1043,19 @@ class FlatAdamW(_FlatOptimizer):
             if self.fused_zero:
                 g.zero_()
 
+    def _update_capturable(self, clip: dict) -> None:
+        for k, (gb, pf, mf, vf) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats, self.exp_avg_sq_flats)):
+            self._kernel().adamw_flat_cap(pf, mf, vf, gb.flat[:gb.numel], self._cap_map(k), self._cap_block, self.fused_zero,
+                                          **clip)
+
     def _sharded_kernel(self, k: int, max_blocks: int) -> None:
         gb = self.buckets[k]
         n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        if self.capturable:
+            self._kernel().sharded_adamw_cap(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs,
+                                             self.exp_avg_flats[k], self.exp_avg_sq_flats[k], self._cap_map(k), self._cap_block,
+                                             n_vec, 1.0 / W, self.fused_zero, gb.world.rank, W, max_blocks)
+            return
         if self._grouped:
             self._kernel().sharded_adamw_grouped(gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs,
                                                  self.exp_avg_flats[k], self.exp_avg_sq_flats[k], self._maps[k], n_vec,
@@ -949,6 +1097,7 @@ class FlatAdamW(_FlatOptimizer):
         self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
         self.steps = int(sd["steps"])
         self._load_group_state(sd)
+        self._sync_hyperparameters()
 
     def named_state(self, model: nn.Module) -> dict:
         """``{name: {"step", "exp_avg", "exp_avg_sq"}}`` (CPU copies), ``torch.optim.AdamW``'s per-parameter state by

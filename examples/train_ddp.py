@@ -9,6 +9,8 @@ the tutorial's loop, on synthetic data.
     python examples/train_ddp.py --optimizer adamw [--sharded-optimizer]   # FlatAdamW; sharded: both moments 1/size per rank
     python examples/train_ddp.py --optimizer lamb                 # FlatLAMB / FlatLARS (--optimizer lars): per-tensor trust
                                                                   # ratios for large global batches
+    python examples/train_ddp.py --backend b200 --size 1 --cuda-graph   # capturable=True: warm-up steps, then every step
+                                                                  # is one replay of a captured CUDA graph
 
 The loop is ``backward(); average_gradients(model); optimizer.step()`` either way.  With ``--sharded-optimizer`` the update
 happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
@@ -40,6 +42,43 @@ class SmallConvNet(nn.Module):
         return self.fc2(F.relu(self.fc1(x.flatten(1))))
 
 
+def batch(step, rank, dev):
+    g = torch.Generator().manual_seed(1000 * step + rank)            # every rank its own part of the global batch
+    return torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
+
+
+def train_graphed(model, optimizer, rank, dev, steps, warmup=3):
+    """--cuda-graph: ``warmup`` eager steps on a side stream (as torch requires before a capture), one step captured, and
+    every later step a ``copy_`` of its batch into the static inputs and one replay.  Returns the last step's loss."""
+    x, y = (t.clone() for t in batch(0, rank, dev))
+
+    def step():
+        loss = F.cross_entropy(model(x), y)
+        loss.backward()
+        dist.average_gradients(model)
+        optimizer.step()
+        return loss
+
+    s = torch.cuda.Stream(dev)
+    s.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(s):
+        for i in range(min(warmup, steps)):
+            for t, src in zip((x, y), batch(i, rank, dev)):
+                t.copy_(src)
+            loss = step()
+    torch.cuda.current_stream(dev).wait_stream(s)
+    if steps <= warmup:
+        return loss
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        loss = step()
+    for i in range(warmup, steps):
+        for t, src in zip((x, y), batch(i, rank, dev)):
+            t.copy_(src)
+        graph.replay()
+    return loss
+
+
 def run(rank, size):
     CFG = json.loads(os.environ["B2_DDP_CFG"])            # spawned ranks re-import this file: pass the CLI through the env
     dev = torch.device("cuda", torch.cuda.current_device()) if CFG["backend"] != "gloo" and torch.cuda.is_available() \
@@ -48,18 +87,21 @@ def run(rank, size):
     model = dist.DistributedDataParallel(SmallConvNet().to(dev), bucket_cap_bytes=64 << 10)
     # --no-decay-bias-norm: biases and norm weights (ndim <= 1) in a group without weight decay, the usual recipe
     groups = [{"params": [p for p in model.parameters() if p.ndim <= 1], "weight_decay": 0.0}] if CFG["no_decay"] else None
+    cap = {"capturable": True} if CFG["cuda_graph"] else {}
     if CFG["optimizer"] == "adamw":
-        optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"], param_groups=groups)
+        optimizer = dist.FlatAdamW(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"], param_groups=groups, **cap)
     elif CFG["optimizer"] == "lamb":
         optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2)
     elif CFG["optimizer"] == "lars":
         optimizer = dist.FlatLARS(model, lr=2.0, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-2)
     else:
-        optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"], param_groups=groups)
+        optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"], param_groups=groups,
+                                 **cap)
     loss = None
-    for step in range(CFG["steps"]):
-        g = torch.Generator().manual_seed(1000 * step + rank)        # every rank its own part of the global batch
-        x, y = torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
+    if CFG["cuda_graph"]:
+        loss = train_graphed(model, optimizer, rank, dev, CFG["steps"])
+    for step in range(0 if CFG["cuda_graph"] else CFG["steps"]):
+        x, y = batch(step, rank, dev)
         optimizer.zero_grad()
         loss = F.cross_entropy(model(x), y)
         loss.backward()
@@ -86,9 +128,14 @@ if __name__ == "__main__":
                     help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatLAMB or FlatLARS (the last two unsharded)")
     ap.add_argument("--no-decay-bias-norm", action="store_true",
                     help="sgd / adamw: no weight decay on biases and norm weights (a param_groups entry with weight_decay=0)")
+    ap.add_argument("--cuda-graph", action="store_true",
+                    help="sgd / adamw on --backend b200: capturable=True, and every step after the warm-up one graph replay")
     a = ap.parse_args()
+    if a.cuda_graph and (a.optimizer not in ("sgd", "adamw") or a.backend != "b200"):
+        ap.error("--cuda-graph is for --optimizer sgd / adamw on --backend b200 (CUDA)")
     if a.no_decay_bias_norm and a.optimizer not in ("sgd", "adamw"):
         ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw; FlatLAMB and FlatLARS exclude them already")
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
-                                                optimizer=a.optimizer, no_decay=a.no_decay_bias_norm))
+                                                optimizer=a.optimizer, no_decay=a.no_decay_bias_norm,
+                                                cuda_graph=a.cuda_graph))
     dist.launch(run, size=a.size, backend=a.backend)
