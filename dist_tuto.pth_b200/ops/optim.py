@@ -537,6 +537,10 @@ class _FlatOptimizer:
             if self._engine is not None:
                 self._engine._reset()
             return
+        if self._engine is not None and self._engine._unexchanged():
+            raise RuntimeError(f"{type(self).__name__}.step(): gradients accumulated under no_sync() were never exchanged; "
+                               "run the last micro-batch's backward outside no_sync(), or call average_gradients(model), "
+                               "before step()")
         if self.capturable:
             self._cap_refresh()
             self._update_capturable(self._clip_on_device() if self.max_grad_norm is not None else {})
@@ -763,7 +767,12 @@ class FlatSGD(_FlatOptimizer):
     :meth:`sync_hyperparameters` does that upload outside a capture (replays read the device table as it stands, so a
     value assigned between replays takes effect with that call).  ``steps``, :meth:`lr_at` and the checkpoints read or write the device counter.  Warm up with eager steps
     on a side stream before capturing, as torch requires.  Refused (``ValueError``) where a bucket would take a torch-op
-    path: CPU (gloo), reduced-precision unsharded gradient buckets, and ``sharded=True`` without one peer-memory world."""
+    path: CPU (gloo), reduced-precision unsharded gradient buckets, and ``sharded=True`` without one peer-memory world.
+
+    Gradient accumulation (every flat optimizer, sharded or not): run all but the last micro-batch's backward inside
+    ``DistributedDataParallel.no_sync()``.  The buckets are exchanged once per optimizer step, so ``steps``, the schedule
+    and the clipping norm see the accumulated, averaged gradient; ``step()`` raises ``RuntimeError`` while a bucket holds
+    accumulated gradients no exchange has taken."""
 
     lr = _group_attr("lr")
     weight_decay = _group_attr("weight_decay")

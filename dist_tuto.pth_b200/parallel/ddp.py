@@ -17,9 +17,12 @@ GPU-first design instead of "one blocking all_reduce + one divide per tensor":
     on a side stream as soon as its last gradient is written, overlapping
     communication with the rest of backward (tuto.md:216,320 points at the
     "official" DDP for this; here it is part of the library).
+    ``no_sync()`` accumulates micro-batches into the buckets without exchanging
+    them (gradient accumulation, as torch's ``no_sync``).
 """
 from __future__ import annotations
 
+import contextlib
 from typing import List, Optional, Sequence
 
 import torch
@@ -201,10 +204,11 @@ def broadcast_parameters(model: nn.Module, src: int = 0, group=None) -> None:
 
 
 class _Bucket:
-    __slots__ = ("gb", "pending", "ready_event", "launched")
+    # accumulated: the bucket holds gradients of backwards run under no_sync() that no exchange has taken yet
+    __slots__ = ("gb", "pending", "ready_event", "launched", "accumulated")
 
     def __init__(self, gb: GradBucket):
-        self.gb, self.pending, self.ready_event, self.launched = gb, 0, None, False
+        self.gb, self.pending, self.ready_event, self.launched, self.accumulated = gb, 0, None, False, False
 
 
 class DistributedDataParallel(nn.Module):
@@ -215,7 +219,12 @@ class DistributedDataParallel(nn.Module):
     gradient of a bucket has been accumulated, the bucket's fused all-reduce is
     enqueued on ``comm_stream`` behind an event, so it runs while autograd keeps
     producing earlier layers' gradients.  ``finish()`` (called by
-    ``average_gradients(model)`` or ``optimizer`` glue) joins the streams."""
+    ``average_gradients(model)`` or ``optimizer`` glue) joins the streams.
+
+    Gradient accumulation: backwards inside :meth:`no_sync` add into the
+    buckets and exchange nothing; the first backward outside it (or
+    ``average_gradients`` after ``no_sync`` backwards only) exchanges each
+    bucket's accumulated sum once."""
 
     def __init__(self, module: nn.Module, group=None, bucket_cap_bytes: int = 8 << 20,
                  overlap: bool = True, broadcast: bool = True, grad_dtype: Optional[torch.dtype] = None,
@@ -251,6 +260,7 @@ class DistributedDataParallel(nn.Module):
         for p in params:
             self._hooks.append(p.register_post_accumulate_grad_hook(self._on_grad))
         object.__setattr__(module, "_ddp_engine", self)   # not a submodule (would be a cycle)
+        self.require_backward_grad_sync = True              # False inside no_sync() (torch's attribute)
         self._reset()
 
     # -- construction -------------------------------------------------------
@@ -281,10 +291,41 @@ class DistributedDataParallel(nn.Module):
         """Zero every bucket (gradients stay views of the flat buffers) and re-arm the per-step hook bookkeeping."""
         for b in self._buckets:
             b.gb.zero_()
+            b.accumulated = False
         self._reset()
+
+    @contextlib.contextmanager
+    def no_sync(self):
+        """Gradient accumulation, as ``torch.nn.parallel.DistributedDataParallel.no_sync``: a backward inside the context
+        adds its gradients into the buckets and exchanges nothing; the first backward outside it exchanges each bucket's
+        accumulated sum once (with the usual overlap), and ``average_gradients(model)`` after ``no_sync`` backwards only
+        exchanges every bucket.  Scale the loss by 1 / micro-batches to get the mean::
+
+            for x, y in micro_batches[:-1]:
+                with model.no_sync():
+                    (loss_fn(model(x), y) / k).backward()
+            (loss_fn(model(x_last), y_last) / k).backward()
+            average_gradients(model)
+            optimizer.step()
+
+        Re-entrant.  ``average_gradients(model)`` inside it raises ``RuntimeError`` (it would average a partial sum), and
+        so does an unsharded optimizer's ``step()`` while a bucket holds accumulated gradients no exchange has taken.
+        ``SyncBatchNorm`` still exchanges its batch statistics in every forward, as torch's does.  bf16 buckets
+        (``grad_dtype=torch.bfloat16``) accumulate in bf16, rounding once per micro-batch."""
+        old = self.require_backward_grad_sync
+        self.require_backward_grad_sync = False
+        try:
+            yield
+        finally:
+            self.require_backward_grad_sync = old
+
+    def _unexchanged(self) -> bool:
+        """True while a bucket holds gradients accumulated under ``no_sync()`` that no exchange has taken."""
+        return any(b.accumulated for b in self._buckets)
 
     def _launch(self, b: _Bucket):
         b.launched = True
+        b.accumulated = False
         if self.world_size == 1:
             return
         if self.overlap:
@@ -303,12 +344,18 @@ class DistributedDataParallel(nn.Module):
         if p.grad is not None and p.grad.data_ptr() != v.data_ptr():
             v.copy_(p.grad)       # optimizer.zero_grad(set_to_none=True) detached the view
             p.grad = v
+        if not self.require_backward_grad_sync:       # no_sync(): accumulate only
+            b.accumulated = True
+            return
         b.pending -= 1
         if b.pending == 0 and not b.launched:
             self._launch(b)
 
     def finish(self):
-        """Complete all outstanding bucket all-reduces for this step."""
+        """Complete all outstanding bucket all-reduces for this step.  ``RuntimeError`` inside :meth:`no_sync`."""
+        if not self.require_backward_grad_sync:
+            raise RuntimeError("average_gradients(model) inside no_sync() would average a partial sum of the micro-batches' "
+                               "gradients; call it after the last backward, outside no_sync()")
         for b in self._buckets:
             if not b.launched:      # unused parameters / hooks not fired
                 self._launch(b)

@@ -11,8 +11,11 @@ the tutorial's loop, on synthetic data.
                                                                   # ratios for large global batches
     python examples/train_ddp.py --backend b200 --size 1 --cuda-graph   # capturable=True: warm-up steps, then every step
                                                                   # is one replay of a captured CUDA graph
+    python examples/train_ddp.py --accumulation-steps 4           # gradient accumulation: 4 micro-batches per step, the
+                                                                  # first 3 backwards under model.no_sync()
 
-The loop is ``backward(); average_gradients(model); optimizer.step()`` either way.  With ``--sharded-optimizer`` the update
+The loop is ``backward(); average_gradients(model); optimizer.step()`` either way; with ``--accumulation-steps k`` the k - 1
+backwards before the last run inside ``model.no_sync()`` on losses scaled by 1 / k.  With ``--sharded-optimizer`` the update
 happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
 gradient buckets the parameters are bit for bit the same.  Prints ``Rank r, step s: loss`` for the last step."""
 import argparse
@@ -42,29 +45,46 @@ class SmallConvNet(nn.Module):
         return self.fc2(F.relu(self.fc1(x.flatten(1))))
 
 
-def batch(step, rank, dev):
-    g = torch.Generator().manual_seed(1000 * step + rank)            # every rank its own part of the global batch
+def batch(step, rank, dev, micro=0):
+    # every rank its own part of the global batch; micro-batch 0 is the whole batch without accumulation
+    g = torch.Generator().manual_seed(1000 * step + rank + 1_000_003 * micro)
     return torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
 
 
-def train_graphed(model, optimizer, rank, dev, steps, warmup=3):
-    """--cuda-graph: ``warmup`` eager steps on a side stream (as torch requires before a capture), one step captured, and
-    every later step a ``copy_`` of its batch into the static inputs and one replay.  Returns the last step's loss."""
-    x, y = (t.clone() for t in batch(0, rank, dev))
+def train_step(model, optimizer, micro_batches):
+    """One optimizer step over ``micro_batches`` (a list of (x, y)): all but the last backward accumulate under no_sync(),
+    the last one exchanges the buckets.  Returns the last micro-batch's loss."""
+    k = len(micro_batches)
+    for x, y in micro_batches[:-1]:
+        with model.no_sync():
+            (F.cross_entropy(model(x), y) / k).backward()
+    x, y = micro_batches[-1]
+    loss = F.cross_entropy(model(x), y)
+    (loss / k).backward()
+    dist.average_gradients(model)       # --sharded-optimizer: the parameters are updated when this returns
+    optimizer.step()
+    return loss
+
+
+def train_graphed(model, optimizer, rank, dev, steps, k, warmup=3):
+    """--cuda-graph: ``warmup`` eager steps on a side stream (as torch requires before a capture), one step (all k
+    micro-batches) captured, and every later step a ``copy_`` of its micro-batches into the static inputs and one replay.
+    Returns the last step's loss."""
+    static = [tuple(t.clone() for t in batch(0, rank, dev, j)) for j in range(k)]
+
+    def load(i):
+        for j, (x, y) in enumerate(static):
+            for t, src in zip((x, y), batch(i, rank, dev, j)):
+                t.copy_(src)
 
     def step():
-        loss = F.cross_entropy(model(x), y)
-        loss.backward()
-        dist.average_gradients(model)
-        optimizer.step()
-        return loss
+        return train_step(model, optimizer, static)
 
     s = torch.cuda.Stream(dev)
     s.wait_stream(torch.cuda.current_stream(dev))
     with torch.cuda.stream(s):
         for i in range(min(warmup, steps)):
-            for t, src in zip((x, y), batch(i, rank, dev)):
-                t.copy_(src)
+            load(i)
             loss = step()
     torch.cuda.current_stream(dev).wait_stream(s)
     if steps <= warmup:
@@ -73,8 +93,7 @@ def train_graphed(model, optimizer, rank, dev, steps, warmup=3):
     with torch.cuda.graph(graph):
         loss = step()
     for i in range(warmup, steps):
-        for t, src in zip((x, y), batch(i, rank, dev)):
-            t.copy_(src)
+        load(i)
         graph.replay()
     return loss
 
@@ -99,14 +118,10 @@ def run(rank, size):
                                  **cap)
     loss = None
     if CFG["cuda_graph"]:
-        loss = train_graphed(model, optimizer, rank, dev, CFG["steps"])
+        loss = train_graphed(model, optimizer, rank, dev, CFG["steps"], CFG["accumulation_steps"])
     for step in range(0 if CFG["cuda_graph"] else CFG["steps"]):
-        x, y = batch(step, rank, dev)
         optimizer.zero_grad()
-        loss = F.cross_entropy(model(x), y)
-        loss.backward()
-        dist.average_gradients(model)       # --sharded-optimizer: the parameters are updated when this returns
-        optimizer.step()
+        loss = train_step(model, optimizer, [batch(step, rank, dev, j) for j in range(CFG["accumulation_steps"])])
     total = loss.detach().clone()
     dist.all_reduce(total)
     if CFG["optimizer"] in ("adamw", "lamb"):
@@ -130,12 +145,16 @@ if __name__ == "__main__":
                     help="sgd / adamw: no weight decay on biases and norm weights (a param_groups entry with weight_decay=0)")
     ap.add_argument("--cuda-graph", action="store_true",
                     help="sgd / adamw on --backend b200: capturable=True, and every step after the warm-up one graph replay")
+    ap.add_argument("--accumulation-steps", type=int, default=1,
+                    help="micro-batches of 16 samples per rank and optimizer step (gradient accumulation with no_sync())")
     a = ap.parse_args()
+    if a.accumulation_steps < 1:
+        ap.error("--accumulation-steps must be at least 1")
     if a.cuda_graph and (a.optimizer not in ("sgd", "adamw") or a.backend != "b200"):
         ap.error("--cuda-graph is for --optimizer sgd / adamw on --backend b200 (CUDA)")
     if a.no_decay_bias_norm and a.optimizer not in ("sgd", "adamw"):
         ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw; FlatLAMB and FlatLARS exclude them already")
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
                                                 optimizer=a.optimizer, no_decay=a.no_decay_bias_norm,
-                                                cuda_graph=a.cuda_graph))
+                                                cuda_graph=a.cuda_graph, accumulation_steps=a.accumulation_steps))
     dist.launch(run, size=a.size, backend=a.backend)
