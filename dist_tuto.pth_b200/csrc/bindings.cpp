@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "adamw.h"
+#include "ema.h"
 #include "executor.h"
 #include "flat_scalars.h"
 #include "batchnorm.h"
@@ -113,6 +114,8 @@ int b2_sharded_sgd_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* p
 int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
                                 float* exp_avg_sq, const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float scale,
                                 int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream);
+int b2_ema_launch(const b2::EmaEntry* table, int n_entries, long long n_vec, long long n_scalar, float w, int mode,
+                  const long long* counter, long long every, long long warmup, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
 int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
@@ -1092,6 +1095,70 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(counter.device());
     ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, advance ? 1 : 0, cur_stream()), "flat_scalars_advance launch");
   }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("advance") = true);
+  // FlatEMA (csrc/ema.h): the entry table of (EMA array, live array) pairs, as (device table, host table); int64 rows of 8 words
+  m.def("ema_table", [](const std::vector<torch::Tensor>& emas, const std::vector<torch::Tensor>& lives) {
+    TORCH_CHECK(!emas.empty() && emas.size() == lives.size() && emas.size() < (size_t)INT32_MAX,
+                "ema_table: one live tensor per EMA tensor, at least one pair");
+    const torch::Device dev = emas[0].device();
+    auto host = torch::zeros({(int64_t)emas.size() * 8}, torch::dtype(torch::kInt64));
+    b2::EmaEntry* rows = reinterpret_cast<b2::EmaEntry*>(host.data_ptr<int64_t>());
+    long long n_vec = 0, n_scalar = 0;
+    for (size_t i = 0; i < emas.size(); ++i) {
+      const torch::Tensor& e = emas[i];
+      const torch::Tensor& p = lives[i];
+      for (const auto* t : {&e, &p})
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32 && t->device() == dev &&
+                    t->numel() >= 1 && t->data_ptr() != nullptr, "ema_table: entry ", i, ": non-empty contiguous fp32 CUDA tensors "
+                    "on one device");
+      TORCH_CHECK(e.numel() == p.numel(), "ema_table: entry ", i, ": the EMA and the live tensor differ in size");
+      const uintptr_t ea = (uintptr_t)e.data_ptr(), pa = (uintptr_t)p.data_ptr();
+      b2::EmaEntry& r = rows[i];
+      r.ema = e.data_ptr<float>();
+      r.live = p.data_ptr<float>();
+      r.n = e.numel();
+      if (ea % 16 == pa % 16) {        // both reach a 16-byte boundary after the same number of elements
+        r.head = std::min<long long>(r.n, (long long)((16 - ea % 16) % 16 / 4));
+        r.n_vec = (r.n - r.head) / 4;
+      } else {
+        r.head = r.n;
+        r.n_vec = 0;
+      }
+      r.vec_begin = n_vec;
+      r.scalar_begin = n_scalar;
+      n_vec += r.n_vec;
+      n_scalar += r.n - 4 * r.n_vec;
+    }
+    return py::make_tuple(host.to(dev), host);
+  }, py::arg("emas"), py::arg("lives"));
+  // One launch over every entry: host-decided (counter None: copy, or lerp with w) or device-counter (counter: the optimizer's
+  // int64 [1] step counter t; skip when t % every != 0, copy when t - every <= warmup_steps, lerp otherwise)
+  m.def("ema_update", [](torch::Tensor table, torch::Tensor host, double w, bool copy, c10::optional<torch::Tensor> counter,
+                         int64_t every, int64_t warmup_steps) {
+    TORCH_CHECK(!host.is_cuda() && host.is_contiguous() && host.scalar_type() == torch::kInt64 && host.numel() >= 8 &&
+                host.numel() % 8 == 0, "ema_update: host: the CPU int64 table from ema_table");
+    TORCH_CHECK(table.is_cuda() && table.is_contiguous() && table.scalar_type() == torch::kInt64 && table.numel() == host.numel(),
+                "ema_update: table: the CUDA int64 table from ema_table");
+    TORCH_CHECK(every >= 1 && warmup_steps >= 0, "ema_update: every must be >= 1 and warmup_steps >= 0, got ", every, " and ",
+                warmup_steps);
+    TORCH_CHECK(std::isfinite(w) && w >= 0.0 && w <= 1.0, "ema_update: w = 1 - decay must be in [0, 1], got ", w);
+    const int n = (int)(host.numel() / 8);
+    const b2::EmaEntry* rows = reinterpret_cast<const b2::EmaEntry*>(host.data_ptr<int64_t>());
+    for (int i = 0; i < n; ++i)
+      TORCH_CHECK(rows[i].ema != nullptr && rows[i].live != nullptr && rows[i].n >= 1, "ema_update: entry ", i, " is empty");
+    const long long n_vec = rows[n - 1].vec_begin + rows[n - 1].n_vec;
+    const long long n_scalar = rows[n - 1].scalar_begin + rows[n - 1].n - 4 * rows[n - 1].n_vec;
+    const long long* ctr = nullptr;
+    if (counter.has_value()) {
+      TORCH_CHECK(counter->is_cuda() && counter->scalar_type() == torch::kInt64 && counter->numel() == 1 &&
+                  counter->device() == table.device(), "ema_update: counter: int64 CUDA [1] on the table's device");
+      ctr = reinterpret_cast<const long long*>(counter->data_ptr<int64_t>());
+    }
+    c10::cuda::CUDAGuard guard(table.device());
+    ck_cuda(b2_ema_launch(reinterpret_cast<const b2::EmaEntry*>(table.data_ptr<int64_t>()), n, n_vec, n_scalar, (float)w,
+                          copy ? b2::EMA_COPY : b2::EMA_LERP, ctr, every, warmup_steps, cur_stream()),
+            "ema_update launch");
+  }, py::arg("table"), py::arg("host"), py::arg("w"), py::arg("copy") = false, py::arg("counter") = py::none(),
+     py::arg("every") = 1, py::arg("warmup_steps") = 0);
   // sgd_flat / sgd_flat_grouped (with group_map) with the scalars from the block: arguments as theirs otherwise
   m.def("sgd_flat_cap", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, c10::optional<torch::Tensor> group_map,
                            torch::Tensor block, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,

@@ -28,9 +28,13 @@ corrections on the device (csrc/flat_scalars.cuh), so a whole DDP step can be ca
 
 ``FlatLAMB`` and ``FlatLARS`` are the large-batch optimizers with a trust ratio per parameter tensor: per bucket two kernels
 (csrc/layerwise.cu) form every tensor's norms in a fixed order over a chunk table of the flat layout, then apply the update.
+
+``FlatEMA`` keeps an exponential moving average of the weights of any of them: one ``ema_update`` launch (csrc/ema.cu) over
+the parameter flats (or this rank's slices of them when sharded) and the fp32 buffers per update.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import struct
 from typing import List, Optional, Sequence
@@ -38,7 +42,7 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "FlatAdamW", "FlatLAMB", "FlatLARS", "LRSchedule", "adamw_scalars", "lamb_scalars", "exclude_1d",
+__all__ = ["FlatSGD", "FlatAdamW", "FlatLAMB", "FlatLARS", "FlatEMA", "LRSchedule", "adamw_scalars", "lamb_scalars", "exclude_1d",
            "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
@@ -525,6 +529,9 @@ class _FlatOptimizer:
     def step(self) -> None:
         """``optimizer.step()`` (train_dist.py:124) for every bucket, and -- with ``zero_grad=True`` -- the
         ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass."""
+        if getattr(self, "_ema_swapped", False):
+            raise RuntimeError(f"{type(self).__name__}.step() inside FlatEMA.average_parameters(): the parameters hold the "
+                               "EMA values there; step after the block")
         if self._shard_mode is not None:      # the buckets' exchanges applied the update already
             if not all(self._done):
                 raise RuntimeError(f"{type(self).__name__}(sharded=True).step(): this step's gradient buckets were not "
@@ -571,6 +578,9 @@ class _FlatOptimizer:
         all-reduce would run on): afterwards every rank holds the updated parameters of the whole bucket."""
         from .. import comm
 
+        if getattr(self, "_ema_swapped", False):
+            raise RuntimeError(f"{type(self).__name__}(sharded=True): a gradient exchange inside FlatEMA.average_parameters() "
+                               "would update the EMA values the parameters hold there; run backward after the block")
         if self._done[k]:
             raise RuntimeError(f"{type(self).__name__}(sharded=True): a gradient bucket was exchanged twice in one step, which "
                                "would apply its update twice; one average_gradients(model) goes with one step()")
@@ -1338,3 +1348,233 @@ class FlatLARS(_LayerwiseOptimizer):
 
     named_momentum = FlatSGD.named_momentum
     load_named_momentum = FlatSGD.load_named_momentum
+
+
+def check_ema_options(decay, every, warmup_steps) -> tuple:
+    """:class:`FlatEMA`'s rules: ``decay`` a finite number in [0, 1], ``every`` an int >= 1, ``warmup_steps`` an int >= 0.
+    Returns them as ``(float, int, int)``."""
+    if isinstance(decay, bool) or not isinstance(decay, (int, float)) or not math.isfinite(float(decay)) \
+            or not 0.0 <= float(decay) <= 1.0:
+        raise ValueError(f"FlatEMA: decay must be a finite number in [0, 1], got {decay!r}")
+    if isinstance(every, bool) or not isinstance(every, int) or every < 1:
+        raise ValueError(f"FlatEMA: every must be an int >= 1, got {every!r}")
+    if isinstance(warmup_steps, bool) or not isinstance(warmup_steps, int) or warmup_steps < 0:
+        raise ValueError(f"FlatEMA: warmup_steps must be an int >= 0, got {warmup_steps!r}")
+    return float(decay), int(every), int(warmup_steps)
+
+
+class FlatEMA:
+    """An exponential moving average of the weights of a model trained by a flat optimizer (:class:`FlatSGD`,
+    :class:`FlatAdamW`, :class:`FlatLAMB`, :class:`FlatLARS`), for evaluation and the final checkpoint: torchvision's
+    ``--model-ema``, timm's ``ModelEma``, ``AveragedModel(model, multi_avg_fn=get_ema_multi_avg_fn(decay), use_buffers=True)``.
+
+    ``ema = FlatEMA(optimizer, decay=0.9999, every=1, warmup_steps=0)`` copies the current parameters, and the floating-point
+    buffers of the model (BatchNorm running statistics), into EMA storage.  The model is the module inside the optimizer's
+    :class:`DistributedDataParallel`; an optimizer built on a plain module needs ``model=`` (that module, or a
+    :class:`DistributedDataParallel` around it), and ``ValueError`` says so.  Call :meth:`update`
+    after every ``optimizer.step()``.  With ``t`` the optimizer's ``steps`` after that step, the update
+
+    * does nothing unless ``t % every == 0``;
+    * copies the live values if ``t - every <= warmup_steps`` (the first update, as ``AveragedModel``'s ``n_averaged == 0``,
+      and torchvision's reset of the average during lr warmup);
+    * otherwise lerps: ``ema = lerp(ema, live, w)`` with ``w = fp32(1 - decay)``, ``1 - decay`` in fp64 as Python computes it
+      for ``torch._foreach_lerp_(..., 1 - decay)``, and torch's roundings: ``fma(w, p - e, e)`` for ``w < 0.5``, else
+      ``fma(-(p - e), 1 - w, p)``, subnormals kept.
+
+    fp32 buffers are averaged by the same rule.  Integer buffers (``num_batches_tracked``) are neither averaged nor swapped:
+    that is the one difference from ``AveragedModel(use_buffers=True)``, which averages them in integer arithmetic.  Buffers
+    are followed in place, so a buffer the model replaces by a new tensor is no longer followed.
+
+    On CUDA one launch of ``ema_update`` (csrc/ema.cu) updates the whole model per :meth:`update`: a table built here lists
+    every bucket's parameter flat (or this rank's slice of it when the optimizer is sharded) and every fp32 buffer.  With a
+    ``capturable=True`` optimizer the kernel reads the optimizer's device step counter and decides skip / copy / lerp itself,
+    so ``update()`` can sit in the CUDA graph of the step and replays follow ``every`` and ``warmup_steps``; otherwise the host
+    decides, launches nothing on a skipped step, and ``update()`` inside a capture raises ``RuntimeError``.  On CPU (gloo)
+    ``torch._foreach_copy_`` / ``torch._foreach_lerp_`` apply the same rule.
+
+    With ``sharded=True`` over several ranks a rank keeps the EMA of the slice of each bucket it owns (:meth:`shard_range` of
+    the optimizer, padding included), so the EMA costs 4/W bytes per parameter as the optimizer state does.  No
+    communication: the owned slice is the one this rank's own update wrote.
+
+    ``with ema.average_parameters():`` puts the EMA into the model's parameters and fp32 buffers and on exit restores the live
+    values bit for bit.  Sharded, it swaps the owned slices and all-gathers the parameter flats, on entry and on exit
+    (collective: every rank enters).  Inside the block ``update()``, ``optimizer.step()`` and, when sharded, the gradient
+    exchange of ``average_gradients`` / the DDP hooks raise ``RuntimeError`` before anything changes, and entering the block
+    during a CUDA-graph capture does too.  ``state_dict()`` and :meth:`named_ema` work there and give the EMA, which the
+    model holds inside the block.
+
+    ``decay``, ``every`` and ``warmup_steps`` are read-only.  ``state_dict()`` / ``load_state_dict()`` follow the optimizers'
+    rules (a shard loads only on its own rank of its own world size; a whole EMA loads into a sharded one as each rank's
+    slice) and refuse a state with other settings; :meth:`named_ema` / :meth:`load_named_ema` cross world sizes."""
+
+    def __init__(self, optimizer, decay: float = 0.9999, every: int = 1, warmup_steps: int = 0,
+                 model: Optional[nn.Module] = None):
+        self._decay, self._every, self._warmup = check_ema_options(decay, every, warmup_steps)
+        if not isinstance(optimizer, _FlatOptimizer):
+            raise ValueError(f"FlatEMA needs a flat optimizer (FlatSGD, FlatAdamW, FlatLAMB, FlatLARS), got "
+                             f"{type(optimizer).__name__}")
+        from ..parallel.ddp import DistributedDataParallel
+
+        opt = optimizer
+        self._kernel_path = opt.param_flats[0].is_cuda
+        if model is None:
+            if opt._engine is None:
+                raise ValueError("FlatEMA: the optimizer was built on a plain module; pass model= (that module) so that its "
+                                 "floating buffers are averaged too")
+            model = opt._engine.module
+        module = model.module if isinstance(model, DistributedDataParallel) else model
+        mine = {id(p) for p in module.parameters()}
+        if any(id(p) not in mine for gb in opt.buckets for p in gb.params):
+            raise ValueError("FlatEMA: model= is not the module the optimizer updates (it lacks some of its parameters)")
+        bufs = [(n, b) for n, b in module.named_buffers() if torch.is_floating_point(b)]
+        for n, b in bufs:
+            if self._kernel_path and (not b.is_cuda or b.dtype != torch.float32 or b.device != opt.param_flats[0].device):
+                raise ValueError(f"FlatEMA averages floating buffers in fp32 on the parameters' device; the buffer {n!r} is "
+                                 f"{b.dtype} on {b.device}")
+        self._opt = opt
+        self._swapped = False
+        self._w = 1.0 - self._decay                  # rounded once to fp32 by the kernel's binding, by torch on CPU
+        self._buf_names = [n for n, _ in bufs]
+        self._bufs = [b for _, b in bufs]
+        with torch.no_grad():
+            self.ema_flats: List[torch.Tensor] = [self._live(k).clone() for k in range(len(opt.buckets))]
+            self.ema_buffers: List[torch.Tensor] = [b.detach().clone() for b in self._bufs]
+        self._table = None
+        if self._kernel_path:
+            self._table = opt._kernel().ema_table(self.ema_flats + self.ema_buffers,
+                                                  [self._live(k) for k in range(len(opt.buckets))] + self._bufs)
+
+    decay = property(lambda self: self._decay, doc="The decay (read-only).")
+    every = property(lambda self: self._every, doc="Update every this many optimizer steps (read-only).")
+    warmup_steps = property(lambda self: self._warmup, doc="Copy instead of averaging up to this step (read-only).")
+
+    def _live(self, k: int) -> torch.Tensor:
+        """Bucket ``k``'s live parameters that this rank averages: the whole flat, or its owned slice of the padded flat."""
+        opt = self._opt
+        if opt._shard_mode is None:
+            return opt.param_flats[k]
+        per = opt._shards[k][2]
+        return opt._shards[k][3][opt._rank * per:(opt._rank + 1) * per]
+
+    def _ema_tensors(self) -> tuple:
+        """(EMA of every bucket, EMA of every buffer): the EMA storage, or inside :meth:`average_parameters` the model's own
+        parameter flats (owned slices when sharded) and buffers, which hold the EMA there."""
+        if self._swapped:
+            return [self._live(k) for k in range(len(self.ema_flats))], list(self._bufs)
+        return self.ema_flats, self.ema_buffers
+
+    def _refuse_inside(self, what: str) -> None:
+        if self._swapped:
+            raise RuntimeError(f"FlatEMA.{what} inside average_parameters(): the model holds the EMA values there")
+
+    @torch.no_grad()
+    def update(self) -> None:
+        """The EMA update after ``optimizer.step()`` (see the class): skip, copy or lerp, decided from the optimizer's
+        ``steps``.  One kernel launch on CUDA, none on a skipped step unless the optimizer is capturable."""
+        self._refuse_inside("update()")
+        opt = self._opt
+        if self._kernel_path and opt.capturable:
+            opt._kernel().ema_update(*self._table, self._w, counter=opt._cap_counter, every=self._every,
+                                     warmup_steps=self._warmup)
+            return
+        if self._kernel_path and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("FlatEMA.update() in a CUDA-graph capture needs a capturable=True optimizer: otherwise the "
+                               "host decides skip / copy / lerp, and the graph would replay the capture's decision")
+        t = opt.steps
+        if t % self._every:
+            return
+        copy = t - self._every <= self._warmup
+        if self._kernel_path:
+            opt._kernel().ema_update(*self._table, self._w, copy=copy)
+            return
+        emas = self.ema_flats + self.ema_buffers
+        lives = [self._live(k) for k in range(len(opt.buckets))] + self._bufs
+        if copy:
+            torch._foreach_copy_(emas, lives)
+        else:
+            torch._foreach_lerp_(emas, lives, self._w)
+
+    @torch.no_grad()
+    def _swap(self) -> None:
+        """Exchange the live values and the EMA (owned slices, then an all-gather of every parameter flat when sharded)."""
+        from .. import comm
+
+        opt = self._opt
+        for k, e in enumerate(self.ema_flats):
+            live = self._live(k)
+            tmp = live.clone()
+            live.copy_(e)
+            e.copy_(tmp)
+            if opt._shard_mode is not None:
+                comm.all_gather_into_tensor(opt._shards[k][3], live.clone(), group=opt._group)
+        for b, e in zip(self._bufs, self.ema_buffers):
+            tmp = b.clone()
+            b.copy_(e)
+            e.copy_(tmp)
+
+    @contextlib.contextmanager
+    def average_parameters(self):
+        """``with ema.average_parameters():`` evaluates the EMA model: the parameters and fp32 buffers hold the EMA inside
+        the block and the live values, bit for bit, after it.  Collective when the optimizer is sharded over several ranks.
+        ``RuntimeError`` when nested or entered during a CUDA-graph capture."""
+        self._refuse_inside("average_parameters()")
+        if self._kernel_path and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("FlatEMA.average_parameters() cannot be entered during a CUDA-graph capture")
+        self._swap()
+        self._swapped = self._opt._ema_swapped = True
+        try:
+            yield self
+        finally:
+            self._swap()
+            self._swapped = self._opt._ema_swapped = False
+
+    # ------------------------------------------------------------------ checkpointing
+    def _settings(self) -> dict:
+        return {"decay": self._decay, "every": self._every, "warmup_steps": self._warmup}
+
+    def state_dict(self) -> dict:
+        """The settings, the EMA flats (CPU copies; this rank's shards when sharded, with ``sharded`` / ``world`` / ``rank``)
+        and the fp32 buffers by name."""
+        flats, bufs = self._ema_tensors()
+        sd = dict(self._settings(), ema=[e.detach().cpu().clone() for e in flats],
+                  buffers={n: e.detach().cpu().clone() for n, e in zip(self._buf_names, bufs)})
+        sd.update(self._opt._shard_tags())
+        return sd
+
+    def _check_loadable(self, sd: dict, what: str) -> None:
+        self._refuse_inside(what)
+        saved = {k: sd.get(k) for k in self._settings()}
+        if saved != self._settings():
+            raise ValueError(f"FlatEMA.{what}: the state was written with {saved}, this EMA has {self._settings()}")
+
+    @torch.no_grad()
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict`.  ``ValueError`` (before anything is loaded) for other settings, other buffers, or a
+        shard of another rank or world size; ``RuntimeError`` inside :meth:`average_parameters`."""
+        self._check_loadable(sd, "load_state_dict()")
+        if sorted(sd["buffers"]) != sorted(self._buf_names):
+            raise ValueError(f"FlatEMA.load_state_dict: the state holds the buffers {sorted(sd['buffers'])}, this EMA "
+                             f"{sorted(self._buf_names)}")
+        self._opt._load_flats(sd, [(self.ema_flats, sd["ema"])], "EMA", "named_ema() / load_named_ema()")
+        for n, e in zip(self._buf_names, self.ema_buffers):
+            e.copy_(sd["buffers"][n])
+
+    def named_ema(self, model: nn.Module) -> dict:
+        """``{name: EMA tensor}`` (CPU copies) for every parameter and averaged buffer, the form that crosses world sizes and
+        sharded and unsharded runs (keys as in the module's ``state_dict()``).  Collective when sharded: every rank calls it
+        and gets the whole tensors."""
+        flats, bufs = self._ema_tensors()
+        out = self._opt._named(model, flats)
+        out.update({n: e.detach().cpu().clone() for n, e in zip(self._buf_names, bufs)})
+        return out
+
+    @torch.no_grad()
+    def load_named_ema(self, model: nn.Module, named: dict) -> int:
+        """Inverse of :meth:`named_ema`; returns how many tensors were restored.  Sharded, each rank keeps its slice."""
+        self._refuse_inside("load_named_ema()")
+        done = self._opt._load_named(model, named, self.ema_flats)
+        for n, e in zip(self._buf_names, self.ema_buffers):
+            if n in named:
+                e.copy_(named[n])
+                done += 1
+        return done

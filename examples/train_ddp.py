@@ -13,11 +13,14 @@ the tutorial's loop, on synthetic data.
                                                                   # is one replay of a captured CUDA graph
     python examples/train_ddp.py --accumulation-steps 4           # gradient accumulation: 4 micro-batches per step, the
                                                                   # first 3 backwards under model.no_sync()
+    python examples/train_ddp.py --ema-decay 0.99 --ema-every 2   # FlatEMA: an EMA of the weights, updated after every
+                                                                  # 2nd step, evaluated on a held-out batch at the end
 
 The loop is ``backward(); average_gradients(model); optimizer.step()`` either way; with ``--accumulation-steps k`` the k - 1
 backwards before the last run inside ``model.no_sync()`` on losses scaled by 1 / k.  With ``--sharded-optimizer`` the update
 happens inside ``average_gradients`` (during backward, bucket by bucket) and ``step()`` only counts the step; with fp32
-gradient buckets the parameters are bit for bit the same.  Prints ``Rank r, step s: loss`` for the last step."""
+gradient buckets the parameters are bit for bit the same.  Prints ``Rank r, step s: loss`` for the last step, and with
+``--ema-decay`` a second line per rank, ``Rank r, EMA model: held-out loss``, the loss of the EMA weights on a fixed batch."""
 import argparse
 import json
 import os
@@ -51,9 +54,9 @@ def batch(step, rank, dev, micro=0):
     return torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
 
 
-def train_step(model, optimizer, micro_batches):
+def train_step(model, optimizer, micro_batches, ema=None):
     """One optimizer step over ``micro_batches`` (a list of (x, y)): all but the last backward accumulate under no_sync(),
-    the last one exchanges the buckets.  Returns the last micro-batch's loss."""
+    the last one exchanges the buckets; then the EMA update, if any.  Returns the last micro-batch's loss."""
     k = len(micro_batches)
     for x, y in micro_batches[:-1]:
         with model.no_sync():
@@ -63,10 +66,12 @@ def train_step(model, optimizer, micro_batches):
     (loss / k).backward()
     dist.average_gradients(model)       # --sharded-optimizer: the parameters are updated when this returns
     optimizer.step()
+    if ema is not None:
+        ema.update()                    # a capturable optimizer: the kernel decides skip / copy / lerp from its step counter
     return loss
 
 
-def train_graphed(model, optimizer, rank, dev, steps, k, warmup=3):
+def train_graphed(model, optimizer, ema, rank, dev, steps, k, warmup=3):
     """--cuda-graph: ``warmup`` eager steps on a side stream (as torch requires before a capture), one step (all k
     micro-batches) captured, and every later step a ``copy_`` of its micro-batches into the static inputs and one replay.
     Returns the last step's loss."""
@@ -78,7 +83,7 @@ def train_graphed(model, optimizer, rank, dev, steps, k, warmup=3):
                 t.copy_(src)
 
     def step():
-        return train_step(model, optimizer, static)
+        return train_step(model, optimizer, static, ema)
 
     s = torch.cuda.Stream(dev)
     s.wait_stream(torch.cuda.current_stream(dev))
@@ -116,12 +121,15 @@ def run(rank, size):
     else:
         optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"], param_groups=groups,
                                  **cap)
+    ema = None
+    if CFG["ema_decay"] is not None:
+        ema = dist.FlatEMA(optimizer, decay=CFG["ema_decay"], every=CFG["ema_every"], warmup_steps=CFG["ema_warmup_steps"])
     loss = None
     if CFG["cuda_graph"]:
-        loss = train_graphed(model, optimizer, rank, dev, CFG["steps"], CFG["accumulation_steps"])
+        loss = train_graphed(model, optimizer, ema, rank, dev, CFG["steps"], CFG["accumulation_steps"])
     for step in range(0 if CFG["cuda_graph"] else CFG["steps"]):
         optimizer.zero_grad()
-        loss = train_step(model, optimizer, [batch(step, rank, dev, j) for j in range(CFG["accumulation_steps"])])
+        loss = train_step(model, optimizer, [batch(step, rank, dev, j) for j in range(CFG["accumulation_steps"])], ema)
     total = loss.detach().clone()
     dist.all_reduce(total)
     if CFG["optimizer"] in ("adamw", "lamb"):
@@ -130,6 +138,11 @@ def run(rank, size):
         state = f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}"
     print(f"Rank {rank}, step {CFG['steps']}: loss {float(loss.detach()):.6f} (mean over ranks {float(total) / size:.9f}), "
           + state)
+    if ema is not None:
+        x, y = batch(-1, rank, dev)     # a batch no step trains on
+        with ema.average_parameters(), torch.no_grad():
+            held_out = F.cross_entropy(model(x), y)
+        print(f"Rank {rank}, EMA model: held-out loss {float(held_out):.6f}")
 
 
 if __name__ == "__main__":
@@ -147,6 +160,11 @@ if __name__ == "__main__":
                     help="sgd / adamw on --backend b200: capturable=True, and every step after the warm-up one graph replay")
     ap.add_argument("--accumulation-steps", type=int, default=1,
                     help="micro-batches of 16 samples per rank and optimizer step (gradient accumulation with no_sync())")
+    ap.add_argument("--ema-decay", type=float, default=None,
+                    help="keep an exponential moving average of the weights (FlatEMA) with this decay")
+    ap.add_argument("--ema-every", type=int, default=1, help="with --ema-decay: update the EMA after every k-th step")
+    ap.add_argument("--ema-warmup-steps", type=int, default=0,
+                    help="with --ema-decay: copy the weights instead of averaging them up to this step")
     a = ap.parse_args()
     if a.accumulation_steps < 1:
         ap.error("--accumulation-steps must be at least 1")
@@ -156,5 +174,7 @@ if __name__ == "__main__":
         ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw; FlatLAMB and FlatLARS exclude them already")
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
                                                 optimizer=a.optimizer, no_decay=a.no_decay_bias_norm,
-                                                cuda_graph=a.cuda_graph, accumulation_steps=a.accumulation_steps))
+                                                cuda_graph=a.cuda_graph, accumulation_steps=a.accumulation_steps,
+                                                ema_decay=a.ema_decay, ema_every=a.ema_every,
+                                                ema_warmup_steps=a.ema_warmup_steps))
     dist.launch(run, size=a.size, backend=a.backend)
