@@ -104,20 +104,20 @@ class SyncBatchNormFunction(torch.autograd.Function):
         else:
             y, stats = _cpu_forward(x, weight, bias, running_mean, running_var, num_batches_tracked, momentum, eps, ex,
                                     comm_)
-        ctx.save_for_backward(x, weight, stats)
+        ctx.save_for_backward(x, weight, stats, bias)
         ctx.comm_, ctx.W = comm_, W
         ctx.tickets = tickets
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, stats = ctx.saved_tensors
+        x, weight, stats, bias = ctx.saved_tensors
         need_x, need_w, need_b = ctx.needs_input_grad[:3]
         if not _same_layout(dy, x):
             dy = torch.empty_like(x).copy_(dy)
         C = x.shape[1]
         gw = torch.empty_like(weight) if need_w and weight is not None else None
-        gb = torch.empty_like(weight) if need_b and weight is not None else None
+        gb = torch.empty_like(bias) if need_b and bias is not None else None
         dx = None
         if not (need_x or gw is not None or gb is not None):
             return (None,) * 10

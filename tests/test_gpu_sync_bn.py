@@ -16,14 +16,12 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 import dist_tuto.pth_b200 as b2
+import sync_bn_checks as S
 import test_gpu_collectives_emulated as CE
 import test_gpu_comm_emulated as E
 from dist_tuto.pth_b200.parallel.sync_bn import SyncBatchNormFunction, exchange_numel
 
 pytestmark = E.pytestmark
-C_BOUND = 3.0
-OUT_EPS = {torch.float32: 0.0, torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}
-OUT_SUB = {dt: torch.finfo(dt).tiny * torch.finfo(dt).eps for dt in OUT_EPS}   # subnormal spacing of the output
 SENT = -12345.0
 
 
@@ -64,14 +62,6 @@ def _sent_ok(big, n_front, what):
 def _bits(a, b):
     return a.shape == b.shape and torch.equal(a.contiguous().view(-1).view(torch.uint8).cpu(),
                                               b.contiguous().view(-1).view(torch.uint8).cpu())
-
-
-def _dims(x):
-    return [0] + list(range(2, x.dim()))
-
-
-def _b(x, v):
-    return v.view([1, -1] + [1] * (x.dim() - 2))
 
 
 CASES = [  # (shape, layouts)
@@ -138,38 +128,15 @@ def test_kernels_world_one_against_fp64(K, sms, dtype, pdtype):
                 out = _run_kernels(K, x, w, b, rm, rv, dy, mb)
                 _sent_ok(rm_big, C, "running_mean")
                 _sent_ok(rv_big, C, "running_var")
-                # fp64 reference
-                xd, dyd, wd, bd = x.double(), dy.double(), w.double(), b.double()
-                N = x.numel() // C
-                mean = xd.mean(_dims(x))
-                var = xd.var(_dims(x), unbiased=False)
-                invstd = 1.0 / torch.sqrt(var + 1e-5)
-                k1, k0 = wd * invstd, bd - mean * wd * invstd
-                yref = xd * _b(x, k1) + _b(x, k0)
-                bound = C_BOUND * 2.0 ** -24 * (xd.abs() * _b(x, k1.abs()) + _b(x, k0.abs())) + OUT_EPS[dtype] * yref.abs() + OUT_SUB[dtype]
+                # fp64 reference and the kernels' bounds (tests/sync_bn_checks.py)
+                fwd = S.forward_ref(x, w, b, rm0, rv0, 0.1)
+                bwd = S.backward_ref(x, dy, fwd, w)
                 what = (str(dtype), pdtype, shape, cl, mb)
-                assert bool(((out["y"].double() - yref).abs() <= bound).all()), ("y", what)
-                assert torch.allclose(out["stats"][:C], mean, rtol=1e-12, atol=1e-12), ("mean", what)
-                assert torch.allclose(out["stats"][C:2 * C], invstd, rtol=1e-9), ("invstd", what)
-                pe = 2.0 ** -23 if pd == torch.float32 else OUT_EPS[pd] * 2
-                rm_ref = 0.9 * rm0.double() + 0.1 * mean
-                rv_ref = 0.9 * rv0.double() + 0.1 * var * N / (N - 1)
-                assert torch.allclose(rm.double(), rm_ref, rtol=pe, atol=pe), ("running_mean", what)
-                assert torch.allclose(rv.double(), rv_ref, rtol=pe, atol=pe), ("running_var", what)
-                xmu = xd - _b(x, mean)
-                sdy, sdx = dyd.sum(_dims(x)), (dyd * xmu).sum(_dims(x))
-                scale = dyd.abs().sum(_dims(x)) * (1 + xmu.abs().amax(_dims(x)))
-                assert bool(((out["gb"].double() - sdy).abs() <= pe * sdy.abs() + 1e-12 * scale).all()), ("grad_bias", what)
-                gwr = sdx * invstd
-                assert bool(((out["gw"].double() - gwr).abs() <= pe * gwr.abs() + 1e-12 * scale * invstd).all()), \
-                    ("grad_weight", what)
-                ka = wd * invstd
-                kb = -ka * invstd * invstd * sdx / N
-                kc = -ka * sdy / N - kb * mean
-                dxr = dyd * _b(x, ka) + xd * _b(x, kb) + _b(x, kc)
-                bound = C_BOUND * 2.0 ** -24 * (dyd.abs() * _b(x, ka.abs()) + xd.abs() * _b(x, kb.abs()) + _b(x, kc.abs())) \
-                    + OUT_EPS[dtype] * dxr.abs() + OUT_SUB[dtype] + 2.0 ** -22 * (_b(x, (kb * mean).abs()))
-                assert bool(((out["dx"].double() - dxr).abs() <= bound).all()), ("dx", what)
+                ratios = S.forward_checks(dict(y=out["y"], mean=out["stats"][:C], invstd=out["stats"][C:2 * C], rm=rm, rv=rv),
+                                          x, fwd, dtype, pd)
+                ratios.update(S.backward_checks(out, x, dy, fwd, bwd, dtype, pd))
+                assert set(ratios) == {"y", "mean", "invstd", "rm", "rv", "dx", "gw", "gb"}
+                assert not S.failures(ratios), (what, ratios)
                 rm.copy_(rm0)
                 rv.copy_(rv0)
                 again = _run_kernels(K, x, w, b, rm, rv, dy, mb)
@@ -212,8 +179,8 @@ def _emulated_case(worlds, sizes, C, spatial, dtype, cl, momentum, seed):
     xg = torch.cat([x.detach().double() for x in xs])
     dyg = torch.cat([d.double() for d in dys])
     N = xg.numel() // C
-    mean = xg.mean(_dims(xg))
-    var = xg.var(_dims(xg), unbiased=False)
+    mean = xg.mean(S.dims(xg))
+    var = xg.var(S.dims(xg), unbiased=False)
     assert int(stats[0][2 * C]) == N
     assert torch.allclose(stats[0][:C], mean, rtol=1e-12, atol=1e-12)
     assert torch.allclose(stats[0][C:2 * C], 1 / torch.sqrt(var + 1e-5), rtol=1e-9)
@@ -224,11 +191,18 @@ def _emulated_case(worlds, sizes, C, spatial, dtype, cl, momentum, seed):
     wr, br = w.detach().double().requires_grad_(True), b.detach().double().requires_grad_(True)
     yr = F.batch_norm(xr, None, None, wr, br, True, 0.0, 1e-5)
     gx, gw, gb = torch.autograd.grad(yr, [xr, wr, br], dyg)
-    tol = 1e-5 if dtype == torch.float32 else 2e-2
+    # y and dx of every rank within the world-1 bounds of the global batch; each rank's parameter gradients its local sums
+    fwd = S.forward_ref(xg, w, b)
+    bwd = S.backward_ref(xg, dyg, fwd, w)
+    torch.testing.assert_close(bwd["dx"], gx.cpu(), rtol=1e-10, atol=1e-12)
     off = 0
     for r, n in enumerate(sizes):
-        torch.testing.assert_close(ys[r].double(), yr[off:off + n].detach(), rtol=tol, atol=tol)
-        torch.testing.assert_close(grads[r][0].double(), gx[off:off + n], rtol=tol, atol=tol)
+        sl = slice(off, off + n)
+        local = S.grad_sums(xs[r], dys[r], fwd["mean"], fwd["invstd"])
+        ratios = dict(y=S.check_y(ys[r], xs[r], dict(fwd, y=fwd["y"][sl]), dtype))
+        ratios.update(S.backward_checks(dict(dx=grads[r][0], gw=grads[r][1], gb=grads[r][2]), xs[r], dys[r], fwd,
+                                        dict(bwd, dx=bwd["dx"][sl]), dtype, torch.float32, local))
+        assert not S.failures(ratios), (r, sizes, str(dtype), ratios)
         off += n
     torch.testing.assert_close(sum(gr[1].double() for gr in grads), gw, rtol=1e-5, atol=1e-4)
     torch.testing.assert_close(sum(gr[2].double() for gr in grads), gb, rtol=1e-5, atol=1e-4)
