@@ -18,6 +18,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
     FlatAdamW (one-launch AdamW over flat buffers)      ops/optim.py
     FlatLAMB FlatLARS (per-tensor trust ratios)         ops/optim.py
     FlatEMA (EMA of the weights, one launch per update) ops/optim.py
+    GradScaler support (fp16 loss scaling, in-kernel)   ops/optim.py
     run / train / TrainConfig                           train.py
     evaluate (test loss / accuracy, sharded over ranks) ops/convnet_eval.py
     partition_eval_dataset default_eval_dataset         data.py

@@ -76,21 +76,23 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const SignalPadsH* sig, float
 int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const long long* steps, float* out, long long n,
                                cudaStream_t stream);
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
-                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream);
+                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, const float* grad_scale,
+                       cudaStream_t stream);
 int b2_sharded_sgd_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* momentum,
                           size_t n_vec, float lr, float mu, float wd, int nesterov, float scale, int zero_grad, int rank,
                           int world, int max_blocks, cudaStream_t stream);
 int b2_adamw_flat_launch(float* p, float* m, float* v, float* g, size_t n, const b2::AdamwScalars* s, int zero_grad,
-                         float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream);
+                         float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, const float* grad_scale,
+                         cudaStream_t stream);
 int b2_sharded_adamw_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
                             float* exp_avg_sq, size_t n_vec, const b2::AdamwScalars* s, float scale, int zero_grad, int rank,
                             int world, int max_blocks, cudaStream_t stream);
 int b2_sgd_flat_grouped_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::SgdGroups* gs,
                                int n_groups, float mu, int zero_grad, int nesterov, float max_norm, const double* sqnorms,
-                               int n_buckets, float* grad_norm_out, cudaStream_t stream);
+                               int n_buckets, float* grad_norm_out, const float* grad_scale, cudaStream_t stream);
 int b2_adamw_flat_grouped_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::AdamwScalars* s,
                                  const b2::AdamwGroups* gs, int n_groups, int zero_grad, float max_norm, const double* sqnorms,
-                                 int n_buckets, float* grad_norm_out, cudaStream_t stream);
+                                 int n_buckets, float* grad_norm_out, const float* grad_scale, cudaStream_t stream);
 int b2_sharded_sgd_grouped_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig,
                                   float* momentum, const uint8_t* map, const b2::SgdGroups* gs, int n_groups, size_t n_vec, float mu,
                                   int nesterov, float scale, int zero_grad, int rank, int world, int max_blocks,
@@ -101,13 +103,13 @@ int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerP
                                     int world, int max_blocks, cudaStream_t stream);
 int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
 int b2_flat_scalars_launch(const b2::FlatHyper* table, unsigned long long* counter, b2::FlatScalars* block, int advance,
-                           cudaStream_t stream);
+                           const float* found_inf, cudaStream_t stream);
 int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk, float mu,
                            int zero_grad, int nesterov, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
-                           cudaStream_t stream);
+                           const float* grad_scale, const float* found_inf, cudaStream_t stream);
 int b2_adamw_flat_cap_launch(float* p, float* m, float* v, float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk,
                              int zero_grad, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
-                             cudaStream_t stream);
+                             const float* grad_scale, const float* found_inf, cudaStream_t stream);
 int b2_sharded_sgd_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* momentum,
                               const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float mu, int nesterov, float scale,
                               int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream);
@@ -117,7 +119,8 @@ int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs*
 int b2_ema_launch(const b2::EmaEntry* table, int n_entries, long long n_vec, long long n_scalar, float w, int mode,
                   const long long* counter, long long every, long long warmup, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
-int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream);
+int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, const float* grad_scale,
+                          cudaStream_t stream);
 size_t b2_clip_ws_floats(size_t n_elems);
 int b2_bn_launch(int kind, int dtype, int vec, int cl, long long M, long long L, int max_blocks, const b2::bn::Args* args,
                  unsigned int* grid_out, cudaStream_t stream);
@@ -232,6 +235,14 @@ float* grad_norm_ptr(const c10::optional<torch::Tensor>& t, const char* what) {
   TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->numel() >= 1, what, ": grad_norm_out: fp32 CUDA [1]");
   return t->data_ptr<float>();
 }
+// GradScaler's grad_scale or found_inf (fp16 loss scaling, csrc/sgd_device.cuh): an fp32 CUDA scalar on the device of `like`,
+// or null when absent
+const float* amp_scalar_ptr(const c10::optional<torch::Tensor>& t, const torch::Tensor& like, const char* what, const char* name) {
+  if (!t.has_value()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->device() == like.device() && t->scalar_type() == torch::kFloat32 && t->numel() == 1, what, ": ",
+              name, ": an fp32 CUDA tensor of one element on the device of the buffers");
+  return t->data_ptr<float>();
+}
 
 // One AdamW update's scalars (csrc/adamw.h), computed by the host in fp64 (ops/optim.py adamw_scalars): (1 - lr*wd,
 // 1 - beta1, beta2, 1 - beta2, lr / bc1, sqrt(bc2), eps), each rounded once to fp32 here.
@@ -297,7 +308,8 @@ py::tuple layerwise_table(const std::vector<int64_t>& offsets, const std::vector
 b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, const std::vector<torch::Tensor*>& states,
                           const torch::Tensor& table, int64_t n_chunks, torch::Tensor& partials, torch::Tensor& tickets,
                           torch::Tensor& sums, torch::Tensor& ratios, bool zero_grad, const py::object& max_grad_norm,
-                          const c10::optional<torch::Tensor>& sqnorms, const c10::optional<torch::Tensor>& grad_norm_out) {
+                          const c10::optional<torch::Tensor>& sqnorms, const c10::optional<torch::Tensor>& grad_norm_out,
+                          const c10::optional<torch::Tensor>& grad_scale) {
   std::vector<const torch::Tensor*> flats = {&p, &g};
   for (torch::Tensor* t : states) flats.push_back(t);
   for (const torch::Tensor* t : flats) {
@@ -337,6 +349,7 @@ b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, 
     a.n_buckets = (int)sqnorms->numel();
   }
   a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
+  a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
   return a;
 }
 
@@ -969,7 +982,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("num_batches_tracked"), py::arg("grad_weight"), py::arg("grad_bias"), py::arg("momentum"), py::arg("eps"),
         py::arg("max_blocks"), "one SyncBatchNorm kernel (csrc/batchnorm.cu); parallel/sync_bn.py drives them");
   m.def("grad_sqnorm_workspace_numel", [] { return b2_grad_sqnorm_ws_floats(); });
-  m.def("grad_sqnorm", [](torch::Tensor g, torch::Tensor sqnorms, int k, torch::Tensor workspace) {
+  m.def("grad_sqnorm", [](torch::Tensor g, torch::Tensor sqnorms, int k, torch::Tensor workspace,
+                          c10::optional<torch::Tensor> grad_scale) {
     // sqnorms[k] = the sum of squares of g (fp32 per thread and CTA, fp64 across the CTAs in CTA order), for sgd_flat's clipping
     check_cuda_contig(g, "g"); check_cuda_contig(sqnorms, "sqnorms"); check_cuda_contig(workspace, "workspace");
     TORCH_CHECK(g.scalar_type() == torch::kFloat32 && (uintptr_t)g.data_ptr() % 16 == 0, "grad_sqnorm: g: 16-byte aligned fp32");
@@ -977,12 +991,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(workspace.scalar_type() == torch::kFloat32 && workspace.numel() >= b2_grad_sqnorm_ws_floats(),
                 "grad_sqnorm: workspace: fp32 [grad_sqnorm_workspace_numel()], zero before its first use");
     c10::cuda::CUDAGuard guard(g.device());
+    const float* gs = amp_scalar_ptr(grad_scale, g, "grad_sqnorm", "grad_scale");
     ck_cuda(b2_grad_sqnorm_launch(g.data_ptr<float>(), (size_t)g.numel(), workspace.data_ptr<float>(), sqnorms.data_ptr<double>(), k,
-                                  cur_stream()), "grad_sqnorm launch");
-  }, py::arg("g"), py::arg("sqnorms"), py::arg("k"), py::arg("workspace"));
+                                  gs, cur_stream()), "grad_sqnorm launch");
+  }, py::arg("g"), py::arg("sqnorms"), py::arg("k"), py::arg("workspace"), py::arg("grad_scale") = py::none());
   m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad,
                        bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
-                       c10::optional<torch::Tensor> grad_norm_out) {
+                       c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
     TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat: nesterov needs a nonzero momentum");
     const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat");
     const double* sq = nullptr;
@@ -999,14 +1014,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel());
     TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0, "16-byte aligned buffers");
     ck_cuda(b2_sgd_flat_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), (float)lr,
-                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn,
+                               amp_scalar_ptr(grad_scale, p, "sgd_flat", "grad_scale"), cur_stream()),
             "sgd_flat launch");
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
      py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none());
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
   m.def("adamw_flat", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
                          std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
-                         c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                         c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                         c10::optional<torch::Tensor> grad_scale) {
     // FlatAdamW's update of one fp32 bucket (csrc/adamw.cu); with max_grad_norm, g is first scaled by the clip coefficient of
     // the norm of grad_sqnorm's per-bucket sums
     const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat");
@@ -1029,10 +1046,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_adamw_flat_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
-                                 (size_t)p.numel(), &sc, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+                                 (size_t)p.numel(), &sc, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
+                                 amp_scalar_ptr(grad_scale, p, "adamw_flat", "grad_scale"), cur_stream()),
             "adamw_flat launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
-     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
+     py::arg("grad_scale") = py::none());
   m.def("max_param_groups", [] { return b2::kMaxGroups; }, "the most parameter groups the grouped optimizer kernels take");
   // Capturable FlatSGD / FlatAdamW (csrc/flat_scalars.cuh): the layout of the scalar block in fp32 words and the byte sizes
   // of the block and the table
@@ -1086,15 +1105,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       std::memcpy(staged.data_ptr<uint8_t>() + nh, &s, sizeof(s));
       counter.view(torch::kUInt8).copy_(staged.narrow(0, nh, 8), /*non_blocking=*/true);
     }
-    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, 0, cur_stream()), "flat_scalars_sync launch");
+    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, 0, nullptr, cur_stream()), "flat_scalars_sync launch");
   }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("lrs"), py::arg("weight_decays"), py::arg("beta1") = 0.0,
      py::arg("beta2") = 0.0, py::arg("eps") = 0.0, py::arg("schedule") = py::none(), py::arg("steps") = py::none());
-  // counter += 1 and the block of the next update, in one single-CTA launch (advance = false: the block only)
-  m.def("flat_scalars_advance", [](torch::Tensor table, torch::Tensor counter, torch::Tensor block, bool advance) {
+  // counter += 1 and the block of the next update, in one single-CTA launch (advance = false: the block only).  found_inf
+  // (GradScaler's, fp32 CUDA [1]): the gated advance, which leaves counter and block untouched when *found_inf != 0
+  m.def("flat_scalars_advance", [](torch::Tensor table, torch::Tensor counter, torch::Tensor block, bool advance,
+                                   c10::optional<torch::Tensor> found_inf) {
     const FlatState st = flat_state(table, counter, block, "flat_scalars_advance");
+    const float* fi = amp_scalar_ptr(found_inf, counter, "flat_scalars_advance", "found_inf");
+    TORCH_CHECK(fi == nullptr || advance, "flat_scalars_advance: found_inf gates an advance; it needs advance=True");
     c10::cuda::CUDAGuard guard(counter.device());
-    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, advance ? 1 : 0, cur_stream()), "flat_scalars_advance launch");
-  }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("advance") = true);
+    ck_cuda(b2_flat_scalars_launch(st.table, st.counter, st.block, advance ? 1 : 0, fi, cur_stream()), "flat_scalars_advance launch");
+  }, py::arg("table"), py::arg("counter"), py::arg("block"), py::arg("advance") = true, py::arg("found_inf") = py::none());
   // FlatEMA (csrc/ema.h): the entry table of (EMA array, live array) pairs, as (device table, host table); int64 rows of 8 words
   m.def("ema_table", [](const std::vector<torch::Tensor>& emas, const std::vector<torch::Tensor>& lives) {
     TORCH_CHECK(!emas.empty() && emas.size() == lives.size() && emas.size() < (size_t)INT32_MAX,
@@ -1162,7 +1185,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // sgd_flat / sgd_flat_grouped (with group_map) with the scalars from the block: arguments as theirs otherwise
   m.def("sgd_flat_cap", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, c10::optional<torch::Tensor> group_map,
                            torch::Tensor block, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
-                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                           c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
     TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_cap: nesterov needs a nonzero momentum");
     const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat_cap");
     const double* sq = nullptr;
@@ -1181,17 +1205,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "sgd_flat_cap");
     const b2::FlatScalars* blk = flat_block(block, p, "sgd_flat_cap");
+    const float* gsc = amp_scalar_ptr(grad_scale, p, "sgd_flat_cap", "grad_scale");
+    const float* fi = amp_scalar_ptr(found_inf, p, "sgd_flat_cap", "found_inf");
+    TORCH_CHECK(fi != nullptr || gsc == nullptr, "sgd_flat_cap: grad_scale comes with found_inf (GradScaler sets both)");
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_sgd_flat_cap_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), map, blk,
-                                   (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+                                   (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, gsc, fi, cur_stream()),
             "sgd_flat_cap launch");
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("block"), py::arg("mu"), py::arg("zero_grad"),
      py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none());
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
   // adamw_flat / adamw_flat_grouped (with group_map) with the scalars from the block
   m.def("adamw_flat_cap", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
                              c10::optional<torch::Tensor> group_map, torch::Tensor block, bool zero_grad, py::object max_grad_norm,
-                             c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                             c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                             c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
     const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat_cap");
     const double* sq = nullptr;
     int n_buckets = 0;
@@ -1209,13 +1237,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "adamw_flat_cap");
     const b2::FlatScalars* blk = flat_block(block, p, "adamw_flat_cap");
+    const float* gsc = amp_scalar_ptr(grad_scale, p, "adamw_flat_cap", "grad_scale");
+    const float* fi = amp_scalar_ptr(found_inf, p, "adamw_flat_cap", "found_inf");
+    TORCH_CHECK(fi != nullptr || gsc == nullptr, "adamw_flat_cap: grad_scale comes with found_inf (GradScaler sets both)");
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_adamw_flat_cap_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
-                                     (size_t)p.numel(), map, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+                                     (size_t)p.numel(), map, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, gsc, fi, cur_stream()),
             "adamw_flat_cap launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("block"),
      py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none());
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
   // sharded_sgd / sharded_sgd_grouped (with group_map: this rank's ids) with the scalars from the block
   m.def("sharded_sgd_cap", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
                               std::vector<unsigned long long> sigs, torch::Tensor momentum, c10::optional<torch::Tensor> group_map,
@@ -1274,7 +1305,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("world"), py::arg("max_blocks") = 0);
   m.def("sgd_flat_grouped", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, torch::Tensor group_map, std::vector<double> lrs,
                                std::vector<double> weight_decays, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
-                               c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                               c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                               c10::optional<torch::Tensor> grad_scale) {
     // sgd_flat with parameter groups (csrc/sgd.cu): parameter vector i takes lrs / weight_decays of group group_map[i]
     TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_grouped: nesterov needs a nonzero momentum");
     for (double wd : weight_decays) TORCH_CHECK(wd >= 0.0, "sgd_flat_grouped: weight_decay must be >= 0, got ", wd);
@@ -1300,15 +1332,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_sgd_flat_grouped_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(),
                                        group_map.data_ptr<uint8_t>(), &gs, n_groups, (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0,
-                                       max_norm, sq, n_buckets, gn, cur_stream()),
+                                       max_norm, sq, n_buckets, gn, amp_scalar_ptr(grad_scale, p, "sgd_flat_grouped", "grad_scale"),
+                                       cur_stream()),
             "sgd_flat_grouped launch");
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"),
      py::arg("zero_grad"), py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none());
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
   m.def("adamw_flat_grouped", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
                                  torch::Tensor group_map, std::vector<double> scalars, std::vector<double> decays,
                                  std::vector<double> step_sizes, bool zero_grad, py::object max_grad_norm,
-                                 c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                                 c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                 c10::optional<torch::Tensor> grad_scale) {
     // adamw_flat with parameter groups (csrc/adamw.cu): `scalars` as adamw_flat's (their decay and step_size are not used),
     // decays / step_sizes: 1 - lr_g*wd_g and lr_g / (1 - beta1^t) of every group, fp64, each rounded once to fp32 here
     const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat_grouped");
@@ -1334,18 +1368,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_adamw_flat_grouped_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
                                          g.data_ptr<float>(), (size_t)p.numel(), group_map.data_ptr<uint8_t>(), &sc, &gs, n_groups,
-                                         zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, cur_stream()),
+                                         zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
+                                         amp_scalar_ptr(grad_scale, p, "adamw_flat_grouped", "grad_scale"), cur_stream()),
             "adamw_flat_grouped launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("scalars"),
      py::arg("decays"), py::arg("step_sizes"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
-     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
   m.def("layerwise_chunk_elems", [] { return (int64_t)b2::kLwChunk; }, "the largest chunk of a layer-wise chunk table");
   m.def("layerwise_table", &layerwise_table, py::arg("offsets"), py::arg("numels"), py::arg("adapt"), py::arg("n"),
         py::arg("device"), "FlatLAMB / FlatLARS: (the chunk table of one bucket on `device`, its number of chunks)");
   m.def("lamb_flat", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g, torch::Tensor table,
                         int64_t n_chunks, torch::Tensor partials, torch::Tensor tickets, torch::Tensor sums, torch::Tensor ratios,
                         std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
-                        c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                        c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                        c10::optional<torch::Tensor> grad_scale) {
     // FlatLAMB's update of one fp32 bucket (csrc/layerwise.cu).  scalars (fp64, each rounded once to fp32 here):
     // (1 - beta1, beta2, 1 - beta2, sqrt(1 - beta2^t), eps, 1 / (1 - beta1^t), lr, weight_decay)
     TORCH_CHECK(scalars.size() == 8, "lamb_flat: scalars: (1 - beta1, beta2, 1 - beta2, sqrt(bc2), eps, 1 / bc1, lr, "
@@ -1353,25 +1389,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     for (double x : scalars) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), "lamb_flat: scalars must be finite in fp32");
     TORCH_CHECK((float)scalars[3] > 0.f && scalars[4] >= 0.0, "lamb_flat: sqrt(bc2) must be > 0 (update t >= 1) and eps >= 0");
     b2::LwArgs a = layerwise_args("lamb_flat", p, g, {&exp_avg, &exp_avg_sq}, table, n_chunks, partials, tickets, sums, ratios,
-                                  zero_grad, max_grad_norm, sqnorms, grad_norm_out);
+                                  zero_grad, max_grad_norm, sqnorms, grad_norm_out, grad_scale);
     a.w1 = (float)scalars[0]; a.beta2 = (float)scalars[1]; a.c2 = (float)scalars[2]; a.sbc2 = (float)scalars[3];
     a.eps = (float)scalars[4]; a.rbc1 = (float)scalars[5]; a.lr = (float)scalars[6]; a.wd = (float)scalars[7];
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_layerwise_launch(1, &a, cur_stream()), "lamb_flat launch");
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("table"), py::arg("n_chunks"),
      py::arg("partials"), py::arg("tickets"), py::arg("sums"), py::arg("ratios"), py::arg("scalars"), py::arg("zero_grad"),
-     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
+     py::arg("grad_scale") = py::none());
   m.def("lars_flat", [](torch::Tensor p, torch::Tensor momentum_buf, torch::Tensor g, torch::Tensor table, int64_t n_chunks,
                         torch::Tensor partials, torch::Tensor tickets, torch::Tensor sums, torch::Tensor ratios, double lr,
                         double momentum, double weight_decay, double trust_coefficient, double eps, bool nesterov, bool zero_grad,
-                        py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out) {
+                        py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                        c10::optional<torch::Tensor> grad_scale) {
     // FlatLARS's update of one fp32 bucket (csrc/layerwise.cu)
     check_sgd_options(weight_decay, nesterov, momentum, "lars_flat");
     TORCH_CHECK(std::isfinite(lr) && std::isfinite(momentum) && std::isfinite(weight_decay) && trust_coefficient > 0.0 &&
                 std::isfinite(trust_coefficient) && eps >= 0.0 && std::isfinite(eps),
                 "lars_flat: lr, momentum and weight_decay finite, trust_coefficient > 0 and eps >= 0 finite");
     b2::LwArgs a = layerwise_args("lars_flat", p, g, {&momentum_buf}, table, n_chunks, partials, tickets, sums, ratios, zero_grad,
-                                  max_grad_norm, sqnorms, grad_norm_out);
+                                  max_grad_norm, sqnorms, grad_norm_out, grad_scale);
     a.lr = (float)lr; a.mu = (float)momentum; a.wd = (float)weight_decay; a.nesterov = nesterov ? 1 : 0;
     a.eta64 = trust_coefficient; a.wd64 = weight_decay; a.eps64 = eps;
     c10::cuda::CUDAGuard guard(p.device());
@@ -1379,7 +1417,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("p"), py::arg("momentum_buffer"), py::arg("g"), py::arg("table"), py::arg("n_chunks"), py::arg("partials"),
      py::arg("tickets"), py::arg("sums"), py::arg("ratios"), py::arg("lr"), py::arg("momentum"), py::arg("weight_decay"),
      py::arg("trust_coefficient"), py::arg("eps"), py::arg("nesterov"), py::arg("zero_grad"),
-     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none());
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
+     py::arg("grad_scale") = py::none());
   // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instance): as sharded_sgd, with this rank's
   // exp_avg / exp_avg_sq shards in place of the momentum shard.
   m.def("sharded_adamw", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,

@@ -5,9 +5,16 @@
 namespace b2 {
 
 // advance = 1: counter += 1, then the block of the update run at the new count; advance = 0: the block of the update run at
-// the current count.  The only writer of the counter and the block while it runs.
+// the current count.  The only writer of the counter and the block while it runs.  kGated: the advance after a step
+// GradScaler may have skipped; with *found_inf != 0 the counter and the block stay as they are, so the skipped step counts
+// for neither the schedule nor the bias corrections.
+template <bool kGated>
 __global__ void __launch_bounds__(kMaxGroups) flat_scalars_kernel(const FlatHyper* __restrict__ h, unsigned long long* counter,
-                                                                  FlatScalars* __restrict__ out, int advance) {
+                                                                  FlatScalars* __restrict__ out, int advance,
+                                                                  const float* found_inf) {
+  if constexpr (kGated) {
+    if (__ldg(found_inf) != 0.f) return;
+  }
   __shared__ unsigned long long s_step;
   if (threadIdx.x == 0) s_step = *counter + (unsigned long long)advance;
   __syncthreads();
@@ -44,10 +51,15 @@ __global__ void __launch_bounds__(kMaxGroups) flat_scalars_kernel(const FlatHype
 
 extern "C" {
 
+// found_inf (fp32 on the device, or null): the gated advance; it needs advance != 0.
 int b2_flat_scalars_launch(const b2::FlatHyper* table, unsigned long long* counter, b2::FlatScalars* block, int advance,
-                           cudaStream_t stream) {
+                           const float* found_inf, cudaStream_t stream) {
   if (table == nullptr || counter == nullptr || block == nullptr) return (int)cudaErrorInvalidValue;
-  b2::flat_scalars_kernel<<<1, b2::kMaxGroups, 0, stream>>>(table, counter, block, advance ? 1 : 0);
+  if (found_inf != nullptr && !advance) return (int)cudaErrorInvalidValue;
+  if (found_inf != nullptr)
+    b2::flat_scalars_kernel<true><<<1, b2::kMaxGroups, 0, stream>>>(table, counter, block, 1, found_inf);
+  else
+    b2::flat_scalars_kernel<false><<<1, b2::kMaxGroups, 0, stream>>>(table, counter, block, advance ? 1 : 0, nullptr);
   return (int)cudaGetLastError();
 }
 

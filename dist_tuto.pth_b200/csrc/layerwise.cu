@@ -34,13 +34,15 @@ __device__ __forceinline__ float4 scale4(float4 g, float c) {
   return make_float4(__fmul_rn(g.x, c), __fmul_rn(g.y, c), __fmul_rn(g.z, c), __fmul_rn(g.w, c));
 }
 
-template <bool kLamb, bool kClip>
+// kScaled: every gradient is read as g * amp_inv_scale(a.grad_scale) (sgd_device.cuh), before the clip coefficient.
+template <bool kLamb, bool kClip, bool kScaled>
 __global__ void __launch_bounds__(kLwThreads) layerwise_norms_kernel(const LwArgs a) {
   __shared__ float2 s_warp[kLwThreads / 32];
   __shared__ float2 s_stage[kLwThreads];
   __shared__ int s_last;
   float c = 1.f;
   if constexpr (kClip) c = lw_clip_coef(a, true);
+  const float inv = kScaled ? amp_inv_scale(a.grad_scale) : 1.f;
   const long long* chunks = a.table;
   const long long* tens = a.table + (size_t)a.n_chunks * kLwRow;
   for (int ch = blockIdx.x; ch < a.n_chunks; ch += gridDim.x) {
@@ -54,6 +56,7 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_norms_kernel(const LwArg
     for (int i = threadIdx.x; i < nv; i += kLwThreads) {
       const float4 pv = reinterpret_cast<const float4*>(a.p)[v0 + i];
       float4 gv = reinterpret_cast<const float4*>(a.g)[v0 + i];
+      if constexpr (kScaled) gv = amp_unscale4(gv, inv);
       if constexpr (kClip) gv = scale4(gv, c);
       sp = fmaf(pv.x, pv.x, sp); sp = fmaf(pv.y, pv.y, sp); sp = fmaf(pv.z, pv.z, sp); sp = fmaf(pv.w, pv.w, sp);
       if constexpr (kLamb) {
@@ -75,7 +78,8 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_norms_kernel(const LwArg
     if (threadIdx.x < tail) {                  // a tensor's last < 4 elements: threads 0..2, one each
       const size_t e = (size_t)start + (size_t)nv * 4 + threadIdx.x;
       const float pe = a.p[e];
-      const float ge = kClip ? __fmul_rn(a.g[e], c) : a.g[e];
+      const float gl = kScaled ? amp_unscale(a.g[e], inv) : a.g[e];
+      const float ge = kClip ? __fmul_rn(gl, c) : gl;
       sp = fmaf(pe, pe, sp);
       if constexpr (kLamb) {
         float me = a.m[e], ve = a.v[e];
@@ -131,11 +135,12 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_norms_kernel(const LwArg
   }
 }
 
-template <bool kLamb, bool kClip>
+template <bool kLamb, bool kClip, bool kScaled>
 __global__ void __launch_bounds__(kLwThreads) layerwise_apply_kernel(const LwArgs a) {
   __shared__ float s_r;
   float c = 1.f;
   if constexpr (kClip) c = lw_clip_coef(a, false);
+  const float inv = kScaled ? amp_inv_scale(a.grad_scale) : 1.f;
   const long long* chunks = a.table;
   const long long* tens = a.table + (size_t)a.n_chunks * kLwRow;
   for (int ch = blockIdx.x; ch < a.n_chunks; ch += gridDim.x) {
@@ -182,6 +187,7 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_apply_kernel(const LwArg
         float4 pv = reinterpret_cast<const float4*>(a.p)[v0 + i];
         float4 mv = reinterpret_cast<const float4*>(a.m)[v0 + i];
         float4 gv = reinterpret_cast<const float4*>(a.g)[v0 + i];
+        if constexpr (kScaled) gv = amp_unscale4(gv, inv);
         if constexpr (kClip) gv = scale4(gv, c);
         lars_elem(pv.x, mv.x, gv.x, r, wd, a);
         lars_elem(pv.y, mv.y, gv.y, r, wd, a);
@@ -194,7 +200,8 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_apply_kernel(const LwArg
       if (threadIdx.x < tail) {
         const size_t e = (size_t)start + (size_t)nv * 4 + threadIdx.x;
         float pe = a.p[e], me = a.m[e];
-        lars_elem(pe, me, kClip ? __fmul_rn(a.g[e], c) : a.g[e], r, wd, a);
+        const float gl = kScaled ? amp_unscale(a.g[e], inv) : a.g[e];
+        lars_elem(pe, me, kClip ? __fmul_rn(gl, c) : gl, r, wd, a);
         a.p[e] = pe;
         a.m[e] = me;
         if (a.zero_grad) a.g[e] = 0.f;
@@ -203,14 +210,14 @@ __global__ void __launch_bounds__(kLwThreads) layerwise_apply_kernel(const LwArg
   }
 }
 
-template <bool kLamb, bool kClip>
+template <bool kLamb, bool kClip, bool kScaled>
 int layerwise_launch_t(const LwArgs& a, cudaStream_t stream) {
   const unsigned blocks = (unsigned)(a.n_chunks < kLwMaxCtas ? a.n_chunks : kLwMaxCtas);
-  layerwise_norms_kernel<kLamb, kClip><<<blocks, kLwThreads, 0, stream>>>(a);
+  layerwise_norms_kernel<kLamb, kClip, kScaled><<<blocks, kLwThreads, 0, stream>>>(a);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
-  // LAMB's second pass does not read g, so it has no clip instance
-  layerwise_apply_kernel<kLamb, kClip && !kLamb><<<blocks, kLwThreads, 0, stream>>>(a);
+  // LAMB's second pass does not read g, so it has no clip or scaled instance
+  layerwise_apply_kernel<kLamb, kClip && !kLamb, kScaled && !kLamb><<<blocks, kLwThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -228,8 +235,18 @@ int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream) {
   if (a->n_tensors < 1 || a->n_chunks < 1 || (size_t)a->n_chunks > a->n) return (int)cudaErrorInvalidValue;
   const bool clip = a->max_norm > 0.f;
   if (clip && (a->sqnorms == nullptr || a->n_buckets < 1 || !(a->max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
-  if (lamb) return clip ? b2::layerwise_launch_t<true, true>(*a, stream) : b2::layerwise_launch_t<true, false>(*a, stream);
-  return clip ? b2::layerwise_launch_t<false, true>(*a, stream) : b2::layerwise_launch_t<false, false>(*a, stream);
+  using namespace b2;
+  const int k = (lamb ? 4 : 0) | (clip ? 2 : 0) | (a->grad_scale != nullptr ? 1 : 0);
+  switch (k) {
+    case 0: return layerwise_launch_t<false, false, false>(*a, stream);
+    case 1: return layerwise_launch_t<false, false, true>(*a, stream);
+    case 2: return layerwise_launch_t<false, true, false>(*a, stream);
+    case 3: return layerwise_launch_t<false, true, true>(*a, stream);
+    case 4: return layerwise_launch_t<true, false, false>(*a, stream);
+    case 5: return layerwise_launch_t<true, false, true>(*a, stream);
+    case 6: return layerwise_launch_t<true, true, false>(*a, stream);
+    default: return layerwise_launch_t<true, true, true>(*a, stream);
+  }
 }
 
 }  // extern "C"

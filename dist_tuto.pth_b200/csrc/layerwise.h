@@ -36,6 +36,8 @@ struct LwArgs {
   int n_buckets;
   float max_norm;
   float* grad_norm_out;
+  // fp16 loss scaling: GradScaler's scale S on the device (fp32), or null; the scaled instances read g * fp32(1 / double(S))
+  const float* grad_scale;
 };
 
 }  // namespace b2

@@ -258,16 +258,19 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const float* __restrict
 }
 
 // Plain flat momentum SGD (generic models: gradients already averaged in `grad`).  kNesterov: step along g + mu*m instead of m.
-template <bool kNesterov>
+// kScaled: the gradient is g * amp_inv_scale(grad_scale) (sgd_device.cuh); the kScaled = false instances never read grad_scale.
+template <bool kNesterov, bool kScaled>
 __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, float* __restrict__ m,
                                                        const float* __restrict__ g, size_t n, float lr, float mu,
-                                                       float wd, int zero_grad, float* gw) {
+                                                       float wd, int zero_grad, float* gw, const float* grad_scale) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t n4 = n / 4;
+  const float inv = kScaled ? amp_inv_scale(grad_scale) : 1.f;
   if (i < n4) {
     float4 gv = reinterpret_cast<const float4*>(g)[i];
     float4 pv = reinterpret_cast<float4*>(p)[i];
     float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kScaled) gv = amp_unscale4(gv, inv);
     gv.x = fmaf(wd, pv.x, gv.x); gv.y = fmaf(wd, pv.y, gv.y); gv.z = fmaf(wd, pv.z, gv.z); gv.w = fmaf(wd, pv.w, gv.w);
     mv.x = fmaf(mu, mv.x, gv.x); mv.y = fmaf(mu, mv.y, gv.y); mv.z = fmaf(mu, mv.z, gv.z); mv.w = fmaf(mu, mv.w, gv.w);
     float4 dv = mv;
@@ -281,7 +284,7 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
   }
   if (i == 0) {
     for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
-      const float gt = fmaf(wd, p[t], g[t]);
+      const float gt = fmaf(wd, p[t], kScaled ? amp_unscale(g[t], inv) : g[t]);
       m[t] = fmaf(mu, m[t], gt);
       p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
       if (zero_grad) gw[t] = 0.f;
@@ -292,20 +295,26 @@ __global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ p, fl
 // FlatSGD's clipping, part 1: the sum of squares of one bucket's gradient g[0, n) into sqnorms[k] (fp64).  Each thread sums
 // its squares in fp32 (its float4 vectors in order; thread 0 of CTA 0 also the < 4 tail elements), each CTA in a fixed
 // tree, and the last CTA to finish adds the CTA partials in CTA order in fp64.  ws: [kClipMaxCtas partials | ticket], the
-// ticket zero between calls (the last CTA resets it).
+// ticket zero between calls (the last CTA resets it).  kScaled: the squares of g * amp_inv_scale(grad_scale).
 constexpr int kSqnormThreads = 256;
+template <bool kScaled>
 __global__ void __launch_bounds__(kSqnormThreads) grad_sqnorm_kernel(const float* __restrict__ g, size_t n, float* ws,
-                                                                      double* __restrict__ sqnorms, int k) {
+                                                                      double* __restrict__ sqnorms, int k, const float* grad_scale) {
   __shared__ float s_part[kClipMaxCtas];
   __shared__ int s_last;
   const size_t n4 = n / 4;
+  const float inv = kScaled ? amp_inv_scale(grad_scale) : 1.f;
   float sq = 0.f;
   for (size_t i = (size_t)blockIdx.x * kSqnormThreads + threadIdx.x; i < n4; i += (size_t)gridDim.x * kSqnormThreads) {
-    const float4 v = reinterpret_cast<const float4*>(g)[i];
+    float4 v = reinterpret_cast<const float4*>(g)[i];
+    if constexpr (kScaled) v = amp_unscale4(v, inv);
     sq = fmaf(v.x, v.x, sq); sq = fmaf(v.y, v.y, sq); sq = fmaf(v.z, v.z, sq); sq = fmaf(v.w, v.w, sq);
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    for (size_t t = n4 * 4; t < n; ++t) sq = fmaf(g[t], g[t], sq);
+    for (size_t t = n4 * 4; t < n; ++t) {
+      const float gt = kScaled ? amp_unscale(g[t], inv) : g[t];
+      sq = fmaf(gt, gt, sq);
+    }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, d);
   if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = sq;
@@ -333,11 +342,12 @@ __global__ void __launch_bounds__(kSqnormThreads) grad_sqnorm_kernel(const float
 
 // FlatSGD's clipping, part 2: sgd_flat_kernel's update of one bucket after g *= coef, where coef comes from the total norm
 // sqrt(sum of sqnorms[0, n_buckets) in bucket order), taken in fp64 and rounded once to fp32 (grad_norm_out, optional).
-template <bool kNesterov>
+template <bool kNesterov, bool kScaled>
 __global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ p, float* __restrict__ m,
                                                             const float* __restrict__ g, size_t n, float lr, float mu,
                                                             float wd, int zero_grad, float* gw, const double* __restrict__ sqnorms,
-                                                            int n_buckets, float max_norm, float* grad_norm_out) {
+                                                            int n_buckets, float max_norm, float* grad_norm_out,
+                                                            const float* grad_scale) {
   __shared__ float s_coef;
   if (threadIdx.x == 0) {
     double s = 0.0;
@@ -350,10 +360,12 @@ __global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ 
   const float c = s_coef;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t n4 = n / 4;
+  const float inv = kScaled ? amp_inv_scale(grad_scale) : 1.f;
   if (i < n4) {
     float4 gv = reinterpret_cast<const float4*>(g)[i];
     float4 pv = reinterpret_cast<float4*>(p)[i];
     float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kScaled) gv = amp_unscale4(gv, inv);
     gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
     gv.x = fmaf(wd, pv.x, gv.x); gv.y = fmaf(wd, pv.y, gv.y); gv.z = fmaf(wd, pv.z, gv.z); gv.w = fmaf(wd, pv.w, gv.w);
     mv.x = fmaf(mu, mv.x, gv.x); mv.y = fmaf(mu, mv.y, gv.y); mv.z = fmaf(mu, mv.z, gv.z); mv.w = fmaf(mu, mv.w, gv.w);
@@ -368,7 +380,7 @@ __global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ 
   }
   if (i == 0) {
     for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
-      const float gt = fmaf(wd, p[t], __fmul_rn(g[t], c));
+      const float gt = fmaf(wd, p[t], __fmul_rn(kScaled ? amp_unscale(g[t], inv) : g[t], c));
       m[t] = fmaf(mu, m[t], gt);
       p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
       if (zero_grad) gw[t] = 0.f;
@@ -379,12 +391,13 @@ __global__ void __launch_bounds__(256) sgd_flat_clip_kernel(float* __restrict__ 
 // sgd_flat_kernel / sgd_flat_clip_kernel with parameter groups: parameter vector i takes the lr and weight decay of group
 // map[i] (param_groups.cuh); the tail (< 4 elements) shares the map entry of its vector.  The per-element sequence is the
 // ungrouped kernels' (sgd4), so running those on each tensor's segment with its group's scalars gives the same bits.
-template <bool kNesterov, bool kClip>
+template <bool kNesterov, bool kClip, bool kScaled>
 __global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict__ p, float* __restrict__ m,
                                                                const float* __restrict__ g, size_t n,
                                                                const uint8_t* __restrict__ map, SgdGroups gs, float mu,
                                                                int zero_grad, float* gw, const double* __restrict__ sqnorms,
-                                                               int n_buckets, float max_norm, float* grad_norm_out) {
+                                                               int n_buckets, float max_norm, float* grad_norm_out,
+                                                               const float* grad_scale) {
   float c = 1.f;
   if constexpr (kClip) {
     __shared__ float s_coef;
@@ -400,11 +413,13 @@ __global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict
   }
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t n4 = n / 4;
+  const float inv = kScaled ? amp_inv_scale(grad_scale) : 1.f;
   if (i < n4) {
     const int gid = map[i];
     float4 gv = reinterpret_cast<const float4*>(g)[i];
     float4 pv = reinterpret_cast<float4*>(p)[i];
     float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kScaled) gv = amp_unscale4(gv, inv);
     if constexpr (kClip) {
       gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
     }
@@ -417,7 +432,8 @@ __global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict
     const int gid = map[n4];
     const float lr = gs.lr[gid], wd = gs.wd[gid];
     for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
-      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(g[t], c) : g[t]);
+      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(kScaled ? amp_unscale(g[t], inv) : g[t], c)
+                                            : (kScaled ? amp_unscale(g[t], inv) : g[t]));
       m[t] = fmaf(mu, m[t], gt);
       p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
       if (zero_grad) gw[t] = 0.f;
@@ -428,15 +444,23 @@ __global__ void __launch_bounds__(256) sgd_flat_grouped_kernel(float* __restrict
 // Capturable instances of sgd_flat_kernel, sgd_flat_clip_kernel and sgd_flat_grouped_kernel (flat_scalars.cuh): the lr and
 // weight decay (kGrouped: every group's) come from the scalar block `blk`, loaded once per CTA through shared memory, instead
 // of the kernel arguments.  The per-element sequence is sgd4, the fmaf sequence of those kernels, so the same scalars give
-// the same bits.
-template <bool kNesterov, bool kClip, bool kGrouped>
+// the same bits.  kScaled: GradScaler's step -- with found_inf != 0 only the zeroing (amp_skip_zero), else the gradient is
+// g * amp_inv_scale(grad_scale) (grad_scale null: already unscaled).
+template <bool kNesterov, bool kClip, bool kGrouped, bool kScaled>
 __global__ void __launch_bounds__(256) sgd_flat_cap_kernel(float* __restrict__ p, float* __restrict__ m,
                                                            const float* __restrict__ g, size_t n, const uint8_t* __restrict__ map,
                                                            const FlatScalars* __restrict__ blk, float mu, int zero_grad, float* gw,
                                                            const double* __restrict__ sqnorms, int n_buckets, float max_norm,
-                                                           float* grad_norm_out) {
+                                                           float* grad_norm_out, const float* grad_scale, const float* found_inf) {
   __shared__ float s_coef, s_lr, s_wd;
   __shared__ SgdGroups s_gs;
+  if constexpr (kScaled) {
+    if (__ldg(found_inf) != 0.f) {
+      amp_skip_zero(gw, n, zero_grad);
+      return;
+    }
+  }
+  const float inv = kScaled && grad_scale != nullptr ? amp_inv_scale(grad_scale) : 1.f;
   if constexpr (kGrouped) flat_block_load(s_gs, blk->sgd);
   if (threadIdx.x == 0) {
     if constexpr (!kGrouped) { s_lr = blk->lr; s_wd = blk->wd; }
@@ -451,6 +475,7 @@ __global__ void __launch_bounds__(256) sgd_flat_cap_kernel(float* __restrict__ p
     float4 gv = reinterpret_cast<const float4*>(g)[i];
     float4 pv = reinterpret_cast<float4*>(p)[i];
     float4 mv = reinterpret_cast<float4*>(m)[i];
+    if constexpr (kScaled) gv = amp_unscale4(gv, inv);
     if constexpr (kClip) {
       gv.x = __fmul_rn(gv.x, c); gv.y = __fmul_rn(gv.y, c); gv.z = __fmul_rn(gv.z, c); gv.w = __fmul_rn(gv.w, c);
     }
@@ -463,7 +488,8 @@ __global__ void __launch_bounds__(256) sgd_flat_cap_kernel(float* __restrict__ p
     const int gid = kGrouped ? map[n4] : 0;
     const float lr = kGrouped ? s_gs.lr[gid] : s_lr, wd = kGrouped ? s_gs.wd[gid] : s_wd;
     for (size_t t = n4 * 4; t < n; ++t) {      // tail (< 4 elements)
-      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(g[t], c) : g[t]);
+      const float gt = fmaf(wd, p[t], kClip ? __fmul_rn(kScaled ? amp_unscale(g[t], inv) : g[t], c)
+                                            : (kScaled ? amp_unscale(g[t], inv) : g[t]));
       m[t] = fmaf(mu, m[t], gt);
       p[t] = fmaf(-lr, kNesterov ? fmaf(mu, m[t], gt) : m[t], p[t]);
       if (zero_grad) gw[t] = 0.f;
@@ -641,24 +667,36 @@ int b2_lr_schedule_eval_launch(const b2::LrSchedule* sched, float base, const lo
   return (int)cudaGetLastError();
 }
 
+// grad_scale (fp32 on the device, or null): GradScaler's loss scale, the scaled instances unscale the gradient as they load it.
 int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, float mu, float wd, int zero_grad, int nesterov,
-                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, cudaStream_t stream) {
+                       float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out, const float* grad_scale,
+                       cudaStream_t stream) {
   const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
   const unsigned blocks = (unsigned)((n4 + 255) / 256);
+  float* gw = const_cast<float*>(g);
+  using namespace b2;
+  const int k = (nesterov ? 2 : 0) | (grad_scale != nullptr ? 1 : 0);
   if (max_norm > 0.f) {            // clipped by the norm of grad_sqnorm's n_buckets sums (0: no clipping)
     if (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY)) return (int)cudaErrorInvalidValue;
-    if (nesterov)
-      b2::sgd_flat_clip_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g), sqnorms,
-                                                                 n_buckets, max_norm, grad_norm_out);
-    else
-      b2::sgd_flat_clip_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g), sqnorms,
-                                                                  n_buckets, max_norm, grad_norm_out);
+#define B2_SGD_CLIP(N, S) sgd_flat_clip_kernel<N, S><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, gw, sqnorms, \
+                                                                               n_buckets, max_norm, grad_norm_out, grad_scale)
+    switch (k) {
+      case 0: B2_SGD_CLIP(false, false); break;
+      case 1: B2_SGD_CLIP(false, true); break;
+      case 2: B2_SGD_CLIP(true, false); break;
+      default: B2_SGD_CLIP(true, true); break;
+    }
+#undef B2_SGD_CLIP
     return (int)cudaGetLastError();
   }
-  if (nesterov)
-    b2::sgd_flat_kernel<true><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
-  else
-    b2::sgd_flat_kernel<false><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, const_cast<float*>(g));
+#define B2_SGD(N, S) sgd_flat_kernel<N, S><<<blocks, 256, 0, stream>>>(p, m, g, n, lr, mu, wd, zero_grad, gw, grad_scale)
+  switch (k) {
+    case 0: B2_SGD(false, false); break;
+    case 1: B2_SGD(false, true); break;
+    case 2: B2_SGD(true, false); break;
+    default: B2_SGD(true, true); break;
+  }
+#undef B2_SGD
   return (int)cudaGetLastError();
 }
 
@@ -667,37 +705,42 @@ int b2_sgd_flat_launch(float* p, float* m, const float* g, size_t n, float lr, f
 // sqnorms; the ids themselves are checked on the host where the map is built.
 int b2_sgd_flat_grouped_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::SgdGroups* gs,
                                int n_groups, float mu, int zero_grad, int nesterov, float max_norm, const double* sqnorms,
-                               int n_buckets, float* grad_norm_out, cudaStream_t stream) {
+                               int n_buckets, float* grad_norm_out, const float* grad_scale, cudaStream_t stream) {
   if (p == nullptr || m == nullptr || g == nullptr || map == nullptr || gs == nullptr || n_groups < 1 ||
       n_groups > b2::kMaxGroups)
     return (int)cudaErrorInvalidValue;
+  const bool clip = max_norm > 0.f;
+  if (clip && (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
   const size_t n4 = (n / 4) > 0 ? n / 4 : 1;
   const unsigned blocks = (unsigned)((n4 + 255) / 256);
   float* gw = const_cast<float*>(g);
-  if (max_norm > 0.f) {
-    if (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY)) return (int)cudaErrorInvalidValue;
-    if (nesterov)
-      b2::sgd_flat_grouped_kernel<true, true><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, sqnorms,
-                                                                          n_buckets, max_norm, grad_norm_out);
-    else
-      b2::sgd_flat_grouped_kernel<false, true><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, sqnorms,
-                                                                           n_buckets, max_norm, grad_norm_out);
-  } else if (nesterov) {
-    b2::sgd_flat_grouped_kernel<true, false><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, nullptr, 0,
-                                                                         0.f, nullptr);
-  } else {
-    b2::sgd_flat_grouped_kernel<false, false><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, nullptr, 0,
-                                                                          0.f, nullptr);
+  using namespace b2;
+#define B2_SGD_GR(N, C, S) sgd_flat_grouped_kernel<N, C, S><<<blocks, 256, 0, stream>>>(p, m, g, n, map, *gs, mu, zero_grad, gw, \
+      C ? sqnorms : nullptr, C ? n_buckets : 0, C ? max_norm : 0.f, C ? grad_norm_out : nullptr, grad_scale)
+  const int k = (nesterov ? 4 : 0) | (clip ? 2 : 0) | (grad_scale != nullptr ? 1 : 0);
+  switch (k) {
+    case 0: B2_SGD_GR(false, false, false); break;
+    case 1: B2_SGD_GR(false, false, true); break;
+    case 2: B2_SGD_GR(false, true, false); break;
+    case 3: B2_SGD_GR(false, true, true); break;
+    case 4: B2_SGD_GR(true, false, false); break;
+    case 5: B2_SGD_GR(true, false, true); break;
+    case 6: B2_SGD_GR(true, true, false); break;
+    default: B2_SGD_GR(true, true, true); break;
   }
+#undef B2_SGD_GR
   return (int)cudaGetLastError();
 }
 
 // The capturable sgd_flat / sgd_flat_grouped (flat_scalars.cuh): the scalars come from the block `blk` on the device.  `map`:
 // null without groups, else one group id per parameter vector.  cudaErrorInvalidValue, without a launch, for a null pointer
 // or clipping without sqnorms.
+// found_inf (fp32 on the device, or null): GradScaler's step, with grad_scale as in b2_sgd_flat_launch (null: already
+// unscaled); without found_inf grad_scale must be null.
 int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk, float mu,
                            int zero_grad, int nesterov, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
-                           cudaStream_t stream) {
+                           const float* grad_scale, const float* found_inf, cudaStream_t stream) {
+  if (found_inf == nullptr && grad_scale != nullptr) return (int)cudaErrorInvalidValue;
   if (p == nullptr || m == nullptr || g == nullptr || blk == nullptr) return (int)cudaErrorInvalidValue;
   const bool clip = max_norm > 0.f;
   if (clip && (sqnorms == nullptr || n_buckets < 1 || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
@@ -705,18 +748,26 @@ int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const u
   const unsigned blocks = (unsigned)((n4 + 255) / 256);
   float* gw = const_cast<float*>(g);
   using namespace b2;
-#define B2_SGD_CAP(N, C, G) sgd_flat_cap_kernel<N, C, G><<<blocks, 256, 0, stream>>>(p, m, g, n, map, blk, mu, zero_grad, gw, \
-                                                                                   sqnorms, n_buckets, max_norm, grad_norm_out)
-  const int k = (nesterov ? 4 : 0) | (clip ? 2 : 0) | (map != nullptr ? 1 : 0);
+#define B2_SGD_CAP(N, C, G, S) sgd_flat_cap_kernel<N, C, G, S><<<blocks, 256, 0, stream>>>(p, m, g, n, map, blk, mu, zero_grad, \
+                                                          gw, sqnorms, n_buckets, max_norm, grad_norm_out, grad_scale, found_inf)
+  const int k = (found_inf != nullptr ? 8 : 0) | (nesterov ? 4 : 0) | (clip ? 2 : 0) | (map != nullptr ? 1 : 0);
   switch (k) {
-    case 0: B2_SGD_CAP(false, false, false); break;
-    case 1: B2_SGD_CAP(false, false, true); break;
-    case 2: B2_SGD_CAP(false, true, false); break;
-    case 3: B2_SGD_CAP(false, true, true); break;
-    case 4: B2_SGD_CAP(true, false, false); break;
-    case 5: B2_SGD_CAP(true, false, true); break;
-    case 6: B2_SGD_CAP(true, true, false); break;
-    default: B2_SGD_CAP(true, true, true); break;
+    case 0: B2_SGD_CAP(false, false, false, false); break;
+    case 1: B2_SGD_CAP(false, false, true, false); break;
+    case 2: B2_SGD_CAP(false, true, false, false); break;
+    case 3: B2_SGD_CAP(false, true, true, false); break;
+    case 4: B2_SGD_CAP(true, false, false, false); break;
+    case 5: B2_SGD_CAP(true, false, true, false); break;
+    case 6: B2_SGD_CAP(true, true, false, false); break;
+    case 7: B2_SGD_CAP(true, true, true, false); break;
+    case 8: B2_SGD_CAP(false, false, false, true); break;
+    case 9: B2_SGD_CAP(false, false, true, true); break;
+    case 10: B2_SGD_CAP(false, true, false, true); break;
+    case 11: B2_SGD_CAP(false, true, true, true); break;
+    case 12: B2_SGD_CAP(true, false, false, true); break;
+    case 13: B2_SGD_CAP(true, false, true, true); break;
+    case 14: B2_SGD_CAP(true, true, false, true); break;
+    default: B2_SGD_CAP(true, true, true, true); break;
   }
 #undef B2_SGD_CAP
   return (int)cudaGetLastError();
@@ -724,11 +775,15 @@ int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const u
 
 // ws: b2_grad_sqnorm_ws_floats() floats, zero before the first call
 int b2_grad_sqnorm_ws_floats() { return b2::kClipMaxCtas + 4; }
-int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, cudaStream_t stream) {
+int b2_grad_sqnorm_launch(const float* g, size_t n, float* ws, double* sqnorms, int k, const float* grad_scale,
+                          cudaStream_t stream) {
   size_t blocks = (n / 4 + b2::kSqnormThreads - 1) / b2::kSqnormThreads;
   if (blocks < 1) blocks = 1;
   if (blocks > (size_t)b2::kClipMaxCtas) blocks = b2::kClipMaxCtas;
-  b2::grad_sqnorm_kernel<<<(unsigned)blocks, b2::kSqnormThreads, 0, stream>>>(g, n, ws, sqnorms, k);
+  if (grad_scale != nullptr)
+    b2::grad_sqnorm_kernel<true><<<(unsigned)blocks, b2::kSqnormThreads, 0, stream>>>(g, n, ws, sqnorms, k, grad_scale);
+  else
+    b2::grad_sqnorm_kernel<false><<<(unsigned)blocks, b2::kSqnormThreads, 0, stream>>>(g, n, ws, sqnorms, k, nullptr);
   return (int)cudaGetLastError();
 }
 

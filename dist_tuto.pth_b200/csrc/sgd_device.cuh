@@ -294,6 +294,33 @@ __device__ __forceinline__ float clip_grid_coef(const SgdArgsClip& a, float sq) 
   return s_coef;
 }
 
+// ----------------------------------------------------------------- fp16 loss scaling (torch.amp.GradScaler)
+// The scaled instances of the flat update kernels (grad_sqnorm, sgd_flat, adamw_flat, their grouped and capturable forms, and
+// the layer-wise kernels) read the loss scale S from the device and use g * inv wherever they read a gradient, before any
+// clip coefficient, with inv = fp32(1 / double(S)) as GradScaler.unscale_ computes it.  The product is rounded to nearest
+// with subnormals kept (mul.rn.f32, not the .ftz form --use_fast_math gives), as torch's unscale kernel computes it, so the
+// update sees the bits GradScaler.unscale_ would have left in p.grad.
+__device__ __forceinline__ float amp_inv_scale(const float* grad_scale) {
+  return __double2float_rn(__ddiv_rn(1.0, (double)__ldg(grad_scale)));
+}
+__device__ __forceinline__ float amp_unscale(float g, float inv) {
+  float r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(g), "f"(inv));
+  return r;
+}
+__device__ __forceinline__ float4 amp_unscale4(float4 g, float inv) {
+  return make_float4(amp_unscale(g.x, inv), amp_unscale(g.y, inv), amp_unscale(g.z, inv), amp_unscale(g.w, inv));
+}
+// A capturable scaled instance whose step GradScaler skips (found_inf != 0) writes nothing but the fused zeroing of the
+// gradient g[0, n): thread i zeroes vector i and tail element i.  Every thread of the grid calls it and then returns.
+__device__ __forceinline__ void amp_skip_zero(float* g, size_t n, int zero_grad) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t n4 = n / 4;
+  if (!zero_grad) return;
+  if (i < n4) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (i < n - n4 * 4) g[n4 * 4 + i] = 0.f;
+}
+
 // Phase B: vector v from the scratch, times the coefficient, through the update.
 __device__ __forceinline__ void clip_apply(const SgdArgsClip& a, size_t v, float coef, float lr) {
   float4 g = __ldcg(reinterpret_cast<const float4*>(a.clip_ws + kClipWsHead) + v);

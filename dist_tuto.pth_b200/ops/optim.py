@@ -251,6 +251,14 @@ def _group_attr(key: str):
     return property(lambda self: self._default_group[key], lambda self, v: self._default_group.__setitem__(key, float(v)))
 
 
+def _fp32_grad(g: torch.Tensor, grad_scale: Optional[torch.Tensor]) -> torch.Tensor:
+    """The gradient a torch-op update reads: ``g`` in fp32, and with GradScaler's ``grad_scale`` S times
+    ``inv = fp32(1 / double(S))``, computed as ``GradScaler.unscale_`` computes it (a new tensor: ``g`` keeps the scaled
+    values)."""
+    gf = g.to(torch.float32)
+    return gf if grad_scale is None else gf * grad_scale.double().reciprocal().float()
+
+
 def _peer_world(gb) -> bool:
     """Does this gradient bucket live in the symmetric memory of ONE peer-memory world (not the two-level world of several
     machines), in a dtype ``sharded_sgd_kernel`` reduces?"""
@@ -267,7 +275,14 @@ class _FlatOptimizer:
     ``sharded=True``, the registration of the sharded update with the buckets' exchange, the ``step()`` bookkeeping, the lr
     schedule, on-device gradient-norm clipping, and the gathering and slicing of per-bucket optimizer state.  A subclass
     allocates its state flats (:meth:`_state_flat`) and updates a whole bucket (``_update``), a bucket in one peer-memory
-    kernel (``_sharded_kernel``) or the owned slice of a bucket with torch ops (``_update_slice``)."""
+    kernel (``_sharded_kernel``) or the owned slice of a bucket with torch ops (``_update_slice``).
+
+    fp16 loss scaling: ``torch.amp.GradScaler.step(opt)`` sees ``_step_supports_amp_scaling`` and, after its own check for
+    non-finite gradients, sets ``grad_scale`` (the loss scale S, or ``None`` after an explicit ``scaler.unscale_(opt)``) and
+    ``found_inf`` on the optimizer, calls :meth:`step` and deletes both; see :meth:`step`."""
+
+    # torch.amp.GradScaler hands this optimizer grad_scale / found_inf instead of unscaling and syncing itself
+    _step_supports_amp_scaling = True
 
     def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
                  max_grad_norm: Optional[float], sharded: bool, param_groups: Optional[list] = None,
@@ -528,10 +543,22 @@ class _FlatOptimizer:
     @torch.no_grad()
     def step(self) -> None:
         """``optimizer.step()`` (train_dist.py:124) for every bucket, and -- with ``zero_grad=True`` -- the
-        ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass."""
+        ``optimizer.zero_grad()`` of the next iteration (train_dist.py:118) in the same pass.  Called by
+        ``torch.amp.GradScaler.step`` (``grad_scale`` / ``found_inf`` set), it is torch's ``unscale_`` + step:
+        every gradient the update reads -- the clipping norm and the LAMB / LARS norms included -- is ``g * inv`` with
+        ``inv = fp32(1 / double(S))``, and when ``found_inf != 0`` the step is skipped: no parameter, state, trust ratio or
+        ``grad_norm`` is written and ``steps`` does not advance, but with ``zero_grad=True`` the buckets are still zeroed
+        and the hooks re-armed.  ``capturable=True`` decides on the device with no host synchronisation; otherwise
+        ``found_inf`` is read once (one synchronisation, as GradScaler makes with a ``torch.optim`` optimizer).  Sharded
+        over more than one rank it raises ``RuntimeError``."""
         if getattr(self, "_ema_swapped", False):
             raise RuntimeError(f"{type(self).__name__}.step() inside FlatEMA.average_parameters(): the parameters hold the "
                                "EMA values there; step after the block")
+        scale, found_inf = getattr(self, "grad_scale", None), getattr(self, "found_inf", None)
+        if self._shard_mode is not None and (scale is not None or found_inf is not None):
+            raise RuntimeError(f"{type(self).__name__}(sharded=True) over {self._world} ranks cannot take GradScaler's step: the "
+                               "gradient exchange already applied this step's update with the scaled gradient during backward, "
+                               "before any overflow check.  fp16 loss scaling needs sharded=False")
         if self._shard_mode is not None:      # the buckets' exchanges applied the update already
             if not all(self._done):
                 raise RuntimeError(f"{type(self).__name__}(sharded=True).step(): this step's gradient buckets were not "
@@ -548,26 +575,42 @@ class _FlatOptimizer:
             raise RuntimeError(f"{type(self).__name__}.step(): gradients accumulated under no_sync() were never exchanged; "
                                "run the last micro-batch's backward outside no_sync(), or call average_gradients(model), "
                                "before step()")
+        # Unsharded, every rank holds the same averaged gradient bit for bit (the exchange sums in a fixed rank order), so
+        # GradScaler's check finds the same found_inf on every rank and all ranks skip or apply together, with no collective.
         if self.capturable:
             self._cap_refresh()
-            self._update_capturable(self._clip_on_device() if self.max_grad_norm is not None else {})
-            self._advance()
+            kw = {} if found_inf is None else dict(grad_scale=scale, found_inf=found_inf)
+            if self.max_grad_norm is not None:
+                kw.update(self._clip_on_device(scale))
+            self._update_capturable(kw)
+            self._advance(found_inf)
             if self.fused_zero and self._engine is not None:
                 self._engine._reset()
             return
+        if found_inf is not None and float(found_inf) != 0.0:      # the one host synchronisation of an eager scaled step
+            if self.fused_zero:
+                for gb in self.buckets:
+                    gb.flat[:gb.numel].zero_()
+                if self._engine is not None:
+                    self._engine._reset()
+            return
         kernel = [pf.is_cuda and gb.flat.dtype == torch.float32 for gb, pf in zip(self.buckets, self.param_flats)]
-        clip = {}
+        kw = {} if scale is None else {"grad_scale": scale}
         if self.max_grad_norm is not None:
             if all(kernel):
-                clip = self._clip_on_device()
+                kw.update(self._clip_on_device(scale))
             else:                        # every bucket by torch itself, before any update
                 params = []
                 for gb in self.buckets:
                     gb.attach()          # p.grad is the bucket's view, so the clip scales the bucket in place
                     params += gb.params
+                    if scale is not None:                  # GradScaler.unscale_'s own op, in place, before the clip
+                        torch._amp_foreach_non_finite_check_and_unscale_(
+                            [gb.flat[:gb.numel]], torch.zeros((), device=scale.device), scale.double().reciprocal().float())
+                kw = {}
                 self._grad_norm = torch.nn.utils.clip_grad_norm_(params, self.max_grad_norm, foreach=False)
                 kernel = [False] * len(kernel)
-        self._update(kernel, clip)
+        self._update(kernel, kw)
         self.steps += 1
         if self.fused_zero and self._engine is not None:
             self._engine._reset()
@@ -611,9 +654,10 @@ class _FlatOptimizer:
         if self.capturable:
             self._sync_device()
 
-    def _advance(self) -> None:
-        """capturable: counter += 1 and the scalars of the next update, one single-CTA launch after this step's updates."""
-        self._kernel().flat_scalars_advance(self._cap_table, self._cap_counter, self._cap_block)
+    def _advance(self, found_inf: Optional[torch.Tensor] = None) -> None:
+        """capturable: counter += 1 and the scalars of the next update, one single-CTA launch after this step's updates;
+        with GradScaler's ``found_inf`` nothing changes when it is nonzero."""
+        self._kernel().flat_scalars_advance(self._cap_table, self._cap_counter, self._cap_block, found_inf=found_inf)
 
     def _cap_map(self, k: int) -> Optional[torch.Tensor]:
         return self._maps[k] if self._grouped else None
@@ -697,9 +741,9 @@ class _FlatOptimizer:
             for m, src in zip(flats, saved):
                 m.copy_(src)
 
-    def _clip_on_device(self) -> dict:
-        """Every bucket's sum of squares into the fp64 device array (grad_sqnorm, one launch per bucket); the update kernel's
-        arguments that take the norm and the coefficient from it."""
+    def _clip_on_device(self, grad_scale: Optional[torch.Tensor] = None) -> dict:
+        """Every bucket's sum of squares (of the unscaled gradient with GradScaler's ``grad_scale``) into the fp64 device array
+        (grad_sqnorm, one launch per bucket); the update kernel's arguments that take the norm and the coefficient from it."""
         C = self._kernel()
         if self._clip_bufs is None:
             dev = self.param_flats[0].device
@@ -708,7 +752,7 @@ class _FlatOptimizer:
                                torch.zeros(1, dtype=torch.float32, device=dev))
         sq, ws, norm = self._clip_bufs
         for k, gb in enumerate(self.buckets):
-            C.grad_sqnorm(gb.flat[:gb.numel], sq, k, ws)
+            C.grad_sqnorm(gb.flat[:gb.numel], sq, k, ws, grad_scale=grad_scale)
         self._grad_norm = norm
         return dict(max_grad_norm=self.max_grad_norm, sqnorms=sq, grad_norm_out=norm)
 
@@ -822,7 +866,7 @@ class FlatSGD(_FlatOptimizer):
                     self._kernel().sgd_flat_grouped(pf, mf, g, self._maps[k], [v[0] for v in vals], [v[1] for v in vals],
                                                     self.momentum, self.fused_zero, self.nesterov, **clip)
                     continue
-                self._sgd_runs(self._runs[k], pf, mf, g)
+                self._sgd_runs(self._runs[k], pf, mf, _fp32_grad(g, clip.get("grad_scale")))
                 if self.fused_zero:
                     g.zero_()
             return
@@ -835,7 +879,7 @@ class FlatSGD(_FlatOptimizer):
                 continue
             # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
             # torch.optim.SGD's order (foreach=False)
-            gf = g.to(torch.float32)
+            gf = _fp32_grad(g, clip.get("grad_scale"))
             if self.weight_decay:
                 gf = gf.add(pf, alpha=self.weight_decay)
             mf.mul_(self.momentum).add_(gf)
@@ -1037,7 +1081,7 @@ class FlatAdamW(_FlatOptimizer):
                 if kern:
                     self._kernel().adamw_flat_grouped(pf, mf, vf, g, self._maps[k], *sc, self.fused_zero, **clip)
                     continue
-                gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+                gf = _fp32_grad(g, clip.get("grad_scale"))
                 # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.AdamW sees it
                 views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
                          for f in (pf, gf, mf, vf)]
@@ -1055,7 +1099,7 @@ class FlatAdamW(_FlatOptimizer):
             if kern:
                 self._kernel().adamw_flat(pf, mf, vf, g, sc, self.fused_zero, **clip)
                 continue
-            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            gf = _fp32_grad(g, clip.get("grad_scale"))
             views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
                      for f in (pf, gf, mf, vf)]
             self._torch_adamw(*views)
@@ -1154,7 +1198,11 @@ def lamb_scalars(lr: float, betas: tuple, eps: float, weight_decay: float, t: in
 
 class _LayerwiseOptimizer(_FlatOptimizer):
     """What :class:`FlatLAMB` and :class:`FlatLARS` share: the per-tensor adaptation flags, the trust ratios of the last
-    update, and on CUDA fp32 buckets the chunk table and the workspaces of the layer-wise kernels (csrc/layerwise.cu)."""
+    update, and on CUDA fp32 buckets the chunk table and the workspaces of the layer-wise kernels (csrc/layerwise.cu).
+    :attr:`param_groups` is one group with every parameter, whose ``lr`` / ``weight_decay`` are the optimizer's."""
+
+    lr = _group_attr("lr")
+    weight_decay = _group_attr("weight_decay")
 
     def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
                  max_grad_norm: Optional[float], sharded: bool, exclude_from_adaptation):
@@ -1221,7 +1269,8 @@ class FlatLAMB(_LayerwiseOptimizer):
                  weight_decay: float = 0.01, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
                  max_grad_norm: Optional[float] = None, sharded: bool = False, exclude_from_adaptation=None):
         self.betas = check_adamw_options(lr, betas, eps, weight_decay)
-        self.lr, self.eps, self.weight_decay = float(lr), float(eps), float(weight_decay)
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.eps = float(eps)
         super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, exclude_from_adaptation)
         self.exp_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
         self.exp_avg_sq_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
@@ -1239,7 +1288,7 @@ class FlatLAMB(_LayerwiseOptimizer):
             if kern:
                 self._kernel().lamb_flat(pf, mf, vf, g, *self._lw[k], self.ratio_flats[k], sc, self.fused_zero, **clip)
                 continue
-            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            gf = _fp32_grad(g, clip.get("grad_scale"))
             ratios = []
             for _, adapt, (p, gt, m, v) in self._tensors(k, [pf, gf, mf, vf]):
                 m.lerp_(gt, w1)
@@ -1298,7 +1347,8 @@ class FlatLARS(_LayerwiseOptimizer):
                  group=None, lr_schedule: Optional[LRSchedule] = None, max_grad_norm: Optional[float] = None,
                  sharded: bool = False, exclude_from_adaptation=None):
         check_lars_options(lr, momentum, weight_decay, trust_coefficient, eps, nesterov)
-        self.lr, self.momentum, self.weight_decay = float(lr), float(momentum), float(weight_decay)
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.momentum = float(momentum)
         self.trust_coefficient, self.eps, self.nesterov = float(trust_coefficient), float(eps), bool(nesterov)
         super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, exclude_from_adaptation)
         self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
@@ -1313,7 +1363,7 @@ class FlatLARS(_LayerwiseOptimizer):
                 self._kernel().lars_flat(pf, mf, g, *self._lw[k], self.ratio_flats[k], lr, self.momentum, wd, eta, eps,
                                          self.nesterov, self.fused_zero, **clip)
                 continue
-            gf = g if g.dtype == torch.float32 else g.to(torch.float32)
+            gf = _fp32_grad(g, clip.get("grad_scale"))
             ratios = []
             for _, adapt, (p, gt, m) in self._tensors(k, [pf, gf, mf]):
                 r = 1.0

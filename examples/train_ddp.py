@@ -15,6 +15,8 @@ the tutorial's loop, on synthetic data.
                                                                   # first 3 backwards under model.no_sync()
     python examples/train_ddp.py --ema-decay 0.99 --ema-every 2   # FlatEMA: an EMA of the weights, updated after every
                                                                   # 2nd step, evaluated on a held-out batch at the end
+    python examples/train_ddp.py --amp                            # fp16 autocast with torch.amp.GradScaler: the optimizer
+                                                                  # unscales, and skips steps whose gradients overflow
 
 The loop is ``backward(); average_gradients(model); optimizer.step()`` either way; with ``--accumulation-steps k`` the k - 1
 backwards before the last run inside ``model.no_sync()`` on losses scaled by 1 / k.  With ``--sharded-optimizer`` the update
@@ -22,6 +24,7 @@ happens inside ``average_gradients`` (during backward, bucket by bucket) and ``s
 gradient buckets the parameters are bit for bit the same.  Prints ``Rank r, step s: loss`` for the last step, and with
 ``--ema-decay`` a second line per rank, ``Rank r, EMA model: held-out loss``, the loss of the EMA weights on a fixed batch."""
 import argparse
+import contextlib
 import json
 import os
 import sys
@@ -54,24 +57,35 @@ def batch(step, rank, dev, micro=0):
     return torch.randn(16, 3, 16, 16, generator=g).to(dev), torch.randint(0, 10, (16,), generator=g).to(dev)
 
 
-def train_step(model, optimizer, micro_batches, ema=None):
+def train_step(model, optimizer, micro_batches, ema=None, scaler=None):
     """One optimizer step over ``micro_batches`` (a list of (x, y)): all but the last backward accumulate under no_sync(),
-    the last one exchanges the buckets; then the EMA update, if any.  Returns the last micro-batch's loss."""
+    the last one exchanges the buckets; then the EMA update, if any.  With ``scaler`` (--amp) the forwards run under fp16
+    autocast, the losses are scaled, and ``scaler.step`` / ``scaler.update`` replace ``optimizer.step()``: the optimizer
+    unscales the gradients and skips a step that overflowed.  Returns the last micro-batch's loss."""
     k = len(micro_batches)
+    amp = contextlib.nullcontext() if scaler is None else torch.autocast(micro_batches[0][0].device.type, dtype=torch.float16)
+    scale = (lambda t: t) if scaler is None else scaler.scale
     for x, y in micro_batches[:-1]:
         with model.no_sync():
-            (F.cross_entropy(model(x), y) / k).backward()
+            with amp:
+                part = F.cross_entropy(model(x), y) / k
+            scale(part).backward()
     x, y = micro_batches[-1]
-    loss = F.cross_entropy(model(x), y)
-    (loss / k).backward()
+    with amp:
+        loss = F.cross_entropy(model(x), y)
+    scale(loss / k).backward()
     dist.average_gradients(model)       # --sharded-optimizer: the parameters are updated when this returns
-    optimizer.step()
+    if scaler is None:
+        optimizer.step()
+    else:
+        scaler.step(optimizer)
+        scaler.update()
     if ema is not None:
         ema.update()                    # a capturable optimizer: the kernel decides skip / copy / lerp from its step counter
     return loss
 
 
-def train_graphed(model, optimizer, ema, rank, dev, steps, k, warmup=3):
+def train_graphed(model, optimizer, ema, rank, dev, steps, k, warmup=3, scaler=None):
     """--cuda-graph: ``warmup`` eager steps on a side stream (as torch requires before a capture), one step (all k
     micro-batches) captured, and every later step a ``copy_`` of its micro-batches into the static inputs and one replay.
     Returns the last step's loss."""
@@ -83,7 +97,7 @@ def train_graphed(model, optimizer, ema, rank, dev, steps, k, warmup=3):
                 t.copy_(src)
 
     def step():
-        return train_step(model, optimizer, static, ema)
+        return train_step(model, optimizer, static, ema, scaler)
 
     s = torch.cuda.Stream(dev)
     s.wait_stream(torch.cuda.current_stream(dev))
@@ -124,12 +138,13 @@ def run(rank, size):
     ema = None
     if CFG["ema_decay"] is not None:
         ema = dist.FlatEMA(optimizer, decay=CFG["ema_decay"], every=CFG["ema_every"], warmup_steps=CFG["ema_warmup_steps"])
+    scaler = torch.amp.GradScaler(dev.type) if CFG.get("amp") else None
     loss = None
     if CFG["cuda_graph"]:
-        loss = train_graphed(model, optimizer, ema, rank, dev, CFG["steps"], CFG["accumulation_steps"])
+        loss = train_graphed(model, optimizer, ema, rank, dev, CFG["steps"], CFG["accumulation_steps"], scaler=scaler)
     for step in range(0 if CFG["cuda_graph"] else CFG["steps"]):
         optimizer.zero_grad()
-        loss = train_step(model, optimizer, [batch(step, rank, dev, j) for j in range(CFG["accumulation_steps"])], ema)
+        loss = train_step(model, optimizer, [batch(step, rank, dev, j) for j in range(CFG["accumulation_steps"])], ema, scaler)
     total = loss.detach().clone()
     dist.all_reduce(total)
     if CFG["optimizer"] in ("adamw", "lamb"):
@@ -143,6 +158,8 @@ def run(rank, size):
         with ema.average_parameters(), torch.no_grad():
             held_out = F.cross_entropy(model(x), y)
         print(f"Rank {rank}, EMA model: held-out loss {float(held_out):.6f}")
+    if scaler is not None:
+        print(f"Rank {rank}, loss scale {scaler.get_scale():g}, updates applied {optimizer.steps} of {CFG['steps']}")
 
 
 if __name__ == "__main__":
@@ -165,7 +182,12 @@ if __name__ == "__main__":
     ap.add_argument("--ema-every", type=int, default=1, help="with --ema-decay: update the EMA after every k-th step")
     ap.add_argument("--ema-warmup-steps", type=int, default=0,
                     help="with --ema-decay: copy the weights instead of averaging them up to this step")
+    ap.add_argument("--amp", action="store_true",
+                    help="fp16 autocast and torch.amp.GradScaler (dynamic loss scale; overflowing steps are skipped)")
     a = ap.parse_args()
+    if a.amp and a.sharded_optimizer and a.size > 1:
+        ap.error("--amp needs an unsharded optimizer when --size > 1: the sharded exchange applies the update during "
+                 "backward, before GradScaler can check the gradients")
     if a.accumulation_steps < 1:
         ap.error("--accumulation-steps must be at least 1")
     if a.cuda_graph and (a.optimizer not in ("sgd", "adamw") or a.backend != "b200"):
@@ -176,5 +198,5 @@ if __name__ == "__main__":
                                                 optimizer=a.optimizer, no_decay=a.no_decay_bias_norm,
                                                 cuda_graph=a.cuda_graph, accumulation_steps=a.accumulation_steps,
                                                 ema_decay=a.ema_decay, ema_every=a.ema_every,
-                                                ema_warmup_steps=a.ema_warmup_steps))
+                                                ema_warmup_steps=a.ema_warmup_steps, amp=a.amp))
     dist.launch(run, size=a.size, backend=a.backend)
