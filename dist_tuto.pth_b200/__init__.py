@@ -16,6 +16,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
     SyncBatchNorm (global-batch statistics)            parallel/sync_bn.py
     FlatSGD (one-launch momentum SGD over flat buffers) ops/optim.py
     FlatAdamW (one-launch AdamW over flat buffers)      ops/optim.py
+    FlatRMSprop (one-launch RMSprop over flat buffers)  ops/optim.py
     FlatLAMB FlatLARS (per-tensor trust ratios)         ops/optim.py
     FlatEMA (EMA of the weights, one launch per update) ops/optim.py
     GradScaler support (fp16 loss scaling, in-kernel)   ops/optim.py
@@ -36,7 +37,7 @@ from .models.convnet import Net  # noqa: F401
 from .parallel.ddp import (average_gradients, GradBucket, DistributedDataParallel,  # noqa: F401
                            broadcast_parameters)
 from .parallel.sync_bn import SyncBatchNorm  # noqa: F401
-from .ops.optim import FlatAdamW, FlatEMA, FlatLAMB, FlatLARS, FlatSGD, LRSchedule  # noqa: F401
+from .ops.optim import FlatAdamW, FlatEMA, FlatLAMB, FlatLARS, FlatRMSprop, FlatSGD, LRSchedule  # noqa: F401
 from .ops.convnet_eval import evaluate  # noqa: F401
 from .train import run, train, TrainConfig  # noqa: F401
 

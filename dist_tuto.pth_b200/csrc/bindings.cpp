@@ -20,6 +20,7 @@
 #include "layerwise.h"
 #include "loader.h"
 #include "param_groups.h"
+#include "rmsprop.h"
 
 #define B2_MAX_RANKS 8
 struct PeerPtrs { void* p[B2_MAX_RANKS]; };
@@ -116,6 +117,18 @@ int b2_sharded_sgd_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* p
 int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* exp_avg,
                                 float* exp_avg_sq, const uint8_t* map, const b2::FlatScalars* blk, size_t n_vec, float scale,
                                 int zero_grad, int rank, int world, int max_blocks, cudaStream_t stream);
+int b2_rmsprop_flat_launch(float* p, float* sq, float* ga, float* buf, float* g, size_t n, const uint8_t* map,
+                           const b2::RmspropScalars* s, const b2::SgdGroups* gs, int n_groups, const b2::FlatScalars* blk,
+                           int zero_grad, float max_norm, const double* sqnorms, int n_buckets, float* grad_norm_out,
+                           const float* grad_scale, const float* found_inf, cudaStream_t stream);
+int b2_sharded_rmsprop_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig, float* square_avg,
+                              float* grad_avg, float* momentum_buffer, const uint8_t* map, const b2::RmspropScalars* s,
+                              const b2::SgdGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank, int world,
+                              int max_blocks, cudaStream_t stream);
+int b2_sharded_rmsprop_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const SignalPadsH* sig,
+                                  float* square_avg, float* grad_avg, float* momentum_buffer, const uint8_t* map,
+                                  const b2::FlatScalars* blk, const b2::RmspropScalars* s, size_t n_vec, float scale, int zero_grad,
+                                  int rank, int world, int max_blocks, cudaStream_t stream);
 int b2_ema_launch(const b2::EmaEntry* table, int n_entries, long long n_vec, long long n_scalar, float w, int mode,
                   const long long* counter, long long every, long long warmup, cudaStream_t stream);
 int b2_grad_sqnorm_ws_floats();
@@ -255,6 +268,40 @@ b2::AdamwScalars to_adamw(const std::vector<double>& v, const char* what) {
   a.decay = (float)v[0]; a.w1 = (float)v[1]; a.beta2 = (float)v[2]; a.c2 = (float)v[3];
   a.step_size = (float)v[4]; a.sbc2 = (float)v[5]; a.eps = (float)v[6];
   return a;
+}
+
+// One RMSprop update's scalars (csrc/rmsprop.h), computed by the host in fp64 (ops/optim.py rmsprop_scalars): (lr,
+// weight_decay, alpha, 1 - alpha, eps, momentum), each rounded once to fp32 here.  `centered` and momentum > 0 say which
+// optional states the update has.
+b2::RmspropScalars to_rmsprop(const std::vector<double>& v, bool centered, const char* what) {
+  TORCH_CHECK(v.size() == 6, what, ": scalars: (lr, weight_decay, alpha, 1 - alpha, eps, momentum), got ", v.size(), " values");
+  for (double x : v) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), what, ": scalars must be finite in fp32");
+  TORCH_CHECK(v[1] >= 0.0 && v[2] >= 0.0 && v[4] >= 0.0 && v[5] >= 0.0, what,
+              ": weight_decay, alpha, eps and momentum must be >= 0");
+  b2::RmspropScalars s;
+  s.lr = (float)v[0]; s.wd = (float)v[1]; s.alpha = (float)v[2]; s.c = (float)v[3]; s.eps = (float)v[4]; s.mu = (float)v[5];
+  s.centered = centered ? 1 : 0;
+  s.momentum = v[5] > 0.0 ? 1 : 0;
+  return s;
+}
+
+// The state flats of an RMSprop update: square_avg, plus grad_avg exactly when centered and momentum_buffer exactly when
+// momentum > 0; contiguous 16-byte aligned fp32 on `like`'s device with `n` elements (at_least: n or more).  Returns the
+// optional states' pointers, null when absent.
+std::pair<float*, float*> rmsprop_state(const torch::Tensor& square_avg, const c10::optional<torch::Tensor>& grad_avg,
+                                        const c10::optional<torch::Tensor>& momentum_buffer, const b2::RmspropScalars& s,
+                                        int64_t n, bool at_least, const torch::Tensor& like, const char* what) {
+  TORCH_CHECK(grad_avg.has_value() == (s.centered != 0), what, ": grad_avg is given exactly when centered=True");
+  TORCH_CHECK(momentum_buffer.has_value() == (s.momentum != 0), what, ": momentum_buffer is given exactly when momentum > 0");
+  for (const torch::Tensor* t : {&square_avg, grad_avg.has_value() ? &*grad_avg : &square_avg,
+                                 momentum_buffer.has_value() ? &*momentum_buffer : &square_avg}) {
+    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32 && t->device() == like.device() &&
+                (at_least ? t->numel() >= n : t->numel() == n) && (uintptr_t)t->data_ptr() % 16 == 0, what,
+                ": square_avg, grad_avg and momentum_buffer: 16-byte aligned contiguous fp32 CUDA of ", at_least ? "at least " : "",
+                n, " elements on the parameters' device");
+  }
+  return {grad_avg.has_value() ? grad_avg->data_ptr<float>() : nullptr,
+          momentum_buffer.has_value() ? momentum_buffer->data_ptr<float>() : nullptr};
 }
 
 // Parameter groups (csrc/param_groups.h): the group map of `n_ids` parameter vectors (uint8 CUDA, 1..64 groups) and two
@@ -1374,6 +1421,163 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("scalars"),
      py::arg("decays"), py::arg("step_sizes"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
      py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
+  // FlatRMSprop's update of one fp32 bucket (csrc/rmsprop.cu).  scalars (fp64, each rounded once to fp32): (lr, weight_decay,
+  // alpha, 1 - alpha, eps, momentum); grad_avg with centered, momentum_buffer with momentum > 0.  With max_grad_norm, g is
+  // first scaled by the clip coefficient of the norm of grad_sqnorm's per-bucket sums; with grad_scale, first unscaled.
+  // group_map (rmsprop_flat_grouped: lrs / weight_decays per group, rmsprop_flat_cap: from the block) picks each parameter
+  // vector's lr and weight decay, which scalars then do not give.
+  auto rmsprop_flat = [](const char* what, torch::Tensor& p, torch::Tensor& square_avg, const c10::optional<torch::Tensor>& grad_avg,
+                         const c10::optional<torch::Tensor>& momentum_buffer, torch::Tensor& g,
+                         const c10::optional<torch::Tensor>& group_map, const std::vector<double>* lrs,
+                         const std::vector<double>* weight_decays, const torch::Tensor* block, const std::vector<double>& scalars,
+                         bool centered, bool zero_grad, const py::object& max_grad_norm, const c10::optional<torch::Tensor>& sqnorms,
+                         const c10::optional<torch::Tensor>& grad_norm_out, const c10::optional<torch::Tensor>& grad_scale,
+                         const c10::optional<torch::Tensor>& found_inf) {
+    const b2::RmspropScalars sc = to_rmsprop(scalars, centered, what);
+    const float max_norm = check_max_grad_norm(max_grad_norm, what);
+    const double* sq = nullptr;
+    int n_buckets = 0;
+    if (max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      sq = sqnorms->data_ptr<double>();
+      n_buckets = (int)sqnorms->numel();
+    }
+    float* gn = grad_norm_ptr(grad_norm_out, what);
+    for (const auto* t : {&p, &g}) {
+      check_cuda_contig(*t, what);
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0, what,
+                  ": p and g: 16-byte aligned fp32 of one size");
+    }
+    const auto opt = rmsprop_state(square_avg, grad_avg, momentum_buffer, sc, p.numel(), false, p, what);
+    const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, what);
+    b2::SgdGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    int n_groups = 0;
+    if (lrs != nullptr) {
+      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
+      n_groups = check_groups(*group_map, (p.numel() + 3) / 4, *lrs, *weight_decays, gs.lr, gs.wd, what);
+    }
+    const b2::FlatScalars* blk = block != nullptr ? flat_block(*block, p, what) : nullptr;
+    const float* gsc = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
+    const float* fi = amp_scalar_ptr(found_inf, p, what, "found_inf");
+    TORCH_CHECK(blk == nullptr || fi != nullptr || gsc == nullptr, what, ": grad_scale comes with found_inf (GradScaler sets both)");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_rmsprop_flat_launch(p.data_ptr<float>(), square_avg.data_ptr<float>(), opt.first, opt.second, g.data_ptr<float>(),
+                                   (size_t)p.numel(), map, &sc, &gs, n_groups, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
+                                   gsc, fi, cur_stream()),
+            what);
+  };
+  m.def("rmsprop_flat", [rmsprop_flat](torch::Tensor p, torch::Tensor square_avg, c10::optional<torch::Tensor> grad_avg,
+                                       c10::optional<torch::Tensor> momentum_buffer, torch::Tensor g, std::vector<double> scalars,
+                                       bool centered, bool zero_grad, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                                       c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
+    rmsprop_flat("rmsprop_flat", p, square_avg, grad_avg, momentum_buffer, g, c10::nullopt, nullptr, nullptr, nullptr, scalars,
+                 centered, zero_grad, max_grad_norm, sqnorms, grad_norm_out, grad_scale, c10::nullopt);
+  }, py::arg("p"), py::arg("square_avg"), py::arg("grad_avg"), py::arg("momentum_buffer"), py::arg("g"), py::arg("scalars"),
+     py::arg("centered"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
+  m.def("rmsprop_flat_grouped", [rmsprop_flat](torch::Tensor p, torch::Tensor square_avg, c10::optional<torch::Tensor> grad_avg,
+                                               c10::optional<torch::Tensor> momentum_buffer, torch::Tensor g, torch::Tensor group_map,
+                                               std::vector<double> scalars, bool centered, std::vector<double> lrs,
+                                               std::vector<double> weight_decays, bool zero_grad, py::object max_grad_norm,
+                                               c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                               c10::optional<torch::Tensor> grad_scale) {
+    rmsprop_flat("rmsprop_flat_grouped", p, square_avg, grad_avg, momentum_buffer, g, group_map, &lrs, &weight_decays, nullptr,
+                 scalars, centered, zero_grad, max_grad_norm, sqnorms, grad_norm_out, grad_scale, c10::nullopt);
+  }, py::arg("p"), py::arg("square_avg"), py::arg("grad_avg"), py::arg("momentum_buffer"), py::arg("g"), py::arg("group_map"),
+     py::arg("scalars"), py::arg("centered"), py::arg("lrs"), py::arg("weight_decays"), py::arg("zero_grad"),
+     py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
+     py::arg("grad_scale") = py::none());
+  m.def("rmsprop_flat_cap", [rmsprop_flat](torch::Tensor p, torch::Tensor square_avg, c10::optional<torch::Tensor> grad_avg,
+                                           c10::optional<torch::Tensor> momentum_buffer, torch::Tensor g,
+                                           c10::optional<torch::Tensor> group_map, torch::Tensor block, std::vector<double> scalars,
+                                           bool centered, bool zero_grad, py::object max_grad_norm,
+                                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                           c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
+    rmsprop_flat("rmsprop_flat_cap", p, square_avg, grad_avg, momentum_buffer, g, group_map, nullptr, nullptr, &block, scalars,
+                 centered, zero_grad, max_grad_norm, sqnorms, grad_norm_out, grad_scale, found_inf);
+  }, py::arg("p"), py::arg("square_avg"), py::arg("grad_avg"), py::arg("momentum_buffer"), py::arg("g"), py::arg("group_map"),
+     py::arg("block"), py::arg("scalars"), py::arg("centered"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
+     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(),
+     py::arg("found_inf") = py::none());
+  // The sharded step of one bucket with RMSprop (csrc/sharded_sgd.cu, the RMSprop instances): as sharded_adamw, with this rank's
+  // square_avg shard and, with centered / momentum > 0, its grad_avg / momentum_buffer shards.  sharded_rmsprop_grouped:
+  // group_map holds this rank's ids and lrs / weight_decays the groups'; sharded_rmsprop_cap: lr and weight decay (with
+  // group_map: every group's) from the block.
+  auto sharded_rmsprop = [](const char* what, bool bf16, const std::vector<unsigned long long>& grads,
+                            const std::vector<unsigned long long>& params, const std::vector<unsigned long long>& sigs,
+                            torch::Tensor& square_avg, const c10::optional<torch::Tensor>& grad_avg,
+                            const c10::optional<torch::Tensor>& momentum_buffer, const c10::optional<torch::Tensor>& group_map,
+                            const std::vector<double>* lrs, const std::vector<double>* weight_decays, const torch::Tensor* block,
+                            size_t n_vec, const std::vector<double>& scalars, bool centered, double scale, bool zero_grad, int rank,
+                            int world, int max_blocks) {
+    check_world(rank, world, what);
+    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world, what,
+                ": one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ", params.size(),
+                " and ", sigs.size(), " for world ", world);
+    TORCH_CHECK(n_vec % (size_t)world == 0, what, ": every rank owns n_vec / world vectors, so n_vec must be a multiple of world "
+                "(pad the buffers), got n_vec ", n_vec, " for world ", world);
+    const b2::RmspropScalars sc = to_rmsprop(scalars, centered, what);
+    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
+    const auto opt = rmsprop_state(square_avg, grad_avg, momentum_buffer, sc, (int64_t)shard, true, square_avg, what);
+    for (const auto* v : {&grads, &params, &sigs})
+      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, what, ": null or misaligned per-rank pointer");
+    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), what);
+    b2::SgdGroups gs;
+    memset(&gs, 0, sizeof(gs));
+    int n_groups = 0;
+    if (lrs != nullptr) {
+      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
+      n_groups = check_groups(*group_map, (int64_t)(shard / 4), *lrs, *weight_decays, gs.lr, gs.wd, what);
+    }
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(square_avg.device());
+    if (block != nullptr) {
+      const b2::FlatScalars* blk = flat_block(*block, square_avg, what);
+      ck_cuda(b2_sharded_rmsprop_cap_launch(bf16 ? 1 : 0, &g, &p, &s, square_avg.data_ptr<float>(), opt.first, opt.second, map, blk,
+                                            &sc, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+              what);
+      return;
+    }
+    ck_cuda(b2_sharded_rmsprop_launch(bf16 ? 1 : 0, &g, &p, &s, square_avg.data_ptr<float>(), opt.first, opt.second, map, &sc, &gs,
+                                      n_groups, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+            what);
+  };
+  m.def("sharded_rmsprop", [sharded_rmsprop](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                             std::vector<unsigned long long> sigs, torch::Tensor square_avg,
+                                             c10::optional<torch::Tensor> grad_avg, c10::optional<torch::Tensor> momentum_buffer,
+                                             size_t n_vec, std::vector<double> scalars, bool centered, double scale, bool zero_grad,
+                                             int rank, int world, int max_blocks) {
+    sharded_rmsprop("sharded_rmsprop", bf16, grads, params, sigs, square_avg, grad_avg, momentum_buffer, c10::nullopt, nullptr,
+                    nullptr, nullptr, n_vec, scalars, centered, scale, zero_grad, rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("square_avg"), py::arg("grad_avg"),
+     py::arg("momentum_buffer"), py::arg("n_vec"), py::arg("scalars"), py::arg("centered"), py::arg("scale"), py::arg("zero_grad"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  m.def("sharded_rmsprop_grouped", [sharded_rmsprop](bool bf16, std::vector<unsigned long long> grads,
+                                                     std::vector<unsigned long long> params, std::vector<unsigned long long> sigs,
+                                                     torch::Tensor square_avg, c10::optional<torch::Tensor> grad_avg,
+                                                     c10::optional<torch::Tensor> momentum_buffer, torch::Tensor group_map, size_t n_vec,
+                                                     std::vector<double> scalars, bool centered, std::vector<double> lrs,
+                                                     std::vector<double> weight_decays, double scale, bool zero_grad, int rank,
+                                                     int world, int max_blocks) {
+    sharded_rmsprop("sharded_rmsprop_grouped", bf16, grads, params, sigs, square_avg, grad_avg, momentum_buffer, group_map, &lrs,
+                    &weight_decays, nullptr, n_vec, scalars, centered, scale, zero_grad, rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("square_avg"), py::arg("grad_avg"),
+     py::arg("momentum_buffer"), py::arg("group_map"), py::arg("n_vec"), py::arg("scalars"), py::arg("centered"), py::arg("lrs"),
+     py::arg("weight_decays"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  m.def("sharded_rmsprop_cap", [sharded_rmsprop](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                                 std::vector<unsigned long long> sigs, torch::Tensor square_avg,
+                                                 c10::optional<torch::Tensor> grad_avg, c10::optional<torch::Tensor> momentum_buffer,
+                                                 c10::optional<torch::Tensor> group_map, torch::Tensor block, size_t n_vec,
+                                                 std::vector<double> scalars, bool centered, double scale, bool zero_grad, int rank,
+                                                 int world, int max_blocks) {
+    sharded_rmsprop("sharded_rmsprop_cap", bf16, grads, params, sigs, square_avg, grad_avg, momentum_buffer, group_map, nullptr,
+                    nullptr, &block, n_vec, scalars, centered, scale, zero_grad, rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("square_avg"), py::arg("grad_avg"),
+     py::arg("momentum_buffer"), py::arg("group_map"), py::arg("block"), py::arg("n_vec"), py::arg("scalars"), py::arg("centered"),
+     py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
   m.def("layerwise_chunk_elems", [] { return (int64_t)b2::kLwChunk; }, "the largest chunk of a layer-wise chunk table");
   m.def("layerwise_table", &layerwise_table, py::arg("offsets"), py::arg("numels"), py::arg("adapt"), py::arg("n"),
         py::arg("device"), "FlatLAMB / FlatLARS: (the chunk table of one bucket on `device`, its number of chunks)");

@@ -33,12 +33,18 @@
 // Capturable<U> (FlatSGD / FlatAdamW capturable=True, flat_scalars.cuh) is U with its scalars read from the device scalar
 // block: the skeleton calls its begin() once per CTA, which copies them to shared memory; the other instances compile
 // without that call.
+//
+// ShardedRmspropUpdate and ShardedRmspropGroupedUpdate (FlatRMSprop) are two more update types of the same skeleton:
+// rmsprop_elem of rmsprop_device.cuh on the slice's square-average shard and, when the update has them, its momentum and
+// centered-average shards.  Capturable<U> takes their lr and weight decay from the block, the other scalars from the
+// arguments.
 #include <cstring>
 #include <type_traits>
 #include "adamw_device.cuh"
 #include "common.cuh"
 #include "flat_scalars.cuh"
 #include "param_groups.cuh"
+#include "rmsprop_device.cuh"
 
 namespace b2 {
 
@@ -93,6 +99,36 @@ struct ShardedAdamwGroupedArgs {
   float scale;
   int rank, world, zero_grad;
   AdamwGroups gs;
+};
+
+// FlatRMSprop: this rank's shards of the square average and, when they exist (s.centered / s.momentum), of the centered
+// gradient average and the momentum buffer; null otherwise.  Grouped: `s` without lr / wd, which come from the vector's group.
+struct ShardedRmspropArgs {
+  PeerPtrs grads;
+  PeerPtrs params;
+  SignalPads sig;
+  float* square_avg;
+  float* grad_avg;
+  float* momentum_buffer;
+  size_t n_vec;
+  RmspropScalars s;
+  float scale;
+  int rank, world, zero_grad;
+};
+
+struct ShardedRmspropGroupedArgs {
+  PeerPtrs grads;
+  PeerPtrs params;
+  SignalPads sig;
+  float* square_avg;
+  float* grad_avg;
+  float* momentum_buffer;
+  const uint8_t* map;
+  size_t n_vec;
+  RmspropScalars s;
+  float scale;
+  int rank, world, zero_grad;
+  SgdGroups gs;
 };
 
 // The per-vector updates of sharded_step_kernel.  q indexes the fp32 state vector within this rank's shard.
@@ -160,6 +196,48 @@ struct ShardedAdamwGroupedUpdate {
   }
 };
 
+// RMSprop: up to three state vectors per parameter vector, so one gradient vector per thread and pass as for AdamW.  The
+// absent states are neither loaded nor stored (uniform branches on s.centered / s.momentum).
+template <class A>
+__device__ __forceinline__ void rmsprop_load(const A& a, size_t q, float4& sq, float4& ga, float4& buf) {
+  sq = reinterpret_cast<float4*>(a.square_avg)[q];
+  if (a.s.centered) ga = reinterpret_cast<float4*>(a.grad_avg)[q];
+  if (a.s.momentum) buf = reinterpret_cast<float4*>(a.momentum_buffer)[q];
+}
+template <class A>
+__device__ __forceinline__ void rmsprop_store(const A& a, size_t q, float4 sq, float4 ga, float4 buf) {
+  reinterpret_cast<float4*>(a.square_avg)[q] = sq;
+  if (a.s.centered) reinterpret_cast<float4*>(a.grad_avg)[q] = ga;
+  if (a.s.momentum) reinterpret_cast<float4*>(a.momentum_buffer)[q] = buf;
+}
+
+struct ShardedRmspropUpdate {
+  using Args = ShardedRmspropArgs;
+  static constexpr int kUnroll = 1;
+  float4 sq, ga, buf;
+  __device__ __forceinline__ void load(const Args& a, size_t q) { rmsprop_load(a, q, sq, ga, buf); }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) { rmsprop4(p, sq, ga, buf, g, a.s); }
+  __device__ __forceinline__ void store(const Args& a, size_t q) { rmsprop_store(a, q, sq, ga, buf); }
+};
+
+struct ShardedRmspropGroupedUpdate {
+  using Args = ShardedRmspropGroupedArgs;
+  static constexpr int kUnroll = 1;
+  float4 sq, ga, buf;
+  int gid;
+  __device__ __forceinline__ void load(const Args& a, size_t q) {
+    rmsprop_load(a, q, sq, ga, buf);
+    gid = a.map[q];
+  }
+  __device__ __forceinline__ void apply(const Args& a, float4& p, float4 g) {
+    RmspropScalars s = a.s;
+    s.lr = a.gs.lr[gid];
+    s.wd = a.gs.wd[gid];
+    rmsprop4(p, sq, ga, buf, g, s);
+  }
+  __device__ __forceinline__ void store(const Args& a, size_t q) { rmsprop_store(a, q, sq, ga, buf); }
+};
+
 // Capturable instances (flat_scalars.cuh): Capturable<U> is the update U with the scalars its apply() reads taken from the
 // scalar block on the device instead of the kernel arguments.  Its begin(), which the skeleton calls once per CTA, copies them
 // into a shared copy of U's arguments; load(), apply() and store() are U's, apply() reading that copy.
@@ -176,6 +254,14 @@ __device__ __forceinline__ void cap_fill(ShardedSgdGroupedArgs& s, const Sharded
 __device__ __forceinline__ void cap_fill(ShardedAdamwGroupedArgs& s, const ShardedAdamwGroupedArgs&, const FlatScalars& b) {
   flat_block_load(s.s, b.adamw);
   flat_block_load(s.gs, b.adamw_groups);
+}
+
+__device__ __forceinline__ void cap_fill(ShardedRmspropArgs& s, const ShardedRmspropArgs& a, const FlatScalars& b) {
+  if (threadIdx.x == 0) { s.s = a.s; s.s.lr = b.lr; s.s.wd = b.wd; }
+}
+__device__ __forceinline__ void cap_fill(ShardedRmspropGroupedArgs& s, const ShardedRmspropGroupedArgs& a, const FlatScalars& b) {
+  flat_block_load(s.gs, b.sgd);
+  if (threadIdx.x == 0) s.s = a.s;
 }
 
 template <class A>
@@ -462,6 +548,77 @@ int b2_sharded_adamw_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs*
   a.scale = scale; a.rank = rank; a.world = world; a.zero_grad = zero_grad; a.blk = blk;
   if (bf16) sharded_step_kernel<true, Capturable<ShardedAdamwUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
   else sharded_step_kernel<false, Capturable<ShardedAdamwUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// The steps with RMSprop (FlatRMSprop): `square_avg` is this rank's shard (n_vec / world x 4 (x 8) floats), and `grad_avg` /
+// `momentum_buffer` its shards of the centered average and the momentum buffer, or null when the update is not centered / has
+// no momentum (s->centered / s->momentum are set here from them).  `map`: null without groups, else this rank's group ids with
+// `gs` the lr and weight decay of n_groups groups.  Same grid, same refusals, and also cudaErrorInvalidValue, without a launch,
+// for n_groups outside 1..64 with a map.
+int b2_sharded_rmsprop_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig, float* square_avg,
+                              float* grad_avg, float* momentum_buffer, const uint8_t* map, const b2::RmspropScalars* s,
+                              const b2::SgdGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank, int world,
+                              int max_blocks, cudaStream_t stream) {
+  if (square_avg == nullptr || s == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world)) return (int)cudaErrorInvalidValue;
+  using namespace b2;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  if (map != nullptr) {
+    if (gs == nullptr || n_groups < 1 || n_groups > kMaxGroups) return (int)cudaErrorInvalidValue;
+    ShardedRmspropGroupedArgs a;
+    memset(&a, 0, sizeof(a));
+    a.grads = *grads; a.params = *params; a.sig = *sig; a.square_avg = square_avg; a.grad_avg = grad_avg;
+    a.momentum_buffer = momentum_buffer; a.map = map; a.n_vec = n_vec; a.s = *s; a.gs = *gs; a.scale = scale; a.rank = rank;
+    a.world = world; a.zero_grad = zero_grad;
+    a.s.centered = grad_avg != nullptr ? 1 : 0;
+    a.s.momentum = momentum_buffer != nullptr ? 1 : 0;
+    if (bf16) sharded_step_kernel<true, ShardedRmspropGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, ShardedRmspropGroupedUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+    return (int)cudaGetLastError();
+  }
+  ShardedRmspropArgs a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.square_avg = square_avg; a.grad_avg = grad_avg;
+  a.momentum_buffer = momentum_buffer; a.n_vec = n_vec; a.s = *s; a.scale = scale; a.rank = rank; a.world = world;
+  a.zero_grad = zero_grad;
+  a.s.centered = grad_avg != nullptr ? 1 : 0;
+  a.s.momentum = momentum_buffer != nullptr ? 1 : 0;
+  if (bf16) sharded_step_kernel<true, ShardedRmspropUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  else sharded_step_kernel<false, ShardedRmspropUpdate><<<grid, kShardThreads, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// The capturable RMSprop steps (Capturable<U>): lr and weight decay (with `map`: every group's) from the block `blk`, alpha,
+// 1 - alpha, eps and momentum from `s`.  Same refusals, and a null block is refused too.
+int b2_sharded_rmsprop_cap_launch(int bf16, const PeerPtrs* grads, const PeerPtrs* params, const b2::SignalPads* sig,
+                                  float* square_avg, float* grad_avg, float* momentum_buffer, const uint8_t* map,
+                                  const b2::FlatScalars* blk, const b2::RmspropScalars* s, size_t n_vec, float scale, int zero_grad,
+                                  int rank, int world, int max_blocks, cudaStream_t stream) {
+  if (square_avg == nullptr || s == nullptr || blk == nullptr || !shard_args_ok(grads, params, sig, n_vec, rank, world))
+    return (int)cudaErrorInvalidValue;
+  using namespace b2;
+  const dim3 grid = shard_grid(n_vec, world, max_blocks);
+  if (map != nullptr) {
+    CapArgs<ShardedRmspropGroupedArgs> a;
+    memset(&a, 0, sizeof(a));
+    a.grads = *grads; a.params = *params; a.sig = *sig; a.square_avg = square_avg; a.grad_avg = grad_avg;
+    a.momentum_buffer = momentum_buffer; a.map = map; a.n_vec = n_vec; a.s = *s; a.scale = scale; a.rank = rank;
+    a.world = world; a.zero_grad = zero_grad; a.blk = blk;
+    a.s.centered = grad_avg != nullptr ? 1 : 0;
+    a.s.momentum = momentum_buffer != nullptr ? 1 : 0;
+    if (bf16) sharded_step_kernel<true, Capturable<ShardedRmspropGroupedUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+    else sharded_step_kernel<false, Capturable<ShardedRmspropGroupedUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+    return (int)cudaGetLastError();
+  }
+  CapArgs<ShardedRmspropArgs> a;
+  memset(&a, 0, sizeof(a));
+  a.grads = *grads; a.params = *params; a.sig = *sig; a.square_avg = square_avg; a.grad_avg = grad_avg;
+  a.momentum_buffer = momentum_buffer; a.n_vec = n_vec; a.s = *s; a.scale = scale; a.rank = rank; a.world = world;
+  a.zero_grad = zero_grad; a.blk = blk;
+  a.s.centered = grad_avg != nullptr ? 1 : 0;
+  a.s.momentum = momentum_buffer != nullptr ? 1 : 0;
+  if (bf16) sharded_step_kernel<true, Capturable<ShardedRmspropUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
+  else sharded_step_kernel<false, Capturable<ShardedRmspropUpdate>><<<grid, kShardThreads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 

@@ -20,6 +20,9 @@ separate update kernel runs.
 and with ``sharded=True`` the AdamW instance of the same sharded kernel, with both moments sharded.  Both optimizers share
 the layout, the sharding, the exchange hooks and the step bookkeeping (``_FlatOptimizer``).
 
+``FlatRMSprop`` is ``torch.optim.RMSprop`` on the same layout: one ``rmsprop_flat_kernel`` launch per bucket (csrc/rmsprop.cu),
+and with ``sharded=True`` the RMSprop instances of the sharded kernel, with every state sharded.
+
 ``FlatSGD`` and ``FlatAdamW`` take torch-style ``param_groups`` (per-group lr and weight decay): the same launches with a
 per-vector group map and the groups' scalars in the kernel arguments.
 
@@ -42,8 +45,8 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "FlatAdamW", "FlatLAMB", "FlatLARS", "FlatEMA", "LRSchedule", "adamw_scalars", "lamb_scalars", "exclude_1d",
-           "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
+__all__ = ["FlatSGD", "FlatAdamW", "FlatRMSprop", "FlatLAMB", "FlatLARS", "FlatEMA", "LRSchedule", "adamw_scalars",
+           "rmsprop_scalars", "lamb_scalars", "exclude_1d", "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -1182,6 +1185,224 @@ class FlatAdamW(_FlatOptimizer):
         return done
 
 
+def check_rmsprop_options(lr: float, alpha: float, eps: float, weight_decay: float, momentum: float) -> None:
+    """``torch.optim.RMSprop``'s rules for the hyper-parameters, with its messages."""
+    if not 0.0 <= float(lr):
+        raise ValueError(f"Invalid learning rate: {lr}")
+    if not 0.0 <= float(eps):
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    if not 0.0 <= float(momentum):
+        raise ValueError(f"Invalid momentum value: {momentum}")
+    if not 0.0 <= float(weight_decay):
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+    if not 0.0 <= float(alpha):
+        raise ValueError(f"Invalid alpha value: {alpha}")
+
+
+def rmsprop_scalars(lr: float, alpha: float, eps: float, weight_decay: float, momentum: float) -> list:
+    """The scalars of one RMSprop update that the kernels take (csrc/rmsprop.h), in fp64:
+    ``[lr, weight_decay, alpha, 1 - alpha, eps, momentum]``.  The bindings round each once to fp32."""
+    return [float(lr), float(weight_decay), float(alpha), 1.0 - float(alpha), float(eps), float(momentum)]
+
+
+class FlatRMSprop(_FlatOptimizer):
+    """``torch.optim.RMSprop`` (``maximize=False``) over flat buffers: ``FlatRMSprop(model)`` where ``model`` is a plain
+    module, a module carrying ``_grad_bucket`` or a :class:`DistributedDataParallel` wrapper, in the same loop as
+    :class:`FlatSGD` (``backward(); average_gradients(model); opt.step()``).  torchvision's classification recipes train
+    with it as ``RMSprop(params, lr, alpha=0.9, eps=0.0316, momentum=0.9, weight_decay=wd)``.
+
+    The state flats have the parameter flats' layout: ``square_avg_flats``, plus ``momentum_buffer_flats`` when
+    ``momentum > 0`` and ``grad_avg_flats`` when ``centered`` (empty lists otherwise).  On CUDA fp32 buckets ONE
+    ``rmsprop_flat`` launch per bucket (csrc/rmsprop.cu) streams the parameters, gradients and states once, and with
+    ``zero_grad=True`` (default) re-zeroes the gradients in the same pass.  ``weight_decay`` is torch's coupled L2 decay
+    (``g + wd * p`` before the square average).  Update k (``steps`` before it) uses ``lr = lr_at()`` (:class:`LRSchedule`).
+    Elsewhere (CPU tensors, bf16 buckets) torch's own single-tensor RMSprop runs on each parameter's views of the flats, so a
+    CPU run is bit for bit ``torch.optim.RMSprop(foreach=False)``.  ``maximize``, ``differentiable`` and ``foreach`` are not
+    taken.
+
+    Everything else is :class:`FlatAdamW`'s: ``max_grad_norm`` (on-device clipping, :meth:`grad_norm`); ``sharded=True``
+    (ZeRO stage 1: per bucket ONE ``sharded_rmsprop`` kernel reduce-scatters the gradients in fp32 in rank order, applies
+    RMSprop to the owned slice with every state sharded 1/W, and stores the new parameters into every rank's flat, inside
+    ``average_gradients`` / the DDP hooks; torch ops without one peer-memory world; nothing changes at world size 1; refused
+    with ``max_grad_norm``); ``param_groups`` (per-group ``lr`` / ``weight_decay``: ``rmsprop_flat_grouped``,
+    ``sharded_rmsprop_grouped``); ``capturable=True`` (the scheduled lr and weight decay of every group come from the device
+    scalar block, so a CUDA graph captures the whole step; RMSprop has no other step-dependent scalar); ``no_sync()``
+    accumulation, :class:`FlatEMA` and ``torch.amp.GradScaler``.  :meth:`named_state` (collective when sharded) is
+    ``torch.optim.RMSprop``'s per-parameter state by parameter name."""
+
+    lr = _group_attr("lr")
+    weight_decay = _group_attr("weight_decay")
+    sync_hyperparameters = _FlatOptimizer._sync_hyperparameters
+
+    def __init__(self, model: nn.Module, lr: float = 1e-2, alpha: float = 0.99, eps: float = 1e-8, weight_decay: float = 0.0,
+                 momentum: float = 0.0, centered: bool = False, zero_grad: bool = True, group=None,
+                 lr_schedule: Optional[LRSchedule] = None, max_grad_norm: Optional[float] = None, sharded: bool = False,
+                 param_groups: Optional[list] = None, capturable: bool = False):
+        check_rmsprop_options(lr, alpha, eps, weight_decay, momentum)
+        if param_groups is not None:
+            param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
+                                               lambda glr, gwd: check_rmsprop_options(glr, alpha, eps, gwd, momentum))
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.alpha, self.eps, self.momentum, self.centered = float(alpha), float(eps), float(momentum), bool(centered)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, param_groups, capturable)
+        nb = range(len(self.buckets))
+        self.square_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in nb]
+        self.momentum_buffer_flats: List[torch.Tensor] = [self._state_flat(k) for k in nb] if self.momentum > 0 else []
+        self.grad_avg_flats: List[torch.Tensor] = [self._state_flat(k) for k in nb] if self.centered else []
+
+    def scalars(self, lr: Optional[float] = None) -> list:
+        """:func:`rmsprop_scalars` of the next update (lr = :meth:`lr_at` unless given)."""
+        return rmsprop_scalars(self.lr_at() if lr is None else lr, self.alpha, self.eps, self.weight_decay, self.momentum)
+
+    def _states(self, k: int) -> tuple:
+        """Bucket ``k``'s ``(square_avg, grad_avg or None, momentum_buffer or None)`` flats, in the kernels' argument order."""
+        return (self.square_avg_flats[k], self.grad_avg_flats[k] if self.centered else None,
+                self.momentum_buffer_flats[k] if self.momentum > 0 else None)
+
+    def _torch_rmsprop(self, p: list, g: list, sq: list, ga: list, buf: list, lr: Optional[float] = None,
+                       weight_decay: Optional[float] = None) -> None:
+        """torch's single-tensor RMSprop on the given views, with the optimizer's lr and weight decay unless a group's are
+        given."""
+        from torch.optim.rmsprop import rmsprop
+
+        steps = [torch.tensor(float(self.steps)) for _ in p]
+        rmsprop(p, g, sq, ga, buf, steps, foreach=False, maximize=False, differentiable=False, capturable=False,
+                lr=self.lr_at() if lr is None else lr, alpha=self.alpha, eps=self.eps,
+                weight_decay=self.weight_decay if weight_decay is None else weight_decay, momentum=self.momentum,
+                centered=self.centered)
+
+    def _torch_runs(self, runs: list, flats: list) -> None:
+        """torch's RMSprop once per group on the ``(lo, hi, group)`` runs of the views ``flats`` = [p, g (fp32), states...]
+        (absent states None), or once on the whole views without groups."""
+        if not self._grouped:
+            self._torch_rmsprop(*[[f] if f is not None else [] for f in flats])
+            return
+        for gi, (lr, wd) in enumerate(self._group_values()):
+            mine = [(lo, hi) for lo, hi, g in runs if g == gi]
+            if mine:
+                self._torch_rmsprop(*[[f[lo:hi] for lo, hi in mine] if f is not None else [] for f in flats], lr=lr, weight_decay=wd)
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        sc = self.scalars() if any(kernel) else None
+        vals = self._group_values() if self._grouped else None
+        for k, (gb, pf, kern) in enumerate(zip(self.buckets, self.param_flats, kernel)):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern:
+                if self._grouped:
+                    self._kernel().rmsprop_flat_grouped(pf, *self._states(k), g, self._maps[k], sc, self.centered,
+                                                        [v[0] for v in vals], [v[1] for v in vals], self.fused_zero, **clip)
+                else:
+                    self._kernel().rmsprop_flat(pf, *self._states(k), g, sc, self.centered, self.fused_zero, **clip)
+                continue
+            gf = _fp32_grad(g, clip.get("grad_scale"))
+            # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.RMSprop sees it
+            flats = (pf, gf) + self._states(k)
+            views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
+                     if f is not None else None for f in flats]
+            if not self._grouped:
+                self._torch_rmsprop(*[v if v is not None else [] for v in views])
+            else:
+                gid = [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
+                for gi, (lr, wd) in enumerate(vals):
+                    idx = [i for i, x in enumerate(gid) if x == gi]
+                    if idx:
+                        self._torch_rmsprop(*[[vs[i] for i in idx] if vs is not None else [] for vs in views], lr=lr,
+                                            weight_decay=wd)
+            if self.fused_zero:
+                g.zero_()
+
+    def _update_capturable(self, clip: dict) -> None:
+        sc = self.scalars(lr=self.lr)    # lr and weight decay come from the device block; reading steps would synchronise
+        for k, (gb, pf) in enumerate(zip(self.buckets, self.param_flats)):
+            self._kernel().rmsprop_flat_cap(pf, *self._states(k), gb.flat[:gb.numel], self._cap_map(k), self._cap_block, sc,
+                                            self.centered, self.fused_zero, **clip)
+
+    def _sharded_kernel(self, k: int, max_blocks: int) -> None:
+        gb = self.buckets[k]
+        n_vec, handle, gh, W = self._shards[k][0], self._shards[k][4], gb.symm_handle, self._world
+        head = (gb.flat.dtype == torch.bfloat16, gh.ptrs, handle.ptrs, gh.sig_ptrs) + self._states(k)
+        tail = (1.0 / W, self.fused_zero, gb.world.rank, W, max_blocks)
+        if self.capturable:
+            self._kernel().sharded_rmsprop_cap(*head, self._cap_map(k), self._cap_block, n_vec, self.scalars(lr=self.lr),
+                                               self.centered, *tail)
+        elif self._grouped:
+            vals = self._group_values()
+            self._kernel().sharded_rmsprop_grouped(*head, self._maps[k], n_vec, self.scalars(), self.centered,
+                                                   [v[0] for v in vals], [v[1] for v in vals], *tail)
+        else:
+            self._kernel().sharded_rmsprop(*head, n_vec, self.scalars(), self.centered, *tail)
+
+    def _update_slice(self, k: int, lo: int, n: int) -> None:
+        gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
+        states = [f[:n] if f is not None else None for f in self._states(k)]
+        self._torch_runs(self._slice_runs(k, lo, n) if self._grouped else None, [self._shards[k][3][lo:lo + n], gf] + states)
+
+    # ------------------------------------------------------------------ checkpointing
+    def _state_pairs(self) -> list:
+        """``(key, flats)`` of every state this optimizer keeps, in torch.optim.RMSprop's names."""
+        return [("square_avg", self.square_avg_flats)] + ([("momentum_buffer", self.momentum_buffer_flats)] if self.momentum > 0
+                                                          else []) + ([("grad_avg", self.grad_avg_flats)] if self.centered else [])
+
+    def state_dict(self) -> dict:
+        """Hyper-parameters, ``steps`` and the flat state buffers (CPU copies): ``square_avg``, ``momentum_buffer`` and
+        ``grad_avg`` (the last two empty lists when the update has none).  Sharded over several ranks, the buffers are this
+        rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that crosses world sizes and modes is
+        :meth:`named_state`."""
+        sd = {"lr": self.lr, "alpha": self.alpha, "eps": self.eps, "weight_decay": self.weight_decay, "momentum": self.momentum,
+              "centered": self.centered, "max_grad_norm": self.max_grad_norm, "steps": self.steps,
+              "square_avg": [f.detach().cpu().clone() for f in self.square_avg_flats],
+              "momentum_buffer": [f.detach().cpu().clone() for f in self.momentum_buffer_flats],
+              "grad_avg": [f.detach().cpu().clone() for f in self.grad_avg_flats]}
+        sd.update(self._shard_tags())
+        sd.update(self._group_state())
+        return sd
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict` (same model => same bucket layout).  ``ValueError`` if the state_dict's ``centered``
+        or whether its momentum is > 0 differs from this optimizer's (those decide which states exist), or if its
+        ``param_groups`` hold other parameters than this optimizer's."""
+        self._load_group_state(sd, apply=False)
+        if bool(sd["centered"]) != self.centered or (float(sd["momentum"]) > 0) != (self.momentum > 0):
+            raise ValueError(f"FlatRMSprop.load_state_dict: the state_dict has centered={bool(sd['centered'])} and momentum "
+                             f"{float(sd['momentum'])}, this optimizer centered={self.centered} and momentum {self.momentum}; "
+                             "build it with the same centered and the same momentum > 0 (they decide which states exist)")
+        check_rmsprop_options(sd["lr"], sd["alpha"], sd["eps"], sd["weight_decay"], sd["momentum"])
+        self._load_flats(sd, [(flats, sd[key]) for key, flats in self._state_pairs()], "RMSprop state",
+                         "named_state() / load_named_state()")
+        self.lr, self.weight_decay = float(sd["lr"]), float(sd["weight_decay"])
+        self.alpha, self.eps, self.momentum = float(sd["alpha"]), float(sd["eps"]), float(sd["momentum"])
+        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
+        self.steps = int(sd["steps"])
+        self._load_group_state(sd)
+        self._sync_hyperparameters()
+
+    def named_state(self, model: nn.Module) -> dict:
+        """``{name: {"step", "square_avg"[, "momentum_buffer"][, "grad_avg"]}}`` (CPU copies), ``torch.optim.RMSprop``'s
+        per-parameter state by parameter name, the form that crosses world sizes, sharded and unsharded runs and
+        ``torch.optim.RMSprop``.  Sharded over several ranks this is collective: every rank calls it and gets the full
+        tensors."""
+        parts = [(key, self._named(model, flats)) for key, flats in self._state_pairs()]
+        return {n: {"step": torch.tensor(float(self.steps)), **{key: named[n] for key, named in parts}} for n in parts[0][1]}
+
+    def load_named_state(self, model: nn.Module, named: dict) -> int:
+        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
+        (common) ``step``.  ``ValueError`` if an entry lacks a state this optimizer keeps.  Sharded over several ranks, each
+        rank keeps its slice (not collective)."""
+        steps = {int(s["step"]) for s in named.values()}
+        if len(steps) > 1:
+            raise ValueError(f"FlatRMSprop keeps one step count for all parameters; this state has steps {sorted(steps)}")
+        for key, _ in self._state_pairs():
+            if any(key not in s for s in named.values()):
+                raise ValueError(f"FlatRMSprop.load_named_state: an entry has no {key!r}; the state is of an RMSprop with "
+                                 "another momentum or centered setting")
+        done = 0
+        for key, flats in self._state_pairs():
+            done = self._load_named(model, {n: s[key] for n, s in named.items()}, flats)
+        if done and steps:
+            self.steps = steps.pop()
+        return done
+
+
 def exclude_1d(name: str, param: torch.Tensor) -> bool:      # noqa: ARG001 - the name is there for custom rules
     """The default ``exclude_from_adaptation`` of :class:`FlatLAMB` and :class:`FlatLARS`: biases and norm weights
     (``param.ndim <= 1``) get no weight decay and a trust ratio of 1, as in the usual LARS and BERT-LAMB recipes."""
@@ -1415,7 +1636,7 @@ def check_ema_options(decay, every, warmup_steps) -> tuple:
 
 class FlatEMA:
     """An exponential moving average of the weights of a model trained by a flat optimizer (:class:`FlatSGD`,
-    :class:`FlatAdamW`, :class:`FlatLAMB`, :class:`FlatLARS`), for evaluation and the final checkpoint: torchvision's
+    :class:`FlatAdamW`, :class:`FlatRMSprop`, :class:`FlatLAMB`, :class:`FlatLARS`), for evaluation and the final checkpoint: torchvision's
     ``--model-ema``, timm's ``ModelEma``, ``AveragedModel(model, multi_avg_fn=get_ema_multi_avg_fn(decay), use_buffers=True)``.
 
     ``ema = FlatEMA(optimizer, decay=0.9999, every=1, warmup_steps=0)`` copies the current parameters, and the floating-point
@@ -1461,7 +1682,7 @@ class FlatEMA:
                  model: Optional[nn.Module] = None):
         self._decay, self._every, self._warmup = check_ema_options(decay, every, warmup_steps)
         if not isinstance(optimizer, _FlatOptimizer):
-            raise ValueError(f"FlatEMA needs a flat optimizer (FlatSGD, FlatAdamW, FlatLAMB, FlatLARS), got "
+            raise ValueError(f"FlatEMA needs a flat optimizer (FlatSGD, FlatAdamW, FlatRMSprop, FlatLAMB, FlatLARS), got "
                              f"{type(optimizer).__name__}")
         from ..parallel.ddp import DistributedDataParallel
 
