@@ -17,6 +17,7 @@ Public surface (tutorial names kept; see each module for file:line parity):
     FlatSGD (one-launch momentum SGD over flat buffers) ops/optim.py
     FlatAdamW (one-launch AdamW over flat buffers)      ops/optim.py
     FlatRMSprop (one-launch RMSprop over flat buffers)  ops/optim.py
+    FlatAdafactor (factored second moments, no sync)    ops/optim.py
     FlatLAMB FlatLARS (per-tensor trust ratios)         ops/optim.py
     FlatEMA (EMA of the weights, one launch per update) ops/optim.py
     GradScaler support (fp16 loss scaling, in-kernel)   ops/optim.py
@@ -37,7 +38,7 @@ from .models.convnet import Net  # noqa: F401
 from .parallel.ddp import (average_gradients, GradBucket, DistributedDataParallel,  # noqa: F401
                            broadcast_parameters)
 from .parallel.sync_bn import SyncBatchNorm  # noqa: F401
-from .ops.optim import FlatAdamW, FlatEMA, FlatLAMB, FlatLARS, FlatRMSprop, FlatSGD, LRSchedule  # noqa: F401
+from .ops.optim import FlatAdafactor, FlatAdamW, FlatEMA, FlatLAMB, FlatLARS, FlatRMSprop, FlatSGD, LRSchedule  # noqa: F401
 from .ops.convnet_eval import evaluate  # noqa: F401
 from .train import run, train, TrainConfig  # noqa: F401
 

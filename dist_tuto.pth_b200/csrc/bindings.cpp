@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 
+#include "adafactor.h"
 #include "adamw.h"
 #include "ema.h"
 #include "executor.h"
@@ -103,6 +104,7 @@ int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerP
                                     const b2::AdamwGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank,
                                     int world, int max_blocks, cudaStream_t stream);
 int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
+int b2_adafactor_launch(const b2::AfArgs* a, cudaStream_t stream);
 int b2_flat_scalars_launch(const b2::FlatHyper* table, unsigned long long* counter, b2::FlatScalars* block, int advance,
                            const float* found_inf, cudaStream_t stream);
 int b2_sgd_flat_cap_launch(float* p, float* m, const float* g, size_t n, const uint8_t* map, const b2::FlatScalars* blk, float mu,
@@ -398,6 +400,101 @@ b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, 
   a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
   a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
   return a;
+}
+
+// FlatAdafactor (csrc/adafactor.cu): the chunk table of one bucket (adafactor.h) from its tensors' offsets, shapes, strides,
+// state offsets and groups, checked on the host and uploaded to `device`; returns (table, chunks, row / column partials,
+// row_var means).  A tensor of dim > 1 is factored over its last two dimensions; its leading dimensions are merged where
+// their strides allow and may number at most kAfMaxLead after that.
+py::tuple adafactor_table(const std::vector<int64_t>& offsets, const std::vector<std::vector<int64_t>>& shapes,
+                          const std::vector<std::vector<int64_t>>& strides, const std::vector<int64_t>& state_offsets,
+                          const std::vector<int64_t>& groups, int64_t n, int64_t n_state, int64_t n_groups, torch::Device device) {
+  const size_t nt = offsets.size();
+  TORCH_CHECK(nt >= 1 && shapes.size() == nt && strides.size() == nt && state_offsets.size() == nt && groups.size() == nt,
+              "adafactor_table: one offset, shape, strides, state offset and group per tensor, at least one tensor");
+  TORCH_CHECK(nt < (size_t)INT32_MAX && n_groups >= 1 && n_groups <= b2::kMaxGroups, "adafactor_table: too many tensors, or a "
+              "group count outside 1..", b2::kMaxGroups);
+  const int64_t K = b2::kAfChunk;
+  std::vector<int64_t> chunks, tens;
+  int64_t end = 0, st_end = 0, rc = 0, means = 0;
+  for (size_t t = 0; t < nt; ++t) {
+    const auto& sh = shapes[t];
+    const auto& sd = strides[t];
+    TORCH_CHECK(sh.size() == sd.size(), "adafactor_table: tensor ", t, ": one stride per dimension");
+    int64_t numel = 1, span = 0;
+    for (size_t k = 0; k < sh.size(); ++k) {
+      TORCH_CHECK(sh[k] >= 0 && sd[k] >= 0, "adafactor_table: tensor ", t, ": sizes and strides must be >= 0");
+      numel *= sh[k];
+      span += sh[k] > 0 ? (sh[k] - 1) * sd[k] : 0;
+    }
+    const int64_t o = offsets[t];
+    TORCH_CHECK(numel < INT32_MAX && o >= end && o + numel <= n && (numel == 0 || span == numel - 1), "adafactor_table: tensor ", t,
+                " at [", o, ", ", o + numel, ") must lie after the previous tensor inside the flat of ", n,
+                " elements, be dense, and hold fewer than 2^31 elements");
+    end = o + numel;
+    const bool fac = sh.size() > 1;
+    int64_t B = 1, R = 1, C = numel, sR = 0, sC = 1;
+    std::vector<int64_t> lsz, lst;                         // merged leading dimensions, innermost first
+    if (fac) {
+      R = sh[sh.size() - 2]; C = sh.back(); sR = sd[sd.size() - 2]; sC = sd.back();
+      for (size_t k = sh.size() - 2; k-- > 0;) {
+        B *= sh[k];
+        if (sh[k] == 1) continue;
+        if (!lsz.empty() && sd[k] == lst.back() * lsz.back()) lsz.back() *= sh[k];
+        else { lsz.push_back(sh[k]); lst.push_back(sd[k]); }
+      }
+      TORCH_CHECK(lsz.size() <= (size_t)b2::kAfMaxLead, "adafactor_table: tensor ", t, " has ", lsz.size(), " leading dimensions "
+                  "after merging; at most ", b2::kAfMaxLead);
+    } else {
+      TORCH_CHECK(numel <= 1 || sd[0] == 1, "adafactor_table: tensor ", t, ": a 1-D tensor must be contiguous");
+    }
+    TORCH_CHECK(state_offsets[t] == st_end, "adafactor_table: tensor ", t, ": state at ", state_offsets[t], ", expected ", st_end,
+                " (row_var, col_var or variance of each tensor in turn)");
+    st_end += fac ? B * R + B * C : numel;
+    TORCH_CHECK(groups[t] >= 0 && groups[t] < n_groups, "adafactor_table: tensor ", t, ": group ", groups[t], " outside [0, ",
+                n_groups, ")");
+    const int64_t first = (int64_t)chunks.size() / b2::kAfChunkRow;
+    const bool whole = fac && R * C <= K;
+    int64_t TR = 0, TC = 0, my_rc = rc;
+    auto add = [&](int64_t b0, int64_t nb, int64_t r0, int64_t nr, int64_t c0, int64_t nc) {
+      for (int64_t v : {(int64_t)t, b0, nb, r0, nr, c0, nc, (int64_t)0}) chunks.push_back(v);
+    };
+    if (numel > 0) {
+      if (!fac) {
+        for (int64_t c0 = 0; c0 < C; c0 += K) add(0, 1, 0, 1, c0, std::min(K, C - c0));
+      } else if (whole) {
+        const int64_t per = K / (R * C);
+        for (int64_t b0 = 0; b0 < B; b0 += per) add(b0, std::min(per, B - b0), 0, R, 0, C);
+      } else {
+        TC = std::min<int64_t>(C, b2::kAfTileCols);
+        TR = std::min<int64_t>(R, K / TC);
+        TC = std::min<int64_t>(C, K / TR);
+        for (int64_t b = 0; b < B; ++b)
+          for (int64_t r0 = 0; r0 < R; r0 += TR)
+            for (int64_t c0 = 0; c0 < C; c0 += TC) add(b, 1, r0, std::min(TR, R - r0), c0, std::min(TC, C - c0));
+        rc += B * R * ((C + TC - 1) / TC) + B * C * ((R + TR - 1) / TR);
+      }
+    }
+    const int64_t count = (int64_t)chunks.size() / b2::kAfChunkRow - first;
+    int64_t row[b2::kAfTensorRow] = {0};
+    row[b2::AF_OFFSET] = o; row[b2::AF_STATE] = state_offsets[t];
+    row[b2::AF_B] = B; row[b2::AF_R] = R; row[b2::AF_C] = C; row[b2::AF_SR] = sR; row[b2::AF_SC] = sC;
+    row[b2::AF_FIRST] = first; row[b2::AF_COUNT] = count; row[b2::AF_FACTORED] = fac ? 1 : 0; row[b2::AF_GROUP] = groups[t];
+    row[b2::AF_WHOLE] = whole ? 1 : 0; row[b2::AF_TR] = TR; row[b2::AF_TC] = TC; row[b2::AF_RC] = my_rc;
+    row[b2::AF_MEAN] = means; row[b2::AF_NLEAD] = (int64_t)lsz.size();
+    for (size_t k = 0; k < lsz.size(); ++k) {            // stored outermost first
+      row[b2::AF_LSIZE + k] = lsz[lsz.size() - 1 - k];
+      row[b2::AF_LSTRIDE + k] = lst[lst.size() - 1 - k];
+    }
+    if (fac) means += B;
+    tens.insert(tens.end(), row, row + b2::kAfTensorRow);
+  }
+  TORCH_CHECK(st_end <= n_state, "adafactor_table: the states need ", st_end, " elements, the state flat has ", n_state);
+  const int64_t n_chunks = (int64_t)chunks.size() / b2::kAfChunkRow;
+  TORCH_CHECK(n_chunks >= 1 && n_chunks < INT32_MAX, "adafactor_table: the tensors hold no element, or too many chunks");
+  chunks.insert(chunks.end(), tens.begin(), tens.end());
+  auto host = torch::tensor(chunks, torch::dtype(torch::kInt64));
+  return py::make_tuple(host.to(device), n_chunks, rc, means);
 }
 
 b2::LrSchedule to_sched(const py::object& o) {
@@ -1623,6 +1720,79 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("trust_coefficient"), py::arg("eps"), py::arg("nesterov"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
      py::arg("grad_scale") = py::none());
+  m.def("adafactor_chunk_elems", [] { return (int64_t)b2::kAfChunk; }, "the largest chunk of an Adafactor chunk table");
+  m.def("adafactor_table", &adafactor_table, py::arg("offsets"), py::arg("shapes"), py::arg("strides"), py::arg("state_offsets"),
+        py::arg("groups"), py::arg("n"), py::arg("n_state"), py::arg("n_groups"), py::arg("device"),
+        "FlatAdafactor: (the chunk table of one bucket on `device`, chunks, row / column partials, row_var means)");
+  m.def("adafactor_flat", [](torch::Tensor p, torch::Tensor state, torch::Tensor g, torch::Tensor table, int64_t n_chunks,
+                             torch::Tensor partials, torch::Tensor rc, torch::Tensor means, torch::Tensor tickets, torch::Tensor alpha,
+                             torch::Tensor step, std::vector<double> scalars, std::vector<double> rho, std::vector<double> decay,
+                             bool zero_grad, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                             c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
+    // FlatAdafactor's update of one fp32 bucket (csrc/adafactor.cu).  scalars (fp64): (t ** beta2_decay, eps1, eps2, d), the
+    // first two rounded once to fp32 here, eps1^2 formed in fp64 and rounded once; per group rho_t (fp64) and
+    // 1 - lr * weight_decay (rounded once to fp32).
+    const char* what = "adafactor_flat";
+    for (const torch::Tensor* t : {&p, &g, &state}) {
+      check_cuda_contig(*t, what);
+      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->device() == p.device(), what,
+                  ": parameters, gradients and state: contiguous fp32 CUDA on one device");
+    }
+    TORCH_CHECK(g.numel() == p.numel(), what, ": the gradient flat has ", g.numel(), " elements, the parameter flat ", p.numel());
+    for (const torch::Tensor* t : {&table, &partials, &rc, &means, &tickets, &alpha, &step}) {
+      check_cuda_contig(*t, what);
+      TORCH_CHECK(t->device() == p.device(), what, ": the table and the workspaces live on the parameters' device");
+    }
+    const int64_t n_tensors = tickets.numel();
+    TORCH_CHECK(n_chunks >= 1 && n_chunks <= p.numel() && n_tensors >= 1 && table.scalar_type() == torch::kInt64 &&
+                table.numel() == n_chunks * b2::kAfChunkRow + n_tensors * b2::kAfTensorRow, what, ": table: int64 of chunks * ",
+                b2::kAfChunkRow, " + tensors * ", b2::kAfTensorRow, " entries from adafactor_table, tickets: one per tensor");
+    TORCH_CHECK(tickets.scalar_type() == torch::kInt32, what, ": tickets: int32 [tensors], zero before the first call");
+    TORCH_CHECK(partials.scalar_type() == torch::kFloat32 && partials.numel() == 2 * n_chunks, what, ": partials: fp32 [2 * chunks]");
+    TORCH_CHECK(rc.scalar_type() == torch::kFloat32 && means.scalar_type() == torch::kFloat32 && rc.numel() >= 1 && means.numel() >= 1,
+                what, ": rc and means: fp32, as many as adafactor_table gives (at least one element each)");
+    TORCH_CHECK(alpha.scalar_type() == torch::kFloat64 && alpha.numel() == n_tensors && step.scalar_type() == torch::kFloat32 &&
+                step.numel() == n_tensors, what, ": alpha: fp64 [tensors], step: fp32 [tensors]");
+    TORCH_CHECK(scalars.size() == 4, what, ": scalars: (t ** beta2_decay, eps1, eps2, d), got ", scalars.size(), " values");
+    for (double x : scalars) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), what, ": scalars must be finite in fp32");
+    TORCH_CHECK(scalars[0] >= 0.0 && scalars[0] <= 1.0 && scalars[1] >= 0.0 && scalars[2] >= 0.0 && scalars[3] >= 1.0, what,
+                ": t ** beta2_decay in [0, 1], eps1 >= 0, eps2 >= 0 and d >= 1");
+    TORCH_CHECK(!rho.empty() && rho.size() <= (size_t)b2::kMaxGroups && rho.size() == decay.size(), what, ": 1..", b2::kMaxGroups,
+                " groups with one rho and one decay each");
+    b2::AfArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.p = p.data_ptr<float>(); a.g = g.data_ptr<float>(); a.state = state.data_ptr<float>();
+    a.n = (size_t)p.numel();
+    a.table = reinterpret_cast<const long long*>(table.data_ptr<int64_t>());
+    a.n_chunks = (int)n_chunks; a.n_tensors = (int)n_tensors;
+    a.partials = partials.data_ptr<float>(); a.rc = rc.data_ptr<float>(); a.means = means.data_ptr<float>();
+    a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int32_t>());
+    a.alpha = alpha.data_ptr<double>(); a.step = step.data_ptr<float>();
+    a.zero_grad = zero_grad ? 1 : 0;
+    a.w = (float)scalars[0]; a.eps1 = (float)scalars[1]; a.eps1sq = (float)(scalars[1] * scalars[1]);
+    a.eps2 = scalars[2]; a.d = scalars[3];
+    a.n_groups = (int)rho.size();
+    for (size_t i = 0; i < rho.size(); ++i) {
+      TORCH_CHECK(std::isfinite(rho[i]) && rho[i] >= 0.0 && std::isfinite((float)decay[i]), what,
+                  ": per-group rho must be finite and >= 0, decay finite in fp32");
+      a.rho[i] = rho[i];
+      a.decay[i] = (float)decay[i];
+    }
+    a.max_norm = check_max_grad_norm(max_grad_norm, what);
+    if (a.max_norm > 0.f) {
+      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                  sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+      a.sqnorms = sqnorms->data_ptr<double>();
+      a.n_buckets = (int)sqnorms->numel();
+    }
+    a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
+    a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
+    c10::cuda::CUDAGuard guard(p.device());
+    ck_cuda(b2_adafactor_launch(&a, cur_stream()), "adafactor_flat launch");
+  }, py::arg("p"), py::arg("state"), py::arg("g"), py::arg("table"), py::arg("n_chunks"), py::arg("partials"), py::arg("rc"),
+     py::arg("means"), py::arg("tickets"), py::arg("alpha"), py::arg("step"), py::arg("scalars"), py::arg("rho"), py::arg("decay"),
+     py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
   // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instance): as sharded_sgd, with this rank's
   // exp_avg / exp_avg_sq shards in place of the momentum shard.
   m.def("sharded_adamw", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,

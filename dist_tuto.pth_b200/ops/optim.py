@@ -29,6 +29,9 @@ per-vector group map and the groups' scalars in the kernel arguments.
 ``FlatSGD(..., capturable=True)`` and ``FlatAdamW(..., capturable=True)`` keep the step counter, the lr schedule and AdamW's bias
 corrections on the device (csrc/flat_scalars.cuh), so a whole DDP step can be captured in a CUDA graph and replayed.
 
+``FlatAdafactor`` is ``torch.optim.Adafactor`` on the same layout: factored second moments (a row and a column vector per
+weight matrix) and per-tensor step sizes, in three launches per bucket (csrc/adafactor.cu) over a chunk table of the layout.
+
 ``FlatLAMB`` and ``FlatLARS`` are the large-batch optimizers with a trust ratio per parameter tensor: per bucket two kernels
 (csrc/layerwise.cu) form every tensor's norms in a fixed order over a chunk table of the flat layout, then apply the update.
 
@@ -45,8 +48,8 @@ from typing import List, Optional, Sequence
 import torch
 import torch.nn as nn
 
-__all__ = ["FlatSGD", "FlatAdamW", "FlatRMSprop", "FlatLAMB", "FlatLARS", "FlatEMA", "LRSchedule", "adamw_scalars",
-           "rmsprop_scalars", "lamb_scalars", "exclude_1d", "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
+__all__ = ["FlatSGD", "FlatAdamW", "FlatRMSprop", "FlatAdafactor", "FlatLAMB", "FlatLARS", "FlatEMA", "LRSchedule", "adamw_scalars",
+           "rmsprop_scalars", "check_adafactor_options", "lamb_scalars", "exclude_1d", "check_sgd_options", "check_max_grad_norm", "MAX_PARAM_GROUPS"]
 
 _KINDS = {"constant": 1, "multistep": 2, "cosine": 3}      # csrc/lr_schedule.h: LRS_CONSTANT, LRS_MULTISTEP, LRS_COSINE
 MAX_MILESTONES = 8
@@ -1403,6 +1406,235 @@ class FlatRMSprop(_FlatOptimizer):
         return done
 
 
+def check_adafactor_options(lr: float, beta2_decay: float, eps, d: float, weight_decay: float) -> tuple:
+    """``torch.optim.Adafactor``'s rules for the hyper-parameters, with its messages.  Returns ``(eps1, eps2)`` with
+    ``eps1=None`` taken as fp32 machine epsilon."""
+    if not 0.0 <= float(lr):
+        raise ValueError(f"Learning rate should be >= 0 but is: {lr}")
+    if not 0.0 >= float(beta2_decay):
+        raise ValueError(f"beta2_decay should be <= 0 but is: {beta2_decay}")
+    if eps[0] is not None and not 0.0 <= float(eps[0]):
+        raise ValueError(f"epsilon1 should be >= 0 but is: {eps[0]}")
+    if not 0.0 <= float(eps[1]):
+        raise ValueError(f"epsilon2 should be >= 0 but is: {eps[1]}")
+    if not 1.0 <= float(d):
+        raise ValueError(f"Clipping threshold d should be >= 1 but is: {d}")
+    if not 0.0 <= float(weight_decay):
+        raise ValueError(f"weight_decay should be >= 0 but is: {weight_decay}")
+    return (torch.finfo(torch.float32).eps if eps[0] is None else float(eps[0])), float(eps[1])
+
+
+def _factors(shape) -> Optional[tuple]:
+    """``(B, R, C)`` of a tensor Adafactor factors (dim > 1: B the product of the leading sizes), ``None`` otherwise."""
+    if len(shape) < 2:
+        return None
+    return math.prod(shape[:-2]), int(shape[-2]), int(shape[-1])
+
+
+class FlatAdafactor(_FlatOptimizer):
+    """``torch.optim.Adafactor`` (``maximize=False``) over flat buffers: ``FlatAdafactor(model)`` where ``model`` is a plain
+    module, a module carrying ``_grad_bucket`` or a :class:`DistributedDataParallel` wrapper, in the loop of
+    :class:`FlatSGD` (``backward(); average_gradients(model); opt.step()``).  Update t = ``steps + 1`` of each parameter
+    tensor, with ``lr = lr_at()``:
+
+    * ``beta2_t = t ** beta2_decay``, ``rho_t = min(lr, 1 / sqrt(t))``, ``alpha = max(eps2, ||p|| / sqrt(numel)) * rho_t``
+      (``||p||`` before the decay), then ``p *= 1 - lr * weight_decay``;
+    * dim > 1, factored over the last two dimensions: ``row_var.lerp_(mean(g^2, -1), beta2_t)``,
+      ``col_var.lerp_(mean(g^2, -2), beta2_t)``, ``v = row_var * col_var / max(mean(row_var, -2), eps1)``; otherwise
+      ``variance.lerp_(g * g, beta2_t)`` and ``v = variance``;
+    * ``u = g / sqrt(max(v, eps1^2))``, ``p += (-alpha / max(1, ||u|| / (sqrt(numel) * d))) * u``.
+
+    ``eps=(None, eps2)`` takes fp32 machine epsilon for eps1.  The state is one fp32 flat per bucket
+    (``state_flats[k]``): for each tensor ``row_var`` then ``col_var`` (``B*R + B*C`` floats, B the product of the leading
+    dimensions), or ``variance`` (its numel), so a factored tensor keeps ``R + C`` floats per slice where AdamW keeps ``2RC``.
+
+    On CUDA fp32 buckets three launches per bucket (csrc/adafactor.cu) update it with no host synchronisation: a stats
+    kernel (``||p||``, the row and column sums of g^2, the lerps, the row_var means and ``alpha``), a norm kernel (``||u||``
+    and the step scalar) and an apply kernel (decay, step, re-zeroed gradients), every sum in an order fixed by the bucket's
+    chunk table, so two runs are bit-identical.  Elsewhere (CPU tensors, bf16 buckets) torch's own single-tensor Adafactor
+    runs on each parameter's views, so a CPU run is bit for bit ``torch.optim.Adafactor(foreach=False)``.
+
+    Like :class:`FlatRMSprop` it takes ``lr_schedule`` (the scheduled lr feeds ``rho_t`` and the decay), ``param_groups``
+    (per-group ``lr`` / ``weight_decay``), ``max_grad_norm`` (on-device clipping first, :meth:`grad_norm`), ``no_sync()``
+    accumulation, :class:`FlatEMA` and ``torch.amp.GradScaler``.  ``maximize``, ``foreach``, ``capturable`` and
+    ``differentiable`` are not taken; ``sharded=True`` raises ``ValueError``.  :meth:`named_state` is
+    ``torch.optim.Adafactor``'s per-parameter state by parameter name."""
+
+    lr = _group_attr("lr")
+    weight_decay = _group_attr("weight_decay")
+
+    def __init__(self, model: nn.Module, lr: float = 1e-2, beta2_decay: float = -0.8, eps=(None, 1e-3), d: float = 1.0,
+                 weight_decay: float = 0.0, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
+                 max_grad_norm: Optional[float] = None, sharded: bool = False, param_groups: Optional[list] = None):
+        eps = tuple(eps)
+        self.eps1, self.eps2 = check_adafactor_options(lr, beta2_decay, eps, d, weight_decay)
+        if sharded:
+            raise ValueError("FlatAdafactor cannot be sharded: a factored tensor's state is its row and column vectors, which do "
+                             "not split along the flat slices of the sharded exchange, and the update needs whole-tensor norms "
+                             "before any element moves; use sharded=False")
+        if param_groups is not None:
+            param_groups = _check_param_groups(type(self).__name__, model, param_groups, lr, weight_decay,
+                                               lambda glr, gwd: check_adafactor_options(glr, beta2_decay, eps, d, gwd))
+        self._default_group = {"params": [], "lr": float(lr), "weight_decay": float(weight_decay)}
+        self.beta2_decay, self.eps, self.d = float(beta2_decay), eps, float(d)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, False, param_groups)
+        # per bucket: the state offset of each tensor, and the state flat
+        self._state_offsets: List[List[int]] = []
+        self.state_flats: List[torch.Tensor] = []
+        for gb, pf in zip(self.buckets, self.param_flats):
+            offs, n = [], 0
+            for gv in gb.views:
+                offs.append(n)
+                f = _factors(gv.shape)
+                n += gv.numel() if f is None else f[0] * (f[1] + f[2])
+            self._state_offsets.append(offs)
+            self.state_flats.append(torch.zeros(max(n, 1), dtype=torch.float32, device=pf.device))
+        self._af = []                    # per bucket on the kernel path: the table and the workspaces, else None
+        for k, (gb, pf) in enumerate(zip(self.buckets, self.param_flats)):
+            if not (pf.is_cuda and gb.flat.dtype == torch.float32):
+                self._af.append(None)
+                continue
+            n_groups = len(self._group_list) if self._grouped else 1
+            table, n_chunks, n_rc, n_means = self._kernel().adafactor_table(
+                list(gb.offsets), [list(gv.shape) for gv in gb.views], [list(gv.stride()) for gv in gb.views],
+                self._state_offsets[k], self._tensor_groups(k), gb.numel, self.state_flats[k].numel(), n_groups, pf.device)
+            n_t, dev = len(gb.params), pf.device
+            self._af.append(dict(table=table, n_chunks=n_chunks,
+                                 partials=torch.zeros(2 * n_chunks, dtype=torch.float32, device=dev),
+                                 rc=torch.zeros(max(n_rc, 1), dtype=torch.float32, device=dev),
+                                 means=torch.zeros(max(n_means, 1), dtype=torch.float32, device=dev),
+                                 tickets=torch.zeros(n_t, dtype=torch.int32, device=dev),
+                                 alpha=torch.zeros(n_t, dtype=torch.float64, device=dev),
+                                 step=torch.zeros(n_t, dtype=torch.float32, device=dev)))
+
+    def _tensor_groups(self, k: int) -> List[int]:
+        """The group of every tensor of bucket ``k`` (all 0 without ``param_groups``)."""
+        gb = self.buckets[k]
+        if not self._grouped:
+            return [0] * len(gb.params)
+        return [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
+
+    def _values(self) -> list:
+        """``(lr, weight_decay)`` of every group for the next update (the one default group without ``param_groups``)."""
+        return self._group_values() if self._grouped else [(self.lr_at(), float(self.weight_decay))]
+
+    def scalars(self) -> tuple:
+        """What ``adafactor_flat`` takes for the next update (t = ``steps + 1``), in fp64: ``([t ** beta2_decay, eps1, eps2,
+        d], [rho_t per group], [1 - lr * weight_decay per group])``."""
+        t = float(self.steps + 1)
+        vals = self._values()
+        return ([t ** self.beta2_decay, self.eps1, self.eps2, self.d], [min(lr, 1 / (t ** 0.5)) for lr, _ in vals],
+                [1 - lr * wd for lr, wd in vals])
+
+    def _state_views(self, k: int, flat: torch.Tensor, i: int) -> dict:
+        """Tensor ``i`` of bucket ``k``'s state in ``flat``, as torch's shaped views: ``row_var`` / ``col_var`` or
+        ``variance``."""
+        gv, so = self.buckets[k].views[i], self._state_offsets[k][i]
+        f = _factors(gv.shape)
+        if f is None:
+            return {"variance": flat[so:so + gv.numel()].as_strided(gv.shape, gv.stride())}
+        B, R, C = f
+        lead = tuple(gv.shape[:-2])
+        return {"row_var": flat[so:so + B * R].view(*lead, R, 1), "col_var": flat[so + B * R:so + B * (R + C)].view(*lead, 1, C)}
+
+    def _torch_adafactor(self, p: list, g: list, states: list, lr: float, weight_decay: float) -> None:
+        from torch.optim._adafactor import adafactor
+
+        steps = [torch.tensor(float(self.steps)) for _ in p]
+        adafactor(p, g, [s.get("row_var") for s in states], [s.get("col_var") for s in states],
+                  [s.get("variance") for s in states], steps, foreach=False, d=self.d, lr=lr, beta2_decay=self.beta2_decay,
+                  weight_decay=weight_decay, eps1=self.eps[0], eps2=self.eps2, maximize=False)
+
+    def _update(self, kernel: List[bool], clip: dict) -> None:
+        vals = self._values()
+        sc = self.scalars() if any(kernel) else None
+        for k, (gb, pf, sf, kern) in enumerate(zip(self.buckets, self.param_flats, self.state_flats, kernel)):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern:
+                w = self._af[k]
+                self._kernel().adafactor_flat(pf, sf, g, w["table"], w["n_chunks"], w["partials"], w["rc"], w["means"],
+                                              w["tickets"], w["alpha"], w["step"], *sc, self.fused_zero, **clip)
+                continue
+            gf = _fp32_grad(g, clip.get("grad_scale"))
+            # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.Adafactor sees it
+            gid = self._tensor_groups(k)
+            for gi, (lr, wd) in enumerate(vals):
+                idx = [i for i, x in enumerate(gid) if x == gi and gb.params[i].numel() > 0]
+                if idx:
+                    views = [(pf[o:o + p.numel()].as_strided(gv.shape, gv.stride()),
+                              gf[o:o + p.numel()].as_strided(gv.shape, gv.stride()), self._state_views(k, sf, i))
+                             for i, (p, o, gv) in enumerate(zip(gb.params, gb.offsets, gb.views)) if i in idx]
+                    self._torch_adafactor([v[0] for v in views], [v[1] for v in views], [v[2] for v in views], lr, wd)
+            if self.fused_zero:
+                g.zero_()
+
+    # ------------------------------------------------------------------ checkpointing
+    def state_dict(self) -> dict:
+        """Hyper-parameters, ``steps`` and the state flats (CPU copies, ``state``); the form that crosses world sizes, bucket
+        layouts and ``torch.optim.Adafactor`` is :meth:`named_state`."""
+        sd = {"lr": self.lr, "beta2_decay": self.beta2_decay, "eps": self.eps, "d": self.d, "weight_decay": self.weight_decay,
+              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
+              "state": [f.detach().cpu().clone() for f in self.state_flats]}
+        sd.update(self._group_state())
+        return sd
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict` (same model => same bucket layout).  ``ValueError`` if its ``param_groups`` hold
+        other parameters than this optimizer's or its state flats have other sizes."""
+        self._load_group_state(sd, apply=False)
+        eps = tuple(sd["eps"])
+        self.eps1, self.eps2 = check_adafactor_options(sd["lr"], sd["beta2_decay"], eps, sd["d"], sd["weight_decay"])
+        if [f.numel() for f in sd["state"]] != [f.numel() for f in self.state_flats]:
+            raise ValueError("FlatAdafactor.load_state_dict: the state flats have other sizes than this optimizer's (another "
+                             "model or bucket layout); carry the state with named_state() / load_named_state()")
+        with torch.no_grad():
+            for f, src in zip(self.state_flats, sd["state"]):
+                f.copy_(src)
+        self.lr, self.weight_decay = float(sd["lr"]), float(sd["weight_decay"])
+        self.beta2_decay, self.eps, self.d = float(sd["beta2_decay"]), eps, float(sd["d"])
+        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
+        self.steps = int(sd["steps"])
+        self._load_group_state(sd)
+
+    def named_state(self, model: nn.Module) -> dict:
+        """``{name: {"step", "row_var", "col_var"}}`` or ``{name: {"step", "variance"}}`` (CPU copies), ``torch.optim.Adafactor``'s
+        per-parameter state by parameter name: the form that crosses world sizes, bucket layouts and ``torch.optim.Adafactor``."""
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        out = {}
+        for k, gb in enumerate(self.buckets):
+            for i, p in enumerate(gb.params):
+                if id(p) in names:
+                    views = self._state_views(k, self.state_flats[k], i)
+                    out[names[id(p)]] = {"step": torch.tensor(float(self.steps)),
+                                         **{key: v.detach().cpu().clone() for key, v in views.items()}}
+        return out
+
+    @torch.no_grad()
+    def load_named_state(self, model: nn.Module, named: dict) -> int:
+        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
+        (common) ``step``.  ``ValueError`` if the steps differ or an entry lacks the state its parameter's shape needs."""
+        steps = {int(s["step"]) for s in named.values()}
+        if len(steps) > 1:
+            raise ValueError(f"FlatAdafactor keeps one step count for all parameters; this state has steps {sorted(steps)}")
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        done = 0
+        for k, gb in enumerate(self.buckets):
+            for i, p in enumerate(gb.params):
+                src = named.get(names.get(id(p)))
+                if src is None:
+                    continue
+                views = self._state_views(k, self.state_flats[k], i)
+                if any(key not in src for key in views):
+                    raise ValueError(f"FlatAdafactor.load_named_state: the entry of {names[id(p)]!r} has no "
+                                     f"{' / '.join(views)}; its parameter has another number of dimensions")
+                for key, v in views.items():
+                    v.copy_(src[key])
+                done += 1
+        if done and steps:
+            self.steps = steps.pop()
+        return done
+
+
 def exclude_1d(name: str, param: torch.Tensor) -> bool:      # noqa: ARG001 - the name is there for custom rules
     """The default ``exclude_from_adaptation`` of :class:`FlatLAMB` and :class:`FlatLARS`: biases and norm weights
     (``param.ndim <= 1``) get no weight decay and a trust ratio of 1, as in the usual LARS and BERT-LAMB recipes."""
@@ -1636,7 +1868,7 @@ def check_ema_options(decay, every, warmup_steps) -> tuple:
 
 class FlatEMA:
     """An exponential moving average of the weights of a model trained by a flat optimizer (:class:`FlatSGD`,
-    :class:`FlatAdamW`, :class:`FlatRMSprop`, :class:`FlatLAMB`, :class:`FlatLARS`), for evaluation and the final checkpoint: torchvision's
+    :class:`FlatAdamW`, :class:`FlatRMSprop`, :class:`FlatAdafactor`, :class:`FlatLAMB`, :class:`FlatLARS`), for evaluation and the final checkpoint: torchvision's
     ``--model-ema``, timm's ``ModelEma``, ``AveragedModel(model, multi_avg_fn=get_ema_multi_avg_fn(decay), use_buffers=True)``.
 
     ``ema = FlatEMA(optimizer, decay=0.9999, every=1, warmup_steps=0)`` copies the current parameters, and the floating-point
@@ -1682,7 +1914,7 @@ class FlatEMA:
                  model: Optional[nn.Module] = None):
         self._decay, self._every, self._warmup = check_ema_options(decay, every, warmup_steps)
         if not isinstance(optimizer, _FlatOptimizer):
-            raise ValueError(f"FlatEMA needs a flat optimizer (FlatSGD, FlatAdamW, FlatRMSprop, FlatLAMB, FlatLARS), got "
+            raise ValueError(f"FlatEMA needs a flat optimizer (FlatSGD, FlatAdamW, FlatRMSprop, FlatAdafactor, FlatLAMB, FlatLARS), got "
                              f"{type(optimizer).__name__}")
         from ..parallel.ddp import DistributedDataParallel
 

@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` (or ``FlatAdamW``, ``FlatRMSprop``, ``FlatLAMB``,
-``FlatLARS``) in the tutorial's loop, on synthetic data.
+"""Your own model, data-parallel: ``DistributedDataParallel`` + ``FlatSGD`` (or ``FlatAdamW``, ``FlatRMSprop``,
+``FlatAdafactor``, ``FlatLAMB``, ``FlatLARS``) in the tutorial's loop, on synthetic data.
 
     python examples/train_ddp.py                                  # CPU, gloo, world 2
     python examples/train_ddp.py --sharded-optimizer              # momentum sharded over the ranks (ZeRO stage 1)
     python examples/train_ddp.py --backend b200 --size 8 --sharded-optimizer   # one process per GPU: per bucket ONE kernel
                                                                   # reduces, updates the owned slice and gathers the parameters
     python examples/train_ddp.py --optimizer adamw [--sharded-optimizer]   # FlatAdamW; sharded: both moments 1/size per rank
+    python examples/train_ddp.py --optimizer adafactor            # FlatAdafactor: factored second moments (unsharded)
     python examples/train_ddp.py --optimizer rmsprop              # FlatRMSprop with torchvision's alpha 0.9, eps 0.0316,
                                                                   # momentum 0.9
     python examples/train_ddp.py --optimizer lamb                 # FlatLAMB / FlatLARS (--optimizer lars): per-tensor trust
@@ -133,6 +134,8 @@ def run(rank, size):
     elif CFG["optimizer"] == "rmsprop":        # torchvision's classification reference: alpha 0.9, eps 0.0316, momentum 0.9
         optimizer = dist.FlatRMSprop(model, lr=1e-3, alpha=0.9, eps=0.0316, momentum=0.9, weight_decay=1e-4,
                                      sharded=CFG["sharded"], param_groups=groups, **cap)
+    elif CFG["optimizer"] == "adafactor":      # torch.optim.Adafactor's defaults, with a little decoupled weight decay
+        optimizer = dist.FlatAdafactor(model, lr=1e-2, weight_decay=1e-4, param_groups=groups)
     elif CFG["optimizer"] == "lamb":
         optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2)
     elif CFG["optimizer"] == "lars":
@@ -157,6 +160,8 @@ def run(rank, size):
     elif CFG["optimizer"] == "rmsprop":
         flats = optimizer.square_avg_flats + optimizer.momentum_buffer_flats + optimizer.grad_avg_flats
         state = f"RMSprop state elements on this rank {sum(m.numel() for m in flats)}"
+    elif CFG["optimizer"] == "adafactor":
+        state = f"Adafactor state elements on this rank {sum(f.numel() for f in optimizer.state_flats)}"
     else:
         state = f"momentum elements on this rank {sum(m.numel() for m in optimizer.momentum_flats)}"
     print(f"Rank {rank}, step {CFG['steps']}: loss {float(loss.detach()):.6f} (mean over ranks {float(total) / size:.9f}), "
@@ -177,11 +182,11 @@ if __name__ == "__main__":
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--sharded-optimizer", action="store_true",
                     help="sharded=True: each rank keeps the optimizer state of, and updates, 1/size of every bucket")
-    ap.add_argument("--optimizer", choices=("sgd", "adamw", "rmsprop", "lamb", "lars"), default="sgd",
-                    help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatRMSprop, FlatLAMB or FlatLARS (the last two "
-                         "unsharded)")
+    ap.add_argument("--optimizer", choices=("sgd", "adamw", "rmsprop", "adafactor", "lamb", "lars"),
+                    default="sgd", help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatRMSprop, FlatAdafactor, FlatLAMB or "
+                                        "FlatLARS (the last three unsharded)")
     ap.add_argument("--no-decay-bias-norm", action="store_true",
-                    help="sgd / adamw / rmsprop: no weight decay on biases and norm weights (a param_groups entry with "
+                    help="sgd / adamw / rmsprop / adafactor: no weight decay on biases and norm weights (a param_groups entry with "
                          "weight_decay=0)")
     ap.add_argument("--cuda-graph", action="store_true",
                     help="sgd / adamw / rmsprop on --backend b200: capturable=True, and every step after the warm-up one graph "
@@ -201,10 +206,15 @@ if __name__ == "__main__":
                  "backward, before GradScaler can check the gradients")
     if a.accumulation_steps < 1:
         ap.error("--accumulation-steps must be at least 1")
+    if a.optimizer == "adafactor" and a.sharded_optimizer:
+        ap.error("--optimizer adafactor cannot be sharded: a factored tensor's state is its row and column vectors, which do "
+                 "not split along the flat slices of the sharded exchange")
+    if a.optimizer == "adafactor" and a.cuda_graph:
+        ap.error("--optimizer adafactor has no capturable form: --cuda-graph needs sgd / adamw / rmsprop")
     if a.cuda_graph and (a.optimizer not in ("sgd", "adamw", "rmsprop") or a.backend != "b200"):
         ap.error("--cuda-graph is for --optimizer sgd / adamw / rmsprop on --backend b200 (CUDA)")
-    if a.no_decay_bias_norm and a.optimizer not in ("sgd", "adamw", "rmsprop"):
-        ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw / rmsprop; FlatLAMB and FlatLARS exclude them already")
+    if a.no_decay_bias_norm and a.optimizer not in ("sgd", "adamw", "rmsprop", "adafactor"):
+        ap.error("--no-decay-bias-norm is for --optimizer sgd / adamw / rmsprop / adafactor; FlatLAMB and FlatLARS exclude them already")
     os.environ["B2_DDP_CFG"] = json.dumps(dict(backend=a.backend, steps=a.steps, sharded=a.sharded_optimizer,
                                                 optimizer=a.optimizer, no_decay=a.no_decay_bias_norm,
                                                 cuda_graph=a.cuda_graph, accumulation_steps=a.accumulation_steps,
