@@ -26,11 +26,12 @@ TARGET = os.path.join(HERE, "_C.so")
 
 CU_SOURCES = ["allreduce.cu", "convnet.cu", "convnet_cluster.cu", "sgd.cu", "gemm_tcgen05.cu", "tc_probe.cu", "convnet_batched.cu",
               "convnet_eval.cu", "p2p.cu", "sharded_sgd.cu", "batchnorm.cu", "adamw.cu", "layerwise.cu",
-              "flat_scalars.cu", "ema.cu", "rmsprop.cu", "adafactor.cu"]
+              "flat_scalars.cu", "ema.cu", "rmsprop.cu", "adafactor.cu", "sharded_layerwise.cu"]
 CPP_SOURCES = ["symm_mem.cpp", "loader.cpp", "executor.cpp", "bindings.cpp"]
 HEADERS = ["common.cuh", "tc_common.cuh", "convnet_args.cuh", "convnet_reduce.cuh", "sgd_device.cuh", "lr_schedule.h", "loader.h", "executor.h",
            "batchnorm.h", "adamw.h", "adamw_device.cuh", "layerwise.h", "layerwise_device.cuh", "param_groups.h", "param_groups.cuh",
-           "flat_scalars.h", "flat_scalars.cuh", "ema.h", "rmsprop.h", "rmsprop_device.cuh", "adafactor.h"]
+           "flat_scalars.h", "flat_scalars.cuh", "ema.h", "rmsprop.h", "rmsprop_device.cuh", "adafactor.h",
+           "shard_grid.h"]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]

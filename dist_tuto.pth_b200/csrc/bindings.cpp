@@ -104,6 +104,9 @@ int b2_sharded_adamw_grouped_launch(int bf16, const PeerPtrs* grads, const PeerP
                                     const b2::AdamwGroups* gs, int n_groups, size_t n_vec, float scale, int zero_grad, int rank,
                                     int world, int max_blocks, cudaStream_t stream);
 int b2_layerwise_launch(int lamb, const b2::LwArgs* a, cudaStream_t stream);
+int b2_sharded_layerwise_launch(int lamb, int bf16, const PeerPtrs* grads, const PeerPtrs* params, const PeerPtrs* sums,
+                                const SignalPadsH* sig, const b2::LwArgs* lw, size_t n_vec, float scale, int rank, int world,
+                                int max_blocks, cudaStream_t stream);
 int b2_adafactor_launch(const b2::AfArgs* a, cudaStream_t stream);
 int b2_flat_scalars_launch(const b2::FlatHyper* table, unsigned long long* counter, b2::FlatScalars* block, int advance,
                            const float* found_inf, cudaStream_t stream);
@@ -322,35 +325,66 @@ int check_groups(const torch::Tensor& map, int64_t n_ids, const std::vector<doub
   return (int)a.size();
 }
 
-// FlatLAMB / FlatLARS (csrc/layerwise.cu): the chunk table of one bucket from its tensors' offsets, sizes and adapt flags,
-// checked on the host and uploaded to `device`; returns (table, number of chunks).
-py::tuple layerwise_table(const std::vector<int64_t>& offsets, const std::vector<int64_t>& numels, const std::vector<bool>& adapt,
-                          int64_t n, torch::Device device) {
+// FlatLAMB / FlatLARS (csrc/layerwise.cu, csrc/sharded_layerwise.cu): the chunk table (layerwise.h) of the elements [lo, hi)
+// of one bucket of n elements, from its tensors' offsets, sizes and adapt flags, checked on the host and uploaded to `device`:
+// each tensor's piece of [lo, hi) cut into chunks of at most kLwChunk elements from the piece's start, then one row per
+// tensor of the bucket.  Returns (table, number of chunks); `what` names the binding in the messages.
+std::pair<torch::Tensor, int64_t> lw_table(const std::vector<int64_t>& offsets, const std::vector<int64_t>& numels,
+                                           const std::vector<bool>& adapt, int64_t n, int64_t lo, int64_t hi, torch::Device device,
+                                           const char* what) {
   TORCH_CHECK(!offsets.empty() && offsets.size() == numels.size() && offsets.size() == adapt.size(),
-              "layerwise_table: one offset, size and adapt flag per tensor, at least one tensor");
-  TORCH_CHECK(offsets.size() < (size_t)INT32_MAX, "layerwise_table: too many tensors");
+              what, ": one offset, size and adapt flag per tensor, at least one tensor");
+  TORCH_CHECK(offsets.size() < (size_t)INT32_MAX, what, ": too many tensors");
   std::vector<int64_t> chunks, tens;
   int64_t end = 0;
   for (size_t t = 0; t < offsets.size(); ++t) {
     const int64_t o = offsets[t], k = numels[t];
-    TORCH_CHECK(o % 4 == 0 && k >= 0 && o >= end && o + k <= n, "layerwise_table: tensor ", t, " at [", o, ", ", o + k,
+    TORCH_CHECK(o % 4 == 0 && k >= 0 && o >= end && o + k <= n, what, ": tensor ", t, " at [", o, ", ", o + k,
                 ") must start at a multiple of 4 elements, after the previous tensor, inside the flat of ", n, " elements");
     end = o + k;
     tens.push_back((int64_t)chunks.size() / b2::kLwRow);
     int64_t c = 0;
-    for (int64_t s = 0; s < k; s += b2::kLwChunk, ++c) {
-      chunks.push_back(o + s);
-      chunks.push_back(std::min<int64_t>(b2::kLwChunk, k - s));
+    const int64_t a = std::max(o, lo), b = std::min(o + k, hi);
+    for (int64_t s = a; s < b; s += b2::kLwChunk, ++c) {
+      chunks.push_back(s);
+      chunks.push_back(std::min<int64_t>(b2::kLwChunk, b - s));
       chunks.push_back((int64_t)t);
     }
     tens.push_back(c);
     tens.push_back(adapt[t] ? 1 : 0);
   }
   const int64_t n_chunks = (int64_t)chunks.size() / b2::kLwRow;
-  TORCH_CHECK(n_chunks >= 1 && n_chunks < INT32_MAX, "layerwise_table: the tensors hold no element, or too many chunks");
   chunks.insert(chunks.end(), tens.begin(), tens.end());
   auto host = torch::tensor(chunks, torch::dtype(torch::kInt64));
-  return py::make_tuple(host.to(device), n_chunks);
+  return {host.to(device), n_chunks};
+}
+
+py::tuple layerwise_table(const std::vector<int64_t>& offsets, const std::vector<int64_t>& numels, const std::vector<bool>& adapt,
+                          int64_t n, torch::Device device) {
+  auto [table, n_chunks] = lw_table(offsets, numels, adapt, n, 0, n, device, "layerwise_table");
+  TORCH_CHECK(n_chunks >= 1 && n_chunks < INT32_MAX, "layerwise_table: the tensors hold no element, or too many chunks");
+  return py::make_tuple(table, n_chunks);
+}
+
+// The table of rank `rank`'s slice [rank * n / world, (rank + 1) * n / world) of a padded bucket of n elements (sharded
+// FlatLAMB / FlatLARS).  A slice of padding only has no chunk; its tensor rows are still there.  The kernels index the state
+// shards relative to the slice start, so the table keeps the slice it was built for, and the launch bindings refuse it for
+// another rank, world size or bucket size.
+struct ShardedLwTable {
+  torch::Tensor table;    // int64 CUDA: n_chunks + tensors rows (layerwise.h)
+  int64_t n_chunks, n;
+  int rank, world;
+};
+
+ShardedLwTable sharded_layerwise_table(const std::vector<int64_t>& offsets, const std::vector<int64_t>& numels,
+                                       const std::vector<bool>& adapt, int64_t n, int rank, int world, torch::Device device) {
+  check_world(rank, world, "sharded_layerwise_table");
+  TORCH_CHECK(n % (4 * (int64_t)world) == 0, "sharded_layerwise_table: the padded bucket of ", n, " elements must split into ", world,
+              " slices of whole 16-byte vectors");
+  const int64_t per = n / world;
+  auto [table, n_chunks] = lw_table(offsets, numels, adapt, n, rank * per, (rank + 1) * per, device, "sharded_layerwise_table");
+  TORCH_CHECK(n_chunks < INT32_MAX, "sharded_layerwise_table: too many chunks");
+  return {table, n_chunks, n, rank, world};
 }
 
 // The arguments every layer-wise launch shares: the table, the workspaces and clipping.  `states` are the state flats.
@@ -399,6 +433,61 @@ b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, 
   }
   a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
   a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
+  return a;
+}
+
+// The checked arguments of a sharded layer-wise launch (csrc/sharded_layerwise.cu): the per-rank pointer lists, and this
+// rank's table (sharded_layerwise_table), workspaces and state flats (`states`: m, then v (lamb) or LARS's gradient workspace), the
+// state flats of at least one slice (n_vec / world x 4, x 8 with bf16) each.
+b2::LwArgs sharded_layerwise_args(const char* what, bool lamb, bool bf16, const std::vector<unsigned long long>& grads,
+                                  const std::vector<unsigned long long>& params, const std::vector<unsigned long long>& sums,
+                                  const std::vector<unsigned long long>& sigs, const std::vector<torch::Tensor*>& states,
+                                  const ShardedLwTable& tab, torch::Tensor& partials, torch::Tensor& tickets,
+                                  torch::Tensor& ratios, size_t n_vec, bool zero_grad, int rank, int world) {
+  check_world(rank, world, what);
+  TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sums.size() == world && (int)sigs.size() == world,
+              what, ": one gradient bucket, parameter flat, sums buffer and signal pad per rank, got ", grads.size(), ", ",
+              params.size(), ", ", sums.size(), " and ", sigs.size(), " for world ", world);
+  TORCH_CHECK(n_vec % (size_t)world == 0, what, ": every rank owns n_vec / world vectors, so n_vec must be a multiple of world "
+              "(pad the buffers), got n_vec ", n_vec, " for world ", world);
+  const int64_t n_elems = (int64_t)n_vec * (bf16 ? 8 : 4);
+  TORCH_CHECK(tab.rank == rank && tab.world == world && tab.n == n_elems, what, ": the table was built for rank ", tab.rank,
+              " of ", tab.world, " on a bucket of ", tab.n, " elements; this launch is rank ", rank, " of ", world, " on ", n_elems);
+  const torch::Tensor& table = tab.table;
+  const int64_t n_chunks = tab.n_chunks;
+  for (const auto* v : {&grads, &params, &sums, &sigs})
+    for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, what, ": null or misaligned per-rank pointer");
+  const int64_t shard = n_elems / world;
+  torch::Tensor& like = *states[0];
+  for (const torch::Tensor* t : states) {
+    check_cuda_contig(*t, what);
+    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() >= shard && t->device() == like.device() &&
+                (uintptr_t)t->data_ptr() % 16 == 0, what, ": state shards: 16-byte aligned fp32 of at least ", shard,
+                " elements (this rank's slice) on one device");
+  }
+  for (const torch::Tensor* t : {&table, (const torch::Tensor*)&partials, (const torch::Tensor*)&tickets,
+                                 (const torch::Tensor*)&ratios}) {
+    check_cuda_contig(*t, what);
+    TORCH_CHECK(t->device() == like.device(), what, ": the table and the workspaces live on the state's device");
+  }
+  const int64_t n_tensors = tickets.numel();
+  TORCH_CHECK(n_chunks >= 0 && n_chunks <= shard && n_tensors >= 1 && table.scalar_type() == torch::kInt64 &&
+              table.numel() == (n_chunks + n_tensors) * b2::kLwRow, what, ": table: int64 of (chunks + tensors) * ", b2::kLwRow,
+              " entries from sharded_layerwise_table, tickets: one per tensor");
+  TORCH_CHECK(tickets.scalar_type() == torch::kInt32, what, ": tickets: int32 [tensors], zero before the first call");
+  TORCH_CHECK(partials.scalar_type() == torch::kFloat32 && partials.numel() == 2 * n_chunks &&
+              (n_chunks == 0 || (uintptr_t)partials.data_ptr() % 8 == 0), what, ": partials: fp32 [2 * chunks]");
+  TORCH_CHECK(ratios.scalar_type() == torch::kFloat32 && ratios.numel() == n_tensors, what, ": ratios: fp32 [tensors]");
+  b2::LwArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.m = states[0]->data_ptr<float>();
+  (lamb ? a.v : a.g) = states[1]->data_ptr<float>();
+  a.table = reinterpret_cast<const long long*>(table.data_ptr<int64_t>());
+  a.n_chunks = (int)n_chunks; a.n_tensors = (int)n_tensors;
+  a.partials = n_chunks > 0 ? partials.data_ptr<float>() : nullptr;
+  a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int32_t>());
+  a.ratios = ratios.data_ptr<float>();
+  a.zero_grad = zero_grad ? 1 : 0;
   return a;
 }
 
@@ -1720,6 +1809,65 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("trust_coefficient"), py::arg("eps"), py::arg("nesterov"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
      py::arg("grad_scale") = py::none());
+  py::class_<ShardedLwTable>(m, "ShardedLwTable", "one rank's chunk table of a sharded FlatLAMB / FlatLARS bucket")
+      .def_readonly("table", &ShardedLwTable::table)
+      .def_readonly("n_chunks", &ShardedLwTable::n_chunks)
+      .def_readonly("n", &ShardedLwTable::n)
+      .def_readonly("rank", &ShardedLwTable::rank)
+      .def_readonly("world", &ShardedLwTable::world);
+  m.def("sharded_layerwise_table", &sharded_layerwise_table, py::arg("offsets"), py::arg("numels"), py::arg("adapt"), py::arg("n"),
+        py::arg("rank"), py::arg("world"), py::arg("device"),
+        "sharded FlatLAMB / FlatLARS: the chunk table of rank `rank`'s slice of a padded bucket of n elements");
+  // The sharded FlatLAMB update of one bucket (csrc/sharded_layerwise.cu): the gradient exchange, LAMB on this rank's slice
+  // with its exp_avg / exp_avg_sq shards, the per-tensor sums exchanged through the symmetric `sums` buffers ([2 * tensors]
+  // fp64 per rank), and the new parameters stored into every rank's flat in `params`.  scalars: lamb_flat's.
+  m.def("sharded_lamb", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                           std::vector<unsigned long long> sums, std::vector<unsigned long long> sigs, torch::Tensor exp_avg,
+                           torch::Tensor exp_avg_sq, const ShardedLwTable& table, torch::Tensor partials,
+                           torch::Tensor tickets, torch::Tensor ratios, size_t n_vec, std::vector<double> scalars, double scale,
+                           bool zero_grad, int rank, int world, int max_blocks) {
+    TORCH_CHECK(scalars.size() == 8, "sharded_lamb: scalars: (1 - beta1, beta2, 1 - beta2, sqrt(bc2), eps, 1 / bc1, lr, "
+                "weight_decay), got ", scalars.size(), " values");
+    for (double x : scalars) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), "sharded_lamb: scalars must be finite in fp32");
+    TORCH_CHECK((float)scalars[3] > 0.f && scalars[4] >= 0.0, "sharded_lamb: sqrt(bc2) must be > 0 (update t >= 1) and eps >= 0");
+    b2::LwArgs a = sharded_layerwise_args("sharded_lamb", true, bf16, grads, params, sums, sigs, {&exp_avg, &exp_avg_sq},
+                                          table, partials, tickets, ratios, n_vec, zero_grad, rank, world);
+    a.w1 = (float)scalars[0]; a.beta2 = (float)scalars[1]; a.c2 = (float)scalars[2]; a.sbc2 = (float)scalars[3];
+    a.eps = (float)scalars[4]; a.rbc1 = (float)scalars[5]; a.lr = (float)scalars[6]; a.wd = (float)scalars[7];
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params), sm = to_ptrs(sums);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(exp_avg.device());
+    ck_cuda(b2_sharded_layerwise_launch(1, bf16 ? 1 : 0, &g, &p, &sm, &s, &a, n_vec, (float)scale, rank, world, max_blocks,
+                                        cur_stream()), "sharded_lamb launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sums"), py::arg("sigs"), py::arg("exp_avg"),
+     py::arg("exp_avg_sq"), py::arg("table"), py::arg("partials"), py::arg("tickets"), py::arg("ratios"),
+     py::arg("n_vec"), py::arg("scalars"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"),
+     py::arg("max_blocks") = 0);
+  // The sharded FlatLARS update: as sharded_lamb, with this rank's momentum shard and `grad_workspace`, a shard that keeps the
+  // averaged gradient of the slice between the two kernels.
+  m.def("sharded_lars", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                           std::vector<unsigned long long> sums, std::vector<unsigned long long> sigs, torch::Tensor momentum_buf,
+                           torch::Tensor grad_workspace, const ShardedLwTable& table, torch::Tensor partials,
+                           torch::Tensor tickets, torch::Tensor ratios, size_t n_vec, double lr, double momentum,
+                           double weight_decay, double trust_coefficient, double eps, bool nesterov, double scale, bool zero_grad,
+                           int rank, int world, int max_blocks) {
+    check_sgd_options(weight_decay, nesterov, momentum, "sharded_lars");
+    TORCH_CHECK(std::isfinite(lr) && std::isfinite(momentum) && std::isfinite(weight_decay) && trust_coefficient > 0.0 &&
+                std::isfinite(trust_coefficient) && eps >= 0.0 && std::isfinite(eps),
+                "sharded_lars: lr, momentum and weight_decay finite, trust_coefficient > 0 and eps >= 0 finite");
+    b2::LwArgs a = sharded_layerwise_args("sharded_lars", false, bf16, grads, params, sums, sigs, {&momentum_buf, &grad_workspace}, table,
+                                          partials, tickets, ratios, n_vec, zero_grad, rank, world);
+    a.lr = (float)lr; a.mu = (float)momentum; a.wd = (float)weight_decay; a.nesterov = nesterov ? 1 : 0;
+    a.eta64 = trust_coefficient; a.wd64 = weight_decay; a.eps64 = eps;
+    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params), sm = to_ptrs(sums);
+    SignalPadsH s = to_sig(sigs);
+    c10::cuda::CUDAGuard guard(momentum_buf.device());
+    ck_cuda(b2_sharded_layerwise_launch(0, bf16 ? 1 : 0, &g, &p, &sm, &s, &a, n_vec, (float)scale, rank, world, max_blocks,
+                                        cur_stream()), "sharded_lars launch");
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sums"), py::arg("sigs"), py::arg("momentum_buffer"),
+     py::arg("grad_workspace"), py::arg("table"), py::arg("partials"), py::arg("tickets"), py::arg("ratios"),
+     py::arg("n_vec"), py::arg("lr"), py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"),
+     py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
   m.def("adafactor_chunk_elems", [] { return (int64_t)b2::kAfChunk; }, "the largest chunk of an Adafactor chunk table");
   m.def("adafactor_table", &adafactor_table, py::arg("offsets"), py::arg("shapes"), py::arg("strides"), py::arg("state_offsets"),
         py::arg("groups"), py::arg("n"), py::arg("n_state"), py::arg("n_groups"), py::arg("device"),

@@ -45,6 +45,7 @@
 #include "flat_scalars.cuh"
 #include "param_groups.cuh"
 #include "rmsprop_device.cuh"
+#include "shard_grid.h"
 
 namespace b2 {
 
@@ -388,15 +389,7 @@ bool shard_args_ok(const PeerPtrs* grads, const PeerPtrs* params, const b2::Sign
   return true;
 }
 
-// The two-shot all-reduce's grid: ceil(ceil(slice / 512) / 2) CTAs, at most max_blocks.
-dim3 shard_grid(size_t n_vec, int world, int max_blocks) {
-  if (max_blocks <= 0 || max_blocks > B2_MAX_BLOCKS) max_blocks = B2_MAX_BLOCKS;
-  size_t blocks = (n_vec / world + b2::kShardThreads - 1) / b2::kShardThreads;
-  blocks = (blocks + 1) / 2;
-  if (blocks < 1) blocks = 1;
-  if (blocks > (size_t)max_blocks) blocks = (size_t)max_blocks;
-  return dim3((unsigned)blocks);
-}
+static_assert(b2::kShardThreads == 512, "shard_grid.h sizes the grid for 512-thread CTAs");
 
 }  // namespace
 

@@ -326,6 +326,7 @@ class _FlatOptimizer:
         self._shard_mode = None
         if self.sharded and self._world > 1:
             self._shard_mode = "kernel" if all(_peer_world(gb) for gb in self.buckets) else "torch"
+        self._check_shard_mode()         # before any parameter is rebound or hook registered
         self._shards: List[tuple] = []   # per bucket: (gradient vectors, padded elements, elements per rank, whole parameter flat, its handle)
         self._done = [False] * len(self.buckets)
         for gb in self.buckets:
@@ -360,6 +361,9 @@ class _FlatOptimizer:
         self._set_groups(param_groups)
         if self.capturable:
             self._init_capturable(name)
+
+    def _check_shard_mode(self) -> None:
+        """Raise if this optimizer has no update for ``_shard_mode``; every mode is supported here."""
 
     # ------------------------------------------------------------------ capturable: step counter and scalars on the device
     def _init_capturable(self, name: str) -> None:
@@ -1652,34 +1656,55 @@ def lamb_scalars(lr: float, betas: tuple, eps: float, weight_decay: float, t: in
 class _LayerwiseOptimizer(_FlatOptimizer):
     """What :class:`FlatLAMB` and :class:`FlatLARS` share: the per-tensor adaptation flags, the trust ratios of the last
     update, and on CUDA fp32 buckets the chunk table and the workspaces of the layer-wise kernels (csrc/layerwise.cu).
-    :attr:`param_groups` is one group with every parameter, whose ``lr`` / ``weight_decay`` are the optimizer's."""
+    :attr:`param_groups` is one group with every parameter, whose ``lr`` / ``weight_decay`` are the optimizer's.
+
+    ``sharded=True`` over several ranks of one peer-memory world: per bucket the two kernels of csrc/sharded_layerwise.cu run
+    in place of the all-reduce, on this rank's chunk table (its slice of the bucket), with a symmetric fp64 buffer of the
+    per-tensor sums that the ranks add in rank order.  Elsewhere (gloo, several machines, NCCL) ``sharded=True`` over
+    several ranks raises ``ValueError``."""
 
     lr = _group_attr("lr")
     weight_decay = _group_attr("weight_decay")
 
     def __init__(self, model: nn.Module, zero_grad: bool, group, lr_schedule: Optional[LRSchedule],
                  max_grad_norm: Optional[float], sharded: bool, exclude_from_adaptation):
-        if sharded:
-            raise ValueError(f"{type(self).__name__} cannot be sharded: the norms of the tensors that straddle shard boundaries "
-                             "would need an exchange between the ranks before any update; use sharded=False")
-        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, False)
+        super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded)
         exclude = exclude_1d if exclude_from_adaptation is None else exclude_from_adaptation
         names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
         self.adapt: List[List[bool]] = [[not bool(exclude(names.get(id(p), ""), p)) for p in gb.params] for gb in self.buckets]
         # the trust ratio of every tensor of a bucket (bucket order) in the last update; 1 before the first
         self.ratio_flats = [torch.ones(len(gb.params), dtype=torch.float32, device=pf.device)
                             for gb, pf in zip(self.buckets, self.param_flats)]
-        self._lw = []                    # per bucket on the kernel path: (table, chunks, partials, tickets, sums), else None
-        for gb, pf, adapt in zip(self.buckets, self.param_flats, self.adapt):
-            if not (pf.is_cuda and gb.flat.dtype == torch.float32):
+        # per bucket on a kernel path: (table, chunks, partials, tickets, sums), else None.  Sharded, the table is this rank's
+        # slice's (a ShardedLwTable) and `sums` the symmetric handle of the [2 * tensors] fp64 sums every rank reads.
+        self._lw = []
+        for k, (gb, pf, adapt) in enumerate(zip(self.buckets, self.param_flats, self.adapt)):
+            n_t, numels = len(gb.params), [p.numel() for p in gb.params]
+            if self._shard_mode == "kernel":
+                table = self._kernel().sharded_layerwise_table(gb.offsets, numels, adapt, self._shards[k][1], gb.world.rank,
+                                                               self._world, pf.device)
+                n_chunks = table.n_chunks
+                sums = gb.world.alloc_bytes(16 * n_t, ll=False)
+            elif self._shard_mode is None and pf.is_cuda and gb.flat.dtype == torch.float32:
+                table, n_chunks = self._kernel().layerwise_table(gb.offsets, numels, adapt, gb.numel, pf.device)
+                sums = torch.zeros(2 * n_t, dtype=torch.float64, device=pf.device)
+            else:
                 self._lw.append(None)
                 continue
-            table, n_chunks = self._kernel().layerwise_table(gb.offsets, [p.numel() for p in gb.params], adapt, gb.numel,
-                                                             pf.device)
-            n_t = len(gb.params)
             self._lw.append((table, n_chunks, torch.zeros(2 * n_chunks, dtype=torch.float32, device=pf.device),
-                             torch.zeros(n_t, dtype=torch.int32, device=pf.device),
-                             torch.zeros(2 * n_t, dtype=torch.float64, device=pf.device)))
+                             torch.zeros(n_t, dtype=torch.int32, device=pf.device), sums))
+
+    def _check_shard_mode(self) -> None:
+        if self._shard_mode == "torch":
+            raise ValueError(f"{type(self).__name__}(sharded=True) over several ranks needs one peer-memory world (backend "
+                             "'b200' on one machine): the norms of the tensors that straddle shard boundaries are exchanged "
+                             "between the ranks inside the sharded kernels; use sharded=False")
+
+    def _sharded_args(self, k: int) -> tuple:
+        """The leading arguments of ``sharded_lamb`` / ``sharded_lars`` for bucket ``k``: dtype flag and per-rank pointers."""
+        gb = self.buckets[k]
+        return (gb.flat.dtype == torch.bfloat16, gb.symm_handle.ptrs, self._shards[k][4].ptrs, self._lw[k][4].ptrs,
+                gb.symm_handle.sig_ptrs)
 
     def _tensors(self, k: int, flats: list):
         """Per tensor of bucket ``k``: (index, adapted?, its 1-D slice of each flat in ``flats``)."""
@@ -1715,8 +1740,9 @@ class FlatLAMB(_LayerwiseOptimizer):
     per-tensor norms in a fixed order (fp32 per thread and CTA, fp64 over the chunks of a tensor) and apply the update with
     no host synchronisation; elsewhere (CPU tensors, bf16 buckets) torch ops run the same semantics on each tensor.
     ``max_grad_norm`` clips first, as in :class:`FlatAdamW`.  :meth:`trust_ratios` gives the last update's ratios.  The
-    checkpoint forms are :class:`FlatAdamW`'s, so LAMB state loads into ``FlatAdamW`` and back.  ``sharded=True`` raises
-    ``ValueError``."""
+    checkpoint forms are :class:`FlatAdamW`'s, so LAMB state loads into ``FlatAdamW`` and back.  ``sharded=True`` is ZeRO
+    stage 1 on one peer-memory world (both moments 1/W per rank, the per-tensor norms exchanged between the ranks inside the
+    sharded kernels, csrc/sharded_layerwise.cu); over several ranks elsewhere it raises ``ValueError``."""
 
     def __init__(self, model: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6,
                  weight_decay: float = 0.01, zero_grad: bool = True, group=None, lr_schedule: Optional[LRSchedule] = None,
@@ -1731,6 +1757,12 @@ class FlatLAMB(_LayerwiseOptimizer):
     def scalars(self) -> list:
         """:func:`lamb_scalars` of the next update (t = ``steps`` + 1, lr = :meth:`lr_at`)."""
         return lamb_scalars(self.lr_at(), self.betas, self.eps, self.weight_decay, self.steps + 1)
+
+    def _sharded_kernel(self, k: int, max_blocks: int) -> None:
+        table, _, partials, tickets, _ = self._lw[k]
+        self._kernel().sharded_lamb(*self._sharded_args(k), self.exp_avg_flats[k], self.exp_avg_sq_flats[k], table, partials,
+                                    tickets, self.ratio_flats[k], self._shards[k][0], self.scalars(), 1.0 / self._world,
+                                    self.fused_zero, self.buckets[k].world.rank, self._world, max_blocks)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
         sc = self.scalars()
@@ -1792,8 +1824,9 @@ class FlatLARS(_LayerwiseOptimizer):
     :func:`exclude_1d`).  On CUDA fp32 buckets two kernels per bucket (csrc/layerwise.cu) form the norms and apply
     :class:`FlatSGD`'s fmaf sequence to ``d``; elsewhere the ratio is formed with torch ops and
     ``torch.optim.SGD(foreach=False)``'s update runs on ``d``.  ``max_grad_norm`` clips ``g`` first.  The checkpoint forms
-    are :class:`FlatSGD`'s (``named_momentum``), so LARS momentum loads into ``FlatSGD`` and back.  ``sharded=True``
-    raises ``ValueError``."""
+    are :class:`FlatSGD`'s (``named_momentum``), so LARS momentum loads into ``FlatSGD`` and back.  ``sharded=True`` is
+    :class:`FlatLAMB`'s: ZeRO stage 1 on one peer-memory world (momentum 1/W per rank), ``ValueError`` over several ranks
+    elsewhere."""
 
     def __init__(self, model: nn.Module, lr: float = 0.1, momentum: float = 0.9, weight_decay: float = 1e-4,
                  trust_coefficient: float = 1e-3, eps: float = 1e-8, nesterov: bool = False, zero_grad: bool = True,
@@ -1805,6 +1838,15 @@ class FlatLARS(_LayerwiseOptimizer):
         self.trust_coefficient, self.eps, self.nesterov = float(trust_coefficient), float(eps), bool(nesterov)
         super().__init__(model, zero_grad, group, lr_schedule, max_grad_norm, sharded, exclude_from_adaptation)
         self.momentum_flats: List[torch.Tensor] = [self._state_flat(k) for k in range(len(self.buckets))]
+        # sharded kernel path: the averaged gradient of this rank's slice, kept between the two kernels
+        self._grad_shards = [self._state_flat(k) for k in range(len(self.buckets))] if self._shard_mode == "kernel" else None
+
+    def _sharded_kernel(self, k: int, max_blocks: int) -> None:
+        table, _, partials, tickets, _ = self._lw[k]
+        self._kernel().sharded_lars(*self._sharded_args(k), self.momentum_flats[k], self._grad_shards[k], table, partials,
+                                    tickets, self.ratio_flats[k], self._shards[k][0], self.lr_at(), self.momentum, self.weight_decay,
+                                    self.trust_coefficient, self.eps, self.nesterov, 1.0 / self._world, self.fused_zero,
+                                    self.buckets[k].world.rank, self._world, max_blocks)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
         from torch.optim.sgd import sgd

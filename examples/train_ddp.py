@@ -137,9 +137,9 @@ def run(rank, size):
     elif CFG["optimizer"] == "adafactor":      # torch.optim.Adafactor's defaults, with a little decoupled weight decay
         optimizer = dist.FlatAdafactor(model, lr=1e-2, weight_decay=1e-4, param_groups=groups)
     elif CFG["optimizer"] == "lamb":
-        optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2)
+        optimizer = dist.FlatLAMB(model, lr=2e-3, weight_decay=1e-2, sharded=CFG["sharded"])
     elif CFG["optimizer"] == "lars":
-        optimizer = dist.FlatLARS(model, lr=2.0, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-2)
+        optimizer = dist.FlatLARS(model, lr=2.0, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-2, sharded=CFG["sharded"])
     else:
         optimizer = dist.FlatSGD(model, lr=0.05, momentum=0.9, weight_decay=1e-4, sharded=CFG["sharded"], param_groups=groups,
                                  **cap)
@@ -184,7 +184,7 @@ if __name__ == "__main__":
                     help="sharded=True: each rank keeps the optimizer state of, and updates, 1/size of every bucket")
     ap.add_argument("--optimizer", choices=("sgd", "adamw", "rmsprop", "adafactor", "lamb", "lars"),
                     default="sgd", help="FlatSGD (momentum SGD, the default), FlatAdamW, FlatRMSprop, FlatAdafactor, FlatLAMB or "
-                                        "FlatLARS (the last three unsharded)")
+                                        "FlatLARS (adafactor unsharded; lamb / lars sharded on --backend b200 only)")
     ap.add_argument("--no-decay-bias-norm", action="store_true",
                     help="sgd / adamw / rmsprop / adafactor: no weight decay on biases and norm weights (a param_groups entry with "
                          "weight_decay=0)")
@@ -209,6 +209,9 @@ if __name__ == "__main__":
     if a.optimizer == "adafactor" and a.sharded_optimizer:
         ap.error("--optimizer adafactor cannot be sharded: a factored tensor's state is its row and column vectors, which do "
                  "not split along the flat slices of the sharded exchange")
+    if a.optimizer in ("lamb", "lars") and a.sharded_optimizer and a.backend != "b200":
+        ap.error(f"--optimizer {a.optimizer} is sharded on --backend b200 only: the per-tensor norms of the slices are exchanged "
+                 "inside the peer-memory kernels")
     if a.optimizer == "adafactor" and a.cuda_graph:
         ap.error("--optimizer adafactor has no capturable form: --cuda-graph needs sgd / adamw / rmsprop")
     if a.cuda_graph and (a.optimizer not in ("sgd", "adamw", "rmsprop") or a.backend != "b200"):
