@@ -321,15 +321,21 @@ __global__ void __launch_bounds__(T, 1) convnet_eval_kernel(EvalArgs a) {
 extern "C" {
 
 // Resident CTAs of the eval kernel on `dev` (0 on error): its grid never exceeds this, and the slot buffer holds 2 + 2 x this.
+// The shared-memory opt-in and the occupancy query act on the current device, so they run with `dev` made current (and the
+// caller's device restored): the opt-in is then in place on `dev` before its first launch, whichever device is current.
 int b2_convnet_eval_max_ctas(int dev) {
   static int cached[64] = {0};
   if (dev < 0 || dev >= 64) return 0;
   if (cached[dev] == 0) {
+    int prev = -1;
+    if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(dev) != cudaSuccess) return 0;
     const int smem = (int)sizeof(ce::Smem);
-    if (cudaFuncSetAttribute(ce::convnet_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return 0;
     int per_sm = 0, sms = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ce::convnet_eval_kernel, ce::T, smem) != cudaSuccess) return 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
+    const bool ok =
+        cudaFuncSetAttribute(ce::convnet_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ce::convnet_eval_kernel, ce::T, smem) == cudaSuccess &&
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess;
+    if (cudaSetDevice(prev) != cudaSuccess || !ok) return 0;
     cached[dev] = per_sm * sms;
   }
   return cached[dev];

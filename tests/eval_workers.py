@@ -77,3 +77,36 @@ def w_fused_evaluate_world(rank, size):
     assert got["n"] == 10007 == int(whole[2]) and got["correct"] == int(whole[1]), (got, whole)
     assert abs(got["loss"] * 10007 - whole[0]) <= 1e-6 * abs(whole[0]), (got, whole)
     b2.barrier()
+
+
+def w_evaluate_cuda_net_gloo(rank, size):
+    """evaluate(Net on cuda:0) over a gloo world whose ranks share one GPU: every rank gets the dict of one process
+    evaluating the whole set, also when a rank's shard is empty (N = 2 over 3 ranks)."""
+    from dist_tuto.pth_b200.ops.convnet_eval import convnet_evaluate
+    from dist_tuto.pth_b200.ops.convnet_fused import pack_params
+    dev = torch.device("cuda", 0)
+    torch.manual_seed(5)
+    net = Net().to(dev)
+    for n in (10, 2):
+        ds = SyntheticMNIST(n=n, seed=31 + n)
+        got = b2.evaluate(net, ds)
+        whole = convnet_evaluate(pack_params(net), ds.images.to(dev), ds.labels.to(dev), ds.mean, ds.std).tolist()
+        assert got["n"] == n == int(whole[2]) and got["correct"] == int(whole[1]), (got, whole)
+        assert abs(got["loss"] * n - whole[0]) <= 1e-6 * abs(whole[0]), (got, whole)
+        assert all(d == got for d in _gathered(got))
+    b2.barrier()
+
+
+def w_evaluate_on_second_gpu(rank, size):
+    """The first evaluation on cuda:1 made while cuda:0 is current gives cuda:0's result, and leaves cuda:0 current."""
+    import copy
+    torch.cuda.set_device(0)
+    ds = SyntheticMNIST(n=3001, seed=17)
+    torch.manual_seed(9)
+    net = Net()
+    on1 = b2.evaluate(copy.deepcopy(net).to("cuda:1"), ds)
+    assert torch.cuda.current_device() == 0
+    on0 = b2.evaluate(net.to("cuda:0"), ds)
+    # bit-equal on two GPUs of one model; another SM count would split the loss sum over other CTAs
+    assert on1["n"] == on0["n"] == 3001 and on1["correct"] == on0["correct"], (on1, on0)
+    assert abs(on1["loss"] - on0["loss"]) <= 1e-6 * abs(on0["loss"]), (on1, on0)
