@@ -261,6 +261,72 @@ const float* amp_scalar_ptr(const c10::optional<torch::Tensor>& t, const torch::
               name, ": an fp32 CUDA tensor of one element on the device of the buffers");
   return t->data_ptr<float>();
 }
+// GradScaler's (grad_scale, found_inf) of an update launch (see amp_scalar_ptr).  A capturable update (`paired`) decides the
+// skip on the device, so it takes grad_scale only with found_inf.
+std::pair<const float*, const float*> amp_pair(const c10::optional<torch::Tensor>& grad_scale,
+                                               const c10::optional<torch::Tensor>& found_inf, bool paired, const torch::Tensor& like,
+                                               const char* what) {
+  TORCH_CHECK(!paired || found_inf.has_value() || !grad_scale.has_value(), what,
+              ": grad_scale comes with found_inf (GradScaler sets both)");
+  return {amp_scalar_ptr(grad_scale, like, what, "grad_scale"), amp_scalar_ptr(found_inf, like, what, "found_inf")};
+}
+
+// The clipping arguments of an update launch: max_norm (0 without clipping), grad_sqnorm's per-bucket sums and their count,
+// and the optional grad_norm_out.
+struct Clip {
+  float max_norm;
+  const double* sq;
+  int n_buckets;
+  float* gn;
+};
+Clip clip_args(const py::object& max_grad_norm, const c10::optional<torch::Tensor>& sqnorms,
+               const c10::optional<torch::Tensor>& grad_norm_out, const char* what) {
+  Clip c{check_max_grad_norm(max_grad_norm, what), nullptr, 0, nullptr};
+  if (c.max_norm > 0.f) {
+    TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
+                sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
+    c.sq = sqnorms->data_ptr<double>();
+    c.n_buckets = (int)sqnorms->numel();
+  }
+  c.gn = grad_norm_ptr(grad_norm_out, what);
+  return c;
+}
+
+// The flat buffers of an update (parameters, gradients, state; null entries are absent optional states): contiguous 16-byte
+// aligned fp32 CUDA tensors on one device with `n` elements each (at_least: n or more).  `names` names them in the message.
+// The first entry is never null.
+void check_flats(const std::vector<const torch::Tensor*>& ts, int64_t n, bool at_least, const char* names, const char* what) {
+  for (const torch::Tensor* t : ts)
+    TORCH_CHECK(t == nullptr || (t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32 &&
+                                 t->device() == ts[0]->device() && (at_least ? t->numel() >= n : t->numel() == n) &&
+                                 (uintptr_t)t->data_ptr() % 16 == 0),
+                what, ": ", names, ": 16-byte aligned contiguous fp32 CUDA tensors on one device, of ",
+                at_least ? "at least " : "one size, ", n, " elements");
+}
+
+// The per-rank pointers of a sharded update (csrc/sharded_sgd.cu, csrc/sharded_layerwise.cu): one gradient bucket,
+// parameter flat, signal pad and, for the layer-wise kernels (`sums` given), sums buffer per rank, none null or misaligned,
+// and a bucket of n_vec 16-byte vectors that splits into `world` slices.  `shard` is the elements of one slice.
+struct Peers {
+  int64_t shard;
+  PeerPtrs grads, params, sums;
+  SignalPadsH sigs;
+};
+Peers sharded_peers(const char* what, const std::vector<unsigned long long>& grads, const std::vector<unsigned long long>& params,
+                    const std::vector<unsigned long long>* sums, const std::vector<unsigned long long>& sigs, size_t n_vec, bool bf16,
+                    int rank, int world) {
+  check_world(rank, world, what);
+  TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world &&
+              (sums == nullptr || (int)sums->size() == world), what, ": one gradient bucket, parameter flat, ",
+              sums != nullptr ? "sums buffer " : "", "and signal pad per rank, got ", grads.size(), ", ", params.size(),
+              sums != nullptr ? ", " + std::to_string(sums->size()) : "", " and ", sigs.size(), " for world ", world);
+  TORCH_CHECK(n_vec % (size_t)world == 0, what, ": every rank owns n_vec / world vectors, so n_vec must be a multiple of world "
+              "(pad the buffers), got n_vec ", n_vec, " for world ", world);
+  for (const auto* v : {&grads, &params, &sigs, sums != nullptr ? sums : &sigs})
+    for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, what, ": null or misaligned per-rank pointer");
+  return {(int64_t)(n_vec / (size_t)world * (bf16 ? 8 : 4)), to_ptrs(grads), to_ptrs(params),
+          to_ptrs(sums != nullptr ? *sums : std::vector<unsigned long long>()), to_sig(sigs)};
+}
 
 // One AdamW update's scalars (csrc/adamw.h), computed by the host in fp64 (ops/optim.py adamw_scalars): (1 - lr*wd,
 // 1 - beta1, beta2, 1 - beta2, lr / bc1, sqrt(bc2), eps), each rounded once to fp32 here.
@@ -291,20 +357,17 @@ b2::RmspropScalars to_rmsprop(const std::vector<double>& v, bool centered, const
 }
 
 // The state flats of an RMSprop update: square_avg, plus grad_avg exactly when centered and momentum_buffer exactly when
-// momentum > 0; contiguous 16-byte aligned fp32 on `like`'s device with `n` elements (at_least: n or more).  Returns the
-// optional states' pointers, null when absent.
-std::pair<float*, float*> rmsprop_state(const torch::Tensor& square_avg, const c10::optional<torch::Tensor>& grad_avg,
+// momentum > 0, checked with the update's other flats `flats` (check_flats).  Returns the optional states' pointers, null
+// when absent.
+std::pair<float*, float*> rmsprop_state(std::vector<const torch::Tensor*> flats, const torch::Tensor& square_avg,
+                                        const c10::optional<torch::Tensor>& grad_avg,
                                         const c10::optional<torch::Tensor>& momentum_buffer, const b2::RmspropScalars& s,
-                                        int64_t n, bool at_least, const torch::Tensor& like, const char* what) {
+                                        int64_t n, bool at_least, const char* names, const char* what) {
   TORCH_CHECK(grad_avg.has_value() == (s.centered != 0), what, ": grad_avg is given exactly when centered=True");
   TORCH_CHECK(momentum_buffer.has_value() == (s.momentum != 0), what, ": momentum_buffer is given exactly when momentum > 0");
-  for (const torch::Tensor* t : {&square_avg, grad_avg.has_value() ? &*grad_avg : &square_avg,
-                                 momentum_buffer.has_value() ? &*momentum_buffer : &square_avg}) {
-    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32 && t->device() == like.device() &&
-                (at_least ? t->numel() >= n : t->numel() == n) && (uintptr_t)t->data_ptr() % 16 == 0, what,
-                ": square_avg, grad_avg and momentum_buffer: 16-byte aligned contiguous fp32 CUDA of ", at_least ? "at least " : "",
-                n, " elements on the parameters' device");
-  }
+  flats.insert(flats.end(), {&square_avg, grad_avg.has_value() ? &*grad_avg : nullptr,
+                             momentum_buffer.has_value() ? &*momentum_buffer : nullptr});
+  check_flats(flats, n, at_least, names, what);
   return {grad_avg.has_value() ? grad_avg->data_ptr<float>() : nullptr,
           momentum_buffer.has_value() ? momentum_buffer->data_ptr<float>() : nullptr};
 }
@@ -394,12 +457,8 @@ b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, 
                           const c10::optional<torch::Tensor>& sqnorms, const c10::optional<torch::Tensor>& grad_norm_out,
                           const c10::optional<torch::Tensor>& grad_scale) {
   std::vector<const torch::Tensor*> flats = {&p, &g};
-  for (torch::Tensor* t : states) flats.push_back(t);
-  for (const torch::Tensor* t : flats) {
-    check_cuda_contig(*t, what);
-    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && t->device() == p.device() &&
-                (uintptr_t)t->data_ptr() % 16 == 0, what, ": parameters, gradients and state: 16-byte aligned fp32 of one size on one device");
-  }
+  flats.insert(flats.end(), states.begin(), states.end());
+  check_flats(flats, p.numel(), false, "parameters, gradients and state", what);
   for (const torch::Tensor* t : {&table, (const torch::Tensor*)&partials, (const torch::Tensor*)&tickets,
                                  (const torch::Tensor*)&sums, (const torch::Tensor*)&ratios}) {
     check_cuda_contig(*t, what);
@@ -424,47 +483,32 @@ b2::LwArgs layerwise_args(const char* what, torch::Tensor& p, torch::Tensor& g, 
   a.partials = partials.data_ptr<float>(); a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int32_t>());
   a.sums = sums.data_ptr<double>(); a.ratios = ratios.data_ptr<float>();
   a.zero_grad = zero_grad ? 1 : 0;
-  a.max_norm = check_max_grad_norm(max_grad_norm, what);
-  if (a.max_norm > 0.f) {
-    TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-    a.sqnorms = sqnorms->data_ptr<double>();
-    a.n_buckets = (int)sqnorms->numel();
-  }
-  a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
+  const Clip c = clip_args(max_grad_norm, sqnorms, grad_norm_out, what);
+  a.max_norm = c.max_norm; a.sqnorms = c.sq; a.n_buckets = c.n_buckets; a.grad_norm_out = c.gn;
   a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
   return a;
 }
 
-// The checked arguments of a sharded layer-wise launch (csrc/sharded_layerwise.cu): the per-rank pointer lists, and this
-// rank's table (sharded_layerwise_table), workspaces and state flats (`states`: m, then v (lamb) or LARS's gradient workspace), the
-// state flats of at least one slice (n_vec / world x 4, x 8 with bf16) each.
-b2::LwArgs sharded_layerwise_args(const char* what, bool lamb, bool bf16, const std::vector<unsigned long long>& grads,
-                                  const std::vector<unsigned long long>& params, const std::vector<unsigned long long>& sums,
-                                  const std::vector<unsigned long long>& sigs, const std::vector<torch::Tensor*>& states,
-                                  const ShardedLwTable& tab, torch::Tensor& partials, torch::Tensor& tickets,
-                                  torch::Tensor& ratios, size_t n_vec, bool zero_grad, int rank, int world) {
-  check_world(rank, world, what);
-  TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sums.size() == world && (int)sigs.size() == world,
-              what, ": one gradient bucket, parameter flat, sums buffer and signal pad per rank, got ", grads.size(), ", ",
-              params.size(), ", ", sums.size(), " and ", sigs.size(), " for world ", world);
-  TORCH_CHECK(n_vec % (size_t)world == 0, what, ": every rank owns n_vec / world vectors, so n_vec must be a multiple of world "
-              "(pad the buffers), got n_vec ", n_vec, " for world ", world);
+// The checked arguments of a sharded layer-wise launch (csrc/sharded_layerwise.cu): the per-rank pointer lists
+// (sharded_peers), and this rank's table (sharded_layerwise_table), workspaces and state flats (`states`: m, then v (lamb) or
+// LARS's gradient workspace), the state flats of at least one slice (n_vec / world x 4, x 8 with bf16) each.
+std::pair<b2::LwArgs, Peers> sharded_layerwise_args(const char* what, bool lamb, bool bf16,
+                                                    const std::vector<unsigned long long>& grads,
+                                                    const std::vector<unsigned long long>& params,
+                                                    const std::vector<unsigned long long>& sums,
+                                                    const std::vector<unsigned long long>& sigs,
+                                                    const std::vector<torch::Tensor*>& states, const ShardedLwTable& tab,
+                                                    torch::Tensor& partials, torch::Tensor& tickets, torch::Tensor& ratios,
+                                                    size_t n_vec, bool zero_grad, int rank, int world) {
+  const Peers peers = sharded_peers(what, grads, params, &sums, sigs, n_vec, bf16, rank, world);
   const int64_t n_elems = (int64_t)n_vec * (bf16 ? 8 : 4);
   TORCH_CHECK(tab.rank == rank && tab.world == world && tab.n == n_elems, what, ": the table was built for rank ", tab.rank,
               " of ", tab.world, " on a bucket of ", tab.n, " elements; this launch is rank ", rank, " of ", world, " on ", n_elems);
   const torch::Tensor& table = tab.table;
   const int64_t n_chunks = tab.n_chunks;
-  for (const auto* v : {&grads, &params, &sums, &sigs})
-    for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, what, ": null or misaligned per-rank pointer");
-  const int64_t shard = n_elems / world;
+  const int64_t shard = peers.shard;
   torch::Tensor& like = *states[0];
-  for (const torch::Tensor* t : states) {
-    check_cuda_contig(*t, what);
-    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() >= shard && t->device() == like.device() &&
-                (uintptr_t)t->data_ptr() % 16 == 0, what, ": state shards: 16-byte aligned fp32 of at least ", shard,
-                " elements (this rank's slice) on one device");
-  }
+  check_flats({states.begin(), states.end()}, shard, true, "state shards (this rank's slice)", what);
   for (const torch::Tensor* t : {&table, (const torch::Tensor*)&partials, (const torch::Tensor*)&tickets,
                                  (const torch::Tensor*)&ratios}) {
     check_cuda_contig(*t, what);
@@ -488,7 +532,7 @@ b2::LwArgs sharded_layerwise_args(const char* what, bool lamb, bool bf16, const 
   a.tickets = reinterpret_cast<unsigned int*>(tickets.data_ptr<int32_t>());
   a.ratios = ratios.data_ptr<float>();
   a.zero_grad = zero_grad ? 1 : 0;
-  return a;
+  return {a, peers};
 }
 
 // FlatAdafactor (csrc/adafactor.cu): the chunk table of one bucket (adafactor.h) from its tensors' offsets, shapes, strides,
@@ -1228,63 +1272,135 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     ck_cuda(b2_grad_sqnorm_launch(g.data_ptr<float>(), (size_t)g.numel(), workspace.data_ptr<float>(), sqnorms.data_ptr<double>(), k,
                                   gs, cur_stream()), "grad_sqnorm launch");
   }, py::arg("g"), py::arg("sqnorms"), py::arg("k"), py::arg("workspace"), py::arg("grad_scale") = py::none());
-  m.def("sgd_flat", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad,
-                       bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
-                       c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
-    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat: nesterov needs a nonzero momentum");
-    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "sgd_flat: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
+  // FlatSGD's update of one fp32 bucket (csrc/sgd.cu): sgd_flat with lr / weight_decay, sgd_flat_grouped with group_map and
+  // the groups' lrs / weight_decays (parameter vector i takes those of group group_map[i]), sgd_flat_cap with the scalars
+  // from the block (with group_map, every group's).  With max_grad_norm, g is first scaled by the clip coefficient of the
+  // norm of grad_sqnorm's per-bucket sums; with grad_scale, first unscaled.
+  auto sgd_flat = [](const char* what, torch::Tensor& p, torch::Tensor& mom, torch::Tensor& g,
+                     const c10::optional<torch::Tensor>& group_map, const std::vector<double>& lrs,
+                     const std::vector<double>& weight_decays, const torch::Tensor* block, double mu, bool zero_grad, bool nesterov,
+                     const py::object& max_grad_norm, const c10::optional<torch::Tensor>& sqnorms,
+                     const c10::optional<torch::Tensor>& grad_norm_out, const c10::optional<torch::Tensor>& grad_scale,
+                     const c10::optional<torch::Tensor>& found_inf) {
+    // every group's weight decay (none: the capturable form's come from the block), checked through the smallest
+    check_sgd_options(weight_decays.empty() ? 0.0 : *std::min_element(weight_decays.begin(), weight_decays.end()), nesterov, mu,
+                      what);
+    const Clip c = clip_args(max_grad_norm, sqnorms, grad_norm_out, what);
+    const auto [gsc, fi] = amp_pair(grad_scale, found_inf, block != nullptr, p, what);
+    check_flats({&p, &mom, &g}, p.numel(), false, "p, m and g", what);
+    const int64_t n_ids = (p.numel() + 3) / 4;
+    c10::cuda::CUDAGuard guard(p.device());
+    if (block != nullptr) {
+      ck_cuda(b2_sgd_flat_cap_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(),
+                                     flat_map(group_map, n_ids, what), flat_block(*block, p, what), (float)mu, zero_grad ? 1 : 0,
+                                     nesterov ? 1 : 0, c.max_norm, c.sq, c.n_buckets, c.gn, gsc, fi, cur_stream()),
+              what);
+    } else if (group_map.has_value()) {
+      b2::SgdGroups gs;
+      memset(&gs, 0, sizeof(gs));
+      const int n_groups = check_groups(*group_map, n_ids, lrs, weight_decays, gs.lr, gs.wd, what);
+      ck_cuda(b2_sgd_flat_grouped_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(),
+                                         group_map->data_ptr<uint8_t>(), &gs, n_groups, (float)mu, zero_grad ? 1 : 0,
+                                         nesterov ? 1 : 0, c.max_norm, c.sq, c.n_buckets, c.gn, gsc, cur_stream()),
+              what);
+    } else {
+      ck_cuda(b2_sgd_flat_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), (float)lrs[0],
+                                 (float)mu, (float)weight_decays[0], zero_grad ? 1 : 0, nesterov ? 1 : 0, c.max_norm, c.sq,
+                                 c.n_buckets, c.gn, gsc, cur_stream()),
+              what);
     }
-    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat");
-    check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
-    TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32);
-    TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel());
-    TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0, "16-byte aligned buffers");
-    ck_cuda(b2_sgd_flat_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), (float)lr,
-                               (float)mu, (float)wd, zero_grad, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn,
-                               amp_scalar_ptr(grad_scale, p, "sgd_flat", "grad_scale"), cur_stream()),
-            "sgd_flat launch");
+  };
+  m.def("sgd_flat", [sgd_flat](torch::Tensor p, torch::Tensor mom, torch::Tensor g, double lr, double mu, double wd, bool zero_grad,
+                               bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                               c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
+    sgd_flat("sgd_flat", p, mom, g, c10::nullopt, {lr}, {wd}, nullptr, mu, zero_grad, nesterov, max_grad_norm, sqnorms,
+             grad_norm_out, grad_scale, c10::nullopt);
   }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("lr"), py::arg("mu"), py::arg("weight_decay"), py::arg("zero_grad"),
      py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
      py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
-  m.def("adamw_flat", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
-                         std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
-                         c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
-                         c10::optional<torch::Tensor> grad_scale) {
-    // FlatAdamW's update of one fp32 bucket (csrc/adamw.cu); with max_grad_norm, g is first scaled by the clip coefficient of
-    // the norm of grad_sqnorm's per-bucket sums
-    const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat");
-    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "adamw_flat: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat");
-    check_cuda_contig(p, "p"); check_cuda_contig(exp_avg, "exp_avg"); check_cuda_contig(exp_avg_sq, "exp_avg_sq");
-    check_cuda_contig(g, "g");
-    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel(), "adamw_flat: p, exp_avg, exp_avg_sq and g: fp32 of ",
-                  "one size");
-      TORCH_CHECK((uintptr_t)t->data_ptr() % 16 == 0, "adamw_flat: 16-byte aligned buffers");
-    }
+  m.def("sgd_flat_grouped", [sgd_flat](torch::Tensor p, torch::Tensor mom, torch::Tensor g, torch::Tensor group_map,
+                                       std::vector<double> lrs, std::vector<double> weight_decays, double mu, bool zero_grad,
+                                       bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                                       c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale) {
+    sgd_flat("sgd_flat_grouped", p, mom, g, group_map, lrs, weight_decays, nullptr, mu, zero_grad, nesterov, max_grad_norm, sqnorms,
+             grad_norm_out, grad_scale, c10::nullopt);
+  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"),
+     py::arg("zero_grad"), py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
+  m.def("sgd_flat_cap", [sgd_flat](torch::Tensor p, torch::Tensor mom, torch::Tensor g, c10::optional<torch::Tensor> group_map,
+                                   torch::Tensor block, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
+                                   c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                   c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
+    sgd_flat("sgd_flat_cap", p, mom, g, group_map, {}, {}, &block, mu, zero_grad, nesterov, max_grad_norm, sqnorms, grad_norm_out,
+             grad_scale, found_inf);
+  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("block"), py::arg("mu"), py::arg("zero_grad"),
+     py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
+  // FlatAdamW's update of one fp32 bucket (csrc/adamw.cu): adamw_flat with `scalars`, adamw_flat_grouped with group_map and
+  // the groups' decays / step_sizes (1 - lr_g*wd_g and lr_g / (1 - beta1^t), fp64, each rounded once to fp32 here; the decay
+  // and step_size of `scalars` are then not used), adamw_flat_cap with the scalars from the block (with group_map, every
+  // group's).  Clipping and grad_scale as sgd_flat's.
+  auto adamw_flat = [](const char* what, torch::Tensor& p, torch::Tensor& exp_avg, torch::Tensor& exp_avg_sq, torch::Tensor& g,
+                       const c10::optional<torch::Tensor>& group_map, const std::vector<double>* scalars,
+                       const std::vector<double>& decays, const std::vector<double>& step_sizes, const torch::Tensor* block,
+                       bool zero_grad, const py::object& max_grad_norm, const c10::optional<torch::Tensor>& sqnorms,
+                       const c10::optional<torch::Tensor>& grad_norm_out, const c10::optional<torch::Tensor>& grad_scale,
+                       const c10::optional<torch::Tensor>& found_inf) {
+    const b2::AdamwScalars sc = scalars != nullptr ? to_adamw(*scalars, what) : b2::AdamwScalars{};
+    const Clip c = clip_args(max_grad_norm, sqnorms, grad_norm_out, what);
+    const auto [gsc, fi] = amp_pair(grad_scale, found_inf, block != nullptr, p, what);
+    check_flats({&p, &exp_avg, &exp_avg_sq, &g}, p.numel(), false, "p, exp_avg, exp_avg_sq and g", what);
+    const int64_t n_ids = (p.numel() + 3) / 4;
     c10::cuda::CUDAGuard guard(p.device());
-    ck_cuda(b2_adamw_flat_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
-                                 (size_t)p.numel(), &sc, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
-                                 amp_scalar_ptr(grad_scale, p, "adamw_flat", "grad_scale"), cur_stream()),
-            "adamw_flat launch");
+    if (block != nullptr) {
+      ck_cuda(b2_adamw_flat_cap_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
+                                       g.data_ptr<float>(), (size_t)p.numel(), flat_map(group_map, n_ids, what),
+                                       flat_block(*block, p, what), zero_grad ? 1 : 0, c.max_norm, c.sq, c.n_buckets, c.gn, gsc, fi,
+                                       cur_stream()),
+              what);
+    } else if (group_map.has_value()) {
+      b2::AdamwGroups gs;
+      memset(&gs, 0, sizeof(gs));
+      const int n_groups = check_groups(*group_map, n_ids, decays, step_sizes, gs.decay, gs.step_size, what);
+      ck_cuda(b2_adamw_flat_grouped_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
+                                           g.data_ptr<float>(), (size_t)p.numel(), group_map->data_ptr<uint8_t>(), &sc, &gs,
+                                           n_groups, zero_grad ? 1 : 0, c.max_norm, c.sq, c.n_buckets, c.gn, gsc, cur_stream()),
+              what);
+    } else {
+      ck_cuda(b2_adamw_flat_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
+                                   (size_t)p.numel(), &sc, zero_grad ? 1 : 0, c.max_norm, c.sq, c.n_buckets, c.gn, gsc, cur_stream()),
+              what);
+    }
+  };
+  m.def("adamw_flat", [adamw_flat](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                                   std::vector<double> scalars, bool zero_grad, py::object max_grad_norm,
+                                   c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                   c10::optional<torch::Tensor> grad_scale) {
+    adamw_flat("adamw_flat", p, exp_avg, exp_avg_sq, g, c10::nullopt, &scalars, {}, {}, nullptr, zero_grad, max_grad_norm, sqnorms,
+               grad_norm_out, grad_scale, c10::nullopt);
   }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("scalars"), py::arg("zero_grad"),
      py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(),
      py::arg("grad_scale") = py::none());
+  m.def("adamw_flat_grouped", [adamw_flat](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                                           torch::Tensor group_map, std::vector<double> scalars, std::vector<double> decays,
+                                           std::vector<double> step_sizes, bool zero_grad, py::object max_grad_norm,
+                                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
+                                           c10::optional<torch::Tensor> grad_scale) {
+    adamw_flat("adamw_flat_grouped", p, exp_avg, exp_avg_sq, g, group_map, &scalars, decays, step_sizes, nullptr, zero_grad,
+               max_grad_norm, sqnorms, grad_norm_out, grad_scale, c10::nullopt);
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("scalars"),
+     py::arg("decays"), py::arg("step_sizes"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
+     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
+  m.def("adamw_flat_cap", [adamw_flat](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
+                                       c10::optional<torch::Tensor> group_map, torch::Tensor block, bool zero_grad,
+                                       py::object max_grad_norm, c10::optional<torch::Tensor> sqnorms,
+                                       c10::optional<torch::Tensor> grad_norm_out, c10::optional<torch::Tensor> grad_scale,
+                                       c10::optional<torch::Tensor> found_inf) {
+    adamw_flat("adamw_flat_cap", p, exp_avg, exp_avg_sq, g, group_map, nullptr, {}, {}, &block, zero_grad, max_grad_norm, sqnorms,
+               grad_norm_out, grad_scale, found_inf);
+  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("block"),
+     py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
+     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
   m.def("max_param_groups", [] { return b2::kMaxGroups; }, "the most parameter groups the grouped optimizer kernels take");
   // Capturable FlatSGD / FlatAdamW (csrc/flat_scalars.cuh): the layout of the scalar block in fp32 words and the byte sizes
   // of the block and the table
@@ -1415,198 +1531,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
             "ema_update launch");
   }, py::arg("table"), py::arg("host"), py::arg("w"), py::arg("copy") = false, py::arg("counter") = py::none(),
      py::arg("every") = 1, py::arg("warmup_steps") = 0);
-  // sgd_flat / sgd_flat_grouped (with group_map) with the scalars from the block: arguments as theirs otherwise
-  m.def("sgd_flat_cap", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, c10::optional<torch::Tensor> group_map,
-                           torch::Tensor block, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
-                           c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
-                           c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
-    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_cap: nesterov needs a nonzero momentum");
-    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat_cap");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "sgd_flat_cap: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat_cap");
-    for (const auto* t : {&p, &mom, &g}) {
-      check_cuda_contig(*t, "sgd_flat_cap: p, m and g");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "sgd_flat_cap: p, m and g: 16-byte aligned fp32 of one size");
-    }
-    const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "sgd_flat_cap");
-    const b2::FlatScalars* blk = flat_block(block, p, "sgd_flat_cap");
-    const float* gsc = amp_scalar_ptr(grad_scale, p, "sgd_flat_cap", "grad_scale");
-    const float* fi = amp_scalar_ptr(found_inf, p, "sgd_flat_cap", "found_inf");
-    TORCH_CHECK(fi != nullptr || gsc == nullptr, "sgd_flat_cap: grad_scale comes with found_inf (GradScaler sets both)");
-    c10::cuda::CUDAGuard guard(p.device());
-    ck_cuda(b2_sgd_flat_cap_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(), map, blk,
-                                   (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0, max_norm, sq, n_buckets, gn, gsc, fi, cur_stream()),
-            "sgd_flat_cap launch");
-  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("block"), py::arg("mu"), py::arg("zero_grad"),
-     py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
-  // adamw_flat / adamw_flat_grouped (with group_map) with the scalars from the block
-  m.def("adamw_flat_cap", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
-                             c10::optional<torch::Tensor> group_map, torch::Tensor block, bool zero_grad, py::object max_grad_norm,
-                             c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
-                             c10::optional<torch::Tensor> grad_scale, c10::optional<torch::Tensor> found_inf) {
-    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat_cap");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "adamw_flat_cap: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat_cap");
-    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
-      check_cuda_contig(*t, "adamw_flat_cap: p, exp_avg, exp_avg_sq and g");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "adamw_flat_cap: p, exp_avg, exp_avg_sq and g: 16-byte aligned fp32 of one size");
-    }
-    const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, "adamw_flat_cap");
-    const b2::FlatScalars* blk = flat_block(block, p, "adamw_flat_cap");
-    const float* gsc = amp_scalar_ptr(grad_scale, p, "adamw_flat_cap", "grad_scale");
-    const float* fi = amp_scalar_ptr(found_inf, p, "adamw_flat_cap", "found_inf");
-    TORCH_CHECK(fi != nullptr || gsc == nullptr, "adamw_flat_cap: grad_scale comes with found_inf (GradScaler sets both)");
-    c10::cuda::CUDAGuard guard(p.device());
-    ck_cuda(b2_adamw_flat_cap_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), g.data_ptr<float>(),
-                                     (size_t)p.numel(), map, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn, gsc, fi, cur_stream()),
-            "adamw_flat_cap launch");
-  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("block"),
-     py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none(), py::arg("found_inf") = py::none());
-  // sharded_sgd / sharded_sgd_grouped (with group_map: this rank's ids) with the scalars from the block
-  m.def("sharded_sgd_cap", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                              std::vector<unsigned long long> sigs, torch::Tensor momentum, c10::optional<torch::Tensor> group_map,
-                              torch::Tensor block, size_t n_vec, double mu, bool nesterov, double scale, bool zero_grad, int rank,
-                              int world, int max_blocks) {
-    check_world(rank, world, "sharded_sgd_cap");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_sgd_cap: one gradient bucket, one parameter flat and one signal pad per rank");
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd_cap: n_vec must be a multiple of world, got ", n_vec, " for ", world);
-    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd_cap: nesterov needs a nonzero momentum");
-    check_cuda_contig(momentum, "momentum");
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
-                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd_cap: momentum: 16-byte aligned fp32 of at least ", shard,
-                " elements (this rank's slice)");
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd_cap: null or misaligned per-rank pointer");
-    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), "sharded_sgd_cap");
-    const b2::FlatScalars* blk = flat_block(block, momentum, "sharded_sgd_cap");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
-    c10::cuda::CUDAGuard guard(momentum.device());
-    ck_cuda(b2_sharded_sgd_cap_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), map, blk, n_vec, (float)mu,
-                                      nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
-            "sharded_sgd_cap launch");
-  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("group_map"),
-     py::arg("block"), py::arg("n_vec"), py::arg("mu"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"),
-     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
-  // sharded_adamw / sharded_adamw_grouped (with group_map: this rank's ids) with the scalars from the block
-  m.def("sharded_adamw_cap", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                                std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
-                                c10::optional<torch::Tensor> group_map, torch::Tensor block, size_t n_vec, double scale,
-                                bool zero_grad, int rank, int world, int max_blocks) {
-    check_world(rank, world, "sharded_adamw_cap");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_adamw_cap: one gradient bucket, one parameter flat and one signal pad per rank");
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw_cap: n_vec must be a multiple of world, got ", n_vec, " for ", world);
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
-      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "sharded_adamw_cap: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements");
-    }
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw_cap: null or misaligned per-rank pointer");
-    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), "sharded_adamw_cap");
-    const b2::FlatScalars* blk = flat_block(block, exp_avg, "sharded_adamw_cap");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
-    c10::cuda::CUDAGuard guard(exp_avg.device());
-    ck_cuda(b2_sharded_adamw_cap_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), map, blk,
-                                        n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
-            "sharded_adamw_cap launch");
-  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
-     py::arg("group_map"), py::arg("block"), py::arg("n_vec"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
-     py::arg("world"), py::arg("max_blocks") = 0);
-  m.def("sgd_flat_grouped", [](torch::Tensor p, torch::Tensor mom, torch::Tensor g, torch::Tensor group_map, std::vector<double> lrs,
-                               std::vector<double> weight_decays, double mu, bool zero_grad, bool nesterov, py::object max_grad_norm,
-                               c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
-                               c10::optional<torch::Tensor> grad_scale) {
-    // sgd_flat with parameter groups (csrc/sgd.cu): parameter vector i takes lrs / weight_decays of group group_map[i]
-    TORCH_CHECK(!nesterov || mu != 0.0, "sgd_flat_grouped: nesterov needs a nonzero momentum");
-    for (double wd : weight_decays) TORCH_CHECK(wd >= 0.0, "sgd_flat_grouped: weight_decay must be >= 0, got ", wd);
-    const float max_norm = check_max_grad_norm(max_grad_norm, "sgd_flat_grouped");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "sgd_flat_grouped: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, "sgd_flat_grouped");
-    check_cuda_contig(p, "p"); check_cuda_contig(mom, "m"); check_cuda_contig(g, "g");
-    TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 && mom.scalar_type() == torch::kFloat32,
-                "sgd_flat_grouped: p, m and g: fp32");
-    TORCH_CHECK(p.numel() == g.numel() && p.numel() == mom.numel(), "sgd_flat_grouped: p, m and g: one size");
-    TORCH_CHECK(((uintptr_t)p.data_ptr() | (uintptr_t)mom.data_ptr() | (uintptr_t)g.data_ptr()) % 16 == 0,
-                "sgd_flat_grouped: 16-byte aligned buffers");
-    b2::SgdGroups gs;
-    memset(&gs, 0, sizeof(gs));
-    const int n_groups = check_groups(group_map, (p.numel() + 3) / 4, lrs, weight_decays, gs.lr, gs.wd, "sgd_flat_grouped");
-    c10::cuda::CUDAGuard guard(p.device());
-    ck_cuda(b2_sgd_flat_grouped_launch(p.data_ptr<float>(), mom.data_ptr<float>(), g.data_ptr<float>(), (size_t)p.numel(),
-                                       group_map.data_ptr<uint8_t>(), &gs, n_groups, (float)mu, zero_grad ? 1 : 0, nesterov ? 1 : 0,
-                                       max_norm, sq, n_buckets, gn, amp_scalar_ptr(grad_scale, p, "sgd_flat_grouped", "grad_scale"),
-                                       cur_stream()),
-            "sgd_flat_grouped launch");
-  }, py::arg("p"), py::arg("m"), py::arg("g"), py::arg("group_map"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"),
-     py::arg("zero_grad"), py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
-     py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
-  m.def("adamw_flat_grouped", [](torch::Tensor p, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor g,
-                                 torch::Tensor group_map, std::vector<double> scalars, std::vector<double> decays,
-                                 std::vector<double> step_sizes, bool zero_grad, py::object max_grad_norm,
-                                 c10::optional<torch::Tensor> sqnorms, c10::optional<torch::Tensor> grad_norm_out,
-                                 c10::optional<torch::Tensor> grad_scale) {
-    // adamw_flat with parameter groups (csrc/adamw.cu): `scalars` as adamw_flat's (their decay and step_size are not used),
-    // decays / step_sizes: 1 - lr_g*wd_g and lr_g / (1 - beta1^t) of every group, fp64, each rounded once to fp32 here
-    const b2::AdamwScalars sc = to_adamw(scalars, "adamw_flat_grouped");
-    const float max_norm = check_max_grad_norm(max_grad_norm, "adamw_flat_grouped");
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, "adamw_flat_grouped: max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, "adamw_flat_grouped");
-    for (const auto* t : {&p, &exp_avg, &exp_avg_sq, &g}) {
-      check_cuda_contig(*t, "adamw_flat_grouped: p, exp_avg, exp_avg_sq and g");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "adamw_flat_grouped: p, exp_avg, exp_avg_sq and g: 16-byte aligned fp32 of one size");
-    }
-    b2::AdamwGroups gs;
-    memset(&gs, 0, sizeof(gs));
-    const int n_groups = check_groups(group_map, (p.numel() + 3) / 4, decays, step_sizes, gs.decay, gs.step_size,
-                                      "adamw_flat_grouped");
-    c10::cuda::CUDAGuard guard(p.device());
-    ck_cuda(b2_adamw_flat_grouped_launch(p.data_ptr<float>(), exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
-                                         g.data_ptr<float>(), (size_t)p.numel(), group_map.data_ptr<uint8_t>(), &sc, &gs, n_groups,
-                                         zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
-                                         amp_scalar_ptr(grad_scale, p, "adamw_flat_grouped", "grad_scale"), cur_stream()),
-            "adamw_flat_grouped launch");
-  }, py::arg("p"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("g"), py::arg("group_map"), py::arg("scalars"),
-     py::arg("decays"), py::arg("step_sizes"), py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(),
-     py::arg("sqnorms") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
   // FlatRMSprop's update of one fp32 bucket (csrc/rmsprop.cu).  scalars (fp64, each rounded once to fp32): (lr, weight_decay,
   // alpha, 1 - alpha, eps, momentum); grad_avg with centered, momentum_buffer with momentum > 0.  With max_grad_norm, g is
   // first scaled by the clip coefficient of the norm of grad_sqnorm's per-bucket sums; with grad_scale, first unscaled.
@@ -1620,38 +1544,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          const c10::optional<torch::Tensor>& grad_norm_out, const c10::optional<torch::Tensor>& grad_scale,
                          const c10::optional<torch::Tensor>& found_inf) {
     const b2::RmspropScalars sc = to_rmsprop(scalars, centered, what);
-    const float max_norm = check_max_grad_norm(max_grad_norm, what);
-    const double* sq = nullptr;
-    int n_buckets = 0;
-    if (max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      sq = sqnorms->data_ptr<double>();
-      n_buckets = (int)sqnorms->numel();
-    }
-    float* gn = grad_norm_ptr(grad_norm_out, what);
-    for (const auto* t : {&p, &g}) {
-      check_cuda_contig(*t, what);
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == p.numel() && (uintptr_t)t->data_ptr() % 16 == 0, what,
-                  ": p and g: 16-byte aligned fp32 of one size");
-    }
-    const auto opt = rmsprop_state(square_avg, grad_avg, momentum_buffer, sc, p.numel(), false, p, what);
+    if (weight_decays != nullptr)
+      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
+    const Clip c = clip_args(max_grad_norm, sqnorms, grad_norm_out, what);
+    const auto [gsc, fi] = amp_pair(grad_scale, found_inf, block != nullptr, p, what);
+    const auto opt = rmsprop_state({&p, &g}, square_avg, grad_avg, momentum_buffer, sc, p.numel(), false,
+                                   "p, g, square_avg, grad_avg and momentum_buffer", what);
     const uint8_t* map = flat_map(group_map, (p.numel() + 3) / 4, what);
     b2::SgdGroups gs;
     memset(&gs, 0, sizeof(gs));
-    int n_groups = 0;
-    if (lrs != nullptr) {
-      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
-      n_groups = check_groups(*group_map, (p.numel() + 3) / 4, *lrs, *weight_decays, gs.lr, gs.wd, what);
-    }
+    const int n_groups = lrs != nullptr ? check_groups(*group_map, (p.numel() + 3) / 4, *lrs, *weight_decays, gs.lr, gs.wd, what) : 0;
     const b2::FlatScalars* blk = block != nullptr ? flat_block(*block, p, what) : nullptr;
-    const float* gsc = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
-    const float* fi = amp_scalar_ptr(found_inf, p, what, "found_inf");
-    TORCH_CHECK(blk == nullptr || fi != nullptr || gsc == nullptr, what, ": grad_scale comes with found_inf (GradScaler sets both)");
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_rmsprop_flat_launch(p.data_ptr<float>(), square_avg.data_ptr<float>(), opt.first, opt.second, g.data_ptr<float>(),
-                                   (size_t)p.numel(), map, &sc, &gs, n_groups, blk, zero_grad ? 1 : 0, max_norm, sq, n_buckets, gn,
-                                   gsc, fi, cur_stream()),
+                                   (size_t)p.numel(), map, &sc, &gs, n_groups, blk, zero_grad ? 1 : 0, c.max_norm, c.sq, c.n_buckets,
+                                   c.gn, gsc, fi, cur_stream()),
             what);
   };
   m.def("rmsprop_flat", [rmsprop_flat](torch::Tensor p, torch::Tensor square_avg, c10::optional<torch::Tensor> grad_avg,
@@ -1698,37 +1605,28 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                             const std::vector<double>* lrs, const std::vector<double>* weight_decays, const torch::Tensor* block,
                             size_t n_vec, const std::vector<double>& scalars, bool centered, double scale, bool zero_grad, int rank,
                             int world, int max_blocks) {
-    check_world(rank, world, what);
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world, what,
-                ": one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ", params.size(),
-                " and ", sigs.size(), " for world ", world);
-    TORCH_CHECK(n_vec % (size_t)world == 0, what, ": every rank owns n_vec / world vectors, so n_vec must be a multiple of world "
-                "(pad the buffers), got n_vec ", n_vec, " for world ", world);
+    const Peers pr = sharded_peers(what, grads, params, nullptr, sigs, n_vec, bf16, rank, world);
     const b2::RmspropScalars sc = to_rmsprop(scalars, centered, what);
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    const auto opt = rmsprop_state(square_avg, grad_avg, momentum_buffer, sc, (int64_t)shard, true, square_avg, what);
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, what, ": null or misaligned per-rank pointer");
-    const uint8_t* map = flat_map(group_map, (int64_t)(shard / 4), what);
+    if (weight_decays != nullptr)
+      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
+    const auto opt = rmsprop_state({}, square_avg, grad_avg, momentum_buffer, sc, pr.shard, true,
+                                   "square_avg, grad_avg and momentum_buffer (this rank's slice)", what);
+    const uint8_t* map = flat_map(group_map, pr.shard / 4, what);
     b2::SgdGroups gs;
     memset(&gs, 0, sizeof(gs));
-    int n_groups = 0;
-    if (lrs != nullptr) {
-      for (double wd : *weight_decays) TORCH_CHECK(wd >= 0.0, what, ": weight_decay must be >= 0, got ", wd);
-      n_groups = check_groups(*group_map, (int64_t)(shard / 4), *lrs, *weight_decays, gs.lr, gs.wd, what);
-    }
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
+    const int n_groups = lrs != nullptr ? check_groups(*group_map, pr.shard / 4, *lrs, *weight_decays, gs.lr, gs.wd, what) : 0;
     c10::cuda::CUDAGuard guard(square_avg.device());
     if (block != nullptr) {
       const b2::FlatScalars* blk = flat_block(*block, square_avg, what);
-      ck_cuda(b2_sharded_rmsprop_cap_launch(bf16 ? 1 : 0, &g, &p, &s, square_avg.data_ptr<float>(), opt.first, opt.second, map, blk,
-                                            &sc, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+      ck_cuda(b2_sharded_rmsprop_cap_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, square_avg.data_ptr<float>(), opt.first,
+                                            opt.second, map, blk, &sc, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks,
+                                            cur_stream()),
               what);
       return;
     }
-    ck_cuda(b2_sharded_rmsprop_launch(bf16 ? 1 : 0, &g, &p, &s, square_avg.data_ptr<float>(), opt.first, opt.second, map, &sc, &gs,
-                                      n_groups, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+    ck_cuda(b2_sharded_rmsprop_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, square_avg.data_ptr<float>(), opt.first,
+                                      opt.second, map, &sc, &gs, n_groups, n_vec, (float)scale, zero_grad ? 1 : 0, rank, world,
+                                      max_blocks, cur_stream()),
             what);
   };
   m.def("sharded_rmsprop", [sharded_rmsprop](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
@@ -1830,15 +1728,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                 "weight_decay), got ", scalars.size(), " values");
     for (double x : scalars) TORCH_CHECK(std::isfinite(x) && std::isfinite((float)x), "sharded_lamb: scalars must be finite in fp32");
     TORCH_CHECK((float)scalars[3] > 0.f && scalars[4] >= 0.0, "sharded_lamb: sqrt(bc2) must be > 0 (update t >= 1) and eps >= 0");
-    b2::LwArgs a = sharded_layerwise_args("sharded_lamb", true, bf16, grads, params, sums, sigs, {&exp_avg, &exp_avg_sq},
+    auto [a, pr] = sharded_layerwise_args("sharded_lamb", true, bf16, grads, params, sums, sigs, {&exp_avg, &exp_avg_sq},
                                           table, partials, tickets, ratios, n_vec, zero_grad, rank, world);
     a.w1 = (float)scalars[0]; a.beta2 = (float)scalars[1]; a.c2 = (float)scalars[2]; a.sbc2 = (float)scalars[3];
     a.eps = (float)scalars[4]; a.rbc1 = (float)scalars[5]; a.lr = (float)scalars[6]; a.wd = (float)scalars[7];
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params), sm = to_ptrs(sums);
-    SignalPadsH s = to_sig(sigs);
     c10::cuda::CUDAGuard guard(exp_avg.device());
-    ck_cuda(b2_sharded_layerwise_launch(1, bf16 ? 1 : 0, &g, &p, &sm, &s, &a, n_vec, (float)scale, rank, world, max_blocks,
-                                        cur_stream()), "sharded_lamb launch");
+    ck_cuda(b2_sharded_layerwise_launch(1, bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sums, &pr.sigs, &a, n_vec, (float)scale, rank,
+                                        world, max_blocks, cur_stream()), "sharded_lamb launch");
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sums"), py::arg("sigs"), py::arg("exp_avg"),
      py::arg("exp_avg_sq"), py::arg("table"), py::arg("partials"), py::arg("tickets"), py::arg("ratios"),
      py::arg("n_vec"), py::arg("scalars"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"),
@@ -1855,15 +1751,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(std::isfinite(lr) && std::isfinite(momentum) && std::isfinite(weight_decay) && trust_coefficient > 0.0 &&
                 std::isfinite(trust_coefficient) && eps >= 0.0 && std::isfinite(eps),
                 "sharded_lars: lr, momentum and weight_decay finite, trust_coefficient > 0 and eps >= 0 finite");
-    b2::LwArgs a = sharded_layerwise_args("sharded_lars", false, bf16, grads, params, sums, sigs, {&momentum_buf, &grad_workspace}, table,
-                                          partials, tickets, ratios, n_vec, zero_grad, rank, world);
+    auto [a, pr] = sharded_layerwise_args("sharded_lars", false, bf16, grads, params, sums, sigs, {&momentum_buf, &grad_workspace},
+                                          table, partials, tickets, ratios, n_vec, zero_grad, rank, world);
     a.lr = (float)lr; a.mu = (float)momentum; a.wd = (float)weight_decay; a.nesterov = nesterov ? 1 : 0;
     a.eta64 = trust_coefficient; a.wd64 = weight_decay; a.eps64 = eps;
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params), sm = to_ptrs(sums);
-    SignalPadsH s = to_sig(sigs);
     c10::cuda::CUDAGuard guard(momentum_buf.device());
-    ck_cuda(b2_sharded_layerwise_launch(0, bf16 ? 1 : 0, &g, &p, &sm, &s, &a, n_vec, (float)scale, rank, world, max_blocks,
-                                        cur_stream()), "sharded_lars launch");
+    ck_cuda(b2_sharded_layerwise_launch(0, bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sums, &pr.sigs, &a, n_vec, (float)scale, rank,
+                                        world, max_blocks, cur_stream()), "sharded_lars launch");
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sums"), py::arg("sigs"), py::arg("momentum_buffer"),
      py::arg("grad_workspace"), py::arg("table"), py::arg("partials"), py::arg("tickets"), py::arg("ratios"),
      py::arg("n_vec"), py::arg("lr"), py::arg("momentum"), py::arg("weight_decay"), py::arg("trust_coefficient"), py::arg("eps"),
@@ -1926,14 +1820,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       a.rho[i] = rho[i];
       a.decay[i] = (float)decay[i];
     }
-    a.max_norm = check_max_grad_norm(max_grad_norm, what);
-    if (a.max_norm > 0.f) {
-      TORCH_CHECK(sqnorms.has_value() && sqnorms->is_cuda() && sqnorms->is_contiguous() && sqnorms->scalar_type() == torch::kFloat64 &&
-                  sqnorms->numel() >= 1, what, ": max_grad_norm needs sqnorms, fp64 CUDA [buckets] from grad_sqnorm");
-      a.sqnorms = sqnorms->data_ptr<double>();
-      a.n_buckets = (int)sqnorms->numel();
-    }
-    a.grad_norm_out = grad_norm_ptr(grad_norm_out, what);
+    const Clip c = clip_args(max_grad_norm, sqnorms, grad_norm_out, what);
+    a.max_norm = c.max_norm; a.sqnorms = c.sq; a.n_buckets = c.n_buckets; a.grad_norm_out = c.gn;
     a.grad_scale = amp_scalar_ptr(grad_scale, p, what, "grad_scale");
     c10::cuda::CUDAGuard guard(p.device());
     ck_cuda(b2_adafactor_launch(&a, cur_stream()), "adafactor_flat launch");
@@ -1941,127 +1829,129 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("means"), py::arg("tickets"), py::arg("alpha"), py::arg("step"), py::arg("scalars"), py::arg("rho"), py::arg("decay"),
      py::arg("zero_grad"), py::arg("max_grad_norm") = py::none(), py::arg("sqnorms") = py::none(),
      py::arg("grad_norm_out") = py::none(), py::arg("grad_scale") = py::none());
-  // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instance): as sharded_sgd, with this rank's
-  // exp_avg / exp_avg_sq shards in place of the momentum shard.
-  m.def("sharded_adamw", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                            std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, size_t n_vec,
-                            std::vector<double> scalars, double scale, bool zero_grad, int rank, int world, int max_blocks) {
-    check_world(rank, world, "sharded_adamw");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_adamw: one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ",
-                params.size(), " and ", sigs.size(), " for world ", world);
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw: every rank owns n_vec / world vectors, so n_vec must be a multiple of "
-                "world (pad the buffers), got n_vec ", n_vec, " for world ", world);
-    const b2::AdamwScalars sc = to_adamw(scalars, "sharded_adamw");
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
-      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "sharded_adamw: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements (this rank's slice)");
-    }
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw: null or misaligned per-rank pointer");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
-    c10::cuda::CUDAGuard guard(exp_avg.device());
-    ck_cuda(b2_sharded_adamw_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(), n_vec, &sc,
-                                    (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
-            "sharded_adamw launch");
-  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
-     py::arg("n_vec"), py::arg("scalars"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"),
-     py::arg("max_blocks") = 0);
   // Sharded optimizer step of one bucket (csrc/sharded_sgd.cu): reduce-scatter of the gradient buckets `grads`, momentum SGD on
   // this rank's slice with its momentum shard, and the new parameters stored into every rank's flat in `params`.  n_vec counts
-  // the 16-byte vectors of one gradient bucket; raw per-rank pointers, like `allreduce`.
-  m.def("sharded_sgd", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                          std::vector<unsigned long long> sigs, torch::Tensor momentum, size_t n_vec, double lr, double mu,
-                          double wd, bool nesterov, double scale, bool zero_grad, int rank, int world, int max_blocks) {
-    check_world(rank, world, "sharded_sgd");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_sgd: one gradient bucket, one parameter flat and one signal pad per rank, got ", grads.size(), ", ",
-                params.size(), " and ", sigs.size(), " for world ", world);
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd: every rank owns n_vec / world vectors, so n_vec must be a multiple of "
-                "world (pad the buffers), got n_vec ", n_vec, " for world ", world);
-    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd: nesterov needs a nonzero momentum");
-    check_cuda_contig(momentum, "momentum");
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
-                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd: momentum: 16-byte aligned fp32 of at least ", shard,
-                " elements (this rank's slice)");
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd: null or misaligned per-rank pointer");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
+  // the 16-byte vectors of one gradient bucket; raw per-rank pointers, like `allreduce`.  sharded_sgd takes lr / weight_decay,
+  // sharded_sgd_grouped group_map (this rank's ids, one per fp32 parameter vector of its slice: n_vec / world x 1, x 2 with
+  // bf16) and the groups' lrs / weight_decays, sharded_sgd_cap the scalars from the block (with group_map, every group's).
+  auto sharded_sgd = [](const char* what, bool bf16, const std::vector<unsigned long long>& grads,
+                        const std::vector<unsigned long long>& params, const std::vector<unsigned long long>& sigs,
+                        torch::Tensor& momentum, const c10::optional<torch::Tensor>& group_map, const std::vector<double>& lrs,
+                        const std::vector<double>& weight_decays, const torch::Tensor* block, size_t n_vec, double mu, bool nesterov,
+                        double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    const Peers pr = sharded_peers(what, grads, params, nullptr, sigs, n_vec, bf16, rank, world);
+    // every group's weight decay (none: the capturable form's come from the block), checked through the smallest
+    check_sgd_options(weight_decays.empty() ? 0.0 : *std::min_element(weight_decays.begin(), weight_decays.end()), nesterov, mu,
+                      what);
+    check_flats({&momentum}, pr.shard, true, "momentum (this rank's slice)", what);
     c10::cuda::CUDAGuard guard(momentum.device());
-    ck_cuda(b2_sharded_sgd_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), n_vec, (float)lr, (float)mu, (float)wd,
-                                  nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
-            "sharded_sgd launch");
+    if (block != nullptr) {
+      ck_cuda(b2_sharded_sgd_cap_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, momentum.data_ptr<float>(),
+                                        flat_map(group_map, pr.shard / 4, what), flat_block(*block, momentum, what), n_vec, (float)mu,
+                                        nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+              what);
+    } else if (group_map.has_value()) {
+      b2::SgdGroups gs;
+      memset(&gs, 0, sizeof(gs));
+      const int n_groups = check_groups(*group_map, pr.shard / 4, lrs, weight_decays, gs.lr, gs.wd, what);
+      ck_cuda(b2_sharded_sgd_grouped_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, momentum.data_ptr<float>(),
+                                            group_map->data_ptr<uint8_t>(), &gs, n_groups, n_vec, (float)mu, nesterov ? 1 : 0,
+                                            (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+              what);
+    } else {
+      ck_cuda(b2_sharded_sgd_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, momentum.data_ptr<float>(), n_vec, (float)lrs[0],
+                                    (float)mu, (float)weight_decays[0], nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world,
+                                    max_blocks, cur_stream()),
+              what);
+    }
+  };
+  m.def("sharded_sgd", [sharded_sgd](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                     std::vector<unsigned long long> sigs, torch::Tensor momentum, size_t n_vec, double lr, double mu,
+                                     double wd, bool nesterov, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    sharded_sgd("sharded_sgd", bf16, grads, params, sigs, momentum, c10::nullopt, {lr}, {wd}, nullptr, n_vec, mu, nesterov, scale,
+                zero_grad, rank, world, max_blocks);
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("n_vec"), py::arg("lr"),
      py::arg("mu"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
      py::arg("world"), py::arg("max_blocks") = 0);
-  // sharded_sgd / sharded_adamw with parameter groups: group_map holds this rank's ids, one per fp32 parameter vector of its
-  // slice (n_vec / world x 1, x 2 with bf16)
-  m.def("sharded_sgd_grouped", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                                  std::vector<unsigned long long> sigs, torch::Tensor momentum, torch::Tensor group_map, size_t n_vec,
-                                  std::vector<double> lrs, std::vector<double> weight_decays, double mu, bool nesterov, double scale,
-                                  bool zero_grad, int rank, int world, int max_blocks) {
-    check_world(rank, world, "sharded_sgd_grouped");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_sgd_grouped: one gradient bucket, one parameter flat and one signal pad per rank");
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_sgd_grouped: n_vec must be a multiple of world, got ", n_vec, " for ", world);
-    TORCH_CHECK(!nesterov || mu != 0.0, "sharded_sgd_grouped: nesterov needs a nonzero momentum");
-    for (double wd : weight_decays) TORCH_CHECK(wd >= 0.0, "sharded_sgd_grouped: weight_decay must be >= 0, got ", wd);
-    check_cuda_contig(momentum, "momentum");
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    TORCH_CHECK(momentum.scalar_type() == torch::kFloat32 && (size_t)momentum.numel() >= shard &&
-                (uintptr_t)momentum.data_ptr() % 16 == 0, "sharded_sgd_grouped: momentum: 16-byte aligned fp32 of at least ", shard,
-                " elements (this rank's slice)");
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_sgd_grouped: null or misaligned per-rank pointer");
-    b2::SgdGroups gs;
-    memset(&gs, 0, sizeof(gs));
-    const int n_groups = check_groups(group_map, (int64_t)(shard / 4), lrs, weight_decays, gs.lr, gs.wd, "sharded_sgd_grouped");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
-    c10::cuda::CUDAGuard guard(momentum.device());
-    ck_cuda(b2_sharded_sgd_grouped_launch(bf16 ? 1 : 0, &g, &p, &s, momentum.data_ptr<float>(), group_map.data_ptr<uint8_t>(), &gs,
-                                          n_groups, n_vec, (float)mu, nesterov ? 1 : 0, (float)scale, zero_grad ? 1 : 0, rank, world,
-                                          max_blocks, cur_stream()),
-            "sharded_sgd_grouped launch");
+  m.def("sharded_sgd_grouped", [sharded_sgd](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                             std::vector<unsigned long long> sigs, torch::Tensor momentum, torch::Tensor group_map,
+                                             size_t n_vec, std::vector<double> lrs, std::vector<double> weight_decays, double mu,
+                                             bool nesterov, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    sharded_sgd("sharded_sgd_grouped", bf16, grads, params, sigs, momentum, group_map, lrs, weight_decays, nullptr, n_vec, mu, nesterov,
+                scale, zero_grad, rank, world, max_blocks);
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("group_map"),
      py::arg("n_vec"), py::arg("lrs"), py::arg("weight_decays"), py::arg("mu"), py::arg("nesterov"), py::arg("scale"),
      py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
-  m.def("sharded_adamw_grouped", [](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
-                                    std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
-                                    torch::Tensor group_map, size_t n_vec, std::vector<double> scalars, std::vector<double> decays,
-                                    std::vector<double> step_sizes, double scale, bool zero_grad, int rank, int world, int max_blocks) {
-    check_world(rank, world, "sharded_adamw_grouped");
-    TORCH_CHECK((int)grads.size() == world && (int)params.size() == world && (int)sigs.size() == world,
-                "sharded_adamw_grouped: one gradient bucket, one parameter flat and one signal pad per rank");
-    TORCH_CHECK(n_vec % (size_t)world == 0, "sharded_adamw_grouped: n_vec must be a multiple of world, got ", n_vec, " for ", world);
-    const b2::AdamwScalars sc = to_adamw(scalars, "sharded_adamw_grouped");
-    const size_t shard = n_vec / (size_t)world * (bf16 ? 8 : 4);
-    for (const auto* t : {&exp_avg, &exp_avg_sq}) {
-      check_cuda_contig(*t, "exp_avg / exp_avg_sq");
-      TORCH_CHECK(t->scalar_type() == torch::kFloat32 && (size_t)t->numel() >= shard && (uintptr_t)t->data_ptr() % 16 == 0,
-                  "sharded_adamw_grouped: exp_avg / exp_avg_sq: 16-byte aligned fp32 of at least ", shard, " elements");
-    }
-    for (const auto* v : {&grads, &params, &sigs})
-      for (unsigned long long q : *v) TORCH_CHECK(q != 0 && q % 16 == 0, "sharded_adamw_grouped: null or misaligned per-rank pointer");
-    b2::AdamwGroups gs;
-    memset(&gs, 0, sizeof(gs));
-    const int n_groups = check_groups(group_map, (int64_t)(shard / 4), decays, step_sizes, gs.decay, gs.step_size,
-                                      "sharded_adamw_grouped");
-    PeerPtrs g = to_ptrs(grads), p = to_ptrs(params);
-    SignalPadsH s = to_sig(sigs);
+  m.def("sharded_sgd_cap", [sharded_sgd](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                         std::vector<unsigned long long> sigs, torch::Tensor momentum,
+                                         c10::optional<torch::Tensor> group_map, torch::Tensor block, size_t n_vec, double mu,
+                                         bool nesterov, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    sharded_sgd("sharded_sgd_cap", bf16, grads, params, sigs, momentum, group_map, {}, {}, &block, n_vec, mu, nesterov, scale, zero_grad,
+                rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("momentum"), py::arg("group_map"),
+     py::arg("block"), py::arg("n_vec"), py::arg("mu"), py::arg("nesterov"), py::arg("scale"), py::arg("zero_grad"),
+     py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  // The sharded step of one bucket with AdamW (csrc/sharded_sgd.cu, the AdamW instances): as sharded_sgd, with this rank's
+  // exp_avg / exp_avg_sq shards in place of the momentum shard; group_map, decays / step_sizes and block as adamw_flat's.
+  auto sharded_adamw = [](const char* what, bool bf16, const std::vector<unsigned long long>& grads,
+                          const std::vector<unsigned long long>& params, const std::vector<unsigned long long>& sigs,
+                          torch::Tensor& exp_avg, torch::Tensor& exp_avg_sq, const c10::optional<torch::Tensor>& group_map,
+                          const std::vector<double>* scalars, const std::vector<double>& decays, const std::vector<double>& step_sizes,
+                          const torch::Tensor* block, size_t n_vec, double scale, bool zero_grad, int rank, int world, int max_blocks) {
+    const Peers pr = sharded_peers(what, grads, params, nullptr, sigs, n_vec, bf16, rank, world);
+    const b2::AdamwScalars sc = scalars != nullptr ? to_adamw(*scalars, what) : b2::AdamwScalars{};
+    check_flats({&exp_avg, &exp_avg_sq}, pr.shard, true, "exp_avg and exp_avg_sq (this rank's slice)", what);
     c10::cuda::CUDAGuard guard(exp_avg.device());
-    ck_cuda(b2_sharded_adamw_grouped_launch(bf16 ? 1 : 0, &g, &p, &s, exp_avg.data_ptr<float>(), exp_avg_sq.data_ptr<float>(),
-                                            group_map.data_ptr<uint8_t>(), &sc, &gs, n_groups, n_vec, (float)scale, zero_grad ? 1 : 0,
-                                            rank, world, max_blocks, cur_stream()),
-            "sharded_adamw_grouped launch");
+    if (block != nullptr) {
+      ck_cuda(b2_sharded_adamw_cap_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, exp_avg.data_ptr<float>(),
+                                          exp_avg_sq.data_ptr<float>(), flat_map(group_map, pr.shard / 4, what),
+                                          flat_block(*block, exp_avg, what), n_vec, (float)scale, zero_grad ? 1 : 0, rank, world,
+                                          max_blocks, cur_stream()),
+              what);
+    } else if (group_map.has_value()) {
+      b2::AdamwGroups gs;
+      memset(&gs, 0, sizeof(gs));
+      const int n_groups = check_groups(*group_map, pr.shard / 4, decays, step_sizes, gs.decay, gs.step_size, what);
+      ck_cuda(b2_sharded_adamw_grouped_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, exp_avg.data_ptr<float>(),
+                                              exp_avg_sq.data_ptr<float>(), group_map->data_ptr<uint8_t>(), &sc, &gs, n_groups, n_vec,
+                                              (float)scale, zero_grad ? 1 : 0, rank, world, max_blocks, cur_stream()),
+              what);
+    } else {
+      ck_cuda(b2_sharded_adamw_launch(bf16 ? 1 : 0, &pr.grads, &pr.params, &pr.sigs, exp_avg.data_ptr<float>(),
+                                      exp_avg_sq.data_ptr<float>(), n_vec, &sc, (float)scale, zero_grad ? 1 : 0, rank, world,
+                                      max_blocks, cur_stream()),
+              what);
+    }
+  };
+  m.def("sharded_adamw", [sharded_adamw](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                         std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
+                                         size_t n_vec, std::vector<double> scalars, double scale, bool zero_grad, int rank, int world,
+                                         int max_blocks) {
+    sharded_adamw("sharded_adamw", bf16, grads, params, sigs, exp_avg, exp_avg_sq, c10::nullopt, &scalars, {}, {}, nullptr, n_vec,
+                  scale, zero_grad, rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+     py::arg("n_vec"), py::arg("scalars"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"), py::arg("world"),
+     py::arg("max_blocks") = 0);
+  m.def("sharded_adamw_grouped", [sharded_adamw](bool bf16, std::vector<unsigned long long> grads,
+                                                 std::vector<unsigned long long> params, std::vector<unsigned long long> sigs,
+                                                 torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor group_map, size_t n_vec,
+                                                 std::vector<double> scalars, std::vector<double> decays,
+                                                 std::vector<double> step_sizes, double scale, bool zero_grad, int rank, int world,
+                                                 int max_blocks) {
+    sharded_adamw("sharded_adamw_grouped", bf16, grads, params, sigs, exp_avg, exp_avg_sq, group_map, &scalars, decays, step_sizes,
+                  nullptr, n_vec, scale, zero_grad, rank, world, max_blocks);
   }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
      py::arg("group_map"), py::arg("n_vec"), py::arg("scalars"), py::arg("decays"), py::arg("step_sizes"), py::arg("scale"),
      py::arg("zero_grad"), py::arg("rank"), py::arg("world"), py::arg("max_blocks") = 0);
+  m.def("sharded_adamw_cap", [sharded_adamw](bool bf16, std::vector<unsigned long long> grads, std::vector<unsigned long long> params,
+                                             std::vector<unsigned long long> sigs, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
+                                             c10::optional<torch::Tensor> group_map, torch::Tensor block, size_t n_vec, double scale,
+                                             bool zero_grad, int rank, int world, int max_blocks) {
+    sharded_adamw("sharded_adamw_cap", bf16, grads, params, sigs, exp_avg, exp_avg_sq, group_map, nullptr, {}, {}, &block, n_vec, scale,
+                  zero_grad, rank, world, max_blocks);
+  }, py::arg("bf16"), py::arg("grads"), py::arg("params"), py::arg("sigs"), py::arg("exp_avg"), py::arg("exp_avg_sq"),
+     py::arg("group_map"), py::arg("block"), py::arg("n_vec"), py::arg("scale"), py::arg("zero_grad"), py::arg("rank"),
+     py::arg("world"), py::arg("max_blocks") = 0);
 
   // ------------------------------------------------------------------ fused ConvNet step
   m.def("convnet_npar", [] { return b2_convnet_npar(); });

@@ -394,7 +394,7 @@ class _FlatOptimizer:
 
     def _hyper(self) -> tuple:
         """What the device table holds: every group's base lr and weight decay, the AdamW constants and the schedule."""
-        groups = self._group_list if self._grouped else [self._default_group]
+        groups = self._group_list
         b1, b2 = getattr(self, "betas", (0.0, 0.0))
         return ([float(g["lr"]) for g in groups], [float(g["weight_decay"]) for g in groups], float(b1), float(b2),
                 float(getattr(self, "eps", 0.0)), schedule_tuple(self.lr_schedule))
@@ -435,25 +435,22 @@ class _FlatOptimizer:
     # ------------------------------------------------------------------ parameter groups
     def _set_groups(self, given: Optional[list]) -> None:
         """The group layout of ``given`` (checked groups, or None: no groups).  ``_group_list`` holds the groups the updates
-        read -- the given ones in order, then the default group if any parameter is in none -- and per bucket ``_runs[k]``
-        cuts ``[0, numel)`` into ``(lo, hi, group)`` runs: each tensor's padded segment takes its tensor's group, and adjacent
-        segments of one group merge.  The kernel paths also get a uint8 group map with one id per fp32 parameter vector: the
-        whole bucket, or this rank's slice of the padded flat (padding in the last group)."""
+        read -- the given ones in order, then the default group if any parameter is in none; without ``given`` the default
+        group alone -- and per bucket ``_tensor_groups[k]`` the group of each tensor and ``_runs[k]`` cuts ``[0, numel)``
+        into ``(lo, hi, group)`` runs: each tensor's padded segment takes its tensor's group, and adjacent segments of one
+        group merge (without ``given``, one run ``(0, numel, 0)``).  With ``given``, the kernel paths also get a uint8 group
+        map with one id per fp32 parameter vector: the whole bucket, or this rank's slice of the padded flat (padding in the
+        last group)."""
         self._grouped = given is not None
-        self._group_list, self._runs, self._maps = None, [], []
-        laid = [p for gb in self.buckets for p in gb.params]
-        default = getattr(self, "_default_group", None)
-        if not self._grouped:
-            if default is not None:
-                default["params"] = laid
-            return
+        given = list(given or [])
+        self._runs, self._tensor_groups, self._maps = [], [], []
         gid = {}
         for i, g in enumerate(given):
             for p in g["params"]:
                 gid[id(p)] = i
-        rest = [p for p in laid if id(p) not in gid]
-        default["params"] = rest
-        self._group_list = list(given) + ([default] if rest else [])
+        rest = [p for gb in self.buckets for p in gb.params if id(p) not in gid]
+        self._default_group["params"] = rest
+        self._group_list = given + ([self._default_group] if rest else [])
         for p in rest:
             gid[id(p)] = len(given)
         n_groups = len(self._group_list)
@@ -466,6 +463,9 @@ class _FlatOptimizer:
                 else:
                     runs.append([lo, hi, gid[id(p)]])
             self._runs.append([tuple(r) for r in runs])
+            self._tensor_groups.append([gid[id(p)] for p in gb.params])
+            if not self._grouped:
+                continue
             if self._shard_mode == "kernel":
                 n_pad, per = self._shards[k][1], self._shards[k][2]
                 whole = self._group_map(runs + [[gb.numel, n_pad, n_groups - 1]], n_pad // 4, n_groups)
@@ -501,13 +501,33 @@ class _FlatOptimizer:
                 out.append((a - lo, b - lo, g))
         return out
 
+    def _run_views(self, runs: list, flats: list):
+        """Per group in group order, as torch's optimizers step their groups: ``(lr, weight_decay, views)``, ``views[j]`` the
+        group's ``(lo, hi, group)`` runs of ``flats[j]`` (``[]`` for a ``None`` flat)."""
+        for gi, (lr, wd) in enumerate(self._group_values()):
+            mine = [(lo, hi) for lo, hi, g in runs if g == gi]
+            if mine:
+                yield lr, wd, [[f[lo:hi] for lo, hi in mine] if f is not None else [] for f in flats]
+
+    def _tensor_views(self, k: int, flats: list, nonempty: bool = False):
+        """Per group in group order: ``(lr, weight_decay, idx, views)``, ``idx`` the group's tensors of bucket ``k``
+        (``nonempty``: those with an element) and ``views[j]`` their views of ``flats[j]`` (``[]`` for a ``None`` flat), each
+        with its tensor's own shape and strides, as torch's optimizers see the tensors."""
+        gb = self.buckets[k]
+        views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
+                 if f is not None else None for f in flats]
+        for gi, (lr, wd) in enumerate(self._group_values()):
+            idx = [i for i, x in enumerate(self._tensor_groups[k]) if x == gi and (gb.params[i].numel() > 0 or not nonempty)]
+            if idx:
+                yield lr, wd, idx, [[vs[i] for i in idx] if vs is not None else [] for vs in views]
+
     @property
     def param_groups(self) -> list:
         """The parameter groups, as torch's optimizers list them: the ``param_groups`` given to the constructor in order,
         then the default group of the parameters named in none (``lr`` / ``weight_decay`` are the optimizer's ``lr`` /
         ``weight_decay``).  Each is a dict with ``"params"``, ``"lr"`` and ``"weight_decay"``; every update reads the values,
         so assigning to them works as in torch.  Without ``param_groups`` it is the one default group."""
-        return list(self._group_list) if self._grouped else [self._default_group]
+        return list(self._group_list)
 
     def _group_state(self) -> dict:
         """What a state_dict records of the groups: ``{"param_groups": [{"params": [names], "lr", "weight_decay"}]}``."""
@@ -868,34 +888,21 @@ class FlatSGD(_FlatOptimizer):
             p.add_(gf.add(m, alpha=self.momentum) if self.nesterov else m, alpha=-lr)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
-        if self._grouped:
-            vals = self._group_values()
-            for k, (gb, pf, mf, kern) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats, kernel)):
-                g = gb.flat[:gb.numel]
-                if kern:
-                    self._kernel().sgd_flat_grouped(pf, mf, g, self._maps[k], [v[0] for v in vals], [v[1] for v in vals],
-                                                    self.momentum, self.fused_zero, self.nesterov, **clip)
-                    continue
+        vals = self._group_values()
+        for k, (gb, pf, mf, kern) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats, kernel)):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern and self._grouped:
+                self._kernel().sgd_flat_grouped(pf, mf, g, self._maps[k], [v[0] for v in vals], [v[1] for v in vals],
+                                                self.momentum, self.fused_zero, self.nesterov, **clip)
+            elif kern:
+                lr, wd = vals[0]
+                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, wd, self.fused_zero, self.nesterov, **clip)
+            else:
+                # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
+                # torch.optim.SGD's order (foreach=False)
                 self._sgd_runs(self._runs[k], pf, mf, _fp32_grad(g, clip.get("grad_scale")))
                 if self.fused_zero:
                     g.zero_()
-            return
-        lr = self.lr_at()
-        for gb, pf, mf, kern in zip(self.buckets, self.param_flats, self.momentum_flats, kernel):
-            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
-            if kern:
-                self._kernel().sgd_flat(pf, mf, g, lr, self.momentum, self.weight_decay, self.fused_zero, self.nesterov,
-                                        **clip)
-                continue
-            # CPU ranks (gloo) and reduced-precision gradient buckets: the same flat update with tensor ops, in
-            # torch.optim.SGD's order (foreach=False)
-            gf = _fp32_grad(g, clip.get("grad_scale"))
-            if self.weight_decay:
-                gf = gf.add(pf, alpha=self.weight_decay)
-            mf.mul_(self.momentum).add_(gf)
-            pf.add_(gf.add(mf, alpha=self.momentum) if self.nesterov else mf, alpha=-lr)
-            if self.fused_zero:
-                g.zero_()
 
     def _update_capturable(self, clip: dict) -> None:
         for k, (gb, pf, mf) in enumerate(zip(self.buckets, self.param_flats, self.momentum_flats)):
@@ -921,17 +928,8 @@ class FlatSGD(_FlatOptimizer):
                                    max_blocks)
 
     def _update_slice(self, k: int, lo: int, n: int) -> None:
-        if self._grouped:
-            self._sgd_runs(self._slice_runs(k, lo, n), self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n],
-                           self.buckets[k].flat[lo:lo + n])
-            return
-        lr = self.lr_at()
-        pv, mv = self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n]
-        gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
-        if self.weight_decay:
-            gf = gf.add(pv, alpha=self.weight_decay)
-        mv.mul_(self.momentum).add_(gf)
-        pv.add_(gf.add(mv, alpha=self.momentum) if self.nesterov else mv, alpha=-lr)
+        self._sgd_runs(self._slice_runs(k, lo, n), self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n],
+                       self.buckets[k].flat[lo:lo + n])
 
     def _full_momentum(self, k: int) -> torch.Tensor:
         """Bucket ``k``'s whole momentum flat; collective in sharded mode (gathers the shards)."""
@@ -1062,59 +1060,29 @@ class FlatAdamW(_FlatOptimizer):
         per = [adamw_scalars(lr, self.betas, self.eps, wd, self.steps + 1) for lr, wd in self._group_values()]
         return self.scalars(), [s[0] for s in per], [s[4] for s in per]
 
-    def _torch_adamw(self, p: list, g: list, m: list, v: list, lr: Optional[float] = None,
-                     weight_decay: Optional[float] = None) -> None:
-        """torch's single-tensor AdamW on the given views (update t = steps + 1), with the optimizer's lr and weight decay
-        unless a group's are given."""
+    def _torch_adamw(self, p: list, g: list, m: list, v: list, lr: float, weight_decay: float) -> None:
+        """torch's single-tensor AdamW on the given views (update t = steps + 1) with one group's lr and weight decay."""
         from torch.optim.adamw import adamw
 
         steps = [torch.tensor(float(self.steps)) for _ in p]
         adamw(p, g, m, v, [], steps, foreach=False, capturable=False, differentiable=False, fused=None, amsgrad=False,
-              beta1=self.betas[0], beta2=self.betas[1], lr=self.lr_at() if lr is None else lr,
-              weight_decay=self.weight_decay if weight_decay is None else weight_decay, eps=self.eps, maximize=False)
-
-    def _adamw_runs(self, runs: list, flats: list) -> None:
-        """torch's AdamW once per group (as torch.optim.AdamW steps its groups), on the group's ``(lo, hi, group)`` runs of the
-        views ``flats`` = [p, g (fp32), m, v]."""
-        vals = self._group_values()
-        for gi, (lr, wd) in enumerate(vals):
-            mine = [(lo, hi) for lo, hi, g in runs if g == gi]
-            if mine:
-                self._torch_adamw(*[[f[lo:hi] for lo, hi in mine] for f in flats], lr=lr, weight_decay=wd)
+              beta1=self.betas[0], beta2=self.betas[1], lr=lr, weight_decay=weight_decay, eps=self.eps, maximize=False)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
-        if self._grouped:
-            sc = self.group_scalars() if any(kernel) else None
-            for k, (gb, pf, mf, vf, kern) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats,
-                                                            self.exp_avg_sq_flats, kernel)):
-                g = gb.flat[:gb.numel]
-                if kern:
-                    self._kernel().adamw_flat_grouped(pf, mf, vf, g, self._maps[k], *sc, self.fused_zero, **clip)
-                    continue
+        sc = (self.group_scalars() if self._grouped else self.scalars()) if any(kernel) else None
+        for k, (gb, pf, mf, vf, kern) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats,
+                                                        self.exp_avg_sq_flats, kernel)):
+            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
+            if kern and self._grouped:
+                self._kernel().adamw_flat_grouped(pf, mf, vf, g, self._maps[k], *sc, self.fused_zero, **clip)
+            elif kern:
+                self._kernel().adamw_flat(pf, mf, vf, g, sc, self.fused_zero, **clip)
+            else:
                 gf = _fp32_grad(g, clip.get("grad_scale"))
-                # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.AdamW sees it
-                views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
-                         for f in (pf, gf, mf, vf)]
-                gid = [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
-                for gi, (lr, wd) in enumerate(self._group_values()):
-                    idx = [i for i, x in enumerate(gid) if x == gi]
-                    if idx:
-                        self._torch_adamw(*[[vs[i] for i in idx] for vs in views], lr=lr, weight_decay=wd)
+                for lr, wd, _, views in self._tensor_views(k, [pf, gf, mf, vf]):
+                    self._torch_adamw(*views, lr=lr, weight_decay=wd)
                 if self.fused_zero:
                     g.zero_()
-            return
-        sc = self.scalars() if any(kernel) else None
-        for gb, pf, mf, vf, kern in zip(self.buckets, self.param_flats, self.exp_avg_flats, self.exp_avg_sq_flats, kernel):
-            g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
-            if kern:
-                self._kernel().adamw_flat(pf, mf, vf, g, sc, self.fused_zero, **clip)
-                continue
-            gf = _fp32_grad(g, clip.get("grad_scale"))
-            views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
-                     for f in (pf, gf, mf, vf)]
-            self._torch_adamw(*views)
-            if self.fused_zero:
-                g.zero_()
 
     def _update_capturable(self, clip: dict) -> None:
         for k, (gb, pf, mf, vf) in enumerate(zip(self.buckets, self.param_flats, self.exp_avg_flats, self.exp_avg_sq_flats)):
@@ -1140,11 +1108,9 @@ class FlatAdamW(_FlatOptimizer):
 
     def _update_slice(self, k: int, lo: int, n: int) -> None:
         gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
-        if self._grouped:
-            self._adamw_runs(self._slice_runs(k, lo, n), [self._shards[k][3][lo:lo + n], gf, self.exp_avg_flats[k][:n],
-                                                          self.exp_avg_sq_flats[k][:n]])
-            return
-        self._torch_adamw([self._shards[k][3][lo:lo + n]], [gf], [self.exp_avg_flats[k][:n]], [self.exp_avg_sq_flats[k][:n]])
+        flats = [self._shards[k][3][lo:lo + n], gf, self.exp_avg_flats[k][:n], self.exp_avg_sq_flats[k][:n]]
+        for lr, wd, views in self._run_views(self._slice_runs(k, lo, n), flats):
+            self._torch_adamw(*views, lr=lr, weight_decay=wd)
 
     # ------------------------------------------------------------------ checkpointing
     def state_dict(self) -> dict:
@@ -1266,57 +1232,30 @@ class FlatRMSprop(_FlatOptimizer):
         return (self.square_avg_flats[k], self.grad_avg_flats[k] if self.centered else None,
                 self.momentum_buffer_flats[k] if self.momentum > 0 else None)
 
-    def _torch_rmsprop(self, p: list, g: list, sq: list, ga: list, buf: list, lr: Optional[float] = None,
-                       weight_decay: Optional[float] = None) -> None:
-        """torch's single-tensor RMSprop on the given views, with the optimizer's lr and weight decay unless a group's are
-        given."""
+    def _torch_rmsprop(self, p: list, g: list, sq: list, ga: list, buf: list, lr: float, weight_decay: float) -> None:
+        """torch's single-tensor RMSprop on the given views with one group's lr and weight decay."""
         from torch.optim.rmsprop import rmsprop
 
         steps = [torch.tensor(float(self.steps)) for _ in p]
-        rmsprop(p, g, sq, ga, buf, steps, foreach=False, maximize=False, differentiable=False, capturable=False,
-                lr=self.lr_at() if lr is None else lr, alpha=self.alpha, eps=self.eps,
-                weight_decay=self.weight_decay if weight_decay is None else weight_decay, momentum=self.momentum,
-                centered=self.centered)
-
-    def _torch_runs(self, runs: list, flats: list) -> None:
-        """torch's RMSprop once per group on the ``(lo, hi, group)`` runs of the views ``flats`` = [p, g (fp32), states...]
-        (absent states None), or once on the whole views without groups."""
-        if not self._grouped:
-            self._torch_rmsprop(*[[f] if f is not None else [] for f in flats])
-            return
-        for gi, (lr, wd) in enumerate(self._group_values()):
-            mine = [(lo, hi) for lo, hi, g in runs if g == gi]
-            if mine:
-                self._torch_rmsprop(*[[f[lo:hi] for lo, hi in mine] if f is not None else [] for f in flats], lr=lr, weight_decay=wd)
+        rmsprop(p, g, sq, ga, buf, steps, foreach=False, maximize=False, differentiable=False, capturable=False, lr=lr,
+                alpha=self.alpha, eps=self.eps, weight_decay=weight_decay, momentum=self.momentum, centered=self.centered)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
         sc = self.scalars() if any(kernel) else None
         vals = self._group_values() if self._grouped else None
         for k, (gb, pf, kern) in enumerate(zip(self.buckets, self.param_flats, kernel)):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
-            if kern:
-                if self._grouped:
-                    self._kernel().rmsprop_flat_grouped(pf, *self._states(k), g, self._maps[k], sc, self.centered,
-                                                        [v[0] for v in vals], [v[1] for v in vals], self.fused_zero, **clip)
-                else:
-                    self._kernel().rmsprop_flat(pf, *self._states(k), g, sc, self.centered, self.fused_zero, **clip)
-                continue
-            gf = _fp32_grad(g, clip.get("grad_scale"))
-            # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.RMSprop sees it
-            flats = (pf, gf) + self._states(k)
-            views = [[f[o:o + p.numel()].as_strided(gv.shape, gv.stride()) for p, o, gv in zip(gb.params, gb.offsets, gb.views)]
-                     if f is not None else None for f in flats]
-            if not self._grouped:
-                self._torch_rmsprop(*[v if v is not None else [] for v in views])
+            if kern and self._grouped:
+                self._kernel().rmsprop_flat_grouped(pf, *self._states(k), g, self._maps[k], sc, self.centered,
+                                                    [v[0] for v in vals], [v[1] for v in vals], self.fused_zero, **clip)
+            elif kern:
+                self._kernel().rmsprop_flat(pf, *self._states(k), g, sc, self.centered, self.fused_zero, **clip)
             else:
-                gid = [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
-                for gi, (lr, wd) in enumerate(vals):
-                    idx = [i for i, x in enumerate(gid) if x == gi]
-                    if idx:
-                        self._torch_rmsprop(*[[vs[i] for i in idx] if vs is not None else [] for vs in views], lr=lr,
-                                            weight_decay=wd)
-            if self.fused_zero:
-                g.zero_()
+                gf = _fp32_grad(g, clip.get("grad_scale"))
+                for lr, wd, _, views in self._tensor_views(k, [pf, gf, *self._states(k)]):
+                    self._torch_rmsprop(*views, lr=lr, weight_decay=wd)
+                if self.fused_zero:
+                    g.zero_()
 
     def _update_capturable(self, clip: dict) -> None:
         sc = self.scalars(lr=self.lr)    # lr and weight decay come from the device block; reading steps would synchronise
@@ -1342,7 +1281,8 @@ class FlatRMSprop(_FlatOptimizer):
     def _update_slice(self, k: int, lo: int, n: int) -> None:
         gf = self.buckets[k].flat[lo:lo + n].to(torch.float32)
         states = [f[:n] if f is not None else None for f in self._states(k)]
-        self._torch_runs(self._slice_runs(k, lo, n) if self._grouped else None, [self._shards[k][3][lo:lo + n], gf] + states)
+        for lr, wd, views in self._run_views(self._slice_runs(k, lo, n), [self._shards[k][3][lo:lo + n], gf] + states):
+            self._torch_rmsprop(*views, lr=lr, weight_decay=wd)
 
     # ------------------------------------------------------------------ checkpointing
     def _state_pairs(self) -> list:
@@ -1498,10 +1438,10 @@ class FlatAdafactor(_FlatOptimizer):
             if not (pf.is_cuda and gb.flat.dtype == torch.float32):
                 self._af.append(None)
                 continue
-            n_groups = len(self._group_list) if self._grouped else 1
             table, n_chunks, n_rc, n_means = self._kernel().adafactor_table(
                 list(gb.offsets), [list(gv.shape) for gv in gb.views], [list(gv.stride()) for gv in gb.views],
-                self._state_offsets[k], self._tensor_groups(k), gb.numel, self.state_flats[k].numel(), n_groups, pf.device)
+                self._state_offsets[k], self._tensor_groups[k], gb.numel, self.state_flats[k].numel(), len(self._group_list),
+                pf.device)
             n_t, dev = len(gb.params), pf.device
             self._af.append(dict(table=table, n_chunks=n_chunks,
                                  partials=torch.zeros(2 * n_chunks, dtype=torch.float32, device=dev),
@@ -1511,22 +1451,11 @@ class FlatAdafactor(_FlatOptimizer):
                                  alpha=torch.zeros(n_t, dtype=torch.float64, device=dev),
                                  step=torch.zeros(n_t, dtype=torch.float32, device=dev)))
 
-    def _tensor_groups(self, k: int) -> List[int]:
-        """The group of every tensor of bucket ``k`` (all 0 without ``param_groups``)."""
-        gb = self.buckets[k]
-        if not self._grouped:
-            return [0] * len(gb.params)
-        return [next(gi for lo, hi, gi in self._runs[k] if lo <= o < hi) for o in gb.offsets]
-
-    def _values(self) -> list:
-        """``(lr, weight_decay)`` of every group for the next update (the one default group without ``param_groups``)."""
-        return self._group_values() if self._grouped else [(self.lr_at(), float(self.weight_decay))]
-
     def scalars(self) -> tuple:
         """What ``adafactor_flat`` takes for the next update (t = ``steps + 1``), in fp64: ``([t ** beta2_decay, eps1, eps2,
         d], [rho_t per group], [1 - lr * weight_decay per group])``."""
         t = float(self.steps + 1)
-        vals = self._values()
+        vals = self._group_values()
         return ([t ** self.beta2_decay, self.eps1, self.eps2, self.d], [min(lr, 1 / (t ** 0.5)) for lr, _ in vals],
                 [1 - lr * wd for lr, wd in vals])
 
@@ -1550,7 +1479,6 @@ class FlatAdafactor(_FlatOptimizer):
                   weight_decay=weight_decay, eps1=self.eps[0], eps2=self.eps2, maximize=False)
 
     def _update(self, kernel: List[bool], clip: dict) -> None:
-        vals = self._values()
         sc = self.scalars() if any(kernel) else None
         for k, (gb, pf, sf, kern) in enumerate(zip(self.buckets, self.param_flats, self.state_flats, kernel)):
             g = gb.flat[:gb.numel]       # a symmetric-memory bucket is padded beyond the laid-out elements
@@ -1560,15 +1488,8 @@ class FlatAdafactor(_FlatOptimizer):
                                               w["tickets"], w["alpha"], w["step"], *sc, self.fused_zero, **clip)
                 continue
             gf = _fp32_grad(g, clip.get("grad_scale"))
-            # per tensor, so that every view has the tensor's own shape and strides, as torch.optim.Adafactor sees it
-            gid = self._tensor_groups(k)
-            for gi, (lr, wd) in enumerate(vals):
-                idx = [i for i, x in enumerate(gid) if x == gi and gb.params[i].numel() > 0]
-                if idx:
-                    views = [(pf[o:o + p.numel()].as_strided(gv.shape, gv.stride()),
-                              gf[o:o + p.numel()].as_strided(gv.shape, gv.stride()), self._state_views(k, sf, i))
-                             for i, (p, o, gv) in enumerate(zip(gb.params, gb.offsets, gb.views)) if i in idx]
-                    self._torch_adafactor([v[0] for v in views], [v[1] for v in views], [v[2] for v in views], lr, wd)
+            for lr, wd, idx, (pv, gv) in self._tensor_views(k, [pf, gf], nonempty=True):
+                self._torch_adafactor(pv, gv, [self._state_views(k, sf, i) for i in idx], lr, wd)
             if self.fused_zero:
                 g.zero_()
 

@@ -233,11 +233,13 @@ def test_one_launch_per_update(capturable):
         _step(ddp, opt, i)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            # once another process has used the GPU, each session loses its first kernel record: a throwaway kernel
-            # takes that place
-            torch.ones(1, device=DEV).add_(1)
+            # once another process has used the GPU, a session loses kernel records at its start, and the profiler keeps
+            # only the device activity inside its window: ~10 ms sleep kernels keep the update well inside it
+            torch.cuda._sleep(20_000_000)
             torch.cuda.synchronize()
             ema.update()
+            torch.cuda.synchronize()
+            torch.cuda._sleep(20_000_000)
             torch.cuda.synchronize()
         kernels = [(e.key, e.count) for e in prof.key_averages()]
         n = sum(c for k, c in kernels if "ema_kernel" in k)

@@ -67,16 +67,22 @@ def test_each_call_launches_the_kernel_the_table_expects(C, table):
     dev = torch.device("cuda", 0)
     ops = [G.int_operands(c, _seed(c), dev) for c in table if c.M * c.K < (1 << 26)]   # the large ones: made in the loop
     torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        # once another process has used the GPU, each profiler session loses its first kernel record: a throwaway
-        # kernel takes that place, so that every GEMM launch is recorded
+    with profile(activities=[ProfilerActivity.CUDA]):       # a first session starts the profiler before anything is counted
         torch.ones(1, device=dev).add_(1)
+        torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        # Once another process has used the GPU, a session loses kernel records at its start, and the profiler keeps
+        # only the device activity inside its window.  ~10 ms sleep kernels before and after the GEMM launches keep
+        # every one of them well inside the window, so that each is recorded.
+        torch.cuda._sleep(20_000_000)
         torch.cuda.synchronize()
         small = iter(ops)
         for c in table:
             A, B, bias = next(small) if c.M * c.K < (1 << 26) else G.int_operands(c, _seed(c), dev)
             C.gemm_bf16(A, B, bias, c.relu, c.out_bf16)
             torch.cuda.synchronize()
+        torch.cuda._sleep(20_000_000)
+        torch.cuda.synchronize()
     pat = re.compile(r"gemm_bf16_kernel<\d+>|gemm_bf16_persistent_kernel")
     ran = [(e.time_range.start, pat.search(e.name).group(0)) for e in prof.events()
            if e.device_type == DeviceType.CUDA and pat.search(e.name)]
