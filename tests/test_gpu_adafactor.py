@@ -10,6 +10,7 @@ import torch
 
 import adafactor_model as M
 from adamw_model import clip_coef
+from emulated_ranks import C  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -24,12 +25,6 @@ LAYOUTS = {
     "tall": [((1 << 20, 1), None), ((5,), None)],
     "wide": [((1, 1 << 20), None), ((40000, 3), None)],
 }
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
 
 
 def _stride(shape, fmt):

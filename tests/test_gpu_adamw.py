@@ -1,9 +1,8 @@
 """FlatAdamW's kernels on one GPU: ``adamw_flat`` (csrc/adamw.cu) and the AdamW instance of the sharded kernel
 (csrc/sharded_sgd.cu) bit for bit against tests/adamw_model.py, the kernel against ``torch.optim.AdamW`` on CUDA and fp64,
-the sharded kernel at emulated worlds 1-8 (the harness of tests/test_gpu_sharded_sgd_emulated.py), and a ResNet-18 trained
+the sharded kernel at emulated worlds 1-8 (the harness of tests/emulated_ranks.py), and a ResNet-18 trained
 through ``DistributedDataParallel`` + ``FlatAdamW`` under bf16 autocast."""
 import math
-import os
 
 import pytest
 import torch
@@ -12,7 +11,7 @@ import torch.nn.functional as F
 import adamw_model as A
 import comm_model as M
 import sharded_sgd_model as S
-from test_gpu_sharded_sgd_emulated import World, _untouched, _with_sentinel
+from emulated_ranks import CO_RESIDENT, C, World, _bits, _untouched, _with_sentinel, sms  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -20,23 +19,8 @@ HP = dict(lr=0.01, betas=(0.8, 0.95), eps=1e-6, wd=0.1)
 SIZES = [1, 2, 3, 4, 5, 6, 7, 1023, 1024, 1025, 1026, 1027, 256 * 4 * 7 + 3, 1 << 20, (1 << 20) + 1, 3 * 1000003]
 
 
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _sc(t, hp=HP):
     return A.scalars64(hp["lr"], hp["betas"], hp["eps"], hp["wd"], t)
-
-
-def _bits(a, b):
-    return torch.equal(a.cpu().view(torch.int32), b.cpu().view(torch.int32))
 
 
 def _state(n, seed):
@@ -187,14 +171,14 @@ def _cases(world, sms):
     return out
 
 
-@pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1", reason="serialized launches: the ranks' grids must be co-resident")
+@CO_RESIDENT
 @pytest.mark.parametrize("world", range(1, 9))
 def test_sharded_adamw_matches_the_model_bit_for_bit(C, sms, world):
     for k, (n_vec, mb, wire, zero_grad) in enumerate(_cases(world, sms)):
         run_sharded(C, World(world, sms), n_vec, mb, wire, zero_grad, seed=100 * world + k)
 
 
-@pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1", reason="serialized launches: the ranks' grids must be co-resident")
+@CO_RESIDENT
 @pytest.mark.parametrize("world", range(1, 9))
 def test_sharded_adamw_fp32_equals_allreduce_then_adamw_flat(C, sms, world):
     big = (524288 + world - 1) // world * world
@@ -202,7 +186,7 @@ def test_sharded_adamw_fp32_equals_allreduce_then_adamw_flat(C, sms, world):
         run_sharded(C, World(world, sms), n_vec, mb, torch.float32, k % 2 == 0, seed=50 * world + k, against_kernels=True)
 
 
-@pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1", reason="serialized launches: the ranks' grids must be co-resident")
+@CO_RESIDENT
 @pytest.mark.parametrize("world", [1, 3, 8])
 def test_sharded_adamw_epochs_wrap_through_zero(C, sms, world):
     W = World(world, sms, pad_start=2 ** 32 - 5)

@@ -1,7 +1,7 @@
 """The all-to-all with variable segments (csrc/allreduce.cu alltoallv_kernel) on ONE GPU with W emulated ranks, bit for bit
 against tests/all_to_all_v_model.py.
 
-The harness is tests/test_gpu_comm_emulated.py's: each rank has its own staging buffer, signal pad and stream, the W launches
+The harness is tests/emulated_ranks.py's: each rank has its own staging buffer, signal pad and stream, the W launches
 go out back to back, and no case runs more CTAs than the GPU has SMs.  Every segment of every input and output sits between
 random sentinel bytes; whole output buffers are compared with the model, every input buffer is checked unchanged, and the
 per-block epochs must advance by the model's barrier count on every rank.  One staging buffer per rank serves all calls of a
@@ -15,14 +15,10 @@ import all_to_all_v_model as AM
 import all_to_all_v_workers as AW
 import collectives_model as CM
 import comm_model as M
-import test_gpu_collectives_emulated as G
-import test_gpu_comm_emulated as E
-import test_gpu_reduce_scatter_alltoall_emulated as RSA
-import test_gpu_scatter_gather_emulated as SGE
+import emulated_ranks as E
+import reduce_scatter_alltoall_model as RS
+from emulated_ranks import C, _bytes, _unaligned, pytestmark, sms  # noqa: F401
 
-pytestmark = E.pytestmark
-C = E.C
-sms = E.sms
 GAP = 32                                         # sentinel bytes at least between two segments
 
 
@@ -200,19 +196,19 @@ def test_alltoallv_shares_pads_and_inboxes_with_every_kind_through_the_epoch_wra
             a2av_call(C, W, A, lens, lens, es, _mis(es, k), _mis(es, k + 2), mb, seed)
         elif call[0] == "rs":
             _, variant, dtype, op, seg_vec, mb, mode = call
-            RSA.reduce_scatter_call(C, W, variant, dtype, op, seg_vec, mb, mode, seed)
+            E.reduce_scatter_call(C, W, variant, dtype, op, seg_vec, mb, mode, seed)
         elif call[0] == "a2a":
             _, variant, seg_vec, mb, mode = call
-            RSA.alltoall_call(C, W, variant, seg_vec, mb, mode, seed)
+            E.alltoall_call(C, W, variant, seg_vec, mb, mode, seed)
         elif call[0] == "ar":
             _, variant, op, n_vec, mb, wire, mode, root = call
-            G.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
+            E.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
         elif call[0] == "bc":
             _, variant, n_vec, mb, mode, root = call
-            G.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
+            E.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
         else:
             kind, variant, seg_vec, mb, mode, root = call
-            (SGE.scatter_call if kind == "sc" else SGE.gather_call)(C, W, variant, seg_vec, mb, mode, root, seed)
+            (E.scatter_call if kind == "sc" else E.gather_call)(C, W, variant, seg_vec, mb, mode, root, seed)
     ep = _epochs(W)
     assert bool((ep == ep[0]).all())
     assert 0 < int(ep[0, 0]) < 1000                                   # block 0 went through the wrap
@@ -222,24 +218,12 @@ def test_alltoallv_shares_pads_and_inboxes_with_every_kind_through_the_epoch_wra
 DTYPES = AW.DTYPES
 
 
-def _bytes(t):
-    return t.detach().reshape(-1).view(torch.uint8).cpu()
-
-
-def _unaligned(x):
-    """``x`` on the GPU as a view one element into its storage (a data pointer that is not 16-byte aligned)."""
-    base = torch.zeros(x.numel() + 1, dtype=x.dtype, device="cuda")
-    v = base[1:].view(x.shape)
-    v.copy_(x)
-    return v
-
-
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
 def test_symm_world_all_to_all_v_single_and_list_forms(C, sms, world):
     """``all_to_all_v_`` of every dtype class, rows of several elements, skewed and empty splits, in the single-tensor form
     (aligned, unaligned, an output that is the input or overlaps it) and the list form (separate tensors, unaligned); the
     group's global ranks are not 0..W-1.  Every output equals plain slicing bit for bit, and inputs are unchanged."""
-    worlds, keep = G.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
+    worlds, keep = E.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
     forms = ["single", "list", "unaligned", "same", "overlap", "list_unaligned"]
     for k in range(2 * len(DTYPES)):
         dtype = DTYPES[k % len(DTYPES)]
@@ -279,14 +263,14 @@ def test_symm_world_all_to_all_v_single_and_list_forms(C, sms, world):
             unal = form == "list_unaligned"
             lin = [[(_unaligned(p) if unal else p.clone()) for p in torch.split(x, S[r])] for r, x in enumerate(ins)]
             lout = [[(_unaligned(p) if unal else p.clone()) for p in torch.split(o, out_splits[r])] for r, o in enumerate(outs)]
-            G.on_ranks(worlds, lambda r, w: w.all_to_all_v_(lout[r], lin[r]))
+            E.on_ranks(worlds, lambda r, w: w.all_to_all_v_(lout[r], lin[r]))
             for r in range(world):
                 got = torch.cat([_bytes(p) for p in lout[r]]) if lout[r] else torch.zeros(0, dtype=torch.uint8)
                 assert torch.equal(got, _bytes(want[r])), ("all_to_all_v_ list", dtype, form, S, r)
                 for s, p in enumerate(lin[r]):
                     assert torch.equal(_bytes(p), _bytes(torch.split(xs[r], S[r])[s])), ("input changed", dtype, r, s)
             continue
-        G.on_ranks(worlds, lambda r, w: w.all_to_all_v_(outs[r], ins[r], out_splits[r], S[r]))
+        E.on_ranks(worlds, lambda r, w: w.all_to_all_v_(outs[r], ins[r], out_splits[r], S[r]))
         for r in range(world):
             assert torch.equal(_bytes(outs[r]), _bytes(want[r])), ("all_to_all_v_", dtype, form, S, r)
             if form in ("single", "unaligned"):
@@ -315,25 +299,25 @@ def test_symm_world_all_to_all_v_single_and_list_forms(C, sms, world):
 def test_symm_world_all_to_all_v_calls_share_the_staging_buffer(C, sms, world):
     """All-to-allv calls with splits that change from call to call, between equal all-to-alls and reduce-scatters on the
     same staging buffer and pads."""
-    worlds, keep = G.symm_worlds(world, sms, list(range(world)))
+    worlds, keep = E.symm_worlds(world, sms, list(range(world)))
     for k in range(6):
         S = AW.split_matrix(world, 500 + k, hot=k % 2 == 1, most=[3, 9000, 40000][k % 3])
         xs = [AW.rows_of(S, s, torch.int64, (2,), k) for s in range(world)]
         want = AM.by_slicing(xs, S)
         ins = [x.cuda() for x in xs]
         outs = [torch.zeros_like(w_).cuda() for w_ in want]
-        G.on_ranks(worlds, lambda r, w: w.all_to_all_v_(outs[r], ins[r], [S[p][r] for p in range(world)], S[r]))
+        E.on_ranks(worlds, lambda r, w: w.all_to_all_v_(outs[r], ins[r], [S[p][r] for p in range(world)], S[r]))
         for r in range(world):
             assert torch.equal(outs[r].cpu(), want[r]), (k, r)
-        ys = [RSA._raw(torch.uint8, world * 3001, 10 * k + r).cuda() for r in range(world)]
+        ys = [E._raw(torch.uint8, world * 3001, 10 * k + r).cuda() for r in range(world)]
         zs = [torch.zeros_like(y) for y in ys]
-        G.on_ranks(worlds, lambda r, w: w.all_to_all_(zs[r], ys[r]))
+        E.on_ranks(worlds, lambda r, w: w.all_to_all_(zs[r], ys[r]))
         for r in range(world):
             assert torch.equal(zs[r].cpu(), torch.cat([y.view(world, -1)[r].cpu() for y in ys])), (k, r)
-        us = RSA.RS.make_inputs(CM.SUM, torch.int32, world, world * 1000, k)
+        us = RS.make_inputs(CM.SUM, torch.int32, world, world * 1000, k)
         vs = [u.cuda() for u in us]
         os_ = [torch.zeros(1000, dtype=torch.int32, device="cuda") for _ in range(world)]
-        G.on_ranks(worlds, lambda r, w: w.reduce_scatter_(os_[r], vs[r]))
+        E.on_ranks(worlds, lambda r, w: w.reduce_scatter_(os_[r], vs[r]))
         for r in range(world):
-            assert torch.equal(os_[r].cpu(), RSA.RS.reduce_scatter_result(CM.SUM, us, r)), (k, r)
+            assert torch.equal(os_[r].cpu(), RS.reduce_scatter_result(CM.SUM, us, r)), (k, r)
     del keep

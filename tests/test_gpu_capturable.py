@@ -7,7 +7,7 @@ import capturable_model as CM
 import capturable_workers as WK
 import dist_tuto.pth_b200 as b2
 from dist_tuto.pth_b200.ops.optim import LRSchedule, schedule_tuple
-from test_gpu_sharded_sgd_emulated import _untouched, _with_sentinel
+from emulated_ranks import C, _untouched, _with_sentinel  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -15,12 +15,6 @@ MU, BETAS, EPS = 0.9, (0.9, 0.999), 1e-8
 LRS, WDS = [0.1, 3e-3, 1.7e-4], [0.0, 0.01, 0.25]
 SCHEDULES = [None, LRSchedule(warmup_steps=7, decay="multistep", milestones=(20, 1000), gamma=0.5),
              LRSchedule(warmup_steps=3, decay="cosine", total_steps=2 ** 41, min_factor=0.1)]
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
 
 
 def _state(C):

@@ -1,5 +1,5 @@
 """The capturable instances of the sharded exchange kernel at emulated worlds 1..8 on one GPU (the harness of
-tests/test_gpu_sharded_sgd_emulated.py): fed the same scalars they equal the existing instances bit for bit, and W graphs of
+tests/emulated_ranks.py): fed the same scalars they equal the existing instances bit for bit, and W graphs of
 each rank's exchange plus step-counter advance, replayed concurrently for 50 steps across a schedule change, equal the
 existing instances launched eagerly with the model's scalars (tests/capturable_model.py) at every step."""
 import pytest
@@ -7,7 +7,7 @@ import torch
 
 import capturable_model as CM
 from dist_tuto.pth_b200.ops.optim import LRSchedule, schedule_tuple
-from test_gpu_sharded_sgd_emulated import World, _untouched, _with_sentinel
+from emulated_ranks import C, World, _untouched, _with_sentinel  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -15,12 +15,6 @@ MU, BETAS, EPS = 0.9, (0.8, 0.95), 1e-6
 LRS, WDS = [0.05, 0.01], [0.02, 0.0]
 SCHED = LRSchedule(warmup_steps=5, decay="multistep", milestones=(30,), gamma=0.25)
 STEPS = 50
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
 
 
 def _ranks(C, world, kind, wire, n_vec, grouped, seed):

@@ -1,69 +1,20 @@
 """PRODUCT / MAX / MIN all-reduce, reduce to a root, broadcast and all-gather (csrc/allreduce.cu) on ONE GPU with W emulated
 ranks, bit for bit against tests/collectives_model.py.
 
-The harness is tests/test_gpu_comm_emulated.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
+The harness is tests/emulated_ranks.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
 launches go out back to back, and no case runs more CTAs than the GPU has SMs (every CTA spins on its peers).  Outputs,
 symmetric buffers and the sentinels behind them are compared whole, so "a non-root leaves its output alone" and "the raw
 moves keep every bit" are checked as well.  The last tests drive ``SymmWorld``'s methods for W ranks built over the
 emulated buffers, one rank per stream.
 """
-import threading
-
 import pytest
 import torch
 
 import collectives_model as CM
 import comm_model as M
-import test_gpu_comm_emulated as E
-
-pytestmark = E.pytestmark
-
-RAW_SENTINEL = 0x5EADBEEF
-VARIANTS = [M.ONESHOT, M.TWOSHOT, M.LL]
-VARIANT_IDS = ["oneshot", "twoshot", "ll"]
-C = E.C
-sms = E.sms
-
-
-def _raw_sentinel(n, dev="cuda"):
-    return torch.full((n,), RAW_SENTINEL, dtype=torch.int32, device=dev)
-
-
-def _inbox(W, variant):
-    return (W.inbox_ptrs, M.LL_CAP_VEC) if variant == M.LL else ([], 0)
-
-
-def _check(what, got, want, epv):
-    M.assert_bits_equal(what, [g.cpu() for g in got], want, epv)
-
-
-# ---------------------------------------------------------------------------------------------------------- reductions
-def reduce_call(C, W, variant, op, n_vec, mb, wire, mode, local, root, seed):
-    world = W.world
-    epv = M.elems_per_vec(wire)
-    n = n_vec * epv
-    scale = 0.3 if op == CM.SUM else 1.0
-    xs = CM.make_reduce_inputs(op, world, n, local, seed)
-    bufs = [E._sentinel(n + E.SENT_VECS * epv, wire) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        for r in range(world):
-            bufs[r][:n].copy_(xs[r])
-        outs = bufs
-    else:
-        src = [torch.cat([xs[r], E._sentinel(E.SENT_VECS * epv, local, "cpu")]).cuda() for r in range(world)]
-        dst = src if mode == "alias" else [E._sentinel(n + E.SENT_VECS * epv, local) for _ in range(world)]
-        outs = dst
-    want = CM.reduce_model(variant, op, xs, wire, scale, mode, root, [o.cpu() for o in outs], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = _inbox(W, variant)
-    W.launch(M.grid_blocks(variant, n_vec, world, mb),
-             lambda r: C.allreduce(variant, wire == torch.bfloat16, ptrs, W.sig_ptrs, 0, src[r], dst[r], n_vec, scale, r,
-                                   world, mb, inbox, cap, op, root))
-    what = (f"{CM.OP_NAMES[op]} root {root} {M.VARIANT_NAMES[variant]} world {world} n_vec {n_vec} max_blocks {mb} "
-            f"wire {wire} {mode} {local}")
-    _check(what + ": output", outs, want["out"], epv)
-    _check(what + ": symmetric buffers", bufs, want["buf"], epv)
+import emulated_ranks as E
+from emulated_ranks import (C, VARIANT_IDS, VARIANTS, _bits_equal, allgather_call, broadcast_call,  # noqa: F401
+                            on_ranks, pytestmark, reduce_call, sms, symm_worlds)
 
 
 # (wire, mode, local): PRODUCT / MAX / MIN take the wire dtype locally; SUM (as a reduce) also fp32 over a bf16 wire
@@ -95,56 +46,6 @@ def test_reductions_match_the_model_bit_for_bit(C, sms, world, variant):
 
 
 # ---------------------------------------------------------------------------------------------------------- raw moves
-def broadcast_call(C, W, variant, n_vec, mb, mode, root, seed):
-    world, n = W.world, n_vec * 4
-    xs = CM.make_raw_inputs(world, n, seed)
-    bufs = [_raw_sentinel(n + 4 * E.SENT_VECS) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        for r in range(world):
-            bufs[r][:n].copy_(xs[r])
-        outs = bufs
-    else:
-        src = [torch.cat([xs[r], _raw_sentinel(4 * E.SENT_VECS, "cpu")]).cuda() for r in range(world)]
-        dst = src if mode == "alias" else [_raw_sentinel(n + 4 * E.SENT_VECS) for _ in range(world)]
-        outs = dst
-    want = CM.broadcast_model(variant, xs, root, mode, [o.cpu() for o in outs], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = _inbox(W, variant)
-    W.launch(M.grid_blocks(variant, n_vec, world, mb),
-             lambda r: C.broadcast(variant, ptrs, W.sig_ptrs, src[r], dst[r], n_vec, root, r, world, mb, inbox, cap))
-    what = f"broadcast root {root} {M.VARIANT_NAMES[variant]} world {world} n_vec {n_vec} max_blocks {mb} {mode}"
-    _check(what + ": output", outs, want["out"], 4)
-    _check(what + ": symmetric buffers", bufs, want["buf"], 4)
-
-
-def allgather_call(C, W, variant, seg_vec, mb, mode, seed):
-    world, seg = W.world, seg_vec * 4
-    n_vec = world * seg_vec
-    xs = CM.make_raw_inputs(world, seg, seed)
-    bufs = [_raw_sentinel(world * seg + 4 * E.SENT_VECS) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        for r in range(world):
-            bufs[r][r * seg:(r + 1) * seg].copy_(xs[r])
-        outs = bufs
-    else:
-        src = [torch.cat([xs[r], _raw_sentinel(4 * E.SENT_VECS, "cpu")]).cuda() for r in range(world)]
-        dst = [_raw_sentinel(world * seg + 4 * E.SENT_VECS) for _ in range(world)]
-        outs = dst
-    want = CM.allgather_model(variant, xs, mode, [o.cpu() for o in outs], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = _inbox(W, variant)
-    blocks = M.grid_blocks(variant, seg_vec if variant == M.LL else n_vec, world, mb)
-    W.launch(blocks, lambda r: C.allgather(variant, ptrs, W.sig_ptrs, src[r], dst[r], n_vec, r, world, mb, inbox, cap))
-    what = f"allgather {M.VARIANT_NAMES[variant]} world {world} per-rank vectors {seg_vec} max_blocks {mb} {mode}"
-    _check(what + ": output", outs, want["out"], 4)
-    _check(what + ": symmetric buffers", bufs, want["buf"], 4)
-    if src[0] is not None:
-        for r in range(world):
-            assert bool((src[r][seg:] == RAW_SENTINEL).all()), f"{what}: rank {r} wrote into src"
-
-
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
 @pytest.mark.parametrize("world", range(1, 9))
 def test_broadcast_matches_the_model_bit_for_bit(C, sms, world, variant):
@@ -209,54 +110,6 @@ def test_every_kind_of_call_shares_pads_and_inboxes_through_the_epoch_wrap(C, sm
 
 
 # ---------------------------------------------------------------------------------------------------------- SymmWorld
-def symm_worlds(world, sms, global_ranks):
-    """W SymmWorld objects over emulated buffers (no process group): world r has rank r, global rank global_ranks[r], and
-    handles whose per-rank pointers are the W emulated allocations, [signal pad | data] as alloc_bytes lays them out."""
-    from dist_tuto.pth_b200.ops import _ext
-    from dist_tuto.pth_b200.parallel import symm
-
-    keep = []
-
-    def alloc(nbytes):
-        ts = [torch.zeros((symm.PAD_BYTES + nbytes) // 4, dtype=torch.int32, device="cuda") for _ in range(world)]
-        keep.extend(ts)
-        return [t.data_ptr() for t in ts]
-
-    staging_bytes = 4 << 20
-    st_ptrs = {dt: alloc(staging_bytes) for dt in (torch.float32, torch.bfloat16)}
-    ll_ptrs = {dt: alloc(2 * world * symm.LL_CAP_VEC * 32) for dt in st_ptrs}
-    worlds = []
-    for r in range(world):
-        w = object.__new__(symm.SymmWorld)
-        w.C, w.group, w.ranks, w.world = _ext.C(), None, list(global_ranks), world
-        w.global_rank, w.rank = global_ranks[r], r
-        w.device = torch.device("cuda", 0)
-        w.multicast, w.mode, w.nvls_error, w.table_world = False, "emulated", None, None
-        w._handles, w._lock, w._staging = [], threading.Lock(), {}
-        w.max_blocks = sms // world
-        w.ll_max, w.oneshot_max, w.nvls_min = 32 << 10, 256 << 10, 1 << 62
-        for dt, ptrs in st_ptrs.items():
-            hd = symm.SymmHandle(w, staging_bytes, staging_bytes, ptrs, 0, [], 0, "emulated")
-            hd.ll = symm.SymmHandle(w, 0, 0, ll_ptrs[dt], 0, [], 0, "emulated")
-            w._staging[dt] = hd
-        worlds.append(w)
-    return worlds, keep
-
-
-def on_ranks(worlds, fn):
-    """fn(r, world_r) for every rank, each on its own stream, issued back to back."""
-    streams = [torch.cuda.Stream() for _ in worlds]
-    torch.cuda.synchronize()
-    for r, w in enumerate(worlds):
-        with torch.cuda.stream(streams[r]):
-            fn(r, w)
-    torch.cuda.synchronize()
-
-
-def _bits_equal(a, b):
-    return torch.equal(a.cpu().view(-1).view(torch.uint8), b.cpu().view(-1).view(torch.uint8))
-
-
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
 def test_symm_world_methods_route_stage_and_copy_out(C, sms, world):
     """Message sizes on both sides of every threshold (LL, one-shot, two-shot) and ragged ones; fp32 and bf16 reductions,

@@ -1,93 +1,20 @@
 """The all-reduce and gradient-exchange kernels (csrc/allreduce.cu, csrc/sgd.cu) on ONE GPU, with W emulated ranks.
 
-The kernels take raw per-rank pointers, so W "ranks" can be W sets of buffers on one device: each rank gets its own data,
-signal pad, inbox and stream, and its own launch.  That runs the arithmetic, indexing, padding, parity and epoch protocol of
+The harness is tests/emulated_ranks.py's: each rank gets its own data, signal pad, inbox and stream, and its own launch,
+and no case runs more CTAs than the GPU has SMs.  That runs the arithmetic, indexing, padding, parity and epoch protocol of
 the one-shot, two-shot and LL all-reduce and of both exchange flavours of ``allreduce_sgd`` at worlds 1-8, and every result
 is compared bit for bit with the model of tests/comm_model.py.  What it cannot cover (the memory model across NVLink, NVLS
 and the IPC / VMM mappings) stays in tests/test_gpu_multi.py.
-
-Every CTA of these kernels spins on its peers, so the W grids of one call must all be resident at once:
-
-* the W launches are issued back to back on W streams between two device synchronisations, never one after another with a
-  wait in between.  With serialized launches (CUDA_LAUNCH_BLOCKING=1, or a tool that serializes kernels) the first rank's
-  grid spins alone until B2_SPIN_LIMIT and traps, so this file is skipped under CUDA_LAUNCH_BLOCKING=1 and is not part of
-  tools/sanitize.sh;
-* the budget is one CTA per SM for all ranks together (``allreduce_oneshot_kernel<false>`` uses 128 registers x 512
-  threads, the whole register file of an SM): the harness computes each launch's grid as the launcher does and refuses
-  any case with ``world x blocks > SM count``.
 """
-import os
-
 import pytest
 import torch
 
 import comm_model as M
-
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900),
-              pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
-                                 reason="serialized launches: every rank's grid would spin alone until it traps")]
-
-SENT_VECS = 3                                   # sentinel vectors behind every buffer
-SENTINEL = {torch.float32: 0x5EADBEEF, torch.bfloat16: 0x5EAD}     # finite bit patterns no kernel result can produce here
-WRAP = 2 ** 32 - 5                              # epoch-wrap test: every pad's epoch and flag words start here
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _sentinel(n, dtype, dev="cuda"):
-    bits = torch.full((n,), SENTINEL[dtype], dtype=torch.int32 if dtype == torch.float32 else torch.int16, device=dev)
-    return bits.view(dtype)
-
-
-def _untouched(t):
-    ib = torch.int32 if t.dtype == torch.float32 else torch.int16
-    return bool((t.view(ib) == SENTINEL[t.dtype]).all())
-
-
-class World:
-    """W emulated ranks on cuda:0: a zeroed signal pad (uint32 [B2_SIGNAL_WORDS]), an LL inbox
-    ([2 parities][W sources][LL_CAP_VEC][2 lines of 16 B]) and a stream per rank."""
-
-    def __init__(self, world, sms, pad_start=0):
-        self.world, self.sms = world, sms
-        self.pads = [torch.zeros(M.SIGNAL_WORDS, dtype=torch.int32, device="cuda") for _ in range(world)]
-        if pad_start:
-            for p in self.pads:                   # per-block epoch words and every flag word
-                p[:M.EPOCH_WORD0 + M.MAX_BLOCKS] = pad_start - 2 ** 32 if pad_start >= 2 ** 31 else pad_start
-        self.inbox = [torch.zeros(2 * world * M.LL_CAP_VEC * 8, dtype=torch.int32, device="cuda") for _ in range(world)]
-        self.streams = [torch.cuda.Stream() for _ in range(world)]
-        self.sig_ptrs = [p.data_ptr() for p in self.pads]
-        self.inbox_ptrs = [b.data_ptr() for b in self.inbox]
-
-    def launch(self, blocks, fn):
-        """fn(r) issues rank r's kernel.  All W launches go out back to back, each on its own stream."""
-        assert self.world * blocks <= self.sms, (
-            f"{self.world} ranks x {blocks} CTAs would not be co-resident on {self.sms} SMs; not launched")
-        torch.cuda.synchronize()
-        for r in range(self.world):
-            with torch.cuda.stream(self.streams[r]):
-                fn(r)
-        torch.cuda.synchronize()
+from emulated_ranks import (C, SENT_VECS, WRAP, World, _typed_sentinel, _untouched, allreduce_cases,  # noqa: F401
+                            pytestmark, sms)
 
 
 # ---------------------------------------------------------------------------------------------------------- all-reduce
-# (wire dtype, mode, local dtype): in place on the symmetric buffers; src / dst; src aliasing dst (parallel/symm.py's
-# staged path)
-COMBOS = [(torch.float32, "inplace", torch.float32), (torch.float32, "staged", torch.float32),
-          (torch.float32, "alias", torch.float32), (torch.bfloat16, "inplace", torch.bfloat16),
-          (torch.bfloat16, "staged", torch.bfloat16), (torch.bfloat16, "staged", torch.float32),
-          (torch.bfloat16, "alias", torch.float32), (torch.bfloat16, "alias", torch.bfloat16)]
-
-
 def allreduce_call(C, W, variant, n_vec, max_blocks, wire, mode, local, scale, seed):
     """One all-reduce over the emulated world with fresh inputs; checks every rank's output, its symmetric buffer and the
     sentinels behind them against the model."""
@@ -96,14 +23,14 @@ def allreduce_call(C, W, variant, n_vec, max_blocks, wire, mode, local, scale, s
     n = n_vec * epv
     xs = M.make_inputs(world, n, local, seed)
     want = M.allreduce_model(variant, xs, wire, scale, local, staged=mode != "inplace")
-    bufs = [_sentinel(n + SENT_VECS * epv, wire) for _ in range(world)]
+    bufs = [_typed_sentinel(n + SENT_VECS * epv, wire) for _ in range(world)]
     src = dst = [None] * world
     if mode == "inplace":
         for r in range(world):
             bufs[r][:n].copy_(xs[r])
     else:
-        src = [torch.cat([xs[r], _sentinel(SENT_VECS * epv, local, "cpu")]).cuda() for r in range(world)]
-        dst = src if mode == "alias" else [_sentinel(n + SENT_VECS * epv, local) for _ in range(world)]
+        src = [torch.cat([xs[r], _typed_sentinel(SENT_VECS * epv, local, "cpu")]).cuda() for r in range(world)]
+        dst = src if mode == "alias" else [_typed_sentinel(n + SENT_VECS * epv, local) for _ in range(world)]
     buf_ptrs = [b.data_ptr() for b in bufs]
     ll = variant == M.LL
     blocks = M.grid_blocks(variant, n_vec, world, max_blocks)
@@ -124,24 +51,6 @@ def allreduce_call(C, W, variant, n_vec, max_blocks, wire, mode, local, scale, s
         if want["buf"][r] is None:
             assert _untouched(bufs[r]), f"{what}: rank {r}'s symmetric buffer was written"
     M.assert_bits_equal(what + ": symmetric buffers", [b[:n] for b in bufs], want["buf"], epv)
-
-
-def allreduce_cases(variant, world, sms):
-    """(n_vec, max_blocks, combo, scale) per case: every size at max_blocks 1, 3 and SMs // world; every (wire, mode, local)
-    combination once per max_blocks and so with every scale."""
-    scales = [1.0, 1.0 / world, 0.3]
-    out = []
-    for m, mb in enumerate([1, 3, sms // world]):
-        tail = 2 * M.THREADS * mb                 # one full pass of the unrolled peer-load loop at mb CTAs
-        if variant == M.LL:
-            sizes = [1, 511, 512, 513, 1023, 1025, 4095, M.LL_CAP_VEC]
-        elif variant == M.ONESHOT:
-            sizes = [1, 511, 512, 513, tail - 1, tail + 1, M.LL_CAP_VEC, 3 * tail + 700]
-        else:                                     # two-shot: slices, several of them not multiples of 512
-            sizes = [world * s for s in (1, 511, 512, 513, tail - 1, tail + 1, 700, 3 * tail + 300)]
-        for i, n_vec in enumerate(sizes):
-            out.append((n_vec, mb, COMBOS[(i + m) % len(COMBOS)], scales[m]))
-    return out
 
 
 @pytest.mark.parametrize("variant", [M.ONESHOT, M.TWOSHOT, M.LL], ids=["oneshot", "twoshot", "ll"])

@@ -9,16 +9,11 @@ import torch
 import torch.nn.functional as F
 
 import gemm_checks as G
+from emulated_ranks import C  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1200)]
 
 GROUPS = ["bn32", "bn64", "bn128", "persistent", "engine", "existing"]
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
 
 
 @pytest.fixture(scope="module")

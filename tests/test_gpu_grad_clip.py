@@ -1,6 +1,6 @@
 """GPU tier: gradient-norm clipping in the optimizer kernels (the clip instances of csrc/sgd.cu, csrc/sgd_device.cuh).
 
-* ``allreduce_sgd`` in both exchange flavours at emulated worlds 1-8 (the harness of tests/test_gpu_comm_emulated.py): the
+* ``allreduce_sgd`` in both exchange flavours at emulated worlds 1-8 (the harness of tests/emulated_ranks.py): the
   norm is bit-identical on every rank and within grad_clip_model.NORM_REL_TOL of the fp64 norm of the model's averaged
   gradient, and parameters, momentum, aux and buckets are bit-equal to the model given that norm; a huge max norm equals
   the instance without clipping; the uint32 epoch wrap; sizes where a thread has several vectors; an inf gradient;
@@ -9,8 +9,6 @@
   engine itself averaged, with the norm checked against fp64;
 * graph replays, ``run_native`` and eager steps agree bit for bit; a resumed checkpoint continues bit-equal; two GPUs.
 """
-import os
-
 import pytest
 import torch
 
@@ -21,25 +19,14 @@ import sgd_options_model as SM
 import dist_tuto.pth_b200 as b2
 from dist_tuto.pth_b200 import LRSchedule
 from dist_tuto.pth_b200 import data as D
-from test_gpu_comm_emulated import World
-from test_gpu_sgd_options import Spy, _batches, _slot_trainer, _state
+from emulated_ranks import SERIALIZED, C, World, sms  # noqa: F401
+from engine_paths import Spy, _batches, _slot_trainer, _state
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900),
-              pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
+              pytest.mark.skipif(SERIALIZED,
                                  reason="serialized launches: every emulated rank's grid would spin alone until it traps")]
 
 SCHED = LRSchedule(warmup_steps=4, decay="multistep", milestones=[7], gamma=0.5)
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.fixture(scope="module")
@@ -168,7 +155,7 @@ def test_an_inf_gradient_follows_torch(C, sms, world, exchange):
 
 # --------------------------------------------------------------------------------------------- engine paths
 class ClipSpy(Spy):
-    """Spy (tests/test_gpu_sgd_options.py) that also reads the norm each optimizer launch reported."""
+    """Spy (tests/engine_paths.py) that also reads the norm each optimizer launch reported."""
 
     def __init__(self, tr):
         super().__init__(tr)

@@ -8,9 +8,9 @@ import random
 import pytest
 import torch
 
+import layerwise_cases as TM
 import layerwise_model as L
-import test_layerwise_model as TM
-from test_gpu_sharded_sgd_emulated import _untouched, _with_sentinel
+from emulated_ranks import C, _bits, _untouched, _with_sentinel  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -23,16 +23,6 @@ LAYOUTS["chunk_multiples"] = [C_ - 1, C_ + 1, 2 * C_ - 1, 5, 2 * C_, 3 * C_ + 1,
 LAYOUTS["tiny_3000"] = [random.randint(1, 9) for _ in range(3000)]
 LAYOUTS["mixed"] = [300, 1, 17, 70001, 64, 4097, 2, 130]
 SENT64, SENT_I32 = 12345.678, 0x5EADBEEF
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-def _bits(a, b):
-    return torch.equal(a.cpu().view(torch.int32), b.cpu().view(torch.int32))
 
 
 def _layout(numels):

@@ -1,6 +1,6 @@
 """The point-to-point batch kernel (``p2p_batch``, csrc/p2p.cu) on ONE GPU with W emulated ranks, bit for bit.
 
-The harness is tests/test_gpu_p2p_emulated.py's: each rank has its own mailbox, every (rank, peer, direction) and every
+The harness is tests/emulated_ranks.py's mailboxes: each rank has its own mailbox, every (rank, peer, direction) and every
 rank's batch gets a CUDA stream of its own (``stream_create``), destinations have sentinels behind them, sources are compared
 with their values before the call, and no round runs more CTAs than the GPU has SMs.  A round is submitted so that no stream
 holds a kernel that waits for one submitted after it behind another of its own: batches go first, and a rank that uses single
@@ -17,28 +17,8 @@ import threading
 import pytest
 import torch
 
-import test_gpu_comm_emulated as E
-import test_gpu_p2p_emulated as P
-
-pytestmark = E.pytestmark
-
-C = E.C
-sms = E.sms
-geo = P.geo
-worlds = P.worlds
-WRAP = P.WRAP
-
-
-@pytest.fixture
-def boxes(C, sms):
-    made = []
-
-    def make(world, start=0):
-        made.append(P.Mailboxes(C, world, sms, start))
-        return made[-1]
-    yield make
-    for m in made:
-        m.close()
+import emulated_ranks as E
+from emulated_ranks import C, WRAP, boxes, geo, pytestmark, sms, worlds  # noqa: F401
 
 
 def _nbytes(t):
@@ -108,22 +88,22 @@ def run_and_check(boxes, world, rounds, seed, start=0):
     for rnd in rounds:
         msgs = []
         for a, b, n in rnd.transfers:
-            x = P._message(n, seed + k)
+            x = E._message(n, seed + k)
             k += 1
-            msgs.append((x, x.cpu(), P._dest(n)))
+            msgs.append((x, x.cpu(), E._dest(n)))
         _run_round(B, rnd, [(x, xb, y[:_nbytes(x)]) for x, xb, y in msgs])
         for (a, b, n), (x, xb, y) in zip(rnd.transfers, msgs):
-            P._check(f"rank {a} -> rank {b}, {n} bytes", x, xb, y)
+            E._check_message(f"rank {a} -> rank {b}, {n} bytes", x, xb, y)
     R = boxes(world, start)
     for rnd in rounds:
-        R.run([(a, b, P._message(n, 0), torch.empty(n, dtype=torch.uint8, device="cuda")) for a, b, n in rnd.transfers])
+        R.run([(a, b, E._message(n, 0), torch.empty(n, dtype=torch.uint8, device="cuda")) for a, b, n in rnd.transfers])
     for r in range(world):
         got, want = B.counters(r), R.counters(r)
         for name in got:
             assert torch.equal(got[name], want[name]), (f"rank {r} {name} after the batches differs from the single "
                                                         f"launches", got[name], want[name])
     pairs = {(a, b) for rnd in rounds for a, b, n in rnd.transfers if n}
-    P._agree(B, sorted(pairs))
+    E._agree(B, sorted(pairs))
     return B
 
 
@@ -263,15 +243,15 @@ def test_symm_world_batches_any_dtype_aligned_or_not(C, sms, worlds, world):
     globals_ = [3 + 2 * r for r in range(world)]
     ws, streams = worlds(world, globals_)
     for k, (dtype, numel) in enumerate(CASES):
-        xs = [P._values(dtype, numel, 100 * world + 10 * k + r).cuda() for r in range(world)]
+        xs = [E._values(dtype, numel, 100 * world + 10 * k + r).cuda() for r in range(world)]
         if dtype == torch.float32 and numel:
             xs[0][0] = float("nan")
         ys = {(r, d): torch.zeros(numel, dtype=dtype, device="cuda") for r in range(world) for d in (-1, 1)}
         if k % 3 == 1:
-            xs = [P._unaligned(x) for x in xs]
+            xs = [E._unaligned(x) for x in xs]
         if k % 3 == 2:
-            ys = {key: P._unaligned(y) for key, y in ys.items()}
-        before = [P._bits(x) for x in xs]
+            ys = {key: E._unaligned(y) for key, y in ys.items()}
+        before = [E._bytes(x) for x in xs]
         torch.cuda.synchronize()
         works = {}
         nbrs = lambda r: sorted({(r + 1) % world, (r - 1) % world})
@@ -285,8 +265,8 @@ def test_symm_world_batches_any_dtype_aligned_or_not(C, sms, worlds, world):
             assert len(works[(r, "s")]) == len(nbrs(r)) and len(works[(r, "r")]) == len(nbrs(r))
             for q in nbrs(r):
                 d = 1 if q == (r + 1) % world else -1
-                assert torch.equal(P._bits(ys[(r, d)]), before[q]), (dtype, numel, r, q)
-            assert torch.equal(P._bits(xs[r]), before[r]), ("source changed", dtype, numel, r)
+                assert torch.equal(E._bytes(ys[(r, d)]), before[q]), (dtype, numel, r, q)
+            assert torch.equal(E._bytes(xs[r]), before[r]), ("source changed", dtype, numel, r)
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])
@@ -298,7 +278,7 @@ def test_symm_world_ring_with_sends_and_receives_in_one_batch(C, sms, worlds, wo
     ws, streams = worlds(world, globals_)
     G, S, CHUNK, _ = C.p2p_config()
     for k, (dtype, numel) in enumerate([(torch.float32, G * S * CHUNK // 4), (torch.int16, 12345), (torch.uint8, 3)]):
-        xs = [P._values(dtype, numel, 1000 * world + 10 * k + r).cuda() for r in range(world)]
+        xs = [E._values(dtype, numel, 1000 * world + 10 * k + r).cuda() for r in range(world)]
         ys = [torch.zeros(numel, dtype=dtype, device="cuda") for _ in range(world)]
         zs = [torch.zeros(numel, dtype=dtype, device="cuda") for _ in range(world)]
         torch.cuda.synchronize()
@@ -316,8 +296,8 @@ def test_symm_world_ring_with_sends_and_receives_in_one_batch(C, sms, worlds, wo
         _in_order(ws, streams, range(world), lambda r, w: [q.wait() for q in reqs[r]])
         torch.cuda.synchronize()
         for r in range(world):
-            assert torch.equal(P._bits(ys[r]), P._bits(xs[left(r)])), (dtype, numel, r)
-            assert torch.equal(P._bits(zs[r]), P._bits(xs[left(left(r))])), (dtype, numel, r)
+            assert torch.equal(E._bytes(ys[r]), E._bytes(xs[left(r)])), (dtype, numel, r)
+            assert torch.equal(E._bytes(zs[r]), E._bytes(xs[left(left(r))])), (dtype, numel, r)
 
 
 def test_request_wait_orders_later_work_on_the_current_stream(C, worlds):
@@ -326,8 +306,8 @@ def test_request_wait_orders_later_work_on_the_current_stream(C, worlds):
     from dist_tuto.pth_b200 import comm
     ws, streams = worlds(2, [0, 1])
     G, S, CHUNK, _ = C.p2p_config()
-    x = P._values(torch.int32, G * CHUNK // 4, 7).cuda()     # with x2, fits the pair's slots: the send batch ends by itself
-    x2 = P._values(torch.int8, 999, 8).cuda()
+    x = E._values(torch.int32, G * CHUNK // 4, 7).cuda()     # with x2, fits the pair's slots: the send batch ends by itself
+    x2 = E._values(torch.int8, 999, 8).cuda()
     y, y2 = torch.zeros_like(x), torch.zeros_like(x2)
     out = torch.zeros_like(x)
     torch.cuda.synchronize()
@@ -351,7 +331,7 @@ def test_is_completed_before_and_after_the_batch(C, worlds):
     """A batch queued behind a long kernel on the current stream has not completed when ``batch_p2p_`` returns, and its
     works share one event; after the peer's batch and a synchronisation every work reports completion."""
     ws, streams = worlds(2, [0, 1])
-    x, x2 = P._values(torch.uint8, 1000, 9).cuda(), P._values(torch.uint8, 70000, 10).cuda()
+    x, x2 = E._values(torch.uint8, 1000, 9).cuda(), E._values(torch.uint8, 70000, 10).cuda()
     y, y2 = torch.zeros_like(x), torch.zeros_like(x2)
     torch.cuda.synchronize()
     with torch.cuda.stream(streams[0]):

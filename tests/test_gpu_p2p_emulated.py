@@ -1,6 +1,6 @@
 """Point-to-point send / recv (csrc/p2p.cu) on ONE GPU with W emulated ranks, bit for bit.
 
-The harness follows tests/test_gpu_comm_emulated.py: each rank has its own mailbox (data and signal pad), and the kernels of
+The harness is tests/emulated_ranks.py's: each rank has its own mailbox (data and signal pad), and the kernels of
 one batch go out back to back between two device synchronisations.  Unlike a collective, a rank runs a send and a receive at
 once, and each waits for its peer, so every (rank, peer, direction) gets a CUDA stream of its own (``stream_create``, never a
 pooled torch stream that could alias another).  Kernels that wait for each other are submitted so that whatever a kernel
@@ -10,114 +10,12 @@ before the call.  The last tests drive ``SymmWorld.send_`` / ``recv_`` / ``isend
 emulated mailboxes, one rank per stream.
 """
 import random
-import threading
 
 import pytest
 import torch
 
-import test_gpu_comm_emulated as E
-
-pytestmark = E.pytestmark
-
-C = E.C
-sms = E.sms
-SENT = 48                                       # sentinel bytes behind every destination
-SENT_BYTE = 0xA5
-WRAP = 2 ** 32 - 5                              # counter-wrap test: every counter word starts here
-
-
-@pytest.fixture(scope="module")
-def geo(C):
-    """(CTAs per transfer, slots per CTA, bytes per slot, signal-pad words)."""
-    return C.p2p_config()
-
-
-def _stream(C):
-    return torch.cuda.ExternalStream(C.stream_create(0), device=torch.device("cuda", 0))
-
-
-class Mailboxes:
-    """W emulated ranks' mailboxes on cuda:0 (data [W - 1 sources][G x S slots][CHUNK] after an 8 KB signal pad, as
-    ``SymmWorld`` allocates them) and a stream per (rank, peer, direction)."""
-
-    def __init__(self, C, world, sms, start=0):
-        from dist_tuto.pth_b200.parallel import symm
-        self.C, self.world, self.sms = C, world, sms
-        self.G, self.S, self.CHUNK, self.pad_words = C.p2p_config()
-        data = max(world - 1, 1) * self.G * self.S * self.CHUNK
-        self.mem = [torch.zeros((symm.PAD_BYTES + data) // 4, dtype=torch.int32, device="cuda") for _ in range(world)]
-        if start:
-            for m in self.mem:
-                m[:self.pad_words] = start - 2 ** 32 if start >= 2 ** 31 else start
-        self.sig_ptrs = [m.data_ptr() for m in self.mem]
-        self.box_ptrs = [p + symm.PAD_BYTES for p in self.sig_ptrs]
-        self.streams = {}
-
-    def stream(self, r, peer, send):
-        if (r, peer, send) not in self.streams:
-            self.streams[(r, peer, send)] = _stream(self.C)
-        return self.streams[(r, peer, send)]
-
-    def grid(self, nbytes):
-        return min(self.G, (nbytes + self.CHUNK - 1) // self.CHUNK)
-
-    def run(self, transfers):
-        """transfers: [(src rank, dst rank, src tensor, dst tensor)], submitted in this order, each as the send on the
-        sender's stream, then the receive on the receiver's."""
-        busy = {}
-        for a, b, x, y in transfers:
-            g = self.grid(x.numel() * x.element_size())
-            for key in ((a, b, True), (b, a, False)):
-                busy[key] = max(busy.get(key, 0), g)
-        assert sum(busy.values()) <= self.sms, f"{sum(busy.values())} CTAs would not be co-resident on {self.sms} SMs"
-        torch.cuda.synchronize()
-        for a, b, x, y in transfers:
-            with torch.cuda.stream(self.stream(a, b, True)):
-                self.C.p2p_send(self.box_ptrs, self.sig_ptrs, x, b, a, self.world)
-            with torch.cuda.stream(self.stream(b, a, False)):
-                self.C.p2p_recv(self.box_ptrs, self.sig_ptrs, y, a, b, self.world)
-        torch.cuda.synchronize()
-
-    def counters(self, r):
-        """Rank r's signal-pad counters as uint32: {name: [peer][slot]}."""
-        words = self.mem[r][:self.pad_words].cpu().to(torch.int64) % 2 ** 32
-        per = self.G * self.S
-        return {name: words[k * 8 * per:(k + 1) * 8 * per].view(8, per) for k, name in
-                enumerate(("flag", "ack", "fills", "consumed"))}
-
-    def close(self):
-        torch.cuda.synchronize()
-        for s in self.streams.values():
-            self.C.stream_destroy(s.cuda_stream)
-        self.streams.clear()
-
-
-@pytest.fixture
-def boxes(C, sms):
-    made = []
-
-    def make(world, start=0):
-        made.append(Mailboxes(C, world, sms, start))
-        return made[-1]
-    yield make
-    for m in made:
-        m.close()
-
-
-def _message(nbytes, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.randint(0, 256, (nbytes,), generator=g, dtype=torch.uint8).cuda()
-
-
-def _dest(nbytes):
-    return torch.full((nbytes + SENT,), SENT_BYTE, dtype=torch.uint8, device="cuda")
-
-
-def _check(what, x, x_before, y):
-    n = x.numel()
-    assert torch.equal(y[:n].cpu(), x_before), f"{what}: received bytes differ"
-    assert bool((y[n:] == SENT_BYTE).all()), f"{what}: bytes written behind the destination"
-    assert torch.equal(x.cpu(), x_before), f"{what}: the source changed"
+from emulated_ranks import (C, WRAP, _agree, _bytes, _check_message, _dest, _message, _unaligned, _values,  # noqa: F401
+                            boxes, geo, on_ranks, pytestmark, sms, worlds)
 
 
 def _transfer(boxes, pairs, seed):
@@ -128,7 +26,7 @@ def _transfer(boxes, pairs, seed):
         msgs.append((a, b, x, x.cpu(), _dest(n)))
     boxes.run([(a, b, x, y[:n]) for (a, b, x, _, y), (_, _, n) in zip(msgs, pairs)])
     for a, b, x, xb, y in msgs:
-        _check(f"rank {a} -> rank {b}, {x.numel()} bytes", x, xb, y)
+        _check_message(f"rank {a} -> rank {b}, {x.numel()} bytes", x, xb, y)
 
 
 def _agree(boxes, pairs):
@@ -218,70 +116,6 @@ def test_counters_wrap_through_zero(C, boxes, geo, world):
 
 
 # ---------------------------------------------------------------------------------------------------------- SymmWorld
-def symm_worlds(C, world, global_ranks):
-    """W SymmWorld objects over emulated mailboxes (no process group): world r has rank r and global rank
-    global_ranks[r]; ``p2p`` is a handle whose per-rank pointers are the W emulated allocations."""
-    from dist_tuto.pth_b200.parallel import symm
-    G, S, CHUNK, _ = C.p2p_config()
-    nbytes = (world - 1) * G * S * CHUNK
-    keep = [torch.zeros((symm.PAD_BYTES + nbytes) // 4, dtype=torch.int32, device="cuda") for _ in range(world)]
-    worlds = []
-    for r in range(world):
-        w = object.__new__(symm.SymmWorld)
-        w.C, w.group, w.ranks, w.world = C, None, list(global_ranks), world
-        w.global_rank, w.rank = global_ranks[r], r
-        w.device = torch.device("cuda", 0)
-        w._handles, w._lock, w._staging = [], threading.Lock(), {}
-        w.p2p = symm.SymmHandle(w, nbytes, nbytes, [t.data_ptr() for t in keep], 0, [], 0, "emulated")
-        w._p2p_streams = {}
-        worlds.append(w)
-    return worlds, keep
-
-
-@pytest.fixture
-def worlds(C):
-    made = []
-
-    def make(world, global_ranks):
-        ws, keep = symm_worlds(C, world, global_ranks)
-        streams = [_stream(C) for _ in range(world)]
-        made.append((ws, keep, streams))
-        return ws, streams
-    yield make
-    torch.cuda.synchronize()
-    for ws, keep, streams in made:
-        for w in ws:
-            for s in w._p2p_streams.values():
-                C.stream_destroy(s.cuda_stream)
-        for s in streams:
-            C.stream_destroy(s.cuda_stream)
-
-
-def on_ranks(streams, worlds, fn):
-    """fn(r, world_r) for every rank, each with its own current stream, issued back to back."""
-    for r, w in enumerate(worlds):
-        with torch.cuda.stream(streams[r]):
-            fn(r, w)
-
-
-def _values(dtype, numel, seed):
-    g = torch.Generator().manual_seed(seed)
-    raw = torch.randint(0, 256, (numel * torch.empty((), dtype=dtype).element_size(),), generator=g, dtype=torch.uint8)
-    return (raw % 2).to(torch.bool) if dtype == torch.bool else raw.view(dtype)
-
-
-def _unaligned(x):
-    """``x`` on the GPU as a view that starts 1 element into its storage (not 16-byte aligned for any dtype here)."""
-    base = torch.zeros(x.numel() + 1, dtype=x.dtype, device="cuda")
-    v = base[1:]
-    v.copy_(x)
-    return v
-
-
-def _bits(t):
-    return t.detach().cpu().contiguous().view(-1).view(torch.uint8)
-
-
 CASES = [(torch.float32, 1), (torch.int64, 3), (torch.bfloat16, 4097), (torch.uint8, 17), (torch.bool, 1000),
          (torch.int16, 40000), (torch.float64, 0), (torch.int32, 100003), (torch.uint8, 1 << 20)]
 
@@ -303,22 +137,22 @@ def test_symm_world_ring_any_dtype_aligned_or_not(C, sms, worlds, world, blockin
             xs = [_unaligned(x) for x in xs]
         if k % 3 == 2:
             ys = [_unaligned(y) for y in ys]
-        before = [_bits(x) for x in xs]
+        before = [_bytes(x) for x in xs]
         torch.cuda.synchronize()
         right = [globals_[(r + 1) % world] for r in range(world)]
         left = [globals_[(r - 1) % world] for r in range(world)]
         if blocking:
-            on_ranks(streams, ws, lambda r, w: w.send_(xs[r], right[r]))
-            on_ranks(streams, ws, lambda r, w: w.recv_(ys[r], left[r]))
+            on_ranks(ws, lambda r, w: w.send_(xs[r], right[r]), streams)
+            on_ranks(ws, lambda r, w: w.recv_(ys[r], left[r]), streams)
         else:
             reqs = [None] * world
-            on_ranks(streams, ws, lambda r, w: reqs.__setitem__(r, [w.isend_(xs[r], right[r])]))
-            on_ranks(streams, ws, lambda r, w: reqs[r].append(w.irecv_(ys[r], left[r])))
-            on_ranks(streams, ws, lambda r, w: [q.wait() for q in reqs[r]])
+            on_ranks(ws, lambda r, w: reqs.__setitem__(r, [w.isend_(xs[r], right[r])]), streams)
+            on_ranks(ws, lambda r, w: reqs[r].append(w.irecv_(ys[r], left[r])), streams)
+            on_ranks(ws, lambda r, w: [q.wait() for q in reqs[r]], streams)
         torch.cuda.synchronize()
         for r in range(world):
-            assert torch.equal(_bits(ys[r]), before[(r - 1) % world]), (dtype, numel, r)
-            assert torch.equal(_bits(xs[r]), before[r]), ("source changed", dtype, numel, r)
+            assert torch.equal(_bytes(ys[r]), before[(r - 1) % world]), (dtype, numel, r)
+            assert torch.equal(_bytes(xs[r]), before[r]), ("source changed", dtype, numel, r)
 
 
 def test_request_wait_orders_later_work_on_the_current_stream(C, worlds):

@@ -1,32 +1,18 @@
 """The grouped optimizer kernels on one GPU.  Oracle: the existing ungrouped kernel run on each tensor's padded segment (or, for
 the sharded kernel, on the whole world) with its group's scalars -- the grouped kernels must match it bit for bit, since the
 per-element sequence is the same and only the scalars' source differs.  Sharded cases use the emulated world of
-tests/test_gpu_sharded_sgd_emulated.py; the end-to-end case trains a ResNet-18 through the public API."""
-import os
-
+tests/emulated_ranks.py; the end-to-end case trains a ResNet-18 through the public API."""
 import pytest
 import torch
 
 import adamw_model as A
 import dist_tuto.pth_b200 as b2
 import param_groups_gpu_workers as WK
-from test_gpu_sharded_sgd_emulated import WRAP, World, _untouched, _with_sentinel
+from emulated_ranks import CO_RESIDENT, WRAP, C, World, _bits, _untouched, _with_sentinel  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
 MU, BETAS, EPS = 0.9, (0.8, 0.95), 1e-6
-NO_BLOCKING = pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
-                                 reason="serialized launches: the ranks' grids must be co-resident")
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-def _bits(a, b):
-    return torch.equal(a.cpu().view(torch.int32), b.cpu().view(torch.int32))
 
 
 def _layout(sizes, gids):
@@ -203,7 +189,7 @@ def _run_sharded(C, world, sms, kind, wire, n_vec, max_blocks, zero_grad, pad_st
             assert _bits(got[1][i][r], want_s[i][r]), f"{what}: state {i} of rank {r}"
 
 
-@NO_BLOCKING
+@CO_RESIDENT
 @pytest.mark.parametrize("world", range(1, 9))
 @pytest.mark.parametrize("kind", ["sgd", "adamw"])
 def test_sharded_grouped_equals_the_ungrouped_kernel_per_group(C, world, kind):

@@ -1,7 +1,7 @@
 """The all-reduce and reduce of fp16, fp64, int8, uint8, int32, int64 and bool (csrc/allreduce.cu lane types) on ONE GPU with
 W emulated ranks, bit for bit against tests/reduce_dtypes_model.py.
 
-The harness is tests/test_gpu_comm_emulated.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
+The harness is tests/emulated_ranks.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
 launches go out back to back, and no case runs more CTAs than the GPU has SMs (every CTA spins on its peers).  Outputs,
 symmetric buffers and the sentinels behind them are compared whole.  The last tests drive ``SymmWorld.all_reduce_`` /
 ``reduce_`` for W ranks built over the emulated buffers, one rank per stream.
@@ -11,23 +11,11 @@ import torch
 
 import collectives_model as CM
 import comm_model as M
+import emulated_ranks as E
 import reduce_dtypes_model as RM
-import test_gpu_collectives_emulated as GC
-import test_gpu_comm_emulated as E
+from emulated_ranks import C, VARIANT_IDS, VARIANTS, _bits_equal, _byte_sentinel, pytestmark, sms  # noqa: F401
 
-pytestmark = E.pytestmark
-
-SENTINEL_BYTE = 0x5E                        # 0x5E5E... is finite in fp16 and fp64, and no result here is all 0x5E bytes
-VARIANTS = [M.ONESHOT, M.TWOSHOT, M.LL]
-VARIANT_IDS = ["oneshot", "twoshot", "ll"]
 OPS = [CM.SUM, CM.PRODUCT, CM.MAX, CM.MIN]
-C = E.C
-sms = E.sms
-
-
-def _sentinel(n, dtype, dev="cuda"):
-    es = torch.empty((), dtype=dtype).element_size()
-    return torch.full((n * es,), SENTINEL_BYTE, dtype=torch.uint8, device=dev).view(dtype)
 
 
 def reduce_call(C, W, variant, dtype, op, n_vec, mb, mode, root, seed):
@@ -36,21 +24,21 @@ def reduce_call(C, W, variant, dtype, op, n_vec, mb, mode, root, seed):
     n = n_vec * epv
     xs = RM.make_inputs(op, dtype, world, n, seed)
     tail = E.SENT_VECS * epv
-    bufs = [_sentinel(n + tail, dtype) for _ in range(world)]
+    bufs = [_byte_sentinel(n + tail, dtype) for _ in range(world)]
     src = dst = [None] * world
     if mode == "inplace":
         for r in range(world):
             bufs[r][:n].copy_(xs[r])
         outs = bufs
     else:
-        src = [torch.cat([RM.as_bytes(xs[r]), RM.as_bytes(_sentinel(tail, dtype, "cpu"))]).cuda().view(dtype)
+        src = [torch.cat([RM.as_bytes(xs[r]), RM.as_bytes(_byte_sentinel(tail, dtype, "cpu"))]).cuda().view(dtype)
                for r in range(world)]
-        dst = src if mode == "alias" else [_sentinel(n + tail, dtype) for _ in range(world)]
+        dst = src if mode == "alias" else [_byte_sentinel(n + tail, dtype) for _ in range(world)]
         outs = dst
     want = RM.reduce_model(variant, op, xs, mode, root, [RM.as_bytes(o).cpu() for o in outs],
                            [RM.as_bytes(b).cpu() for b in bufs])
     ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = GC._inbox(W, variant)
+    inbox, cap = E._inbox(W, variant)
     kop = RM.kernel_op(op, dtype)
     W.launch(M.grid_blocks(variant, n_vec, world, mb),
              lambda r: C.allreduce(variant, False, ptrs, W.sig_ptrs, 0, src[r], dst[r], n_vec, 1.0, r, world, mb, inbox, cap,
@@ -123,13 +111,13 @@ def test_new_dtypes_share_pads_and_inboxes_with_every_call_through_the_epoch_wra
             reduce_call(C, W, variant, dtype, op, n_vec, mb, mode, root, seed)
         elif c[0] == "ar":
             _, variant, op, n_vec, mb, wire, mode, root = c
-            GC.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
+            E.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
         elif c[0] == "bc":
             _, variant, n_vec, mb, mode, root = c
-            GC.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
+            E.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
         else:
             _, variant, seg_vec, mb, mode = c
-            GC.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
+            E.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
     ep = torch.stack([p[M.EPOCH_WORD0:M.EPOCH_WORD0 + M.MAX_BLOCKS] for p in W.pads]).cpu()
     assert bool((ep == ep[0]).all())
     assert 0 < int(ep[0, 0]) < 100
@@ -160,17 +148,13 @@ def test_nan_results_have_the_pinned_bit_patterns(C, sms):
 
 
 # ---------------------------------------------------------------------------------------------------------- SymmWorld
-def _bits_equal(a, b):
-    return torch.equal(a.cpu().view(-1).view(torch.uint8), b.cpu().view(-1).view(torch.uint8))
-
-
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
 def test_symm_world_reduces_every_dtype_with_ragged_and_unaligned_tensors(C, sms, world):
     """``all_reduce_`` and ``reduce_`` of every new dtype on both sides of the LL / one-shot / two-shot thresholds, ragged
     sizes, and views that start one element into their storage (not 16-byte aligned); a bool SUM is a MAX; roots are global
     ranks of a group whose ranks are not 0..W-1."""
     globals_ = [10 + 3 * r for r in range(world)]
-    worlds, keep = GC.symm_worlds(world, sms, globals_)
+    worlds, keep = E.symm_worlds(world, sms, globals_)
     for k, numel in enumerate([5, 1024, 3001, 12288, 40000, 200003]):
         for d, dtype in enumerate(RM.DTYPES):
             op = OPS[(k + d) % 4]
@@ -180,12 +164,12 @@ def test_symm_world_reduces_every_dtype_with_ragged_and_unaligned_tensors(C, sms
             unaligned = (k + d) % 2 == 1
             bases = [torch.cat([x[:1], x]).cuda() if unaligned else x.cuda() for x in xs]
             ts = [b[1:] if unaligned else b for b in bases]
-            GC.on_ranks(worlds, lambda r, w: w.all_reduce_(ts[r], op=op))
+            E.on_ranks(worlds, lambda r, w: w.all_reduce_(ts[r], op=op))
             RM.assert_bits_equal(f"all_reduce_ {RM.NAMES[dtype]} {CM.OP_NAMES[op]} {numel}", [t.cpu() for t in ts],
                                  [want] * world, any_nan)
             root_local = [0, world - 1, world // 2][(k + d) % 3]
             ts = [x.cuda() for x in xs]
-            GC.on_ranks(worlds, lambda r, w: w.reduce_(ts[r], globals_[root_local], op))
+            E.on_ranks(worlds, lambda r, w: w.reduce_(ts[r], globals_[root_local], op))
             for r in range(world):
                 if r == root_local:
                     RM.assert_bits_equal(f"reduce_ {RM.NAMES[dtype]} {numel}", [ts[r].cpu()], [want], any_nan)
@@ -208,7 +192,7 @@ def test_evaluate_sums_its_float64_totals_on_the_fp64_kernels(C, sms, world, mon
     fp64 sum."""
     from dist_tuto.pth_b200 import comm
     from dist_tuto.pth_b200.ops import convnet_eval
-    worlds, keep = GC.symm_worlds(world, sms, list(range(world)))
+    worlds, keep = E.symm_worlds(world, sms, list(range(world)))
     current = {}
     monkeypatch.setattr(comm, "is_initialized", lambda: True)
     monkeypatch.setattr(comm, "get_world_size", lambda group=None: world)
@@ -230,7 +214,7 @@ def test_evaluate_sums_its_float64_totals_on_the_fp64_kernels(C, sms, world, mon
     def one(r, w):
         current["w"] = w
         got[r] = convnet_eval._group_sum(ts[r], None)
-    GC.on_ranks(worlds, one)
+    E.on_ranks(worlds, one)
     for r in range(world):
         assert got[r].is_cuda and got[r].data_ptr() == ts[r].data_ptr(), "the sum left the device"
         assert torch.equal(got[r].cpu().view(torch.int64), want.view(torch.int64)), (r, got[r], want)

@@ -1,7 +1,7 @@
 """Reduce-scatter and all-to-all (csrc/allreduce.cu segments_pull_kernel / segments_ll_kernel) on ONE GPU with W emulated
 ranks, bit for bit against tests/reduce_scatter_alltoall_model.py.
 
-The harness is tests/test_gpu_comm_emulated.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
+The harness is tests/emulated_ranks.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
 launches go out back to back, and no case runs more CTAs than the GPU has SMs.  Outputs, symmetric buffers, the sentinels
 behind them and every src are compared whole.  The reduce-scatter is also compared with the all-reduce kernels' slice on the
 same inputs, the new calls share pads and inboxes with every other kind of call through the uint32 epoch wrap, and the last
@@ -12,92 +12,15 @@ import torch
 
 import collectives_model as CM
 import comm_model as M
+import emulated_ranks as E
 import reduce_dtypes_model as RM
 import reduce_scatter_alltoall_model as RS
-import test_gpu_collectives_emulated as G
-import test_gpu_comm_emulated as E
-import test_gpu_reduce_dtypes_emulated as GD
-import test_gpu_scatter_gather_emulated as SGE
-
-pytestmark = E.pytestmark
+from emulated_ranks import (C, _any_nan, _bytes_cpu, _grid, _raw, _unaligned, alltoall_call, pytestmark,  # noqa: F401
+                            reduce_scatter_call, sms)
 
 VARIANTS = [M.ONESHOT, M.LL]                     # pull (what one-shot, two-shot and NVLS run here) and LL
 VARIANT_IDS = ["pull", "ll"]
 OPS = [CM.SUM, CM.PRODUCT, CM.MAX, CM.MIN]
-C = E.C
-sms = E.sms
-
-
-def _grid(variant, seg_vec, mb):
-    """The launchers' grid: one thread per vector of a segment; LL never capped by max_blocks."""
-    return M.grid_blocks(M.LL, seg_vec, 1, 0) if variant == M.LL else M.grid_blocks(M.ONESHOT, seg_vec, 1, mb)
-
-
-def _any_nan(op, dtype):
-    return dtype in (torch.float32, torch.bfloat16) or RM.nan_any(op, dtype)
-
-
-def _bytes_cpu(ts):
-    return [RM.as_bytes(t).cpu() for t in ts]
-
-
-def reduce_scatter_call(C, W, variant, dtype, op, seg_vec, mb, mode, seed):
-    world = W.world
-    epv = RS.elems_per_vec(dtype)
-    seg = seg_vec * epv
-    n = world * seg
-    xs = RS.make_inputs(op, dtype, world, n, seed)
-    tail = E.SENT_VECS * epv
-    bufs = [GD._sentinel(n + tail, dtype) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        for r in range(world):
-            RM.as_bytes(bufs[r])[:n].copy_(RM.as_bytes(xs[r]))
-        outs = bufs
-    else:
-        src = [torch.cat([RM.as_bytes(xs[r]), RM.as_bytes(GD._sentinel(tail, dtype, "cpu"))]).cuda().view(dtype)
-               for r in range(world)]
-        dst = [GD._sentinel(seg + tail, dtype) for _ in range(world)]
-        outs = dst
-    src_before = [RM.as_bytes(s).cpu() if s is not None else None for s in src]
-    want = RS.reduce_scatter_model(variant, op, xs, mode, _bytes_cpu(outs), _bytes_cpu(bufs))
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = G._inbox(W, variant)
-    W.launch(_grid(variant, seg_vec, mb),
-             lambda r: C.reduce_scatter(variant, ptrs, W.sig_ptrs, src[r], dst[r], world * seg_vec, r, world, mb, inbox, cap,
-                                        RM.kernel_op(op, dtype), RM.CODES[dtype]))
-    what = (f"reduce-scatter {RS.NAMES[dtype]} {CM.OP_NAMES[op]} {M.VARIANT_NAMES[variant]} world {world} seg_vec {seg_vec} "
-            f"max_blocks {mb} {mode}")
-    any_nan = _any_nan(op, dtype)
-    RM.assert_bits_equal(what + ": output", _bytes_cpu(outs), want["out"], any_nan)
-    RM.assert_bits_equal(what + ": symmetric buffers", _bytes_cpu(bufs), want["buf"], any_nan)
-    if mode != "inplace":
-        RM.assert_bits_equal(what + ": src", _bytes_cpu(src), src_before)
-
-
-def alltoall_call(C, W, variant, seg_vec, mb, mode, seed):
-    world, seg = W.world, seg_vec * 4
-    n = world * seg
-    xs = CM.make_raw_inputs(world, n, seed)
-    bufs = [G._raw_sentinel(n + SGE.SENT) for _ in range(world)]
-    src = [None] * world
-    if mode == "buffer":
-        for r in range(world):
-            bufs[r][:n].copy_(xs[r])
-    else:
-        src = [torch.cat([xs[r], G._raw_sentinel(SGE.SENT, "cpu")]).cuda() for r in range(world)]
-    dst = [G._raw_sentinel(n + SGE.SENT) for _ in range(world)]
-    src_before = [s.cpu() if s is not None else None for s in src]
-    want = RS.alltoall_model(variant, xs, mode, [d.cpu() for d in dst], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = G._inbox(W, variant)
-    W.launch(_grid(variant, seg_vec, mb),
-             lambda r: C.alltoall(variant, ptrs, W.sig_ptrs, src[r], dst[r], n // 4, r, world, mb, inbox, cap))
-    what = f"all-to-all {M.VARIANT_NAMES[variant]} world {world} seg_vec {seg_vec} max_blocks {mb} {mode}"
-    G._check(what + ": output", dst, want["out"], 4)
-    G._check(what + ": symmetric buffers", bufs, want["buf"], 4)
-    if mode != "buffer":
-        G._check(what + ": src", src, src_before, 4)
 
 
 def segment_sizes(variant, mb):
@@ -159,7 +82,7 @@ def test_reduce_scatter_equals_the_all_reduce_slice_on_the_same_inputs(C, sms, w
                 W = E.World(world, sms)
                 ar_bufs = [x.clone() for x in xs]
                 ptrs = [b.data_ptr() for b in ar_bufs]
-                inbox, cap = G._inbox(W, ar_variant)
+                inbox, cap = E._inbox(W, ar_variant)
                 W.launch(M.grid_blocks(ar_variant, world * seg_vec, world, 3),
                          lambda r: C.allreduce(ar_variant, dtype == torch.bfloat16, ptrs, W.sig_ptrs, 0, None, None,
                                                world * seg_vec, 1.0, r, world, 3, inbox, cap, kop, -1, dtype=code))
@@ -167,7 +90,7 @@ def test_reduce_scatter_equals_the_all_reduce_slice_on_the_same_inputs(C, sms, w
                     bufs = [torch.zeros_like(x) for x in xs]
                     outs = [torch.zeros(seg_vec * epv, dtype=dtype, device="cuda") for _ in range(world)]
                     bptrs = [b.data_ptr() for b in bufs]
-                    inbox, cap = G._inbox(W, variant)
+                    inbox, cap = E._inbox(W, variant)
                     W.launch(_grid(variant, seg_vec, 3),
                              lambda r: C.reduce_scatter(variant, bptrs, W.sig_ptrs, xs[r], outs[r], world * seg_vec, r, world,
                                                         3, inbox, cap, kop, code))
@@ -207,37 +130,29 @@ def test_new_calls_share_pads_and_inboxes_with_every_kind_through_the_epoch_wrap
             alltoall_call(C, W, variant, seg_vec, mb, mode, seed)
         elif c[0] == "ar":
             _, variant, op, n_vec, mb, wire, mode, root = c
-            G.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
+            E.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
         elif c[0] == "bc":
             _, variant, n_vec, mb, mode, root = c
-            G.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
+            E.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
         elif c[0] == "ag":
             _, variant, seg_vec, mb, mode = c
-            G.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
+            E.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
         else:
             kind, variant, seg_vec, mb, mode, root = c
-            (SGE.scatter_call if kind == "sc" else SGE.gather_call)(C, W, variant, seg_vec, mb, mode, root, seed)
+            (E.scatter_call if kind == "sc" else E.gather_call)(C, W, variant, seg_vec, mb, mode, root, seed)
     ep = torch.stack([p[M.EPOCH_WORD0:M.EPOCH_WORD0 + M.MAX_BLOCKS] for p in W.pads]).cpu()
     assert bool((ep == ep[0]).all())
     assert 0 < int(ep[0, 0]) < 100
 
 
 # ---------------------------------------------------------------------------------------------------------- SymmWorld
-def _unaligned(x):
-    return SGE._unaligned(x)
-
-
-def _raw(dtype, numel, seed):
-    return SGE._raw(dtype, numel, seed)
-
-
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
 def test_symm_world_reduce_scatter_routes_stages_and_copies_out(C, sms, world):
     """``reduce_scatter_`` of every dtype with tensor and list inputs (one block, separate tensors), ragged segments,
     unaligned tensors, an output that aliases the input's own slice or another whole slice (written in the kernel) or lies
     inside the input at half a segment's offset (through the staging buffer), on both sides of the LL / pull threshold; the
     group's global ranks are not 0..W-1.  Every rank's output is checked bit for bit against the model's segment r."""
-    worlds, keep = G.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
+    worlds, keep = E.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
     for k, numel in enumerate([5, 1024, 3001, 12288, 40000]):
         for d, dtype in enumerate(RS.DTYPES):
             op = OPS[(k + d) % 4]
@@ -267,7 +182,7 @@ def test_symm_world_reduce_scatter_routes_stages_and_copies_out(C, sms, world):
                 args = [[s.clone() for s in x.view(world, numel).unbind(0)] for x in ins]
             else:
                 args = ins
-            G.on_ranks(worlds, lambda r, w: w.reduce_scatter_(outs[r], args[r], op))
+            E.on_ranks(worlds, lambda r, w: w.reduce_scatter_(outs[r], args[r], op))
             RM.assert_bits_equal(f"reduce_scatter_ {RS.NAMES[dtype]} {CM.OP_NAMES[op]} {numel} {form} unaligned {unaligned}",
                                  _bytes_cpu(outs), want, _any_nan(op, dtype))
     w0 = worlds[0]
@@ -291,7 +206,7 @@ def test_symm_world_all_to_all_routes_stages_and_copies_out(C, sms, world):
     """``all_to_all_`` of int64 / bf16 / uint8 payloads at ragged sizes, aligned and unaligned, an output that is the input
     (ragged through the staging buffer; aligned in place in the kernel, pull and LL), and segments of LL_CAP_VEC and
     LL_CAP_VEC + 1 vectors (the last one LL can take, the first it cannot)."""
-    worlds, keep = G.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
+    worlds, keep = E.symm_worlds(world, sms, [10 + 3 * r for r in range(world)])
     for k, numel in enumerate([5, 1024, 3001, 12288, 40000, 16 * M.LL_CAP_VEC, 16 * (M.LL_CAP_VEC + 1), 512]):
         dtype = [torch.int64, torch.bfloat16, torch.uint8][k % 3] if k < 5 else torch.uint8
         unaligned = k % 3 == 1 and k < 5
@@ -303,11 +218,11 @@ def test_symm_world_all_to_all_routes_stages_and_copies_out(C, sms, world):
         if unaligned:
             ins = [_unaligned(x) for x in ins]
             outs = [_unaligned(o) for o in outs]
-        G.on_ranks(worlds, lambda r, w: w.all_to_all_(outs[r], ins[r]))
+        E.on_ranks(worlds, lambda r, w: w.all_to_all_(outs[r], ins[r]))
         for r in range(world):
-            assert G._bits_equal(outs[r], want[r]), ("all_to_all_", dtype, numel, unaligned, same, r)
+            assert E._bits_equal(outs[r], want[r]), ("all_to_all_", dtype, numel, unaligned, same, r)
             if not same:
-                assert G._bits_equal(ins[r], xs[r]), ("all_to_all_: input changed", numel, r)
+                assert E._bits_equal(ins[r], xs[r]), ("all_to_all_: input changed", numel, r)
     w0 = worlds[0]
     if world > 1:
         with pytest.raises(ValueError, match="multiple of world"):

@@ -1,11 +1,10 @@
 """FlatRMSprop's kernels on one GPU: every instance of ``rmsprop_flat`` (csrc/rmsprop.cu) bit for bit against
 tests/rmsprop_model.py with sentinels behind every buffer, the clip / scaled / grouped / capturable instances against the plain
 one fed the same scalars, the kernel against ``torch.optim.RMSprop`` on CUDA and fp64, the RMSprop instances of the sharded
-kernel (csrc/sharded_sgd.cu) at emulated worlds 1-8 (the harness of tests/test_gpu_sharded_sgd_emulated.py), a captured
+kernel (csrc/sharded_sgd.cu) at emulated worlds 1-8 (the harness of tests/emulated_ranks.py), a captured
 DDP step against eager steps, and a ResNet-18 trained through ``DistributedDataParallel`` + ``FlatRMSprop`` under bf16
 autocast."""
 import math
-import os
 
 import pytest
 import torch
@@ -14,7 +13,7 @@ import comm_model as M
 import rmsprop_model as R
 import sharded_sgd_model as S
 from adamw_model import clip_coef, f32
-from test_gpu_sharded_sgd_emulated import World, _untouched, _with_sentinel
+from emulated_ranks import CO_RESIDENT, C, World, _bits, _untouched, _with_sentinel, sms  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -22,28 +21,11 @@ SIZES = [1, 2, 3, 4, 5, 6, 7, 1023, 1024, 1025, 1026, 1027, 256 * 4 * 7 + 3, 1 <
 # (momentum, centered, weight decay): every momentum x centered combination, decay on in two of them
 OPTIONS = [(0.0, False, 0.0), (0.9, False, 0.05), (0.0, True, 0.05), (0.9, True, 0.0)]
 HP = dict(lr=0.01, alpha=0.9, eps=1e-3)
-SERIAL = pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
-                            reason="serialized launches: the ranks' grids must be co-resident")
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _sc(opt, lr=HP["lr"]):
     mu, _, wd = opt
     return R.scalars64(lr, HP["alpha"], HP["eps"], wd, mu)
-
-
-def _bits(a, b):
-    return torch.equal(a.cpu().view(torch.int32), b.cpu().view(torch.int32))
 
 
 def _state(n, seed):
@@ -405,14 +387,14 @@ def _cases(world, sms):
     return out
 
 
-@SERIAL
+@CO_RESIDENT
 @pytest.mark.parametrize("world", range(1, 9))
 def test_sharded_rmsprop_matches_the_model_bit_for_bit(C, sms, world):
     for k, (n_vec, mb, wire, zero_grad, opt, kind) in enumerate(_cases(world, sms)):
         run_sharded(C, World(world, sms), n_vec, mb, wire, zero_grad, opt, kind, seed=100 * world + k)
 
 
-@SERIAL
+@CO_RESIDENT
 @pytest.mark.parametrize("world", range(1, 9))
 def test_sharded_rmsprop_fp32_equals_allreduce_then_rmsprop_flat(C, sms, world):
     big = (524288 + world - 1) // world * world

@@ -1,7 +1,7 @@
 """Scatter from a root and gather to a root (csrc/allreduce.cu) on ONE GPU with W emulated ranks, bit for bit against
 tests/scatter_gather_model.py.
 
-The harness is tests/test_gpu_comm_emulated.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
+The harness is tests/emulated_ranks.py's: each rank has its own buffers, signal pad, LL inbox and stream, the W
 launches go out back to back, and no case runs more CTAs than the GPU has SMs.  Outputs, symmetric buffers, the sentinels
 behind them and every src are compared whole, so "a non-root leaves its output alone", "a non-root's src is never read" and
 "src is left untouched" are checked too.  The last tests drive ``SymmWorld.scatter_`` / ``gather_`` for W ranks built over
@@ -12,79 +12,9 @@ import torch
 
 import collectives_model as CM
 import comm_model as M
-import scatter_gather_model as SG
-import test_gpu_collectives_emulated as G
-import test_gpu_comm_emulated as E
-
-pytestmark = E.pytestmark
-
-VARIANTS, VARIANT_IDS = G.VARIANTS, G.VARIANT_IDS
-C = E.C
-sms = E.sms
-SENT = 4 * E.SENT_VECS                            # sentinel words behind every buffer
-
-
-def _launch_blocks(kind, variant, seg_vec, world, mb):
-    """The launcher's grid: LL and the one-shot scatter by one segment, the rest like an all-gather of world segments."""
-    by_seg = variant == M.LL or (kind == "scatter" and variant == M.ONESHOT)
-    return M.grid_blocks(variant, seg_vec if by_seg else world * seg_vec, world, mb)
-
-
-def gather_call(C, W, variant, seg_vec, mb, mode, root, seed):
-    world, seg = W.world, seg_vec * 4
-    n_vec = world * seg_vec
-    xs = CM.make_raw_inputs(world, seg, seed)
-    bufs = [G._raw_sentinel(world * seg + SENT) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        for r in range(world):
-            bufs[r][r * seg:(r + 1) * seg].copy_(xs[r])
-        outs = bufs
-    else:
-        src = [torch.cat([xs[r], G._raw_sentinel(SENT, "cpu")]).cuda() for r in range(world)]
-        dst = [G._raw_sentinel(world * seg + SENT) for _ in range(world)]
-        outs = dst
-    src_before = [s.cpu() if s is not None else None for s in src]
-    want = SG.gather_model(variant, xs, root, mode, [o.cpu() for o in outs], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = G._inbox(W, variant)
-    W.launch(_launch_blocks("gather", variant, seg_vec, world, mb),
-             lambda r: C.gather(variant, ptrs, W.sig_ptrs, src[r], dst[r], n_vec, root, r, world, mb, inbox, cap))
-    what = f"gather root {root} {M.VARIANT_NAMES[variant]} world {world} per-rank vectors {seg_vec} max_blocks {mb} {mode}"
-    G._check(what + ": output", outs, want["out"], 4)
-    G._check(what + ": symmetric buffers", bufs, want["buf"], 4)
-    if mode != "inplace":
-        G._check(what + ": src", src, src_before, 4)
-
-
-def scatter_call(C, W, variant, seg_vec, mb, mode, root, seed):
-    """The root's src holds the world segments; every other rank passes a src of the same size holding other words, which
-    must neither be read (the outputs would show it) nor written."""
-    world, seg = W.world, seg_vec * 4
-    n_vec = world * seg_vec
-    xs = CM.make_raw_inputs(world, seg, seed)
-    decoy = CM.make_raw_inputs(world, seg, seed + 1)
-    bufs = [G._raw_sentinel(world * seg + SENT) for _ in range(world)]
-    src = dst = [None] * world
-    if mode == "inplace":
-        bufs[root][:world * seg].copy_(torch.cat(xs))
-        outs = bufs
-    else:
-        src = [torch.cat(xs + [G._raw_sentinel(SENT, "cpu")]).cuda() if r == root else
-               torch.cat(decoy + [G._raw_sentinel(SENT, "cpu")]).cuda() for r in range(world)]
-        dst = [G._raw_sentinel(seg + SENT) for _ in range(world)]
-        outs = dst
-    src_before = [s.cpu() if s is not None else None for s in src]
-    want = SG.scatter_model(variant, xs, root, mode, [o.cpu() for o in outs], [b.cpu() for b in bufs])
-    ptrs = [b.data_ptr() for b in bufs]
-    inbox, cap = G._inbox(W, variant)
-    W.launch(_launch_blocks("scatter", variant, seg_vec, world, mb),
-             lambda r: C.scatter(variant, ptrs, W.sig_ptrs, src[r], dst[r], n_vec, root, r, world, mb, inbox, cap))
-    what = f"scatter root {root} {M.VARIANT_NAMES[variant]} world {world} per-rank vectors {seg_vec} max_blocks {mb} {mode}"
-    G._check(what + ": output", outs, want["out"], 4)
-    G._check(what + ": symmetric buffers", bufs, want["buf"], 4)
-    if mode != "inplace":
-        G._check(what + ": src", src, src_before, 4)
+import emulated_ranks as E
+from emulated_ranks import (C, VARIANT_IDS, VARIANTS, _raw, _unaligned, gather_call, pytestmark,  # noqa: F401
+                            scatter_call, sms)
 
 
 def segment_sizes(kind, variant, world, mb):
@@ -147,13 +77,13 @@ def test_scatter_and_gather_share_pads_and_inboxes_with_every_kind_through_the_e
             W.launch(1, lambda r: C.barrier(W.sig_ptrs, r, world))
         elif c[0] == "ar":
             _, variant, op, n_vec, mb, wire, mode, root = c
-            G.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
+            E.reduce_call(C, W, variant, op, n_vec, mb, wire, mode, wire, root, seed)
         elif c[0] == "bc":
             _, variant, n_vec, mb, mode, root = c
-            G.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
+            E.broadcast_call(C, W, variant, n_vec, mb, mode, root, seed)
         elif c[0] == "ag":
             _, variant, seg_vec, mb, mode = c
-            G.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
+            E.allgather_call(C, W, variant, seg_vec, mb, mode, seed)
         else:
             kind, variant, seg_vec, mb, mode, root = c
             (scatter_call if kind == "sc" else gather_call)(C, W, variant, seg_vec, mb, mode, root, seed)
@@ -163,13 +93,6 @@ def test_scatter_and_gather_share_pads_and_inboxes_with_every_kind_through_the_e
 
 
 # ---------------------------------------------------------------------------------------------------------- SymmWorld
-def _raw(dtype, numel, seed):
-    g = torch.Generator().manual_seed(seed)
-    if dtype == torch.bfloat16:
-        return CM.make_raw_inputs(1, (numel + 1) // 2, seed)[0].view(torch.bfloat16)[:numel].clone()
-    return torch.randint(-2 ** 62, 2 ** 62, (numel,), generator=g, dtype=torch.int64).to(dtype)
-
-
 def _lists(world, numel, dtype, block):
     """world outputs per rank: views of one block, or separate tensors."""
     if block:
@@ -178,21 +101,13 @@ def _lists(world, numel, dtype, block):
     return [[torch.zeros(numel, dtype=dtype, device="cuda") for _ in range(world)] for _ in range(world)]
 
 
-def _unaligned(x):
-    """``x`` on the GPU as a view that starts 1 element into its storage (a data pointer not 16-byte aligned)."""
-    base = torch.zeros(x.numel() + 1, dtype=x.dtype, device="cuda")
-    v = base[1:]
-    v.copy_(x)
-    return v
-
-
 @pytest.mark.parametrize("world", [1, 2, 3, 5, 8])
 def test_symm_world_scatter_and_gather_route_stage_and_copy_out(C, sms, world):
     """int64 / bf16 / uint8 at sizes on both sides of the LL and one-shot thresholds and ragged ones, block and separate
     lists, aligned and unaligned tensors; roots given as global ranks of a group whose ranks are not 0..W-1.  A non-root's
     list is never read or written."""
     globals_ = [10 + 3 * r for r in range(world)]
-    worlds, keep = G.symm_worlds(world, sms, globals_)
+    worlds, keep = E.symm_worlds(world, sms, globals_)
     for k, numel in enumerate([5, 1024, 3001, 12288, 40000, 24000, 60001]):
         dtype = [torch.int64, torch.bfloat16, torch.uint8][k % 3]
         root = [0, world - 1, world // 2][k % 3]
@@ -208,11 +123,11 @@ def test_symm_world_scatter_and_gather_route_stage_and_copy_out(C, sms, world):
         ts = [torch.zeros(numel, dtype=dtype, device="cuda") for _ in range(world)]
         if unaligned:
             ts = [_unaligned(t) for t in ts]
-        G.on_ranks(worlds, lambda r, w: w.scatter_(ts[r], lists[r], globals_[root]))
+        E.on_ranks(worlds, lambda r, w: w.scatter_(ts[r], lists[r], globals_[root]))
         for r in range(world):
-            assert G._bits_equal(ts[r], segs[r]), ("scatter", dtype, numel, block, unaligned, r)
+            assert E._bits_equal(ts[r], segs[r]), ("scatter", dtype, numel, block, unaligned, r)
             for s in range(world):
-                assert G._bits_equal(lists[r][s], segs[s] if r == root else decoy), ("scatter: list written", numel, r, s)
+                assert E._bits_equal(lists[r][s], segs[s] if r == root else decoy), ("scatter: list written", numel, r, s)
         # gather: rank r's tensor lands in the root's list; the others' lists are left alone
         ins = [segs[r].cuda() for r in range(world)]
         if unaligned:
@@ -221,18 +136,18 @@ def test_symm_world_scatter_and_gather_route_stage_and_copy_out(C, sms, world):
         for r in range(world):
             for s in range(world):
                 outs[r][s].copy_(decoy)
-        G.on_ranks(worlds, lambda r, w: w.gather_(ins[r], outs[r] if r == root else None, globals_[root]))
+        E.on_ranks(worlds, lambda r, w: w.gather_(ins[r], outs[r] if r == root else None, globals_[root]))
         for r in range(world):
             for s in range(world):
-                assert G._bits_equal(outs[r][s], segs[s] if r == root else decoy), ("gather", dtype, numel, block, r, s)
-            assert G._bits_equal(ins[r], segs[r]), ("gather: input changed", numel, r)
+                assert E._bits_equal(outs[r][s], segs[s] if r == root else decoy), ("gather", dtype, numel, block, r, s)
+            assert E._bits_equal(ins[r], segs[r]), ("gather: input changed", numel, r)
     del keep
 
 
 def test_symm_world_refuses_a_bad_root_list_before_any_launch(C, sms):
     """World 1: the root's list of the wrong length, dtype or size raises (as torch does), and so does a root outside the
     world; nothing is launched."""
-    worlds, keep = G.symm_worlds(1, sms, [4])
+    worlds, keep = E.symm_worlds(1, sms, [4])
     w = worlds[0]
     t = torch.zeros(8, dtype=torch.int64, device="cuda")
     for fn in (w.scatter_, w.gather_):

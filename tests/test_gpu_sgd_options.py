@@ -1,6 +1,6 @@
 """GPU tier: weight decay and Nesterov momentum in the optimizer kernels (csrc/sgd_device.cuh, csrc/sgd.cu).
 
-* both exchange flavours of ``allreduce_sgd`` at emulated worlds 1-8 (the harness of tests/test_gpu_comm_emulated.py),
+* both exchange flavours of ``allreduce_sgd`` at emulated worlds 1-8 (the harness of tests/emulated_ranks.py),
   bit for bit against the model, through the uint32 epoch wrap;
 * every engine path -- the one-GPU slot path, the cluster path, ``deterministic=True``, the batched engine and
   ``sgd_flat`` -- bit for bit against an fp32 oracle that applies the update with exact fmaf to the gradient the engine
@@ -8,8 +8,6 @@
 * graph replays, ``run_native`` and eager steps agree bit for bit, with and without an lr schedule; explicit defaults
   equal no options; a resumed checkpoint continues bit-equal; two GPUs over the push exchange.
 """
-import os
-
 import pytest
 import torch
 
@@ -19,26 +17,16 @@ import sgd_options_workers as SW
 import dist_tuto.pth_b200 as b2
 from dist_tuto.pth_b200 import LRSchedule
 from dist_tuto.pth_b200 import data as D
-from test_gpu_comm_emulated import World
+from emulated_ranks import SERIALIZED, C, World, sms  # noqa: F401
+from engine_paths import Spy, _batches, _slot_trainer, _state
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900),
-              pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
+              pytest.mark.skipif(SERIALIZED,
                                  reason="serialized launches: every emulated rank's grid would spin alone until it traps")]
 
 OPTIONS = [(1e-2, False), (0.0, True), (1e-2, True)]
 OPT_IDS = ["wd", "nesterov", "wd+nesterov"]
 SCHED = LRSchedule(warmup_steps=4, decay="multistep", milestones=[7], gamma=0.5)
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.fixture(scope="module")
@@ -123,50 +111,6 @@ def test_options_across_the_uint32_epoch_wrap(C, sms, world, exchange):
 
 
 # --------------------------------------------------------------------------------------------- engine paths
-class Spy:
-    """Wraps a trainer's extension handle: before each optimizer launch it records the parameters, the momentum and the
-    averaged gradient that launch will apply -- the bucket of this step's parity for ``allreduce_sgd``, and for
-    ``reduce_sgd`` (whose gradient never leaves registers) the momentum of a plain launch with mu = 0 and lr = 0 on copies,
-    which is the fixed-order reduction of the same slots.  Eager steps only (graph capture would record the copies)."""
-
-    def __init__(self, tr):
-        self._C, self.tr, self.log = tr.C, tr, []
-        tr.C = self
-
-    def __getattr__(self, name):
-        return getattr(self._C, name)
-
-    def _grad_of_bucket(self, stride):
-        from dist_tuto.pth_b200.ops.convnet_fused import NPAR_ALLOC
-        cur = int(self.tr.step_counter.item()) & 1 if stride > 0 else 0
-        return M.reduce_scaled([self.tr.grads[cur * NPAR_ALLOC:cur * NPAR_ALLOC + NPAR_ALLOC]], 1.0)   # 0 + bucket, as the kernel
-
-    def allreduce_sgd(self, grads, sigs, params, momentum, step, lr, mu, scale, rank, world, zero_grads, grad_stride, *a, **k):
-        torch.cuda.current_stream().synchronize()
-        assert world == 1 and scale == 1.0
-        self.log.append((params.clone(), momentum.clone(), self._grad_of_bucket(grad_stride), int(step.item())))
-        return self._C.allreduce_sgd(grads, sigs, params, momentum, step, lr, mu, scale, rank, world, zero_grads, grad_stride,
-                                     *a, **k)
-
-    def reduce_sgd(self, slots, n_slots, factors, n_samples, params, momentum, step, *a, **k):
-        torch.cuda.current_stream().synchronize()
-        g = torch.zeros_like(momentum)
-        self._C.reduce_sgd(slots, n_slots, factors, n_samples, params.clone(), g, None, None, 0.0, 0.0)
-        torch.cuda.current_stream().synchronize()
-        self.log.append((params.clone(), momentum.clone(), g, int(step.item())))
-        return self._C.reduce_sgd(slots, n_slots, factors, n_samples, params, momentum, step, *a, **k)
-
-
-def _batches(n, bsz, seed, raw=True):
-    g = torch.Generator().manual_seed(seed)
-    out = []
-    for _ in range(n):
-        x = torch.randint(0, 256, (bsz, 1, 28, 28), generator=g, dtype=torch.uint8) if raw else \
-            torch.randn(bsz, 1, 28, 28, generator=g)
-        out.append((x, torch.randint(0, 10, (bsz,), generator=g)))
-    return out
-
-
 def _check_against_oracles(tr, spy, lr, sched, wd, nesterov):
     """Each logged launch against the exact fp32 update (bit for bit), and the whole run against fp64 torch.optim.SGD on
     the same gradients: |p - p64| <= 2^-16 * (|p64| + 1) after the run's steps (fp32 rounding of every operation, with
@@ -236,17 +180,6 @@ def test_sgd_flat_matches_the_fp32_oracle(C, n, wd, nesterov):
 
 
 # --------------------------------------------------------------------------------------------- launch paths
-def _slot_trainer(dev, **kw):
-    from dist_tuto.pth_b200.ops.convnet_fused import FusedTrainer
-    return FusedTrainer(128, lr=0.05, seed=11, device=dev, raw_uint8=True, **kw)
-
-
-def _state(tr):
-    tr.sync_lag(0)
-    torch.cuda.synchronize()
-    return tr.params.clone(), tr.momentum.clone(), float(tr.loss_acc[0].item()), int(tr.step_counter.item())
-
-
 @pytest.mark.parametrize("sched", [None, SCHED], ids=["const", "schedule"])
 def test_graph_native_and_eager_steps_are_bit_equal(dev, sched):
     ds = D.SyntheticMNIST(n=12 * 128, seed=4)

@@ -2,41 +2,26 @@
 
 ``C.sharded_lamb`` / ``C.sharded_lars`` take raw per-rank pointers, so W "ranks" are W sets of buffers on one device, each
 with its own gradient bucket, parameter flat, sums buffer, table, workspaces, state shards, signal pad and stream (the
-``World`` harness of tests/test_gpu_sharded_sgd_emulated.py: the W launches go out back to back on W streams, and
+``World`` harness of tests/emulated_ranks.py: the W launches go out back to back on W streams, and
 ``world x blocks <= SM count`` is asserted before any launch).  Every rank's parameters, state shards, ratios and gradient
 bucket are compared bit for bit with tests/sharded_layerwise_model.py after each of 3 steps with fresh gradients, sentinels
 sit behind every buffer, the tickets are zero after every call, and every rank writes the same ratios.  For fp32 buckets the
 tensors inside one slice also equal the one-shot and two-shot all-reduce followed by ``lamb_flat`` / ``lars_flat``.
 """
-import os
-
 import pytest
 import torch
 
 import comm_model as M
 import sharded_layerwise_model as S
 import sharded_sgd_model as SM
-from test_gpu_sharded_sgd_emulated import World, _untouched, _with_sentinel
+from emulated_ranks import C, SERIAL_SKIP, World, _untouched, _with_sentinel, sms  # noqa: F401
 
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800),
-              pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
-                                 reason="serialized launches: every rank's grid would spin alone until it traps")]
+pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800), SERIAL_SKIP]
 
 CHUNK = S.CHUNK
 LAMB_HP = dict(lr=2e-2, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01)
 LARS_HP = dict(lr=0.1, momentum=0.9, weight_decay=1e-4, trust_coefficient=1e-3, eps=1e-8, nesterov=True)
 SUMS_SENTINEL = 12345.0
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def lay(numels, n_vec_min=0, world=1, epv=4):

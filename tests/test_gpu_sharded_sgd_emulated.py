@@ -7,74 +7,18 @@ bit with the model of tests/sharded_sgd_model.py and, for fp32 buckets, with the
 ``C.sgd_flat``) run on the same inputs.  What it cannot cover (the memory model across NVLink and the symmetric mappings) is
 in tests/test_gpu_sharded_sgd_multi.py.
 
-Every CTA spins on its peers, so the W grids of one call must be co-resident: the W launches go out back to back on W streams
-between two device synchronisations, ``world x blocks <= SM count`` is asserted before any launch, and the file is skipped
-under CUDA_LAUNCH_BLOCKING=1 (with serialized launches the first rank's grid would spin alone until it traps).
+The W grids of one call must be co-resident; tests/emulated_ranks.py's ``World`` issues them back to back on W streams and
+asserts ``world x blocks <= SM count`` before any launch.
 """
-import os
-
 import pytest
 import torch
 
 import comm_model as M
 import sharded_sgd_model as S
+from emulated_ranks import C, WRAP, World, _untouched, _with_sentinel, pytestmark, sms  # noqa: F401
 
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900),
-              pytest.mark.skipif(os.environ.get("CUDA_LAUNCH_BLOCKING") == "1",
-                                 reason="serialized launches: every rank's grid would spin alone until it traps")]
-
-SENT_VECS = 3                                   # sentinel vectors behind every buffer
-SENTINEL = {torch.float32: 0x5EADBEEF, torch.bfloat16: 0x5EAD}     # finite bit patterns no result can produce here
-WRAP = 2 ** 32 - 5                              # epoch-wrap test: every pad's epoch and flag words start here
 OPTIONS = [(0.0, False), (0.01, False), (0.0, True), (0.01, True)]  # (weight decay, nesterov)
 LR, MU = 0.07, 0.9
-
-
-@pytest.fixture(scope="module")
-def C():
-    from dist_tuto.pth_b200.ops import _ext
-    return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _with_sentinel(x, dtype=None):
-    """``x`` on the GPU followed by SENT_VECS sentinel vectors."""
-    dtype = dtype or x.dtype
-    epv = M.elems_per_vec(dtype)
-    bits = torch.full((SENT_VECS * epv,), SENTINEL[dtype], dtype=torch.int32 if dtype == torch.float32 else torch.int16)
-    return torch.cat([x.to(dtype), bits.view(dtype)]).cuda()
-
-
-def _untouched(t):
-    ib = torch.int32 if t.dtype == torch.float32 else torch.int16
-    return bool((t.view(ib) == SENTINEL[t.dtype]).all())
-
-
-class World:
-    """W emulated ranks on cuda:0: a signal pad (uint32 [B2_SIGNAL_WORDS]) and a stream per rank."""
-
-    def __init__(self, world, sms, pad_start=0):
-        self.world, self.sms = world, sms
-        self.pads = [torch.zeros(M.SIGNAL_WORDS, dtype=torch.int32, device="cuda") for _ in range(world)]
-        if pad_start:
-            for p in self.pads:                   # per-block epoch words and every flag word
-                p[:M.EPOCH_WORD0 + M.MAX_BLOCKS] = pad_start - 2 ** 32 if pad_start >= 2 ** 31 else pad_start
-        self.streams = [torch.cuda.Stream() for _ in range(world)]
-        self.sig_ptrs = [p.data_ptr() for p in self.pads]
-
-    def launch(self, blocks, fn):
-        """fn(r) issues rank r's kernel.  All W launches go out back to back, each on its own stream."""
-        assert self.world * blocks <= self.sms, (
-            f"{self.world} ranks x {blocks} CTAs would not be co-resident on {self.sms} SMs; not launched")
-        torch.cuda.synchronize()
-        for r in range(self.world):
-            with torch.cuda.stream(self.streams[r]):
-                fn(r)
-        torch.cuda.synchronize()
 
 
 def run_steps(C, W, n_vec, max_blocks, wire, wd, nesterov, zero_grad, seed, steps=3, against_kernels=False):

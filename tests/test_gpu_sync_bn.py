@@ -4,7 +4,7 @@
   C in {1, 3, 64, 512, 2049}, N x L from 2 through the ResNet stem, odd sizes for every tail, a grid cap that makes CTAs
   stride over tiles; every output against fp64 within c 2^-24 (|x k1| + |k0|) plus the output's rounding, sentinels behind
   every output, two runs bit-identical;
-* emulated ranks, worlds 1-8 on one GPU (tests/test_gpu_collectives_emulated.symm_worlds, one stream per rank): forward and
+* emulated ranks, worlds 1-8 on one GPU (tests/emulated_ranks.symm_worlds, one stream per rank): forward and
   backward through ``SyncBatchNormFunction`` with uneven and zero local batches; mean, invstd and running stats bit-identical
   on every rank and within the bound of the fp64 global reference;
 * the module at world size 1: against cuDNN ``BatchNorm2d``, no host synchronisation (``momentum=None`` included), a
@@ -16,12 +16,11 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 import dist_tuto.pth_b200 as b2
+import emulated_ranks as E
 import sync_bn_checks as S
-import test_gpu_collectives_emulated as CE
-import test_gpu_comm_emulated as E
 from dist_tuto.pth_b200.parallel.sync_bn import SyncBatchNormFunction, exchange_numel
+from emulated_ranks import pytestmark, sms  # noqa: F401
 
-pytestmark = E.pytestmark
 SENT = -12345.0
 
 
@@ -29,11 +28,6 @@ SENT = -12345.0
 def K():
     from dist_tuto.pth_b200.ops import _ext
     return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _fmt(shape, cl):
@@ -169,8 +163,8 @@ def _emulated_case(worlds, sizes, C, spatial, dtype, cl, momentum, seed):
     def bwd(r, world):
         grads[r] = torch.autograd.grad(ys[r], [xs[r], w, b], dys[r], retain_graph=True)
 
-    CE.on_ranks(worlds, fwd)
-    CE.on_ranks(worlds, bwd)
+    E.on_ranks(worlds, fwd)
+    E.on_ranks(worlds, bwd)
     stats = [y.grad_fn.saved_tensors[2] for y in ys]
     for r in range(1, W):
         for a, bb, what in ((stats[r], stats[0], "mean / invstd / N"), (rms[r], rms[0], "running_mean"),
@@ -211,12 +205,12 @@ def _emulated_case(worlds, sizes, C, spatial, dtype, cl, momentum, seed):
 @pytest.mark.parametrize("world", range(1, 9))
 def test_emulated_ranks_share_bit_identical_statistics(sms, world):
     # every kernel instance runs once at world 1 first: a module loaded lazily while a peer's kernel spins may wait for it
-    warm = CE.symm_worlds(1, sms, [0])
+    warm = E.symm_worlds(1, sms, [0])
     cases = [(64, (5, 6), torch.bfloat16, True, 0.1), (3, (7,), torch.float32, False, None),
              (130, (), torch.float16, False, 0.2)]
     for k, (C, spatial, dtype, cl, mom) in enumerate(cases):
         _emulated_case(warm[0], [4], C, spatial, dtype, cl, mom, k)
-    worlds, keep = CE.symm_worlds(world, sms, list(range(world)))
+    worlds, keep = E.symm_worlds(world, sms, list(range(world)))
     for k, (C, spatial, dtype, cl, mom) in enumerate(cases):
         sizes = [(3 * r + k) % 5 for r in range(world)]
         sizes[0] = max(sizes[0], 2)                      # the global batch holds more than one value per channel

@@ -13,7 +13,7 @@ fp64 reference and bounds of tests/sync_bn_checks.py.
   eval: affine x track_running_stats x momentum in {0.1, None}; and every branch of ``SyncBatchNormFunction``: a contiguous
   ``dy`` for a channels-last ``x`` and the reverse, a channel slice, ``x`` without grad (``bn_backward_reduce`` only), frozen
   affine parameters, a zero weight, and a bias without a weight.
-* Emulated ranks, worlds 1-8 (tests/test_gpu_collectives_emulated.symm_worlds): no affine, no running stats, mixed dtypes,
+* Emulated ranks, worlds 1-8 (tests/emulated_ranks.symm_worlds): no affine, no running stats, mixed dtypes,
   misaligned local inputs and a zero-size local batch; y and dx within the world-1 bound of the global batch, the
   parameters' gradients within it of each rank's local sums, statistics and running stats bit-identical across ranks.
 * A global count of one at world >= 2: the running var is NaN, as torch's ``batch_norm_gather_stats_with_counts`` makes it
@@ -25,14 +25,13 @@ import torch
 import torch.nn as nn
 
 import dist_tuto.pth_b200 as b2
+import emulated_ranks as E
 import sync_bn_checks as S
-import test_gpu_collectives_emulated as CE
-import test_gpu_comm_emulated as E
 from dist_tuto.pth_b200.ops import _ext
 from dist_tuto.pth_b200.parallel import sync_bn as SB
 from dist_tuto.pth_b200.parallel.sync_bn import SyncBatchNormFunction, exchange_numel
+from emulated_ranks import pytestmark, sms  # noqa: F401
 
-pytestmark = E.pytestmark
 SENT = -12345.0
 DT = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
 # (input, parameter, running-stat) dtypes: each of the latter two fp32 or the input's
@@ -43,11 +42,6 @@ TRIPLES = ["fp32-fp32-fp32", "bf16-fp32-fp32", "bf16-bf16-fp32", "bf16-fp32-bf16
 @pytest.fixture(scope="module")
 def K():
     return _ext.C()
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _fmt(ndim, cl):
@@ -470,8 +464,8 @@ def emulated_case(worlds, sizes, case, seed, x_grad=True):
     def bwd_(r, world):
         grads[r] = torch.autograd.grad(ys[r], ([xs[r]] if x_grad else []) + wants, dys[r], retain_graph=True)
 
-    CE.on_ranks(worlds, fwd_)
-    CE.on_ranks(worlds, bwd_)
+    E.on_ranks(worlds, fwd_)
+    E.on_ranks(worlds, bwd_)
     stats = [y.grad_fn.saved_tensors[2] for y in ys]
     for r in range(1, W):
         for a, bb, what in ((stats[r], stats[0], "mean / invstd / N"), (rms[r], rms[0], "running_mean"),
@@ -501,12 +495,12 @@ def emulated_case(worlds, sizes, case, seed, x_grad=True):
 @pytest.mark.parametrize("world", range(1, 9))
 def test_emulated_ranks_new_configurations(sms, world, monkeypatch):
     # every kernel instance runs once at world 1 first: a module loaded lazily while a peer's kernel spins may wait for it
-    warm = CE.symm_worlds(1, sms, [0])
+    warm = E.symm_worlds(1, sms, [0])
     for k, case in enumerate(EMU_CASES):
         emulated_case(warm[0], [4], case, k)
         if case[5]:
             emulated_case(warm[0], [4], case, k, x_grad=False)
-    worlds, keep = CE.symm_worlds(world, sms, list(range(world)))
+    worlds, keep = E.symm_worlds(world, sms, list(range(world)))
     for k, case in enumerate(EMU_CASES):
         sizes = [(2 * r + k + 1) % 4 for r in range(world)]
         sizes[0] = max(sizes[0], 2)                      # the global batch holds more than one value per channel
@@ -527,10 +521,10 @@ def test_global_count_of_one(sms, world):
     """One rank holds one value per channel, the others none.  The kernels follow torch's formula: running_var takes
     var N / (N - 1) = 0 / 0, a NaN, where torch's batch_norm_gather_stats_with_counts divides by n - 1 = 0 as well and gets a
     non-finite value; mean, y (= bias) and dx (= 0) stay finite."""
-    warm = CE.symm_worlds(1, sms, [0])
+    warm = E.symm_worlds(1, sms, [0])
     case = (12, (), "fp32", "fp32", "fp32", True, True, False, 0.1, False)
     emulated_case(warm[0], [4], case, 0)
-    worlds, keep = CE.symm_worlds(world, sms, list(range(world)))
+    worlds, keep = E.symm_worlds(world, sms, list(range(world)))
     C = 12
     g = torch.Generator(device="cuda").manual_seed(world)
     xs = [torch.randn(1 if r == 0 else 0, C, generator=g, device="cuda").requires_grad_(True) for r in range(world)]
@@ -548,8 +542,8 @@ def test_global_count_of_one(sms, world):
     def bwd_(r, wd):
         grads[r] = torch.autograd.grad(ys[r], [xs[r], w, b], dys[r], retain_graph=True)
 
-    CE.on_ranks(worlds, fwd_)
-    CE.on_ranks(worlds, bwd_)
+    E.on_ranks(worlds, fwd_)
+    E.on_ranks(worlds, bwd_)
     fwd = S.forward_ref(xs[0], w, b, rm0, rv0, 0.1)
     assert fwd["N"] == 1 and bool(torch.isnan(fwd["rv"]).all())
     for r in range(world):

@@ -1,15 +1,15 @@
 """The sharded LAMB / LARS model of tests/sharded_layerwise_model.py: within the unsharded model's bound against fp64,
 bit for bit the unsharded model on every tensor that lies inside one slice, and planted faults that the checks catch.
 
-The bound is tests/test_layerwise_model.py's: after 50 updates the largest parameter error against fp64 is at most 4x the
+The bound is tests/layerwise_cases.py's: after 50 updates the largest parameter error against fp64 is at most 4x the
 error of the fp32 torch-op path on the same inputs, plus one fp32 ulp of the largest parameter.  In the bound test rank 0
 holds the whole gradient and the other ranks zeros (scale 1), so the averaged gradient is exact and the fp64 reference is the
 unsharded one; the rank-order average itself is tested with W different gradients in the bit-for-bit tests."""
 import pytest
 import torch
 
+import layerwise_cases as TL
 import sharded_layerwise_model as S
-import test_layerwise_model as TL
 
 WORLDS = [2, 3, 5, 8]
 
@@ -23,7 +23,7 @@ def states0(kind, n):
 
 
 def run_sharded(kind, hp, seed, world, fault=None, chunk=TL.CHUNK, steps=TL.STEPS):
-    """``steps`` sharded updates of tests/test_layerwise_model.py's inputs; returns (params of rank 0, ratios per rank)."""
+    """``steps`` sharded updates of tests/layerwise_cases.py's inputs; returns (params of rank 0, ratios per rank)."""
     offsets, numels, p0, grads = TL.inputs(seed, steps)
     n = padded(p0.numel(), world)
     p = torch.cat([p0, torch.zeros(n - p0.numel())])
