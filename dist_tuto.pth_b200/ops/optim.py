@@ -701,6 +701,54 @@ class _FlatOptimizer:
         per = self._shards[k][2]
         return min(self._rank * per, numel), min((self._rank + 1) * per, numel)
 
+    # ------------------------------------------------------------------ checkpointing
+    # A subclass declares what differs: _state_pairs() gives (state_dict key, flats) of every state buffer (flats empty for
+    # a state its configuration does not keep); _options names the options a state_dict records besides max_grad_norm and
+    # steps; _check_options(sd) raises ValueError unless its constructor would take the options of sd, and returns the
+    # attributes loading them sets; _defaults() and _state_views() where they differ from these.
+    _noun = "state"                                        # what the buffers hold, in the refusal of another rank's shard
+    _carry = "named_state() / load_named_state()"          # the per-name form that crosses world sizes and layouts
+    # the per-name loader's refusal of an entry without a part its tensor's state needs
+    _lacks = "{cls}.load_named_state: the entry of {name!r} has no {key!r}; the state is not this optimizer's"
+
+    def _defaults(self) -> dict:
+        """The values of the keys that state_dicts written before their option existed lack."""
+        return {"max_grad_norm": None}
+
+    def state_dict(self) -> dict:
+        """The options, ``max_grad_norm``, ``steps`` and the state flats (CPU copies), for
+        ``utils.checkpoint.save_checkpoint``.  Sharded over several ranks, the buffers are this rank's shards, and
+        ``sharded`` / ``world`` / ``rank`` say so; with ``param_groups`` the groups are recorded by parameter name.  The form
+        that crosses world sizes and engines is the per-name one (``named_state`` or ``named_momentum``)."""
+        sd = {key: getattr(self, key) for key in self._options}
+        sd.update(max_grad_norm=self.max_grad_norm, steps=self.steps)
+        sd.update((key, [f.detach().cpu().clone() for f in flats]) for key, flats in self._state_pairs())
+        sd.update(self._shard_tags())
+        sd.update(self._group_state())
+        return sd
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Inverse of :meth:`state_dict` (same model => same bucket layout); a state_dict with ``param_groups`` restores each
+        group's lr / weight_decay.  ``ValueError``, before anything is loaded, if its groups hold other parameters than this
+        optimizer's, its options are ones the constructor refuses or that decide other states, its buffers are the shards of
+        another rank or world size, or they have other numbers or sizes."""
+        sd = {**self._defaults(), **sd}
+        self._load_group_state(sd, apply=False)
+        options = self._check_options(sd)
+        max_grad_norm, steps = check_max_grad_norm(sd["max_grad_norm"]), int(sd["steps"])
+        self._check_shard_tags(sd, self._noun, self._carry)
+        whole = self._shard_mode is not None and not sd.get("sharded")    # each rank will take its slice of whole buffers
+        for key, flats in self._state_pairs():
+            if [s.numel() for s in sd[key]] != [self.buckets[k].numel if whole else f.numel() for k, f in enumerate(flats)]:
+                raise ValueError(f"{type(self).__name__}.load_state_dict: the state flats have other sizes than this "
+                                 f"optimizer's (another model or bucket layout); carry the state with {self._carry}")
+        self._load_flats(sd, [(flats, sd[key]) for key, flats in self._state_pairs()], self._noun, self._carry)
+        for attr, value in options.items():
+            setattr(self, attr, value)
+        self.max_grad_norm, self.steps = max_grad_norm, steps
+        self._load_group_state(sd)
+        self._sync_hyperparameters()
+
     def _full_flat(self, k: int, flat: torch.Tensor) -> torch.Tensor:
         """Bucket ``k``'s whole state flat of which ``flat`` is this rank's part; collective in sharded mode (gathers)."""
         from .. import comm
@@ -711,55 +759,115 @@ class _FlatOptimizer:
         comm.all_gather_into_tensor(full, flat, group=self._group)
         return full
 
-    def _named(self, model: nn.Module, flats: List[torch.Tensor]) -> dict:
-        """``{parameter name: its part of the state flats}`` (CPU copies); collective in sharded mode."""
+    def _flat_views(self, k: int, flat: torch.Tensor, i: int, key: str) -> dict:
+        """``{key: tensor i's part of flat}``, ``flat`` a whole flat of bucket ``k`` laid out as the parameters, the part with
+        the tensor's shape and strides."""
+        gb = self.buckets[k]
+        o, gv = gb.offsets[i], gb.views[i]
+        return {key: flat[o:o + gv.numel()].as_strided(gv.shape, gv.stride())}
+
+    _state_views = _flat_views           # the per-tensor parts of a state flat, as the per-name forms hold them
+
+    def _named_parts(self, model: nn.Module, pairs: list, views) -> dict:
+        """``{parameter name: {part: CPU copy}}`` of the parts ``views(k, whole flat, i, key)`` of every tensor in the flats of
+        ``pairs`` = ``[(key, flats)]``; collective in sharded mode (gathers the flats)."""
         names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
         out = {}
-        for k, gb in enumerate(self.buckets):
-            f = self._full_flat(k, flats[k])
-            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
-                if id(p) in names:
-                    out[names[id(p)]] = f[o:o + p.numel()].as_strided(gv.shape, gv.stride()).detach().cpu().clone()
+        for key, flats in pairs:
+            for k, gb in enumerate(self.buckets):
+                full = self._full_flat(k, flats[k])
+                for i, p in enumerate(gb.params):
+                    if id(p) in names:
+                        parts = views(k, full, i, key).items()
+                        out.setdefault(names[id(p)], {}).update((x, v.detach().cpu().clone()) for x, v in parts)
         return out
 
     @torch.no_grad()
+    def _load_parts(self, model: nn.Module, named: dict, pairs: list, views) -> int:
+        """Inverse of :meth:`_named_parts`; returns how many tensors were restored.  ``ValueError`` (:attr:`_lacks`), before
+        anything is written, if an entry lacks a part of its tensor.  Sharded over several ranks, each rank keeps its slice of
+        the full tensors (not collective)."""
+        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
+        sharded = self._shard_mode is not None
+        for check in (True, False):            # every entry is checked before the first write
+            for key, flats in pairs:
+                for k, (gb, mf) in enumerate(zip(self.buckets, flats)):
+                    if sharded:                    # lay the tensors out in a whole flat, then cut this rank's slice out
+                        shard = mf             # (the check needs the parts' names and shapes only: a meta flat)
+                        mf = torch.zeros_like(self._shards[k][3], device="meta" if check else None)
+                        given = torch.zeros_like(mf, dtype=torch.bool)
+                    for i, (p, o) in enumerate(zip(gb.params, gb.offsets)):
+                        src = named.get(names.get(id(p)))
+                        parts = views(k, mf, i, key) if src is not None else {}
+                        missing = [x for x in parts if x not in src]
+                        if missing:
+                            raise ValueError(self._lacks.format(cls=type(self).__name__, name=names[id(p)], key=missing[0],
+                                                                keys=" / ".join(parts)))
+                        if parts and not check:
+                            for x, v in parts.items():
+                                v.copy_(src[x])
+                            if sharded:
+                                given[o:o + p.numel()] = True
+                    if sharded and not check:
+                        lo, per = self._rank * self._shards[k][2], self._shards[k][2]
+                        shard.copy_(torch.where(given[lo:lo + per], mf[lo:lo + per], shard))
+        return sum(named.get(names.get(id(p))) is not None for gb in self.buckets for p in gb.params)
+
+    def _named(self, model: nn.Module, flats: List[torch.Tensor]) -> dict:
+        """``{parameter name: its part of the flats}`` (CPU copies), the flats laid out as the parameters; collective in
+        sharded mode."""
+        return {n: parts["flat"] for n, parts in self._named_parts(model, [("flat", flats)], self._flat_views).items()}
+
     def _load_named(self, model: nn.Module, named: dict, flats: List[torch.Tensor]) -> int:
         """Inverse of :meth:`_named`; returns how many tensors were restored.  Sharded over several ranks, each rank keeps its
         slice of the full tensors (not collective)."""
-        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
-        done = 0
-        for k, (gb, mf) in enumerate(zip(self.buckets, flats)):
-            if self._shard_mode is not None:       # lay the tensors out in a whole flat, then cut this rank's slice out
-                shard = mf
-                mf = torch.zeros_like(self._shards[k][3])
-                given = torch.zeros_like(mf, dtype=torch.bool)
-            for p, o, gv in zip(gb.params, gb.offsets, gb.views):
-                src = named.get(names.get(id(p)))
-                if src is not None:
-                    mf[o:o + p.numel()].as_strided(gv.shape, gv.stride()).copy_(src)
-                    if self._shard_mode is not None:
-                        given[o:o + p.numel()] = True
-                    done += 1
-            if self._shard_mode is not None:
-                lo, per = self._rank * self._shards[k][2], self._shards[k][2]
-                shard.copy_(torch.where(given[lo:lo + per], mf[lo:lo + per], shard))
+        return self._load_parts(model, {n: {"flat": t} for n, t in named.items()}, [("flat", flats)], self._flat_views)
+
+    def _named_state(self, model: nn.Module) -> dict:
+        """``{name: {"step", <state>: tensor, ...}}`` (CPU copies), the torch optimizer's per-parameter state by parameter
+        name: the form that crosses world sizes, bucket layouts, sharded and unsharded runs and the torch optimizer.  Sharded
+        over several ranks this is collective: every rank calls it and gets the full tensors."""
+        step = float(self.steps)
+        parts = self._named_parts(model, [(key, flats) for key, flats in self._state_pairs() if flats], self._state_views)
+        return {n: {"step": torch.tensor(step), **s} for n, s in parts.items()}
+
+    def _load_named_state(self, model: nn.Module, named: dict) -> int:
+        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
+        (common) ``step``.  ``ValueError``, before anything is loaded, if the steps differ or an entry lacks a state its
+        parameter needs.  Sharded over several ranks, each rank keeps its slice (not collective)."""
+        steps = {int(s["step"]) for s in named.values()}
+        if len(steps) > 1:
+            raise ValueError(f"{type(self).__name__} keeps one step count for all parameters; this state has steps "
+                             f"{sorted(steps)}")
+        pairs = [(key, flats) for key, flats in self._state_pairs() if flats]
+        for key, _ in pairs if self._state_views == self._flat_views else []:     # states kept whole: every entry has each
+            lacking = [n for n, s in named.items() if key not in s]
+            if lacking:
+                raise ValueError(self._lacks.format(cls=type(self).__name__, name=lacking[0], key=key, keys=key))
+        done = self._load_parts(model, named, pairs, self._state_views)
+        if done and steps:
+            self.steps = steps.pop()
         return done
 
     def _shard_tags(self) -> dict:
         """What a state_dict records when its buffers are one rank's shards."""
         return dict(sharded=True, world=self._world, rank=self._rank) if self._shard_mode is not None else {}
 
+    def _check_shard_tags(self, sd: dict, noun: str, carry: str) -> None:
+        """``ValueError`` if the buffers of ``sd`` are shards that do not load here: shards load on their own rank of their
+        own world size only.  ``noun`` names the state and ``carry`` the per-name methods that cross world sizes."""
+        if sd.get("sharded") and (self._shard_mode is None or (sd["world"], sd["rank"]) != (self._world, self._rank)):
+            raise ValueError(f"this state_dict holds the {noun} shard of rank {sd['rank']} of {sd['world']}; it loads "
+                             f"into a sharded {type(self).__name__} on that rank of a world of that size only.  To change "
+                             f"the world size or the engine, carry the {noun} with {carry}")
+
     @torch.no_grad()
     def _load_flats(self, sd: dict, pairs: list, noun: str, carry: str) -> None:
         """The buffers of ``sd`` into the state flats, ``pairs`` = [(flats, saved buffers)]: shards load on their own rank of
-        their own world size only; whole buffers of an unsharded optimizer load into a sharded one as this rank's slice.
-        ``noun`` names the state and ``carry`` the per-name methods that cross world sizes."""
-        if sd.get("sharded"):                                    # the buffers are the shards of one rank of one world size
-            if self._shard_mode is None or (sd["world"], sd["rank"]) != (self._world, self._rank):
-                raise ValueError(f"this state_dict holds the {noun} shard of rank {sd['rank']} of {sd['world']}; it loads "
-                                 f"into a sharded {type(self).__name__} on that rank of a world of that size only.  To change "
-                                 f"the world size or the engine, carry the {noun} with {carry}")
-        elif self._shard_mode is not None:                       # whole buffers of an unsharded optimizer: take the slice
+        their own world size only (:meth:`_check_shard_tags`); whole buffers of an unsharded optimizer load into a sharded
+        one as this rank's slice."""
+        self._check_shard_tags(sd, noun, carry)
+        if self._shard_mode is not None and not sd.get("sharded"):   # whole buffers of an unsharded optimizer: the slice
             for flats, saved in pairs:
                 for k, (m, src) in enumerate(zip(flats, saved)):
                     per = self._shards[k][2]
@@ -931,21 +1039,21 @@ class FlatSGD(_FlatOptimizer):
         self._sgd_runs(self._slice_runs(k, lo, n), self._shards[k][3][lo:lo + n], self.momentum_flats[k][:n],
                        self.buckets[k].flat[lo:lo + n])
 
-    def _full_momentum(self, k: int) -> torch.Tensor:
-        """Bucket ``k``'s whole momentum flat; collective in sharded mode (gathers the shards)."""
-        return self._full_flat(k, self.momentum_flats[k])
-
     # ------------------------------------------------------------------ checkpointing
-    def state_dict(self) -> dict:
-        """Hyper-parameters + the flat momentum buffers (CPU copies), for ``utils.checkpoint.save_checkpoint``.  Sharded over
-        several ranks, the buffers are this rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that
-        crosses world sizes and engines is :meth:`named_momentum`."""
-        sd = {"lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay, "nesterov": self.nesterov,
-              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
-              "momentum_buffers": [m.detach().cpu().clone() for m in self.momentum_flats]}
-        sd.update(self._shard_tags())
-        sd.update(self._group_state())
-        return sd
+    _options = ("lr", "momentum", "weight_decay", "nesterov")
+    _noun, _carry = "momentum", "named_momentum() / load_named_momentum()"
+
+    def _state_pairs(self) -> list:
+        return [("momentum_buffers", self.momentum_flats)]
+
+    def _defaults(self) -> dict:
+        # SGD state_dicts written before Nesterov, clipping and the step count: plain momentum, no clipping, steps as they are
+        return {"nesterov": False, "max_grad_norm": None, "steps": self.steps}
+
+    def _check_options(self, sd: dict) -> dict:
+        check_sgd_options(sd["momentum"], sd["weight_decay"], sd["nesterov"])
+        return {"lr": float(sd["lr"]), "momentum": float(sd["momentum"]), "weight_decay": float(sd["weight_decay"]),
+                "nesterov": bool(sd["nesterov"])}
 
     def named_momentum(self, model: nn.Module) -> dict:
         """Momentum per parameter NAME (CPU copies) -- the canonical, engine-independent form written to checkpoints: the
@@ -958,19 +1066,6 @@ class FlatSGD(_FlatOptimizer):
         """Inverse of :meth:`named_momentum`; returns how many tensors were restored.  Sharded over several ranks, each rank
         keeps its slice of the full tensors (not collective)."""
         return self._load_named(model, named, self.momentum_flats)
-
-    def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout).  A state_dict with ``param_groups`` restores each
-        group's lr / weight_decay and raises ``ValueError`` if its groups hold other parameters than this optimizer's."""
-        self._load_group_state(sd, apply=False)
-        self.lr, self.momentum, self.weight_decay = float(sd["lr"]), float(sd["momentum"]), float(sd["weight_decay"])
-        self.nesterov = bool(sd.get("nesterov", False))          # checkpoints written before the option: plain momentum
-        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))   # ... and before clipping: none
-        self.steps = int(sd.get("steps", self.steps))
-        self._load_flats(sd, [(self.momentum_flats, sd["momentum_buffers"])], "momentum",
-                         "named_momentum() / load_named_momentum()")
-        self._load_group_state(sd)
-        self._sync_hyperparameters()
 
 
 def check_adamw_options(lr: float, betas, eps: float, weight_decay: float) -> tuple:
@@ -1112,50 +1207,18 @@ class FlatAdamW(_FlatOptimizer):
         for lr, wd, views in self._run_views(self._slice_runs(k, lo, n), flats):
             self._torch_adamw(*views, lr=lr, weight_decay=wd)
 
-    # ------------------------------------------------------------------ checkpointing
-    def state_dict(self) -> dict:
-        """Hyper-parameters, ``steps`` and the flat moment buffers (CPU copies).  Sharded over several ranks, the buffers are
-        this rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that crosses world sizes and modes is
-        :meth:`named_state`."""
-        sd = {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
-              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
-              "exp_avg": [m.detach().cpu().clone() for m in self.exp_avg_flats],
-              "exp_avg_sq": [v.detach().cpu().clone() for v in self.exp_avg_sq_flats]}
-        sd.update(self._shard_tags())
-        sd.update(self._group_state())
-        return sd
+    # ------------------------------------------------------------------ checkpointing: torch.optim.AdamW's names
+    _options = ("lr", "betas", "eps", "weight_decay")
+    _noun = "AdamW state"
+    named_state = _FlatOptimizer._named_state
+    load_named_state = _FlatOptimizer._load_named_state
 
-    def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout).  A state_dict with ``param_groups`` restores each
-        group's lr / weight_decay and raises ``ValueError`` if its groups hold other parameters than this optimizer's."""
-        self._load_group_state(sd, apply=False)
-        self._load_flats(sd, [(self.exp_avg_flats, sd["exp_avg"]), (self.exp_avg_sq_flats, sd["exp_avg_sq"])],
-                         "AdamW state", "named_state() / load_named_state()")
-        self.betas = check_adamw_options(sd["lr"], sd["betas"], sd["eps"], sd["weight_decay"])
-        self.lr, self.eps, self.weight_decay = float(sd["lr"]), float(sd["eps"]), float(sd["weight_decay"])
-        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
-        self.steps = int(sd["steps"])
-        self._load_group_state(sd)
-        self._sync_hyperparameters()
+    def _state_pairs(self) -> list:
+        return [("exp_avg", self.exp_avg_flats), ("exp_avg_sq", self.exp_avg_sq_flats)]
 
-    def named_state(self, model: nn.Module) -> dict:
-        """``{name: {"step", "exp_avg", "exp_avg_sq"}}`` (CPU copies), ``torch.optim.AdamW``'s per-parameter state by
-        parameter name, the form that crosses world sizes, sharded and unsharded runs and ``torch.optim.AdamW``.  Sharded
-        over several ranks this is collective: every rank calls it and gets the full tensors."""
-        m, v = self._named(model, self.exp_avg_flats), self._named(model, self.exp_avg_sq_flats)
-        return {n: {"step": torch.tensor(float(self.steps)), "exp_avg": m[n], "exp_avg_sq": v[n]} for n in m}
-
-    def load_named_state(self, model: nn.Module, named: dict) -> int:
-        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
-        (common) ``step``.  Sharded over several ranks, each rank keeps its slice (not collective)."""
-        steps = {int(s["step"]) for s in named.values()}
-        if len(steps) > 1:
-            raise ValueError(f"FlatAdamW keeps one step count for all parameters; this state has steps {sorted(steps)}")
-        done = self._load_named(model, {n: s["exp_avg"] for n, s in named.items()}, self.exp_avg_flats)
-        self._load_named(model, {n: s["exp_avg_sq"] for n, s in named.items()}, self.exp_avg_sq_flats)
-        if done and steps:
-            self.steps = steps.pop()
-        return done
+    def _check_options(self, sd: dict) -> dict:
+        return {"betas": check_adamw_options(sd["lr"], sd["betas"], sd["eps"], sd["weight_decay"]), "lr": float(sd["lr"]),
+                "eps": float(sd["eps"]), "weight_decay": float(sd["weight_decay"])}
 
 
 def check_rmsprop_options(lr: float, alpha: float, eps: float, weight_decay: float, momentum: float) -> None:
@@ -1284,70 +1347,26 @@ class FlatRMSprop(_FlatOptimizer):
         for lr, wd, views in self._run_views(self._slice_runs(k, lo, n), [self._shards[k][3][lo:lo + n], gf] + states):
             self._torch_rmsprop(*views, lr=lr, weight_decay=wd)
 
-    # ------------------------------------------------------------------ checkpointing
+    # ------------------------------------------------------------------ checkpointing: torch.optim.RMSprop's names
+    _options = ("lr", "alpha", "eps", "weight_decay", "momentum", "centered")
+    _noun = "RMSprop state"
+    _lacks = ("FlatRMSprop.load_named_state: an entry has no {key!r}; the state is of an RMSprop with another momentum or "
+              "centered setting")
+    named_state = _FlatOptimizer._named_state
+    load_named_state = _FlatOptimizer._load_named_state
+
     def _state_pairs(self) -> list:
-        """``(key, flats)`` of every state this optimizer keeps, in torch.optim.RMSprop's names."""
-        return [("square_avg", self.square_avg_flats)] + ([("momentum_buffer", self.momentum_buffer_flats)] if self.momentum > 0
-                                                          else []) + ([("grad_avg", self.grad_avg_flats)] if self.centered else [])
+        return [("square_avg", self.square_avg_flats), ("momentum_buffer", self.momentum_buffer_flats),
+                ("grad_avg", self.grad_avg_flats)]
 
-    def state_dict(self) -> dict:
-        """Hyper-parameters, ``steps`` and the flat state buffers (CPU copies): ``square_avg``, ``momentum_buffer`` and
-        ``grad_avg`` (the last two empty lists when the update has none).  Sharded over several ranks, the buffers are this
-        rank's shards, and ``sharded`` / ``world`` / ``rank`` say so; the form that crosses world sizes and modes is
-        :meth:`named_state`."""
-        sd = {"lr": self.lr, "alpha": self.alpha, "eps": self.eps, "weight_decay": self.weight_decay, "momentum": self.momentum,
-              "centered": self.centered, "max_grad_norm": self.max_grad_norm, "steps": self.steps,
-              "square_avg": [f.detach().cpu().clone() for f in self.square_avg_flats],
-              "momentum_buffer": [f.detach().cpu().clone() for f in self.momentum_buffer_flats],
-              "grad_avg": [f.detach().cpu().clone() for f in self.grad_avg_flats]}
-        sd.update(self._shard_tags())
-        sd.update(self._group_state())
-        return sd
-
-    def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout).  ``ValueError`` if the state_dict's ``centered``
-        or whether its momentum is > 0 differs from this optimizer's (those decide which states exist), or if its
-        ``param_groups`` hold other parameters than this optimizer's."""
-        self._load_group_state(sd, apply=False)
+    def _check_options(self, sd: dict) -> dict:
         if bool(sd["centered"]) != self.centered or (float(sd["momentum"]) > 0) != (self.momentum > 0):
             raise ValueError(f"FlatRMSprop.load_state_dict: the state_dict has centered={bool(sd['centered'])} and momentum "
                              f"{float(sd['momentum'])}, this optimizer centered={self.centered} and momentum {self.momentum}; "
                              "build it with the same centered and the same momentum > 0 (they decide which states exist)")
         check_rmsprop_options(sd["lr"], sd["alpha"], sd["eps"], sd["weight_decay"], sd["momentum"])
-        self._load_flats(sd, [(flats, sd[key]) for key, flats in self._state_pairs()], "RMSprop state",
-                         "named_state() / load_named_state()")
-        self.lr, self.weight_decay = float(sd["lr"]), float(sd["weight_decay"])
-        self.alpha, self.eps, self.momentum = float(sd["alpha"]), float(sd["eps"]), float(sd["momentum"])
-        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
-        self.steps = int(sd["steps"])
-        self._load_group_state(sd)
-        self._sync_hyperparameters()
-
-    def named_state(self, model: nn.Module) -> dict:
-        """``{name: {"step", "square_avg"[, "momentum_buffer"][, "grad_avg"]}}`` (CPU copies), ``torch.optim.RMSprop``'s
-        per-parameter state by parameter name, the form that crosses world sizes, sharded and unsharded runs and
-        ``torch.optim.RMSprop``.  Sharded over several ranks this is collective: every rank calls it and gets the full
-        tensors."""
-        parts = [(key, self._named(model, flats)) for key, flats in self._state_pairs()]
-        return {n: {"step": torch.tensor(float(self.steps)), **{key: named[n] for key, named in parts}} for n in parts[0][1]}
-
-    def load_named_state(self, model: nn.Module, named: dict) -> int:
-        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
-        (common) ``step``.  ``ValueError`` if an entry lacks a state this optimizer keeps.  Sharded over several ranks, each
-        rank keeps its slice (not collective)."""
-        steps = {int(s["step"]) for s in named.values()}
-        if len(steps) > 1:
-            raise ValueError(f"FlatRMSprop keeps one step count for all parameters; this state has steps {sorted(steps)}")
-        for key, _ in self._state_pairs():
-            if any(key not in s for s in named.values()):
-                raise ValueError(f"FlatRMSprop.load_named_state: an entry has no {key!r}; the state is of an RMSprop with "
-                                 "another momentum or centered setting")
-        done = 0
-        for key, flats in self._state_pairs():
-            done = self._load_named(model, {n: s[key] for n, s in named.items()}, flats)
-        if done and steps:
-            self.steps = steps.pop()
-        return done
+        return {"lr": float(sd["lr"]), "weight_decay": float(sd["weight_decay"]), "alpha": float(sd["alpha"]),
+                "eps": float(sd["eps"]), "momentum": float(sd["momentum"])}
 
 
 def check_adafactor_options(lr: float, beta2_decay: float, eps, d: float, weight_decay: float) -> tuple:
@@ -1459,9 +1478,9 @@ class FlatAdafactor(_FlatOptimizer):
         return ([t ** self.beta2_decay, self.eps1, self.eps2, self.d], [min(lr, 1 / (t ** 0.5)) for lr, _ in vals],
                 [1 - lr * wd for lr, wd in vals])
 
-    def _state_views(self, k: int, flat: torch.Tensor, i: int) -> dict:
-        """Tensor ``i`` of bucket ``k``'s state in ``flat``, as torch's shaped views: ``row_var`` / ``col_var`` or
-        ``variance``."""
+    def _state_views(self, k: int, flat: torch.Tensor, i: int, key: str = "state") -> dict:
+        """Tensor ``i`` of bucket ``k``'s state in ``flat`` (the one state flat, ``key`` ``"state"``), as torch's shaped
+        views: ``row_var`` / ``col_var`` or ``variance``."""
         gv, so = self.buckets[k].views[i], self._state_offsets[k][i]
         f = _factors(gv.shape)
         if f is None:
@@ -1493,71 +1512,21 @@ class FlatAdafactor(_FlatOptimizer):
             if self.fused_zero:
                 g.zero_()
 
-    # ------------------------------------------------------------------ checkpointing
-    def state_dict(self) -> dict:
-        """Hyper-parameters, ``steps`` and the state flats (CPU copies, ``state``); the form that crosses world sizes, bucket
-        layouts and ``torch.optim.Adafactor`` is :meth:`named_state`."""
-        sd = {"lr": self.lr, "beta2_decay": self.beta2_decay, "eps": self.eps, "d": self.d, "weight_decay": self.weight_decay,
-              "max_grad_norm": self.max_grad_norm, "steps": self.steps,
-              "state": [f.detach().cpu().clone() for f in self.state_flats]}
-        sd.update(self._group_state())
-        return sd
+    # ------------------------------------------------------------------ checkpointing: torch.optim.Adafactor's names
+    _options = ("lr", "beta2_decay", "eps", "d", "weight_decay")
+    _lacks = ("FlatAdafactor.load_named_state: the entry of {name!r} has no {keys}; its parameter has another number of "
+              "dimensions")
+    named_state = _FlatOptimizer._named_state
+    load_named_state = _FlatOptimizer._load_named_state
 
-    def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict` (same model => same bucket layout).  ``ValueError`` if its ``param_groups`` hold
-        other parameters than this optimizer's or its state flats have other sizes."""
-        self._load_group_state(sd, apply=False)
+    def _state_pairs(self) -> list:
+        return [("state", self.state_flats)]
+
+    def _check_options(self, sd: dict) -> dict:
         eps = tuple(sd["eps"])
-        self.eps1, self.eps2 = check_adafactor_options(sd["lr"], sd["beta2_decay"], eps, sd["d"], sd["weight_decay"])
-        if [f.numel() for f in sd["state"]] != [f.numel() for f in self.state_flats]:
-            raise ValueError("FlatAdafactor.load_state_dict: the state flats have other sizes than this optimizer's (another "
-                             "model or bucket layout); carry the state with named_state() / load_named_state()")
-        with torch.no_grad():
-            for f, src in zip(self.state_flats, sd["state"]):
-                f.copy_(src)
-        self.lr, self.weight_decay = float(sd["lr"]), float(sd["weight_decay"])
-        self.beta2_decay, self.eps, self.d = float(sd["beta2_decay"]), eps, float(sd["d"])
-        self.max_grad_norm = check_max_grad_norm(sd.get("max_grad_norm"))
-        self.steps = int(sd["steps"])
-        self._load_group_state(sd)
-
-    def named_state(self, model: nn.Module) -> dict:
-        """``{name: {"step", "row_var", "col_var"}}`` or ``{name: {"step", "variance"}}`` (CPU copies), ``torch.optim.Adafactor``'s
-        per-parameter state by parameter name: the form that crosses world sizes, bucket layouts and ``torch.optim.Adafactor``."""
-        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
-        out = {}
-        for k, gb in enumerate(self.buckets):
-            for i, p in enumerate(gb.params):
-                if id(p) in names:
-                    views = self._state_views(k, self.state_flats[k], i)
-                    out[names[id(p)]] = {"step": torch.tensor(float(self.steps)),
-                                         **{key: v.detach().cpu().clone() for key, v in views.items()}}
-        return out
-
-    @torch.no_grad()
-    def load_named_state(self, model: nn.Module, named: dict) -> int:
-        """Inverse of :meth:`named_state`; returns how many parameters' state was restored and sets ``steps`` from their
-        (common) ``step``.  ``ValueError`` if the steps differ or an entry lacks the state its parameter's shape needs."""
-        steps = {int(s["step"]) for s in named.values()}
-        if len(steps) > 1:
-            raise ValueError(f"FlatAdafactor keeps one step count for all parameters; this state has steps {sorted(steps)}")
-        names = {id(p): n for n, p in getattr(model, "module", model).named_parameters()}
-        done = 0
-        for k, gb in enumerate(self.buckets):
-            for i, p in enumerate(gb.params):
-                src = named.get(names.get(id(p)))
-                if src is None:
-                    continue
-                views = self._state_views(k, self.state_flats[k], i)
-                if any(key not in src for key in views):
-                    raise ValueError(f"FlatAdafactor.load_named_state: the entry of {names[id(p)]!r} has no "
-                                     f"{' / '.join(views)}; its parameter has another number of dimensions")
-                for key, v in views.items():
-                    v.copy_(src[key])
-                done += 1
-        if done and steps:
-            self.steps = steps.pop()
-        return done
+        eps1, eps2 = check_adafactor_options(sd["lr"], sd["beta2_decay"], eps, sd["d"], sd["weight_decay"])
+        return {"lr": float(sd["lr"]), "weight_decay": float(sd["weight_decay"]), "beta2_decay": float(sd["beta2_decay"]),
+                "eps": eps, "d": float(sd["d"]), "eps1": eps1, "eps2": eps2}
 
 
 def exclude_1d(name: str, param: torch.Tensor) -> bool:      # noqa: ARG001 - the name is there for custom rules
@@ -1714,10 +1683,10 @@ class FlatLAMB(_LayerwiseOptimizer):
                 g.zero_()
 
     # ------------------------------------------------------------------ checkpointing: FlatAdamW's forms
-    state_dict = FlatAdamW.state_dict
-    load_state_dict = FlatAdamW.load_state_dict
-    named_state = FlatAdamW.named_state
-    load_named_state = FlatAdamW.load_named_state
+    _options, _noun = FlatAdamW._options, FlatAdamW._noun
+    _state_pairs, _check_options = FlatAdamW._state_pairs, FlatAdamW._check_options
+    named_state = _FlatOptimizer._named_state
+    load_named_state = _FlatOptimizer._load_named_state
 
 
 def check_lars_options(lr: float, momentum: float, weight_decay: float, trust_coefficient: float, eps: float,
@@ -1798,19 +1767,16 @@ class FlatLARS(_LayerwiseOptimizer):
                 g.zero_()
 
     # ------------------------------------------------------------------ checkpointing: FlatSGD's forms
-    def state_dict(self) -> dict:
-        """:meth:`FlatSGD.state_dict` plus ``trust_coefficient`` and ``eps``; loads into ``FlatSGD`` as well."""
-        sd = FlatSGD.state_dict(self)
-        sd.update(trust_coefficient=self.trust_coefficient, eps=self.eps)
-        return sd
+    _options = FlatSGD._options + ("trust_coefficient", "eps")
+    _noun, _carry, _state_pairs = FlatSGD._noun, FlatSGD._carry, FlatSGD._state_pairs
 
-    def load_state_dict(self, sd: dict) -> None:
-        """Inverse of :meth:`state_dict`; a ``FlatSGD`` state_dict loads too (the LARS hyper-parameters stay)."""
-        check_lars_options(sd["lr"], sd["momentum"], sd["weight_decay"], sd.get("trust_coefficient", self.trust_coefficient),
-                           sd.get("eps", self.eps), bool(sd.get("nesterov", False)))
-        FlatSGD.load_state_dict(self, sd)
-        self.trust_coefficient = float(sd.get("trust_coefficient", self.trust_coefficient))
-        self.eps = float(sd.get("eps", self.eps))
+    def _defaults(self) -> dict:
+        # a FlatSGD state_dict loads too: the LARS options stay
+        return dict(FlatSGD._defaults(self), trust_coefficient=self.trust_coefficient, eps=self.eps)
+
+    def _check_options(self, sd: dict) -> dict:
+        check_lars_options(sd["lr"], sd["momentum"], sd["weight_decay"], sd["trust_coefficient"], sd["eps"], sd["nesterov"])
+        return dict(FlatSGD._check_options(self, sd), trust_coefficient=float(sd["trust_coefficient"]), eps=float(sd["eps"]))
 
     named_momentum = FlatSGD.named_momentum
     load_named_momentum = FlatSGD.load_named_momentum
