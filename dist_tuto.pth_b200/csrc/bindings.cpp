@@ -152,7 +152,8 @@ int b2_convnet_step_launch(const float* params, float* grads, const void* x, int
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream);
+                         float max_norm, float* clip_ws, float* grad_norm_out, int n_cta, cudaStream_t stream);
+int b2_reduce_units();
 int b2_convnet_eval_max_ctas(int dev);
 int b2_convnet_eval_samples_per_cta();
 int b2_convnet_eval_launch(const float* params, const void* x, int x_u8, const long long* target, double* result, int* slots,
@@ -2083,10 +2084,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          double lr, double mu, c10::optional<torch::Tensor> aux, c10::optional<torch::Tensor> loss_acc,
                          c10::optional<torch::Tensor> grads, int64_t grad_stride, py::object lr_schedule, double weight_decay,
                          bool nesterov, py::object max_grad_norm, c10::optional<torch::Tensor> clip_workspace,
-                         c10::optional<torch::Tensor> grad_norm_out) {
+                         c10::optional<torch::Tensor> grad_norm_out, int n_cta) {
     // one-GPU optimizer step from convnet_step(..., det_partials=slots, factors=factors): the local gradient is summed from
     // the first n_slots slots and n_samples factor rows in a fixed order, then SGD is applied to it.  The gradient bucket is
     // not read; given `grads`, its other-parity half is re-zeroed like allreduce_sgd does, so a bucket step may follow.
+    // n_cta: the kernel's grid; 0 is min(SMs, RED_UNITS), the grid every trainer uses.  A smaller grid runs several reduction
+    // units per CTA, as on a card with fewer SMs.  A CTA past the last unit never reaches its first unit's check-in on
+    // done_counter, so the step counter would never advance: grids above RED_UNITS are refused.
     check_cuda_contig(slots, "slots"); check_cuda_contig(factors, "factors");
     check_cuda_contig(params, "params"); check_cuda_contig(momentum, "momentum");
     TORCH_CHECK(slots.scalar_type() == torch::kFloat32 && slots.numel() >= (int64_t)n_slots * 21888, "slots: [n_slots, 21888] fp32");
@@ -2108,19 +2112,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     }
     const b2::LrSchedule sched = to_sched(lr_schedule);
     check_sgd_options(weight_decay, nesterov, mu, "reduce_sgd");
+    TORCH_CHECK(n_cta >= 0 && n_cta <= b2_reduce_units(), "reduce_sgd: n_cta must be 0 (the default grid) or 1..",
+                b2_reduce_units(), ", got ", n_cta);
     const float max_norm = check_max_grad_norm(max_grad_norm, "reduce_sgd");
     float* ws = clip_ws_ptr(max_norm, clip_workspace, params.numel(), "reduce_sgd");
     float* gn = grad_norm_ptr(grad_norm_out, "reduce_sgd");
     c10::cuda::CUDAGuard guard(params.device());
     ck_cuda(b2_reduce_sgd_launch(params.data_ptr<float>(), momentum.data_ptr<float>(), st, dc, (float)lr, (float)mu, ax, la, nullptr,
                                  slots.data_ptr<float>(), n_slots, factors.data_ptr<float>(), n_samples, g, grad_stride, &sched,
-                                 (float)weight_decay, nesterov ? 1 : 0, max_norm, ws, gn, cur_stream()),
+                                 (float)weight_decay, nesterov ? 1 : 0, max_norm, ws, gn, n_cta, cur_stream()),
             "reduce_sgd launch");
   }, py::arg("slots"), py::arg("n_slots"), py::arg("factors"), py::arg("n_samples"), py::arg("params"), py::arg("momentum"),
      py::arg("step"), py::arg("done_counter"), py::arg("lr"), py::arg("mu"), py::arg("aux") = py::none(), py::arg("loss_acc") = py::none(),
      py::arg("grads") = py::none(), py::arg("grad_stride") = 0, py::arg("lr_schedule") = py::none(),
      py::arg("weight_decay") = 0.0, py::arg("nesterov") = false, py::arg("max_grad_norm") = py::none(),
-     py::arg("clip_workspace") = py::none(), py::arg("grad_norm_out") = py::none());
+     py::arg("clip_workspace") = py::none(), py::arg("grad_norm_out") = py::none(), py::arg("n_cta") = 0);
   m.def("lr_schedule_eval", [](py::object schedule, double lr, torch::Tensor steps) {
     // the fp32 lr the optimizer kernels apply at each step-counter value of `steps`, computed by the same device function
     check_cuda_contig(steps, "steps");

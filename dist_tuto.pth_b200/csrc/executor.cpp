@@ -36,7 +36,7 @@ int b2_allreduce_sgd_launch(const PeerPtrsC* grads, const SignalPadsC* sig, floa
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream);
+                         float max_norm, float* clip_ws, float* grad_norm_out, int n_cta, cudaStream_t stream);
 int b2_convnet_cluster_launch(const float* params, float* grads, const void* x, int x_u8, const long long* target,
                               float* loss_acc, float* out_logp, float* mask_out, const unsigned long long* step,
                               unsigned long long seed, long long sample_base, int B, int training, int backward,
@@ -101,7 +101,7 @@ void StepExecutor::record_step(const void* x, const long long* y, float* loss_sn
     rc2 = b2_reduce_sgd_launch(cfg_.params, cfg_.momentum, cfg_.step_counter, cfg_.done_counter, cfg_.lr, cfg_.mu, cfg_.aux,
                                cfg_.loss_acc, loss_snapshot, cfg_.grad_slots, cfg_.B, cfg_.factors, cfg_.B, cfg_.grads_local,
                                cfg_.grad_stride, &cfg_.sched, cfg_.wd, cfg_.nesterov, cfg_.max_norm, cfg_.clip_ws, cfg_.grad_norm,
-                               compute_);
+                               /*n_cta=*/0, compute_);
   } else {
     PeerPtrsC g;
     SignalPadsC sg;

@@ -591,8 +591,9 @@ int b2_allreduce_sgd_launch(const PeerPtrs* grads, const b2::SignalPads* sig, fl
 int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* step, unsigned int* done_counter, float lr, float mu,
                          float* aux, float* loss_acc, float* loss_snapshot, const float* slots, int n_slots, const float* factors,
                          int n_samples, float* grads, long long grad_stride, const b2::LrSchedule* sched, float wd, int nesterov,
-                         float max_norm, float* clip_ws, float* grad_norm_out, cudaStream_t stream) {
+                         float max_norm, float* clip_ws, float* grad_norm_out, int n_cta, cudaStream_t stream) {
   if (step != nullptr && done_counter == nullptr) return (int)cudaErrorInvalidValue;
+  if (n_cta < 0 || n_cta > cn::RED_UNITS) return (int)cudaErrorInvalidValue;
   if (!(wd >= 0.f)) return (int)cudaErrorInvalidValue;
   const bool clip = max_norm > 0.f;     // max_norm 0: no clipping
   if (clip && (clip_ws == nullptr || !(max_norm < INFINITY))) return (int)cudaErrorInvalidValue;
@@ -612,7 +613,8 @@ int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* ste
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   }
-  const int blocks = sms < cn::RED_UNITS ? sms : cn::RED_UNITS;   // at most one CTA per SM
+  // at most one CTA per SM; n_cta > 0 asks for that grid instead (a CTA then runs every n_cta-th unit, as on a smaller card)
+  const int blocks = n_cta > 0 ? n_cta : (sms < cn::RED_UNITS ? sms : cn::RED_UNITS);
   static const int pdl = [] { const char* e = getenv("B200DIST_PDL"); return (e == nullptr || e[0] != '0') ? 1 : 0; }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -643,6 +645,8 @@ int b2_reduce_sgd_launch(float* params, float* momentum, unsigned long long* ste
   if (rc != 0) return rc;
   return (int)cudaLaunchKernelEx(&cfg, b2::reduce_sgd_kernel<true, b2::SgdArgsClip>, a, slots, n_slots, factors, n_samples, loss_acc);
 }
+
+int b2_reduce_units() { return cn::RED_UNITS; }
 
 int b2_det_reduce_launch(const float* partials, int n_slots, long long slot_stride, float* grads, const unsigned long long* step,
                          long long grad_stride, size_t n_elems, float* loss_acc, cudaStream_t stream) {

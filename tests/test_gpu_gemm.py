@@ -65,27 +65,34 @@ def test_each_call_launches_the_kernel_the_table_expects(C, table):
     with profile(activities=[ProfilerActivity.CUDA]):       # a first session starts the profiler before anything is counted
         torch.ones(1, device=dev).add_(1)
         torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        # Once another process has used the GPU, a session loses kernel records at its start, and the profiler keeps
-        # only the device activity inside its window.  ~10 ms sleep kernels before and after the GEMM launches keep
-        # every one of them well inside the window, so that each is recorded.
-        torch.cuda._sleep(20_000_000)
-        torch.cuda.synchronize()
-        small = iter(ops)
-        for c in table:
-            A, B, bias = next(small) if c.M * c.K < (1 << 26) else G.int_operands(c, _seed(c), dev)
+    pat = re.compile(r"gemm_bf16_kernel<\d+>|gemm_bf16_persistent_kernel")
+
+    def launched(A, B, bias, c):
+        """The GEMM kernels one call launched, from a profiler session around that call alone."""
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            # Once another process has used the GPU, a session loses kernel records at its start, and the profiler keeps
+            # only the device activity inside its window.  After many sessions in one process (the whole suite) the loss
+            # reaches past a single ~10 ms sleep kernel: twenty ~5 ms sleep kernels before the GEMM launch and one ~10 ms
+            # after it keep the launch well inside the window.
+            for _ in range(20):
+                torch.cuda._sleep(10_000_000)
+            torch.cuda.synchronize()
             C.gemm_bf16(A, B, bias, c.relu, c.out_bf16)
             torch.cuda.synchronize()
-        torch.cuda._sleep(20_000_000)
-        torch.cuda.synchronize()
-    pat = re.compile(r"gemm_bf16_kernel<\d+>|gemm_bf16_persistent_kernel")
-    ran = [(e.time_range.start, pat.search(e.name).group(0)) for e in prof.events()
-           if e.device_type == DeviceType.CUDA and pat.search(e.name)]
-    ran = [name for _, name in sorted(ran)]
-    want = [G.KERNEL_NAME[c.path] for c in table]
-    assert len(ran) == len(want), (len(ran), len(want), ran)
-    wrong = [(c, r) for c, r in zip(table, ran) if G.KERNEL_NAME[c.path] != r]
-    assert not wrong, wrong[:5]
+            torch.cuda._sleep(20_000_000)
+            torch.cuda.synchronize()
+        return [pat.search(e.name).group(0) for e in prof.events() if e.device_type == DeviceType.CUDA and pat.search(e.name)]
+
+    small = iter(ops)
+    for c in table:
+        A, B, bias = next(small) if c.M * c.K < (1 << 26) else G.int_operands(c, _seed(c), dev)
+        # A session that recorded no GEMM at all is run again; one call recorded as another kernel, or as more than one
+        # launch, fails at once.
+        for _ in range(3):
+            ran = launched(A, B, bias, c)
+            if ran:
+                break
+        assert ran == [G.KERNEL_NAME[c.path]], (c, ran)
     counts = {p: sum(1 for c in table if c.path == p) for p in G.PATHS}
     print(f"\n[gemm] profiler: calls per kernel {counts}")
 

@@ -5,7 +5,8 @@
 #   racecheck: shared-memory hazards (phase barriers of the fused ConvNet kernels, staging tiles of the tensor-core kernels)
 #   synccheck: divergent / mismatched barriers (incl. named barriers and mbarrier use in the wgmma kernels)
 # Coverage: per-sample kernel (1 CTA and 4-CTA cluster per sample), deterministic flush + det_reduce, the batched tensor-core
-# engine (B = 2 eval: every kernel of the pipeline), sgd_flat, the TMA + wgmma GEMM (both kernels); with 2 GPUs, memcheck of
+# engine (B = 2 eval: every kernel of the pipeline), sgd_flat, the TMA + wgmma GEMM (both kernels), reduce_sgd's instances (memcheck,
+# the clip instance at a 3-CTA grid) and det_reduce; with 2 GPUs, memcheck of
 # the push exchange and the all-reduce variants under `--target-processes all`.
 set -u
 cd "$(dirname "$0")/.."
@@ -18,6 +19,9 @@ for tool in memcheck racecheck synccheck; do
   timeout 1200 compute-sanitizer --tool $tool --error-exitcode 1 python -m pytest tests/test_gpu_batched.py -q -m gpu -p no:cacheprovider -k "test_every_stage_matches_the_rounding_exact_model[2-False] or test_uint8" > "$OUT/${tool}_batched.txt" 2>&1
   echo "$tool batched rc=$?" | tee -a "$OUT/summary.txt"; grep -E "ERROR SUMMARY|passed|failed" "$OUT/${tool}_batched.txt" | tail -3 | tee -a "$OUT/summary.txt"
 done
+SEL2='test_every_grid_reduces_in_the_model_order[5x24] or test_every_instance_matches_the_model_with_guard_bands[wd+nesterov+cosine] or test_every_instance_matches_the_model_with_guard_bands[clip+wd+nesterov] or test_det_reduce_sums_in_slot_order[33]'
+timeout 1200 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_reduce_sgd_order.py -q -m gpu -p no:cacheprovider -k "$SEL2" > "$OUT/memcheck_reduce_sgd.txt" 2>&1
+echo "memcheck reduce_sgd rc=$?" | tee -a "$OUT/summary.txt"; grep -E "ERROR SUMMARY|passed|failed" "$OUT/memcheck_reduce_sgd.txt" | tail -3 | tee -a "$OUT/summary.txt"
 if [ "$(nvidia-smi -L | wc -l)" -ge 2 ]; then
   B200DIST_STRESS_ITERS=200 timeout 1500 compute-sanitizer --tool memcheck --target-processes all --error-exitcode 1 python -m pytest tests/test_gpu_multi.py -q -p no:cacheprovider -k "test_push_exchange_equals_barrier_exchange or test_symmetric_allreduce_all_variants_vs_nccl" > "$OUT/memcheck_multigpu.txt" 2>&1
   echo "memcheck multi-GPU rc=$?" | tee -a "$OUT/summary.txt"; grep -E "ERROR SUMMARY|passed|failed" "$OUT/memcheck_multigpu.txt" | tail -4 | tee -a "$OUT/summary.txt"
